@@ -509,6 +509,10 @@ inline std::string normalized_image_name(std::string name) {
 }
 
 inline void compile_cluster(const Plan &plan, Compiled &out) {
+    // Open-Local LVM volumes are placed by the Python host side only (simon_b200/storage.py): asking this host side for them is an
+    // error, not a run that would refuse or ignore the volumes differently
+    if (const J *ol = plan.request.get("openLocal"))
+        if (ol->truthy()) throw CompileError("\"openLocal\": Open-Local volumes are not implemented by the native host side");
     const std::vector<const J *> &nodes = plan.nodes;
     const std::vector<PodRec> &pods = plan.pods;
     std::vector<int> order = node_tree_list(nodes);

@@ -201,6 +201,13 @@ struct simon_ctx {
     // multi-scenario state
     std::vector<ScenState *> scen_states;
     ScenBatch *batch = nullptr;
+    // Open-Local LVM volumes (simon_storage_upload); single-scenario state: VG requested [V][N] and the raw score scratch [N]
+    bool have_storage = false;
+    uint32_t V = 0;
+    DevBuf<int32_t> d_node_n_vg, d_vg_name, d_vol_vg, d_local_raw;
+    DevBuf<int64_t> d_vg_cap, d_vg_req0, d_vg_req, d_vol_size;
+    DevBuf<uint8_t> d_class_local;
+    DevBuf<uint32_t> d_vol_off;
 };
 
 namespace {
@@ -257,6 +264,9 @@ int reset_state(simon_ctx *ctx, ScenState &s) {
     // the run that wrote them: a state that restarts from empty - possibly with another scenario's node list - must not
     // inherit them (the kernel validates a summary only against flips of nodes it currently owns)
     if (s.csum.p) CU(cudaMemsetAsync(s.csum.p, 0, 8ull * std::max<size_t>(1, (size_t)ctx->n_classes * SK_CSUM_W), st));
+    // VG requested restarts from what the node annotations state
+    if (&s == &ctx->st && ctx->have_storage)
+        CU(cudaMemcpyAsync(ctx->d_vg_req.p, ctx->d_vg_req0.p, 8ull * ctx->V * N, cudaMemcpyDeviceToDevice, st));
     return SIMON_OK;
 }
 
@@ -291,6 +301,11 @@ void fill_params(simon_ctx *ctx, SkParams &P) {
     P.n_sigs = ctx->n_sigs; P.use_scache = ctx->use_scache; P.simon32 = ctx->simon32; P.scache = ctx->d_scache.p;
     P.cls_aux = ctx->d_cls_aux.p;
     P.dump_pod = 0xffffffffu; P.dump_total = nullptr; P.dump_code = nullptr;
+    if (ctx->have_storage) {
+        P.V = ctx->V; P.node_n_vg = ctx->d_node_n_vg.p; P.vg_name = ctx->d_vg_name.p; P.vg_cap = ctx->d_vg_cap.p;
+        P.class_local = ctx->d_class_local.p; P.vol_off = ctx->d_vol_off.p; P.vol_size = ctx->d_vol_size.p; P.vol_vg = ctx->d_vol_vg.p;
+        P.vg_req = ctx->d_vg_req.p; P.local_raw = ctx->d_local_raw.p;
+    }
 }
 
 #define SIMON_MAX_TPB 384u       // largest compiled variant: 12 warps, 168 registers/thread, no spills (640 threads = 96 registers spilled and measured slower)
@@ -480,7 +495,11 @@ int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t T
     if (ctx->big) {
         CU(ctx->d_gnode.alloc(ctx->gnode_stride * (size_t)n_scen * CS));
         P.gnode = ctx->d_gnode.p; P.gnode_stride = ctx->gnode_stride;
-        fn = simon_place_kernel_big;
+        fn = P.class_local ? simon_local_kernel_big : simon_place_kernel_big;
+    } else if (P.class_local) {
+        // Open-Local storage uploaded: the variants that carry its filter, score and bind (runtime node slots per thread)
+        if (prof) return fail(ctx, SIMON_ERR_LIMIT, "no kernel variant with phase timers and Open-Local storage");
+        fn = TPB <= 256 ? simon_local_kernel_256 : TPB <= 320 ? simon_local_kernel_320 : simon_local_kernel_384;
     } else {
         fn = pick_kernel(TPB, npt, prof);
         if (!fn) return fail(ctx, SIMON_ERR_LIMIT, "no kernel variant for %u threads per CTA%s", TPB, prof ? " with phase timers" : "");
@@ -601,6 +620,7 @@ int simon_snapshot_upload(simon_ctx *ctx, const simon_snapshot *s) {
     CU(cudaStreamSynchronize(st));
     ctx->have_snap = true;
     ctx->have_pods = false;
+    ctx->have_storage = false;
     return SIMON_OK;
 }
 
@@ -609,6 +629,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     if (!ctx->have_snap) return fail(ctx, SIMON_ERR_STATE, "simon_pods_upload before simon_snapshot_upload");
     CU(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
+    ctx->have_storage = false;          // the storage tables are per class: a new pod set needs its own upload
     ctx->n_classes = p->n_classes; ctx->n_pods = p->n_pods; ctx->n_counters = p->n_counters;
     // validate classes; derive limits
     uint32_t max_words = SCW_HDR_WORDS, emax = 0;
@@ -903,6 +924,7 @@ int simon_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *req_mem, in
 int simon_scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, simon_scenario_result *out, int32_t *out_node) {
     if (!ctx || !scen || !out) return SIMON_ERR_INVALID;
     if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_scenarios_run before uploads");
+    if (ctx->have_storage) return fail(ctx, SIMON_ERR_LIMIT, "scenario batches do not carry Open-Local storage state yet: use simon_schedule");
     CU(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     if (n == 0) return SIMON_OK;
@@ -1019,6 +1041,84 @@ int simon_state_download_ext(simon_ctx *ctx, int64_t *req_scalar, int64_t *gpu_u
     const uint32_t N = ctx->N;
     if (req_scalar && ctx->K) CU(cudaMemcpy(req_scalar, ctx->st.req_scalar.p, 8ull * ctx->K * N, cudaMemcpyDeviceToHost));
     if (gpu_used) CU(cudaMemcpy(gpu_used, ctx->st.gpu_used.p, 8ull * SIMON_MAX_GPU_DEV * N, cudaMemcpyDeviceToHost));
+    return SIMON_OK;
+}
+
+int simon_storage_upload(simon_ctx *ctx, const simon_storage *sg) {
+    if (!ctx || !sg) return SIMON_ERR_INVALID;
+    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_storage_upload before simon_pods_upload");
+    const uint32_t N = ctx->N, V = sg->n_vgs, C = ctx->n_classes;
+    if (sg->n_classes != C) return fail(ctx, SIMON_ERR_INVALID, "storage table has %u classes, the pod set %u", sg->n_classes, C);
+    if (V > SIMON_MAX_VGS) return fail(ctx, SIMON_ERR_LIMIT, "more than %d VGs per node", SIMON_MAX_VGS);
+    if (!sg->node_n_vg || !sg->class_local || !sg->vol_off || (V && N && (!sg->vg_capacity || !sg->vg_requested || !sg->vg_name)))
+        return fail(ctx, SIMON_ERR_INVALID, "missing storage column");
+    for (uint32_t g = 0; g < N; g++) {
+        const int32_t nv = sg->node_n_vg[g];
+        if (nv < -1 || nv > (int32_t)V) return fail(ctx, SIMON_ERR_INVALID, "node %u: bad VG count %d", g, nv);
+        for (int32_t a = 0; a < nv; a++)
+            for (int32_t b = 0; b < a; b++)
+                if (sg->vg_name[(size_t)a * N + g] == sg->vg_name[(size_t)b * N + g]) return fail(ctx, SIMON_ERR_INVALID, "node %u: duplicate VG name", g);
+    }
+    if (sg->vol_off[0] != 0) return fail(ctx, SIMON_ERR_INVALID, "vol_off[0] must be 0");
+    for (uint32_t c = 0; c < C; c++) {
+        if (sg->vol_off[c + 1] < sg->vol_off[c] || sg->vol_off[c + 1] - sg->vol_off[c] > SIMON_MAX_VOLS)
+            return fail(ctx, SIMON_ERR_LIMIT, "class %u: more than %d volumes", c, SIMON_MAX_VOLS);
+        if (sg->vol_off[c + 1] > sg->vol_off[c] && !sg->class_local[c]) return fail(ctx, SIMON_ERR_INVALID, "class %u: volumes without the local flag", c);
+    }
+    const uint32_t n_vol = C ? sg->vol_off[C] : 0;
+    if (n_vol && (!sg->vol_size || !sg->vol_vg)) return fail(ctx, SIMON_ERR_INVALID, "missing volume column");
+    for (uint32_t q = 0; q < n_vol; q++) {
+        if (sg->vol_size[q] <= 0) return fail(ctx, SIMON_ERR_INVALID, "volume %u: size must be > 0", q);
+        if (sg->vol_vg[q] < -1) return fail(ctx, SIMON_ERR_INVALID, "volume %u: VG name id must be >= -1", q);
+    }
+    CU(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    const size_t VN = std::max<size_t>(1, (size_t)V * N);
+    std::vector<int64_t> zero64(VN, 0);
+    std::vector<int32_t> zero32(VN, 0);
+    CU(ctx->d_node_n_vg.upload(sg->node_n_vg, std::max(1u, N), st));
+    CU(ctx->d_vg_cap.upload(V && N ? sg->vg_capacity : zero64.data(), VN, st));
+    CU(ctx->d_vg_req0.upload(V && N ? sg->vg_requested : zero64.data(), VN, st));
+    CU(ctx->d_vg_name.upload(V && N ? sg->vg_name : zero32.data(), VN, st));
+    CU(ctx->d_vg_req.alloc(VN)); CU(ctx->d_local_raw.alloc(std::max(1u, N)));
+    CU(ctx->d_class_local.upload(sg->class_local, std::max(1u, C), st));
+    CU(ctx->d_vol_off.upload(sg->vol_off, C + 1, st));
+    std::vector<int64_t> vs(sg->vol_size, sg->vol_size + n_vol); vs.push_back(0);
+    std::vector<int32_t> vv(sg->vol_vg, sg->vol_vg + n_vol); vv.push_back(0);
+    CU(ctx->d_vol_size.upload(vs.data(), vs.size(), st)); CU(ctx->d_vol_vg.upload(vv.data(), vv.size(), st));
+    // pods of classes with local storage read the VGs of every node: off the pinned-run fast path (-4) ...
+    if (ctx->n_pin_fast) {
+        std::vector<int32_t> fixed(ctx->n_pods), cls(ctx->n_pods);
+        CU(cudaMemcpyAsync(fixed.data(), ctx->d_pod_fixed.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(cls.data(), ctx->d_pod_class.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        for (uint32_t i = 0; i < ctx->n_pods; i++)
+            if (fixed[i] == -4 && sg->class_local[cls[i]]) { fixed[i] = -1; ctx->n_pin_fast--; }
+        CU(ctx->d_pod_fixed.upload(fixed.data(), ctx->n_pods, st));
+        CU(cudaStreamSynchronize(st));      // `fixed` leaves scope
+    }
+    // ... and not candidates of the move scoring
+    {
+        std::vector<SmvClass> mc(std::max(1u, C));
+        CU(cudaMemcpyAsync(mc.data(), ctx->d_mv_classes.p, sizeof(SmvClass) * mc.size(), cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        for (uint32_t c = 0; c < C; c++) if (sg->class_local[c]) mc[c].bits |= SMC_NOT_MOVABLE;
+        CU(ctx->d_mv_classes.upload(mc.data(), mc.size(), st));
+        CU(cudaStreamSynchronize(st));      // `mc` leaves scope
+    }
+    ctx->V = V;
+    ctx->have_storage = true;
+    int rc = reset_state(ctx, ctx->st);
+    if (rc) return rc;
+    CU(cudaStreamSynchronize(st));
+    return SIMON_OK;
+}
+
+int simon_storage_state_download(simon_ctx *ctx, int64_t *vg_requested) {
+    if (!ctx || !vg_requested) return SIMON_ERR_INVALID;
+    if (!ctx->have_storage) return fail(ctx, SIMON_ERR_STATE, "no storage uploaded");
+    CU(cudaSetDevice(ctx->device));
+    if (ctx->V && ctx->N) CU(cudaMemcpy(vg_requested, ctx->d_vg_req.p, 8ull * ctx->V * ctx->N, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 

@@ -147,6 +147,60 @@ __device__ __noinline__ int gpu_allocate(const SkParams &P, const SkScenario &SC
     return got == req_num ? got : 0;
 }
 
+// Open-Local LVM Filter / Score / Bind of class `cls` on node g (include/simon_gpu.h, simon_storage; ProcessLVMPVCPredicate
+// OL/scheduler/algorithm/algo/common.go:59-143, Binpack :574-619, ScoreLVM :660-692): the raw score, -1 if the node fails.
+// commit: add the PVCs to the VGs they were placed on (Bind, open-local.go:175-254).
+__device__ __noinline__ int local_eval(const SkParams &P, uint32_t cls, uint32_t g, bool commit) {
+    const int nv = P.node_n_vg[g];
+    if (nv < 0) return -1;                                  // no simon/node-local-storage annotation
+    const uint32_t q0 = P.vol_off[cls], q1 = P.vol_off[cls + 1];
+    if (q0 == q1) return 0;                                 // no LVM PVC: ProcessLVMPVCPredicate does not run (open-local.go:76-81)
+    const uint32_t N = P.N;
+    int64_t req[SIMON_MAX_VGS], used[SIMON_MAX_VGS];
+    #pragma unroll
+    for (int v = 0; v < SIMON_MAX_VGS; v++) { req[v] = v < nv ? P.vg_req[(uint64_t)v * N + g] : 0; used[v] = 0; }
+    #pragma unroll 1
+    for (uint32_t q = q0; q < q1; q++) {                    // PVCs whose class names a vgName come first
+        const int32_t id = P.vol_vg[q];
+        if (id < 0) continue;
+        int hit = -1;
+        #pragma unroll 1
+        for (int v = 0; v < nv; v++) if (P.vg_name[(uint64_t)v * N + g] == id) hit = v;
+        const int64_t sz = P.vol_size[q];
+        if (hit < 0 || P.vg_cap[(uint64_t)hit * N + g] - req[hit] < sz) return -1;
+        req[hit] += sz; used[hit] += sz;
+    }
+    if (nv == 0) return -1;                                 // NoAvailableVGError
+    #pragma unroll 1
+    for (uint32_t q = q0; q < q1; q++) {                    // the others: the VG of least free size that holds the PVC
+        if (P.vol_vg[q] >= 0) continue;
+        const int64_t sz = P.vol_size[q];
+        int best = -1;
+        int64_t bf = 0;
+        #pragma unroll 1
+        for (int v = 0; v < nv; v++) {
+            const int64_t fr = P.vg_cap[(uint64_t)v * N + g] - req[v];
+            if (fr >= sz && (best < 0 || fr < bf)) { best = v; bf = fr; }
+        }
+        if (best < 0) return -1;
+        req[best] += sz; used[best] += sz;
+    }
+    double sf = 0.0;
+    int cnt = 0;
+    #pragma unroll 1
+    for (int v = 0; v < nv; v++)
+        if (used[v] > 0) { sf += (double)used[v] / (double)P.vg_cap[(uint64_t)v * N + g]; cnt++; }
+    if (commit)
+        #pragma unroll 1
+        for (int v = 0; v < nv; v++) if (used[v] > 0) P.vg_req[(uint64_t)v * N + g] = req[v];
+    return cnt ? (int)f2i(sf / (double)cnt * 10.0) : 0;
+}
+
+// ClassState.cflags bits of classes that request Open-Local storage (simon_storage.class_local) and of classes with a GPU-share
+// request: bits of a word that is live anyway, so that the common path tests both extra filters at once
+#define SK_CLS_LOCAL (1u << 31)
+#define SK_CLS_GPU (1u << 30)
+
 #define ENT(row, e) S.ent[(row) * SK_MAX_ENT + (e)]
 #define A64(k, idx) S.a64[(k) * L + (idx)]
 #define A32(k, idx) S.a32[(k) * L + (idx)]
@@ -159,7 +213,7 @@ struct ClassState {
     uint32_t E, n_ports, n_hard, n_soft, n_aff, n_isc;
     uint32_t e_hard, e_soft, e_aff, e_anti, e_exist, e_isc;
     uint32_t cflags;
-    bool any_table, has_gpu;
+    bool any_table;
     bool pinned;         // SIMON_CLS_PINNED: the static verdict of the pin node depends on the pod, nothing is carried from pod to pod
     int64_t aff_total;
     // summary of the feasible set
@@ -171,8 +225,11 @@ struct ClassState {
 };
 
 // ---------------------------------------------------------------------------------------------------------
-template <int MAXT, int NPT_T, bool PROF, bool BIG = false>
+// LOCAL: the variants launched when Open-Local storage was uploaded (simon_storage_upload); every other run uses variants whose
+// code has none of it
+template <int MAXT, int NPT_T, bool PROF, bool BIG = false, bool LOCAL = false>
 __device__ __forceinline__ void simon_place_body(const SkParams &P) {
+    constexpr uint32_t CLS_LOCAL = LOCAL ? SK_CLS_LOCAL : 0u;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     cg::cluster_group cluster = cg::this_cluster();
     const uint32_t CS = cluster.num_blocks();
@@ -350,11 +407,14 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
         #pragma unroll 1
         for (uint32_t e = C.e_exist; e < C.e_isc; e++)
             if (DOM(ENT(ER_T, e), idx) >= 0 && VAL(e, idx) > 0) return 1u << SFC_IPA_EXIST;
-        if (C.has_gpu) {
+        if (C.cflags & (CLS_LOCAL | SK_CLS_GPU)) {
             uint32_t g = (uint32_t)A32(B_NODE_G, idx);
-            int slots[64];
-            int64_t total = P.gpu_total_mem ? P.gpu_total_mem[g] : 0;
-            if (total < cw[SCW_GPU_MEM] || gpu_allocate(P, SC, cw[SCW_GPU_MEM], cw[SCW_GPU_COUNT], g, slots) == 0) return 1u << SFC_GPU;
+            if ((C.cflags & CLS_LOCAL) && P.local_raw[g] < 0) return 1u << SFC_LOCAL;
+            if (C.cflags & SK_CLS_GPU) {
+                int slots[64];
+                int64_t total = P.gpu_total_mem ? P.gpu_total_mem[g] : 0;
+                if (total < cw[SCW_GPU_MEM] || gpu_allocate(P, SC, cw[SCW_GPU_MEM], cw[SCW_GPU_COUNT], g, slots) == 0) return 1u << SFC_GPU;
+            }
         }
         return 0;
     };
@@ -694,7 +754,8 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             const uint32_t n_anti = (uint32_t)cw[SCW_N_IPA_ANTI], n_exist = (uint32_t)cw[SCW_N_IPA_EXIST];
             C.e_hard = C.n_ports; C.e_soft = C.e_hard + C.n_hard; C.e_aff = C.e_soft + C.n_soft; C.e_anti = C.e_aff + C.n_aff;
             C.e_exist = C.e_anti + n_anti; C.e_isc = C.e_exist + n_exist; C.E = C.e_isc + C.n_isc;
-            C.has_gpu = cw[SCW_GPU_MEM] > 0;
+            if (cw[SCW_GPU_MEM] > 0) C.cflags |= SK_CLS_GPU;
+            if (LOCAL && P.class_local && P.class_local[cls]) C.cflags |= CLS_LOCAL;
             C.sum_valid = false;
             C.snorm_valid = false;
             C.any_table = cw[SCW_ANY_TABLE] != 0;
@@ -960,6 +1021,17 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             for (int q = 0; q < SK_MAX_HARD; q++) hard_min[q] = (int32_t)hv[q];
         }
 
+        // ---- Open-Local (rare): verdict and raw score of every node on the current VG state, read by the filters and the totals
+        //      below (a pass of its own: the per-node loops of the common path stay free of calls) ----
+        if (C.cflags & CLS_LOCAL) {
+            #pragma unroll 1
+            for (uint32_t s = 0; s < NPT; s++) {
+                uint32_t idx = s * TPB + tid;
+                if (!(A8(C_NFLAGS, idx) & NF_VALID)) continue;
+                const uint32_t g = (uint32_t)A32(B_NODE_G, idx);
+                P.local_raw[g] = local_eval(P, (uint32_t)cls, g, false);
+            }
+        }
         TICK(3);
         // ---- P1: filters on cached state ----
         uint32_t my_fl = 0;                 // bit 0: some node flipped; bit 1: the last winner became infeasible; bits 2..5: it held an extreme
@@ -1174,6 +1246,31 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             }
         }
 
+        // ---- Open-Local: range of the feasible nodes' raw scores, then each one's normalised score (NormalizeScore,
+        //      open-local.go:146-171, weight 1) in place of its raw score, and added to B_SNORM for the totals of P3 (taken off
+        //      again right after: P3's per-node loop stays as it is for every other class) ----
+        if ((C.cflags & CLS_LOCAL) && C.F > 1) {
+            uint32_t lv[2] = {w_enc(INT32_MAX), w_enc(INT32_MIN)};
+            const int lop[2] = {W_MIN, W_MAX};
+            #pragma unroll 1
+            for (uint32_t s = 0; s < NPT; s++) {
+                uint32_t idx = s * TPB + tid;
+                if (!(A8(C_NFLAGS, idx) & NF_FEASIBLE)) continue;
+                const uint32_t e = w_enc(P.local_raw[(uint32_t)A32(B_NODE_G, idx)]);
+                lv[0] = e < lv[0] ? e : lv[0];
+                lv[1] = e > lv[1] ? e : lv[1];
+            }
+            sk_allreduce_w<2>(R, lv, lop);
+            const int32_t lo = w_dec(lv[0]), range = w_dec(lv[1]) - lo;
+            #pragma unroll 1
+            for (uint32_t s = 0; s < NPT; s++) {
+                uint32_t idx = s * TPB + tid;
+                if (!(A8(C_NFLAGS, idx) & NF_FEASIBLE)) continue;
+                int32_t *x = P.local_raw + (uint32_t)A32(B_NODE_G, idx);
+                *x = range == 0 ? 0 : (*x - lo) * 100 / range;
+                A32(B_SNORM, idx) += *x;
+            }
+        }
         TICK(6);
         if (!PROF && i == P.dump_pod && P.dump_code) {
             // debug: the per-node filter verdict of this pod (tests compare it with the oracle's)
@@ -1243,6 +1340,13 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             unsigned long long key = ((unsigned long long)(total + 1) << 24) | (unsigned long long)(0xFFFFFFu - r);
             best = key > best ? key : best;
         }
+        if ((C.cflags & CLS_LOCAL) && C.F > 1) {
+            #pragma unroll 1
+            for (uint32_t s = 0; s < NPT; s++) {
+                uint32_t idx = s * TPB + tid;
+                if (A8(C_NFLAGS, idx) & NF_FEASIBLE) A32(B_SNORM, idx) -= P.local_raw[(uint32_t)A32(B_NODE_G, idx)];
+            }
+        }
         TICK(7);
         // The exchange of the arg-max is the longest wait of a decision.  Meanwhile the owner of every warp's best candidate evaluates
         // what its node's Fit verdict and own-state score WOULD be after receiving this pod, so that the one true winner
@@ -1300,7 +1404,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                     SC.out_node[i] = (int32_t)g;
                     if (SC.out_score) SC.out_score[i] = C.F > 1 ? win_total : 0;
                     uint32_t gpu_pack = 0;
-                    if (C.has_gpu) {
+                    if (C.cflags & SK_CLS_GPU) {
                         // Reserve (open-gpu-share.go:147-188): the devices AllocateGpuId picks; reported as 4 bits per device
                         int slots[64];
                         int ns = gpu_allocate(P, SC, cw[SCW_GPU_MEM], cw[SCW_GPU_COUNT], g, slots);
@@ -1312,6 +1416,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                         }
                     }
                     if (SC.out_gpu) SC.out_gpu[i] = gpu_pack;
+                    if (C.cflags & CLS_LOCAL) local_eval(P, (uint32_t)cls, g, true);      // Bind: the VGs the Filter's choice took
                 }
                 const int64_t *inc = cw + cw[SCW_OFF_INC];
                 const uint32_t n_inc_list = (uint32_t)cw[SCW_N_INC];
@@ -1331,7 +1436,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                 __syncwarp();
             }
         }
-        if (C.has_gpu) __syncthreads();      // the owner's next filter pass reads gpu_used, written by the helper warp
+        if (C.cflags & (SK_CLS_GPU | CLS_LOCAL)) __syncthreads();      // the owner's next filter pass reads gpu_used / vg_req, written by the helper warp
         // every thread folds the winner into its cached counter values (S.inc was built at the class change; the
         // reductions in between contain __syncthreads)
         {
@@ -1467,3 +1572,16 @@ SIMON_KERNEL_PLAIN(384, 0)
 SIMON_KERNEL_PLAIN(384, 1)
 SIMON_KERNEL_PLAIN(384, 2)
 SIMON_KERNEL_PLAIN(384, 3)
+// Open-Local: one variant per thread count (node slots per thread at run time) and a large-cluster one
+extern "C" __global__ void __launch_bounds__(256, 1) simon_local_kernel_256(const __grid_constant__ SkParams P) {
+    simon_place_body<256, 0, false, false, true>(P);
+}
+extern "C" __global__ void __launch_bounds__(320, 1) simon_local_kernel_320(const __grid_constant__ SkParams P) {
+    simon_place_body<320, 0, false, false, true>(P);
+}
+extern "C" __global__ void __launch_bounds__(384, 1) simon_local_kernel_384(const __grid_constant__ SkParams P) {
+    simon_place_body<384, 0, false, false, true>(P);
+}
+extern "C" __global__ void __launch_bounds__(320, 1) simon_local_kernel_big(const __grid_constant__ SkParams P) {
+    simon_place_body<320, 0, false, true, true>(P);
+}

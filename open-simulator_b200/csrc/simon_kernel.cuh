@@ -112,6 +112,14 @@ struct SkParams {
     long long *dump_total;         // [N]
     int32_t *dump_code;            // [N] 0 = feasible, else the reason bitmask
     unsigned long long *scache;    // [n_sigs][N] packed {st_code, flags, tt, 0, na:int32}
+    // Open-Local LVM volumes (simon_storage); class_local == nullptr: no class requests local storage
+    uint32_t V, pad_v;
+    const int32_t *node_n_vg, *vg_name, *vol_vg;
+    const int64_t *vg_cap, *vol_size;
+    const uint8_t *class_local;
+    const uint32_t *vol_off;
+    int64_t *vg_req;               // [V][N] VG requested (single-scenario state: scenario batches refuse storage)
+    int32_t *local_raw;            // [N] the current decision's per-node verdict / raw score, then normalised score (scratch)
 };
 
 __host__ __device__ inline size_t sk_align(size_t x) { return (x + 15) & ~(size_t)15; }

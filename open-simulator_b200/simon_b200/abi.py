@@ -53,6 +53,22 @@ class SimonMovesResult(C.Structure):
                 ("kernel_ms", C.c_float), ("reserved", C.c_uint32)]
 
 
+class SimonStorage(C.Structure):
+    _fields_ = [("n_vgs", C.c_uint32), ("n_classes", C.c_uint32),
+                ("node_n_vg", C.c_void_p), ("vg_capacity", C.c_void_p), ("vg_requested", C.c_void_p), ("vg_name", C.c_void_p),
+                ("class_local", C.c_void_p), ("vol_off", C.c_void_p), ("vol_size", C.c_void_p), ("vol_vg", C.c_void_p)]
+
+
+def marshal_storage(st):
+    """storage.StorageTables -> (SimonStorage, arrays that must outlive the upload call)."""
+    keep = [np.ascontiguousarray(a, dtype=t) for a, t in (
+        (st.node_n_vg, np.int32), (st.vg_capacity, np.int64), (st.vg_requested, np.int64), (st.vg_name, np.int32),
+        (st.class_local, np.uint8), (st.vol_off, np.uint32), (st.vol_size, np.int64), (st.vol_vg, np.int32))]
+    keep = [a if a.size else np.zeros(1, a.dtype) for a in keep]
+    s = SimonStorage(st.n_vgs, len(st.class_local), *[a.ctypes.data for a in keep])
+    return s, keep
+
+
 MOVE_NOOP, MOVE_NOT_PLACED, MOVE_NOT_MOVABLE, MOVE_BAD_INDEX = 1 << 24, 1 << 25, 1 << 26, 1 << 27
 MOVE_GAIN_BIAS = 1000
 

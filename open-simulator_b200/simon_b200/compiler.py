@@ -176,6 +176,7 @@ class Compiled:
     topo_keys: List[str]
     counters: List[Tuple[frozenset, int]]
     pod_recs: List[PodRec]
+    storage: Optional[object] = None      # storage.StorageTables when compiled with open_local=True
 
     def node_index(self, name: str) -> int:
         if not hasattr(self, "_nidx"):
@@ -236,7 +237,7 @@ def _term_parts(pod_ns: str, term: Obj):
     return nsset, (None if reqs is None else tuple(reqs)), term.get("topologyKey", "") or ""
 
 
-def _parse_class(cid: int, tmpl: PodTemplate) -> ClassInfo:
+def _parse_class(cid: int, tmpl: PodTemplate, open_local: bool = False) -> ClassInfo:
     pod = tmpl.pod
     spec = pod.get("spec") or {}
     ci = ClassInfo(cid, tmpl, O.namespace_of(pod) or "default", dict(O.labels_of(pod)), spec)
@@ -330,11 +331,11 @@ def _parse_class(cid: int, tmpl: PodTemplate) -> ClassInfo:
             pass
     if GPU_INDEX_NAME in ann and ci.gpu_mem > 0:
         raise CompileError("pods with a preset alibabacloud.com/gpu-index annotation are not supported")
-    # Open-Local (pkg/simulator/plugin/open-local.go:51-138) is out of scope (SURVEY 8a row 26): pods that REQUEST local
-    # storage would be filtered / scored / reserved by it, so they are refused instead of being placed as if it did not
-    # exist.  A StatefulSet without open-local volumeClaimTemplates carries the annotation with an empty list
-    # (pkg/utils/utils.go:249-292) and is unaffected: GetPodLocalPVCs returns nothing and the plugin is inert.
-    if O.ANNO_POD_LOCAL_STORAGE in ann:
+    # Open-Local (pkg/simulator/plugin/open-local.go:51-254) runs only when the caller opts in (open_local=True, storage.py):
+    # otherwise pods that REQUEST local storage would be filtered / scored / bound by it, so they are refused instead of being
+    # placed as if it did not exist.  A StatefulSet without open-local volumeClaimTemplates carries the annotation with an empty
+    # list (pkg/utils/utils.go:249-292) and is unaffected: GetPodLocalPVCs returns nothing and the plugin is inert.
+    if not open_local and O.ANNO_POD_LOCAL_STORAGE in ann:
         import json as _json
         try:
             vols = (_json.loads(ann[O.ANNO_POD_LOCAL_STORAGE]) or {}).get("volumes") or []
@@ -421,13 +422,23 @@ class ExtraScorePlugin:
 
 
 def compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[ClusterContext] = None,
-                    extra_log: int = 0, extra_plugins: Optional[List[ExtraScorePlugin]] = None) -> Compiled:
+                    extra_log: int = 0, extra_plugins: Optional[List[ExtraScorePlugin]] = None,
+                    open_local: bool = False, storage_classes: Optional[List[Obj]] = None) -> Compiled:
+    """open_local: run the Open-Local plugin's LVM part (storage.py) instead of refusing pods that request local storage;
+    storage_classes: the StorageClasses of the cluster and the apps (their vgName / mediaType parameters)."""
     with O.gc_paused():
-        return _compile_cluster(nodes, pods, ctx, extra_log, extra_plugins)
+        c = _compile_cluster(nodes, pods, ctx, extra_log, extra_plugins, open_local)
+        if open_local:
+            from .storage import StorageError, compile_storage
+            try:
+                c.storage = compile_storage(c.node_objs, [ci.tmpl.pod for ci in c.classes], list(storage_classes or []))
+            except StorageError as e:
+                raise CompileError(str(e)) from None
+        return c
 
 
 def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[ClusterContext],
-                     extra_log: int, extra_plugins: Optional[List[ExtraScorePlugin]]) -> Compiled:
+                     extra_log: int, extra_plugins: Optional[List[ExtraScorePlugin]], open_local: bool = False) -> Compiled:
     ctx = ctx or ClusterContext()
     order = node_tree_list(nodes)
     snodes = [nodes[i] for i in order]
@@ -447,7 +458,7 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
         if cid is None:
             cid = len(classes)
             key_to_cid[k] = cid
-            classes.append(_parse_class(cid, t))
+            classes.append(_parse_class(cid, t, open_local))
         tmpl_seen[id(t)] = cid
         t.class_id = cid
     pod_class = np.fromiter((r.tmpl.class_id for r in pods), dtype=np.int32, count=len(pods))

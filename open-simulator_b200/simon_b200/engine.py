@@ -23,7 +23,8 @@ EXPORTS = ["simon_gpu_version", "simon_ctx_create", "simon_ctx_destroy", "simon_
            "simon_gpu_slots_download", "simon_state_download_ext", "simon_debug_set_dump_pod", "simon_debug_dump_read",
            "simon_moves_upload", "simon_moves_run", "simon_moves_replay", "simon_host_go118_sort",
            "simon_host_last_error", "simon_host_compile", "simon_host_plan_free", "simon_host_plan_columns", "simon_host_plan_describe",
-           "simon_host_simulate", "simon_host_free", "simon_host_quantity_probe", "simon_host_plan_fit_error", "simon_host_capacity_search"]
+           "simon_host_simulate", "simon_host_free", "simon_host_quantity_probe", "simon_host_plan_fit_error", "simon_host_capacity_search",
+           "simon_storage_upload", "simon_storage_state_download"]
 
 
 class EngineUnavailable(RuntimeError):
@@ -83,6 +84,10 @@ def lib():
         L.simon_moves_replay.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_float)]
         L.simon_host_go118_sort.restype = C.c_int
         L.simon_host_go118_sort.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
+        L.simon_storage_upload.restype = C.c_int
+        L.simon_storage_upload.argtypes = [C.c_void_p, C.c_void_p]
+        L.simon_storage_state_download.restype = C.c_int
+        L.simon_storage_state_download.argtypes = [C.c_void_p, C.c_void_p]
     except AttributeError:
         if not os.environ.get("SIMON_GPU_LIB"):       # an experiment library may lack the newer entry points; the shipped one may not
             raise
@@ -109,6 +114,9 @@ class Engine:
         self.snap, self.pods, self._keep = abi.marshal(compiled)
         self._check(L.simon_snapshot_upload(self.h, C.byref(self.snap)))
         self._check(L.simon_pods_upload(self.h, C.byref(self.pods)))
+        if getattr(compiled, "storage", None) is not None:      # Open-Local LVM volumes (compile_cluster(open_local=True))
+            self.storage, keep = abi.marshal_storage(compiled.storage)
+            self._check(L.simon_storage_upload(self.h, C.byref(self.storage)))
 
     def _check(self, rc: int):
         if rc != 0:
@@ -190,6 +198,13 @@ class Engine:
         arrs = [np.zeros(N, np.int64) for _ in range(5)] + [np.zeros(N, np.int32)]
         self._check(lib().simon_state_download(self.h, *[a.ctypes.data for a in arrs]))
         return dict(zip(["req_mcpu", "req_mem", "req_eph", "nz_mcpu", "nz_mem", "num_pods"], arrs))
+
+    def storage_state(self) -> np.ndarray:
+        """Open-Local VG requested after scheduling, [V][N]."""
+        V, N = self.c.storage.n_vgs, self.c.n_nodes
+        a = np.zeros(max(V * N, 1), np.int64)
+        self._check(lib().simon_storage_state_download(self.h, a.ctypes.data))
+        return a[:V * N].reshape(V, N)
 
     def gpu_slots(self, first: int = 0, count: Optional[int] = None):
         """GPU-share Reserve results: per pod a list of device ids (one per GPU slot, ascending), [] if none."""

@@ -58,6 +58,7 @@ class SimulatorOptions:
     patchPodFuncMap: dict = field(default_factory=dict)
     device: int = 0
     record_scores: bool = False
+    openLocal: bool = False
 
 
 Option = Callable[[SimulatorOptions], None]
@@ -82,6 +83,12 @@ def WithExtraRegistry(reg: dict) -> Option:
 
 def WithDevice(device: int) -> Option:
     return lambda o: setattr(o, "device", device)
+
+
+def WithOpenLocal() -> Option:
+    """Run the Open-Local plugin's LVM volumes (pkg/simulator/plugin/open-local.go; simon_b200/storage.py for what is covered
+    and the tie-breaking it fixes) instead of refusing pods that request local storage."""
+    return lambda o: setattr(o, "openLocal", True)
 
 
 @dataclass
@@ -156,10 +163,12 @@ def _static_reasons(compiled: Compiled, rec: PodRec, idxs) -> dict:
 
 
 def format_fit_error(compiled: Compiled, rec: PodRec, counts: np.ndarray, active: Optional[List[int]] = None,
-                     gpu_nodes: Optional[List[str]] = None, static_memo: Optional[dict] = None) -> str:
+                     gpu_nodes: Optional[List[str]] = None, static_memo: Optional[dict] = None,
+                     local_reasons: Optional[List[Optional[str]]] = None) -> str:
     """FitError.Error() (generic_scheduler.go:72-90) + the wrapper of Simulator.update (simulator.go:465).
     gpu_nodes: names of the nodes the Open-Gpu-Share filter rejected - its status message is "Node:<name>"
-    (pkg/simulator/plugin/open-gpu-share.go:66-79), so every such node contributes its own reason string with count 1."""
+    (pkg/simulator/plugin/open-gpu-share.go:66-79), so every such node contributes its own reason string with count 1.
+    local_reasons: the Open-Local Filter's message of every node it rejected (None: Unschedulable without a reason), in any order."""
     idxs = range(compiled.n_nodes) if active is None else active
     # the node-static reasons depend on the pod's template and the node list alone: failing replicas of one workload share them
     mkey = (id(rec.tmpl), None if active is None else tuple(active))
@@ -184,6 +193,13 @@ def format_fit_error(compiled: Compiled, rec: PodRec, counts: np.ndarray, active
                 reasons["Node:" + nm] = reasons.get("Node:" + nm, 0) + 1
         else:       # node list not collected (more failing GPU pods than the re-evaluation budget): counts only
             reasons["Node:<%d nodes rejected by Open-Gpu-Share>" % int(counts[19])] = int(counts[19])
+    if len(counts) > 20 and int(counts[20]):
+        if local_reasons is not None and len(local_reasons) == int(counts[20]):
+            for r in local_reasons:
+                if r:
+                    reasons[r] = reasons.get(r, 0) + 1
+        else:       # per-node texts not collected: counts only
+            reasons["<%d nodes rejected by Open-Local>" % int(counts[20])] = int(counts[20])
     total = len(idxs)
     parts = sorted(f"{v} {k}" for k, v in reasons.items())
     msg = f"0/{total} nodes are available: {', '.join(parts)}."
@@ -191,7 +207,8 @@ def format_fit_error(compiled: Compiled, rec: PodRec, counts: np.ndarray, active
     return f"failed to schedule pod ({ns}/{rec.name}): Unschedulable: {msg}"
 
 
-def build_result(compiled: Compiled, p: Plan, out_node: np.ndarray, fail_counts, fail_pod, gpu_fail_nodes=None) -> SimulateResult:
+def build_result(compiled: Compiled, p: Plan, out_node: np.ndarray, fail_counts, fail_pod, gpu_fail_nodes=None,
+                 local_fail_reasons=None) -> SimulateResult:
     res = SimulateResult()
     statuses = [NodeStatus(Node=n) for n in p.nodes]
     by_sorted = {i: statuses[compiled.node_orig_index[i]] for i in range(compiled.n_nodes)}
@@ -208,7 +225,8 @@ def build_result(compiled: Compiled, p: Plan, out_node: np.ndarray, fail_counts,
             j = fail_idx.get(i)
             counts = fail_counts[j] if j is not None and j < len(fail_counts) else np.zeros(24, np.uint32)
             res.UnscheduledPods.append(UnscheduledPod(rec, format_fit_error(compiled, rec, counts, gpu_nodes=(gpu_fail_nodes or {}).get(i),
-                                                                              static_memo=static_memo)))
+                                                                              static_memo=static_memo,
+                                                                              local_reasons=(local_fail_reasons or {}).get(i))))
     res.NodeStatus = statuses
     return res
 
@@ -247,7 +265,9 @@ def _simulate(cluster: ResourceTypes, apps: List[AppResource], *opts: Option) ->
     p = plan(cluster, apps)
     tm["plan_s"] = time.perf_counter() - t0
     t0 = time.perf_counter()
-    compiled = compile_cluster(p.nodes, p.pods, p.ctx, extra_plugins=extra_plugins or None)
+    storage_classes = list(cluster.StorageClasss) + [sc for a in apps for sc in a.Resource.StorageClasss] if options.openLocal else None
+    compiled = compile_cluster(p.nodes, p.pods, p.ctx, extra_plugins=extra_plugins or None, open_local=options.openLocal,
+                               storage_classes=storage_classes)
     tm["compile_s"] = time.perf_counter() - t0
     gpu_fail_nodes = {}
     t0 = time.perf_counter()
@@ -264,11 +284,60 @@ def _simulate(cluster: ResourceTypes, apps: List[AppResource], *opts: Option) ->
         for pod in todo:
             _o, _t, code = eng.dump_pod(pod)
             gpu_fail_nodes[pod] = [compiled.node_names[g] for g in np.nonzero(code & gpu_bit)[0]]
+        local_fail_reasons = {}
+        if compiled.storage is not None:
+            # Open-Local's messages name VG sizes as of the pod's turn: the node list comes from the verdict dump (a bounded number
+            # of pods, like GPU-share's), the sizes from the replay of Bind in placement order
+            local_fail_reasons = _local_fail_reasons(eng, compiled, out_node, fail_counts, fail_pod)
         tm["gpu_fail_detail_s"] = time.perf_counter() - t0
         t0 = time.perf_counter()
     tm["engine_close_s"] = time.perf_counter() - t0
     t0 = time.perf_counter()
-    res = build_result(compiled, p, out_node, fail_counts, fail_pod, gpu_fail_nodes)
+    res = build_result(compiled, p, out_node, fail_counts, fail_pod, gpu_fail_nodes, local_fail_reasons)
+    if compiled.storage is not None:
+        _write_storage_annotations(compiled, res, out_node)
     tm["build_result_s"] = time.perf_counter() - t0
     Simulate.last_timing = tm       # where the wall clock of the last call went (bench.py reports it beside e2e_api)
     return res
+
+
+def _bound_by_scheduler(compiled: Compiled, out_node: np.ndarray):
+    """(pod, node) of the pods that went through a scheduling cycle and landed: pre-bound pods never reach Bind."""
+    fixed = compiled.pods["pod_fixed_node"]
+    for i, n in enumerate(np.asarray(out_node).tolist()):
+        if n >= 0 and int(fixed[i]) == -1:
+            yield i, n
+
+
+def _local_fail_reasons(eng, compiled: Compiled, out_node: np.ndarray, fail_counts, fail_pod) -> dict:
+    from .storage import StorageReplay
+    pod_class = compiled.pods["pod_class"]
+    todo = sorted(int(pod) for j, pod in enumerate(fail_pod) if j < len(fail_counts) and int(fail_counts[j][20]) > 0)[:MAX_GPU_FAIL_DETAIL]
+    if not todo:
+        return {}
+    codes = {pod: eng.dump_pod(pod)[2] for pod in todo}
+    rep = StorageReplay(compiled.storage, compiled.node_names)
+    out = {}
+    bound = iter(_bound_by_scheduler(compiled, out_node))
+    nxt = next(bound, None)
+    for pod in todo:
+        while nxt is not None and nxt[0] < pod:
+            rep.bind(int(pod_class[nxt[0]]), nxt[1])
+            nxt = next(bound, None)
+        cls = int(pod_class[pod])
+        out[pod] = [rep.reason(cls, g) for g in np.nonzero(codes[pod] & (1 << 20))[0].tolist()]
+    return out
+
+
+def _write_storage_annotations(compiled: Compiled, res: SimulateResult, out_node: np.ndarray) -> None:
+    """Bind rewrites simon/node-local-storage of the node it binds to (open-local.go:232-251); getClusterNodeStatus returns
+    the updated node, so NodeStatus.Node carries it (a copy: the caller's cluster objects stay as they were)."""
+    from .storage import StorageReplay
+    rep = StorageReplay(compiled.storage, compiled.node_names)
+    pod_class = compiled.pods["pod_class"]
+    for i, n in _bound_by_scheduler(compiled, out_node):
+        rep.bind(int(pod_class[i]), n)
+    for g in sorted(rep.touched):
+        ns = res.NodeStatus[compiled.node_orig_index[g]]
+        ns.Node = O.deep_copy(ns.Node)
+        O.meta(ns.Node)["annotations"] = dict(O.annotations_of(ns.Node), **{O.ANNO_NODE_LOCAL_STORAGE: rep.annotation(g)})
