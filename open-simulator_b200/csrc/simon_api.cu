@@ -208,6 +208,12 @@ struct simon_ctx {
     DevBuf<int64_t> d_vg_cap, d_vg_req0, d_vg_req, d_vol_size;
     DevBuf<uint8_t> d_class_local;
     DevBuf<uint32_t> d_vol_off;
+    std::vector<uint8_t> h_class_local;
+    // Open-Local devices (simon_devices_upload); allocated-slot masks [N], as uploaded and the current state
+    bool have_devices = false;
+    DevBuf<uint8_t> d_node_n_ssd, d_node_n_hdd;
+    DevBuf<int64_t> d_dev_cap, d_ssd_size, d_hdd_size;
+    DevBuf<uint32_t> d_ssd_off, d_hdd_off, d_dev_alloc0, d_dev_alloc;
 };
 
 namespace {
@@ -267,6 +273,9 @@ int reset_state(simon_ctx *ctx, ScenState &s) {
     // VG requested restarts from what the node annotations state
     if (&s == &ctx->st && ctx->have_storage)
         CU(cudaMemcpyAsync(ctx->d_vg_req.p, ctx->d_vg_req0.p, 8ull * ctx->V * N, cudaMemcpyDeviceToDevice, st));
+    // and the devices from what they state
+    if (&s == &ctx->st && ctx->have_devices)
+        CU(cudaMemcpyAsync(ctx->d_dev_alloc.p, ctx->d_dev_alloc0.p, 4ull * std::max(1u, N), cudaMemcpyDeviceToDevice, st));
     return SIMON_OK;
 }
 
@@ -305,6 +314,11 @@ void fill_params(simon_ctx *ctx, SkParams &P) {
         P.V = ctx->V; P.node_n_vg = ctx->d_node_n_vg.p; P.vg_name = ctx->d_vg_name.p; P.vg_cap = ctx->d_vg_cap.p;
         P.class_local = ctx->d_class_local.p; P.vol_off = ctx->d_vol_off.p; P.vol_size = ctx->d_vol_size.p; P.vol_vg = ctx->d_vol_vg.p;
         P.vg_req = ctx->d_vg_req.p; P.local_raw = ctx->d_local_raw.p;
+    }
+    if (ctx->have_devices) {
+        P.node_n_ssd = ctx->d_node_n_ssd.p; P.node_n_hdd = ctx->d_node_n_hdd.p; P.dev_cap = ctx->d_dev_cap.p;
+        P.ssd_off = ctx->d_ssd_off.p; P.ssd_size = ctx->d_ssd_size.p; P.hdd_off = ctx->d_hdd_off.p; P.hdd_size = ctx->d_hdd_size.p;
+        P.dev_alloc = ctx->d_dev_alloc.p;
     }
 }
 
@@ -621,6 +635,7 @@ int simon_snapshot_upload(simon_ctx *ctx, const simon_snapshot *s) {
     ctx->have_snap = true;
     ctx->have_pods = false;
     ctx->have_storage = false;
+    ctx->have_devices = false;
     return SIMON_OK;
 }
 
@@ -630,6 +645,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     CU(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     ctx->have_storage = false;          // the storage tables are per class: a new pod set needs its own upload
+    ctx->have_devices = false;
     ctx->n_classes = p->n_classes; ctx->n_pods = p->n_pods; ctx->n_counters = p->n_counters;
     // validate classes; derive limits
     uint32_t max_words = SCW_HDR_WORDS, emax = 0;
@@ -1047,6 +1063,7 @@ int simon_state_download_ext(simon_ctx *ctx, int64_t *req_scalar, int64_t *gpu_u
 int simon_storage_upload(simon_ctx *ctx, const simon_storage *sg) {
     if (!ctx || !sg) return SIMON_ERR_INVALID;
     if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_storage_upload before simon_pods_upload");
+    ctx->have_devices = false;          // device tables belong to the storage upload they followed
     const uint32_t N = ctx->N, V = sg->n_vgs, C = ctx->n_classes;
     if (sg->n_classes != C) return fail(ctx, SIMON_ERR_INVALID, "storage table has %u classes, the pod set %u", sg->n_classes, C);
     if (V > SIMON_MAX_VGS) return fail(ctx, SIMON_ERR_LIMIT, "more than %d VGs per node", SIMON_MAX_VGS);
@@ -1107,6 +1124,7 @@ int simon_storage_upload(simon_ctx *ctx, const simon_storage *sg) {
         CU(cudaStreamSynchronize(st));      // `mc` leaves scope
     }
     ctx->V = V;
+    ctx->h_class_local.assign(sg->class_local, sg->class_local + C);
     ctx->have_storage = true;
     int rc = reset_state(ctx, ctx->st);
     if (rc) return rc;
@@ -1119,6 +1137,70 @@ int simon_storage_state_download(simon_ctx *ctx, int64_t *vg_requested) {
     if (!ctx->have_storage) return fail(ctx, SIMON_ERR_STATE, "no storage uploaded");
     CU(cudaSetDevice(ctx->device));
     if (ctx->V && ctx->N) CU(cudaMemcpy(vg_requested, ctx->d_vg_req.p, 8ull * ctx->V * ctx->N, cudaMemcpyDeviceToHost));
+    return SIMON_OK;
+}
+
+int simon_devices_upload(simon_ctx *ctx, const simon_devices *dv) {
+    if (!ctx || !dv) return SIMON_ERR_INVALID;
+    if (!ctx->have_storage) return fail(ctx, SIMON_ERR_STATE, "simon_devices_upload before simon_storage_upload");
+    const uint32_t N = ctx->N, D = dv->n_slots, C = ctx->n_classes;
+    if (dv->n_classes != C) return fail(ctx, SIMON_ERR_INVALID, "device table has %u classes, the pod set %u", dv->n_classes, C);
+    if (D > SIMON_MAX_DEVS) return fail(ctx, SIMON_ERR_LIMIT, "more than %d devices per node", SIMON_MAX_DEVS);
+    if (!dv->node_n_ssd || !dv->node_n_hdd || !dv->dev_alloc || !dv->ssd_off || !dv->hdd_off || (D && N && !dv->dev_capacity))
+        return fail(ctx, SIMON_ERR_INVALID, "missing device column");
+    for (uint32_t g = 0; g < N; g++) {
+        const uint32_t ns = dv->node_n_ssd[g], nd = ns + dv->node_n_hdd[g];
+        if (nd > D) return fail(ctx, SIMON_ERR_INVALID, "node %u: %u devices in %u slots", g, nd, D);
+        if (dv->dev_alloc[g] >> nd) return fail(ctx, SIMON_ERR_INVALID, "node %u: allocated bit of an empty slot", g);
+        for (uint32_t s = 1; s < nd; s++)
+            if (s != ns && dv->dev_capacity[(size_t)s * N + g] < dv->dev_capacity[(size_t)(s - 1) * N + g])
+                return fail(ctx, SIMON_ERR_INVALID, "node %u: device slots of one media type not ascending by capacity", g);
+    }
+    const uint32_t *offs[2] = {dv->ssd_off, dv->hdd_off};
+    const int64_t *sizes[2] = {dv->ssd_size, dv->hdd_size};
+    for (int m = 0; m < 2; m++) {
+        if (offs[m][0] != 0) return fail(ctx, SIMON_ERR_INVALID, "device volume offsets must start at 0");
+        for (uint32_t c = 0; c < C; c++)
+            if (offs[m][c + 1] < offs[m][c]) return fail(ctx, SIMON_ERR_INVALID, "class %u: device volume offsets decrease", c);
+        const uint32_t n = C ? offs[m][C] : 0;
+        if (n && !sizes[m]) return fail(ctx, SIMON_ERR_INVALID, "missing device volume column");
+        for (uint32_t c = 0; c < C; c++)
+            for (uint32_t q = offs[m][c]; q < offs[m][c + 1]; q++) {
+                if (sizes[m][q] <= 0) return fail(ctx, SIMON_ERR_INVALID, "device volume %u: size must be > 0", q);
+                if (q > offs[m][c] && sizes[m][q] < sizes[m][q - 1]) return fail(ctx, SIMON_ERR_INVALID, "class %u: device volume sizes not ascending", c);
+            }
+    }
+    for (uint32_t c = 0; c < C; c++) {
+        const uint32_t n = (dv->ssd_off[c + 1] - dv->ssd_off[c]) + (dv->hdd_off[c + 1] - dv->hdd_off[c]);
+        if (n > SIMON_MAX_DEV_VOLS) return fail(ctx, SIMON_ERR_LIMIT, "class %u: more than %d device volumes", c, SIMON_MAX_DEV_VOLS);
+        if (n && !ctx->h_class_local[c]) return fail(ctx, SIMON_ERR_INVALID, "class %u: device volumes without the local flag", c);
+    }
+    CU(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    const size_t DN = std::max<size_t>(1, (size_t)D * N);
+    std::vector<int64_t> zero64(DN, 0);
+    CU(ctx->d_node_n_ssd.upload(dv->node_n_ssd, std::max(1u, N), st));
+    CU(ctx->d_node_n_hdd.upload(dv->node_n_hdd, std::max(1u, N), st));
+    CU(ctx->d_dev_cap.upload(D && N ? dv->dev_capacity : zero64.data(), DN, st));
+    CU(ctx->d_dev_alloc0.upload(dv->dev_alloc, std::max(1u, N), st));
+    CU(ctx->d_dev_alloc.alloc(std::max(1u, N)));
+    CU(ctx->d_ssd_off.upload(dv->ssd_off, C + 1, st));
+    CU(ctx->d_hdd_off.upload(dv->hdd_off, C + 1, st));
+    std::vector<int64_t> ss(dv->ssd_size, dv->ssd_size + (C ? dv->ssd_off[C] : 0)); ss.push_back(0);
+    std::vector<int64_t> hs(dv->hdd_size, dv->hdd_size + (C ? dv->hdd_off[C] : 0)); hs.push_back(0);
+    CU(ctx->d_ssd_size.upload(ss.data(), ss.size(), st)); CU(ctx->d_hdd_size.upload(hs.data(), hs.size(), st));
+    ctx->have_devices = true;
+    int rc = reset_state(ctx, ctx->st);
+    if (rc) return rc;
+    CU(cudaStreamSynchronize(st));      // `ss` / `hs` leave scope
+    return SIMON_OK;
+}
+
+int simon_devices_state_download(simon_ctx *ctx, uint32_t *alloc_mask) {
+    if (!ctx || !alloc_mask) return SIMON_ERR_INVALID;
+    if (!ctx->have_devices) return fail(ctx, SIMON_ERR_STATE, "no devices uploaded");
+    CU(cudaSetDevice(ctx->device));
+    if (ctx->N) CU(cudaMemcpy(alloc_mask, ctx->d_dev_alloc.p, 4ull * ctx->N, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 

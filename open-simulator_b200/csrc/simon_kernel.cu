@@ -147,53 +147,93 @@ __device__ __noinline__ int gpu_allocate(const SkParams &P, const SkScenario &SC
     return got == req_num ? got : 0;
 }
 
-// Open-Local LVM Filter / Score / Bind of class `cls` on node g (include/simon_gpu.h, simon_storage; ProcessLVMPVCPredicate
-// OL/scheduler/algorithm/algo/common.go:59-143, Binpack :574-619, ScoreLVM :660-692): the raw score, -1 if the node fails.
-// commit: add the PVCs to the VGs they were placed on (Bind, open-local.go:175-254).
+// Open-Local Filter / Score / Bind of class `cls` on node g (include/simon_gpu.h, simon_storage and simon_devices): the raw score
+// ScoreLVM + ScoreDevice, -1 if the node fails.  LVM: ProcessLVMPVCPredicate OL/scheduler/algorithm/algo/common.go:59-143, Binpack
+// :574-619, ScoreLVM :660-692.  Devices: ProcessDevicePVC :394-448, CheckExclusiveResourceMeetsPVCSize :290-350, ScoreDevice
+// :753-762.  commit: add the PVCs to the VGs they were placed on and mark the devices they took (Bind, open-local.go:175-254).
 __device__ __noinline__ int local_eval(const SkParams &P, uint32_t cls, uint32_t g, bool commit) {
     const int nv = P.node_n_vg[g];
     if (nv < 0) return -1;                                  // no simon/node-local-storage annotation
-    const uint32_t q0 = P.vol_off[cls], q1 = P.vol_off[cls + 1];
-    if (q0 == q1) return 0;                                 // no LVM PVC: ProcessLVMPVCPredicate does not run (open-local.go:76-81)
     const uint32_t N = P.N;
-    int64_t req[SIMON_MAX_VGS], used[SIMON_MAX_VGS];
-    #pragma unroll
-    for (int v = 0; v < SIMON_MAX_VGS; v++) { req[v] = v < nv ? P.vg_req[(uint64_t)v * N + g] : 0; used[v] = 0; }
-    #pragma unroll 1
-    for (uint32_t q = q0; q < q1; q++) {                    // PVCs whose class names a vgName come first
-        const int32_t id = P.vol_vg[q];
-        if (id < 0) continue;
-        int hit = -1;
+    int score = 0;
+    const uint32_t q0 = P.vol_off[cls], q1 = P.vol_off[cls + 1];
+    if (q0 < q1) {                                          // without LVM PVCs ProcessLVMPVCPredicate does not run (open-local.go:76-81)
+        int64_t req[SIMON_MAX_VGS], used[SIMON_MAX_VGS];
+        #pragma unroll
+        for (int v = 0; v < SIMON_MAX_VGS; v++) { req[v] = v < nv ? P.vg_req[(uint64_t)v * N + g] : 0; used[v] = 0; }
         #pragma unroll 1
-        for (int v = 0; v < nv; v++) if (P.vg_name[(uint64_t)v * N + g] == id) hit = v;
-        const int64_t sz = P.vol_size[q];
-        if (hit < 0 || P.vg_cap[(uint64_t)hit * N + g] - req[hit] < sz) return -1;
-        req[hit] += sz; used[hit] += sz;
-    }
-    if (nv == 0) return -1;                                 // NoAvailableVGError
-    #pragma unroll 1
-    for (uint32_t q = q0; q < q1; q++) {                    // the others: the VG of least free size that holds the PVC
-        if (P.vol_vg[q] >= 0) continue;
-        const int64_t sz = P.vol_size[q];
-        int best = -1;
-        int64_t bf = 0;
-        #pragma unroll 1
-        for (int v = 0; v < nv; v++) {
-            const int64_t fr = P.vg_cap[(uint64_t)v * N + g] - req[v];
-            if (fr >= sz && (best < 0 || fr < bf)) { best = v; bf = fr; }
+        for (uint32_t q = q0; q < q1; q++) {                // PVCs whose class names a vgName come first
+            const int32_t id = P.vol_vg[q];
+            if (id < 0) continue;
+            int hit = -1;
+            #pragma unroll 1
+            for (int v = 0; v < nv; v++) if (P.vg_name[(uint64_t)v * N + g] == id) hit = v;
+            const int64_t sz = P.vol_size[q];
+            if (hit < 0 || P.vg_cap[(uint64_t)hit * N + g] - req[hit] < sz) return -1;
+            req[hit] += sz; used[hit] += sz;
         }
-        if (best < 0) return -1;
-        req[best] += sz; used[best] += sz;
-    }
-    double sf = 0.0;
-    int cnt = 0;
-    #pragma unroll 1
-    for (int v = 0; v < nv; v++)
-        if (used[v] > 0) { sf += (double)used[v] / (double)P.vg_cap[(uint64_t)v * N + g]; cnt++; }
-    if (commit)
+        if (nv == 0) return -1;                             // NoAvailableVGError
         #pragma unroll 1
-        for (int v = 0; v < nv; v++) if (used[v] > 0) P.vg_req[(uint64_t)v * N + g] = req[v];
-    return cnt ? (int)f2i(sf / (double)cnt * 10.0) : 0;
+        for (uint32_t q = q0; q < q1; q++) {                // the others: the VG of least free size that holds the PVC
+            if (P.vol_vg[q] >= 0) continue;
+            const int64_t sz = P.vol_size[q];
+            int best = -1;
+            int64_t bf = 0;
+            #pragma unroll 1
+            for (int v = 0; v < nv; v++) {
+                const int64_t fr = P.vg_cap[(uint64_t)v * N + g] - req[v];
+                if (fr >= sz && (best < 0 || fr < bf)) { best = v; bf = fr; }
+            }
+            if (best < 0) return -1;
+            req[best] += sz; used[best] += sz;
+        }
+        double sf = 0.0;
+        int cnt = 0;
+        #pragma unroll 1
+        for (int v = 0; v < nv; v++)
+            if (used[v] > 0) { sf += (double)used[v] / (double)P.vg_cap[(uint64_t)v * N + g]; cnt++; }
+        if (commit)
+            #pragma unroll 1
+            for (int v = 0; v < nv; v++) if (used[v] > 0) P.vg_req[(uint64_t)v * N + g] = req[v];
+        score = cnt ? (int)f2i(sf / (double)cnt * 10.0) : 0;
+    }
+    if (P.dev_alloc) {
+        // SSD PVCs, then HDD PVCs, each ascending by size, walk the node's free slots of that media type ascending by capacity:
+        // a slot smaller than the current PVC is skipped, unless it is the last free one (the node fails); otherwise it takes
+        // the PVC.  Slots that run out before every PVC has one leave the node passing with fewer units (common.go:312-349).
+        const uint32_t alloc = P.dev_alloc[g];
+        const int n_ssd = P.node_n_ssd[g], n_dev = n_ssd + P.node_n_hdd[g];
+        uint32_t take = 0;
+        double df = 0.0;
+        int units = 0;
+        #pragma unroll 1
+        for (int m = 0; m < 2; m++) {
+            const uint32_t *off = m ? P.hdd_off : P.ssd_off;
+            const int64_t *size = m ? P.hdd_size : P.ssd_size;
+            uint32_t p = off[cls];
+            const uint32_t p1 = off[cls + 1];
+            if (p == p1) continue;
+            const int s0 = m ? n_ssd : 0, s1 = m ? n_dev : n_ssd;
+            const uint32_t fr = ((1u << s1) - 1u) & ~((1u << s0) - 1u) & ~alloc;
+            if ((uint32_t)__popc(fr) < p1 - p) return -1;  // fewer free devices than PVCs
+            const int last = 31 - __clz(fr);
+            #pragma unroll 1
+            for (int s = s0; s < s1 && p < p1; s++) {
+                if (!((fr >> s) & 1u)) continue;
+                const int64_t cap = P.dev_cap[(uint64_t)s * N + g], sz = size[p];
+                if (cap < sz) {
+                    if (s == last) return -1;
+                    continue;
+                }
+                take |= 1u << s; df += (double)sz / (double)cap; units++; p++;
+            }
+        }
+        if (units) {
+            score += (int)f2i(df / (double)units * 10.0);
+            if (commit) P.dev_alloc[g] = alloc | take;
+        }
+    }
+    return score;
 }
 
 // ClassState.cflags bits of classes that request Open-Local storage (simon_storage.class_local) and of classes with a GPU-share
@@ -1416,7 +1456,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                         }
                     }
                     if (SC.out_gpu) SC.out_gpu[i] = gpu_pack;
-                    if (C.cflags & CLS_LOCAL) local_eval(P, (uint32_t)cls, g, true);      // Bind: the VGs the Filter's choice took
+                    if (C.cflags & CLS_LOCAL) local_eval(P, (uint32_t)cls, g, true);      // Bind: the VGs and devices the Filter's choice took
                 }
                 const int64_t *inc = cw + cw[SCW_OFF_INC];
                 const uint32_t n_inc_list = (uint32_t)cw[SCW_N_INC];
@@ -1436,7 +1476,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                 __syncwarp();
             }
         }
-        if (C.cflags & (SK_CLS_GPU | CLS_LOCAL)) __syncthreads();      // the owner's next filter pass reads gpu_used / vg_req, written by the helper warp
+        if (C.cflags & (SK_CLS_GPU | CLS_LOCAL)) __syncthreads();      // the owner's next filter pass reads gpu_used / vg_req / dev_alloc, written by the helper warp
         // every thread folds the winner into its cached counter values (S.inc was built at the class change; the
         // reductions in between contain __syncthreads)
         {

@@ -120,6 +120,11 @@ struct SkParams {
     const uint32_t *vol_off;
     int64_t *vg_req;               // [V][N] VG requested (single-scenario state: scenario batches refuse storage)
     int32_t *local_raw;            // [N] the current decision's per-node verdict / raw score, then normalised score (scratch)
+    // Open-Local SSD / HDD devices (simon_devices); dev_alloc == nullptr: none uploaded
+    const uint8_t *node_n_ssd, *node_n_hdd;
+    const int64_t *dev_cap, *ssd_size, *hdd_size;
+    const uint32_t *ssd_off, *hdd_off;
+    uint32_t *dev_alloc;           // [N] bit s: slot s allocated (single-scenario state, like vg_req)
 };
 
 __host__ __device__ inline size_t sk_align(size_t x) { return (x + 15) & ~(size_t)15; }

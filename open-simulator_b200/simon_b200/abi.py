@@ -69,6 +69,22 @@ def marshal_storage(st):
     return s, keep
 
 
+class SimonDevices(C.Structure):
+    _fields_ = [("n_slots", C.c_uint32), ("n_classes", C.c_uint32),
+                ("node_n_ssd", C.c_void_p), ("node_n_hdd", C.c_void_p), ("dev_capacity", C.c_void_p), ("dev_alloc", C.c_void_p),
+                ("ssd_off", C.c_void_p), ("ssd_size", C.c_void_p), ("hdd_off", C.c_void_p), ("hdd_size", C.c_void_p)]
+
+
+def marshal_devices(st):
+    """storage.StorageTables compiled with devices=True -> (SimonDevices, arrays that must outlive the upload call)."""
+    keep = [np.ascontiguousarray(a, dtype=t) for a, t in (
+        (st.node_n_ssd, np.uint8), (st.node_n_hdd, np.uint8), (st.dev_capacity, np.int64), (st.dev_alloc, np.uint32),
+        (st.ssd_off, np.uint32), (st.ssd_size, np.int64), (st.hdd_off, np.uint32), (st.hdd_size, np.int64))]
+    keep = [a if a.size else np.zeros(1, a.dtype) for a in keep]
+    s = SimonDevices(st.n_dev_slots, len(st.class_local), *[a.ctypes.data for a in keep])
+    return s, keep
+
+
 MOVE_NOOP, MOVE_NOT_PLACED, MOVE_NOT_MOVABLE, MOVE_BAD_INDEX = 1 << 24, 1 << 25, 1 << 26, 1 << 27
 MOVE_GAIN_BIAS = 1000
 

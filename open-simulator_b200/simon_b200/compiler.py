@@ -423,15 +423,19 @@ class ExtraScorePlugin:
 
 def compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[ClusterContext] = None,
                     extra_log: int = 0, extra_plugins: Optional[List[ExtraScorePlugin]] = None,
-                    open_local: bool = False, storage_classes: Optional[List[Obj]] = None) -> Compiled:
+                    open_local: bool = False, storage_classes: Optional[List[Obj]] = None, local_devices: bool = False) -> Compiled:
     """open_local: run the Open-Local plugin's LVM part (storage.py) instead of refusing pods that request local storage;
+    local_devices: its exclusive SSD / HDD devices too (requires open_local);
     storage_classes: the StorageClasses of the cluster and the apps (their vgName / mediaType parameters)."""
+    if local_devices and not open_local:
+        raise ValueError("local_devices=True needs open_local=True: devices are part of the Open-Local plugin")
     with O.gc_paused():
         c = _compile_cluster(nodes, pods, ctx, extra_log, extra_plugins, open_local)
         if open_local:
             from .storage import StorageError, compile_storage
             try:
-                c.storage = compile_storage(c.node_objs, [ci.tmpl.pod for ci in c.classes], list(storage_classes or []))
+                c.storage = compile_storage(c.node_objs, [ci.tmpl.pod for ci in c.classes], list(storage_classes or []),
+                                            devices=local_devices)
             except StorageError as e:
                 raise CompileError(str(e)) from None
         return c

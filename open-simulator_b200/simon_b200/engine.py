@@ -24,7 +24,7 @@ EXPORTS = ["simon_gpu_version", "simon_ctx_create", "simon_ctx_destroy", "simon_
            "simon_moves_upload", "simon_moves_run", "simon_moves_replay", "simon_host_go118_sort",
            "simon_host_last_error", "simon_host_compile", "simon_host_plan_free", "simon_host_plan_columns", "simon_host_plan_describe",
            "simon_host_simulate", "simon_host_free", "simon_host_quantity_probe", "simon_host_plan_fit_error", "simon_host_capacity_search",
-           "simon_storage_upload", "simon_storage_state_download"]
+           "simon_storage_upload", "simon_storage_state_download", "simon_devices_upload", "simon_devices_state_download"]
 
 
 class EngineUnavailable(RuntimeError):
@@ -88,6 +88,10 @@ def lib():
         L.simon_storage_upload.argtypes = [C.c_void_p, C.c_void_p]
         L.simon_storage_state_download.restype = C.c_int
         L.simon_storage_state_download.argtypes = [C.c_void_p, C.c_void_p]
+        L.simon_devices_upload.restype = C.c_int
+        L.simon_devices_upload.argtypes = [C.c_void_p, C.c_void_p]
+        L.simon_devices_state_download.restype = C.c_int
+        L.simon_devices_state_download.argtypes = [C.c_void_p, C.c_void_p]
     except AttributeError:
         if not os.environ.get("SIMON_GPU_LIB"):       # an experiment library may lack the newer entry points; the shipped one may not
             raise
@@ -117,6 +121,9 @@ class Engine:
         if getattr(compiled, "storage", None) is not None:      # Open-Local LVM volumes (compile_cluster(open_local=True))
             self.storage, keep = abi.marshal_storage(compiled.storage)
             self._check(L.simon_storage_upload(self.h, C.byref(self.storage)))
+            if compiled.storage.devices:                        # SSD / HDD devices (compile_cluster(local_devices=True))
+                self.devices, keep = abi.marshal_devices(compiled.storage)
+                self._check(L.simon_devices_upload(self.h, C.byref(self.devices)))
 
     def _check(self, rc: int):
         if rc != 0:
@@ -205,6 +212,12 @@ class Engine:
         a = np.zeros(max(V * N, 1), np.int64)
         self._check(lib().simon_storage_state_download(self.h, a.ctypes.data))
         return a[:V * N].reshape(V, N)
+
+    def device_state(self) -> np.ndarray:
+        """Open-Local allocated device slots after scheduling, [N] masks (bit s: slot s of storage.StorageTables)."""
+        a = np.zeros(max(self.c.n_nodes, 1), np.uint32)
+        self._check(lib().simon_devices_state_download(self.h, a.ctypes.data))
+        return a[:self.c.n_nodes]
 
     def gpu_slots(self, first: int = 0, count: Optional[int] = None):
         """GPU-share Reserve results: per pod a list of device ids (one per GPU slot, ascending), [] if none."""

@@ -59,6 +59,7 @@ class SimulatorOptions:
     device: int = 0
     record_scores: bool = False
     openLocal: bool = False
+    openLocalDevices: bool = False
 
 
 Option = Callable[[SimulatorOptions], None]
@@ -85,10 +86,14 @@ def WithDevice(device: int) -> Option:
     return lambda o: setattr(o, "device", device)
 
 
-def WithOpenLocal() -> Option:
+def WithOpenLocal(devices: bool = False) -> Option:
     """Run the Open-Local plugin's LVM volumes (pkg/simulator/plugin/open-local.go; simon_b200/storage.py for what is covered
-    and the tie-breaking it fixes) instead of refusing pods that request local storage."""
-    return lambda o: setattr(o, "openLocal", True)
+    and the tie-breaking it fixes) instead of refusing pods that request local storage; devices: its exclusive SSD / HDD
+    device volumes too."""
+    def opt(o):
+        o.openLocal = True
+        o.openLocalDevices = devices
+    return opt
 
 
 @dataclass
@@ -267,7 +272,7 @@ def _simulate(cluster: ResourceTypes, apps: List[AppResource], *opts: Option) ->
     t0 = time.perf_counter()
     storage_classes = list(cluster.StorageClasss) + [sc for a in apps for sc in a.Resource.StorageClasss] if options.openLocal else None
     compiled = compile_cluster(p.nodes, p.pods, p.ctx, extra_plugins=extra_plugins or None, open_local=options.openLocal,
-                               storage_classes=storage_classes)
+                               storage_classes=storage_classes, local_devices=options.openLocalDevices)
     tm["compile_s"] = time.perf_counter() - t0
     gpu_fail_nodes = {}
     t0 = time.perf_counter()
@@ -286,7 +291,7 @@ def _simulate(cluster: ResourceTypes, apps: List[AppResource], *opts: Option) ->
             gpu_fail_nodes[pod] = [compiled.node_names[g] for g in np.nonzero(code & gpu_bit)[0]]
         local_fail_reasons = {}
         if compiled.storage is not None:
-            # Open-Local's messages name VG sizes as of the pod's turn: the node list comes from the verdict dump (a bounded number
+            # Open-Local's messages name VG sizes and free devices as of the pod's turn: the node list comes from the verdict dump (a bounded number
             # of pods, like GPU-share's), the sizes from the replay of Bind in placement order
             local_fail_reasons = _local_fail_reasons(eng, compiled, out_node, fail_counts, fail_pod)
         tm["gpu_fail_detail_s"] = time.perf_counter() - t0

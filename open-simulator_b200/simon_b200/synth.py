@@ -246,6 +246,49 @@ def make_c4(n_nodes: int = 2000, n_workloads: int = 50, replicas: int = 100, fil
     return cluster, [app], specs
 
 
+def make_open_local(n_nodes: int = 10000, n_workloads: int = 200, replicas: int = 250, seed_no: int = 6
+                    ) -> Tuple[ResourceTypes, List[AppResource]]:
+    """Open-Local storage: ~60 % of the nodes carry the simon/node-local-storage annotation with 1-4 VGs and 0-8 SSD / HDD
+    devices (~5 % of them allocated); the Deployments request no volume, LVM volumes only, devices only, or both, a quarter
+    each.  The two device StorageClasses are in the cluster."""
+    import json
+    from .objects import ANNO_NODE_LOCAL_STORAGE, ANNO_POD_LOCAL_STORAGE
+    gi = 1 << 30
+    rng = SplitMix64(SEED_BASE + seed_no)
+    cluster = ResourceTypes()
+    for m in ("ssd", "hdd"):
+        cluster.StorageClasss.append({"apiVersion": "storage.k8s.io/v1", "kind": "StorageClass",
+                                      "metadata": {"name": f"open-local-device-{m}"}, "parameters": {"mediaType": m}})
+    for i in range(n_nodes):
+        n = _node(f"node-{i:05d}", rng.pick(CPU_SHAPES), f"zone-{i % 16:02d}", "", 1000)
+        if rng.chance(60):
+            vgs = [{"name": f"pool{v}", "capacity": str(rng.pick([100, 200, 500, 1000]) * gi),
+                    "requested": str(rng.below(5) * 10 * gi)} for v in range(1 + rng.below(4))]
+            devs = [{"name": f"/dev/vd{k}", "device": f"/dev/vd{k}", "capacity": str(rng.pick([100, 200, 400, 800, 1600]) * gi),
+                     "mediaType": rng.pick(["ssd", "hdd"]), "isAllocated": "true" if rng.chance(5) else "false"}
+                    for k in range(rng.below(9))]
+            n["metadata"]["annotations"] = {ANNO_NODE_LOCAL_STORAGE: json.dumps({"vgs": vgs, "devices": devs})}
+        cluster.Nodes.append(n)
+    app = AppResource("open-local", ResourceTypes())
+    for w in range(n_workloads):
+        name = f"ol-{w:04d}"
+        d = _deployment(name, "default", replicas, {"app": name}, _log_uniform(rng, 100, 2000, 50), _log_uniform(rng, 128, 4096, 64))
+        kind = w % 4          # 0: no volume, 1: LVM, 2: devices, 3: both
+        vols = []
+        if kind in (1, 3):
+            vols += [{"size": str(_log_uniform(rng, 5, 100, 5) * gi), "kind": "LVM", "scName": "open-local-lvm"}
+                     for _ in range(1 + rng.below(3))]
+        if kind in (2, 3):
+            for _ in range(1 + rng.below(2)):
+                m = rng.pick(["SSD", "HDD"])
+                vols.append({"size": str(rng.pick([50, 100, 200, 400, 1000]) * gi), "kind": m,
+                             "scName": f"open-local-device-{m.lower()}"})
+        if vols:
+            d["spec"]["template"]["metadata"]["annotations"] = {ANNO_POD_LOCAL_STORAGE: json.dumps({"volumes": vols})}
+        app.Resource.Deployments.append(d)
+    return cluster, [app]
+
+
 def make_mix(seed_no: int = 100, n_nodes: int = 40, n_workloads: int = 30, max_replicas: int = 6, with_images: bool = False):
     """Small clusters that exercise EVERY predicate / score input the path knows, in random combinations: unschedulable
     nodes, NoSchedule / NoExecute / PreferNoSchedule taints and all toleration shapes, nodeSelector, required and
