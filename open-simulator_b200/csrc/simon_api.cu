@@ -115,7 +115,50 @@ struct ScenBatch {
     DevBuf<simon_scenario_result> results;
     std::vector<uint32_t> h_order;
     std::vector<int32_t> h_rank;
+    // Open-Local state of simon_scenarios_run_local, one slice per scenario: VG requested [n][V][N], allocated device slots [n][N],
+    // the per-decision raw-score scratch [n][N] (clusters of a batch run concurrently: a shared one would be a race)
+    DevBuf<int64_t> vg_req;
+    DevBuf<uint32_t> dev_alloc;
+    DevBuf<int32_t> local_raw;
+    DevBuf<simon_scenario_local_result> local_results;
+    uint32_t n_storage = 0;     // scenarios of the last storage batch whose state the slices hold (0: none since the last upload)
 };
+
+// dst[i][0 .. len) = src[0 .. len) for every i < n: the scenarios of a batch start from the uploaded Open-Local state
+template <typename T>
+__global__ void simon_bcast(const T *__restrict__ src, size_t len, uint32_t n, T *__restrict__ dst) {
+    const size_t total = len * n;
+    for (size_t q = blockIdx.x * (size_t)blockDim.x + threadIdx.x; q < total; q += (size_t)gridDim.x * blockDim.x) dst[q] = src[q % len];
+}
+
+// satisfyResourceSetting's VG sums (pkg/apply/apply.go:746-755) per scenario: requested and capacity of every VG of the active nodes
+// that carry the simon/node-local-storage annotation, on the scenario's own VG state
+__global__ void simon_scen_reduce_local(const SkScenario *scen, const int32_t *node_n_vg, const int64_t *vg_cap, const int64_t *vg_req,
+                                        uint64_t vg_stride, uint32_t N, simon_scenario_local_result *out) {
+    const SkScenario &sc = scen[blockIdx.x];
+    const int64_t *req = vg_req + (uint64_t)blockIdx.x * vg_stride;
+    long long v[2] = {0, 0};
+    for (uint32_t r = threadIdx.x; r < sc.n_active; r += blockDim.x) {
+        const uint32_t g = sc.order ? sc.order[r] : r;
+        for (int32_t a = 0; a < node_n_vg[g]; a++) { v[0] += req[(uint64_t)a * N + g]; v[1] += vg_cap[(uint64_t)a * N + g]; }
+    }
+    __shared__ long long part[2][8];
+#pragma unroll
+    for (int q = 0; q < 2; q++) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v[q] += __shfl_down_sync(0xffffffffu, v[q], o);
+        if ((threadIdx.x & 31) == 0) part[q][threadIdx.x >> 5] = v[q];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        simon_scenario_local_result o;
+        long long t[2] = {0, 0};
+        for (int q = 0; q < 2; q++)
+            for (unsigned w = 0; w < (blockDim.x + 31) / 32; w++) t[q] += part[q][w];
+        o.vg_requested = t[0]; o.vg_capacity = t[1]; o.reserved = 0;
+        out[blockIdx.x] = o;
+    }
+}
 
 // satisfyResourceSetting's sums (pkg/apply/apply.go:747-757) per scenario over its active nodes, plus the scenario's counters
 __global__ void simon_scen_reduce(const SkScenario *scen, const int64_t *alloc_mcpu, const int64_t *alloc_mem, simon_scenario_result *out) {
@@ -341,6 +384,14 @@ sk_kernel_fn pick_kernel(uint32_t TPB, uint32_t npt, bool prof) {
     return npt == 1 ? simon_place_kernel_256_1 : npt == 2 ? simon_place_kernel_256_2 : npt == 3 ? simon_place_kernel_256_3 : npt == 4 ? simon_place_kernel_256_4 : simon_place_kernel_256_0;
 }
 
+// the variant launch() runs for this shape, which is what the geometry must be sized for: with Open-Local storage uploaded the
+// local variants (more registers than the plain ones), else pick_kernel's
+sk_kernel_fn launch_kernel(const simon_ctx *ctx, uint32_t TPB, uint32_t npt) {
+    if (!ctx->have_storage) return pick_kernel(TPB, npt, false);
+    if (TPB > SIMON_MAX_TPB) return nullptr;
+    return TPB <= 256 ? simon_local_kernel_256 : TPB <= 320 ? simon_local_kernel_320 : simon_local_kernel_384;
+}
+
 // clusters of `cs` CTAs x `t` threads with `smem` bytes each that the device holds at once (GPC boundaries included)
 int max_active_clusters(sk_kernel_fn fn, uint32_t cs, uint32_t t, size_t smem) {
     if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return 0; }
@@ -395,7 +446,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
             if (npt > 64) continue;
             const size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs);
             if (b > (size_t)max_smem) continue;
-            sk_kernel_fn fn = pick_kernel(t, npt, false);
+            sk_kernel_fn fn = launch_kernel(ctx, t, npt);
             if (!fn) continue;
             const int active = max_active_clusters(fn, cs, t, b);
             if (active <= 0) continue;
@@ -454,7 +505,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
             if (n384 < npt_p) { t_p = 384; npt_p = n384; }
         }
         const size_t b = sk_smem_bytes(npt_p * t_p, ctx->T, ctx->emax, ctx->max_blob_words, cs_p);
-        if (npt_p <= 64 && b <= (size_t)max_smem && resident(pick_kernel(t_p, npt_p, false), cs_p, t_p, b)) {
+        if (npt_p <= 64 && b <= (size_t)max_smem && resident(launch_kernel(ctx, t_p, npt_p), cs_p, t_p, b)) {
             CS = cs_p; TPB = t_p; NPT = npt_p; smem = b; return SIMON_OK;
         }
     }
@@ -475,7 +526,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
             }
             if (t > SIMON_MAX_TPB) return fail(ctx, SIMON_ERR_LIMIT, "threads per CTA must be <= %u (got %u)", SIMON_MAX_TPB, t);
             size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs);
-            if (b <= (size_t)max_smem && (want_cs || resident(pick_kernel(t, npt, false), cs, t, b))) {
+            if (b <= (size_t)max_smem && (want_cs || resident(launch_kernel(ctx, t, npt), cs, t, b))) {
                 CS = cs; TPB = t; NPT = npt; smem = b; return SIMON_OK;
             }
             if (want_t) break;
@@ -487,7 +538,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
         const uint32_t cs = 16, t = 320;
         const uint32_t npt = (n_active + cs * t - 1) / (cs * t);
         const size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs, false);
-        if (npt <= 64 && b <= (size_t)max_smem && resident(simon_place_kernel_big, cs, t, b)) {
+        if (npt <= 64 && b <= (size_t)max_smem && resident(ctx->have_storage ? simon_local_kernel_big : simon_place_kernel_big, cs, t, b)) {
             CS = cs; TPB = t; NPT = npt; smem = b;
             ctx->big = true;
             ctx->gnode_stride = (sk_node_bytes(npt * t, ctx->T, ctx->emax) + 255) & ~(size_t)255;
@@ -636,6 +687,7 @@ int simon_snapshot_upload(simon_ctx *ctx, const simon_snapshot *s) {
     ctx->have_pods = false;
     ctx->have_storage = false;
     ctx->have_devices = false;
+    if (ctx->batch) ctx->batch->n_storage = 0;
     return SIMON_OK;
 }
 
@@ -646,6 +698,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     cudaStream_t st = ctx->stream;
     ctx->have_storage = false;          // the storage tables are per class: a new pod set needs its own upload
     ctx->have_devices = false;
+    if (ctx->batch) ctx->batch->n_storage = 0;
     ctx->n_classes = p->n_classes; ctx->n_pods = p->n_pods; ctx->n_counters = p->n_counters;
     // validate classes; derive limits
     uint32_t max_words = SCW_HDR_WORDS, emax = 0;
@@ -937,10 +990,9 @@ int simon_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *req_mem, in
     return SIMON_OK;
 }
 
-int simon_scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, simon_scenario_result *out, int32_t *out_node) {
-    if (!ctx || !scen || !out) return SIMON_ERR_INVALID;
-    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_scenarios_run before uploads");
-    if (ctx->have_storage) return fail(ctx, SIMON_ERR_LIMIT, "scenario batches do not carry Open-Local storage state yet: use simon_schedule");
+// simon_scenarios_run and simon_scenarios_run_local (out_local != nullptr: each scenario carries its own Open-Local state)
+static int scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, simon_scenario_result *out,
+                         simon_scenario_local_result *out_local, int32_t *out_node) {
     CU(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     if (n == 0) return SIMON_OK;
@@ -948,6 +1000,8 @@ int simon_scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, 
     const size_t cntw = std::max<uint64_t>(1, ctx->cnt_words), nct = std::max(1u, ctx->n_counters), ncl = std::max(1u, ctx->n_classes);
     if (!ctx->batch) { ctx->batch = new (std::nothrow) ScenBatch(); if (!ctx->batch) return SIMON_ERR_NOMEM; }
     ScenBatch &B = *ctx->batch;
+    const bool local = out_local != nullptr;
+    if (local) B.n_storage = 0;         // the slices are overwritten below
     // ---- node lists: validated on the host, uploaded in ONE copy each (scenario order and its inverse) ----
     uint32_t max_active = 0;
     B.h_order.assign((size_t)n * N1, 0u);
@@ -990,6 +1044,22 @@ int simon_scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, 
     // call (another node list!); fbits are only read under a valid summary record
     CU(cudaMemsetAsync(B.csum.p, 0, 8ull * n * ncl * SK_CSUM_W, st)); CU(cudaMemsetAsync(B.ocache.p, 0, 8ull * n * ncl * N1, st));
     CU(cudaMemsetAsync(B.counters.p, 0, 8ull * n, st)); CU(cudaMemsetAsync(B.clk.p, 0, 16ull * n, st));
+    // Open-Local: every scenario starts from the uploaded VG requested values and device masks, one broadcast per column; the
+    // single-scenario state (d_vg_req, d_dev_alloc) is not touched
+    const size_t VN = std::max<size_t>(1, (size_t)ctx->V * N);
+    if (local) {
+        int sms = 132;
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
+        const uint32_t cap = (uint32_t)sms * 8;
+        CU(B.vg_req.alloc((size_t)n * VN)); CU(B.local_raw.alloc((size_t)n * N1)); CU(B.local_results.alloc(n));
+        simon_bcast<<<(uint32_t)std::min<size_t>(((size_t)n * VN + 255) / 256, cap), 256, 0, st>>>(ctx->d_vg_req0.p, VN, n, B.vg_req.p);
+        CU(cudaGetLastError());
+        if (ctx->have_devices) {
+            CU(B.dev_alloc.alloc((size_t)n * N1));
+            simon_bcast<<<(uint32_t)std::min<size_t>(((size_t)n * N1 + 255) / 256, cap), 256, 0, st>>>(ctx->d_dev_alloc0.p, N1, n, B.dev_alloc.p);
+            CU(cudaGetLastError());
+        }
+    }
     std::vector<SkScenario> h(n);
     for (uint32_t i = 0; i < n; i++) {
         SkScenario &o = h[i];
@@ -1016,16 +1086,55 @@ int simon_scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, 
     SkParams Pm;
     fill_params(ctx, Pm);
     Pm.first = 0; Pm.count = ctx->n_pods; Pm.max_fail = 0; Pm.npt = NPT; Pm.scen = ctx->d_scen.p;
+    if (local) {
+        Pm.vg_req = B.vg_req.p; Pm.local_raw = B.local_raw.p; Pm.vg_req_stride = VN; Pm.node_stride = N1;
+        if (ctx->have_devices) Pm.dev_alloc = B.dev_alloc.p;
+    }
     rc = launch(ctx, Pm, n, CS, TPB, smem);
     if (rc) return rc;
     // per-scenario sums over the active nodes on the device; ONE copy of the result structs comes back
     simon_scen_reduce<<<n, 256, 0, st>>>(ctx->d_scen.p, ctx->d_alloc_mcpu.p, ctx->d_alloc_mem.p, B.results.p);
     CU(cudaGetLastError());
+    if (local) {
+        simon_scen_reduce_local<<<n, 256, 0, st>>>(ctx->d_scen.p, ctx->d_node_n_vg.p, ctx->d_vg_cap.p, B.vg_req.p, VN, N, B.local_results.p);
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(out_local, B.local_results.p, sizeof(simon_scenario_local_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    }
     CU(cudaMemcpyAsync(out, B.results.p, sizeof(simon_scenario_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
     if (out_node) CU(cudaMemcpyAsync(out_node, B.out_node.p, 4ull * n * P, cudaMemcpyDeviceToHost, st));
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    if (local) B.n_storage = n;
+    return SIMON_OK;
+}
+
+int simon_scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, simon_scenario_result *out, int32_t *out_node) {
+    if (!ctx || !scen || !out) return SIMON_ERR_INVALID;
+    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_scenarios_run before uploads");
+    if (ctx->have_storage) return fail(ctx, SIMON_ERR_LIMIT, "scenario batches with Open-Local storage uploaded: use simon_scenarios_run_local");
+    return scenarios_run(ctx, scen, n, out, nullptr, out_node);
+}
+
+int simon_scenarios_run_local(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, simon_scenario_result *out,
+                              simon_scenario_local_result *out_local, int32_t *out_node) {
+    if (!ctx || !scen || !out || !out_local) return SIMON_ERR_INVALID;
+    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_scenarios_run_local before uploads");
+    if (!ctx->have_storage) return fail(ctx, SIMON_ERR_STATE, "simon_scenarios_run_local before simon_storage_upload");
+    return scenarios_run(ctx, scen, n, out, out_local, out_node);
+}
+
+int simon_scenarios_storage_download(simon_ctx *ctx, uint32_t scenario, int64_t *vg_requested, uint32_t *dev_alloc) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->batch || !ctx->batch->n_storage) return fail(ctx, SIMON_ERR_STATE, "no simon_scenarios_run_local batch since the last upload");
+    const ScenBatch &B = *ctx->batch;
+    if (scenario >= B.n_storage) return fail(ctx, SIMON_ERR_INVALID, "scenario %u of a batch of %u", scenario, B.n_storage);
+    if (dev_alloc && !ctx->have_devices) return fail(ctx, SIMON_ERR_STATE, "no devices uploaded");
+    CU(cudaSetDevice(ctx->device));
+    const uint32_t N = ctx->N, N1 = std::max(1u, N);
+    const size_t VN = std::max<size_t>(1, (size_t)ctx->V * N);
+    if (vg_requested && ctx->V && N) CU(cudaMemcpy(vg_requested, B.vg_req.p + (size_t)scenario * VN, 8ull * ctx->V * N, cudaMemcpyDeviceToHost));
+    if (dev_alloc && N) CU(cudaMemcpy(dev_alloc, B.dev_alloc.p + (size_t)scenario * N1, 4ull * N, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
@@ -1064,6 +1173,7 @@ int simon_storage_upload(simon_ctx *ctx, const simon_storage *sg) {
     if (!ctx || !sg) return SIMON_ERR_INVALID;
     if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_storage_upload before simon_pods_upload");
     ctx->have_devices = false;          // device tables belong to the storage upload they followed
+    if (ctx->batch) ctx->batch->n_storage = 0;      // and so does the state of the last storage batch
     const uint32_t N = ctx->N, V = sg->n_vgs, C = ctx->n_classes;
     if (sg->n_classes != C) return fail(ctx, SIMON_ERR_INVALID, "storage table has %u classes, the pod set %u", sg->n_classes, C);
     if (V > SIMON_MAX_VGS) return fail(ctx, SIMON_ERR_LIMIT, "more than %d VGs per node", SIMON_MAX_VGS);
@@ -1143,6 +1253,7 @@ int simon_storage_state_download(simon_ctx *ctx, int64_t *vg_requested) {
 int simon_devices_upload(simon_ctx *ctx, const simon_devices *dv) {
     if (!ctx || !dv) return SIMON_ERR_INVALID;
     if (!ctx->have_storage) return fail(ctx, SIMON_ERR_STATE, "simon_devices_upload before simon_storage_upload");
+    if (ctx->batch) ctx->batch->n_storage = 0;      // the last storage batch ran on the device tables this upload replaces
     const uint32_t N = ctx->N, D = dv->n_slots, C = ctx->n_classes;
     if (dv->n_classes != C) return fail(ctx, SIMON_ERR_INVALID, "device table has %u classes, the pod set %u", dv->n_classes, C);
     if (D > SIMON_MAX_DEVS) return fail(ctx, SIMON_ERR_LIMIT, "more than %d devices per node", SIMON_MAX_DEVS);

@@ -151,6 +151,7 @@ __device__ __noinline__ int gpu_allocate(const SkParams &P, const SkScenario &SC
 // ScoreLVM + ScoreDevice, -1 if the node fails.  LVM: ProcessLVMPVCPredicate OL/scheduler/algorithm/algo/common.go:59-143, Binpack
 // :574-619, ScoreLVM :660-692.  Devices: ProcessDevicePVC :394-448, CheckExclusiveResourceMeetsPVCSize :290-350, ScoreDevice
 // :753-762.  commit: add the PVCs to the VGs they were placed on and mark the devices they took (Bind, open-local.go:175-254).
+// The VG and device state is this cluster's scenario's (sk_slice).
 __device__ __noinline__ int local_eval(const SkParams &P, uint32_t cls, uint32_t g, bool commit) {
     const int nv = P.node_n_vg[g];
     if (nv < 0) return -1;                                  // no simon/node-local-storage annotation
@@ -158,9 +159,10 @@ __device__ __noinline__ int local_eval(const SkParams &P, uint32_t cls, uint32_t
     int score = 0;
     const uint32_t q0 = P.vol_off[cls], q1 = P.vol_off[cls + 1];
     if (q0 < q1) {                                          // without LVM PVCs ProcessLVMPVCPredicate does not run (open-local.go:76-81)
+        int64_t *const vg_req = sk_slice(P.vg_req, P.vg_req_stride);
         int64_t req[SIMON_MAX_VGS], used[SIMON_MAX_VGS];
         #pragma unroll
-        for (int v = 0; v < SIMON_MAX_VGS; v++) { req[v] = v < nv ? P.vg_req[(uint64_t)v * N + g] : 0; used[v] = 0; }
+        for (int v = 0; v < SIMON_MAX_VGS; v++) { req[v] = v < nv ? vg_req[(uint64_t)v * N + g] : 0; used[v] = 0; }
         #pragma unroll 1
         for (uint32_t q = q0; q < q1; q++) {                // PVCs whose class names a vgName come first
             const int32_t id = P.vol_vg[q];
@@ -194,14 +196,15 @@ __device__ __noinline__ int local_eval(const SkParams &P, uint32_t cls, uint32_t
             if (used[v] > 0) { sf += (double)used[v] / (double)P.vg_cap[(uint64_t)v * N + g]; cnt++; }
         if (commit)
             #pragma unroll 1
-            for (int v = 0; v < nv; v++) if (used[v] > 0) P.vg_req[(uint64_t)v * N + g] = req[v];
+            for (int v = 0; v < nv; v++) if (used[v] > 0) vg_req[(uint64_t)v * N + g] = req[v];
         score = cnt ? (int)f2i(sf / (double)cnt * 10.0) : 0;
     }
     if (P.dev_alloc) {
         // SSD PVCs, then HDD PVCs, each ascending by size, walk the node's free slots of that media type ascending by capacity:
         // a slot smaller than the current PVC is skipped, unless it is the last free one (the node fails); otherwise it takes
         // the PVC.  Slots that run out before every PVC has one leave the node passing with fewer units (common.go:312-349).
-        const uint32_t alloc = P.dev_alloc[g];
+        uint32_t *const dev_alloc = sk_slice(P.dev_alloc, P.node_stride);
+        const uint32_t alloc = dev_alloc[g];
         const int n_ssd = P.node_n_ssd[g], n_dev = n_ssd + P.node_n_hdd[g];
         uint32_t take = 0;
         double df = 0.0;
@@ -230,7 +233,7 @@ __device__ __noinline__ int local_eval(const SkParams &P, uint32_t cls, uint32_t
         }
         if (units) {
             score += (int)f2i(df / (double)units * 10.0);
-            if (commit) P.dev_alloc[g] = alloc | take;
+            if (commit) dev_alloc[g] = alloc | take;
         }
     }
     return score;
@@ -449,7 +452,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             if (DOM(ENT(ER_T, e), idx) >= 0 && VAL(e, idx) > 0) return 1u << SFC_IPA_EXIST;
         if (C.cflags & (CLS_LOCAL | SK_CLS_GPU)) {
             uint32_t g = (uint32_t)A32(B_NODE_G, idx);
-            if ((C.cflags & CLS_LOCAL) && P.local_raw[g] < 0) return 1u << SFC_LOCAL;
+            if ((C.cflags & CLS_LOCAL) && sk_slice(P.local_raw, P.node_stride)[g] < 0) return 1u << SFC_LOCAL;
             if (C.cflags & SK_CLS_GPU) {
                 int slots[64];
                 int64_t total = P.gpu_total_mem ? P.gpu_total_mem[g] : 0;
@@ -1069,7 +1072,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                 uint32_t idx = s * TPB + tid;
                 if (!(A8(C_NFLAGS, idx) & NF_VALID)) continue;
                 const uint32_t g = (uint32_t)A32(B_NODE_G, idx);
-                P.local_raw[g] = local_eval(P, (uint32_t)cls, g, false);
+                sk_slice(P.local_raw, P.node_stride)[g] = local_eval(P, (uint32_t)cls, g, false);
             }
         }
         TICK(3);
@@ -1296,7 +1299,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             for (uint32_t s = 0; s < NPT; s++) {
                 uint32_t idx = s * TPB + tid;
                 if (!(A8(C_NFLAGS, idx) & NF_FEASIBLE)) continue;
-                const uint32_t e = w_enc(P.local_raw[(uint32_t)A32(B_NODE_G, idx)]);
+                const uint32_t e = w_enc(sk_slice(P.local_raw, P.node_stride)[(uint32_t)A32(B_NODE_G, idx)]);
                 lv[0] = e < lv[0] ? e : lv[0];
                 lv[1] = e > lv[1] ? e : lv[1];
             }
@@ -1306,7 +1309,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             for (uint32_t s = 0; s < NPT; s++) {
                 uint32_t idx = s * TPB + tid;
                 if (!(A8(C_NFLAGS, idx) & NF_FEASIBLE)) continue;
-                int32_t *x = P.local_raw + (uint32_t)A32(B_NODE_G, idx);
+                int32_t *x = sk_slice(P.local_raw, P.node_stride) + (uint32_t)A32(B_NODE_G, idx);
                 *x = range == 0 ? 0 : (*x - lo) * 100 / range;
                 A32(B_SNORM, idx) += *x;
             }
@@ -1384,7 +1387,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             #pragma unroll 1
             for (uint32_t s = 0; s < NPT; s++) {
                 uint32_t idx = s * TPB + tid;
-                if (A8(C_NFLAGS, idx) & NF_FEASIBLE) A32(B_SNORM, idx) -= P.local_raw[(uint32_t)A32(B_NODE_G, idx)];
+                if (A8(C_NFLAGS, idx) & NF_FEASIBLE) A32(B_SNORM, idx) -= sk_slice(P.local_raw, P.node_stride)[(uint32_t)A32(B_NODE_G, idx)];
             }
         }
         TICK(7);

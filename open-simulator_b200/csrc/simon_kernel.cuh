@@ -118,14 +118,27 @@ struct SkParams {
     const int64_t *vg_cap, *vol_size;
     const uint8_t *class_local;
     const uint32_t *vol_off;
-    int64_t *vg_req;               // [V][N] VG requested (single-scenario state: scenario batches refuse storage)
+    int64_t *vg_req;               // [V][N] VG requested
     int32_t *local_raw;            // [N] the current decision's per-node verdict / raw score, then normalised score (scratch)
     // Open-Local SSD / HDD devices (simon_devices); dev_alloc == nullptr: none uploaded
     const uint8_t *node_n_ssd, *node_n_hdd;
     const int64_t *dev_cap, *ssd_size, *hdd_size;
     const uint32_t *ssd_off, *hdd_off;
-    uint32_t *dev_alloc;           // [N] bit s: slot s allocated (single-scenario state, like vg_req)
+    uint32_t *dev_alloc;           // [N] bit s: slot s allocated
+    // vg_req, local_raw and dev_alloc hold one slice per cluster of the launch (scenario batches), these many elements apart;
+    // 0: the launch has one scenario, the single-scenario state
+    uint64_t vg_req_stride, node_stride;
 };
+
+// the index of this thread-block cluster in the (1-D) grid: the scenario of the launch (blockIdx.x / cluster size)
+__device__ __forceinline__ uint32_t sk_cluster_id() {
+    uint32_t r;
+    asm("mov.u32 %0, %%clusterid.x;" : "=r"(r));
+    return r;
+}
+// this cluster's slice of a per-scenario Open-Local state column (SkParams::vg_req_stride / node_stride)
+template <typename T>
+__device__ __forceinline__ T *sk_slice(T *base, uint64_t stride) { return base + (uint64_t)sk_cluster_id() * stride; }
 
 __host__ __device__ inline size_t sk_align(size_t x) { return (x + 15) & ~(size_t)15; }
 

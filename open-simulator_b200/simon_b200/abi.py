@@ -48,6 +48,10 @@ class SimonScenarioResult(C.Structure):
                 ("elapsed_ms", C.c_float), ("reserved", C.c_uint32)]
 
 
+class SimonScenarioLocalResult(C.Structure):
+    _fields_ = [("vg_requested", C.c_int64), ("vg_capacity", C.c_int64), ("reserved", C.c_uint64)]
+
+
 class SimonMovesResult(C.Structure):
     _fields_ = [("best_key", C.c_uint64), ("n_feasible", C.c_uint32), ("n_topk", C.c_uint32),
                 ("kernel_ms", C.c_float), ("reserved", C.c_uint32)]

@@ -73,31 +73,41 @@ def load_config(path: str, base_dir: Optional[str] = None):
 
 
 def auto_add_nodes(cluster: ResourceTypes, apps: List[AppResource], new_node, runner_factory: Callable, kmax: int = 64,
-                   method: str = "sweep", max_cpu: Optional[int] = None, max_mem: Optional[int] = None) -> ApplyResult:
+                   method: str = "sweep", max_cpu: Optional[int] = None, max_mem: Optional[int] = None,
+                   open_local: bool = False, local_devices: bool = False, max_vg: Optional[int] = None) -> ApplyResult:
     """Minimal k in [0, kmax] such that cluster + k copies of new_node places every pod within the occupancy caps.
 
-    runner_factory(ss) -> capacity.Runner for that scenario set (GPU: capacity.gpu_runner(device, engine=Engine(ss.compiled)))."""
+    runner_factory(ss) -> capacity.Runner for that scenario set (GPU: capacity.gpu_runner(device, engine=Engine(ss.compiled))).
+    open_local / local_devices: place pods that request Open-Local storage (capacity.build_scenarios); per_k then also holds
+    vg_requested / vg_capacity and the MaxVG cap (max_vg, default: the environment) applies.  Bisection stays valid: once every
+    pod is placed, ΣVG requested is fixed, and ΣVG capacity can only grow with k."""
     if max_cpu is None or max_mem is None:
         ec, em = capacity.env_caps()
         max_cpu = ec if max_cpu is None else max_cpu
         max_mem = em if max_mem is None else max_mem
+    if max_vg is None:
+        max_vg = capacity.env_vg_cap() if open_local else 100
     specs = [new_node] if new_node is not None else []
     if not specs:
         kmax = 0
     ks = list(range(0, kmax + 1))
-    ss = capacity.build_scenarios(cluster, apps, specs or [cluster.Nodes[0]], ks if specs else [0])
+    ss = capacity.build_scenarios(cluster, apps, specs or [cluster.Nodes[0]], ks if specs else [0],
+                                  open_local=open_local, local_devices=local_devices)
     runner = runner_factory(ss)
     by_k = {sc.k: sc for sc in ss.scenarios}
     per_k: Dict[int, Dict[str, int]] = {}
+    keys = ("n_unscheduled", "n_scheduled", "req_mcpu", "alloc_mcpu", "req_mem", "alloc_mem")
+    if open_local:
+        keys += ("vg_requested", "vg_capacity")
 
     def evaluate(klist):
         todo = [by_k[k] for k in klist if k not in per_k]
         for sc, res in zip(todo, runner(ss, todo)):
-            per_k[sc.k] = {q: int(res[q]) for q in ("n_unscheduled", "n_scheduled", "req_mcpu", "alloc_mcpu", "req_mem", "alloc_mem")}
+            per_k[sc.k] = {q: int(res[q]) for q in keys}
 
     def ok(k):
         r = per_k[k]
-        return r["n_unscheduled"] == 0 and capacity.occupancy_ok(r, max_cpu, max_mem)
+        return r["n_unscheduled"] == 0 and capacity.occupancy_ok(r, max_cpu, max_mem, max_vg)
 
     rounds = 0
     if method == "sweep" or not specs:
@@ -131,6 +141,10 @@ def main(argv=None):
     ap.add_argument("--kmax", type=int, default=64)
     ap.add_argument("--method", default="sweep", choices=["sweep", "bisect"])
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--open-local", action="store_true",
+                    help="place pods that request Open-Local storage (LVM volumes); the MaxVG cap applies")
+    ap.add_argument("--open-local-devices", action="store_true",
+                    help="also their exclusive SSD / HDD device volumes (implies --open-local)")
     a = ap.parse_args(argv)
     cluster, apps, new_node = load_config(a.simon_config)
     from .engine import Engine            # no CPU fallback: raises without the library / a CUDA device
@@ -142,7 +156,8 @@ def main(argv=None):
         engines.append(eng)
         return capacity.gpu_runner(a.device, engine=eng)
 
-    res = auto_add_nodes(cluster, apps, new_node, factory, kmax=a.kmax, method=a.method)
+    res = auto_add_nodes(cluster, apps, new_node, factory, kmax=a.kmax, method=a.method,
+                         open_local=a.open_local or a.open_local_devices, local_devices=a.open_local_devices)
     for e in engines:
         e.close()
     print(json.dumps({"new_node_num": res.new_node_num, "unscheduled_without_new_nodes": res.unscheduled_without_new_nodes,

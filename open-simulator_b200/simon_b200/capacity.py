@@ -14,6 +14,7 @@ satisfyResourceSetting (apply.go:689-775: average CPU / memory occupancy <= MaxC
 from __future__ import annotations
 
 import os
+import re
 from dataclasses import dataclass, field
 from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
@@ -45,8 +46,13 @@ class ScenarioSet:
     n_base: int
 
 
-def build_scenarios(cluster: ResourceTypes, apps: List[AppResource], specs: Sequence[Obj], ks: Sequence[int]) -> ScenarioSet:
-    """Superset cluster + one scenario per (spec, k in ks)."""
+def build_scenarios(cluster: ResourceTypes, apps: List[AppResource], specs: Sequence[Obj], ks: Sequence[int],
+                    open_local: bool = False, local_devices: bool = False) -> ScenarioSet:
+    """Superset cluster + one scenario per (spec, k in ks).
+
+    open_local / local_devices: compile the superset with the Open-Local plugin (compile_cluster's switches), the StorageClasses
+    taken from the cluster and the apps as Simulate() does.  The pool copies of a spec carry its simon/node-local-storage
+    annotation (make_valid_node_by_node keeps annotations, like NewFakeNodes), so each copy adds the spec's VGs and devices."""
     kmax = max(ks) if len(ks) else 0
     base = list(cluster.Nodes)
     pool: List[Tuple[int, int, Obj]] = []
@@ -69,7 +75,8 @@ def build_scenarios(cluster: ResourceTypes, apps: List[AppResource], specs: Sequ
         pods.extend(app_pods)
     ctx = ClusterContext(services=list(cluster.Services), replicasets=list(cluster.ReplicaSets),
                          statefulsets=list(cluster.StatefulSets))
-    compiled = compile_cluster(nodes, pods, ctx)
+    storage_classes = list(cluster.StorageClasss) + [sc for a in apps for sc in a.Resource.StorageClasss] if open_local else None
+    compiled = compile_cluster(nodes, pods, ctx, open_local=open_local, storage_classes=storage_classes, local_devices=local_devices)
     orig_to_compiled = np.zeros(len(nodes), np.int64)
     for ci, oi in enumerate(compiled.node_orig_index):
         orig_to_compiled[oi] = ci
@@ -85,13 +92,17 @@ def build_scenarios(cluster: ResourceTypes, apps: List[AppResource], specs: Sequ
     return ScenarioSet(compiled, scenarios, pods, nb)
 
 
-def occupancy_ok(res: Dict[str, int], max_cpu: int = 100, max_mem: int = 100) -> bool:
-    """satisfyResourceSetting (pkg/apply/apply.go:689-775), CPU and memory parts."""
+def occupancy_ok(res: Dict[str, int], max_cpu: int = 100, max_mem: int = 100, max_vg: int = 100) -> bool:
+    """satisfyResourceSetting (pkg/apply/apply.go:689-775): CPU, memory and, for results that carry the VG sums of a run with
+    Open-Local storage (vg_requested / vg_capacity), the VG occupancy; a VG capacity of 0 skips that test (apply.go:766)."""
     if res["alloc_mcpu"] > 0:
         if int(float(res["req_mcpu"]) / float(res["alloc_mcpu"]) * 100) > max_cpu:
             return False
     if res["alloc_mem"] > 0:
         if int(float(res["req_mem"]) / float(res["alloc_mem"]) * 100) > max_mem:
+            return False
+    if res.get("vg_capacity"):
+        if int(float(res["vg_requested"]) / float(res["vg_capacity"]) * 100) > max_vg:
             return False
     return True
 
@@ -107,8 +118,20 @@ def env_caps() -> Tuple[int, int]:
     return cap("MaxCPU"), cap("MaxMemory")
 
 
-def scenario_key(sc: Scenario, res: Dict[str, int], max_cpu: int, max_mem: int) -> int:
-    feasible = res["n_unscheduled"] == 0 and occupancy_ok(res, max_cpu, max_mem)
+def env_vg_cap() -> int:
+    """EnvMaxVG (pkg/type/const.go:31; apply.go:712-719): unset or empty gives 100, a value outside [0, 100] gives 100, and a
+    value strconv.Atoi rejects is an error (ValueError)."""
+    v = os.environ.get("MaxVG", "")
+    if not v:
+        return 100
+    if not re.fullmatch(r"[+-]?[0-9]+", v):
+        raise ValueError(f"failed to convert env MaxVG to int: {v!r}")
+    x = int(v)
+    return 100 if x > 100 or x < 0 else x
+
+
+def scenario_key(sc: Scenario, res: Dict[str, int], max_cpu: int, max_mem: int, max_vg: int = 100) -> int:
+    feasible = res["n_unscheduled"] == 0 and occupancy_ok(res, max_cpu, max_mem, max_vg)
     return ((sc.k << 32) | sc.sid) if feasible else INFEASIBLE_KEY
 
 
@@ -116,39 +139,45 @@ Runner = Callable[[ScenarioSet, List[Scenario]], List[Dict[str, int]]]
 
 
 def gpu_runner(device: int = 0, engine=None) -> Runner:
-    """Runs a shard of scenarios on one GPU through simon_scenarios_run (one thread-block cluster per scenario).
-    With `engine` (an Engine holding ss.compiled) the context, its uploaded snapshot and its pooled scenario buffers are
-    reused across calls - the shape of a capacity search that tries several candidate sets on one cluster."""
+    """Runs a shard of scenarios on one GPU through simon_scenarios_run (one thread-block cluster per scenario), or
+    simon_scenarios_run_local when the superset was compiled with Open-Local storage (its results carry vg_requested /
+    vg_capacity).  With `engine` (an Engine holding ss.compiled) the context, its uploaded snapshot and its pooled scenario
+    buffers are reused across calls - the shape of a capacity search that tries several candidate sets on one cluster."""
+    def go(eng, ss: ScenarioSet, shard: List[Scenario]):
+        fn = eng.run_scenarios_local if ss.compiled.storage is not None else eng.run_scenarios
+        return fn([sc.nodes for sc in shard])[0]
+
     def run(ss: ScenarioSet, shard: List[Scenario]) -> List[Dict[str, int]]:
         from .engine import Engine
         if not shard:
             return []
         if engine is not None:
-            out, _ = engine.run_scenarios([sc.nodes for sc in shard])
-            return out
+            return go(engine, ss, shard)
         with Engine(ss.compiled, device=device) as eng:
-            out, _ = eng.run_scenarios([sc.nodes for sc in shard])
-        return out
+            return go(eng, ss, shard)
     return run
 
 
 def search(ss: ScenarioSet, runner: Runner, rank: int = 0, world: int = 1, all_reduce_min=None,
-           max_cpu: Optional[int] = None, max_mem: Optional[int] = None):
+           max_cpu: Optional[int] = None, max_mem: Optional[int] = None, max_vg: Optional[int] = None):
     """Shard scenarios round-robin over `world` ranks, run the local shard, reduce the packed key with MIN.
 
     all_reduce_min: callable(int) -> int performing the collective (torch.distributed all_reduce MIN over NCCL/gloo);
-    None for a single process.  Returns (best_key, local results keyed by scenario id)."""
+    None for a single process.  max_vg applies to results with VG sums (an Open-Local superset).  Returns (best_key, local
+    results keyed by scenario id)."""
     if max_cpu is None or max_mem is None:
         ec, em = env_caps()
         max_cpu = ec if max_cpu is None else max_cpu
         max_mem = em if max_mem is None else max_mem
+    if max_vg is None:
+        max_vg = env_vg_cap()
     shard = [sc for sc in ss.scenarios if sc.sid % world == rank]
     results = runner(ss, shard)
     local_best = INFEASIBLE_KEY
     by_sid = {}
     for sc, res in zip(shard, results):
         by_sid[sc.sid] = res
-        local_best = min(local_best, scenario_key(sc, res, max_cpu, max_mem))
+        local_best = min(local_best, scenario_key(sc, res, max_cpu, max_mem, max_vg))
     best = all_reduce_min(local_best) if all_reduce_min is not None else local_best
     return best, by_sid
 

@@ -24,7 +24,8 @@ EXPORTS = ["simon_gpu_version", "simon_ctx_create", "simon_ctx_destroy", "simon_
            "simon_moves_upload", "simon_moves_run", "simon_moves_replay", "simon_host_go118_sort",
            "simon_host_last_error", "simon_host_compile", "simon_host_plan_free", "simon_host_plan_columns", "simon_host_plan_describe",
            "simon_host_simulate", "simon_host_free", "simon_host_quantity_probe", "simon_host_plan_fit_error", "simon_host_capacity_search",
-           "simon_storage_upload", "simon_storage_state_download", "simon_devices_upload", "simon_devices_state_download"]
+           "simon_storage_upload", "simon_storage_state_download", "simon_devices_upload", "simon_devices_state_download",
+           "simon_scenarios_run_local", "simon_scenarios_storage_download"]
 
 
 class EngineUnavailable(RuntimeError):
@@ -92,6 +93,10 @@ def lib():
         L.simon_devices_upload.argtypes = [C.c_void_p, C.c_void_p]
         L.simon_devices_state_download.restype = C.c_int
         L.simon_devices_state_download.argtypes = [C.c_void_p, C.c_void_p]
+        L.simon_scenarios_run_local.restype = C.c_int
+        L.simon_scenarios_run_local.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.simon_scenarios_storage_download.restype = C.c_int
+        L.simon_scenarios_storage_download.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     except AttributeError:
         if not os.environ.get("SIMON_GPU_LIB"):       # an experiment library may lack the newer entry points; the shipped one may not
             raise
@@ -119,10 +124,11 @@ class Engine:
         self._check(L.simon_snapshot_upload(self.h, C.byref(self.snap)))
         self._check(L.simon_pods_upload(self.h, C.byref(self.pods)))
         if getattr(compiled, "storage", None) is not None:      # Open-Local LVM volumes (compile_cluster(open_local=True))
-            self.storage, keep = abi.marshal_storage(compiled.storage)
+            # the marshalled structs stay usable for a later re-upload: their arrays are kept with them
+            self.storage, self._storage_keep = abi.marshal_storage(compiled.storage)
             self._check(L.simon_storage_upload(self.h, C.byref(self.storage)))
             if compiled.storage.devices:                        # SSD / HDD devices (compile_cluster(local_devices=True))
-                self.devices, keep = abi.marshal_devices(compiled.storage)
+                self.devices, self._devices_keep = abi.marshal_devices(compiled.storage)
                 self._check(L.simon_devices_upload(self.h, C.byref(self.devices)))
 
     def _check(self, rc: int):
@@ -280,6 +286,15 @@ class Engine:
 
     def run_scenarios(self, scenarios: List[np.ndarray], want_nodes: bool = False):
         """scenarios: list of uint32 arrays (active node indices in scenario order)."""
+        return self._run_scenarios(scenarios, want_nodes, False)
+
+    def run_scenarios_local(self, scenarios: List[np.ndarray], want_nodes: bool = False):
+        """run_scenarios for a cluster compiled with open_local=True: every scenario places its pods on its own copy of the
+        uploaded VG and device state; each result also carries vg_requested / vg_capacity, the sums over the scenario's
+        annotated nodes after the run (satisfyResourceSetting's MaxVG input)."""
+        return self._run_scenarios(scenarios, want_nodes, True)
+
+    def _run_scenarios(self, scenarios, want_nodes, local):
         n = len(scenarios)
         arr = (abi.SimonScenario * n)()
         keep = []
@@ -291,7 +306,23 @@ class Engine:
         res = (abi.SimonScenarioResult * n)()
         P = self.c.pods_dims["n_pods"]
         out_node = np.full((n, P), -9, np.int32) if want_nodes else None
-        self._check(lib().simon_scenarios_run(self.h, arr, n, res, out_node.ctypes.data if want_nodes else None))
+        if local:
+            loc = (abi.SimonScenarioLocalResult * n)()
+            self._check(lib().simon_scenarios_run_local(self.h, arr, n, res, loc, out_node.ctypes.data if want_nodes else None))
+        else:
+            self._check(lib().simon_scenarios_run(self.h, arr, n, res, out_node.ctypes.data if want_nodes else None))
         out = [dict(n_unscheduled=r.n_unscheduled, n_scheduled=r.n_scheduled, req_mcpu=r.req_mcpu, alloc_mcpu=r.alloc_mcpu,
                     req_mem=r.req_mem, alloc_mem=r.alloc_mem, elapsed_ms=r.elapsed_ms) for r in res]
+        if local:
+            for o, r in zip(out, loc):
+                o["vg_requested"], o["vg_capacity"] = int(r.vg_requested), int(r.vg_capacity)
         return out, out_node
+
+    def scenario_storage_state(self, i: int):
+        """Scenario i of the last run_scenarios_local batch: (VG requested [V][N], allocated device slot masks [N] or None without
+        devices), node-indexed like the snapshot."""
+        V, N = self.c.storage.n_vgs, self.c.n_nodes
+        vg = np.zeros(max(V * N, 1), np.int64)
+        dev = np.zeros(max(N, 1), np.uint32) if self.c.storage.devices else None
+        self._check(lib().simon_scenarios_storage_download(self.h, i, vg.ctypes.data, None if dev is None else dev.ctypes.data))
+        return vg[:V * N].reshape(V, N), None if dev is None else dev[:N]
