@@ -329,8 +329,9 @@ int simon_debug_dump_read(simon_ctx *ctx, int64_t *out_total, int32_t *out_code)
  * (device time by CUDA events). */
 #define SIMON_MOVE_NOOP (1u << 24)         /* target is the pod's current node */
 #define SIMON_MOVE_NOT_PLACED (1u << 25)   /* the pod is not running on a node of the snapshot */
-#define SIMON_MOVE_NOT_MOVABLE (1u << 26)  /* class with DoNotSchedule spread constraints, a GPU-share request, local storage volumes
-                                              (simon_storage), or pinned (DaemonSet pod) */
+#define SIMON_MOVE_NOT_MOVABLE (1u << 26)  /* class with local storage volumes (simon_storage) or pinned (DaemonSet pod), under every
+                                              scope; or with DoNotSchedule spread constraints / a GPU-share request that the move
+                                              scope (simon_moves_set_scope) does not admit */
 #define SIMON_MOVE_BAD_INDEX (1u << 27)
 #define SIMON_MOVE_GAIN_BIAS 1000
 
@@ -348,6 +349,26 @@ int simon_moves_upload(simon_ctx *ctx, const simon_move *moves, uint32_t n_moves
 int simon_moves_run(simon_ctx *ctx, uint32_t k, int32_t *out_gain, uint32_t *out_code, uint64_t *out_best_per_pod,
                     simon_move_rank *out_topk, simon_moves_result *out);
 int simon_moves_replay(simon_ctx *ctx, uint32_t steps, float *out_ms_total);
+
+/* Move scope (opt-in; 0, the default, scores exactly as above).  A scope bit admits the classes whose only reason to be
+ * SIMON_MOVE_NOT_MOVABLE is in the scope (a class with both needs both bits); their moves are filtered on the target instead,
+ * in the placement path's order: static, NodePorts, NodeResourcesFit, PodTopologySpread (hard), InterPodAffinity, Open-Gpu-Share.
+ *   SIMON_MOVES_SCOPE_HARD_SPREAD  for each DoNotSchedule constraint of the class (filtering.go:276-328): SFC_PTS_MISSING if the
+ *       target has no domain on its topology; else SFC_PTS_SKEW if match_b + selfMatch - min' > maxSkew, where match_b is the
+ *       counter at the target's domain (the pod's own count taken out if it sits there; 0 if that domain is not registered) and
+ *       min' the minimum over the registered domains with the pod removed.  A domain is registered when a node that passes the
+ *       class's node selection carries all of its hard topology keys.
+ *   SIMON_MOVES_SCOPE_GPU_SHARE    (open-gpu-share.go:51-81) SFC_GPU if the target's total gpu-mem is below the request or
+ *       AllocateGpuId (cache/gpunodeinfo.go:232-290) finds no assignment on its live free device memory.
+ * Pinned classes and classes with local storage stay SIMON_MOVE_NOT_MOVABLE under every scope.  The scope applies to later
+ * simon_moves_run / simon_moves_replay calls and stays on the ctx until changed; unknown bits: SIMON_ERR_INVALID. */
+#define SIMON_MOVES_SCOPE_GPU_SHARE 1u
+#define SIMON_MOVES_SCOPE_HARD_SPREAD 2u
+int simon_moves_set_scope(simon_ctx *ctx, uint32_t scope);
+/* Moves [first, first+count) of the last simon_moves_run: the target's device slots of each feasible GPU-share move, in the
+ * format of simon_gpu_slots_download (what a rebalancer writes into alibabacloud.com/gpu-index); 0 for every other move.
+ * SIMON_ERR_STATE unless that run's scope had SIMON_MOVES_SCOPE_GPU_SHARE (a simon_moves_upload or _replay ends it). */
+int simon_moves_gpu_slots_download(simon_ctx *ctx, uint32_t first, uint32_t count, uint32_t *out_slots);
 
 /* ---- Open-Local LVM volumes (pkg/simulator/plugin/open-local.go:51-254; OL = vendor/github.com/alibaba/open-local/pkg) ------------
  * Optional, uploaded after simon_snapshot_upload + simon_pods_upload; without it no class requests local storage.

@@ -228,6 +228,17 @@ struct simon_ctx {
     DevBuf<SmvClass> d_mv_classes;
     DevBuf<SmvPod> d_mv_pods;
     uint32_t mv_n = 0, mv_base = 0;
+    // move scope (simon_moves_set_scope): per class SmvClass::bits on the host, the (class, hard constraint) pairs with their
+    // bitmap offsets, and what the current scope launches (rebuilt when the scope or the classes change)
+    uint32_t mv_scope = 0, mv_last_scope = 0;
+    bool mv_ran = false, mv_scope_dirty = true, mv_scoped = false;
+    std::vector<uint32_t> h_mv_bits;
+    std::vector<uint4> h_mv_pairs;
+    uint32_t mv_n_prep = 0;
+    DevBuf<uint4> d_mv_prep;
+    DevBuf<uint32_t> d_mv_hreg, d_mv_slots;
+    DevBuf<int2> d_mv_hs;
+    DevBuf<SmvGpu> d_mv_gpu;
     uint32_t n_pin_fast = 0;            // pods marked for the pinned-run fast path (-4 in the device copy of pod_fixed_node)
     std::vector<uint8_t> bypass;        // per pod: never reaches the scheduler in a single-scenario run (pre-bound or absent)
     DevBuf<unsigned char> d_gnode;      // large-cluster variant: per-node arrays in global memory
@@ -818,6 +829,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     {
         // compact per-class header of the move kernel (simon_moves.cu): scoring + Fit inputs and a few counts in 64 bytes
         std::vector<SmvClass> mc(std::max(1u, p->n_classes));
+        ctx->h_mv_bits.assign(std::max(1u, p->n_classes), 0u);
         for (uint32_t c = 0; c < p->n_classes; c++) {
             const int64_t *cw = p->class_blob + p->class_off[c];
             SmvClass &k = mc[c];
@@ -827,6 +839,10 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
             k.sig = (uint32_t)cw[SCW_STATIC_SIG];
             uint32_t bits = (uint32_t)cw[SCW_FLAGS] & 0xffu;
             if (cw[SCW_N_PTS_HARD] > 0 || cw[SCW_GPU_MEM] > 0 || (cw[SCW_FLAGS] & SIMON_CLS_PINNED)) bits |= SMC_NOT_MOVABLE;
+            // what a move scope needs to admit the class (simon_moves_set_scope); a pinned class is never admitted
+            if (cw[SCW_GPU_MEM] > 0) bits |= SMC_NEED_GPU;
+            if (cw[SCW_N_PTS_HARD] > 0) bits |= SMC_NEED_HARD | ((uint32_t)cw[SCW_N_PTS_HARD] << 25);
+            if (cw[SCW_FLAGS] & SIMON_CLS_PINNED) bits |= SMC_NEVER;
             const int64_t *sc = cw + cw[SCW_OFF_SCALARS];
             for (uint32_t q = 0; q < ctx->K; q++) if (sc[q] != 0) bits |= SMC_HAS_SCALAR;
             const uint32_t n_filt = (uint32_t)(cw[SCW_N_IPA_AFF] + cw[SCW_N_IPA_ANTI] + cw[SCW_N_IPA_EXIST]);
@@ -836,7 +852,22 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
             const uint32_t E = (uint32_t)cw[SCW_N_ENT];
             for (uint32_t e = 0; e < E; e++) if (et[8ull * e + ER_INC]) bits |= SMC_OWN_INC;
             k.bits = bits;
+            ctx->h_mv_bits[c] = bits;
         }
+        // registered-domain bitmaps of the hard constraints, one per (class, constraint), for scoped runs
+        ctx->h_mv_pairs.clear();
+        uint32_t words = 0;
+        for (uint32_t c = 0; c < p->n_classes; c++) {
+            const int64_t *cw = p->class_blob + p->class_off[c];
+            for (uint32_t j = 0; (int64_t)j < cw[SCW_N_PTS_HARD]; j++) {
+                const int64_t t = (cw + cw[SCW_OFF_PTS_HARD])[4 * j + 1];
+                ctx->h_mv_pairs.push_back(make_uint4(c, j, words, 0));
+                words += (ctx->topo_ndom[t] + 31) / 32;
+            }
+        }
+        CU(ctx->d_mv_hreg.alloc(std::max(1u, words)));
+        CU(ctx->d_mv_hs.alloc((size_t)std::max(1u, p->n_classes) * SMV_MAX_HARD));
+        ctx->mv_scope_dirty = true;
         std::vector<uint32_t> sig_class(std::max(1u, p->n_static_sigs), 0u);
         for (uint32_t c = p->n_classes; c-- > 0;) {
             const int64_t sg = (p->class_blob + p->class_off[c])[SCW_STATIC_SIG];
@@ -1229,7 +1260,9 @@ int simon_storage_upload(simon_ctx *ctx, const simon_storage *sg) {
         std::vector<SmvClass> mc(std::max(1u, C));
         CU(cudaMemcpyAsync(mc.data(), ctx->d_mv_classes.p, sizeof(SmvClass) * mc.size(), cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
-        for (uint32_t c = 0; c < C; c++) if (sg->class_local[c]) mc[c].bits |= SMC_NOT_MOVABLE;
+        for (uint32_t c = 0; c < C; c++)
+            if (sg->class_local[c]) { mc[c].bits |= SMC_NOT_MOVABLE | SMC_NEVER; ctx->h_mv_bits[c] = mc[c].bits; }
+        ctx->mv_scope_dirty = true;
         CU(ctx->d_mv_classes.upload(mc.data(), mc.size(), st));
         CU(cudaStreamSynchronize(st));      // `mc` leaves scope
     }
@@ -1316,10 +1349,46 @@ int simon_devices_state_download(simon_ctx *ctx, uint32_t *alloc_mask) {
 }
 
 // ---- candidate-move scoring (config 5) ------------------------------------------------------------------------------
+// What the current scope launches: the scoped kernel iff some class is admitted, and the prep pairs of the admitted hard classes
+static int moves_scope_refresh(simon_ctx *ctx) {
+    if (!ctx->mv_scope_dirty) return SIMON_OK;
+    const uint32_t scope = ctx->mv_scope;
+    auto admitted = [&](uint32_t c) {
+        const uint32_t b = ctx->h_mv_bits[c];
+        return scope && (b & SMC_NOT_MOVABLE) && !(b & SMC_NEVER) && !(SMC_NEED(b) & ~scope);
+    };
+    ctx->mv_scoped = false;
+    for (uint32_t c = 0; c < ctx->n_classes; c++) ctx->mv_scoped |= admitted(c);
+    std::vector<uint4> prep;
+    for (const uint4 &q : ctx->h_mv_pairs) if (admitted(q.x)) prep.push_back(q);
+    ctx->mv_n_prep = (uint32_t)prep.size();
+    if (!prep.empty()) {
+        CU(ctx->d_mv_prep.upload(prep.data(), prep.size(), ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));      // `prep` leaves scope
+    }
+    ctx->mv_scope_dirty = false;
+    return SIMON_OK;
+}
+
 static int moves_launch(simon_ctx *ctx, bool record) {
     cudaStream_t st = ctx->stream;
-    const uint32_t N = ctx->N, n = ctx->mv_n;
+    const uint32_t N = ctx->N, n = ctx->mv_n, scope = ctx->mv_scope;
+    const bool scoped = ctx->mv_scoped;
+    if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && n) CU(ctx->d_mv_slots.alloc(n));
     if (record) CU(cudaEventRecord(ctx->ev0, st));
+    if (scoped && (scope & SIMON_MOVES_SCOPE_GPU_SHARE) && N) {
+        CU(ctx->d_mv_gpu.alloc(N));
+        simon_moves_pack_gpu<<<(N + 255) / 256, 256, 0, st>>>(N, ctx->d_gpu_count.p, ctx->d_gpu_dev_mem.p, ctx->d_gpu_total_mem.p,
+                                                               ctx->st.gpu_used.p, ctx->d_mv_gpu.p);
+        ctx->launches++;
+    }
+    if (scoped && ctx->mv_n_prep) {
+        simon_moves_hard_prep<<<ctx->mv_n_prep, 256, 0, st>>>(N, ctx->use_scache, ctx->d_scache.p, ctx->d_label_bits.p, ctx->d_topo_dom.p,
+                                                              ctx->d_topo_ndom.p, ctx->d_class_off.p, ctx->d_class_blob.p, ctx->st.cnt.p,
+                                                              ctx->d_mv_prep.p, ctx->d_mv_hreg.p, ctx->d_mv_hs.p);
+        ctx->launches++;
+    }
+    if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && !scoped && n) CU(cudaMemsetAsync(ctx->d_mv_slots.p, 0, 4ull * n, st));
     simon_moves_pack<<<std::max(std::max(1u, (N + 255) / 256), std::min(1184u, (ctx->n_pods + 255) / 256)), 256, 0, st>>>(N, ctx->T, ctx->d_alloc_mcpu.p, ctx->d_alloc_mem.p, ctx->d_alloc_eph.p, ctx->d_alloc_pods.p,
                                                                      ctx->d_topo_dom.p, ctx->st.req_mcpu.p, ctx->st.req_mem.p, ctx->st.req_eph.p,
                                                                      ctx->st.nz_mcpu.p, ctx->st.nz_mem.p, ctx->st.num_pods.p, ctx->d_mv_nodes.p,
@@ -1335,6 +1404,8 @@ static int moves_launch(simon_ctx *ctx, bool record) {
     P.cnt = ctx->st.cnt.p; P.cnt_total = ctx->st.cnt_total.p; P.scache = ctx->d_scache.p; P.moves = ctx->d_moves.p;
     P.out_gain = ctx->d_mv_gain.p; P.out_code = ctx->d_mv_code.p; P.best_per_pod = ctx->d_mv_best_pod.p; P.best_global = ctx->d_mv_best.p;
     P.hist = ctx->d_mv_hist.p; P.move_base = ctx->mv_base;
+    P.scope = scope; P.gpu = ctx->d_mv_gpu.p; P.hs = ctx->d_mv_hs.p; P.hreg = ctx->d_mv_hreg.p;
+    P.out_slots = (scope & SIMON_MOVES_SCOPE_GPU_SHARE) ? ctx->d_mv_slots.p : nullptr;
     if (n) {
         int sms = 132;
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
@@ -1342,8 +1413,13 @@ static int moves_launch(simon_ctx *ctx, bool record) {
         // 2-CTA variant without spills (diagnostic switch)
         static const int occ = getenv("SIMON_MOVES_OCC") ? atoi(getenv("SIMON_MOVES_OCC")) : 4;
         const uint32_t grid = std::min<uint32_t>((n + 255) / 256, (uint32_t)sms * (occ == 2 ? 2u : 4u) * 2u);
-        if (occ == 2) simon_moves_kernel<2><<<grid, 256, 0, st>>>(P);
-        else simon_moves_kernel<4><<<grid, 256, 0, st>>>(P);
+        if (scoped) {
+            if (occ == 2) simon_moves_kernel<2, true><<<grid, 256, 0, st>>>(P);
+            else simon_moves_kernel<4, true><<<grid, 256, 0, st>>>(P);
+        } else {
+            if (occ == 2) simon_moves_kernel<2, false><<<grid, 256, 0, st>>>(P);
+            else simon_moves_kernel<4, false><<<grid, 256, 0, st>>>(P);
+        }
         ctx->launches++;
     }
     if (record) CU(cudaEventRecord(ctx->ev1, st));
@@ -1360,7 +1436,7 @@ int simon_moves_upload(simon_ctx *ctx, const simon_move *moves, uint32_t n_moves
     CU(ctx->d_mv_gain.alloc(n_moves)); CU(ctx->d_mv_code.alloc(n_moves)); CU(ctx->d_mv_hist.alloc(SMV_NBINS)); CU(ctx->d_mv_topn.alloc(2));
     CU(ctx->d_mv_best_pod.alloc(std::max(1u, ctx->n_pods))); CU(ctx->d_mv_best.alloc(1)); CU(ctx->d_mv_nodes.alloc(std::max(1u, ctx->N)));
     CU(ctx->d_mv_pods.alloc(std::max(1u, ctx->n_pods)));
-    ctx->mv_n = n_moves; ctx->mv_base = move_base;
+    ctx->mv_n = n_moves; ctx->mv_base = move_base; ctx->mv_ran = false;
     if (!ctx->static_filled && ctx->use_scache && ctx->N && ctx->n_classes) {
         // once per uploaded pod list: the static verdicts of every (signature, node) pair, densely
         SkParams Pm;
@@ -1383,7 +1459,10 @@ int simon_moves_run(simon_ctx *ctx, uint32_t k, int32_t *out_gain, uint32_t *out
     CU(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     const uint32_t n = ctx->mv_n;
-    int rc = moves_launch(ctx, true);
+    ctx->mv_ran = false;
+    int rc = moves_scope_refresh(ctx);
+    if (rc) return rc;
+    rc = moves_launch(ctx, true);
     if (rc) return rc;
     uint32_t hist[SMV_NBINS];
     unsigned long long best = 0;
@@ -1423,6 +1502,26 @@ int simon_moves_run(simon_ctx *ctx, uint32_t k, int32_t *out_gain, uint32_t *out
     if (out_code && n) CU(cudaMemcpyAsync(out_code, ctx->d_mv_code.p, 4ull * n, cudaMemcpyDeviceToHost, st));
     if (out_best_per_pod && ctx->n_pods) CU(cudaMemcpyAsync(out_best_per_pod, ctx->d_mv_best_pod.p, 8ull * ctx->n_pods, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
+    ctx->mv_ran = true;
+    ctx->mv_last_scope = ctx->mv_scope;
+    return SIMON_OK;
+}
+
+int simon_moves_set_scope(simon_ctx *ctx, uint32_t scope) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (scope & ~(SIMON_MOVES_SCOPE_GPU_SHARE | SIMON_MOVES_SCOPE_HARD_SPREAD)) return fail(ctx, SIMON_ERR_INVALID, "unknown move scope bits 0x%x", scope);
+    if (scope != ctx->mv_scope) ctx->mv_scope_dirty = true;
+    ctx->mv_scope = scope;
+    return SIMON_OK;
+}
+
+int simon_moves_gpu_slots_download(simon_ctx *ctx, uint32_t first, uint32_t count, uint32_t *out_slots) {
+    if (!ctx || (!out_slots && count)) return SIMON_ERR_INVALID;
+    if (!ctx->mv_ran || !(ctx->mv_last_scope & SIMON_MOVES_SCOPE_GPU_SHARE))
+        return fail(ctx, SIMON_ERR_STATE, "no simon_moves_run with GPU share in its scope since the last simon_moves_upload");
+    if ((uint64_t)first + count > ctx->mv_n) return fail(ctx, SIMON_ERR_INVALID, "range out of bounds");
+    CU(cudaSetDevice(ctx->device));
+    if (count) CU(cudaMemcpy(out_slots, ctx->d_mv_slots.p + first, 4ull * count, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
@@ -1431,6 +1530,9 @@ int simon_moves_replay(simon_ctx *ctx, uint32_t steps, float *out_ms_total) {
     if (!ctx->have_pods || !ctx->d_moves.p) return fail(ctx, SIMON_ERR_STATE, "simon_moves_replay before simon_moves_upload");
     CU(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
+    int rc0 = moves_scope_refresh(ctx);
+    if (rc0) return rc0;
+    ctx->mv_ran = false;        // the slots of the last simon_moves_run may be overwritten
     CU(cudaEventRecord(ctx->ev0, st));
     for (uint32_t s = 0; s < steps; s++) {
         int rc = moves_launch(ctx, false);

@@ -16,6 +16,13 @@
 // Every move is independent: one thread per move over a read-only snapshot.  Node columns are packed per launch into one
 // 96-byte record per node (three 32-byte sectors) so that the two random gathers per move (target, source) cost six
 // sectors instead of two dozen; the move list itself streams through coalesced 8-byte loads.
+//
+// Move scope (simon_moves_set_scope): classes with a GPU-share request and / or DoNotSchedule spread constraints are refused
+// (SMV_NOT_MOVABLE) unless the scope admits them; then the scoped instantiation of the kernel adds, in the placement kernel's
+// filter order, PodTopologySpread (hard) after NodeResourcesFit and Open-Gpu-Share after InterPodAffinity.  Its inputs are
+// built per scoped launch: simon_moves_hard_prep gives every (admitted class, hard constraint) its registered-domain bitmap
+// and the minimum of the live counter over those domains, simon_moves_pack_gpu one 96-byte record of free device memory per
+// node.  The default instantiation compiles none of it.
 #pragma once
 
 struct __align__(32) SmvNode {          // 96 bytes = three 32-byte sectors, ordered by who needs them:
@@ -32,6 +39,7 @@ struct __align__(32) SmvClass {
     int64_t req_mcpu, req_mem, req_eph;                  // sector 1: Fit
     uint32_t sig;                                        //           static signature
     uint32_t bits;                                       //           flags:8 | not movable:1 | has scalar request:1 | n_ports:5 | n_filter entries (aff+anti+exist):6 | own increments:1
+                                                         //           | scope bits the class needs:2 | never movable:1 | n_hard:4
 };
 static_assert(sizeof(SmvClass) == 64, "SmvClass layout");
 // per-pod record built by the pack kernel of every launch: everything a move needs to know about its pod in ONE 16-byte load,
@@ -45,11 +53,25 @@ struct __align__(16) SmvPod {
 #define SMC_NPORTS(b) (((b) >> 10) & 31u)
 #define SMC_NFILT(b) (((b) >> 15) & 63u)
 #define SMC_OWN_INC (1u << 21)
+#define SMC_NEED(b) (((b) >> 22) & 3u)   // SIMON_MOVES_SCOPE_* bits that admit a not-movable class (GPU share, hard spread)
+#define SMC_NEED_GPU (1u << 22)
+#define SMC_NEED_HARD (1u << 23)
+#define SMC_NEVER (1u << 24)             // pinned (DaemonSet) or Open-Local class: not movable under any scope
+#define SMC_NHARD(b) (((b) >> 25) & 15u)
+#define SMV_MAX_HARD 8                   // == SK_MAX_HARD: stride of the per-class rows of SmvParams::hs
+
+// free memory per GPU-share device of a node (-1 past gpu_count) and its total gpu-mem: AllocateGpuId's input
+struct __align__(32) SmvGpu {
+    int64_t free_mem[SIMON_MAX_GPU_DEV];
+    int64_t total, pad[3];
+};
+static_assert(sizeof(SmvGpu) == 96, "SmvGpu layout");
 
 #define SMV_OK 0u
 #define SMV_NOOP (1u << 24)            // target == current node
 #define SMV_NOT_PLACED (1u << 25)      // the pod is not running anywhere (unscheduled / absent / bound outside the cluster)
-#define SMV_NOT_MOVABLE (1u << 26)     // class with DoNotSchedule spread constraints, a GPU-share request or a pin (DaemonSet pod): not a candidate
+#define SMV_NOT_MOVABLE (1u << 26)     // pinned (DaemonSet) or Open-Local class, or one with DoNotSchedule spread constraints / a GPU-share
+                                       // request that the move scope does not admit: not a candidate
 #define SMV_BAD_INDEX (1u << 27)
 #define SMV_GAIN_BIAS 1000
 #define SMV_NBINS 401                  // gains lie in [-200, 200]
@@ -75,6 +97,12 @@ struct SmvParams {
     unsigned long long *best_global;    // [1]
     uint32_t *hist;                     // [SMV_NBINS] feasible moves per gain
     uint32_t move_base, pad2;           // global index of moves[0] (multi-GPU shards)
+    // scoped instantiation only
+    uint32_t scope, pad3;               // SIMON_MOVES_SCOPE_* of this launch
+    const SmvGpu *gpu;                  // [N] (GPU share in scope)
+    const int2 *hs;                     // [n_classes][SMV_MAX_HARD] (minimum over the registered domains, word offset in hreg)
+    const uint32_t *hreg;               // registered-domain bitmaps
+    uint32_t *out_slots;                // [n_moves] device slots of feasible GPU-share moves, or NULL
 };
 
 __global__ void simon_moves_pack(uint32_t N, uint32_t T, const int64_t *alloc_mcpu, const int64_t *alloc_mem, const int64_t *alloc_eph,
@@ -103,6 +131,94 @@ __global__ void simon_moves_pack(uint32_t N, uint32_t T, const int64_t *alloc_mc
 #pragma unroll
     for (int t = 0; t < 6; t++) r.dom[t] = (uint32_t)(t + 1) < T ? topo_dom[(uint64_t)(t + 1) * N + g] : -1;
     out[g] = r;
+}
+
+// GPU record per node for scoped runs with GPU share in scope, from the live device memory in use
+__global__ void simon_moves_pack_gpu(uint32_t N, const int32_t *gpu_count, const int64_t *dev_mem, const int64_t *total_mem,
+                                     const int64_t *gpu_used, SmvGpu *out) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= N) return;
+    const int nd = gpu_count ? gpu_count[g] : 0;
+    SmvGpu r;
+#pragma unroll
+    for (int d = 0; d < SIMON_MAX_GPU_DEV; d++) r.free_mem[d] = d < nd ? dev_mem[g] - gpu_used[(uint64_t)d * N + g] : -1;
+    r.total = total_mem ? total_mem[g] : 0;
+    r.pad[0] = r.pad[1] = r.pad[2] = 0;
+    out[g] = r;
+}
+
+// For scoped runs with hard spread in scope: one block per (admitted class, hard constraint j) pair (cls, j, word offset of its
+// bitmap in hreg).  The registered domains of the constraint (filtering.go:221-243: nodes that pass the class's node selection and
+// carry all of its hard topology keys) from the static verdict cache, or evaluated here where the cache has no record (cache
+// disabled, or a record not stored); then the minimum of the live counter over them (INT32_MAX: none), into hs[cls][j].
+__global__ void __launch_bounds__(256) simon_moves_hard_prep(uint32_t N, uint32_t use_scache, const unsigned long long *scache,
+                                                             const uint64_t *label_bits, const int32_t *topo_dom, const uint32_t *topo_ndom,
+                                                             const uint64_t *class_off, const int64_t *class_blob, const int32_t *cnt,
+                                                             const uint4 *pairs, uint32_t *hreg, int2 *hs) {
+    __shared__ int32_t s_min[8];
+    const uint4 pr = pairs[blockIdx.x];
+    const int64_t *cw = class_blob + class_off[pr.x];
+    const int64_t *r = cw + cw[SCW_OFF_ENT] + 8ull * (uint64_t)(cw[SCW_N_PORTS] + pr.y);
+    const int64_t t = r[ER_T];
+    const uint32_t nd = topo_ndom[t], nw = (nd + 31) / 32;
+    uint32_t *reg = hreg + pr.z;
+    for (uint32_t w = threadIdx.x; w < nw; w += blockDim.x) reg[w] = 0u;
+    __syncthreads();
+    const ReqCtx RC{label_bits, N};
+    const uint64_t sig = (uint64_t)cw[SCW_STATIC_SIG];
+    const int64_t *hard = cw + cw[SCW_OFF_PTS_HARD];
+    for (uint32_t g = threadIdx.x; g < N; g += blockDim.x) {
+        const unsigned long long rec = use_scache ? __ldcg(scache + sig * N + g) : 0ull;
+        bool elig;
+        if (rec & (1ull << 24)) elig = ((rec >> 8) & (NF_SEL_OK | NF_HARDKEYS)) == (NF_SEL_OK | NF_HARDKEYS);
+        else {
+            elig = selection_ok(cw, RC, g);
+            for (int64_t q = 0; q < cw[SCW_N_PTS_HARD]; q++)
+                if (topo_dom[(uint64_t)hard[4 * q + 1] * N + g] < 0) elig = false;
+        }
+        if (elig) {
+            const int32_t d = topo_dom[(uint64_t)t * N + g];
+            atomicOr(reg + (d >> 5), 1u << (d & 31));
+        }
+    }
+    __syncthreads();
+    int32_t mn = INT32_MAX;
+    for (uint32_t d = threadIdx.x; d < nd; d += blockDim.x)
+        if ((__ldcg(reg + (d >> 5)) >> (d & 31)) & 1u) mn = min(mn, cnt[(uint32_t)r[ER_BASE] + d]);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+    if ((threadIdx.x & 31) == 0) s_min[threadIdx.x >> 5] = mn;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (uint32_t w = 1; w < blockDim.x / 32; w++) mn = min(mn, s_min[w]);
+        hs[(uint64_t)pr.x * SMV_MAX_HARD + pr.y] = make_int2(mn, (int32_t)pr.z);
+    }
+}
+
+// AllocateGpuId (cache/gpunodeinfo.go:232-290) on a node's free device memory, in registers: the slots in the 4-bits-per-device
+// format of simon_gpu_slots_download (saturating at 15), 0 = no assignment.  One GPU: the device of least free memory that holds the
+// request, first on ties.  Several: the greedy scan fills device d while it holds the request, then moves on to d + 1, so it can fail
+// with enough memory free in total.
+__device__ __forceinline__ uint32_t smv_gpu_fit(const SmvGpu &n, int64_t req, int64_t num) {
+    if (req <= 0 || num <= 0) return 0u;
+    if (num == 1) {
+        int cand = -1;
+        int64_t cm = 0;
+#pragma unroll
+        for (int d = 0; d < SIMON_MAX_GPU_DEV; d++)
+            if (n.free_mem[d] >= req && (cand < 0 || n.free_mem[d] < cm)) { cand = d; cm = n.free_mem[d]; }
+        return cand < 0 ? 0u : 1u << (4 * cand);
+    }
+    uint32_t out = 0;
+    int64_t got = 0;
+#pragma unroll 1
+    for (int d = 0; d < SIMON_MAX_GPU_DEV && got < num; d++) {
+        int64_t take = 0;
+        for (int64_t av = n.free_mem[d]; av >= req && got + take < num; av -= req) take++;
+        got += take;
+        out |= (uint32_t)(take < 15 ? take : 15) << (4 * d);
+    }
+    return got == num ? out : 0u;
 }
 
 // one 32-byte sector as two 128-bit loads (sm_90 has no wider global load; both halves fall in the same sector, so the
@@ -167,7 +283,8 @@ __device__ __forceinline__ int32_t smv_dom(const SmvParams &P, const SmvNode &n,
     return __ldg(P.topo_dom + (uint64_t)t * P.N + g);
 }
 
-template <int MINB>
+// SCOPED: the instantiation for runs whose scope admits a class (see the top of this file)
+template <int MINB, bool SCOPED>
 __global__ void __launch_bounds__(256, MINB) simon_moves_kernel(const __grid_constant__ SmvParams P) {
     __shared__ uint32_t s_hist[SMV_NBINS];
     for (uint32_t q = threadIdx.x; q < SMV_NBINS; q += blockDim.x) s_hist[q] = 0;
@@ -177,7 +294,7 @@ __global__ void __launch_bounds__(256, MINB) simon_moves_kernel(const __grid_con
     for (uint32_t m = blockIdx.x * blockDim.x + threadIdx.x; m < P.n_moves; m += gridDim.x * blockDim.x) {
         const uint2 mv = __ldg(P.moves + m);
         const uint32_t pod = mv.x, b = mv.y;
-        uint32_t code = SMV_OK;
+        uint32_t code = SMV_OK, slots = 0;
         int32_t gain = 0;
         int32_t a = -1;
         SmvPod pr;
@@ -189,7 +306,7 @@ __global__ void __launch_bounds__(256, MINB) simon_moves_kernel(const __grid_con
             a = pr.node;
             if (a < 0 || (uint32_t)a >= P.N) code = SMV_NOT_PLACED;
             else if ((uint32_t)a == b) code = SMV_NOOP;
-            else if (pr.bits & SMC_NOT_MOVABLE) code = SMV_NOT_MOVABLE;
+            else if ((pr.bits & SMC_NOT_MOVABLE) && (!SCOPED || (pr.bits & SMC_NEVER) || (SMC_NEED(pr.bits) & ~P.scope))) code = SMV_NOT_MOVABLE;
         }
         if (code == SMV_OK) {
             const int32_t cls = pr.cls;
@@ -200,8 +317,8 @@ __global__ void __launch_bounds__(256, MINB) simon_moves_kernel(const __grid_con
             smv_ld_sector(reinterpret_cast<unsigned long long *>(&kc) + 4, reinterpret_cast<const unsigned long long *>(P.classes + cls) + 4);
             const uint32_t bits = kc.bits, cflags = bits & 0xffu;
             {
-                const uint32_t n_ports = SMC_NPORTS(bits), n_filt = SMC_NFILT(bits);
-                const bool need_ent = (n_ports | n_filt) != 0;
+                const uint32_t n_ports = SMC_NPORTS(bits), n_filt = SMC_NFILT(bits), n_hard = SCOPED ? SMC_NHARD(bits) : 0u;
+                const bool need_ent = (n_ports | n_filt | n_hard) != 0;
                 const SmvNode nb = smv_load<7>(P.nodes + b);
                 SmvNode na = smv_load<1>(P.nodes + a);
                 if (need_ent && (bits & SMC_OWN_INC)) smv_load_sector(na, P.nodes + a, 2);       // the source's domains: only to take p's own counts out
@@ -252,11 +369,34 @@ __global__ void __launch_bounds__(256, MINB) simon_moves_kernel(const __grid_con
                     }
                     code = rs;
                 }
+                // ---- PodTopologySpread, DoNotSchedule constraints (filtering.go:276-328) with p removed: b's count loses p's own
+                // count if p's sits at b's domain (val_at), and the minimum over the registered domains becomes
+                // min(min, cnt[dom_a] - 1) when p's count sits at a registered dom_a
+                if (SCOPED && code == SMV_OK && n_hard) {
+                    const int2 *hs = P.hs + (uint64_t)cls * SMV_MAX_HARD;
+#pragma unroll 1
+                    for (uint32_t j = 0; j < n_hard; j++) {
+                        const int64_t *r = et + 8ull * (n_ports + j);
+                        const int64_t t = r[ER_T];
+                        const int32_t db = smv_dom(P, nb, b, t);
+                        if (db < 0) { code = 1u << SFC_PTS_MISSING; break; }
+                        const int2 h = __ldg(hs + j);
+                        const uint32_t *reg = P.hreg + (uint32_t)h.y;
+                        const int32_t match = ((__ldg(reg + (db >> 5)) >> (db & 31)) & 1u) ? val_at(n_ports + j, db) : 0;
+                        int32_t mn = h.x;
+                        if (r[ER_INC]) {
+                            const int32_t da = smv_dom(P, na, (uint32_t)a, t);
+                            if (da >= 0 && ((__ldg(reg + (da >> 5)) >> (da & 31)) & 1u))
+                                mn = min(mn, __ldg(P.cnt + (uint32_t)r[ER_BASE] + (uint32_t)da) - 1);
+                        }
+                        if ((int64_t)match + r[ER_B] - (int64_t)mn > r[ER_A]) { code = 1u << SFC_PTS_SKEW; break; }
+                    }
+                }
                 // ---- InterPodAffinity (filtering.go:317-401) on the counters, p's own increments taken out
                 if (code == SMV_OK && n_filt) {
                     const uint32_t n_soft = (uint32_t)cw[SCW_N_PTS_SOFT], n_aff = (uint32_t)cw[SCW_N_IPA_AFF];
                     const uint32_t n_anti = (uint32_t)cw[SCW_N_IPA_ANTI], n_exist = (uint32_t)cw[SCW_N_IPA_EXIST];
-                    const uint32_t e_aff = n_ports + n_soft, e_anti = e_aff + n_aff, e_exist = e_anti + n_anti, e_end = e_exist + n_exist;
+                    const uint32_t e_aff = n_ports + n_hard + n_soft, e_anti = e_aff + n_aff, e_exist = e_anti + n_anti, e_end = e_exist + n_exist;
                     if (n_aff) {
                         bool pods_exist = true, missing = false;
                         long long aff_total = 0;
@@ -284,6 +424,17 @@ __global__ void __launch_bounds__(256, MINB) simon_moves_kernel(const __grid_con
                             if (d >= 0 && val_at(e, d) > 0) { code = 1u << SFC_IPA_EXIST; break; }
                         }
                 }
+                // ---- Open-Gpu-Share (open-gpu-share.go:51-81) on b's live device memory; p's devices on a do not matter (b != a)
+                if (SCOPED && code == SMV_OK && (bits & SMC_NEED_GPU)) {
+                    if (!cw) cw = P.class_blob + __ldg(P.class_off + cls);
+                    const int64_t req = cw[SCW_GPU_MEM];
+                    SmvGpu gr;
+#pragma unroll
+                    for (int sec = 0; sec < 3; sec++)
+                        smv_ld_sector(reinterpret_cast<unsigned long long *>(&gr) + 4 * sec, reinterpret_cast<const unsigned long long *>(P.gpu + b) + 4 * sec);
+                    slots = smv_gpu_fit(gr, req, cw[SCW_GPU_COUNT]);
+                    if (gr.total < req || slots == 0u) { code = 1u << SFC_GPU; slots = 0u; }
+                }
                 if (code == SMV_OK) {
                     const int32_t on_b = smv_own(nb.alloc_mcpu, nb.alloc_mem, nb.nz_mcpu, nb.nz_mem, kc.score_mcpu, kc.score_mem);
                     const int32_t on_a = smv_own(na.alloc_mcpu, na.alloc_mem, na.nz_mcpu - kc.nz_mcpu, na.nz_mem - kc.nz_mem, kc.score_mcpu, kc.score_mem);
@@ -293,6 +444,7 @@ __global__ void __launch_bounds__(256, MINB) simon_moves_kernel(const __grid_con
         }
         P.out_gain[m] = gain;
         P.out_code[m] = code;
+        if (SCOPED && P.out_slots) P.out_slots[m] = slots;
         if (code == SMV_OK) {
             const uint32_t gm = P.move_base + m;
             const unsigned long long key = ((unsigned long long)(uint32_t)(gain + SMV_GAIN_BIAS) << 32) | (unsigned long long)(0xffffffffu - gm);

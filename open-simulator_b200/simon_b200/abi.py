@@ -91,6 +91,8 @@ def marshal_devices(st):
 
 MOVE_NOOP, MOVE_NOT_PLACED, MOVE_NOT_MOVABLE, MOVE_BAD_INDEX = 1 << 24, 1 << 25, 1 << 26, 1 << 27
 MOVE_GAIN_BIAS = 1000
+# simon_moves_set_scope: admit GPU-share classes / classes with DoNotSchedule spread constraints as move candidates
+MOVES_SCOPE_GPU_SHARE, MOVES_SCOPE_HARD_SPREAD = 1, 2
 
 
 _SNAP_DTYPES = {

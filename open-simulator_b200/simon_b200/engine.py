@@ -25,7 +25,7 @@ EXPORTS = ["simon_gpu_version", "simon_ctx_create", "simon_ctx_destroy", "simon_
            "simon_host_last_error", "simon_host_compile", "simon_host_plan_free", "simon_host_plan_columns", "simon_host_plan_describe",
            "simon_host_simulate", "simon_host_free", "simon_host_quantity_probe", "simon_host_plan_fit_error", "simon_host_capacity_search",
            "simon_storage_upload", "simon_storage_state_download", "simon_devices_upload", "simon_devices_state_download",
-           "simon_scenarios_run_local", "simon_scenarios_storage_download"]
+           "simon_scenarios_run_local", "simon_scenarios_storage_download", "simon_moves_set_scope", "simon_moves_gpu_slots_download"]
 
 
 class EngineUnavailable(RuntimeError):
@@ -97,6 +97,10 @@ def lib():
         L.simon_scenarios_run_local.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.simon_scenarios_storage_download.restype = C.c_int
         L.simon_scenarios_storage_download.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+        L.simon_moves_set_scope.restype = C.c_int
+        L.simon_moves_set_scope.argtypes = [C.c_void_p, C.c_uint32]
+        L.simon_moves_gpu_slots_download.restype = C.c_int
+        L.simon_moves_gpu_slots_download.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
     except AttributeError:
         if not os.environ.get("SIMON_GPU_LIB"):       # an experiment library may lack the newer entry points; the shipped one may not
             raise
@@ -265,8 +269,14 @@ class Engine:
         self._check(lib().simon_moves_upload(self.h, a.ctypes.data, len(a), move_base))
         return len(a)
 
-    def moves_run(self, k: int = 0, want_arrays: bool = True, want_per_pod: bool = False):
-        """-> dict(best_key, n_feasible, kernel_ms, gain, code, best_per_pod, topk=[(move, gain)...])."""
+    def moves_set_scope(self, scope: int):
+        """Admit GPU-share classes (abi.MOVES_SCOPE_GPU_SHARE) and / or classes with DoNotSchedule spread constraints
+        (abi.MOVES_SCOPE_HARD_SPREAD) as move candidates in later runs; 0 = the default scoring."""
+        self._check(lib().simon_moves_set_scope(self.h, scope))
+
+    def moves_run(self, k: int = 0, want_arrays: bool = True, want_per_pod: bool = False, want_gpu_slots: bool = False):
+        """-> dict(best_key, n_feasible, kernel_ms, gain, code, best_per_pod, topk=[(move, gain)...]); with want_gpu_slots (the
+        scope must include GPU share) also gpu_slots: per move the target's device slots, 4 bits per device, 0 if none."""
         n = len(self._moves_keep)
         gain = np.zeros(max(n, 1), np.int32) if want_arrays else None
         code = np.zeros(max(n, 1), np.uint32) if want_arrays else None
@@ -275,9 +285,14 @@ class Engine:
         res = abi.SimonMovesResult()
         self._check(lib().simon_moves_run(self.h, k, gain.ctypes.data if want_arrays else None, code.ctypes.data if want_arrays else None,
                                           bpp.ctypes.data if want_per_pod else None, topk.ctypes.data if k else None, C.byref(res)))
-        return dict(best_key=int(res.best_key), n_feasible=int(res.n_feasible), kernel_ms=float(res.kernel_ms),
-                    gain=None if gain is None else gain[:n], code=None if code is None else code[:n],
-                    best_per_pod=bpp, topk=[(int(topk[q, 0]) & 0xffffffff, int(topk[q, 1])) for q in range(res.n_topk)])
+        out = dict(best_key=int(res.best_key), n_feasible=int(res.n_feasible), kernel_ms=float(res.kernel_ms),
+                   gain=None if gain is None else gain[:n], code=None if code is None else code[:n],
+                   best_per_pod=bpp, topk=[(int(topk[q, 0]) & 0xffffffff, int(topk[q, 1])) for q in range(res.n_topk)])
+        if want_gpu_slots:
+            slots = np.zeros(max(n, 1), np.uint32)
+            self._check(lib().simon_moves_gpu_slots_download(self.h, 0, n, slots.ctypes.data))
+            out["gpu_slots"] = slots[:n]
+        return out
 
     def moves_replay(self, steps: int = 1) -> float:
         ms = C.c_float(0)

@@ -40,9 +40,11 @@ Runner = Callable[[np.ndarray, int, int], Dict]
 """runner(moves_shard [n, 2] uint32, move_base, k) -> dict(best_key, n_feasible, topk=[(global move, gain)], ...)"""
 
 
-def gpu_runner(engine) -> Runner:
-    """Scores a shard on one GPU through the C ABI (simon_moves_upload + simon_moves_run)."""
+def gpu_runner(engine, scope: int = 0) -> Runner:
+    """Scores a shard on one GPU through the C ABI (simon_moves_upload + simon_moves_run); scope: abi.MOVES_SCOPE_* bits that
+    admit GPU-share classes / classes with DoNotSchedule spread constraints (simon_moves_set_scope)."""
     def run(shard: np.ndarray, move_base: int, k: int) -> Dict:
+        engine.moves_set_scope(scope)
         engine.moves_upload(shard, move_base)
         return engine.moves_run(k=k, want_arrays=False)
     return run

@@ -116,8 +116,12 @@ def make_c2(n_nodes: int = 1000, n_workloads: int = 100, replicas: int = 100, se
 
 
 def make_c3(n_nodes: int = 10000, n_workloads: int = 1000, replicas: int = 100, seed_no: int = 3,
-            n_apps: int = 10, prefill_pct: int = 10, prefill_pods: int = 20) -> Tuple[ResourceTypes, List[AppResource]]:
+            n_apps: int = 10, prefill_pct: int = 10, prefill_pods: int = 20, gpu_pct: int = 0) -> Tuple[ResourceTypes, List[AppResource]]:
+    """gpu_pct > 0: GPU-share devices on ~gpu_pct % of the nodes, GPU-share requests on ~15 % of the workloads and a DoNotSchedule
+    zone spread on another ~10 % (placed by the scheduler, so they hold device memory).  These draws come from a second random
+    stream: with gpu_pct = 0 the cluster is the same as without the keyword."""
     rng = SplitMix64(SEED_BASE + seed_no)
+    grng = SplitMix64(SEED_BASE + 0x3000 + seed_no)
     cluster = ResourceTypes()
     hard_taints = [{"key": f"dedicated-{i}", "value": f"team-{i}", "effect": "NoSchedule"} for i in range(8)]
     soft_taints = [{"key": f"degraded-{i}", "value": "true", "effect": "PreferNoSchedule"} for i in range(4)]
@@ -137,6 +141,12 @@ def make_c3(n_nodes: int = 10000, n_workloads: int = 1000, replicas: int = 100, 
         if rng.chance(5):
             taints.append(dict(rng.pick(soft_taints)))
         cluster.Nodes.append(_node(f"node-{i:05d}", cores, zone, region, eph, labels, taints or None))
+        if gpu_pct and grng.chance(gpu_pct):
+            cnt = grng.pick([1, 2, 4, 8])
+            mem = f"{cnt * grng.pick([16, 32, 80])}Gi"
+            for sect in ("allocatable", "capacity"):
+                cluster.Nodes[-1]["status"][sect]["alibabacloud.com/gpu-count"] = str(cnt)
+                cluster.Nodes[-1]["status"][sect]["alibabacloud.com/gpu-mem"] = mem
     # running pods on ~prefill_pct % of the nodes (pre-bound: spec.nodeName set)
     for i in range(n_nodes):
         if not rng.chance(prefill_pct):
@@ -207,7 +217,15 @@ def make_c3(n_nodes: int = 10000, n_workloads: int = 1000, replicas: int = 100, 
                 {"maxSkew": 1 + rng.below(5), "topologyKey": "topology.kubernetes.io/zone",
                  "whenUnsatisfiable": rng.pick(["DoNotSchedule", "ScheduleAnyway"]),
                  "labelSelector": {"matchLabels": {"app": name}}}]
-        apps[w % n_apps].Resource.Deployments.append(_deployment(name, ns, replicas, labels, cpu, mem, extra))
+        if gpu_pct and "topologySpreadConstraints" not in extra and grng.chance(10):
+            extra["topologySpreadConstraints"] = [
+                {"maxSkew": 1 + grng.below(3), "topologyKey": "topology.kubernetes.io/zone", "whenUnsatisfiable": "DoNotSchedule",
+                 "labelSelector": {"matchLabels": {"app": name}}}]
+        dep = _deployment(name, ns, replicas, labels, cpu, mem, extra)
+        if gpu_pct and grng.chance(15):
+            dep["spec"]["template"]["metadata"]["annotations"] = {"alibabacloud.com/gpu-mem": f"{grng.pick([4, 8, 16, 24])}Gi",
+                                                                  "alibabacloud.com/gpu-count": str(grng.pick([1, 1, 1, 2]))}
+        apps[w % n_apps].Resource.Deployments.append(dep)
         cluster.Services.append(_service(name, ns, {"app": name}))
     return cluster, apps
 
