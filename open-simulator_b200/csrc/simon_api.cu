@@ -87,42 +87,39 @@ struct DevBuf {
     ~DevBuf() { release(); }
 };
 
-struct ScenState {
+// The dynamic state of n scenarios, one allocation per column; scenario i owns slice i of each (alloc_pool, clear_pool, fill_scen).
+// The context keeps two: the single-scenario pool (n = 1) and the batch pool, so a batch never touches the single-scenario state.
+struct ScenPool {
+    uint32_t n = 0;
+    // elements of one scenario's slice: node-indexed, req_scalar, counters, counter totals, classes (csum / fbits / ocache rows),
+    // soft and hard constraint tables, out_node, Open-Local VG requested
+    size_t nodes = 1, scal = 1, cntw = 1, nct = 1, ncl = 1, tabw = 1, regw = 1, pods = 1, vn = 1;
     DevBuf<int64_t> req_mcpu, req_mem, req_eph, nz_mcpu, nz_mem, req_scalar, gpu_used;
-    DevBuf<int32_t> num_pods, cnt, cnt_total, tp, fcount, size;
-    DevBuf<long long> csum;
-    DevBuf<uint8_t> fbits;
-    DevBuf<unsigned long long> ocache;
-    DevBuf<uint8_t> hard_reg;
-    DevBuf<int32_t> out_node;
-    DevBuf<int64_t> out_score;
-    DevBuf<uint32_t> out_gpu;
-    DevBuf<uint32_t> fail_counts, fail_pod, counters;   // counters: [0]=n_fail [1]=n_sched
-    DevBuf<unsigned long long> clk;
-    DevBuf<uint32_t> order;
-    DevBuf<int32_t> rank_of;
-};
-
-}  // namespace
-
-struct ScenBatch {
-    DevBuf<int64_t> req_mcpu, req_mem, req_eph, nz_mcpu, nz_mem, req_scalar, gpu_used;
-    DevBuf<int32_t> num_pods, cnt, cnt_total, tp, fcount, size, out_node, rank_of;
+    DevBuf<int32_t> num_pods, cnt, cnt_total, tp, fcount, size, out_node;
     DevBuf<long long> csum;
     DevBuf<uint8_t> fbits, hard_reg;
     DevBuf<unsigned long long> ocache, clk;
-    DevBuf<uint32_t> counters, order;
-    DevBuf<simon_scenario_result> results;
+    DevBuf<uint32_t> counters;          // [n][2]: n_fail, n_sched
+    DevBuf<SkScenario> scen;
+    // per-pod outputs of single runs (null in a batch pool): scores (SIMON_OPT_RECORD_SCORES), GPU-share slots, failure histograms
+    DevBuf<int64_t> out_score;
+    DevBuf<uint32_t> out_gpu, fail_counts, fail_pod;
+    // batches only: each scenario's node order and its inverse (a single run covers every node in index order), the results
+    DevBuf<uint32_t> order;
+    DevBuf<int32_t> rank_of;
     std::vector<uint32_t> h_order;
     std::vector<int32_t> h_rank;
-    // Open-Local state of simon_scenarios_run_local, one slice per scenario: VG requested [n][V][N], allocated device slots [n][N],
-    // the per-decision raw-score scratch [n][N] (clusters of a batch run concurrently: a shared one would be a race)
+    DevBuf<simon_scenario_result> results;
+    DevBuf<simon_scenario_local_result> local_results;
+    uint32_t n_storage = 0;     // scenarios of the last storage batch whose Open-Local slices are kept (0: none since the last upload)
+    // Open-Local, with storage uploaded: VG requested [n][V][N], allocated device slots [n][N] (with devices uploaded) and the
+    // per-decision raw-score scratch [n][N] (clusters of a batch run concurrently: a shared one would be a race)
     DevBuf<int64_t> vg_req;
     DevBuf<uint32_t> dev_alloc;
     DevBuf<int32_t> local_raw;
-    DevBuf<simon_scenario_local_result> local_results;
-    uint32_t n_storage = 0;     // scenarios of the last storage batch whose state the slices hold (0: none since the last upload)
 };
+
+}  // namespace
 
 // dst[i][0 .. len) = src[0 .. len) for every i < n: the scenarios of a batch start from the uploaded Open-Local state
 template <typename T>
@@ -190,7 +187,7 @@ __global__ void simon_scen_reduce(const SkScenario *scen, const int64_t *alloc_m
 }
 
 struct simon_ctx {
-    int device = 0;
+    int device = 0, sms = 132;          // sms: the device's multiprocessor count
     uint32_t opt_cluster = 0, opt_threads = 0, opt_flags = 0;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -201,7 +198,6 @@ struct simon_ctx {
     // snapshot
     uint32_t N = 0, K = 0, WL = 0, WT = 0, T = 0, NC = 0, n_log = 0, max_dom = 1;
     std::vector<uint32_t> topo_ndom;
-    std::vector<int64_t> h_alloc_mcpu, h_alloc_mem;
     DevBuf<uint32_t> d_topo_ndom, d_node_flags;
     DevBuf<int64_t> d_alloc_mcpu, d_alloc_mem, d_alloc_eph, d_alloc_scalar, d_gpu_dev_mem, d_gpu_total_mem;
     DevBuf<int32_t> d_alloc_pods, d_topo_dom, d_node_class, d_gpu_count;
@@ -246,28 +242,24 @@ struct simon_ctx {
     size_t gnode_stride = 0;
     DevBuf<uint32_t> d_sig_class;       // a class per static signature (dense fill of the static verdict cache)
     bool static_filled = false;
-    // single-scenario state
-    ScenState st;
+    // scenario state: single runs (simon_schedule, simon_replay, ...) and scenario batches
+    ScenPool single, batch;
     uint32_t max_fail = 0;
-    DevBuf<SkScenario> d_scen;
     DevBuf<unsigned long long> d_stats, d_scache;
     uint32_t n_sigs = 1, use_scache = 0, simon32 = 0;
-    // multi-scenario state
-    std::vector<ScenState *> scen_states;
-    ScenBatch *batch = nullptr;
-    // Open-Local LVM volumes (simon_storage_upload); single-scenario state: VG requested [V][N] and the raw score scratch [N]
+    // Open-Local LVM volumes (simon_storage_upload); VG requested [V][N] as uploaded (every scenario starts from it)
     bool have_storage = false;
     uint32_t V = 0;
-    DevBuf<int32_t> d_node_n_vg, d_vg_name, d_vol_vg, d_local_raw;
-    DevBuf<int64_t> d_vg_cap, d_vg_req0, d_vg_req, d_vol_size;
+    DevBuf<int32_t> d_node_n_vg, d_vg_name, d_vol_vg;
+    DevBuf<int64_t> d_vg_cap, d_vg_req0, d_vol_size;
     DevBuf<uint8_t> d_class_local;
     DevBuf<uint32_t> d_vol_off;
     std::vector<uint8_t> h_class_local;
-    // Open-Local devices (simon_devices_upload); allocated-slot masks [N], as uploaded and the current state
+    // Open-Local devices (simon_devices_upload); allocated-slot masks [N] as uploaded
     bool have_devices = false;
     DevBuf<uint8_t> d_node_n_ssd, d_node_n_hdd;
     DevBuf<int64_t> d_dev_cap, d_ssd_size, d_hdd_size;
-    DevBuf<uint32_t> d_ssd_off, d_hdd_off, d_dev_alloc0, d_dev_alloc;
+    DevBuf<uint32_t> d_ssd_off, d_hdd_off, d_dev_alloc0;
 };
 
 namespace {
@@ -288,66 +280,92 @@ int fail(simon_ctx *c, int code, const char *fmt, ...) {
         if (e__ != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "%s: %s", #call, cudaGetErrorString(e__)); \
     } while (0)
 
-int alloc_state(simon_ctx *ctx, ScenState &s, uint32_t max_fail, bool scores) {
-    const uint32_t N = ctx->N, K = ctx->K ? ctx->K : 1;
-    CU(s.req_mcpu.alloc(N)); CU(s.req_mem.alloc(N)); CU(s.req_eph.alloc(N)); CU(s.nz_mcpu.alloc(N)); CU(s.nz_mem.alloc(N));
-    CU(s.req_scalar.alloc((size_t)K * N)); CU(s.gpu_used.alloc((size_t)SIMON_MAX_GPU_DEV * N)); CU(s.num_pods.alloc(N));
-    CU(s.cnt.alloc(ctx->cnt_words)); CU(s.cnt_total.alloc(ctx->n_counters));
-    CU(s.tp.alloc((size_t)SK_MAX_SOFT * ctx->max_dom)); CU(s.fcount.alloc((size_t)SK_MAX_SOFT * ctx->max_dom));
-    CU(s.size.alloc(SK_MAX_SOFT)); CU(s.hard_reg.alloc((size_t)SK_MAX_HARD * ctx->max_dom));
-    CU(s.csum.alloc((size_t)ctx->n_classes * SK_CSUM_W));
-    CU(s.fbits.alloc((size_t)ctx->n_classes * N));
-    CU(s.ocache.alloc((size_t)ctx->n_classes * N));
-    CU(cudaMemsetAsync(s.ocache.p, 0, 8ull * std::max<size_t>(1, (size_t)ctx->n_classes * N), ctx->stream));
-    CU(cudaMemsetAsync(s.csum.p, 0, 8ull * std::max<size_t>(1, (size_t)ctx->n_classes * SK_CSUM_W), ctx->stream));
-    CU(cudaMemsetAsync(s.fbits.p, 0, std::max<size_t>(1, (size_t)ctx->n_classes * N), ctx->stream));
-    CU(s.out_node.alloc(ctx->n_pods));
-    if (scores) CU(s.out_score.alloc(ctx->n_pods));
-    CU(s.out_gpu.alloc(ctx->n_pods));
-    CU(s.fail_counts.alloc((size_t)max_fail * SIMON_N_FAIL_CODES)); CU(s.fail_pod.alloc(max_fail)); CU(s.counters.alloc(2));
-    CU(s.clk.alloc(2));
-    return SIMON_OK;
+// The SkScenario of scenario i of the pool, over its first n_active nodes (identity: every node in index order, no node list).
+// The per-pod outputs of single runs are not sliced: a pool that has them holds one scenario.
+SkScenario fill_scen(const ScenPool &s, uint32_t i, uint32_t n_active, bool identity) {
+    SkScenario o{};
+    const size_t nn = (size_t)i * s.nodes;
+    o.order = identity ? nullptr : s.order.p + nn;
+    o.rank_of = identity ? nullptr : s.rank_of.p + nn;
+    o.n_active = n_active;
+    o.req_mcpu = s.req_mcpu.p + nn; o.req_mem = s.req_mem.p + nn; o.req_eph = s.req_eph.p + nn;
+    o.nz_mcpu = s.nz_mcpu.p + nn; o.nz_mem = s.nz_mem.p + nn;
+    o.req_scalar = s.req_scalar.p + i * s.scal; o.gpu_used = s.gpu_used.p + nn * SIMON_MAX_GPU_DEV;
+    o.num_pods = s.num_pods.p + nn; o.cnt = s.cnt.p + i * s.cntw; o.cnt_total = s.cnt_total.p + i * s.nct;
+    o.tp = s.tp.p + i * s.tabw; o.fcount = s.fcount.p + i * s.tabw; o.size = s.size.p + (size_t)i * SK_MAX_SOFT;
+    o.hard_reg = s.hard_reg.p + i * s.regw;
+    o.csum = s.csum.p + i * s.ncl * SK_CSUM_W; o.fbits = s.fbits.p + nn * s.ncl; o.ocache = s.ocache.p + nn * s.ncl;
+    o.out_node = s.out_node.p + i * s.pods; o.out_score = s.out_score.p; o.out_gpu = s.out_gpu.p;
+    o.fail_counts = s.fail_counts.p; o.fail_pod = s.fail_pod.p; o.n_fail = s.counters.p + 2ull * i; o.n_sched = s.counters.p + 2ull * i + 1;
+    o.clk = s.clk.p + 2ull * i;
+    return o;
 }
 
-int reset_state(simon_ctx *ctx, ScenState &s) {
+// dst[i][0 .. len) = src[0 .. len) for every i < n, on the context's stream
+template <typename T>
+cudaError_t bcast(simon_ctx *ctx, const T *src, size_t len, uint32_t n, T *dst) {
+    simon_bcast<<<(uint32_t)std::min<size_t>((n * len + 255) / 256, (size_t)ctx->sms * 8), 256, 0, ctx->stream>>>(src, len, n, dst);
+    return cudaGetLastError();
+}
+
+// Every scenario of the pool back to the empty cluster: one memset per column, and the Open-Local state from the uploaded values
+// with one broadcast per column.  The constraint tables (tp, fcount, size, hard_reg) are not cleared: the kernel zeroes the rows
+// it uses.  Each kind of run clears its own counters (and a batch its clocks).
+int clear_pool(simon_ctx *ctx, ScenPool &s) {
     cudaStream_t st = ctx->stream;
-    const uint32_t N = ctx->N, K = ctx->K ? ctx->K : 1;
-    CU(cudaMemsetAsync(s.req_mcpu.p, 0, 8ull * N, st)); CU(cudaMemsetAsync(s.req_mem.p, 0, 8ull * N, st));
-    CU(cudaMemsetAsync(s.req_eph.p, 0, 8ull * N, st)); CU(cudaMemsetAsync(s.nz_mcpu.p, 0, 8ull * N, st));
-    CU(cudaMemsetAsync(s.nz_mem.p, 0, 8ull * N, st)); CU(cudaMemsetAsync(s.req_scalar.p, 0, 8ull * K * N, st));
-    CU(cudaMemsetAsync(s.gpu_used.p, 0, 8ull * SIMON_MAX_GPU_DEV * N, st)); CU(cudaMemsetAsync(s.num_pods.p, 0, 4ull * N, st));
-    CU(cudaMemsetAsync(s.cnt.p, 0, 4ull * (ctx->cnt_words ? ctx->cnt_words : 1), st));
-    CU(cudaMemsetAsync(s.cnt_total.p, 0, 4ull * (ctx->n_counters ? ctx->n_counters : 1), st));
+    const size_t n = s.n, nn = n * s.nodes;
+    CU(cudaMemsetAsync(s.req_mcpu.p, 0, 8 * nn, st)); CU(cudaMemsetAsync(s.req_mem.p, 0, 8 * nn, st));
+    CU(cudaMemsetAsync(s.req_eph.p, 0, 8 * nn, st)); CU(cudaMemsetAsync(s.nz_mcpu.p, 0, 8 * nn, st));
+    CU(cudaMemsetAsync(s.nz_mem.p, 0, 8 * nn, st)); CU(cudaMemsetAsync(s.req_scalar.p, 0, 8 * n * s.scal, st));
+    CU(cudaMemsetAsync(s.gpu_used.p, 0, 8 * nn * SIMON_MAX_GPU_DEV, st)); CU(cudaMemsetAsync(s.num_pods.p, 0, 4 * nn, st));
+    CU(cudaMemsetAsync(s.cnt.p, 0, 4 * n * s.cntw, st)); CU(cudaMemsetAsync(s.cnt_total.p, 0, 4 * n * s.nct, st));
     // the own-score cache is keyed by the node's pod count, which restarts with the state
-    if (s.ocache.p) CU(cudaMemsetAsync(s.ocache.p, 0, 8ull * std::max<size_t>(1, (size_t)ctx->n_classes * N), st));
+    CU(cudaMemsetAsync(s.ocache.p, 0, 8 * nn * s.ncl, st));
     // the stored feasible-set summaries (and the feasibility bits they are exact for) describe the node set and order of
     // the run that wrote them: a state that restarts from empty - possibly with another scenario's node list - must not
     // inherit them (the kernel validates a summary only against flips of nodes it currently owns)
-    if (s.csum.p) CU(cudaMemsetAsync(s.csum.p, 0, 8ull * std::max<size_t>(1, (size_t)ctx->n_classes * SK_CSUM_W), st));
-    // VG requested restarts from what the node annotations state
-    if (&s == &ctx->st && ctx->have_storage)
-        CU(cudaMemcpyAsync(ctx->d_vg_req.p, ctx->d_vg_req0.p, 8ull * ctx->V * N, cudaMemcpyDeviceToDevice, st));
-    // and the devices from what they state
-    if (&s == &ctx->st && ctx->have_devices)
-        CU(cudaMemcpyAsync(ctx->d_dev_alloc.p, ctx->d_dev_alloc0.p, 4ull * std::max(1u, N), cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemsetAsync(s.csum.p, 0, 8 * n * s.ncl * SK_CSUM_W, st));
+    // VG requested and the devices restart from what the node annotations state
+    if (ctx->have_storage) CU(bcast(ctx, ctx->d_vg_req0.p, s.vn, s.n, s.vg_req.p));
+    if (ctx->have_devices) CU(bcast(ctx, ctx->d_dev_alloc0.p, s.nodes, s.n, s.dev_alloc.p));
     return SIMON_OK;
 }
 
-void fill_scen(simon_ctx *ctx, ScenState &s, SkScenario &o, uint32_t n_active, bool identity) {
-    o.order = identity ? nullptr : s.order.p;
-    o.rank_of = identity ? nullptr : s.rank_of.p;
-    o.n_active = n_active;
-    o.pad = 0;
-    o.req_mcpu = s.req_mcpu.p; o.req_mem = s.req_mem.p; o.req_eph = s.req_eph.p; o.nz_mcpu = s.nz_mcpu.p; o.nz_mem = s.nz_mem.p;
-    o.req_scalar = s.req_scalar.p; o.gpu_used = s.gpu_used.p; o.num_pods = s.num_pods.p; o.cnt = s.cnt.p; o.cnt_total = s.cnt_total.p;
-    o.tp = s.tp.p; o.fcount = s.fcount.p; o.size = s.size.p; o.hard_reg = s.hard_reg.p; o.csum = s.csum.p; o.fbits = s.fbits.p; o.ocache = s.ocache.p;
-    o.out_node = s.out_node.p; o.out_score = s.out_score.p; o.out_gpu = s.out_gpu.p;
-    o.fail_counts = s.fail_counts.p; o.fail_pod = s.fail_pod.p; o.n_fail = s.counters.p; o.n_sched = s.counters.p + 1;
-    o.clk = s.clk.p;
-    (void)ctx;
+// Size every column of `s` for n scenarios of the current uploads (DevBuf keeps the capacity) and clear it.  single: the pool of
+// single runs, with their per-pod outputs and its one SkScenario (every node) uploaded; else a batch pool, with node lists and results.
+int alloc_pool(simon_ctx *ctx, ScenPool &s, uint32_t n, bool single) {
+    s.n = n;
+    s.nodes = std::max(1u, ctx->N); s.scal = (size_t)(ctx->K ? ctx->K : 1) * s.nodes;
+    s.cntw = std::max<uint64_t>(1, ctx->cnt_words); s.nct = std::max(1u, ctx->n_counters); s.ncl = std::max(1u, ctx->n_classes);
+    s.tabw = (size_t)SK_MAX_SOFT * ctx->max_dom; s.regw = (size_t)SK_MAX_HARD * ctx->max_dom; s.pods = std::max(1u, ctx->n_pods);
+    s.vn = std::max<size_t>(1, (size_t)ctx->V * ctx->N);
+    const size_t nn = (size_t)n * s.nodes;
+    CU(s.req_mcpu.alloc(nn)); CU(s.req_mem.alloc(nn)); CU(s.req_eph.alloc(nn)); CU(s.nz_mcpu.alloc(nn)); CU(s.nz_mem.alloc(nn));
+    CU(s.req_scalar.alloc(n * s.scal)); CU(s.gpu_used.alloc(nn * SIMON_MAX_GPU_DEV)); CU(s.num_pods.alloc(nn));
+    CU(s.cnt.alloc(n * s.cntw)); CU(s.cnt_total.alloc(n * s.nct));
+    CU(s.tp.alloc(n * s.tabw)); CU(s.fcount.alloc(n * s.tabw)); CU(s.size.alloc((size_t)n * SK_MAX_SOFT)); CU(s.hard_reg.alloc(n * s.regw));
+    CU(s.csum.alloc(n * s.ncl * SK_CSUM_W)); CU(s.fbits.alloc(nn * s.ncl)); CU(s.ocache.alloc(nn * s.ncl));
+    CU(s.out_node.alloc(n * s.pods)); CU(s.counters.alloc(2ull * n)); CU(s.clk.alloc(2ull * n)); CU(s.scen.alloc(n));
+    if (single) {
+        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(s.out_score.alloc(ctx->n_pods));
+        CU(s.out_gpu.alloc(ctx->n_pods));
+        CU(s.fail_counts.alloc((size_t)ctx->max_fail * SIMON_N_FAIL_CODES)); CU(s.fail_pod.alloc(ctx->max_fail));
+        // fbits are cleared here for single runs and never for batches: the kernel reads them only under a valid csum record
+        CU(cudaMemsetAsync(s.fbits.p, 0, nn * s.ncl, ctx->stream));
+        const SkScenario sc = fill_scen(s, 0, ctx->N, true);
+        CU(cudaMemcpyAsync(s.scen.p, &sc, sizeof(sc), cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));        // `sc` leaves scope
+    } else {
+        CU(s.order.alloc(nn)); CU(s.rank_of.alloc(nn)); CU(s.results.alloc(n));
+        if (ctx->have_storage) CU(s.local_results.alloc(n));
+    }
+    if (ctx->have_storage) { CU(s.vg_req.alloc(n * s.vn)); CU(s.local_raw.alloc(nn)); }
+    if (ctx->have_devices) CU(s.dev_alloc.alloc(nn));
+    return clear_pool(ctx, s);
 }
 
-void fill_params(simon_ctx *ctx, SkParams &P) {
+// the launch parameters of the current uploads on pool `s` (its SkScenario array and Open-Local slices)
+void fill_params(simon_ctx *ctx, const ScenPool &s, SkParams &P) {
     memset(&P, 0, sizeof(P));
     P.N = ctx->N; P.K = ctx->K; P.WL = ctx->WL; P.WT = ctx->WT; P.T = ctx->T; P.NC = ctx->NC; P.n_log = ctx->n_log; P.max_dom = ctx->max_dom;
     P.topo_ndom = ctx->d_topo_ndom.p; P.alloc_mcpu = ctx->d_alloc_mcpu.p; P.alloc_mem = ctx->d_alloc_mem.p; P.alloc_eph = ctx->d_alloc_eph.p;
@@ -364,15 +382,16 @@ void fill_params(simon_ctx *ctx, SkParams &P) {
     P.n_sigs = ctx->n_sigs; P.use_scache = ctx->use_scache; P.simon32 = ctx->simon32; P.scache = ctx->d_scache.p;
     P.cls_aux = ctx->d_cls_aux.p;
     P.dump_pod = 0xffffffffu; P.dump_total = nullptr; P.dump_code = nullptr;
+    P.scen = s.scen.p;
     if (ctx->have_storage) {
         P.V = ctx->V; P.node_n_vg = ctx->d_node_n_vg.p; P.vg_name = ctx->d_vg_name.p; P.vg_cap = ctx->d_vg_cap.p;
         P.class_local = ctx->d_class_local.p; P.vol_off = ctx->d_vol_off.p; P.vol_size = ctx->d_vol_size.p; P.vol_vg = ctx->d_vol_vg.p;
-        P.vg_req = ctx->d_vg_req.p; P.local_raw = ctx->d_local_raw.p;
+        P.vg_req = s.vg_req.p; P.local_raw = s.local_raw.p; P.vg_req_stride = s.vn; P.node_stride = s.nodes;
     }
     if (ctx->have_devices) {
         P.node_n_ssd = ctx->d_node_n_ssd.p; P.node_n_hdd = ctx->d_node_n_hdd.p; P.dev_cap = ctx->d_dev_cap.p;
         P.ssd_off = ctx->d_ssd_off.p; P.ssd_size = ctx->d_ssd_size.p; P.hdd_off = ctx->d_hdd_off.p; P.hdd_size = ctx->d_hdd_size.p;
-        P.dev_alloc = ctx->d_dev_alloc.p;
+        P.dev_alloc = s.dev_alloc.p;
     }
 }
 
@@ -380,9 +399,17 @@ void fill_params(simon_ctx *ctx, SkParams &P) {
 #define SIMON_AUTO_TPB 320u
 
 typedef void (*sk_kernel_fn)(const SkParams);
-// the compiled kernel variant for (threads per CTA, node slots per thread); nullptr: none
-sk_kernel_fn pick_kernel(uint32_t TPB, uint32_t npt, bool prof) {
-    if (TPB > 384) return nullptr;
+// The compiled kernel variant for (threads per CTA, node slots per thread) on the context's uploads, which is what launch() runs
+// and what the geometry is sized for.  big: the large-cluster variant; prof: with per-phase clock64 timers.  With Open-Local
+// storage uploaded, the local variants (more registers than the plain ones, runtime node slots per thread, no timers).
+// nullptr: none.
+sk_kernel_fn kernel_variant(const simon_ctx *ctx, uint32_t TPB, uint32_t npt, bool big, bool prof) {
+    if (big) return ctx->have_storage ? simon_local_kernel_big : simon_place_kernel_big;
+    if (TPB > SIMON_MAX_TPB) return nullptr;
+    if (ctx->have_storage) {
+        if (prof) return nullptr;
+        return TPB <= 256 ? simon_local_kernel_256 : TPB <= 320 ? simon_local_kernel_320 : simon_local_kernel_384;
+    }
     if (TPB > 320) {
         if (prof) return nullptr;
         return npt == 1 ? simon_place_kernel_384_1 : npt == 2 ? simon_place_kernel_384_2 : npt == 3 ? simon_place_kernel_384_3 : simon_place_kernel_384_0;
@@ -395,35 +422,39 @@ sk_kernel_fn pick_kernel(uint32_t TPB, uint32_t npt, bool prof) {
     return npt == 1 ? simon_place_kernel_256_1 : npt == 2 ? simon_place_kernel_256_2 : npt == 3 ? simon_place_kernel_256_3 : npt == 4 ? simon_place_kernel_256_4 : simon_place_kernel_256_0;
 }
 
-// the variant launch() runs for this shape, which is what the geometry must be sized for: with Open-Local storage uploaded the
-// local variants (more registers than the plain ones), else pick_kernel's
-sk_kernel_fn launch_kernel(const simon_ctx *ctx, uint32_t TPB, uint32_t npt) {
-    if (!ctx->have_storage) return pick_kernel(TPB, npt, false);
-    if (TPB > SIMON_MAX_TPB) return nullptr;
-    return TPB <= 256 ? simon_local_kernel_256 : TPB <= 320 ? simon_local_kernel_320 : simon_local_kernel_384;
-}
-
-// clusters of `cs` CTAs x `t` threads with `smem` bytes each that the device holds at once (GPC boundaries included)
-int max_active_clusters(sk_kernel_fn fn, uint32_t cs, uint32_t t, size_t smem) {
-    if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return 0; }
-    if (cs > 8 && cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1) != cudaSuccess) { cudaGetLastError(); return 0; }
-    cudaLaunchConfig_t cfg;
+// A launch of fn on `ctas` CTAs in clusters of `cs`, `t` threads and `smem` bytes of shared memory each, with fn's attributes set
+// for that shape.  cfg points to attr.
+cudaError_t cluster_config(sk_kernel_fn fn, uint32_t ctas, uint32_t cs, uint32_t t, size_t smem, cudaStream_t st, cudaLaunchConfig_t &cfg,
+                           cudaLaunchAttribute &attr) {
+    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess && cs > 8) e = cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(cs, 1, 1);
+    cfg.gridDim = dim3(ctas, 1, 1);
     cfg.blockDim = dim3(t, 1, 1);
     cfg.dynamicSmemBytes = smem;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
+    cfg.stream = st;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = cs; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
     cfg.numAttrs = 1;
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, fn, &cfg) != cudaSuccess) { cudaGetLastError(); return 0; }
-    return n;
+    return e;
 }
 
-// whether one cluster of this shape can be resident at all (a 16-CTA cluster needs 16 free SMs in one GPC)
-bool resident(sk_kernel_fn fn, uint32_t cs, uint32_t t, size_t smem) { return fn && max_active_clusters(fn, cs, t, smem) > 0; }
+// Clusters of `cs` CTAs x `t` threads x `npt` node slots with `smem` bytes each of the variant for that shape that the device
+// holds at once, GPC boundaries included (0: not even one; a 16-CTA cluster needs 16 free SMs in one GPC).  The variants with
+// phase timers run in the geometry of the default ones.
+int max_active_clusters(const simon_ctx *ctx, bool big, uint32_t cs, uint32_t t, uint32_t npt, size_t smem) {
+    const sk_kernel_fn fn = kernel_variant(ctx, t, npt, big, false);
+    if (!fn) return 0;
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute attr;
+    int n = 0;
+    if (cluster_config(fn, cs, cs, t, smem, nullptr, cfg, attr) != cudaSuccess || cudaOccupancyMaxActiveClusters(&n, fn, &cfg) != cudaSuccess) {
+        cudaGetLastError();
+        return 0;
+    }
+    return n;
+}
 
 // choose cluster size / threads / nodes-per-thread for n_active nodes
 int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &TPB, uint32_t &NPT, size_t &smem, uint32_t n_scen = 1) {
@@ -433,7 +464,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
     const uint32_t want_cs = ctx->opt_cluster, want_t = ctx->opt_threads;
     if (n_active == 0) n_active = 1;
     ctx->big = false;
-    if (n_scen > 1 && !want_cs && !want_t && !getenv("SIMON_OLD_BATCH_GEOMETRY")) {
+    if (n_scen > 1 && !want_cs && !want_t) {
         // Batches are throughput work.  For every cluster size 1..16 (any integer: clusters need not be powers of two) take the
         // thread count with the fewest node slots per thread, ask the driver how many such clusters the device holds at once
         // (shared memory, registers and GPC boundaries included), and minimise  waves x time of one scenario,  the latter a
@@ -457,45 +488,14 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
             if (npt > 64) continue;
             const size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs);
             if (b > (size_t)max_smem) continue;
-            sk_kernel_fn fn = launch_kernel(ctx, t, npt);
-            if (!fn) continue;
-            const int active = max_active_clusters(fn, cs, t, b);
+            const int active = max_active_clusters(ctx, false, cs, t, npt, b);
             if (active <= 0) continue;
             const uint32_t waves = (n_scen + (uint32_t)active - 1) / (uint32_t)active;
             const double cost = waves * (265.0 + 196.0 * npt + (t > 320 ? 18.0 : 0.0) + 5.0 * cs);
             if (!b_cs || cost < best_cost) { best_cost = cost; b_cs = cs; b_t = t; b_npt = npt; b_smem = b; }
         }
         if (b_cs) { CS = b_cs; TPB = b_t; NPT = b_npt; smem = b_smem; return SIMON_OK; }
-    }
-    if (n_scen > 1 && !want_cs && !want_t) {
-        // (fallback: the rule used before cudaOccupancyMaxActiveClusters was consulted)  Batches are throughput work: small clusters
-        // waste the least on synchronisation (fewer CTAs wait in each cluster-wide exchange).  Take the
-        // smallest cluster that fits shared memory while the batch still fills about half of the SMs; a batch too small for
-        // that gets the largest cluster with which it still runs in one wave.
-        uint32_t fit_cs[5], fit_t[5], fit_npt[5], nfit = 0;
-        size_t fit_smem[5];
-        for (uint32_t cs = 1; cs <= 16; cs *= 2) {
-            const uint32_t per_cta = (n_active + cs - 1) / cs;
-            uint32_t t = per_cta >= 256 ? 256u : std::max(64u, ((per_cta + 31) / 32) * 32);
-            if (per_cta > 256 && (per_cta + 319) / 320 < (per_cta + 255) / 256) t = 320;      // fewer nodes per thread wins (C3: 8 x 320 x 4)
-            const uint32_t npt = (per_cta + t - 1) / t;
-            const size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs);
-            if (npt <= 64 && b <= (size_t)max_smem) { fit_cs[nfit] = cs; fit_t[nfit] = t; fit_npt[nfit] = npt; fit_smem[nfit] = b; nfit++; }
-        }
-        if (nfit) {
-            int sms = 132;
-            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
-            int pick = -1;
-            for (uint32_t q = 0; q < nfit && pick < 0; q++)
-                if ((uint64_t)n_scen * fit_cs[q] >= (uint64_t)sms / 2) pick = (int)q;
-            if (pick < 0) {
-                pick = 0;
-                for (uint32_t q = 0; q < nfit; q++)
-                    if ((uint64_t)n_scen * fit_cs[q] <= (uint64_t)sms) pick = (int)q;
-            }
-            CS = fit_cs[pick]; TPB = fit_t[pick]; NPT = fit_npt[pick]; smem = fit_smem[pick];
-            return SIMON_OK;
-        }
+        // no resident geometry of that form: the residency-checked search below, then the large-cluster variant
     }
     if (want_cs > SK_MAX_CS) return fail(ctx, SIMON_ERR_LIMIT, "CTAs per scenario must be <= %u (got %u)", (unsigned)SK_MAX_CS, want_cs);
     if (n_scen <= 1 && !want_cs && !want_t && n_active > 128) {
@@ -516,7 +516,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
             if (n384 < npt_p) { t_p = 384; npt_p = n384; }
         }
         const size_t b = sk_smem_bytes(npt_p * t_p, ctx->T, ctx->emax, ctx->max_blob_words, cs_p);
-        if (npt_p <= 64 && b <= (size_t)max_smem && resident(launch_kernel(ctx, t_p, npt_p), cs_p, t_p, b)) {
+        if (npt_p <= 64 && b <= (size_t)max_smem && max_active_clusters(ctx, false, cs_p, t_p, npt_p, b) > 0) {
             CS = cs_p; TPB = t_p; NPT = npt_p; smem = b; return SIMON_OK;
         }
     }
@@ -537,7 +537,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
             }
             if (t > SIMON_MAX_TPB) return fail(ctx, SIMON_ERR_LIMIT, "threads per CTA must be <= %u (got %u)", SIMON_MAX_TPB, t);
             size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs);
-            if (b <= (size_t)max_smem && (want_cs || resident(launch_kernel(ctx, t, npt), cs, t, b))) {
+            if (b <= (size_t)max_smem && (want_cs || max_active_clusters(ctx, false, cs, t, npt, b) > 0)) {
                 CS = cs; TPB = t; NPT = npt; smem = b; return SIMON_OK;
             }
             if (want_t) break;
@@ -549,7 +549,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
         const uint32_t cs = 16, t = 320;
         const uint32_t npt = (n_active + cs * t - 1) / (cs * t);
         const size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs, false);
-        if (npt <= 64 && b <= (size_t)max_smem && resident(ctx->have_storage ? simon_local_kernel_big : simon_place_kernel_big, cs, t, b)) {
+        if (npt <= 64 && b <= (size_t)max_smem && max_active_clusters(ctx, true, cs, t, npt, b) > 0) {
             CS = cs; TPB = t; NPT = npt; smem = b;
             ctx->big = true;
             ctx->gnode_stride = (sk_node_bytes(npt * t, ctx->T, ctx->emax) + 255) & ~(size_t)255;
@@ -562,39 +562,20 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
 static_assert(sizeof(SkScenario) % 8 == 0, "SkScenario is copied in 8-byte words");
 
 int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t TPB, size_t smem, bool record = true) {
-    sk_kernel_fn fn;
-    const uint32_t npt = P.npt;
-    if (TPB > SIMON_MAX_TPB) return fail(ctx, SIMON_ERR_LIMIT, "threads per CTA must be <= %u", SIMON_MAX_TPB);
     // SIMON_PROFILE=1 selects the variants with per-phase clock64 timers (simon_stats cycles); the default variants
     // carry no timers
     static const bool prof = getenv("SIMON_PROFILE") != nullptr;
+    const sk_kernel_fn fn = kernel_variant(ctx, TPB, P.npt, ctx->big, prof);
+    if (!fn)
+        return fail(ctx, SIMON_ERR_LIMIT, "no kernel variant for %u threads per CTA%s%s", TPB, prof ? " with phase timers" : "",
+                    ctx->have_storage ? " and Open-Local storage" : "");
     if (ctx->big) {
         CU(ctx->d_gnode.alloc(ctx->gnode_stride * (size_t)n_scen * CS));
         P.gnode = ctx->d_gnode.p; P.gnode_stride = ctx->gnode_stride;
-        fn = P.class_local ? simon_local_kernel_big : simon_place_kernel_big;
-    } else if (P.class_local) {
-        // Open-Local storage uploaded: the variants that carry its filter, score and bind (runtime node slots per thread)
-        if (prof) return fail(ctx, SIMON_ERR_LIMIT, "no kernel variant with phase timers and Open-Local storage");
-        fn = TPB <= 256 ? simon_local_kernel_256 : TPB <= 320 ? simon_local_kernel_320 : simon_local_kernel_384;
-    } else {
-        fn = pick_kernel(TPB, npt, prof);
-        if (!fn) return fail(ctx, SIMON_ERR_LIMIT, "no kernel variant for %u threads per CTA%s", TPB, prof ? " with phase timers" : "");
     }
-    CU(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if (CS > 8) CU(cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(n_scen * CS, 1, 1);
-    cfg.blockDim = dim3(TPB, 1, 1);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CS;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
+    cudaLaunchAttribute attr;
+    CU(cluster_config(fn, n_scen * CS, CS, TPB, smem, ctx->stream, cfg, attr));
     if (record) CU(cudaEventRecord(ctx->ev0, ctx->stream));
     CU(cudaLaunchKernelEx(&cfg, fn, P));
     if (record) CU(cudaEventRecord(ctx->ev1, ctx->stream));
@@ -610,9 +591,7 @@ int launch_range(simon_ctx *ctx, SkParams &P, uint32_t CS, uint32_t TPB, size_t 
     if (n_pre < 256) n_pre = 0;
     if (record) CU(cudaEventRecord(ctx->ev0, ctx->stream));
     if (n_pre) {
-        int sms = 132;
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
-        const uint32_t grid = std::min<uint32_t>((n_pre + 255) / 256, (uint32_t)sms * 4);
+        const uint32_t grid = std::min<uint32_t>((n_pre + 255) / 256, (uint32_t)ctx->sms * 4);
         simon_import_kernel<<<grid, 256, 0, ctx->stream>>>(P, first, n_pre);
         CU(cudaGetLastError());
         ctx->launches++;
@@ -652,6 +631,7 @@ int simon_ctx_create(const simon_ctx_opts *opts, simon_ctx **out) {
         delete ctx;
         return SIMON_ERR_CUDA;
     }
+    cudaDeviceGetAttribute(&ctx->sms, cudaDevAttrMultiProcessorCount, ctx->device);
     *out = ctx;
     return SIMON_OK;
 }
@@ -659,8 +639,6 @@ int simon_ctx_create(const simon_ctx_opts *opts, simon_ctx **out) {
 void simon_ctx_destroy(simon_ctx *ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
-    for (auto *s : ctx->scen_states) delete s;
-    delete ctx->batch;
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
@@ -681,8 +659,6 @@ int simon_snapshot_upload(simon_ctx *ctx, const simon_snapshot *s) {
     ctx->topo_ndom.assign(s->topo_ndom, s->topo_ndom + s->n_topos);
     ctx->max_dom = 1;
     for (uint32_t t = 0; t < s->n_topos; t++) ctx->max_dom = std::max(ctx->max_dom, s->topo_ndom[t]);
-    ctx->h_alloc_mcpu.assign(s->alloc_mcpu, s->alloc_mcpu + N);
-    ctx->h_alloc_mem.assign(s->alloc_mem, s->alloc_mem + N);
     const uint32_t K1 = ctx->K ? ctx->K : 1;
     CU(ctx->d_topo_ndom.upload(s->topo_ndom, s->n_topos, st));
     CU(ctx->d_alloc_mcpu.upload(s->alloc_mcpu, N, st)); CU(ctx->d_alloc_mem.upload(s->alloc_mem, N, st));
@@ -698,7 +674,7 @@ int simon_snapshot_upload(simon_ctx *ctx, const simon_snapshot *s) {
     ctx->have_pods = false;
     ctx->have_storage = false;
     ctx->have_devices = false;
-    if (ctx->batch) ctx->batch->n_storage = 0;
+    ctx->batch.n_storage = 0;
     return SIMON_OK;
 }
 
@@ -709,7 +685,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     cudaStream_t st = ctx->stream;
     ctx->have_storage = false;          // the storage tables are per class: a new pod set needs its own upload
     ctx->have_devices = false;
-    if (ctx->batch) ctx->batch->n_storage = 0;
+    ctx->batch.n_storage = 0;
     ctx->n_classes = p->n_classes; ctx->n_pods = p->n_pods; ctx->n_counters = p->n_counters;
     // validate classes; derive limits
     uint32_t max_words = SCW_HDR_WORDS, emax = 0;
@@ -882,11 +858,8 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     for (uint32_t i = 0; i < p->n_pods; i++) ctx->bypass[i] = (guard[i] == -2 || p->pod_fixed_node[i] != -1) ? 1 : 0;
     CU(cudaStreamSynchronize(st));
     ctx->max_fail = std::max(1u, p->n_pods);      // every pod of the list may fail: one histogram row each (96 B)
-    int rc = alloc_state(ctx, ctx->st, ctx->max_fail, (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) != 0);
+    int rc = alloc_pool(ctx, ctx->single, 1, true);
     if (rc) return rc;
-    rc = reset_state(ctx, ctx->st);
-    if (rc) return rc;
-    CU(ctx->d_scen.alloc(1));
     ctx->n_sigs = std::max(1u, p->n_static_sigs);
     {
         size_t words = (size_t)ctx->n_sigs * std::max(1u, ctx->N);
@@ -907,7 +880,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
 int simon_state_reset(simon_ctx *ctx) {
     if (!ctx || !ctx->have_pods) return ctx ? fail(ctx, SIMON_ERR_STATE, "no pods uploaded") : SIMON_ERR_INVALID;
     CU(cudaSetDevice(ctx->device));
-    int rc = reset_state(ctx, ctx->st);
+    int rc = clear_pool(ctx, ctx->single);
     if (rc) return rc;
     CU(cudaStreamSynchronize(ctx->stream));
     return SIMON_OK;
@@ -917,9 +890,9 @@ int simon_results_download(simon_ctx *ctx, uint32_t first, uint32_t count, int32
     if (!ctx || !ctx->have_pods) return SIMON_ERR_STATE;
     if ((uint64_t)first + count > ctx->n_pods) return fail(ctx, SIMON_ERR_INVALID, "range out of bounds");
     CU(cudaSetDevice(ctx->device));
-    if (out_node) CU(cudaMemcpyAsync(out_node, ctx->st.out_node.p + first, 4ull * count, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_score && ctx->st.out_score.p)
-        CU(cudaMemcpyAsync(out_score, ctx->st.out_score.p + first, 8ull * count, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_node) CU(cudaMemcpyAsync(out_node, ctx->single.out_node.p + first, 4ull * count, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_score && ctx->single.out_score.p)
+        CU(cudaMemcpyAsync(out_score, ctx->single.out_score.p + first, 8ull * count, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
     return SIMON_OK;
 }
@@ -932,18 +905,16 @@ int simon_schedule(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_
     CU(cudaSetDevice(ctx->device));
     if (count == 0) { if (out_n_fail) *out_n_fail = 0; return SIMON_OK; }
     cudaStream_t st = ctx->stream;
+    const ScenPool &S = ctx->single;
     uint32_t CS, TPB, NPT;
     size_t smem;
     int rc = choose_geometry(ctx, ctx->N, CS, TPB, NPT, smem);
     if (rc) return rc;
-    SkScenario sc;
-    fill_scen(ctx, ctx->st, sc, ctx->N, true);
-    CU(cudaMemcpyAsync(ctx->d_scen.p, &sc, sizeof(sc), cudaMemcpyHostToDevice, st));
-    CU(cudaMemsetAsync(ctx->st.fail_counts.p, 0, 4ull * ctx->max_fail * SIMON_N_FAIL_CODES, st));
-    CU(cudaMemsetAsync(ctx->st.counters.p, 0, 8, st));
     SkParams P;
-    fill_params(ctx, P);
-    P.first = first; P.count = count; P.max_fail = ctx->max_fail; P.npt = NPT; P.scen = ctx->d_scen.p;
+    fill_params(ctx, S, P);
+    P.first = first; P.count = count; P.max_fail = ctx->max_fail; P.npt = NPT;
+    CU(cudaMemsetAsync(S.fail_counts.p, 0, 4ull * ctx->max_fail * SIMON_N_FAIL_CODES, st));
+    CU(cudaMemsetAsync(S.counters.p, 0, 8, st));
     if (ctx->dump_pod >= first && ctx->dump_pod < first + count) {
         P.dump_pod = ctx->dump_pod; P.dump_total = ctx->d_dump_total.p; P.dump_code = ctx->d_dump_code.p;
         CU(cudaMemsetAsync(ctx->d_dump_total.p, 0xff, 8ull * std::max(1u, ctx->N), st));     // -1: node not scored (infeasible)
@@ -955,13 +926,13 @@ int simon_schedule(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     uint32_t counters[2] = {0, 0};
-    CU(cudaMemcpy(counters, ctx->st.counters.p, 8, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(counters, S.counters.p, 8, cudaMemcpyDeviceToHost));
     if (out_n_fail) *out_n_fail = counters[0];
-    if (out_node) CU(cudaMemcpy(out_node, ctx->st.out_node.p + first, 4ull * count, cudaMemcpyDeviceToHost));
-    if (out_score && ctx->st.out_score.p) CU(cudaMemcpy(out_score, ctx->st.out_score.p + first, 8ull * count, cudaMemcpyDeviceToHost));
+    if (out_node) CU(cudaMemcpy(out_node, S.out_node.p + first, 4ull * count, cudaMemcpyDeviceToHost));
+    if (out_score && S.out_score.p) CU(cudaMemcpy(out_score, S.out_score.p + first, 8ull * count, cudaMemcpyDeviceToHost));
     uint32_t nf = std::min(std::min(counters[0], max_fail), ctx->max_fail);
-    if (nf && out_fail_counts) CU(cudaMemcpy(out_fail_counts, ctx->st.fail_counts.p, 4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
-    if (nf && out_fail_pod) CU(cudaMemcpy(out_fail_pod, ctx->st.fail_pod.p, 4ull * nf, cudaMemcpyDeviceToHost));
+    if (nf && out_fail_counts) CU(cudaMemcpy(out_fail_counts, S.fail_counts.p, 4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
+    if (nf && out_fail_pod) CU(cudaMemcpy(out_fail_pod, S.fail_pod.p, 4ull * nf, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
@@ -970,22 +941,20 @@ int simon_replay(simon_ctx *ctx, uint32_t steps, float *out_ms_total) {
     if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_replay before uploads");
     CU(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
+    ScenPool &S = ctx->single;
     uint32_t CS, TPB, NPT;
     size_t smem;
     int rc = choose_geometry(ctx, ctx->N, CS, TPB, NPT, smem);
     if (rc) return rc;
-    SkScenario sc;
-    fill_scen(ctx, ctx->st, sc, ctx->N, true);
-    CU(cudaMemcpyAsync(ctx->d_scen.p, &sc, sizeof(sc), cudaMemcpyHostToDevice, st));
     SkParams P;
-    fill_params(ctx, P);
-    P.first = 0; P.count = ctx->n_pods; P.max_fail = ctx->max_fail; P.npt = NPT; P.scen = ctx->d_scen.p;
+    fill_params(ctx, S, P);
+    P.first = 0; P.count = ctx->n_pods; P.max_fail = ctx->max_fail; P.npt = NPT;
     CU(cudaEventRecord(ctx->ev0, st));
     for (uint32_t s = 0; s < steps; s++) {
-        rc = reset_state(ctx, ctx->st);
+        rc = clear_pool(ctx, S);
         if (rc) return rc;
-        CU(cudaMemsetAsync(ctx->st.fail_counts.p, 0, 4ull * ctx->max_fail * SIMON_N_FAIL_CODES, st));
-        CU(cudaMemsetAsync(ctx->st.counters.p, 0, 8, st));
+        CU(cudaMemsetAsync(S.fail_counts.p, 0, 4ull * ctx->max_fail * SIMON_N_FAIL_CODES, st));
+        CU(cudaMemsetAsync(S.counters.p, 0, 8, st));
         rc = launch_range(ctx, P, CS, TPB, smem, 0, ctx->n_pods, false);
         if (rc) return rc;
     }
@@ -1012,12 +981,13 @@ int simon_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *req_mem, in
     if (!ctx || !ctx->have_pods) return SIMON_ERR_STATE;
     CU(cudaSetDevice(ctx->device));
     const uint32_t N = ctx->N;
-    if (req_mcpu) CU(cudaMemcpy(req_mcpu, ctx->st.req_mcpu.p, 8ull * N, cudaMemcpyDeviceToHost));
-    if (req_mem) CU(cudaMemcpy(req_mem, ctx->st.req_mem.p, 8ull * N, cudaMemcpyDeviceToHost));
-    if (req_eph) CU(cudaMemcpy(req_eph, ctx->st.req_eph.p, 8ull * N, cudaMemcpyDeviceToHost));
-    if (nz_mcpu) CU(cudaMemcpy(nz_mcpu, ctx->st.nz_mcpu.p, 8ull * N, cudaMemcpyDeviceToHost));
-    if (nz_mem) CU(cudaMemcpy(nz_mem, ctx->st.nz_mem.p, 8ull * N, cudaMemcpyDeviceToHost));
-    if (num_pods) CU(cudaMemcpy(num_pods, ctx->st.num_pods.p, 4ull * N, cudaMemcpyDeviceToHost));
+    const ScenPool &S = ctx->single;
+    if (req_mcpu) CU(cudaMemcpy(req_mcpu, S.req_mcpu.p, 8ull * N, cudaMemcpyDeviceToHost));
+    if (req_mem) CU(cudaMemcpy(req_mem, S.req_mem.p, 8ull * N, cudaMemcpyDeviceToHost));
+    if (req_eph) CU(cudaMemcpy(req_eph, S.req_eph.p, 8ull * N, cudaMemcpyDeviceToHost));
+    if (nz_mcpu) CU(cudaMemcpy(nz_mcpu, S.nz_mcpu.p, 8ull * N, cudaMemcpyDeviceToHost));
+    if (nz_mem) CU(cudaMemcpy(nz_mem, S.nz_mem.p, 8ull * N, cudaMemcpyDeviceToHost));
+    if (num_pods) CU(cudaMemcpy(num_pods, S.num_pods.p, 4ull * N, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
@@ -1027,112 +997,55 @@ static int scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n,
     CU(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     if (n == 0) return SIMON_OK;
-    const uint32_t N = ctx->N, N1 = std::max(1u, N), K1 = ctx->K ? ctx->K : 1, P = ctx->n_pods, P1 = std::max(1u, P);
-    const size_t cntw = std::max<uint64_t>(1, ctx->cnt_words), nct = std::max(1u, ctx->n_counters), ncl = std::max(1u, ctx->n_classes);
-    if (!ctx->batch) { ctx->batch = new (std::nothrow) ScenBatch(); if (!ctx->batch) return SIMON_ERR_NOMEM; }
-    ScenBatch &B = *ctx->batch;
+    const uint32_t N = ctx->N, N1 = std::max(1u, N);
+    ScenPool &B = ctx->batch;
     const bool local = out_local != nullptr;
     if (local) B.n_storage = 0;         // the slices are overwritten below
     // ---- node lists: validated on the host, uploaded in ONE copy each (scenario order and its inverse) ----
     uint32_t max_active = 0;
     B.h_order.assign((size_t)n * N1, 0u);
     B.h_rank.assign((size_t)n * N1, -1);
-    std::vector<uint8_t> ident(n, 0);
     for (uint32_t i = 0; i < n; i++) {
         if (scen[i].n_nodes > N) return fail(ctx, SIMON_ERR_INVALID, "scenario %u: too many nodes", i);
-        uint32_t *ord = B.h_order.data() + (size_t)i * N1;
         int32_t *rank = B.h_rank.data() + (size_t)i * N1;
-        bool id = scen[i].n_nodes == N;
         for (uint32_t r = 0; r < scen[i].n_nodes; r++) {
-            uint32_t g = scen[i].nodes[r];
+            const uint32_t g = scen[i].nodes[r];
             if (g >= N || rank[g] != -1) return fail(ctx, SIMON_ERR_INVALID, "scenario %u: bad node list", i);
             rank[g] = (int32_t)r;
-            ord[r] = g;
-            if (g != r) id = false;
         }
-        ident[i] = id ? 1 : 0;
+        std::copy(scen[i].nodes, scen[i].nodes + scen[i].n_nodes, B.h_order.begin() + (size_t)i * N1);
         max_active = std::max(max_active, scen[i].n_nodes);
     }
-    // ---- pooled state of all scenarios: one allocation and one memset per column ----
-    CU(B.req_mcpu.alloc((size_t)n * N1)); CU(B.req_mem.alloc((size_t)n * N1)); CU(B.req_eph.alloc((size_t)n * N1));
-    CU(B.nz_mcpu.alloc((size_t)n * N1)); CU(B.nz_mem.alloc((size_t)n * N1)); CU(B.req_scalar.alloc((size_t)n * K1 * N1));
-    CU(B.gpu_used.alloc((size_t)n * SIMON_MAX_GPU_DEV * N1)); CU(B.num_pods.alloc((size_t)n * N1));
-    CU(B.cnt.alloc((size_t)n * cntw)); CU(B.cnt_total.alloc((size_t)n * nct));
-    const size_t tabw = (size_t)SK_MAX_SOFT * ctx->max_dom;
-    CU(B.tp.alloc((size_t)n * tabw)); CU(B.fcount.alloc((size_t)n * tabw)); CU(B.size.alloc((size_t)n * SK_MAX_SOFT));
-    CU(B.hard_reg.alloc((size_t)n * SK_MAX_HARD * ctx->max_dom));
-    CU(B.csum.alloc((size_t)n * ncl * SK_CSUM_W)); CU(B.fbits.alloc((size_t)n * ncl * N1)); CU(B.ocache.alloc((size_t)n * ncl * N1));
-    CU(B.out_node.alloc((size_t)n * P1)); CU(B.counters.alloc((size_t)n * 2)); CU(B.clk.alloc((size_t)n * 2));
-    CU(B.order.alloc((size_t)n * N1)); CU(B.rank_of.alloc((size_t)n * N1)); CU(B.results.alloc(n));
+    // ---- pooled state of all scenarios: one allocation and one memset (or broadcast) per column; Open-Local: every scenario
+    // starts from the uploaded VG requested values and device masks ----
+    int rc = alloc_pool(ctx, B, n, false);
+    if (rc) return rc;
     CU(cudaMemcpyAsync(B.order.p, B.h_order.data(), 4ull * n * N1, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(B.rank_of.p, B.h_rank.data(), 4ull * n * N1, cudaMemcpyHostToDevice, st));
-    CU(cudaMemsetAsync(B.req_mcpu.p, 0, 8ull * n * N1, st)); CU(cudaMemsetAsync(B.req_mem.p, 0, 8ull * n * N1, st));
-    CU(cudaMemsetAsync(B.req_eph.p, 0, 8ull * n * N1, st)); CU(cudaMemsetAsync(B.nz_mcpu.p, 0, 8ull * n * N1, st));
-    CU(cudaMemsetAsync(B.nz_mem.p, 0, 8ull * n * N1, st)); CU(cudaMemsetAsync(B.req_scalar.p, 0, 8ull * n * K1 * N1, st));
-    CU(cudaMemsetAsync(B.gpu_used.p, 0, 8ull * n * SIMON_MAX_GPU_DEV * N1, st)); CU(cudaMemsetAsync(B.num_pods.p, 0, 4ull * n * N1, st));
-    CU(cudaMemsetAsync(B.cnt.p, 0, 4ull * n * cntw, st)); CU(cudaMemsetAsync(B.cnt_total.p, 0, 4ull * n * nct, st));
-    // each scenario starts from an empty state: no stored class summary / own-score cache may survive from an earlier
-    // call (another node list!); fbits are only read under a valid summary record
-    CU(cudaMemsetAsync(B.csum.p, 0, 8ull * n * ncl * SK_CSUM_W, st)); CU(cudaMemsetAsync(B.ocache.p, 0, 8ull * n * ncl * N1, st));
     CU(cudaMemsetAsync(B.counters.p, 0, 8ull * n, st)); CU(cudaMemsetAsync(B.clk.p, 0, 16ull * n, st));
-    // Open-Local: every scenario starts from the uploaded VG requested values and device masks, one broadcast per column; the
-    // single-scenario state (d_vg_req, d_dev_alloc) is not touched
-    const size_t VN = std::max<size_t>(1, (size_t)ctx->V * N);
-    if (local) {
-        int sms = 132;
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
-        const uint32_t cap = (uint32_t)sms * 8;
-        CU(B.vg_req.alloc((size_t)n * VN)); CU(B.local_raw.alloc((size_t)n * N1)); CU(B.local_results.alloc(n));
-        simon_bcast<<<(uint32_t)std::min<size_t>(((size_t)n * VN + 255) / 256, cap), 256, 0, st>>>(ctx->d_vg_req0.p, VN, n, B.vg_req.p);
-        CU(cudaGetLastError());
-        if (ctx->have_devices) {
-            CU(B.dev_alloc.alloc((size_t)n * N1));
-            simon_bcast<<<(uint32_t)std::min<size_t>(((size_t)n * N1 + 255) / 256, cap), 256, 0, st>>>(ctx->d_dev_alloc0.p, N1, n, B.dev_alloc.p);
-            CU(cudaGetLastError());
-        }
-    }
     std::vector<SkScenario> h(n);
-    for (uint32_t i = 0; i < n; i++) {
-        SkScenario &o = h[i];
-        memset(&o, 0, sizeof(o));
-        o.order = ident[i] ? nullptr : B.order.p + (size_t)i * N1;
-        o.rank_of = ident[i] ? nullptr : B.rank_of.p + (size_t)i * N1;
-        o.n_active = scen[i].n_nodes;
-        o.req_mcpu = B.req_mcpu.p + (size_t)i * N1; o.req_mem = B.req_mem.p + (size_t)i * N1; o.req_eph = B.req_eph.p + (size_t)i * N1;
-        o.nz_mcpu = B.nz_mcpu.p + (size_t)i * N1; o.nz_mem = B.nz_mem.p + (size_t)i * N1;
-        o.req_scalar = B.req_scalar.p + (size_t)i * K1 * N1; o.gpu_used = B.gpu_used.p + (size_t)i * SIMON_MAX_GPU_DEV * N1;
-        o.num_pods = B.num_pods.p + (size_t)i * N1; o.cnt = B.cnt.p + (size_t)i * cntw; o.cnt_total = B.cnt_total.p + (size_t)i * nct;
-        o.tp = B.tp.p + (size_t)i * tabw; o.fcount = B.fcount.p + (size_t)i * tabw; o.size = B.size.p + (size_t)i * SK_MAX_SOFT;
-        o.hard_reg = B.hard_reg.p + (size_t)i * SK_MAX_HARD * ctx->max_dom;
-        o.csum = B.csum.p + (size_t)i * ncl * SK_CSUM_W; o.fbits = B.fbits.p + (size_t)i * ncl * N1; o.ocache = B.ocache.p + (size_t)i * ncl * N1;
-        o.out_node = B.out_node.p + (size_t)i * P1; o.out_score = nullptr; o.out_gpu = nullptr;
-        o.fail_counts = nullptr; o.fail_pod = nullptr; o.n_fail = B.counters.p + 2ull * i; o.n_sched = B.counters.p + 2ull * i + 1;
-        o.clk = B.clk.p + 2ull * i;
-    }
-    CU(ctx->d_scen.upload(h.data(), n, st));
+    for (uint32_t i = 0; i < n; i++)     // all N nodes in index order (distinct, so sorted) need no node list
+        h[i] = fill_scen(B, i, scen[i].n_nodes, scen[i].n_nodes == N && std::is_sorted(scen[i].nodes, scen[i].nodes + N));
+    CU(B.scen.upload(h.data(), n, st));
     uint32_t CS, TPB, NPT;
     size_t smem;
-    int rc = choose_geometry(ctx, max_active, CS, TPB, NPT, smem, n);
+    rc = choose_geometry(ctx, max_active, CS, TPB, NPT, smem, n);
     if (rc) return rc;
     SkParams Pm;
-    fill_params(ctx, Pm);
-    Pm.first = 0; Pm.count = ctx->n_pods; Pm.max_fail = 0; Pm.npt = NPT; Pm.scen = ctx->d_scen.p;
-    if (local) {
-        Pm.vg_req = B.vg_req.p; Pm.local_raw = B.local_raw.p; Pm.vg_req_stride = VN; Pm.node_stride = N1;
-        if (ctx->have_devices) Pm.dev_alloc = B.dev_alloc.p;
-    }
+    fill_params(ctx, B, Pm);
+    Pm.first = 0; Pm.count = ctx->n_pods; Pm.max_fail = 0; Pm.npt = NPT;
     rc = launch(ctx, Pm, n, CS, TPB, smem);
     if (rc) return rc;
     // per-scenario sums over the active nodes on the device; ONE copy of the result structs comes back
-    simon_scen_reduce<<<n, 256, 0, st>>>(ctx->d_scen.p, ctx->d_alloc_mcpu.p, ctx->d_alloc_mem.p, B.results.p);
+    simon_scen_reduce<<<n, 256, 0, st>>>(B.scen.p, ctx->d_alloc_mcpu.p, ctx->d_alloc_mem.p, B.results.p);
     CU(cudaGetLastError());
     if (local) {
-        simon_scen_reduce_local<<<n, 256, 0, st>>>(ctx->d_scen.p, ctx->d_node_n_vg.p, ctx->d_vg_cap.p, B.vg_req.p, VN, N, B.local_results.p);
+        simon_scen_reduce_local<<<n, 256, 0, st>>>(B.scen.p, ctx->d_node_n_vg.p, ctx->d_vg_cap.p, B.vg_req.p, B.vn, N, B.local_results.p);
         CU(cudaGetLastError());
         CU(cudaMemcpyAsync(out_local, B.local_results.p, sizeof(simon_scenario_local_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
     }
     CU(cudaMemcpyAsync(out, B.results.p, sizeof(simon_scenario_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
-    if (out_node) CU(cudaMemcpyAsync(out_node, B.out_node.p, 4ull * n * P, cudaMemcpyDeviceToHost, st));
+    if (out_node) CU(cudaMemcpyAsync(out_node, B.out_node.p, 4ull * n * ctx->n_pods, cudaMemcpyDeviceToHost, st));
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
@@ -1157,15 +1070,14 @@ int simon_scenarios_run_local(simon_ctx *ctx, const simon_scenario *scen, uint32
 
 int simon_scenarios_storage_download(simon_ctx *ctx, uint32_t scenario, int64_t *vg_requested, uint32_t *dev_alloc) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->batch || !ctx->batch->n_storage) return fail(ctx, SIMON_ERR_STATE, "no simon_scenarios_run_local batch since the last upload");
-    const ScenBatch &B = *ctx->batch;
+    const ScenPool &B = ctx->batch;
+    if (!B.n_storage) return fail(ctx, SIMON_ERR_STATE, "no simon_scenarios_run_local batch since the last upload");
     if (scenario >= B.n_storage) return fail(ctx, SIMON_ERR_INVALID, "scenario %u of a batch of %u", scenario, B.n_storage);
     if (dev_alloc && !ctx->have_devices) return fail(ctx, SIMON_ERR_STATE, "no devices uploaded");
     CU(cudaSetDevice(ctx->device));
-    const uint32_t N = ctx->N, N1 = std::max(1u, N);
-    const size_t VN = std::max<size_t>(1, (size_t)ctx->V * N);
-    if (vg_requested && ctx->V && N) CU(cudaMemcpy(vg_requested, B.vg_req.p + (size_t)scenario * VN, 8ull * ctx->V * N, cudaMemcpyDeviceToHost));
-    if (dev_alloc && N) CU(cudaMemcpy(dev_alloc, B.dev_alloc.p + (size_t)scenario * N1, 4ull * N, cudaMemcpyDeviceToHost));
+    const uint32_t N = ctx->N;
+    if (vg_requested && ctx->V && N) CU(cudaMemcpy(vg_requested, B.vg_req.p + scenario * B.vn, 8ull * ctx->V * N, cudaMemcpyDeviceToHost));
+    if (dev_alloc && N) CU(cudaMemcpy(dev_alloc, B.dev_alloc.p + scenario * B.nodes, 4ull * N, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
@@ -1187,7 +1099,7 @@ int simon_gpu_slots_download(simon_ctx *ctx, uint32_t first, uint32_t count, uin
     if (!ctx || !ctx->have_pods || !out_slots) return SIMON_ERR_STATE;
     if ((uint64_t)first + count > ctx->n_pods) return fail(ctx, SIMON_ERR_INVALID, "range out of bounds");
     CU(cudaSetDevice(ctx->device));
-    CU(cudaMemcpy(out_slots, ctx->st.out_gpu.p + first, 4ull * count, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(out_slots, ctx->single.out_gpu.p + first, 4ull * count, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
@@ -1195,8 +1107,8 @@ int simon_state_download_ext(simon_ctx *ctx, int64_t *req_scalar, int64_t *gpu_u
     if (!ctx || !ctx->have_pods) return SIMON_ERR_STATE;
     CU(cudaSetDevice(ctx->device));
     const uint32_t N = ctx->N;
-    if (req_scalar && ctx->K) CU(cudaMemcpy(req_scalar, ctx->st.req_scalar.p, 8ull * ctx->K * N, cudaMemcpyDeviceToHost));
-    if (gpu_used) CU(cudaMemcpy(gpu_used, ctx->st.gpu_used.p, 8ull * SIMON_MAX_GPU_DEV * N, cudaMemcpyDeviceToHost));
+    if (req_scalar && ctx->K) CU(cudaMemcpy(req_scalar, ctx->single.req_scalar.p, 8ull * ctx->K * N, cudaMemcpyDeviceToHost));
+    if (gpu_used) CU(cudaMemcpy(gpu_used, ctx->single.gpu_used.p, 8ull * SIMON_MAX_GPU_DEV * N, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
@@ -1204,7 +1116,7 @@ int simon_storage_upload(simon_ctx *ctx, const simon_storage *sg) {
     if (!ctx || !sg) return SIMON_ERR_INVALID;
     if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_storage_upload before simon_pods_upload");
     ctx->have_devices = false;          // device tables belong to the storage upload they followed
-    if (ctx->batch) ctx->batch->n_storage = 0;      // and so does the state of the last storage batch
+    ctx->batch.n_storage = 0;           // and so does the state of the last storage batch
     const uint32_t N = ctx->N, V = sg->n_vgs, C = ctx->n_classes;
     if (sg->n_classes != C) return fail(ctx, SIMON_ERR_INVALID, "storage table has %u classes, the pod set %u", sg->n_classes, C);
     if (V > SIMON_MAX_VGS) return fail(ctx, SIMON_ERR_LIMIT, "more than %d VGs per node", SIMON_MAX_VGS);
@@ -1238,7 +1150,6 @@ int simon_storage_upload(simon_ctx *ctx, const simon_storage *sg) {
     CU(ctx->d_vg_cap.upload(V && N ? sg->vg_capacity : zero64.data(), VN, st));
     CU(ctx->d_vg_req0.upload(V && N ? sg->vg_requested : zero64.data(), VN, st));
     CU(ctx->d_vg_name.upload(V && N ? sg->vg_name : zero32.data(), VN, st));
-    CU(ctx->d_vg_req.alloc(VN)); CU(ctx->d_local_raw.alloc(std::max(1u, N)));
     CU(ctx->d_class_local.upload(sg->class_local, std::max(1u, C), st));
     CU(ctx->d_vol_off.upload(sg->vol_off, C + 1, st));
     std::vector<int64_t> vs(sg->vol_size, sg->vol_size + n_vol); vs.push_back(0);
@@ -1269,7 +1180,7 @@ int simon_storage_upload(simon_ctx *ctx, const simon_storage *sg) {
     ctx->V = V;
     ctx->h_class_local.assign(sg->class_local, sg->class_local + C);
     ctx->have_storage = true;
-    int rc = reset_state(ctx, ctx->st);
+    int rc = alloc_pool(ctx, ctx->single, 1, true);
     if (rc) return rc;
     CU(cudaStreamSynchronize(st));
     return SIMON_OK;
@@ -1279,14 +1190,14 @@ int simon_storage_state_download(simon_ctx *ctx, int64_t *vg_requested) {
     if (!ctx || !vg_requested) return SIMON_ERR_INVALID;
     if (!ctx->have_storage) return fail(ctx, SIMON_ERR_STATE, "no storage uploaded");
     CU(cudaSetDevice(ctx->device));
-    if (ctx->V && ctx->N) CU(cudaMemcpy(vg_requested, ctx->d_vg_req.p, 8ull * ctx->V * ctx->N, cudaMemcpyDeviceToHost));
+    if (ctx->V && ctx->N) CU(cudaMemcpy(vg_requested, ctx->single.vg_req.p, 8ull * ctx->V * ctx->N, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
 int simon_devices_upload(simon_ctx *ctx, const simon_devices *dv) {
     if (!ctx || !dv) return SIMON_ERR_INVALID;
     if (!ctx->have_storage) return fail(ctx, SIMON_ERR_STATE, "simon_devices_upload before simon_storage_upload");
-    if (ctx->batch) ctx->batch->n_storage = 0;      // the last storage batch ran on the device tables this upload replaces
+    ctx->batch.n_storage = 0;           // the last storage batch ran on the device tables this upload replaces
     const uint32_t N = ctx->N, D = dv->n_slots, C = ctx->n_classes;
     if (dv->n_classes != C) return fail(ctx, SIMON_ERR_INVALID, "device table has %u classes, the pod set %u", dv->n_classes, C);
     if (D > SIMON_MAX_DEVS) return fail(ctx, SIMON_ERR_LIMIT, "more than %d devices per node", SIMON_MAX_DEVS);
@@ -1327,14 +1238,13 @@ int simon_devices_upload(simon_ctx *ctx, const simon_devices *dv) {
     CU(ctx->d_node_n_hdd.upload(dv->node_n_hdd, std::max(1u, N), st));
     CU(ctx->d_dev_cap.upload(D && N ? dv->dev_capacity : zero64.data(), DN, st));
     CU(ctx->d_dev_alloc0.upload(dv->dev_alloc, std::max(1u, N), st));
-    CU(ctx->d_dev_alloc.alloc(std::max(1u, N)));
     CU(ctx->d_ssd_off.upload(dv->ssd_off, C + 1, st));
     CU(ctx->d_hdd_off.upload(dv->hdd_off, C + 1, st));
     std::vector<int64_t> ss(dv->ssd_size, dv->ssd_size + (C ? dv->ssd_off[C] : 0)); ss.push_back(0);
     std::vector<int64_t> hs(dv->hdd_size, dv->hdd_size + (C ? dv->hdd_off[C] : 0)); hs.push_back(0);
     CU(ctx->d_ssd_size.upload(ss.data(), ss.size(), st)); CU(ctx->d_hdd_size.upload(hs.data(), hs.size(), st));
     ctx->have_devices = true;
-    int rc = reset_state(ctx, ctx->st);
+    int rc = alloc_pool(ctx, ctx->single, 1, true);
     if (rc) return rc;
     CU(cudaStreamSynchronize(st));      // `ss` / `hs` leave scope
     return SIMON_OK;
@@ -1344,7 +1254,7 @@ int simon_devices_state_download(simon_ctx *ctx, uint32_t *alloc_mask) {
     if (!ctx || !alloc_mask) return SIMON_ERR_INVALID;
     if (!ctx->have_devices) return fail(ctx, SIMON_ERR_STATE, "no devices uploaded");
     CU(cudaSetDevice(ctx->device));
-    if (ctx->N) CU(cudaMemcpy(alloc_mask, ctx->d_dev_alloc.p, 4ull * ctx->N, cudaMemcpyDeviceToHost));
+    if (ctx->N) CU(cudaMemcpy(alloc_mask, ctx->single.dev_alloc.p, 4ull * ctx->N, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
@@ -1374,52 +1284,44 @@ static int moves_launch(simon_ctx *ctx, bool record) {
     cudaStream_t st = ctx->stream;
     const uint32_t N = ctx->N, n = ctx->mv_n, scope = ctx->mv_scope;
     const bool scoped = ctx->mv_scoped;
+    const ScenPool &S = ctx->single;
     if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && n) CU(ctx->d_mv_slots.alloc(n));
     if (record) CU(cudaEventRecord(ctx->ev0, st));
     if (scoped && (scope & SIMON_MOVES_SCOPE_GPU_SHARE) && N) {
         CU(ctx->d_mv_gpu.alloc(N));
         simon_moves_pack_gpu<<<(N + 255) / 256, 256, 0, st>>>(N, ctx->d_gpu_count.p, ctx->d_gpu_dev_mem.p, ctx->d_gpu_total_mem.p,
-                                                               ctx->st.gpu_used.p, ctx->d_mv_gpu.p);
+                                                               S.gpu_used.p, ctx->d_mv_gpu.p);
         ctx->launches++;
     }
     if (scoped && ctx->mv_n_prep) {
         simon_moves_hard_prep<<<ctx->mv_n_prep, 256, 0, st>>>(N, ctx->use_scache, ctx->d_scache.p, ctx->d_label_bits.p, ctx->d_topo_dom.p,
-                                                              ctx->d_topo_ndom.p, ctx->d_class_off.p, ctx->d_class_blob.p, ctx->st.cnt.p,
+                                                              ctx->d_topo_ndom.p, ctx->d_class_off.p, ctx->d_class_blob.p, S.cnt.p,
                                                               ctx->d_mv_prep.p, ctx->d_mv_hreg.p, ctx->d_mv_hs.p);
         ctx->launches++;
     }
     if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && !scoped && n) CU(cudaMemsetAsync(ctx->d_mv_slots.p, 0, 4ull * n, st));
     simon_moves_pack<<<std::max(std::max(1u, (N + 255) / 256), std::min(1184u, (ctx->n_pods + 255) / 256)), 256, 0, st>>>(N, ctx->T, ctx->d_alloc_mcpu.p, ctx->d_alloc_mem.p, ctx->d_alloc_eph.p, ctx->d_alloc_pods.p,
-                                                                     ctx->d_topo_dom.p, ctx->st.req_mcpu.p, ctx->st.req_mem.p, ctx->st.req_eph.p,
-                                                                     ctx->st.nz_mcpu.p, ctx->st.nz_mem.p, ctx->st.num_pods.p, ctx->d_mv_nodes.p,
+                                                                     ctx->d_topo_dom.p, S.req_mcpu.p, S.req_mem.p, S.req_eph.p,
+                                                                     S.nz_mcpu.p, S.nz_mem.p, S.num_pods.p, ctx->d_mv_nodes.p,
                                                                      ctx->d_mv_best_pod.p, ctx->n_pods, ctx->d_mv_best.p, ctx->d_mv_hist.p,
-                                                                     ctx->d_pod_class.p, ctx->st.out_node.p, ctx->d_mv_classes.p, ctx->d_mv_pods.p);
+                                                                     ctx->d_pod_class.p, S.out_node.p, ctx->d_mv_classes.p, ctx->d_mv_pods.p);
     SmvParams P;
     memset(&P, 0, sizeof(P));
     P.N = N; P.K = ctx->K; P.WT = ctx->WT; P.T = ctx->T; P.n_pods = ctx->n_pods; P.n_moves = n; P.use_scache = ctx->use_scache;
-    P.nodes = ctx->d_mv_nodes.p; P.alloc_scalar = ctx->d_alloc_scalar.p; P.req_scalar = ctx->st.req_scalar.p; P.node_flags = ctx->d_node_flags.p;
+    P.nodes = ctx->d_mv_nodes.p; P.alloc_scalar = ctx->d_alloc_scalar.p; P.req_scalar = S.req_scalar.p; P.node_flags = ctx->d_node_flags.p;
     P.label_bits = ctx->d_label_bits.p; P.taint_hard = ctx->d_taint_hard.p; P.topo_dom = ctx->d_topo_dom.p;
     P.pods = ctx->d_mv_pods.p;
-    P.class_off = ctx->d_class_off.p; P.class_blob = ctx->d_class_blob.p; P.classes = ctx->d_mv_classes.p; P.pod_class = ctx->d_pod_class.p; P.placement = ctx->st.out_node.p;
-    P.cnt = ctx->st.cnt.p; P.cnt_total = ctx->st.cnt_total.p; P.scache = ctx->d_scache.p; P.moves = ctx->d_moves.p;
+    P.class_off = ctx->d_class_off.p; P.class_blob = ctx->d_class_blob.p; P.classes = ctx->d_mv_classes.p; P.pod_class = ctx->d_pod_class.p; P.placement = S.out_node.p;
+    P.cnt = S.cnt.p; P.cnt_total = S.cnt_total.p; P.scache = ctx->d_scache.p; P.moves = ctx->d_moves.p;
     P.out_gain = ctx->d_mv_gain.p; P.out_code = ctx->d_mv_code.p; P.best_per_pod = ctx->d_mv_best_pod.p; P.best_global = ctx->d_mv_best.p;
     P.hist = ctx->d_mv_hist.p; P.move_base = ctx->mv_base;
     P.scope = scope; P.gpu = ctx->d_mv_gpu.p; P.hs = ctx->d_mv_hs.p; P.hreg = ctx->d_mv_hreg.p;
     P.out_slots = (scope & SIMON_MOVES_SCOPE_GPU_SHARE) ? ctx->d_mv_slots.p : nullptr;
     if (n) {
-        int sms = 132;
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
-        // occupancy variant: 4 resident CTAs per SM (64 registers, a few spills) by default; SIMON_MOVES_OCC=2 selects the
-        // 2-CTA variant without spills (diagnostic switch)
-        static const int occ = getenv("SIMON_MOVES_OCC") ? atoi(getenv("SIMON_MOVES_OCC")) : 4;
-        const uint32_t grid = std::min<uint32_t>((n + 255) / 256, (uint32_t)sms * (occ == 2 ? 2u : 4u) * 2u);
-        if (scoped) {
-            if (occ == 2) simon_moves_kernel<2, true><<<grid, 256, 0, st>>>(P);
-            else simon_moves_kernel<4, true><<<grid, 256, 0, st>>>(P);
-        } else {
-            if (occ == 2) simon_moves_kernel<2, false><<<grid, 256, 0, st>>>(P);
-            else simon_moves_kernel<4, false><<<grid, 256, 0, st>>>(P);
-        }
+        // 4 resident CTAs per SM (64 registers, a few spills), two rounds of them
+        const uint32_t grid = std::min<uint32_t>((n + 255) / 256, (uint32_t)ctx->sms * 4u * 2u);
+        if (scoped) simon_moves_kernel<4, true><<<grid, 256, 0, st>>>(P);
+        else simon_moves_kernel<4, false><<<grid, 256, 0, st>>>(P);
         ctx->launches++;
     }
     if (record) CU(cudaEventRecord(ctx->ev1, st));
@@ -1440,10 +1342,8 @@ int simon_moves_upload(simon_ctx *ctx, const simon_move *moves, uint32_t n_moves
     if (!ctx->static_filled && ctx->use_scache && ctx->N && ctx->n_classes) {
         // once per uploaded pod list: the static verdicts of every (signature, node) pair, densely
         SkParams Pm;
-        fill_params(ctx, Pm);
-        int sms = 132;
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
-        simon_static_fill<<<sms * 8, 256, 0, ctx->stream>>>(Pm, ctx->d_sig_class.p, ctx->n_sigs);
+        fill_params(ctx, ctx->single, Pm);
+        simon_static_fill<<<ctx->sms * 8, 256, 0, ctx->stream>>>(Pm, ctx->d_sig_class.p, ctx->n_sigs);
         CU(cudaGetLastError());
         ctx->launches++;
         ctx->static_filled = true;

@@ -125,8 +125,8 @@ struct SkParams {
     const int64_t *dev_cap, *ssd_size, *hdd_size;
     const uint32_t *ssd_off, *hdd_off;
     uint32_t *dev_alloc;           // [N] bit s: slot s allocated
-    // vg_req, local_raw and dev_alloc hold one slice per cluster of the launch (scenario batches), these many elements apart;
-    // 0: the launch has one scenario, the single-scenario state
+    // vg_req, local_raw and dev_alloc hold one slice per cluster of the launch, these many elements apart (a single-scenario
+    // launch is one cluster: it reads slice 0)
     uint64_t vg_req_stride, node_stride;
 };
 
