@@ -237,6 +237,11 @@ struct simon_ctx {
     DevBuf<SmvGpu> d_mv_gpu;
     uint32_t n_pin_fast = 0;            // pods marked for the pinned-run fast path (-4 in the device copy of pod_fixed_node)
     std::vector<uint8_t> bypass;        // per pod: never reaches the scheduler in a single-scenario run (pre-bound or absent)
+    // resumed runs (simon_schedule_resume): per pod the uploaded pod_fixed_node and guard (what its prefix entry is checked against),
+    // the prefix on the device and its per-node grouping (counts, offsets, fill cursors, pod list)
+    std::vector<int32_t> h_fixed, h_guard;
+    DevBuf<int32_t> d_prefix;
+    DevBuf<uint32_t> d_rs_cnt, d_rs_off, d_rs_cur, d_rs_list;
     DevBuf<unsigned char> d_gnode;      // large-cluster variant: per-node arrays in global memory
     bool big = false;                   // set by choose_geometry for the next launch
     size_t gnode_stride = 0;
@@ -592,7 +597,7 @@ int launch_range(simon_ctx *ctx, SkParams &P, uint32_t CS, uint32_t TPB, size_t 
     if (record) CU(cudaEventRecord(ctx->ev0, ctx->stream));
     if (n_pre) {
         const uint32_t grid = std::min<uint32_t>((n_pre + 255) / 256, (uint32_t)ctx->sms * 4);
-        simon_import_kernel<<<grid, 256, 0, ctx->stream>>>(P, first, n_pre);
+        simon_import_kernel<<<grid, 256, 0, ctx->stream>>>(P, first, n_pre, nullptr);
         CU(cudaGetLastError());
         ctx->launches++;
     }
@@ -856,6 +861,8 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     }
     ctx->bypass.assign(std::max(1u, p->n_pods), 0);
     for (uint32_t i = 0; i < p->n_pods; i++) ctx->bypass[i] = (guard[i] == -2 || p->pod_fixed_node[i] != -1) ? 1 : 0;
+    ctx->h_fixed.assign(p->pod_fixed_node, p->pod_fixed_node + p->n_pods);
+    ctx->h_guard.assign(guard.begin(), guard.begin() + p->n_pods);
     CU(cudaStreamSynchronize(st));
     ctx->max_fail = std::max(1u, p->n_pods);      // every pod of the list may fail: one histogram row each (96 B)
     int rc = alloc_pool(ctx, ctx->single, 1, true);
@@ -930,6 +937,86 @@ int simon_schedule(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_
     if (out_n_fail) *out_n_fail = counters[0];
     if (out_node) CU(cudaMemcpy(out_node, S.out_node.p + first, 4ull * count, cudaMemcpyDeviceToHost));
     if (out_score && S.out_score.p) CU(cudaMemcpy(out_score, S.out_score.p + first, 8ull * count, cudaMemcpyDeviceToHost));
+    uint32_t nf = std::min(std::min(counters[0], max_fail), ctx->max_fail);
+    if (nf && out_fail_counts) CU(cudaMemcpy(out_fail_counts, S.fail_counts.p, 4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
+    if (nf && out_fail_pod) CU(cudaMemcpy(out_fail_pod, S.fail_pod.p, 4ull * nf, cudaMemcpyDeviceToHost));
+    return SIMON_OK;
+}
+
+int simon_schedule_resume(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n_prefix, int32_t *out_node, int64_t *out_score,
+                          uint32_t *out_fail_counts, uint32_t *out_fail_pod, uint32_t max_fail, uint32_t *out_n_fail) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_schedule_resume before uploads");
+    if (n_prefix > ctx->n_pods) return fail(ctx, SIMON_ERR_INVALID, "prefix of %u pods exceeds the %u uploaded", n_prefix, ctx->n_pods);
+    if (n_prefix && !prefix_node) return fail(ctx, SIMON_ERR_INVALID, "prefix_node is NULL");
+    const int32_t N = (int32_t)ctx->N;
+    for (uint32_t i = 0; i < n_prefix; i++) {
+        const int32_t e = prefix_node[i], f = ctx->h_fixed[i], gd = ctx->h_guard[i];
+        if (e < -3 || e >= N) return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u: node %d out of range", i, e);
+        if (ctx->bypass[i]) {
+            // what the import gives a pod that does not reach the scheduler: absent -3, bound to a node outside the cluster -2
+            const int32_t want = gd == -2 ? -3 : (f >= 0 ? f : -2);
+            if (e != want) return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u does not reach the scheduler and is reported as %d, not %d", i, want, e);
+        } else if (e < -1) {
+            return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u reaches the scheduler: %d is not a node or -1", i, e);
+        } else if (gd >= 0 && e != -1 && e != gd) {
+            return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u is pinned to node %d, not %d", i, gd, e);
+        }
+    }
+    CU(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    ScenPool &S = ctx->single;
+    uint32_t CS, TPB, NPT;
+    size_t smem;
+    int rc = choose_geometry(ctx, ctx->N, CS, TPB, NPT, smem);
+    if (rc) return rc;
+    SkParams P;
+    fill_params(ctx, S, P);
+    P.max_fail = ctx->max_fail; P.npt = NPT;
+    const uint32_t first = n_prefix, count = ctx->n_pods - n_prefix;
+    rc = clear_pool(ctx, S);
+    if (rc) return rc;
+    CU(cudaMemsetAsync(S.fail_counts.p, 0, 4ull * ctx->max_fail * SIMON_N_FAIL_CODES, st));
+    CU(cudaMemsetAsync(S.counters.p, 0, 8, st));
+    if (ctx->dump_pod >= first && ctx->dump_pod < first + count) {
+        P.dump_pod = ctx->dump_pod; P.dump_total = ctx->d_dump_total.p; P.dump_code = ctx->d_dump_code.p;
+        CU(cudaMemsetAsync(ctx->d_dump_total.p, 0xff, 8ull * std::max(1u, ctx->N), st));     // -1: node not scored (infeasible)
+        CU(cudaMemsetAsync(ctx->d_dump_code.p, 0, 4ull * std::max(1u, ctx->N), st));
+    }
+    CU(cudaEventRecord(ctx->ev0, st));
+    if (n_prefix) {
+        // the sums of the prefix (requests, pod counts, scalars, counters) and its per-pod results, by the import
+        CU(ctx->d_prefix.upload(prefix_node, n_prefix, st));
+        const uint32_t grid = std::min<uint32_t>((n_prefix + 255) / 256, (uint32_t)ctx->sms * 4);
+        simon_import_kernel<<<grid, 256, 0, st>>>(P, 0, n_prefix, ctx->d_prefix.p);
+        CU(cudaGetLastError());
+        ctx->launches++;
+        // GPU-share memory and Open-Local state: each node replays its own prefix pods in placement order
+        const uint32_t N1 = std::max(1u, ctx->N);
+        CU(ctx->d_rs_cnt.alloc(N1)); CU(ctx->d_rs_off.alloc(N1 + 1)); CU(ctx->d_rs_cur.alloc(N1)); CU(ctx->d_rs_list.alloc(n_prefix));
+        CU(cudaMemsetAsync(ctx->d_rs_cnt.p, 0, 4ull * N1, st));
+        SkParams R = P;
+        R.vg_req_stride = 0; R.node_stride = 0;      // plain CTAs, not one cluster per scenario: every CTA reads slice 0
+        simon_resume_count<<<grid, 256, 0, st>>>(R, ctx->d_prefix.p, n_prefix, ctx->d_rs_cnt.p);
+        simon_resume_scan<<<1, 1024, 0, st>>>(ctx->d_rs_cnt.p, ctx->N, ctx->d_rs_off.p, ctx->d_rs_cur.p);
+        simon_resume_fill<<<grid, 256, 0, st>>>(R, ctx->d_prefix.p, n_prefix, ctx->d_rs_cur.p, ctx->d_rs_list.p);
+        simon_resume_replay<<<(N1 + 127) / 128, 128, 0, st>>>(R, ctx->d_rs_off.p, ctx->d_rs_list.p);
+        CU(cudaGetLastError());
+        ctx->launches += 4;
+    }
+    if (count) {
+        rc = launch_range(ctx, P, CS, TPB, smem, first, count, false);
+        if (rc) return rc;
+    }
+    CU(cudaEventRecord(ctx->ev1, st));
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    uint32_t counters[2] = {0, 0};
+    CU(cudaMemcpy(counters, S.counters.p, 8, cudaMemcpyDeviceToHost));
+    if (out_n_fail) *out_n_fail = counters[0];
+    if (out_node && ctx->n_pods) CU(cudaMemcpy(out_node, S.out_node.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost));
+    if (out_score && S.out_score.p && ctx->n_pods) CU(cudaMemcpy(out_score, S.out_score.p, 8ull * ctx->n_pods, cudaMemcpyDeviceToHost));
     uint32_t nf = std::min(std::min(counters[0], max_fail), ctx->max_fail);
     if (nf && out_fail_counts) CU(cudaMemcpy(out_fail_counts, S.fail_counts.p, 4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
     if (nf && out_fail_pod) CU(cudaMemcpy(out_fail_pod, S.fail_pod.p, 4ull * nf, cudaMemcpyDeviceToHost));

@@ -25,7 +25,8 @@ EXPORTS = ["simon_gpu_version", "simon_ctx_create", "simon_ctx_destroy", "simon_
            "simon_host_last_error", "simon_host_compile", "simon_host_plan_free", "simon_host_plan_columns", "simon_host_plan_describe",
            "simon_host_simulate", "simon_host_free", "simon_host_quantity_probe", "simon_host_plan_fit_error", "simon_host_capacity_search",
            "simon_storage_upload", "simon_storage_state_download", "simon_devices_upload", "simon_devices_state_download",
-           "simon_scenarios_run_local", "simon_scenarios_storage_download", "simon_moves_set_scope", "simon_moves_gpu_slots_download"]
+           "simon_scenarios_run_local", "simon_scenarios_storage_download", "simon_moves_set_scope", "simon_moves_gpu_slots_download",
+           "simon_schedule_resume"]
 
 
 class EngineUnavailable(RuntimeError):
@@ -101,6 +102,9 @@ def lib():
         L.simon_moves_set_scope.argtypes = [C.c_void_p, C.c_uint32]
         L.simon_moves_gpu_slots_download.restype = C.c_int
         L.simon_moves_gpu_slots_download.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
+        L.simon_schedule_resume.restype = C.c_int
+        L.simon_schedule_resume.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_uint32, C.c_void_p]
     except AttributeError:
         if not os.environ.get("SIMON_GPU_LIB"):       # an experiment library may lack the newer entry points; the shipped one may not
             raise
@@ -179,6 +183,25 @@ class Engine:
         nf = min(n_fail.value, max_fail)
         return out_node, out_score, fail_counts[:nf], fail_pod[:nf]
 
+    def schedule_resume(self, prefix_node, max_fail: Optional[int] = None):
+        """simon_schedule_resume: rebuild the state pods [0, len(prefix_node)) leave at the nodes an earlier call gave them (its
+        out_node), then place the rest.  Returns (out_node, out_score, fail_counts, fail_pod) over ALL pods; the scores of the prefix
+        pods are 0 (not recomputed) and the failures are those of the placed rest only."""
+        P = self.c.pods_dims["n_pods"]
+        prefix = np.ascontiguousarray(prefix_node, dtype=np.int32)
+        n_prefix = len(prefix)
+        max_fail = max(P - n_prefix, 0) if max_fail is None else max_fail
+        n_fail = C.c_uint32(0)
+        out_node = np.full(max(P, 1), -9, np.int32)
+        out_score = np.zeros(max(P, 1), np.int64)
+        fail_counts = np.zeros((max(max_fail, 1), abi.N_FAIL_CODES), np.uint32)
+        fail_pod = np.zeros(max(max_fail, 1), np.uint32)
+        self._check(lib().simon_schedule_resume(self.h, prefix.ctypes.data if n_prefix else None, n_prefix, out_node.ctypes.data,
+                                                out_score.ctypes.data if self.record_scores else None,
+                                                fail_counts.ctypes.data, fail_pod.ctypes.data, max_fail, C.byref(n_fail)))
+        nf = min(n_fail.value, max_fail)
+        return out_node[:P], out_score[:P], fail_counts[:nf], fail_pod[:nf]
+
     def results(self, first: int = 0, count: Optional[int] = None):
         P = self.c.pods_dims["n_pods"]
         count = P - first if count is None else count
@@ -229,14 +252,18 @@ class Engine:
         self._check(lib().simon_devices_state_download(self.h, a.ctypes.data))
         return a[:self.c.n_nodes]
 
-    def gpu_slots(self, first: int = 0, count: Optional[int] = None):
-        """GPU-share Reserve results: per pod a list of device ids (one per GPU slot, ascending), [] if none."""
+    def gpu_slot_words(self, first: int = 0, count: Optional[int] = None) -> np.ndarray:
+        """GPU-share Reserve results as simon_gpu_slots_download packs them: per pod 4 bits per device = its slots there."""
         P = self.c.pods_dims["n_pods"]
         count = P - first if count is None else count
         a = np.zeros(max(count, 1), np.uint32)
         self._check(lib().simon_gpu_slots_download(self.h, first, count, a.ctypes.data))
+        return a[:count]
+
+    def gpu_slots(self, first: int = 0, count: Optional[int] = None):
+        """GPU-share Reserve results: per pod a list of device ids (one per GPU slot, ascending), [] if none."""
         out = []
-        for v in a[:count]:
+        for v in self.gpu_slot_words(first, count):
             v = int(v)
             out.append([d for d in range(8) for _ in range((v >> (4 * d)) & 15)])
         return out
@@ -248,12 +275,18 @@ class Engine:
         self._check(lib().simon_state_download_ext(self.h, rs.ctypes.data, gu.ctypes.data))
         return dict(req_scalar=rs[:K, :N], gpu_used=gu[:, :N])
 
-    def dump_pod(self, pod: int):
+    def dump_pod(self, pod: int, placed: Optional[np.ndarray] = None):
         """From the EMPTY state, schedule up to and including `pod`; return (out_node of the range, per-node totals,
-        per-node filter verdicts of that pod).  Leaves the context in that partial state."""
-        self.reset()
-        self._check(lib().simon_debug_set_dump_pod(self.h, pod))
-        out = self.schedule(0, pod + 1)[0]
+        per-node filter verdicts of that pod).  Leaves the context in that partial state.  placed: the out_node of an earlier run
+        of this pod list - the pods before `pod` are then not placed again but rebuilt at those nodes (simon_schedule_resume), and
+        the rest of the list is placed too."""
+        if placed is not None:
+            self._check(lib().simon_debug_set_dump_pod(self.h, pod))
+            out = self.schedule_resume(np.asarray(placed)[:pod], max_fail=0)[0][:pod + 1]
+        else:
+            self.reset()
+            self._check(lib().simon_debug_set_dump_pod(self.h, pod))
+            out = self.schedule(0, pod + 1)[0]
         self._check(lib().simon_debug_set_dump_pod(self.h, 0xffffffff))
         N = self.c.n_nodes
         tot = np.zeros(max(N, 1), np.int64)
