@@ -225,6 +225,9 @@ typedef struct simon_ctx_opts {
 #define SIMON_OPT_RECORD_SCORES 1u   /* also produce the winning total score per pod */
 #define SIMON_OPT_NO_PIN_FAST 2u     /* place the pods of pinned classes (DaemonSet pods) one decision at a time through the general
                                         path instead of evaluating a run of them in one pass (same results; for verification) */
+#define SIMON_OPT_FORCE_LARGE 4u     /* run the large-cluster variant (per-node arrays in global memory) at any cluster size, on
+                                        cluster_ctas x threads_per_cta when given (threads <= 320), else 16 x 320; a geometry that does
+                                        not fit is SIMON_ERR_LIMIT (same results; for verification) */
 
 /* One what-if scenario of the capacity-planning search (pkg/apply/apply.go:203-259):
  * the uploaded snapshot holds the base nodes plus a pool of candidate new nodes; a scenario
@@ -306,6 +309,23 @@ int simon_stats(simon_ctx *ctx, uint64_t *out32);
 float simon_last_kernel_ms(simon_ctx *ctx);
 /* Number of kernel launches issued by this ctx so far. */
 uint64_t simon_launch_count(simon_ctx *ctx);
+
+/* Diagnostic: the placement kernel the last simon_schedule / simon_schedule_resume / simon_replay / simon_scenarios_run[_local]
+ * launched and its geometry.  kernel is "" (and every other field 0) when that call ran no placement kernel, e.g. when the
+ * import kernel accounted every pod.  No placement depends on it. */
+typedef struct simon_launch_info {
+    char kernel[48];           /* the variant's symbol, e.g. "simon_place_kernel_384_2" */
+    uint32_t n_nodes;          /* nodes of the scenario the geometry was sized for (the largest of a batch) */
+    uint32_t cluster_ctas;     /* CTAs per scenario */
+    uint32_t threads_per_cta;
+    uint32_t node_slots;       /* node slots per thread */
+    uint32_t n_scenarios;
+    uint32_t large;            /* 1: the large-cluster variant (per-node arrays in global memory) */
+    uint32_t local;            /* 1: an Open-Local variant */
+    uint32_t reserved;
+    uint64_t smem_bytes;       /* dynamic shared memory per CTA */
+} simon_launch_info;
+int simon_last_launch(simon_ctx *ctx, simon_launch_info *out);
 
 /* Dynamic per-node state after scheduling: each pointer may be NULL. */
 int simon_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *req_mem, int64_t *req_eph,

@@ -245,6 +245,8 @@ struct simon_ctx {
     DevBuf<unsigned char> d_gnode;      // large-cluster variant: per-node arrays in global memory
     bool big = false;                   // set by choose_geometry for the next launch
     size_t gnode_stride = 0;
+    uint32_t geom_nodes = 0;            // the node count choose_geometry sized the next launch for
+    simon_launch_info last_launch{};    // what the last scheduling call launched (simon_last_launch)
     DevBuf<uint32_t> d_sig_class;       // a class per static signature (dense fill of the static verdict cache)
     bool static_filled = false;
     // scenario state: single runs (simon_schedule, simon_replay, ...) and scenario batches
@@ -427,6 +429,29 @@ sk_kernel_fn kernel_variant(const simon_ctx *ctx, uint32_t TPB, uint32_t npt, bo
     return npt == 1 ? simon_place_kernel_256_1 : npt == 2 ? simon_place_kernel_256_2 : npt == 3 ? simon_place_kernel_256_3 : npt == 4 ? simon_place_kernel_256_4 : simon_place_kernel_256_0;
 }
 
+// The symbol of every variant kernel_variant() returns (simon_last_launch)
+#define SK_NAMED(k) {k, #k}
+const struct { sk_kernel_fn fn; const char *name; } kernel_names[] = {
+    SK_NAMED(simon_place_kernel_256_0), SK_NAMED(simon_place_kernel_256_1), SK_NAMED(simon_place_kernel_256_2),
+    SK_NAMED(simon_place_kernel_256_3), SK_NAMED(simon_place_kernel_256_4), SK_NAMED(simon_place_kernel_320_0),
+    SK_NAMED(simon_place_kernel_320_1), SK_NAMED(simon_place_kernel_320_2), SK_NAMED(simon_place_kernel_320_3),
+    SK_NAMED(simon_place_kernel_320_4), SK_NAMED(simon_place_kernel_384_0), SK_NAMED(simon_place_kernel_384_1),
+    SK_NAMED(simon_place_kernel_384_2), SK_NAMED(simon_place_kernel_384_3), SK_NAMED(simon_place_kernel_big),
+    SK_NAMED(simon_local_kernel_256), SK_NAMED(simon_local_kernel_320), SK_NAMED(simon_local_kernel_384),
+    SK_NAMED(simon_local_kernel_big),
+    SK_NAMED(simon_prof_kernel_256_0), SK_NAMED(simon_prof_kernel_256_1), SK_NAMED(simon_prof_kernel_256_2),
+    SK_NAMED(simon_prof_kernel_256_3), SK_NAMED(simon_prof_kernel_256_4), SK_NAMED(simon_prof_kernel_320_0),
+    SK_NAMED(simon_prof_kernel_320_1), SK_NAMED(simon_prof_kernel_320_2), SK_NAMED(simon_prof_kernel_320_3),
+    SK_NAMED(simon_prof_kernel_320_4),
+};
+#undef SK_NAMED
+
+const char *kernel_name(sk_kernel_fn fn) {
+    for (const auto &k : kernel_names)
+        if (k.fn == fn) return k.name;
+    return "?";
+}
+
 // A launch of fn on `ctas` CTAs in clusters of `cs`, `t` threads and `smem` bytes of shared memory each, with fn's attributes set
 // for that shape.  cfg points to attr.
 cudaError_t cluster_config(sk_kernel_fn fn, uint32_t ctas, uint32_t cs, uint32_t t, size_t smem, cudaStream_t st, cudaLaunchConfig_t &cfg,
@@ -469,6 +494,21 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
     const uint32_t want_cs = ctx->opt_cluster, want_t = ctx->opt_threads;
     if (n_active == 0) n_active = 1;
     ctx->big = false;
+    ctx->geom_nodes = n_active;
+    if (ctx->opt_flags & SIMON_OPT_FORCE_LARGE) {
+        // the large-cluster variant at any size (verification: its code at few node slots per thread, on clusters a CPU checks)
+        const uint32_t cs = want_cs ? want_cs : 16, t = want_t ? want_t : 320;
+        if (cs > SK_MAX_CS) return fail(ctx, SIMON_ERR_LIMIT, "CTAs per scenario must be <= %u (got %u)", (unsigned)SK_MAX_CS, cs);
+        if (t > 320) return fail(ctx, SIMON_ERR_LIMIT, "the large-cluster variant runs at most 320 threads per CTA (got %u)", t);
+        const uint32_t npt = (n_active + cs * t - 1) / (cs * t);
+        const size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs, false);
+        if (npt > 64 || b > (size_t)max_smem)
+            return fail(ctx, SIMON_ERR_LIMIT, "%u nodes on %u CTAs x %u threads do not fit the large-cluster variant", n_active, cs, t);
+        CS = cs; TPB = t; NPT = npt; smem = b;
+        ctx->big = true;
+        ctx->gnode_stride = (sk_node_bytes(npt * t, ctx->T, ctx->emax) + 255) & ~(size_t)255;
+        return SIMON_OK;
+    }
     if (n_scen > 1 && !want_cs && !want_t) {
         // Batches are throughput work.  For every cluster size 1..16 (any integer: clusters need not be powers of two) take the
         // thread count with the fewest node slots per thread, ask the driver how many such clusters the device holds at once
@@ -585,6 +625,11 @@ int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t T
     CU(cudaLaunchKernelEx(&cfg, fn, P));
     if (record) CU(cudaEventRecord(ctx->ev1, ctx->stream));
     ctx->launches++;
+    simon_launch_info &li = ctx->last_launch;
+    li = simon_launch_info{};
+    snprintf(li.kernel, sizeof(li.kernel), "%s", kernel_name(fn));
+    li.n_nodes = ctx->geom_nodes; li.cluster_ctas = CS; li.threads_per_cta = TPB; li.node_slots = P.npt; li.n_scenarios = n_scen;
+    li.large = ctx->big; li.local = ctx->have_storage; li.smem_bytes = smem;
     return SIMON_OK;
 }
 
@@ -910,6 +955,7 @@ int simon_schedule(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_
     if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_schedule before uploads");
     if ((uint64_t)first + count > ctx->n_pods) return fail(ctx, SIMON_ERR_INVALID, "pod range out of bounds");
     CU(cudaSetDevice(ctx->device));
+    ctx->last_launch = simon_launch_info{};
     if (count == 0) { if (out_n_fail) *out_n_fail = 0; return SIMON_OK; }
     cudaStream_t st = ctx->stream;
     const ScenPool &S = ctx->single;
@@ -964,6 +1010,7 @@ int simon_schedule_resume(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n
         }
     }
     CU(cudaSetDevice(ctx->device));
+    ctx->last_launch = simon_launch_info{};
     cudaStream_t st = ctx->stream;
     ScenPool &S = ctx->single;
     uint32_t CS, TPB, NPT;
@@ -1027,6 +1074,7 @@ int simon_replay(simon_ctx *ctx, uint32_t steps, float *out_ms_total) {
     if (!ctx) return SIMON_ERR_INVALID;
     if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_replay before uploads");
     CU(cudaSetDevice(ctx->device));
+    ctx->last_launch = simon_launch_info{};
     cudaStream_t st = ctx->stream;
     ScenPool &S = ctx->single;
     uint32_t CS, TPB, NPT;
@@ -1063,6 +1111,12 @@ int simon_stats(simon_ctx *ctx, uint64_t *out8) {
 float simon_last_kernel_ms(simon_ctx *ctx) { return ctx ? ctx->last_ms : 0.f; }
 uint64_t simon_launch_count(simon_ctx *ctx) { return ctx ? ctx->launches : 0; }
 
+int simon_last_launch(simon_ctx *ctx, simon_launch_info *out) {
+    if (!ctx || !out) return SIMON_ERR_INVALID;
+    *out = ctx->last_launch;
+    return SIMON_OK;
+}
+
 int simon_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *req_mem, int64_t *req_eph, int64_t *nz_mcpu,
                          int64_t *nz_mem, int32_t *num_pods) {
     if (!ctx || !ctx->have_pods) return SIMON_ERR_STATE;
@@ -1082,6 +1136,7 @@ int simon_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *req_mem, in
 static int scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, simon_scenario_result *out,
                          simon_scenario_local_result *out_local, int32_t *out_node) {
     CU(cudaSetDevice(ctx->device));
+    ctx->last_launch = simon_launch_info{};
     cudaStream_t st = ctx->stream;
     if (n == 0) return SIMON_OK;
     const uint32_t N = ctx->N, N1 = std::max(1u, N);

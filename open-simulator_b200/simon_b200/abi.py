@@ -8,6 +8,7 @@ import numpy as np
 N_FAIL_CODES = 24
 OPT_RECORD_SCORES = 1
 OPT_NO_PIN_FAST = 2
+OPT_FORCE_LARGE = 4
 
 
 class SimonSnapshot(C.Structure):
@@ -36,6 +37,12 @@ class SimonPodset(C.Structure):
 class SimonCtxOpts(C.Structure):
     _fields_ = [("device", C.c_int32), ("cluster_ctas", C.c_uint32), ("threads_per_cta", C.c_uint32),
                 ("flags", C.c_uint32)]
+
+
+class SimonLaunchInfo(C.Structure):
+    _fields_ = [("kernel", C.c_char * 48), ("n_nodes", C.c_uint32), ("cluster_ctas", C.c_uint32), ("threads_per_cta", C.c_uint32),
+                ("node_slots", C.c_uint32), ("n_scenarios", C.c_uint32), ("large", C.c_uint32), ("local", C.c_uint32),
+                ("reserved", C.c_uint32), ("smem_bytes", C.c_uint64)]
 
 
 class SimonScenario(C.Structure):

@@ -26,7 +26,7 @@ EXPORTS = ["simon_gpu_version", "simon_ctx_create", "simon_ctx_destroy", "simon_
            "simon_host_simulate", "simon_host_free", "simon_host_quantity_probe", "simon_host_plan_fit_error", "simon_host_capacity_search",
            "simon_storage_upload", "simon_storage_state_download", "simon_devices_upload", "simon_devices_state_download",
            "simon_scenarios_run_local", "simon_scenarios_storage_download", "simon_moves_set_scope", "simon_moves_gpu_slots_download",
-           "simon_schedule_resume"]
+           "simon_schedule_resume", "simon_last_launch"]
 
 
 class EngineUnavailable(RuntimeError):
@@ -105,6 +105,8 @@ def lib():
         L.simon_schedule_resume.restype = C.c_int
         L.simon_schedule_resume.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                             C.c_uint32, C.c_void_p]
+        L.simon_last_launch.restype = C.c_int
+        L.simon_last_launch.argtypes = [C.c_void_p, C.c_void_p]
     except AttributeError:
         if not os.environ.get("SIMON_GPU_LIB"):       # an experiment library may lack the newer entry points; the shipped one may not
             raise
@@ -116,13 +118,15 @@ class Engine:
     """One device context holding one compiled cluster (snapshot + ordered pod list)."""
 
     def __init__(self, compiled, device: int = 0, record_scores: bool = False, cluster_ctas: int = 0,
-                 threads_per_cta: int = 0, pin_fast: bool = True):
+                 threads_per_cta: int = 0, pin_fast: bool = True, force_large: bool = False):
         L = lib()
         self.c = compiled
         self.h = C.c_void_p()
         # pin_fast=False: DaemonSet pods take the general one-decision-at-a-time path (SIMON_OPT_NO_PIN_FAST; same results)
+        # force_large=True: the large-cluster kernel variant at any size (SIMON_OPT_FORCE_LARGE; same results)
         opts = abi.SimonCtxOpts(device, cluster_ctas, threads_per_cta,
-                                (abi.OPT_RECORD_SCORES if record_scores else 0) | (0 if pin_fast else abi.OPT_NO_PIN_FAST))
+                                (abi.OPT_RECORD_SCORES if record_scores else 0) | (0 if pin_fast else abi.OPT_NO_PIN_FAST) |
+                                (abi.OPT_FORCE_LARGE if force_large else 0))
         rc = L.simon_ctx_create(C.byref(opts), C.byref(self.h))
         if rc != 0 or not self.h:
             raise EngineUnavailable(f"simon_ctx_create failed (rc={rc}): no usable CUDA device {device}; "
@@ -232,6 +236,15 @@ class Engine:
 
     def launch_count(self) -> int:
         return int(lib().simon_launch_count(self.h))
+
+    def last_launch(self) -> dict:
+        """The placement kernel the last schedule / schedule_resume / replay / run_scenarios call launched and its geometry;
+        kernel "" when none ran."""
+        li = abi.SimonLaunchInfo()
+        self._check(lib().simon_last_launch(self.h, C.byref(li)))
+        return dict(kernel=li.kernel.decode(), n_nodes=li.n_nodes, cluster_ctas=li.cluster_ctas, threads_per_cta=li.threads_per_cta,
+                    node_slots=li.node_slots, n_scenarios=li.n_scenarios, large=bool(li.large), local=bool(li.local),
+                    smem_bytes=int(li.smem_bytes))
 
     def state(self):
         N = self.c.n_nodes

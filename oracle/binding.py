@@ -37,6 +37,9 @@ def lib():
         _LIB.simon_oracle_schedule.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
                                                C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
         _LIB.simon_oracle_state.argtypes = [C.c_void_p] + [C.c_void_p] * 6
+        _LIB.simon_oracle_state_ext.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        _LIB.simon_oracle_gpu_slots.restype = C.c_int
+        _LIB.simon_oracle_gpu_slots.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
         _LIB.simon_oracle_moves_score.restype = C.c_int
         _LIB.simon_oracle_moves_score.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _LIB.simon_oracle_set_threads.restype = C.c_int
@@ -123,3 +126,21 @@ class Oracle:
         arrs = [np.zeros(N, np.int64) for _ in range(5)] + [np.zeros(N, np.int32)]
         lib().simon_oracle_state(self.h, *[a.ctypes.data for a in arrs])
         return dict(zip(["req_mcpu", "req_mem", "req_eph", "nz_mcpu", "nz_mem", "num_pods"], arrs))
+
+    def state_ext(self):
+        """Engine.state_ext's columns: req_scalar [K][N] and GPU-share device memory in use gpu_used [8][N]."""
+        N, K = self.c.n_nodes, int(self.c.snap_dims["n_scalars"])
+        rs = np.zeros((max(K, 1), max(N, 1)), np.int64)
+        gu = np.zeros((8, max(N, 1)), np.int64)
+        lib().simon_oracle_state_ext(self.h, rs.ctypes.data, gu.ctypes.data)
+        return dict(req_scalar=rs[:K, :N], gpu_used=gu[:, :N])
+
+    def gpu_slot_words(self, first=0, count=None):
+        """Engine.gpu_slot_words: per pod 4 bits per device = the GPU-share slots Reserve gave it there."""
+        P = self.c.pods_dims["n_pods"]
+        count = P - first if count is None else count
+        a = np.zeros(max(count, 1), np.uint32)
+        rc = lib().simon_oracle_gpu_slots(self.h, first, count, a.ctypes.data)
+        if rc != 0:
+            raise RuntimeError(f"simon_oracle_gpu_slots rc={rc}")
+        return a[:count]

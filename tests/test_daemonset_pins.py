@@ -8,7 +8,7 @@ import pytest
 
 from simon_b200 import objects as O, simulator, synth
 from simon_b200.compiler import CLS_PINNED, SCW_FLAGS, SCW_GUARD_NODE, compile_cluster
-from util import run_oracle, run_pyref
+from util import assert_ext_equal, run_oracle, run_oracle_ext, run_pyref
 
 
 def _node(name, cpu="4", zone=None, taints=None, unschedulable=False, labels=None):
@@ -132,11 +132,12 @@ def test_mixed_clusters_with_daemonsets_cpu(seed):
 def _gpu_cmp(c):
     """Both device paths of pinned pods - the run-at-once fast path and the general decision path - against the oracle."""
     from simon_b200.engine import Engine
-    (ref, rscore, rfc, rfp), rstate = run_oracle(c)
+    (ref, rscore, rfc, rfp), rstate, rext, rslots = run_oracle_ext(c)
     for pin_fast in (True, False):
         with Engine(c, device=0, record_scores=True, pin_fast=pin_fast) as eng:
             out, score, fc, fp = eng.schedule()
             st = eng.state()
+            assert_ext_equal(eng, rext, rslots, f"pin_fast={pin_fast}")
             eng.reset()
             half = len(ref) // 2                                    # split calls: a run of pinned pods cut by the call boundary
             out2 = np.concatenate([eng.schedule(0, half)[0], eng.schedule(half, len(ref) - half)[0]])

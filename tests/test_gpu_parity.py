@@ -2,7 +2,7 @@
 import numpy as np
 import pytest
 
-from util import make_case, run_oracle
+from util import assert_ext_equal, make_case, run_oracle, run_oracle_ext
 
 pytestmark = pytest.mark.gpu
 
@@ -44,10 +44,11 @@ def test_parity_mixed_features(seed):
     """synth.make_mix: every predicate / score input in random combination (see tests/test_oracle_cpu.py), incl. GPU share,
     host ports, extended resources, hard spread constraints, required pod affinity, DaemonSets and pre-bound pods."""
     p, c = make_case("mix", seed_no=seed, n_nodes=20 + (seed % 5) * 25, n_workloads=20 + (seed % 7) * 10, max_replicas=4 + seed % 6)
-    (ref, rscore, rfc, rfp), rstate = run_oracle(c)
+    (ref, rscore, rfc, rfp), rstate, rext, rslots = run_oracle_ext(c)
     with _engine(c) as eng:
         out, score, fc, fp = eng.schedule()
         st = eng.state()
+        assert_ext_equal(eng, rext, rslots)
     np.testing.assert_array_equal(out, ref)
     sched = ref >= 0
     np.testing.assert_array_equal(score[sched & (rscore > 0)], rscore[sched & (rscore > 0)])

@@ -336,17 +336,24 @@ def test_engine_matches_cpu_port_with_restated_open_local(seed, n_nodes, n_pods)
     Filter, ScoreLVM and NormalizeScore are applied on top from the VG state the engine's earlier Binds left (storage.py).
     Clusters with several feasible storage nodes whose raw scores differ exercise the score path; 41,000 nodes the
     large-cluster variant; zero-VG annotated nodes and dropped-device-only pods the no-LVM case."""
-    import ctypes
-    from oracle.binding import Oracle
     from simon_b200.engine import Engine
-    from simon_b200.storage import StorageReplay, lvm_place, normalize_scores
     rng = np.random.default_rng(seed)
     nodes, pods, scs = _oracle_cluster(rng, n_nodes, n_pods)
     c = compile_cluster(nodes, pods, open_local=True, storage_classes=scs)
-    st = c.storage
     with Engine(c, record_scores=True) as eng:
         out, score, _fc, _fp = eng.schedule()
         final = eng.storage_state()
+    assert check_restated_open_local(c, out, score, final) > 0     # the score path decided some placements
+
+
+def check_restated_open_local(c, out, score, final):
+    """The composition above, pod by pod, for an engine run of a cluster of _oracle_cluster: out / score are its placements and
+    recorded winning scores, final its VG requested state.  Returns the number of storage pods that had several feasible nodes
+    with different raw Open-Local scores."""
+    import ctypes
+    from oracle.binding import Oracle
+    from simon_b200.storage import StorageReplay, lvm_place, normalize_scores
+    st = c.storage
     orc = Oracle(c)
     orc.enable_dump()
     P = c.pods_dims["n_pods"]
@@ -393,7 +400,7 @@ def test_engine_matches_cpu_port_with_restated_open_local(seed, n_nodes, n_pods)
             rep.bind(cls, int(out[i]))
     orc.close()
     assert np.array_equal(final, rep.requested())
-    assert multi > 0          # the score path decided some placements
+    return multi
 
 
 @pytest.mark.gpu

@@ -3,8 +3,9 @@ driver's; the file sorts last so that a failure here cannot mask the rest of the
 
   * soft spread over a topology with more domains than the per-decision bitmask holds (SCW_ANY_TABLE: per-domain tables
     in global memory instead of the 6 x 64-bit presence words);
-  * the kernel variants with a run-time number of nodes per thread (NPT_T = 0: more than 4 nodes per thread at <= 256
-    threads, more than 2 at 320 threads).
+  * the kernel variant with a run-time number of nodes per thread at <= 256 threads (NPT_T = 0: more than 4 nodes per thread),
+    and next to it the unrolled 3-slot variant at 320 threads; tests/test_zz_kernel_variants_gpu.py covers every variant,
+    simon_place_kernel_320_0 (more than 4 nodes per thread at 257-320 threads) included.
 """
 import os
 import sys
@@ -68,6 +69,12 @@ def test_soft_spread_over_a_topology_larger_than_the_bitmask():
 
 @pytest.mark.parametrize("cs,tpb", [(1, 64), (1, 320), (1, 128)])
 def test_runtime_nodes_per_thread_variants(cs, tpb):
+    """700 nodes on one CTA: 11 and 6 node slots per thread at 64 and 128 threads (run-time slot count), 3 at 320 threads."""
     from util import make_case
     p, c = make_case("c3", n_nodes=700, n_workloads=80, replicas=12, n_apps=2, seed_no=13)
     _cmp(c, cluster_ctas=cs, threads_per_cta=tpb)
+    kernel = {64: "simon_place_kernel_256_0", 128: "simon_place_kernel_256_0", 320: "simon_place_kernel_320_3"}[tpb]
+    from simon_b200.engine import Engine
+    with Engine(c, device=0, cluster_ctas=cs, threads_per_cta=tpb) as eng:
+        eng.schedule(download=False)
+        assert eng.last_launch()["kernel"] == kernel

@@ -21,6 +21,24 @@ def run_oracle(c):
     return out, st
 
 
+def run_oracle_ext(c):
+    """run_oracle plus the state the parity of extended resources and GPU share needs: (out, state, state_ext, GPU slot words)."""
+    from oracle.binding import Oracle
+    o = Oracle(c)
+    out = o.schedule()
+    res = out, o.state(), o.state_ext(), o.gpu_slot_words()
+    o.close()
+    return res
+
+
+def assert_ext_equal(eng, rext, rslots, what=""):
+    """Engine.state_ext() and the per-pod GPU-share device slots equal the oracle's."""
+    ext = eng.state_ext()
+    for k in rext:
+        np.testing.assert_array_equal(ext[k], rext[k], err_msg=f"{what} {k}")
+    np.testing.assert_array_equal(eng.gpu_slot_words(), rslots, err_msg=f"{what} GPU slots")
+
+
 def run_pyref(p, c):
     from oracle.pyref import PyRef
     ref = PyRef(c.node_objs, services=p.ctx.services, replicasets=p.ctx.replicasets, statefulsets=p.ctx.statefulsets,
