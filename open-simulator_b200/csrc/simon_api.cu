@@ -267,6 +267,18 @@ struct simon_ctx {
     DevBuf<uint8_t> d_node_n_ssd, d_node_n_hdd;
     DevBuf<int64_t> d_dev_cap, d_ssd_size, d_hdd_size;
     DevBuf<uint32_t> d_ssd_off, d_hdd_off, d_dev_alloc0;
+    // drain batches (simon_drain_run).  The last batch: dr_n scenarios (0: none since the last upload), per scenario its evicted pods (CSR dr_off / dr_pods, pod order),
+    // blocked pods (dr_boff / dr_blocked) and failures; on the device the evicted pods' nodes, scores, GPU slots and failure records
+    // (dr_max rows per scenario: its largest evictee list); the device times of the setup (ev0 .. evm) and the placement (evm .. ev1)
+    std::vector<int32_t> h_class;
+    cudaEvent_t evm = nullptr;
+    uint32_t dr_n = 0, dr_max = 0;
+    std::vector<uint32_t> dr_off, dr_pods, dr_boff, dr_blocked, dr_nfail;
+    DevBuf<uint32_t> d_dr_pods, d_dr_off, d_dr_gpu, d_dr_fail_counts, d_dr_fail_pod;
+    DevBuf<int32_t> d_dr_node;
+    DevBuf<int64_t> d_dr_score;
+    DevBuf<uint2> d_dr_pairs;
+    float dr_setup_ms = 0.f, dr_place_ms = 0.f;
 };
 
 namespace {
@@ -338,13 +350,14 @@ int clear_pool(simon_ctx *ctx, ScenPool &s) {
     return SIMON_OK;
 }
 
-// Size every column of `s` for n scenarios of the current uploads (DevBuf keeps the capacity) and clear it.  single: the pool of
-// single runs, with their per-pod outputs and its one SkScenario (every node) uploaded; else a batch pool, with node lists and results.
-int alloc_pool(simon_ctx *ctx, ScenPool &s, uint32_t n, bool single) {
+// Size every column of `s` for n scenarios of the current uploads (DevBuf keeps the capacity), without clearing it.  single: the pool
+// of single runs, with their per-pod outputs and its one SkScenario (every node) uploaded; else a batch pool, with node lists and
+// results, and with out_node [n][P] unless pod_outputs is false (drain batches keep their per-pod outputs elsewhere).
+int size_pool(simon_ctx *ctx, ScenPool &s, uint32_t n, bool single, bool pod_outputs = true) {
     s.n = n;
     s.nodes = std::max(1u, ctx->N); s.scal = (size_t)(ctx->K ? ctx->K : 1) * s.nodes;
     s.cntw = std::max<uint64_t>(1, ctx->cnt_words); s.nct = std::max(1u, ctx->n_counters); s.ncl = std::max(1u, ctx->n_classes);
-    s.tabw = (size_t)SK_MAX_SOFT * ctx->max_dom; s.regw = (size_t)SK_MAX_HARD * ctx->max_dom; s.pods = std::max(1u, ctx->n_pods);
+    s.tabw = (size_t)SK_MAX_SOFT * ctx->max_dom; s.regw = (size_t)SK_MAX_HARD * ctx->max_dom; s.pods = pod_outputs ? std::max(1u, ctx->n_pods) : 1;
     s.vn = std::max<size_t>(1, (size_t)ctx->V * ctx->N);
     const size_t nn = (size_t)n * s.nodes;
     CU(s.req_mcpu.alloc(nn)); CU(s.req_mem.alloc(nn)); CU(s.req_eph.alloc(nn)); CU(s.nz_mcpu.alloc(nn)); CU(s.nz_mem.alloc(nn));
@@ -368,7 +381,13 @@ int alloc_pool(simon_ctx *ctx, ScenPool &s, uint32_t n, bool single) {
     }
     if (ctx->have_storage) { CU(s.vg_req.alloc(n * s.vn)); CU(s.local_raw.alloc(nn)); }
     if (ctx->have_devices) CU(s.dev_alloc.alloc(nn));
-    return clear_pool(ctx, s);
+    return SIMON_OK;
+}
+
+// size_pool, then every scenario back to the empty cluster (clear_pool)
+int alloc_pool(simon_ctx *ctx, ScenPool &s, uint32_t n, bool single) {
+    const int rc = size_pool(ctx, s, n, single);
+    return rc ? rc : clear_pool(ctx, s);
 }
 
 // the launch parameters of the current uploads on pool `s` (its SkScenario array and Open-Local slices)
@@ -408,9 +427,14 @@ void fill_params(simon_ctx *ctx, const ScenPool &s, SkParams &P) {
 typedef void (*sk_kernel_fn)(const SkParams);
 // The compiled kernel variant for (threads per CTA, node slots per thread) on the context's uploads, which is what launch() runs
 // and what the geometry is sized for.  big: the large-cluster variant; prof: with per-phase clock64 timers.  With Open-Local
-// storage uploaded, the local variants (more registers than the plain ones, runtime node slots per thread, no timers).
-// nullptr: none.
-sk_kernel_fn kernel_variant(const simon_ctx *ctx, uint32_t TPB, uint32_t npt, bool big, bool prof) {
+// storage uploaded, the local variants (more registers than the plain ones, runtime node slots per thread, no timers).  drain: the
+// drain-batch variants (simon_drain_run), whatever was uploaded.  nullptr: none.
+sk_kernel_fn kernel_variant(const simon_ctx *ctx, uint32_t TPB, uint32_t npt, bool big, bool prof, bool drain) {
+    if (drain) {            // runtime node slots per thread, no timers, no Open-Local code
+        if (big) return simon_drain_kernel_big;
+        if (TPB > SIMON_MAX_TPB) return nullptr;
+        return TPB <= 256 ? simon_drain_kernel_256 : TPB <= 320 ? simon_drain_kernel_320 : simon_drain_kernel_384;
+    }
     if (big) return ctx->have_storage ? simon_local_kernel_big : simon_place_kernel_big;
     if (TPB > SIMON_MAX_TPB) return nullptr;
     if (ctx->have_storage) {
@@ -439,6 +463,7 @@ const struct { sk_kernel_fn fn; const char *name; } kernel_names[] = {
     SK_NAMED(simon_place_kernel_384_2), SK_NAMED(simon_place_kernel_384_3), SK_NAMED(simon_place_kernel_big),
     SK_NAMED(simon_local_kernel_256), SK_NAMED(simon_local_kernel_320), SK_NAMED(simon_local_kernel_384),
     SK_NAMED(simon_local_kernel_big),
+    SK_NAMED(simon_drain_kernel_256), SK_NAMED(simon_drain_kernel_320), SK_NAMED(simon_drain_kernel_384), SK_NAMED(simon_drain_kernel_big),
     SK_NAMED(simon_prof_kernel_256_0), SK_NAMED(simon_prof_kernel_256_1), SK_NAMED(simon_prof_kernel_256_2),
     SK_NAMED(simon_prof_kernel_256_3), SK_NAMED(simon_prof_kernel_256_4), SK_NAMED(simon_prof_kernel_320_0),
     SK_NAMED(simon_prof_kernel_320_1), SK_NAMED(simon_prof_kernel_320_2), SK_NAMED(simon_prof_kernel_320_3),
@@ -473,8 +498,8 @@ cudaError_t cluster_config(sk_kernel_fn fn, uint32_t ctas, uint32_t cs, uint32_t
 // Clusters of `cs` CTAs x `t` threads x `npt` node slots with `smem` bytes each of the variant for that shape that the device
 // holds at once, GPC boundaries included (0: not even one; a 16-CTA cluster needs 16 free SMs in one GPC).  The variants with
 // phase timers run in the geometry of the default ones.
-int max_active_clusters(const simon_ctx *ctx, bool big, uint32_t cs, uint32_t t, uint32_t npt, size_t smem) {
-    const sk_kernel_fn fn = kernel_variant(ctx, t, npt, big, false);
+int max_active_clusters(const simon_ctx *ctx, bool big, uint32_t cs, uint32_t t, uint32_t npt, size_t smem, bool drain) {
+    const sk_kernel_fn fn = kernel_variant(ctx, t, npt, big, false, drain);
     if (!fn) return 0;
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute attr;
@@ -486,8 +511,9 @@ int max_active_clusters(const simon_ctx *ctx, bool big, uint32_t cs, uint32_t t,
     return n;
 }
 
-// choose cluster size / threads / nodes-per-thread for n_active nodes
-int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &TPB, uint32_t &NPT, size_t &smem, uint32_t n_scen = 1) {
+// choose cluster size / threads / nodes-per-thread for n_active nodes, for the variants launch(..., drain) runs
+int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &TPB, uint32_t &NPT, size_t &smem, uint32_t n_scen = 1,
+                    bool drain = false) {
     int max_smem = 0;
     cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device);
     const uint32_t cs_opts[5] = {16, 8, 4, 2, 1};
@@ -533,7 +559,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
             if (npt > 64) continue;
             const size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs);
             if (b > (size_t)max_smem) continue;
-            const int active = max_active_clusters(ctx, false, cs, t, npt, b);
+            const int active = max_active_clusters(ctx, false, cs, t, npt, b, drain);
             if (active <= 0) continue;
             const uint32_t waves = (n_scen + (uint32_t)active - 1) / (uint32_t)active;
             const double cost = waves * (265.0 + 196.0 * npt + (t > 320 ? 18.0 : 0.0) + 5.0 * cs);
@@ -561,7 +587,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
             if (n384 < npt_p) { t_p = 384; npt_p = n384; }
         }
         const size_t b = sk_smem_bytes(npt_p * t_p, ctx->T, ctx->emax, ctx->max_blob_words, cs_p);
-        if (npt_p <= 64 && b <= (size_t)max_smem && max_active_clusters(ctx, false, cs_p, t_p, npt_p, b) > 0) {
+        if (npt_p <= 64 && b <= (size_t)max_smem && max_active_clusters(ctx, false, cs_p, t_p, npt_p, b, drain) > 0) {
             CS = cs_p; TPB = t_p; NPT = npt_p; smem = b; return SIMON_OK;
         }
     }
@@ -582,7 +608,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
             }
             if (t > SIMON_MAX_TPB) return fail(ctx, SIMON_ERR_LIMIT, "threads per CTA must be <= %u (got %u)", SIMON_MAX_TPB, t);
             size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs);
-            if (b <= (size_t)max_smem && (want_cs || max_active_clusters(ctx, false, cs, t, npt, b) > 0)) {
+            if (b <= (size_t)max_smem && (want_cs || max_active_clusters(ctx, false, cs, t, npt, b, drain) > 0)) {
                 CS = cs; TPB = t; NPT = npt; smem = b; return SIMON_OK;
             }
             if (want_t) break;
@@ -594,7 +620,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
         const uint32_t cs = 16, t = 320;
         const uint32_t npt = (n_active + cs * t - 1) / (cs * t);
         const size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs, false);
-        if (npt <= 64 && b <= (size_t)max_smem && max_active_clusters(ctx, true, cs, t, npt, b) > 0) {
+        if (npt <= 64 && b <= (size_t)max_smem && max_active_clusters(ctx, true, cs, t, npt, b, drain) > 0) {
             CS = cs; TPB = t; NPT = npt; smem = b;
             ctx->big = true;
             ctx->gnode_stride = (sk_node_bytes(npt * t, ctx->T, ctx->emax) + 255) & ~(size_t)255;
@@ -606,11 +632,12 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
 
 static_assert(sizeof(SkScenario) % 8 == 0, "SkScenario is copied in 8-byte words");
 
-int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t TPB, size_t smem, bool record = true) {
+// drain: a drain-batch variant (P carries drain_pods / drain_off)
+int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t TPB, size_t smem, bool record = true, bool drain = false) {
     // SIMON_PROFILE=1 selects the variants with per-phase clock64 timers (simon_stats cycles); the default variants
     // carry no timers
     static const bool prof = getenv("SIMON_PROFILE") != nullptr;
-    const sk_kernel_fn fn = kernel_variant(ctx, TPB, P.npt, ctx->big, prof);
+    const sk_kernel_fn fn = kernel_variant(ctx, TPB, P.npt, ctx->big, prof, drain);
     if (!fn)
         return fail(ctx, SIMON_ERR_LIMIT, "no kernel variant for %u threads per CTA%s%s", TPB, prof ? " with phase timers" : "",
                     ctx->have_storage ? " and Open-Local storage" : "");
@@ -629,7 +656,7 @@ int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t T
     li = simon_launch_info{};
     snprintf(li.kernel, sizeof(li.kernel), "%s", kernel_name(fn));
     li.n_nodes = ctx->geom_nodes; li.cluster_ctas = CS; li.threads_per_cta = TPB; li.node_slots = P.npt; li.n_scenarios = n_scen;
-    li.large = ctx->big; li.local = ctx->have_storage; li.smem_bytes = smem;
+    li.large = ctx->big; li.local = ctx->have_storage && !drain; li.smem_bytes = smem;
     return SIMON_OK;
 }
 
@@ -655,6 +682,50 @@ int launch_range(simon_ctx *ctx, SkParams &P, uint32_t CS, uint32_t TPB, size_t 
     return SIMON_OK;
 }
 
+// simon_schedule_resume's checks of a placed prefix (include/simon_gpu.h), on the host before any device work
+int check_prefix(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n_prefix) {
+    const int32_t N = (int32_t)ctx->N;
+    for (uint32_t i = 0; i < n_prefix; i++) {
+        const int32_t e = prefix_node[i], f = ctx->h_fixed[i], gd = ctx->h_guard[i];
+        if (e < -3 || e >= N) return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u: node %d out of range", i, e);
+        if (ctx->bypass[i]) {
+            // what the import gives a pod that does not reach the scheduler: absent -3, bound to a node outside the cluster -2
+            const int32_t want = gd == -2 ? -3 : (f >= 0 ? f : -2);
+            if (e != want) return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u does not reach the scheduler and is reported as %d, not %d", i, want, e);
+        } else if (e < -1) {
+            return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u reaches the scheduler: %d is not a node or -1", i, e);
+        } else if (gd >= 0 && e != -1 && e != gd) {
+            return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u is pinned to node %d, not %d", i, gd, e);
+        }
+    }
+    return SIMON_OK;
+}
+
+// On the cleared single-scenario pool of P: the state a checked prefix leaves, enqueued on the ctx stream.  The import accounts the
+// sums (requests, pod counts, scalars, counters) and writes the prefix's per-pod results; GPU-share memory and Open-Local state are
+// replayed node by node in placement order.
+int rebuild_prefix(simon_ctx *ctx, const SkParams &P, const int32_t *prefix_node, uint32_t n_prefix) {
+    if (!n_prefix) return SIMON_OK;
+    cudaStream_t st = ctx->stream;
+    CU(ctx->d_prefix.upload(prefix_node, n_prefix, st));
+    const uint32_t grid = std::min<uint32_t>((n_prefix + 255) / 256, (uint32_t)ctx->sms * 4);
+    simon_import_kernel<<<grid, 256, 0, st>>>(P, 0, n_prefix, ctx->d_prefix.p);
+    CU(cudaGetLastError());
+    ctx->launches++;
+    const uint32_t N1 = std::max(1u, ctx->N);
+    CU(ctx->d_rs_cnt.alloc(N1)); CU(ctx->d_rs_off.alloc(N1 + 1)); CU(ctx->d_rs_cur.alloc(N1)); CU(ctx->d_rs_list.alloc(n_prefix));
+    CU(cudaMemsetAsync(ctx->d_rs_cnt.p, 0, 4ull * N1, st));
+    SkParams R = P;
+    R.vg_req_stride = 0; R.node_stride = 0;      // plain CTAs, not one cluster per scenario: every CTA reads slice 0
+    simon_resume_count<<<grid, 256, 0, st>>>(R, ctx->d_prefix.p, n_prefix, ctx->d_rs_cnt.p);
+    simon_resume_scan<<<1, 1024, 0, st>>>(ctx->d_rs_cnt.p, ctx->N, ctx->d_rs_off.p, ctx->d_rs_cur.p);
+    simon_resume_fill<<<grid, 256, 0, st>>>(R, ctx->d_prefix.p, n_prefix, ctx->d_rs_cur.p, ctx->d_rs_list.p);
+    simon_resume_replay<<<(N1 + 127) / 128, 128, 0, st>>>(R, ctx->d_rs_off.p, ctx->d_rs_list.p);
+    CU(cudaGetLastError());
+    ctx->launches += 4;
+    return SIMON_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -677,7 +748,7 @@ int simon_ctx_create(const simon_ctx_opts *opts, simon_ctx **out) {
         return SIMON_ERR_CUDA;
     }
     if (cudaSetDevice(ctx->device) != cudaSuccess || cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreate(&ctx->ev0) != cudaSuccess || cudaEventCreate(&ctx->ev1) != cudaSuccess) {
+        cudaEventCreate(&ctx->ev0) != cudaSuccess || cudaEventCreate(&ctx->ev1) != cudaSuccess || cudaEventCreate(&ctx->evm) != cudaSuccess) {
         delete ctx;
         return SIMON_ERR_CUDA;
     }
@@ -691,6 +762,7 @@ void simon_ctx_destroy(simon_ctx *ctx) {
     cudaSetDevice(ctx->device);
     if (ctx->ev0) cudaEventDestroy(ctx->ev0);
     if (ctx->ev1) cudaEventDestroy(ctx->ev1);
+    if (ctx->evm) cudaEventDestroy(ctx->evm);
     if (ctx->stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
 }
@@ -725,6 +797,7 @@ int simon_snapshot_upload(simon_ctx *ctx, const simon_snapshot *s) {
     ctx->have_storage = false;
     ctx->have_devices = false;
     ctx->batch.n_storage = 0;
+    ctx->dr_n = 0;
     return SIMON_OK;
 }
 
@@ -736,6 +809,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     ctx->have_storage = false;          // the storage tables are per class: a new pod set needs its own upload
     ctx->have_devices = false;
     ctx->batch.n_storage = 0;
+    ctx->dr_n = 0;
     ctx->n_classes = p->n_classes; ctx->n_pods = p->n_pods; ctx->n_counters = p->n_counters;
     // validate classes; derive limits
     uint32_t max_words = SCW_HDR_WORDS, emax = 0;
@@ -908,6 +982,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     for (uint32_t i = 0; i < p->n_pods; i++) ctx->bypass[i] = (guard[i] == -2 || p->pod_fixed_node[i] != -1) ? 1 : 0;
     ctx->h_fixed.assign(p->pod_fixed_node, p->pod_fixed_node + p->n_pods);
     ctx->h_guard.assign(guard.begin(), guard.begin() + p->n_pods);
+    ctx->h_class.assign(p->pod_class, p->pod_class + p->n_pods);
     CU(cudaStreamSynchronize(st));
     ctx->max_fail = std::max(1u, p->n_pods);      // every pod of the list may fail: one histogram row each (96 B)
     int rc = alloc_pool(ctx, ctx->single, 1, true);
@@ -995,27 +1070,15 @@ int simon_schedule_resume(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n
     if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_schedule_resume before uploads");
     if (n_prefix > ctx->n_pods) return fail(ctx, SIMON_ERR_INVALID, "prefix of %u pods exceeds the %u uploaded", n_prefix, ctx->n_pods);
     if (n_prefix && !prefix_node) return fail(ctx, SIMON_ERR_INVALID, "prefix_node is NULL");
-    const int32_t N = (int32_t)ctx->N;
-    for (uint32_t i = 0; i < n_prefix; i++) {
-        const int32_t e = prefix_node[i], f = ctx->h_fixed[i], gd = ctx->h_guard[i];
-        if (e < -3 || e >= N) return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u: node %d out of range", i, e);
-        if (ctx->bypass[i]) {
-            // what the import gives a pod that does not reach the scheduler: absent -3, bound to a node outside the cluster -2
-            const int32_t want = gd == -2 ? -3 : (f >= 0 ? f : -2);
-            if (e != want) return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u does not reach the scheduler and is reported as %d, not %d", i, want, e);
-        } else if (e < -1) {
-            return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u reaches the scheduler: %d is not a node or -1", i, e);
-        } else if (gd >= 0 && e != -1 && e != gd) {
-            return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u is pinned to node %d, not %d", i, gd, e);
-        }
-    }
+    int rc = check_prefix(ctx, prefix_node, n_prefix);
+    if (rc) return rc;
     CU(cudaSetDevice(ctx->device));
     ctx->last_launch = simon_launch_info{};
     cudaStream_t st = ctx->stream;
     ScenPool &S = ctx->single;
     uint32_t CS, TPB, NPT;
     size_t smem;
-    int rc = choose_geometry(ctx, ctx->N, CS, TPB, NPT, smem);
+    rc = choose_geometry(ctx, ctx->N, CS, TPB, NPT, smem);
     if (rc) return rc;
     SkParams P;
     fill_params(ctx, S, P);
@@ -1031,26 +1094,8 @@ int simon_schedule_resume(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n
         CU(cudaMemsetAsync(ctx->d_dump_code.p, 0, 4ull * std::max(1u, ctx->N), st));
     }
     CU(cudaEventRecord(ctx->ev0, st));
-    if (n_prefix) {
-        // the sums of the prefix (requests, pod counts, scalars, counters) and its per-pod results, by the import
-        CU(ctx->d_prefix.upload(prefix_node, n_prefix, st));
-        const uint32_t grid = std::min<uint32_t>((n_prefix + 255) / 256, (uint32_t)ctx->sms * 4);
-        simon_import_kernel<<<grid, 256, 0, st>>>(P, 0, n_prefix, ctx->d_prefix.p);
-        CU(cudaGetLastError());
-        ctx->launches++;
-        // GPU-share memory and Open-Local state: each node replays its own prefix pods in placement order
-        const uint32_t N1 = std::max(1u, ctx->N);
-        CU(ctx->d_rs_cnt.alloc(N1)); CU(ctx->d_rs_off.alloc(N1 + 1)); CU(ctx->d_rs_cur.alloc(N1)); CU(ctx->d_rs_list.alloc(n_prefix));
-        CU(cudaMemsetAsync(ctx->d_rs_cnt.p, 0, 4ull * N1, st));
-        SkParams R = P;
-        R.vg_req_stride = 0; R.node_stride = 0;      // plain CTAs, not one cluster per scenario: every CTA reads slice 0
-        simon_resume_count<<<grid, 256, 0, st>>>(R, ctx->d_prefix.p, n_prefix, ctx->d_rs_cnt.p);
-        simon_resume_scan<<<1, 1024, 0, st>>>(ctx->d_rs_cnt.p, ctx->N, ctx->d_rs_off.p, ctx->d_rs_cur.p);
-        simon_resume_fill<<<grid, 256, 0, st>>>(R, ctx->d_prefix.p, n_prefix, ctx->d_rs_cur.p, ctx->d_rs_list.p);
-        simon_resume_replay<<<(N1 + 127) / 128, 128, 0, st>>>(R, ctx->d_rs_off.p, ctx->d_rs_list.p);
-        CU(cudaGetLastError());
-        ctx->launches += 4;
-    }
+    rc = rebuild_prefix(ctx, P, prefix_node, n_prefix);
+    if (rc) return rc;
     if (count) {
         rc = launch_range(ctx, P, CS, TPB, smem, first, count, false);
         if (rc) return rc;
@@ -1132,6 +1177,30 @@ int simon_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *req_mem, in
     return SIMON_OK;
 }
 
+// The node lists of a batch into the batch pool's host columns h_order / h_rank (scenario order and its inverse), each checked: at most
+// N nodes, every one in range and listed once.  `what` names a scenario in the messages.
+static int scenario_lists(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, const char *what, uint32_t &max_active) {
+    const uint32_t N = ctx->N, N1 = std::max(1u, N);
+    ScenPool &B = ctx->batch;
+    max_active = 0;
+    B.h_order.assign((size_t)n * N1, 0u);
+    B.h_rank.assign((size_t)n * N1, -1);
+    for (uint32_t i = 0; i < n; i++) {
+        if (scen[i].n_nodes > N) return fail(ctx, SIMON_ERR_INVALID, "%s %u: too many nodes", what, i);
+        if (scen[i].n_nodes && !scen[i].nodes) return fail(ctx, SIMON_ERR_INVALID, "%s %u: nodes is NULL", what, i);
+        int32_t *rank = B.h_rank.data() + (size_t)i * N1;
+        for (uint32_t r = 0; r < scen[i].n_nodes; r++) {
+            const uint32_t g = scen[i].nodes[r];
+            if (g >= N) return fail(ctx, SIMON_ERR_INVALID, "%s %u: bad node list (node %u out of range)", what, i, g);
+            if (rank[g] != -1) return fail(ctx, SIMON_ERR_INVALID, "%s %u: bad node list (node %u listed twice)", what, i, g);
+            rank[g] = (int32_t)r;
+        }
+        std::copy(scen[i].nodes, scen[i].nodes + scen[i].n_nodes, B.h_order.begin() + (size_t)i * N1);
+        max_active = std::max(max_active, scen[i].n_nodes);
+    }
+    return SIMON_OK;
+}
+
 // simon_scenarios_run and simon_scenarios_run_local (out_local != nullptr: each scenario carries its own Open-Local state)
 static int scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, simon_scenario_result *out,
                          simon_scenario_local_result *out_local, int32_t *out_node) {
@@ -1145,22 +1214,11 @@ static int scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n,
     if (local) B.n_storage = 0;         // the slices are overwritten below
     // ---- node lists: validated on the host, uploaded in ONE copy each (scenario order and its inverse) ----
     uint32_t max_active = 0;
-    B.h_order.assign((size_t)n * N1, 0u);
-    B.h_rank.assign((size_t)n * N1, -1);
-    for (uint32_t i = 0; i < n; i++) {
-        if (scen[i].n_nodes > N) return fail(ctx, SIMON_ERR_INVALID, "scenario %u: too many nodes", i);
-        int32_t *rank = B.h_rank.data() + (size_t)i * N1;
-        for (uint32_t r = 0; r < scen[i].n_nodes; r++) {
-            const uint32_t g = scen[i].nodes[r];
-            if (g >= N || rank[g] != -1) return fail(ctx, SIMON_ERR_INVALID, "scenario %u: bad node list", i);
-            rank[g] = (int32_t)r;
-        }
-        std::copy(scen[i].nodes, scen[i].nodes + scen[i].n_nodes, B.h_order.begin() + (size_t)i * N1);
-        max_active = std::max(max_active, scen[i].n_nodes);
-    }
+    int rc = scenario_lists(ctx, scen, n, "scenario", max_active);
+    if (rc) return rc;
     // ---- pooled state of all scenarios: one allocation and one memset (or broadcast) per column; Open-Local: every scenario
     // starts from the uploaded VG requested values and device masks ----
-    int rc = alloc_pool(ctx, B, n, false);
+    rc = alloc_pool(ctx, B, n, false);
     if (rc) return rc;
     CU(cudaMemcpyAsync(B.order.p, B.h_order.data(), 4ull * n * N1, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(B.rank_of.p, B.h_rank.data(), 4ull * n * N1, cudaMemcpyHostToDevice, st));
@@ -1220,6 +1278,220 @@ int simon_scenarios_storage_download(simon_ctx *ctx, uint32_t scenario, int64_t 
     const uint32_t N = ctx->N;
     if (vg_requested && ctx->V && N) CU(cudaMemcpy(vg_requested, B.vg_req.p + scenario * B.vn, 8ull * ctx->V * N, cudaMemcpyDeviceToHost));
     if (dev_alloc && N) CU(cudaMemcpy(dev_alloc, B.dev_alloc.p + scenario * B.nodes, 4ull * N, cudaMemcpyDeviceToHost));
+    return SIMON_OK;
+}
+
+// ---- drain batches --------------------------------------------------------------------------------------------------------------
+// Device bytes one scenario of a drain batch holds in the batch pool: the columns size_pool sizes per scenario (pod_outputs false).
+// Not counted, because they depend on the drains: the per-evicted-pod outputs (node, GPU slots, score: 16 B per evicted pod of the
+// batch), the failure records (100 B x the batch's largest evicted-pod list per scenario) and, when the large-cluster variant runs,
+// its per-node arrays in global memory (the node arrays of one cluster per scenario).  Engine.drain_run keeps the margin for them by
+// sizing a batch to a fraction of the free memory.
+static uint64_t drain_scenario_bytes(const simon_ctx *ctx) {
+    const uint64_t nodes = std::max(1u, ctx->N), scal = (uint64_t)(ctx->K ? ctx->K : 1) * nodes, cntw = std::max<uint64_t>(1, ctx->cnt_words);
+    const uint64_t nct = std::max(1u, ctx->n_counters), ncl = std::max(1u, ctx->n_classes);
+    const uint64_t tabw = (uint64_t)SK_MAX_SOFT * ctx->max_dom, regw = (uint64_t)SK_MAX_HARD * ctx->max_dom;
+    uint64_t b = 8 * nodes * 5 + 8 * scal + 8 * nodes * SIMON_MAX_GPU_DEV + 4 * nodes + 4 * cntw + 4 * nct;   // requests .. counter totals
+    b += 4 * tabw * 2 + 4 * SK_MAX_SOFT + regw;                                                                 // tp, fcount, size, hard_reg
+    b += 8 * ncl * SK_CSUM_W + nodes * ncl + 8 * nodes * ncl;                                                   // csum, fbits, ocache
+    b += 4 + 8 + 16 + sizeof(SkScenario) + 4 * nodes * 2 + sizeof(simon_scenario_result);                       // out_node .. results
+    if (ctx->have_storage) b += sizeof(simon_scenario_local_result) + 8 * std::max<uint64_t>(1, (uint64_t)ctx->V * ctx->N) + 4 * nodes;
+    if (ctx->have_devices) b += 4 * nodes;
+    return b;
+}
+
+extern "C" int simon_drain_budget(simon_ctx *ctx, uint64_t *scenario_bytes, uint64_t *free_bytes) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_drain_budget before uploads");
+    CU(cudaSetDevice(ctx->device));
+    const uint64_t per = drain_scenario_bytes(ctx);
+    if (scenario_bytes) *scenario_bytes = per;
+    if (free_bytes) {
+        size_t fr = 0, tot = 0;
+        CU(cudaMemGetInfo(&fr, &tot));
+        uint64_t cached = 0;          // blocks the stream-ordered pool keeps for reuse (pool_alloc) are free to this ctx as well
+        cudaMemPool_t pool;
+        if (cudaDeviceGetDefaultMemPool(&pool, ctx->device) == cudaSuccess) {
+            uint64_t reserved = 0, used = 0;
+            if (cudaMemPoolGetAttribute(pool, cudaMemPoolAttrReservedMemCurrent, &reserved) == cudaSuccess &&
+                cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemCurrent, &used) == cudaSuccess && reserved > used)
+                cached = reserved - used;
+        }
+        cudaGetLastError();
+        *free_bytes = (uint64_t)fr + cached + (uint64_t)ctx->batch.n * per;     // the batch pool's columns are reused in place
+    }
+    return SIMON_OK;
+}
+
+extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario *remain, uint32_t n, simon_drain_result *out) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_drain_run before uploads");
+    if ((ctx->n_pods && !placed) || (n && (!remain || !out))) return fail(ctx, SIMON_ERR_INVALID, "simon_drain_run: NULL argument");
+    const uint32_t N = ctx->N, N1 = std::max(1u, N), P = ctx->n_pods;
+    // ---- refusals before any device work: the live placement as a resume prefix checks it, then the node lists ----
+    int rc = check_prefix(ctx, placed, P);
+    if (rc) return rc;
+    for (uint32_t i = 0; i < n; i++)
+        if (remain[i].n_nodes == 0) return fail(ctx, SIMON_ERR_INVALID, "drain %u leaves no node", i);
+    uint32_t max_active = 0;
+    rc = scenario_lists(ctx, remain, n, "drain", max_active);
+    if (rc) return rc;
+    CU(cudaSetDevice(ctx->device));
+    ctx->last_launch = simon_launch_info{};
+    ctx->dr_n = 0;
+    ScenPool &S = ctx->single, &B = ctx->batch;
+    B.n_storage = 0;                    // the batch pool's Open-Local slices are no longer a storage batch's
+    if (n == 0) return SIMON_OK;
+    cudaStream_t st = ctx->stream;
+    // ---- per scenario, from the pods each node holds (one CSR): the pods of its removed nodes in pod order, as (scenario, pod)
+    // pairs for the un-import, and split into vanished (DaemonSet pods of a removed node), blocked (bound by spec.nodeName or with
+    // Open-Local volumes) and evicted pods ----
+    std::vector<uint32_t> node_off(N1 + 1, 0u), node_pods;
+    for (uint32_t q = 0; q < P; q++)
+        if (placed[q] >= 0) node_off[placed[q] + 1]++;
+    for (uint32_t g = 0; g < N1; g++) node_off[g + 1] += node_off[g];
+    node_pods.resize(node_off[N1]);
+    {
+        std::vector<uint32_t> cur(node_off.begin(), node_off.end() - 1);
+        for (uint32_t q = 0; q < P; q++)
+            if (placed[q] >= 0) node_pods[cur[placed[q]]++] = q;
+    }
+    ctx->dr_off.assign(1, 0u); ctx->dr_pods.clear(); ctx->dr_boff.assign(1, 0u); ctx->dr_blocked.clear();
+    std::vector<uint2> pairs;
+    std::vector<uint32_t> n_vanished(n, 0u), rm;
+    ctx->dr_max = 0;
+    for (uint32_t i = 0; i < n; i++) {
+        const int32_t *rank = B.h_rank.data() + (size_t)i * N1;
+        rm.clear();
+        for (uint32_t g = 0; g < N; g++)
+            if (rank[g] < 0) rm.insert(rm.end(), node_pods.begin() + node_off[g], node_pods.begin() + node_off[g + 1]);
+        std::sort(rm.begin(), rm.end());
+        for (uint32_t q : rm) {
+            pairs.push_back(make_uint2(i, q));
+            const int32_t gd = ctx->h_guard[q];
+            if (gd >= 0 && rank[gd] < 0) n_vanished[i]++;
+            else if (ctx->h_fixed[q] >= 0 || (ctx->have_storage && ctx->h_class_local[ctx->h_class[q]])) ctx->dr_blocked.push_back(q);
+            else ctx->dr_pods.push_back(q);
+        }
+        ctx->dr_off.push_back((uint32_t)ctx->dr_pods.size());
+        ctx->dr_boff.push_back((uint32_t)ctx->dr_blocked.size());
+        ctx->dr_max = std::max(ctx->dr_max, ctx->dr_off[i + 1] - ctx->dr_off[i]);
+    }
+    const size_t n_ev = ctx->dr_pods.size();
+    // ---- geometry of the drain variant, the batch pool and the outputs (allocations before the timed work) ----
+    uint32_t CS, TPB, NPT;
+    size_t smem;
+    rc = choose_geometry(ctx, max_active, CS, TPB, NPT, smem, n, true);
+    if (rc) return rc;
+    rc = size_pool(ctx, B, n, false, false);
+    if (rc) return rc;
+    CU(ctx->d_dr_pods.upload(ctx->dr_pods.data(), n_ev, st));
+    CU(ctx->d_dr_off.upload(ctx->dr_off.data(), n + 1, st));
+    CU(ctx->d_dr_pairs.upload(pairs.data(), pairs.size(), st));
+    CU(ctx->d_dr_node.alloc(n_ev)); CU(ctx->d_dr_gpu.alloc(n_ev));
+    if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(ctx->d_dr_score.alloc(n_ev));
+    CU(ctx->d_dr_fail_counts.alloc((size_t)n * ctx->dr_max * SIMON_N_FAIL_CODES)); CU(ctx->d_dr_fail_pod.alloc((size_t)n * ctx->dr_max));
+    CU(cudaMemcpyAsync(B.order.p, B.h_order.data(), 4ull * n * N1, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(B.rank_of.p, B.h_rank.data(), 4ull * n * N1, cudaMemcpyHostToDevice, st));
+    std::vector<SkScenario> h(n);
+    for (uint32_t i = 0; i < n; i++) {
+        h[i] = fill_scen(B, i, remain[i].n_nodes, remain[i].n_nodes == N && std::is_sorted(remain[i].nodes, remain[i].nodes + N));
+        h[i].out_node = ctx->d_dr_node.p; h[i].out_gpu = ctx->d_dr_gpu.p;
+        h[i].out_score = (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) ? ctx->d_dr_score.p : nullptr;
+        h[i].fail_counts = ctx->d_dr_fail_counts.p + (size_t)i * ctx->dr_max * SIMON_N_FAIL_CODES;
+        h[i].fail_pod = ctx->d_dr_fail_pod.p + (size_t)i * ctx->dr_max;
+    }
+    CU(B.scen.upload(h.data(), n, st));
+    // ---- setup: the live state in the single-scenario pool (the resume's rebuild, its failure records cleared as the resume clears
+    // them), copied into every slot, minus what each scenario's removed nodes' pods contributed to the counters.  Of the batch pool
+    // only what the copies do not overwrite is cleared: the per-class summaries and own-score caches, the counters and failure
+    // records ----
+    CU(cudaEventRecord(ctx->ev0, st));
+    SkParams Ps;
+    fill_params(ctx, S, Ps);
+    rc = clear_pool(ctx, S);
+    if (rc) return rc;
+    CU(cudaMemsetAsync(S.fail_counts.p, 0, 4ull * ctx->max_fail * SIMON_N_FAIL_CODES, st));
+    CU(cudaMemsetAsync(S.counters.p, 0, 8, st));
+    rc = rebuild_prefix(ctx, Ps, placed, P);
+    if (rc) return rc;
+    CU(cudaMemsetAsync(B.csum.p, 0, 8 * n * B.ncl * SK_CSUM_W, st));
+    CU(cudaMemsetAsync(B.ocache.p, 0, 8 * n * B.nodes * B.ncl, st));
+    CU(cudaMemsetAsync(B.counters.p, 0, 8ull * n, st)); CU(cudaMemsetAsync(B.clk.p, 0, 16ull * n, st));
+    CU(cudaMemsetAsync(ctx->d_dr_fail_counts.p, 0, 4ull * n * ctx->dr_max * SIMON_N_FAIL_CODES, st));
+    CU(bcast(ctx, S.req_mcpu.p, S.nodes, n, B.req_mcpu.p)); CU(bcast(ctx, S.req_mem.p, S.nodes, n, B.req_mem.p));
+    CU(bcast(ctx, S.req_eph.p, S.nodes, n, B.req_eph.p)); CU(bcast(ctx, S.nz_mcpu.p, S.nodes, n, B.nz_mcpu.p));
+    CU(bcast(ctx, S.nz_mem.p, S.nodes, n, B.nz_mem.p)); CU(bcast(ctx, S.num_pods.p, S.nodes, n, B.num_pods.p));
+    CU(bcast(ctx, S.req_scalar.p, S.scal, n, B.req_scalar.p));
+    CU(bcast(ctx, S.gpu_used.p, S.nodes * SIMON_MAX_GPU_DEV, n, B.gpu_used.p));
+    CU(bcast(ctx, S.cnt.p, S.cntw, n, B.cnt.p)); CU(bcast(ctx, S.cnt_total.p, S.nct, n, B.cnt_total.p));
+    ctx->launches += 10;
+    SkParams Pb;
+    fill_params(ctx, B, Pb);
+    if (!pairs.empty()) {
+        const uint32_t grid = (uint32_t)std::min<size_t>((pairs.size() + 255) / 256, (size_t)ctx->sms * 4);
+        simon_drain_unimport<<<grid, 256, 0, st>>>(Pb, ctx->d_prefix.p, ctx->d_dr_pairs.p, (uint32_t)pairs.size());
+        CU(cudaGetLastError());
+        ctx->launches++;
+    }
+    CU(cudaEventRecord(ctx->evm, st));
+    // ---- placement of every scenario's evicted pods ----
+    Pb.drain_pods = ctx->d_dr_pods.p; Pb.drain_off = ctx->d_dr_off.p;
+    Pb.first = 0; Pb.count = 0; Pb.max_fail = ctx->dr_max; Pb.npt = NPT;
+    rc = launch(ctx, Pb, n, CS, TPB, smem, false, true);
+    if (rc) return rc;
+    CU(cudaEventRecord(ctx->ev1, st));
+    simon_scen_reduce<<<n, 256, 0, st>>>(B.scen.p, ctx->d_alloc_mcpu.p, ctx->d_alloc_mem.p, B.results.p);
+    CU(cudaGetLastError());
+    std::vector<simon_scenario_result> res(n);
+    CU(cudaMemcpyAsync(res.data(), B.results.p, sizeof(simon_scenario_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    CU(cudaEventElapsedTime(&ctx->dr_setup_ms, ctx->ev0, ctx->evm));
+    CU(cudaEventElapsedTime(&ctx->dr_place_ms, ctx->evm, ctx->ev1));
+    CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    ctx->dr_nfail.resize(n);
+    for (uint32_t i = 0; i < n; i++) {
+        simon_drain_result &o = out[i];
+        o.n_evicted = ctx->dr_off[i + 1] - ctx->dr_off[i];
+        o.n_placed = res[i].n_scheduled; o.n_unscheduled = res[i].n_unscheduled;
+        o.n_blocked = ctx->dr_boff[i + 1] - ctx->dr_boff[i];
+        o.n_vanished = n_vanished[i]; o.reserved = 0;
+        o.req_mcpu = res[i].req_mcpu; o.alloc_mcpu = res[i].alloc_mcpu; o.req_mem = res[i].req_mem; o.alloc_mem = res[i].alloc_mem;
+        ctx->dr_nfail[i] = res[i].n_unscheduled;
+    }
+    ctx->dr_n = n;
+    return SIMON_OK;
+}
+
+extern "C" int simon_drain_times(simon_ctx *ctx, float *setup_ms, float *place_ms) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (setup_ms) *setup_ms = ctx->dr_setup_ms;
+    if (place_ms) *place_ms = ctx->dr_place_ms;
+    return SIMON_OK;
+}
+
+extern "C" int simon_drain_download(simon_ctx *ctx, uint32_t scenario, uint32_t *evicted_pod, int32_t *node, uint32_t *gpu_slots,
+                                    int64_t *score, uint32_t *blocked_pod, uint32_t *fail_counts, uint32_t *fail_pod) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->dr_n) return fail(ctx, SIMON_ERR_STATE, "no simon_drain_run batch since the last upload");
+    if (scenario >= ctx->dr_n) return fail(ctx, SIMON_ERR_INVALID, "drain %u of a batch of %u", scenario, ctx->dr_n);
+    CU(cudaSetDevice(ctx->device));
+    const uint32_t b = ctx->dr_off[scenario], ne = ctx->dr_off[scenario + 1] - b;
+    const uint32_t bb = ctx->dr_boff[scenario], nb = ctx->dr_boff[scenario + 1] - bb;
+    const uint32_t nf = std::min(ctx->dr_nfail[scenario], ctx->dr_max);
+    if (evicted_pod) std::copy(ctx->dr_pods.begin() + b, ctx->dr_pods.begin() + b + ne, evicted_pod);
+    if (blocked_pod) std::copy(ctx->dr_blocked.begin() + bb, ctx->dr_blocked.begin() + bb + nb, blocked_pod);
+    if (node && ne) CU(cudaMemcpy(node, ctx->d_dr_node.p + b, 4ull * ne, cudaMemcpyDeviceToHost));
+    if (gpu_slots && ne) CU(cudaMemcpy(gpu_slots, ctx->d_dr_gpu.p + b, 4ull * ne, cudaMemcpyDeviceToHost));
+    if (score && ne) {
+        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(cudaMemcpy(score, ctx->d_dr_score.p + b, 8ull * ne, cudaMemcpyDeviceToHost));
+        else memset(score, 0, 8ull * ne);
+    }
+    if (fail_counts && nf)
+        CU(cudaMemcpy(fail_counts, ctx->d_dr_fail_counts.p + (size_t)scenario * ctx->dr_max * SIMON_N_FAIL_CODES,
+                      4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
+    if (fail_pod && nf) CU(cudaMemcpy(fail_pod, ctx->d_dr_fail_pod.p + (size_t)scenario * ctx->dr_max, 4ull * nf, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 

@@ -128,6 +128,9 @@ struct SkParams {
     // vg_req, local_raw and dev_alloc hold one slice per cluster of the launch, these many elements apart (a single-scenario
     // launch is one cluster: it reads slice 0)
     uint64_t vg_req_stride, node_stride;
+    // drain batches (simon_drain_kernel_*): scenario s places pods drain_pods[drain_off[s] .. drain_off[s + 1]) (pod indices, in
+    // pod-list order); the per-pod outputs of SkScenario are indexed by the position in drain_pods, not by the pod
+    const uint32_t *drain_pods, *drain_off;
 };
 
 // the index of this thread-block cluster in the (1-D) grid: the scenario of the launch (blockIdx.x / cluster size)

@@ -55,6 +55,12 @@ class SimonScenarioResult(C.Structure):
                 ("elapsed_ms", C.c_float), ("reserved", C.c_uint32)]
 
 
+class SimonDrainResult(C.Structure):
+    _fields_ = [("n_evicted", C.c_uint32), ("n_placed", C.c_uint32), ("n_unscheduled", C.c_uint32), ("n_blocked", C.c_uint32),
+                ("n_vanished", C.c_uint32), ("reserved", C.c_uint32),
+                ("req_mcpu", C.c_int64), ("alloc_mcpu", C.c_int64), ("req_mem", C.c_int64), ("alloc_mem", C.c_int64)]
+
+
 class SimonScenarioLocalResult(C.Structure):
     _fields_ = [("vg_requested", C.c_int64), ("vg_capacity", C.c_int64), ("reserved", C.c_uint64)]
 

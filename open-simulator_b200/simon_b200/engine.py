@@ -26,7 +26,8 @@ EXPORTS = ["simon_gpu_version", "simon_ctx_create", "simon_ctx_destroy", "simon_
            "simon_host_simulate", "simon_host_free", "simon_host_quantity_probe", "simon_host_plan_fit_error", "simon_host_capacity_search",
            "simon_storage_upload", "simon_storage_state_download", "simon_devices_upload", "simon_devices_state_download",
            "simon_scenarios_run_local", "simon_scenarios_storage_download", "simon_moves_set_scope", "simon_moves_gpu_slots_download",
-           "simon_schedule_resume", "simon_last_launch"]
+           "simon_schedule_resume", "simon_last_launch", "simon_drain_run", "simon_drain_download", "simon_drain_times",
+           "simon_drain_budget"]
 
 
 class EngineUnavailable(RuntimeError):
@@ -107,6 +108,14 @@ def lib():
                                             C.c_uint32, C.c_void_p]
         L.simon_last_launch.restype = C.c_int
         L.simon_last_launch.argtypes = [C.c_void_p, C.c_void_p]
+        L.simon_drain_run.restype = C.c_int
+        L.simon_drain_run.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
+        L.simon_drain_download.restype = C.c_int
+        L.simon_drain_download.argtypes = [C.c_void_p, C.c_uint32] + [C.c_void_p] * 7
+        L.simon_drain_times.restype = C.c_int
+        L.simon_drain_times.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float)]
+        L.simon_drain_budget.restype = C.c_int
+        L.simon_drain_budget.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     except AttributeError:
         if not os.environ.get("SIMON_GPU_LIB"):       # an experiment library may lack the newer entry points; the shipped one may not
             raise
@@ -387,3 +396,68 @@ class Engine:
         dev = np.zeros(max(N, 1), np.uint32) if self.c.storage.devices else None
         self._check(lib().simon_scenarios_storage_download(self.h, i, vg.ctypes.data, None if dev is None else dev.ctypes.data))
         return vg[:V * N].reshape(V, N), None if dev is None else dev[:N]
+
+    # ---- node drains (simon_drain_run) ----
+    # share of the memory simon_drain_budget reports that one batch's pooled state may take: the rest is the margin for what the
+    # per-scenario bytes do not count (per-evicted-pod outputs, failure records, the large-cluster variant's node arrays)
+    DRAIN_MEM_FRACTION = 0.5
+
+    def drain_budget(self):
+        """(device bytes of one drain scenario's pooled state, bytes a batch may use now)."""
+        per, free = C.c_uint64(0), C.c_uint64(0)
+        self._check(lib().simon_drain_budget(self.h, C.byref(per), C.byref(free)))
+        return int(per.value), int(free.value)
+
+    def drain_run(self, placed, remain_lists: List[np.ndarray], detail: bool = True, chunk: Optional[int] = None):
+        """Drains on the live state `placed` (out_node of a full placement of the pod list): each entry of remain_lists lists the
+        nodes that remain, in their nodeTree.list() order.  The list runs in batches (chunks) sized so that one batch's pooled state
+        fits the device: chunk scenarios of simon_drain_budget's per-scenario bytes in DRAIN_MEM_FRACTION of what it reports free
+        (chunk: an explicit batch size).  Returns one dict per drain: n_evicted, n_placed, n_unscheduled, n_blocked, n_vanished and
+        the sums req_mcpu / alloc_mcpu / req_mem / alloc_mem over the remaining nodes; with detail also evicted (pod indices in
+        pod order), node (per evicted pod, -1 unschedulable), gpu_slots, score, blocked, fail_counts [n_unscheduled][24] and
+        fail_pod.  self.last_drain: chunks, scenario_bytes, setup_ms / place_ms (device time summed over the batches)."""
+        L = lib()
+        pl = np.ascontiguousarray(placed, dtype=np.int32)
+        n = len(remain_lists)
+        per, free = self.drain_budget()
+        if chunk is None:
+            chunk = max(1, int(free * self.DRAIN_MEM_FRACTION) // max(per, 1))
+        out = []
+        info = dict(chunks=0, scenario_bytes=per, chunk=chunk, setup_ms=0.0, place_ms=0.0, launches=[])
+        for b in range(0, n, chunk):
+            part = remain_lists[b:b + chunk]
+            m = len(part)
+            arr = (abi.SimonScenario * m)()
+            keep = []
+            for i, nodes in enumerate(part):
+                a = np.ascontiguousarray(nodes, dtype=np.uint32)
+                keep.append(a)
+                arr[i].n_nodes = len(a)
+                arr[i].nodes = a.ctypes.data if len(a) else None
+            res = (abi.SimonDrainResult * m)()
+            self._check(L.simon_drain_run(self.h, pl.ctypes.data, arr, m, res))
+            su, pm = C.c_float(0), C.c_float(0)
+            self._check(L.simon_drain_times(self.h, C.byref(su), C.byref(pm)))
+            info["chunks"] += 1
+            info["setup_ms"] += float(su.value)
+            info["place_ms"] += float(pm.value)
+            info["launches"].append(self.last_launch())
+            for i, r in enumerate(res):
+                d = dict(n_evicted=r.n_evicted, n_placed=r.n_placed, n_unscheduled=r.n_unscheduled, n_blocked=r.n_blocked,
+                         n_vanished=r.n_vanished, req_mcpu=r.req_mcpu, alloc_mcpu=r.alloc_mcpu, req_mem=r.req_mem, alloc_mem=r.alloc_mem)
+                if detail:
+                    ne, nb, nf = r.n_evicted, r.n_blocked, r.n_unscheduled
+                    ev = np.zeros(max(ne, 1), np.uint32)
+                    node = np.zeros(max(ne, 1), np.int32)
+                    slots = np.zeros(max(ne, 1), np.uint32)
+                    score = np.zeros(max(ne, 1), np.int64)
+                    blk = np.zeros(max(nb, 1), np.uint32)
+                    fc = np.zeros((max(nf, 1), abi.N_FAIL_CODES), np.uint32)
+                    fp = np.zeros(max(nf, 1), np.uint32)
+                    self._check(L.simon_drain_download(self.h, i, ev.ctypes.data, node.ctypes.data, slots.ctypes.data, score.ctypes.data,
+                                                       blk.ctypes.data, fc.ctypes.data, fp.ctypes.data))
+                    d.update(evicted=ev[:ne], node=node[:ne], gpu_slots=slots[:ne], score=score[:ne], blocked=blk[:nb],
+                             fail_counts=fc[:nf], fail_pod=fp[:nf])
+                out.append(d)
+        self.last_drain = info
+        return out

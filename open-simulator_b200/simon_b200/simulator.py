@@ -528,6 +528,44 @@ class Simulator:
         return res
 
 
+    # ---- node drains and scale-down (this project's extension: the reference names the use case, README.md:16, without code) ----
+    def DrainNodes(self, drains: List[List[str]]):
+        """Each entry names nodes to remove together; per entry a scaledown.DrainResult on the session's live state (the last
+        call's placements and compiled cluster, on its device context: no new compile)."""
+        from . import scaledown
+        eng, compiled = self._live()
+        order = scaledown.NodeOrder(compiled)
+        removed = []
+        for names in drains:
+            idx = [compiled.node_index(nm) for nm in names]
+            bad = [nm for nm, g in zip(names, idx) if g < 0]
+            if bad:
+                raise ValueError(f"DrainNodes: no node named {bad[0]!r}")
+            removed.append(idx)
+        remain = [order.remaining(r) for r in removed]
+        raw = eng.drain_run(self.placements, remain, detail=True)
+        return scaledown.drain_results(compiled, self.placements, removed, remain, raw)
+
+    def PlanScaleDown(self, candidates: Optional[List[str]] = None, max_remove: Optional[int] = None):
+        """scaledown.ScaleDownPlan on the session's live state: candidates (node names; all nodes by default) drained alone, the
+        drainable ones ordered by utilisation, and the longest prefix of that order whose every prefix drains within the caps."""
+        from . import scaledown
+        eng, compiled = self._live()
+        cand = None
+        if candidates is not None:
+            cand = [compiled.node_index(nm) for nm in candidates]
+            if any(g < 0 for g in cand):
+                raise ValueError("PlanScaleDown: a candidate names no node of the cluster")
+        return scaledown.plan_scale_down(compiled, self.placements, lambda rl: eng.drain_run(self.placements, rl, detail=False),
+                                         candidates=cand, max_remove=max_remove)
+
+    def _live(self):
+        self._check_open()
+        if self.engine is None or self.compiled is None:
+            raise RuntimeError("drains need a running cluster: call RunCluster first")
+        return self.engine, self.compiled
+
+
 class _ResumedDump:
     """Engine.dump_pod over a resumed run: the pods before the dumped one are rebuilt at the nodes `placed` gives them."""
 
