@@ -52,6 +52,7 @@ extern "C" {
 
 #define SIMON_MAX_SCALARS 8     /* extended/scalar resource columns (K) */
 #define SIMON_MAX_GPU_DEV 8     /* GPU-share devices per node */
+#define SIMON_MAX_GPU_SLOTS 64  /* alibabacloud.com/gpu-count of a GPU-share pod (Reserve's slot list); more is refused */
 #define SIMON_MAX_LABEL_WORDS 16
 #define SIMON_MAX_TAINT_WORDS 4
 #define SIMON_MAX_TOPOS 8

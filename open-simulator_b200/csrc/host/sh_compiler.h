@@ -293,6 +293,10 @@ inline ClassInfo parse_class(int cid, PodTemplate *tmpl) {
     }
     if (ann.has(GPU_INDEX_NAME) && ci.gpu_mem > 0)
         throw CompileError("pods with a preset alibabacloud.com/gpu-index annotation are not supported");
+    // Reserve records at most SIMON_MAX_GPU_SLOTS slots per pod (the kernels' and the oracle's slot lists): refused, never narrowed
+    if (ci.gpu_mem > 0 && ci.gpu_count > SIMON_MAX_GPU_SLOTS)
+        throw CompileError("pod " + ci.ns + "/" + name_of(pod) + " requests " + std::to_string(ci.gpu_count) +
+                           " GPU-share slots (alibabacloud.com/gpu-count): at most 64 are supported");
     // Open-Local (pkg/simulator/plugin/open-local.go:51-138) is out of scope (SURVEY 8a row 26): pods that REQUEST local storage
     // would be filtered / scored / reserved by it, so they are refused instead of being placed as if it did not exist
     if (const J *st = ann.get(ANNO_POD_LOCAL_STORAGE)) {

@@ -946,7 +946,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
             const int64_t *sc = cw + cw[SCW_OFF_SCALARS];
             for (uint32_t q = 0; q < ctx->K; q++) if (sc[q] != 0) bits |= SMC_HAS_SCALAR;
             const uint32_t n_filt = (uint32_t)(cw[SCW_N_IPA_AFF] + cw[SCW_N_IPA_ANTI] + cw[SCW_N_IPA_EXIST]);
-            bits |= ((uint32_t)cw[SCW_N_PORTS] & 31u) << 10;
+            bits |= ((uint32_t)cw[SCW_N_PORTS] & 31u) << 10 | ((uint32_t)cw[SCW_N_PORTS] & 32u) << 24;     // SMC_NPORTS
             bits |= (n_filt & 63u) << 15;
             const int64_t *et = cw + cw[SCW_OFF_ENT];
             const uint32_t E = (uint32_t)cw[SCW_N_ENT];

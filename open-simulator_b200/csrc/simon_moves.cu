@@ -38,8 +38,8 @@ struct __align__(32) SmvClass {
     int64_t score_mcpu, score_mem, nz_mcpu, nz_mem;      // sector 0: scoring
     int64_t req_mcpu, req_mem, req_eph;                  // sector 1: Fit
     uint32_t sig;                                        //           static signature
-    uint32_t bits;                                       //           flags:8 | not movable:1 | has scalar request:1 | n_ports:5 | n_filter entries (aff+anti+exist):6 | own increments:1
-                                                         //           | scope bits the class needs:2 | never movable:1 | n_hard:4
+    uint32_t bits;                                       //           flags:8 | not movable:1 | has scalar request:1 | n_ports, low 5 bits | n_filter entries (aff+anti+exist):6 | own increments:1
+                                                         //           | scope bits the class needs:2 | never movable:1 | n_hard:4 | n_ports, bit 5 (32 ports: SK_MAX_ENT)
 };
 static_assert(sizeof(SmvClass) == 64, "SmvClass layout");
 // per-pod record built by the pack kernel of every launch: everything a move needs to know about its pod in ONE 16-byte load,
@@ -50,7 +50,7 @@ struct __align__(16) SmvPod {
 };
 #define SMC_NOT_MOVABLE (1u << 8)
 #define SMC_HAS_SCALAR (1u << 9)
-#define SMC_NPORTS(b) (((b) >> 10) & 31u)
+#define SMC_NPORTS(b) ((((b) >> 10) & 31u) | (((b) >> 24) & 32u))   // bits 10..14 and 29: 0..63 (a class has at most SK_MAX_ENT = 32)
 #define SMC_NFILT(b) (((b) >> 15) & 63u)
 #define SMC_OWN_INC (1u << 21)
 #define SMC_NEED(b) (((b) >> 22) & 3u)   // SIMON_MOVES_SCOPE_* bits that admit a not-movable class (GPU share, hard spread)

@@ -39,6 +39,7 @@ from .workloads import PodRec, PodTemplate
 # ---- format constants: keep in sync with include/simon_gpu.h ----
 MAX_SCALARS = 8
 MAX_GPU_DEV = 8
+MAX_GPU_SLOTS = 64      # alibabacloud.com/gpu-count of a GPU-share pod
 MAX_LABEL_WORDS = 16
 MAX_TAINT_WORDS = 4
 MAX_TOPOS = 8
@@ -331,6 +332,10 @@ def _parse_class(cid: int, tmpl: PodTemplate, open_local: bool = False) -> Class
             pass
     if GPU_INDEX_NAME in ann and ci.gpu_mem > 0:
         raise CompileError("pods with a preset alibabacloud.com/gpu-index annotation are not supported")
+    # Reserve records at most MAX_GPU_SLOTS slots per pod (the kernels' and the oracle's slot lists): refused, never narrowed
+    if ci.gpu_mem > 0 and ci.gpu_count > MAX_GPU_SLOTS:
+        raise CompileError(f"pod {ci.namespace}/{O.name_of(pod)} requests {ci.gpu_count} GPU-share slots "
+                           f"(alibabacloud.com/gpu-count): at most {MAX_GPU_SLOTS} are supported")
     # Open-Local (pkg/simulator/plugin/open-local.go:51-254) runs only when the caller opts in (open_local=True, storage.py):
     # otherwise pods that REQUEST local storage would be filtered / scored / bound by it, so they are refused instead of being
     # placed as if it did not exist.  A StatefulSet without open-local volumeClaimTemplates carries the annotation with an empty
