@@ -412,6 +412,50 @@ int simon_moves_set_scope(simon_ctx *ctx, uint32_t scope);
  * SIMON_ERR_STATE unless that run's scope had SIMON_MOVES_SCOPE_GPU_SHARE (a simon_moves_upload or _replay ends it). */
 int simon_moves_gpu_slots_download(simon_ctx *ctx, uint32_t first, uint32_t count, uint32_t *out_slots);
 
+/* ---- migration plans: a sequence of applied moves (this library's definition; the reference has no code for it) -----------
+ * simon_moves_plan builds an ordered list of migrations on the device, each move chosen on the state the earlier ones leave.
+ * Inputs: the live single-scenario state (after simon_schedule, simon_schedule_resume, simon_replay or a drain's rebuild), the
+ * move list of simon_moves_upload (move_base 0), the current move scope, max_moves >= 1 and min_gain in [1, 200].
+ * The plan state starts as a copy of the live state; then, step by step:
+ *   1. every move is scored on the plan state exactly as simon_moves_run scores it on a live state equal to it;
+ *   2. skipped: moves of pods that already moved in this plan (each pod moves at most once) and moves of excluded pods;
+ *   3. the best remaining feasible move by (gain descending, move index ascending) is taken; if there is none, or its gain is
+ *      below min_gain, the plan stops with SIMON_PLAN_STOP_NO_MOVE;
+ *   4. it is applied: the pod p is taken off its node a (requests, non-zero requests, pod count, scalars, its class's counter
+ *      increments at a's domains, eligibility-conditional entries as the import counts them) and put on the target b (the same
+ *      additions at b);
+ *   5. a GPU-share pod releases its device memory on a as its slot word states it, then Reserve (AllocateGpuId) runs on b; the
+ *      slots equal the ones the scoring reported for the move.  Pre-bound GPU-share pods hold no device memory: they release 0;
+ *   6. placement[p] = b and the step is recorded; the plan stops with SIMON_PLAN_STOP_MAX_MOVES after max_moves steps.
+ * Excluded pods: placed pods of a GPU-share class that is neither pinned nor Open-Local whose live slot word has a saturated
+ * nibble (15: the word saturates there, so the pod's slots on that device, and the memory to release, are not known exactly).  They are counted in n_excluded, under every scope.
+ * The live state is not changed: simon_state_download, later simon_moves_run calls, drains and the scenario and drain downloads
+ * see what they saw before.  After a plan, simon_moves_gpu_slots_download answers SIMON_ERR_STATE.
+ * Refused with SIMON_ERR_INVALID: max_moves 0, min_gain outside [1, 200], a move list uploaded with move_base != 0; with
+ * SIMON_ERR_STATE: no move list, no placement since the last pod upload (or simon_state_reset).  An inconsistency found while
+ * applying a step (recomputed GPU slots differ from the scored ones, a count would go negative) stops the plan with
+ * SIMON_ERR_CUDA and a message.  out_steps has room for max_moves steps. */
+#define SIMON_PLAN_STOP_NO_MOVE 1u
+#define SIMON_PLAN_STOP_MAX_MOVES 2u
+typedef struct simon_plan_step {
+    uint32_t move, pod;      /* index in the move list, the pod */
+    int32_t from, to;        /* its node before the step, the target */
+    int32_t gain;
+    uint32_t gpu_slots;      /* device slots Reserve gave it on the target (format of simon_gpu_slots_download), 0 if none */
+} simon_plan_step;
+typedef struct simon_moves_plan_result {
+    uint32_t n_steps, stop_reason, n_excluded, reserved;
+    float kernel_ms;         /* device time of the setup and every step */
+    uint32_t reserved2;
+} simon_moves_plan_result;
+int simon_moves_plan(simon_ctx *ctx, uint32_t max_moves, int32_t min_gain, simon_plan_step *out_steps, simon_moves_plan_result *out);
+/* After a plan: every pod's node and GPU slot word (the layout of simon_results_download / simon_gpu_slots_download), and the plan
+ * state in the layouts of simon_state_download and simon_state_download_ext (any pointer may be NULL).  SIMON_ERR_STATE before any
+ * plan since the last upload. */
+int simon_moves_plan_download(simon_ctx *ctx, int32_t *placement, uint32_t *gpu_slots);
+int simon_moves_plan_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *req_mem, int64_t *req_eph, int64_t *nz_mcpu,
+                                    int64_t *nz_mem, int32_t *num_pods, int64_t *req_scalar, int64_t *gpu_used);
+
 /* ---- Open-Local LVM volumes (pkg/simulator/plugin/open-local.go:51-254; OL = vendor/github.com/alibaba/open-local/pkg) ------------
  * Optional, uploaded after simon_snapshot_upload + simon_pods_upload; without it no class requests local storage.
  * Node side: the annotation simon/node-local-storage (GetNodeCache, pkg/utils/utils.go:527-563): its VGs in annotation order.

@@ -235,7 +235,15 @@ struct simon_ctx {
     DevBuf<uint32_t> d_mv_hreg, d_mv_slots;
     DevBuf<int2> d_mv_hs;
     DevBuf<SmvGpu> d_mv_gpu;
-    uint32_t n_pin_fast = 0;            // pods marked for the pinned-run fast path (-4 in the device copy of pod_fixed_node)
+    // migration plans (simon_moves_plan): plan-owned copies of the dynamic columns of the single-scenario state, the steps and the
+    // control words.  have_live: the single-scenario state holds a placement (a schedule, resume, replay or drain rebuild since the
+    // last pod upload or reset); pl_valid: the plan columns hold the last plan's end state
+    bool have_live = false, pl_valid = false;
+    DevBuf<int64_t> d_pl_req_mcpu, d_pl_req_mem, d_pl_req_eph, d_pl_nz_mcpu, d_pl_nz_mem, d_pl_req_scalar, d_pl_gpu_used;
+    DevBuf<int32_t> d_pl_num_pods, d_pl_cnt, d_pl_cnt_total, d_pl_place;
+    DevBuf<uint32_t> d_pl_slots, d_pl_ctl;
+    DevBuf<simon_plan_step> d_pl_steps;
+    uint32_t n_pin_fast = 0;           // pods marked for the pinned-run fast path (-4 in the device copy of pod_fixed_node)
     std::vector<uint8_t> bypass;        // per pod: never reaches the scheduler in a single-scenario run (pre-bound or absent)
     // resumed runs (simon_schedule_resume): per pod the uploaded pod_fixed_node and guard (what its prefix entry is checked against),
     // the prefix on the device and its per-node grouping (counts, offsets, fill cursors, pod list)
@@ -798,6 +806,7 @@ int simon_snapshot_upload(simon_ctx *ctx, const simon_snapshot *s) {
     ctx->have_devices = false;
     ctx->batch.n_storage = 0;
     ctx->dr_n = 0;
+    ctx->have_live = ctx->pl_valid = false;
     return SIMON_OK;
 }
 
@@ -810,6 +819,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     ctx->have_devices = false;
     ctx->batch.n_storage = 0;
     ctx->dr_n = 0;
+    ctx->have_live = ctx->pl_valid = false;
     ctx->n_classes = p->n_classes; ctx->n_pods = p->n_pods; ctx->n_counters = p->n_counters;
     // validate classes; derive limits
     uint32_t max_words = SCW_HDR_WORDS, emax = 0;
@@ -1007,6 +1017,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
 int simon_state_reset(simon_ctx *ctx) {
     if (!ctx || !ctx->have_pods) return ctx ? fail(ctx, SIMON_ERR_STATE, "no pods uploaded") : SIMON_ERR_INVALID;
     CU(cudaSetDevice(ctx->device));
+    ctx->have_live = false;
     int rc = clear_pool(ctx, ctx->single);
     if (rc) return rc;
     CU(cudaStreamSynchronize(ctx->stream));
@@ -1052,6 +1063,7 @@ int simon_schedule(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_
     if (rc) return rc;
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    ctx->have_live = true;
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     uint32_t counters[2] = {0, 0};
     CU(cudaMemcpy(counters, S.counters.p, 8, cudaMemcpyDeviceToHost));
@@ -1103,6 +1115,7 @@ int simon_schedule_resume(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n
     CU(cudaEventRecord(ctx->ev1, st));
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    ctx->have_live = true;
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     uint32_t counters[2] = {0, 0};
     CU(cudaMemcpy(counters, S.counters.p, 8, cudaMemcpyDeviceToHost));
@@ -1141,6 +1154,7 @@ int simon_replay(simon_ctx *ctx, uint32_t steps, float *out_ms_total) {
     CU(cudaEventRecord(ctx->ev1, st));
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    if (steps) ctx->have_live = true;
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     if (out_ms_total) *out_ms_total = ctx->last_ms;
     return SIMON_OK;
@@ -1447,6 +1461,7 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
     CU(cudaMemcpyAsync(res.data(), B.results.p, sizeof(simon_scenario_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    ctx->have_live = true;
     CU(cudaEventElapsedTime(&ctx->dr_setup_ms, ctx->ev0, ctx->evm));
     CU(cudaEventElapsedTime(&ctx->dr_place_ms, ctx->evm, ctx->ev1));
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
@@ -1594,6 +1609,7 @@ int simon_storage_upload(simon_ctx *ctx, const simon_storage *sg) {
     ctx->V = V;
     ctx->h_class_local.assign(sg->class_local, sg->class_local + C);
     ctx->have_storage = true;
+    ctx->have_live = false;
     int rc = alloc_pool(ctx, ctx->single, 1, true);
     if (rc) return rc;
     CU(cudaStreamSynchronize(st));
@@ -1658,6 +1674,7 @@ int simon_devices_upload(simon_ctx *ctx, const simon_devices *dv) {
     std::vector<int64_t> hs(dv->hdd_size, dv->hdd_size + (C ? dv->hdd_off[C] : 0)); hs.push_back(0);
     CU(ctx->d_ssd_size.upload(ss.data(), ss.size(), st)); CU(ctx->d_hdd_size.upload(hs.data(), hs.size(), st));
     ctx->have_devices = true;
+    ctx->have_live = false;
     int rc = alloc_pool(ctx, ctx->single, 1, true);
     if (rc) return rc;
     CU(cudaStreamSynchronize(st));      // `ss` / `hs` leave scope
@@ -1857,6 +1874,153 @@ int simon_moves_replay(simon_ctx *ctx, uint32_t steps, float *out_ms_total) {
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "move kernel failed: %s", cudaGetErrorString(e));
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     if (out_ms_total) *out_ms_total = ctx->last_ms;
+    return SIMON_OK;
+}
+
+// ---- migration plans (simon_moves_plan) ---------------------------------------------------------------------------------------------
+// The plan columns start as device-to-device copies of the single-scenario state; the batch pool is not touched, so drain and scenario
+// downloads stay valid.  The move kernel's scratch (gains, codes, slots, packed records, histogram, best keys) is the one simon_moves_run
+// rebuilds on every call.  Steps are enqueued in chunks; the host reads the stop word between chunks, so at most one chunk's passes
+// after the stop score for nothing (a stopped plan's apply returns at once).
+int simon_moves_plan(simon_ctx *ctx, uint32_t max_moves, int32_t min_gain, simon_plan_step *out_steps, simon_moves_plan_result *out) {
+    if (!ctx || !out) return SIMON_ERR_INVALID;
+    if (max_moves == 0) return fail(ctx, SIMON_ERR_INVALID, "simon_moves_plan: max_moves must be at least 1");
+    if (!out_steps) return fail(ctx, SIMON_ERR_INVALID, "simon_moves_plan: out_steps is NULL");
+    if (min_gain < 1 || min_gain > 200) return fail(ctx, SIMON_ERR_INVALID, "simon_moves_plan: min_gain %d outside [1, 200]", min_gain);
+    if (!ctx->have_pods || !ctx->d_moves.p) return fail(ctx, SIMON_ERR_STATE, "simon_moves_plan before simon_moves_upload");
+    if (ctx->mv_base != 0) return fail(ctx, SIMON_ERR_INVALID, "simon_moves_plan: the move list was uploaded with move_base %u, not 0", ctx->mv_base);
+    if (!ctx->have_live) return fail(ctx, SIMON_ERR_STATE, "simon_moves_plan: no placement since the last pod upload or reset");
+    CU(cudaSetDevice(ctx->device));
+    int rc = moves_scope_refresh(ctx);
+    if (rc) return rc;
+    ctx->mv_ran = false;            // the per-move slots are overwritten
+    ctx->pl_valid = false;
+    cudaStream_t st = ctx->stream;
+    const ScenPool &S = ctx->single;
+    const uint32_t N = ctx->N, P = ctx->n_pods, n = ctx->mv_n, scope = ctx->mv_scope;
+    const bool scoped = ctx->mv_scoped, gpu = scoped && (scope & SIMON_MOVES_SCOPE_GPU_SHARE) && N;
+    const size_t nn = S.nodes, P1 = std::max(1u, P);
+    const uint32_t cap = (uint32_t)std::min<uint64_t>(max_moves, P1);
+    CU(ctx->d_pl_req_mcpu.alloc(nn)); CU(ctx->d_pl_req_mem.alloc(nn)); CU(ctx->d_pl_req_eph.alloc(nn));
+    CU(ctx->d_pl_nz_mcpu.alloc(nn)); CU(ctx->d_pl_nz_mem.alloc(nn)); CU(ctx->d_pl_num_pods.alloc(nn));
+    CU(ctx->d_pl_req_scalar.alloc(S.scal)); CU(ctx->d_pl_gpu_used.alloc(nn * SIMON_MAX_GPU_DEV));
+    CU(ctx->d_pl_cnt.alloc(S.cntw)); CU(ctx->d_pl_cnt_total.alloc(S.nct));
+    CU(ctx->d_pl_place.alloc(P1)); CU(ctx->d_pl_slots.alloc(P1)); CU(ctx->d_pl_ctl.alloc(4)); CU(ctx->d_pl_steps.alloc(cap));
+    if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && n) CU(ctx->d_mv_slots.alloc(n));
+    if (gpu) CU(ctx->d_mv_gpu.alloc(N));
+    CU(cudaEventRecord(ctx->ev0, st));
+    CU(cudaMemcpyAsync(ctx->d_pl_req_mcpu.p, S.req_mcpu.p, 8 * nn, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pl_req_mem.p, S.req_mem.p, 8 * nn, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pl_req_eph.p, S.req_eph.p, 8 * nn, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pl_nz_mcpu.p, S.nz_mcpu.p, 8 * nn, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pl_nz_mem.p, S.nz_mem.p, 8 * nn, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pl_num_pods.p, S.num_pods.p, 4 * nn, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pl_req_scalar.p, S.req_scalar.p, 8 * S.scal, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pl_gpu_used.p, S.gpu_used.p, 8 * nn * SIMON_MAX_GPU_DEV, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pl_cnt.p, S.cnt.p, 4 * S.cntw, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pl_cnt_total.p, S.cnt_total.p, 4 * S.nct, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pl_place.p, S.out_node.p, 4 * P1, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_pl_slots.p, S.out_gpu.p, 4 * P1, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemsetAsync(ctx->d_pl_ctl.p, 0, 16, st));
+    // ---- setup: the packed records of the plan state, once ----
+    if (gpu) {
+        simon_moves_pack_gpu<<<(N + 255) / 256, 256, 0, st>>>(N, ctx->d_gpu_count.p, ctx->d_gpu_dev_mem.p, ctx->d_gpu_total_mem.p,
+                                                               ctx->d_pl_gpu_used.p, ctx->d_mv_gpu.p);
+        ctx->launches++;
+    }
+    simon_moves_pack<<<std::max(std::max(1u, (N + 255) / 256), std::min(1184u, (P + 255) / 256)), 256, 0, st>>>(N, ctx->T, ctx->d_alloc_mcpu.p, ctx->d_alloc_mem.p, ctx->d_alloc_eph.p, ctx->d_alloc_pods.p,
+                                                                 ctx->d_topo_dom.p, ctx->d_pl_req_mcpu.p, ctx->d_pl_req_mem.p, ctx->d_pl_req_eph.p,
+                                                                 ctx->d_pl_nz_mcpu.p, ctx->d_pl_nz_mem.p, ctx->d_pl_num_pods.p, ctx->d_mv_nodes.p,
+                                                                 ctx->d_mv_best_pod.p, P, ctx->d_mv_best.p, ctx->d_mv_hist.p,
+                                                                 ctx->d_pod_class.p, ctx->d_pl_place.p, ctx->d_mv_classes.p, ctx->d_mv_pods.p);
+    simon_moves_plan_setup<<<std::max(1u, std::min(1184u, (P + 255) / 256)), 256, 0, st>>>(P, ctx->d_pl_slots.p, ctx->d_mv_pods.p, ctx->d_pl_ctl.p);
+    ctx->launches += 2;
+    CU(cudaGetLastError());
+    SmvParams M;
+    memset(&M, 0, sizeof(M));
+    M.N = N; M.K = ctx->K; M.WT = ctx->WT; M.T = ctx->T; M.n_pods = P; M.n_moves = n; M.use_scache = ctx->use_scache;
+    M.nodes = ctx->d_mv_nodes.p; M.alloc_scalar = ctx->d_alloc_scalar.p; M.req_scalar = ctx->d_pl_req_scalar.p; M.node_flags = ctx->d_node_flags.p;
+    M.label_bits = ctx->d_label_bits.p; M.taint_hard = ctx->d_taint_hard.p; M.topo_dom = ctx->d_topo_dom.p;
+    M.pods = ctx->d_mv_pods.p;
+    M.class_off = ctx->d_class_off.p; M.class_blob = ctx->d_class_blob.p; M.classes = ctx->d_mv_classes.p; M.pod_class = ctx->d_pod_class.p;
+    M.placement = ctx->d_pl_place.p;
+    M.cnt = ctx->d_pl_cnt.p; M.cnt_total = ctx->d_pl_cnt_total.p; M.scache = ctx->d_scache.p; M.moves = ctx->d_moves.p;
+    M.out_gain = ctx->d_mv_gain.p; M.out_code = ctx->d_mv_code.p; M.best_per_pod = ctx->d_mv_best_pod.p; M.best_global = ctx->d_mv_best.p;
+    M.hist = ctx->d_mv_hist.p; M.move_base = 0;
+    M.scope = scope; M.gpu = ctx->d_mv_gpu.p; M.hs = ctx->d_mv_hs.p; M.hreg = ctx->d_mv_hreg.p;
+    M.out_slots = (scope & SIMON_MOVES_SCOPE_GPU_SHARE) ? ctx->d_mv_slots.p : nullptr;
+    SkParams Pk;
+    fill_params(ctx, S, Pk);
+    SmvPlan Q;
+    memset(&Q, 0, sizeof(Q));
+    Q.max_moves = max_moves; Q.min_gain = min_gain;
+    Q.req_mcpu = ctx->d_pl_req_mcpu.p; Q.req_mem = ctx->d_pl_req_mem.p; Q.req_eph = ctx->d_pl_req_eph.p;
+    Q.nz_mcpu = ctx->d_pl_nz_mcpu.p; Q.nz_mem = ctx->d_pl_nz_mem.p; Q.req_scalar = ctx->d_pl_req_scalar.p; Q.gpu_used = ctx->d_pl_gpu_used.p;
+    Q.num_pods = ctx->d_pl_num_pods.p; Q.cnt = ctx->d_pl_cnt.p; Q.cnt_total = ctx->d_pl_cnt_total.p; Q.place = ctx->d_pl_place.p;
+    Q.slots = ctx->d_pl_slots.p; Q.moves = ctx->d_moves.p; Q.mv_slots = M.out_slots;
+    Q.best_global = ctx->d_mv_best.p; Q.hist = ctx->d_mv_hist.p; Q.nodes = ctx->d_mv_nodes.p; Q.gpu = gpu ? ctx->d_mv_gpu.p : nullptr;
+    Q.pods = ctx->d_mv_pods.p; Q.steps = ctx->d_pl_steps.p; Q.ctl = ctx->d_pl_ctl.p;
+    // ---- steps: [hard prep] + scoring + apply, in chunks of growing length ----
+    const uint32_t grid = std::min<uint32_t>((n + 255) / 256, (uint32_t)ctx->sms * 4u * 2u);
+    const uint64_t limit = std::min<uint64_t>(max_moves, (uint64_t)P + 1);     // after P steps every pod has moved: the next pass stops
+    uint32_t ctl[4] = {0, 0, 0, 0};
+    uint64_t enq = 0;
+    for (uint32_t chunk = 4; enq < limit && !ctl[1]; chunk = std::min(chunk * 2, 64u)) {
+        const uint64_t end = std::min<uint64_t>(limit, enq + chunk);
+        for (; enq < end; enq++) {
+            if (scoped && ctx->mv_n_prep)
+                simon_moves_hard_prep<<<ctx->mv_n_prep, 256, 0, st>>>(N, ctx->use_scache, ctx->d_scache.p, ctx->d_label_bits.p, ctx->d_topo_dom.p,
+                                                                      ctx->d_topo_ndom.p, ctx->d_class_off.p, ctx->d_class_blob.p, ctx->d_pl_cnt.p,
+                                                                      ctx->d_mv_prep.p, ctx->d_mv_hreg.p, ctx->d_mv_hs.p);
+            if (n) {
+                if (scoped) simon_moves_kernel<4, true><<<grid, 256, 0, st>>>(M);
+                else simon_moves_kernel<4, false><<<grid, 256, 0, st>>>(M);
+            }
+            simon_moves_plan_apply<<<1, 32, 0, st>>>(Pk, Q);
+            ctx->launches += (scoped && ctx->mv_n_prep ? 1 : 0) + (n ? 1 : 0) + 1;
+        }
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(ctl, ctx->d_pl_ctl.p, 16, cudaMemcpyDeviceToHost, st));
+        cudaError_t e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "move plan failed: %s", cudaGetErrorString(e));
+    }
+    CU(cudaEventRecord(ctx->ev1, st));
+    CU(cudaEventSynchronize(ctx->ev1));
+    CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    if (ctl[1] == SMV_PLAN_ERROR)
+        return fail(ctx, SIMON_ERR_CUDA, "move plan: inconsistent state at step %u (%s)", ctl[0],
+                    ctl[2] == SMV_PLAN_ERR_SLOTS ? "Reserve on the target differs from the scored GPU slots" : "a count of the source node went negative");
+    if (!ctl[1]) return fail(ctx, SIMON_ERR_CUDA, "move plan: no stop after %llu steps", (unsigned long long)limit);
+    if (ctl[0]) CU(cudaMemcpy(out_steps, ctx->d_pl_steps.p, sizeof(simon_plan_step) * ctl[0], cudaMemcpyDeviceToHost));
+    memset(out, 0, sizeof(*out));
+    out->n_steps = ctl[0]; out->stop_reason = ctl[1]; out->n_excluded = ctl[3]; out->kernel_ms = ctx->last_ms;
+    ctx->pl_valid = true;
+    return SIMON_OK;
+}
+
+int simon_moves_plan_download(simon_ctx *ctx, int32_t *placement, uint32_t *gpu_slots) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->pl_valid) return fail(ctx, SIMON_ERR_STATE, "no simon_moves_plan since the last upload");
+    CU(cudaSetDevice(ctx->device));
+    if (placement && ctx->n_pods) CU(cudaMemcpy(placement, ctx->d_pl_place.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost));
+    if (gpu_slots && ctx->n_pods) CU(cudaMemcpy(gpu_slots, ctx->d_pl_slots.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost));
+    return SIMON_OK;
+}
+
+int simon_moves_plan_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *req_mem, int64_t *req_eph, int64_t *nz_mcpu,
+                                    int64_t *nz_mem, int32_t *num_pods, int64_t *req_scalar, int64_t *gpu_used) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->pl_valid) return fail(ctx, SIMON_ERR_STATE, "no simon_moves_plan since the last upload");
+    CU(cudaSetDevice(ctx->device));
+    const uint64_t N = ctx->N;
+    if (req_mcpu) CU(cudaMemcpy(req_mcpu, ctx->d_pl_req_mcpu.p, 8 * N, cudaMemcpyDeviceToHost));
+    if (req_mem) CU(cudaMemcpy(req_mem, ctx->d_pl_req_mem.p, 8 * N, cudaMemcpyDeviceToHost));
+    if (req_eph) CU(cudaMemcpy(req_eph, ctx->d_pl_req_eph.p, 8 * N, cudaMemcpyDeviceToHost));
+    if (nz_mcpu) CU(cudaMemcpy(nz_mcpu, ctx->d_pl_nz_mcpu.p, 8 * N, cudaMemcpyDeviceToHost));
+    if (nz_mem) CU(cudaMemcpy(nz_mem, ctx->d_pl_nz_mem.p, 8 * N, cudaMemcpyDeviceToHost));
+    if (num_pods) CU(cudaMemcpy(num_pods, ctx->d_pl_num_pods.p, 4 * N, cudaMemcpyDeviceToHost));
+    if (req_scalar && ctx->K) CU(cudaMemcpy(req_scalar, ctx->d_pl_req_scalar.p, 8 * ctx->K * N, cudaMemcpyDeviceToHost));
+    if (gpu_used) CU(cudaMemcpy(gpu_used, ctx->d_pl_gpu_used.p, 8 * SIMON_MAX_GPU_DEV * N, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 

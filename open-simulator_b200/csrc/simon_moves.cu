@@ -534,3 +534,143 @@ __global__ void __launch_bounds__(1024) simon_moves_collect(uint32_t n_moves, co
     }
     if (threadIdx.x == 0) { out_n[0] = base_gt < k ? base_gt : k; out_n[1] = base_eq < need_eq ? base_eq : need_eq; }
 }
+
+// ---- migration plans (simon_moves_plan, include/simon_gpu.h) ----------------------------------------------------------------------
+// A plan runs the scoring kernels above unchanged on plan-owned copies of the dynamic columns; between two scoring passes the apply
+// kernel below moves the winner and patches the packed records (SmvNode of a and b, SmvGpu of a and b, SmvPod of p) in place, so no
+// pack runs after the setup.  Control words: ctl[0] steps recorded, ctl[1] stop reason (SMV_PLAN_ERROR: inconsistency), ctl[2] the
+// inconsistency (SMV_PLAN_ERR_*), ctl[3] the excluded pods.
+#define SMV_PLAN_ERROR 0xffu
+#define SMV_PLAN_ERR_SLOTS 1u            // Reserve on the target gave other slots than the scoring reported
+#define SMV_PLAN_ERR_NEGATIVE 2u         // a count of the source node would go negative
+
+struct SmvPlan {
+    uint32_t max_moves;
+    int32_t min_gain;
+    int64_t *req_mcpu, *req_mem, *req_eph, *nz_mcpu, *nz_mem, *req_scalar, *gpu_used;
+    int32_t *num_pods, *cnt, *cnt_total, *place;
+    uint32_t *slots;                    // [P] GPU slot word of every pod
+    const uint2 *moves;
+    const uint32_t *mv_slots;           // [n_moves] slots the scoring reported (GPU share in scope), or NULL
+    unsigned long long *best_global;
+    uint32_t *hist;
+    SmvNode *nodes;
+    SmvGpu *gpu;                        // NULL unless the scoring reads it
+    SmvPod *pods;
+    simon_plan_step *steps;
+    uint32_t *ctl;
+};
+
+// After simon_moves_pack on the plan copies: the excluded pods (placed, of a GPU-share class that is neither pinned nor Open-Local,
+// with a saturated nibble in the slot word) become never movable, and are counted
+__global__ void simon_moves_plan_setup(uint32_t n_pods, const uint32_t *slots, SmvPod *pods, uint32_t *ctl) {
+    for (uint32_t q = blockIdx.x * blockDim.x + threadIdx.x; q < n_pods; q += gridDim.x * blockDim.x) {
+        const SmvPod r = pods[q];
+        if (!(r.bits & SMC_NEED_GPU) || (r.bits & SMC_NEVER) || r.node < 0) continue;
+        const uint32_t w = slots[q];
+        bool sat = false;
+#pragma unroll
+        for (int d = 0; d < SIMON_MAX_GPU_DEV; d++) sat |= ((w >> (4 * d)) & 15u) == 15u;
+        if (sat) {
+            pods[q].bits = r.bits | SMC_NOT_MOVABLE | SMC_NEVER;
+            atomicAdd(ctl + 3, 1u);
+        }
+    }
+}
+
+// One step's apply (one warp): the best key of the scoring pass, the stop conditions, then pod p moves from a to b on the plan
+// columns - lane 0 the node sums and the devices, every lane a share of the scalars and of the commit list (eligibility-conditional
+// entries as simon_import_kernel counts them) - and the packed records follow.  Clears the best key and the histogram for the next pass.
+__global__ void __launch_bounds__(32) simon_moves_plan_apply(const __grid_constant__ SkParams P, const __grid_constant__ SmvPlan Q) {
+    const uint32_t lane = threadIdx.x;
+    if (Q.ctl[1]) return;                // stopped: the passes enqueued after the stop score for nothing
+    const unsigned long long key = *Q.best_global;
+    const int32_t gain = (int32_t)(uint32_t)(key >> 32) - SMV_GAIN_BIAS;
+    __syncwarp();
+    if (key == 0ull || gain < Q.min_gain) {
+        if (lane == 0) Q.ctl[1] = SIMON_PLAN_STOP_NO_MOVE;
+        return;
+    }
+    const uint32_t m = 0xffffffffu - (uint32_t)key;
+    const uint2 mv = Q.moves[m];
+    const uint32_t p = mv.x, b = mv.y, N = P.N;
+    const uint32_t a = (uint32_t)Q.place[p];
+    const int64_t *cw = P.class_blob + P.class_off[P.pod_class[p]];
+    bool neg = false;
+    uint32_t pack = 0, err = 0;
+    if (lane == 0) {
+        Q.req_mcpu[a] -= cw[SCW_REQ_MCPU]; Q.req_mem[a] -= cw[SCW_REQ_MEM]; Q.req_eph[a] -= cw[SCW_REQ_EPH];
+        Q.nz_mcpu[a] -= cw[SCW_NZ_MCPU]; Q.nz_mem[a] -= cw[SCW_NZ_MEM]; Q.num_pods[a] -= 1;
+        neg |= Q.req_mcpu[a] < 0 || Q.req_mem[a] < 0 || Q.req_eph[a] < 0 || Q.nz_mcpu[a] < 0 || Q.nz_mem[a] < 0 || Q.num_pods[a] < 0;
+        Q.req_mcpu[b] += cw[SCW_REQ_MCPU]; Q.req_mem[b] += cw[SCW_REQ_MEM]; Q.req_eph[b] += cw[SCW_REQ_EPH];
+        Q.nz_mcpu[b] += cw[SCW_NZ_MCPU]; Q.nz_mem[b] += cw[SCW_NZ_MEM]; Q.num_pods[b] += 1;
+        if (cw[SCW_GPU_MEM] > 0) {
+            // release on a what the slot word states (0 for a pre-bound pod), then Reserve on b
+            const uint32_t w = Q.slots[p];
+#pragma unroll 1
+            for (int d = 0; d < SIMON_MAX_GPU_DEV; d++) {
+                const int64_t n = (w >> (4 * d)) & 15u;
+                if (!n) continue;
+                Q.gpu_used[(uint64_t)d * N + a] -= n * cw[SCW_GPU_MEM];
+                neg |= Q.gpu_used[(uint64_t)d * N + a] < 0;
+            }
+            SkScenario SC{};
+            SC.gpu_used = Q.gpu_used;
+            pack = gpu_reserve(P, SC, cw, b);
+            if (pack != (Q.mv_slots ? Q.mv_slots[m] : 0u)) err = SMV_PLAN_ERR_SLOTS;
+        }
+    }
+    const int64_t *sc = cw + cw[SCW_OFF_SCALARS];
+    for (uint32_t k = lane; k < P.K; k += 32) {
+        if (sc[k] == 0) continue;
+        Q.req_scalar[(uint64_t)k * N + a] -= sc[k];
+        neg |= Q.req_scalar[(uint64_t)k * N + a] < 0;
+        Q.req_scalar[(uint64_t)k * N + b] += sc[k];
+    }
+    const ReqCtx RC{P.label_bits, N, -1};
+    const int64_t *inc = cw + cw[SCW_OFF_INC];
+    for (int64_t u = lane; u < cw[SCW_N_INC]; u += 32) {
+        const int64_t k = inc[3 * u], t = inc[3 * u + 1], sig = inc[3 * u + 2];
+        const int32_t da = P.topo_dom[(uint64_t)t * N + a], db = P.topo_dom[(uint64_t)t * N + b];
+        if (da >= 0 && (sig < 0 || elig_eval(P, sig, RC, a))) {
+            neg |= atomicSub(&Q.cnt[P.cnt_off[k] + da], 1) <= 0;
+            neg |= atomicSub(&Q.cnt_total[k], 1) <= 0;
+        }
+        if (db >= 0 && (sig < 0 || elig_eval(P, sig, RC, b))) {
+            atomicAdd(&Q.cnt[P.cnt_off[k] + db], 1);
+            atomicAdd(&Q.cnt_total[k], 1);
+        }
+    }
+    if (__any_sync(0xffffffffu, neg) && !err) err = SMV_PLAN_ERR_NEGATIVE;
+    for (uint32_t q = lane; q < SMV_NBINS; q += 32) Q.hist[q] = 0u;
+    if (lane != 0) return;
+    if (err) {
+        Q.ctl[2] = err;
+        Q.ctl[1] = SMV_PLAN_ERROR;
+        return;
+    }
+    Q.place[p] = (int32_t)b;
+    if (cw[SCW_GPU_MEM] > 0) Q.slots[p] = pack;
+    const uint32_t ends[2] = {a, b};
+#pragma unroll
+    for (int e = 0; e < 2; e++) {
+        const uint32_t g = ends[e];
+        SmvNode &r = Q.nodes[g];
+        r.req_mcpu = Q.req_mcpu[g]; r.req_mem = Q.req_mem[g]; r.req_eph = Q.req_eph[g];
+        r.nz_mcpu = Q.nz_mcpu[g]; r.nz_mem = Q.nz_mem[g]; r.num_pods = Q.num_pods[g];
+        if (Q.gpu) {
+            const int nd = P.gpu_count ? P.gpu_count[g] : 0;
+#pragma unroll 1
+            for (int d = 0; d < SIMON_MAX_GPU_DEV; d++) Q.gpu[g].free_mem[d] = d < nd ? P.gpu_dev_mem[g] - Q.gpu_used[(uint64_t)d * N + g] : -1;
+        }
+    }
+    Q.pods[p].node = (int32_t)b;
+    Q.pods[p].bits |= SMC_NOT_MOVABLE | SMC_NEVER;          // each pod moves at most once
+    const uint32_t s = Q.ctl[0];
+    simon_plan_step st;
+    st.move = m; st.pod = p; st.from = (int32_t)a; st.to = (int32_t)b; st.gain = gain; st.gpu_slots = pack;
+    Q.steps[s] = st;
+    Q.ctl[0] = s + 1;
+    if (s + 1 >= Q.max_moves) Q.ctl[1] = SIMON_PLAN_STOP_MAX_MOVES;
+    *Q.best_global = 0ull;
+}

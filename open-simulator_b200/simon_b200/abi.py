@@ -106,6 +106,22 @@ MOVE_NOOP, MOVE_NOT_PLACED, MOVE_NOT_MOVABLE, MOVE_BAD_INDEX = 1 << 24, 1 << 25,
 MOVE_GAIN_BIAS = 1000
 # simon_moves_set_scope: admit GPU-share classes / classes with DoNotSchedule spread constraints as move candidates
 MOVES_SCOPE_GPU_SHARE, MOVES_SCOPE_HARD_SPREAD = 1, 2
+# simon_moves_plan stop reasons
+PLAN_STOP_NO_MOVE, PLAN_STOP_MAX_MOVES = 1, 2
+
+
+class SimonPlanStep(C.Structure):
+    _fields_ = [("move", C.c_uint32), ("pod", C.c_uint32), ("from_", C.c_int32), ("to", C.c_int32), ("gain", C.c_int32),
+                ("gpu_slots", C.c_uint32)]
+
+
+PLAN_STEP_DTYPE = np.dtype([("move", np.uint32), ("pod", np.uint32), ("from", np.int32), ("to", np.int32), ("gain", np.int32),
+                            ("gpu_slots", np.uint32)])
+
+
+class SimonMovesPlanResult(C.Structure):
+    _fields_ = [("n_steps", C.c_uint32), ("stop_reason", C.c_uint32), ("n_excluded", C.c_uint32), ("reserved", C.c_uint32),
+                ("kernel_ms", C.c_float), ("reserved2", C.c_uint32)]
 
 
 _SNAP_DTYPES = {

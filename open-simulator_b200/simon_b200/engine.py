@@ -27,7 +27,7 @@ EXPORTS = ["simon_gpu_version", "simon_ctx_create", "simon_ctx_destroy", "simon_
            "simon_storage_upload", "simon_storage_state_download", "simon_devices_upload", "simon_devices_state_download",
            "simon_scenarios_run_local", "simon_scenarios_storage_download", "simon_moves_set_scope", "simon_moves_gpu_slots_download",
            "simon_schedule_resume", "simon_last_launch", "simon_drain_run", "simon_drain_download", "simon_drain_times",
-           "simon_drain_budget"]
+           "simon_drain_budget", "simon_moves_plan", "simon_moves_plan_download", "simon_moves_plan_state_download"]
 
 
 class EngineUnavailable(RuntimeError):
@@ -116,6 +116,12 @@ def lib():
         L.simon_drain_times.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float)]
         L.simon_drain_budget.restype = C.c_int
         L.simon_drain_budget.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+        L.simon_moves_plan.restype = C.c_int
+        L.simon_moves_plan.argtypes = [C.c_void_p, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p]
+        L.simon_moves_plan_download.restype = C.c_int
+        L.simon_moves_plan_download.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.simon_moves_plan_state_download.restype = C.c_int
+        L.simon_moves_plan_state_download.argtypes = [C.c_void_p] + [C.c_void_p] * 8
     except AttributeError:
         if not os.environ.get("SIMON_GPU_LIB"):       # an experiment library may lack the newer entry points; the shipped one may not
             raise
@@ -353,6 +359,34 @@ class Engine:
         ms = C.c_float(0)
         self._check(lib().simon_moves_replay(self.h, steps, C.byref(ms)))
         return float(ms.value)
+
+    def moves_plan(self, max_moves: int, min_gain: int = 1):
+        """A migration plan over the uploaded move list (move_base 0) on the live state, under the current move scope
+        (simon_moves_plan): -> dict(steps: structured array of abi.PLAN_STEP_DTYPE, stop_reason, excluded, kernel_ms).
+        The live state is not changed."""
+        steps = np.zeros(max(max_moves, 1), abi.PLAN_STEP_DTYPE)
+        res = abi.SimonMovesPlanResult()
+        self._check(lib().simon_moves_plan(self.h, max_moves, min_gain, steps.ctypes.data, C.byref(res)))
+        return dict(steps=steps[:res.n_steps].copy(), stop_reason=int(res.stop_reason), excluded=int(res.n_excluded),
+                    kernel_ms=float(res.kernel_ms))
+
+    def moves_plan_download(self):
+        """After moves_plan: (placement [P] int32, GPU slot words [P] uint32) of the plan's end state."""
+        P = self.c.pods_dims["n_pods"]
+        pl = np.zeros(max(P, 1), np.int32)
+        sl = np.zeros(max(P, 1), np.uint32)
+        self._check(lib().simon_moves_plan_download(self.h, pl.ctypes.data, sl.ctypes.data))
+        return pl[:P], sl[:P]
+
+    def moves_plan_state(self):
+        """After moves_plan: the plan's end state as (state(), state_ext()) dicts."""
+        N, K = self.c.n_nodes, int(self.c.snap_dims["n_scalars"])
+        arrs = [np.zeros(max(N, 1), np.int64) for _ in range(5)] + [np.zeros(max(N, 1), np.int32)]
+        rs = np.zeros((max(K, 1), max(N, 1)), np.int64)
+        gu = np.zeros((8, max(N, 1)), np.int64)
+        self._check(lib().simon_moves_plan_state_download(self.h, *[a.ctypes.data for a in arrs], rs.ctypes.data, gu.ctypes.data))
+        st = dict(zip(["req_mcpu", "req_mem", "req_eph", "nz_mcpu", "nz_mem", "num_pods"], [a[:N] for a in arrs]))
+        return st, dict(req_scalar=rs[:K, :N], gpu_used=gu[:, :N])
 
     def run_scenarios(self, scenarios: List[np.ndarray], want_nodes: bool = False):
         """scenarios: list of uint32 arrays (active node indices in scenario order)."""

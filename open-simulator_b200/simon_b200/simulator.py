@@ -559,6 +559,24 @@ class Simulator:
         return scaledown.plan_scale_down(compiled, self.placements, lambda rl: eng.drain_run(self.placements, rl, detail=False),
                                          candidates=cand, max_remove=max_remove)
 
+    def PlanMigrations(self, sources: Optional[List[str]] = None, targets: Optional[List[str]] = None, max_moves: int = 100,
+                       min_gain: int = 1, move_scope: int = 0):
+        """rebalance.MigrationPlan on the session's live state: the pods of the source nodes (all by default) as candidates onto the
+        target nodes (all by default), planned on the device (simon_moves_plan).  The session's state is not changed by it."""
+        from . import rebalance
+        eng, compiled = self._live()
+        idx = {}
+        for what, names in (("sources", sources), ("targets", targets)):
+            if names is None:
+                idx[what] = None
+                continue
+            idx[what] = [compiled.node_index(nm) for nm in names]
+            bad = [nm for nm, g in zip(names, idx[what]) if g < 0]
+            if bad:
+                raise ValueError(f"PlanMigrations: no node named {bad[0]!r} among the {what}")
+        moves = rebalance.candidates(compiled, self.placements, idx["sources"], idx["targets"])
+        return rebalance.plan(eng, compiled, moves, max_moves, min_gain, move_scope)
+
     def _live(self):
         self._check_open()
         if self.engine is None or self.compiled is None:
