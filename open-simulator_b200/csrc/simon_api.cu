@@ -87,15 +87,64 @@ struct DevBuf {
     ~DevBuf() { release(); }
 };
 
-// The dynamic state of n scenarios, one allocation per column; scenario i owns slice i of each (alloc_pool, clear_pool, fill_scen).
+// The engine's dynamic node state, n copies of it: one allocation per column, copy i owns slice i of each.  The columns and their
+// elements per copy are listed once, in each(); allocating, clearing, copying, slicing and downloading them all go through it.
+struct NodeState {
+    static constexpr int COLS = 10;
+    uint32_t n = 0;
+    uint64_t N = 0, K = 0, cw = 0, nc = 0;      // nodes, scalar resources, counter words and counters of one copy
+    DevBuf<int64_t> req_mcpu, req_mem, req_eph, nz_mcpu, nz_mem;
+    DevBuf<int32_t> num_pods;
+    DevBuf<int64_t> req_scalar, gpu_used;
+    DevBuf<int32_t> cnt, cnt_total;
+
+    // f(column, the same column of o, elements of one copy) for every column in this order, until f returns an error.  Counts as
+    // uploaded, or padded: at least one node, scalar and counter word, as allocated.
+    template <typename F>
+    cudaError_t each(NodeState &o, bool padded, F &&f) {
+        auto pad = [&](uint64_t x) { return padded ? std::max<uint64_t>(1, x) : x; };
+        const uint64_t n1 = pad(N);
+        cudaError_t e = cudaSuccess;
+        auto col = [&](auto &a, auto &b, uint64_t count) { if (e == cudaSuccess) e = f(a, b, count); };
+        col(req_mcpu, o.req_mcpu, n1); col(req_mem, o.req_mem, n1); col(req_eph, o.req_eph, n1);
+        col(nz_mcpu, o.nz_mcpu, n1); col(nz_mem, o.nz_mem, n1); col(num_pods, o.num_pods, n1);
+        col(req_scalar, o.req_scalar, pad(K) * n1); col(gpu_used, o.gpu_used, SIMON_MAX_GPU_DEV * n1);
+        col(cnt, o.cnt, pad(cw)); col(cnt_total, o.cnt_total, pad(nc));
+        return e;
+    }
+    void shape(uint32_t copies, uint64_t nodes, uint64_t scalars, uint64_t words, uint64_t counters) { n = copies; N = nodes; K = scalars; cw = words; nc = counters; }
+    // every column sized for the shape (DevBuf keeps the capacity), without clearing it
+    cudaError_t alloc() { return each(*this, true, [&](auto &c, auto &, uint64_t k) { return c.alloc(n * k); }); }
+    cudaError_t clear(cudaStream_t st) { return each(*this, true, [&](auto &c, auto &, uint64_t k) { return cudaMemsetAsync(c.p, 0, n * k * sizeof(*c.p), st); }); }
+    // copy 0 = copy 0 of src, device to device
+    cudaError_t copy(NodeState &src, cudaStream_t st) {
+        return each(src, true, [&](auto &d, auto &s, uint64_t k) { return cudaMemcpyAsync(d.p, s.p, k * sizeof(*d.p), cudaMemcpyDeviceToDevice, st); });
+    }
+    // copy 0 into dst[c] for column c in each()'s order (null: not wanted), at the uploaded sizes
+    cudaError_t download(void *const dst[COLS]) {
+        int c = 0;
+        return each(*this, false, [&](auto &col, auto &, uint64_t k) {
+            void *d = dst[c++];
+            return d && k ? cudaMemcpy(d, col.p, k * sizeof(*col.p), cudaMemcpyDeviceToHost) : cudaSuccess;
+        });
+    }
+    // copy i of every column into the same-named pointers of a kernel argument (SkScenario, SmvPlan); a column holds n equal slices
+    template <typename D>
+    void slice(uint32_t i, D &o) const {
+        auto at = [&](const auto &c) { return c.p + i * (c.n / n); };
+        o.req_mcpu = at(req_mcpu); o.req_mem = at(req_mem); o.req_eph = at(req_eph); o.nz_mcpu = at(nz_mcpu); o.nz_mem = at(nz_mem);
+        o.num_pods = at(num_pods); o.req_scalar = at(req_scalar); o.gpu_used = at(gpu_used); o.cnt = at(cnt); o.cnt_total = at(cnt_total);
+    }
+};
+
+// The dynamic state of n scenarios, one allocation per column; scenario i owns slice i of each (size_pool, clear_pool, fill_scen).
 // The context keeps two: the single-scenario pool (n = 1) and the batch pool, so a batch never touches the single-scenario state.
 struct ScenPool {
     uint32_t n = 0;
-    // elements of one scenario's slice: node-indexed, req_scalar, counters, counter totals, classes (csum / fbits / ocache rows),
-    // soft and hard constraint tables, out_node, Open-Local VG requested
-    size_t nodes = 1, scal = 1, cntw = 1, nct = 1, ncl = 1, tabw = 1, regw = 1, pods = 1, vn = 1;
-    DevBuf<int64_t> req_mcpu, req_mem, req_eph, nz_mcpu, nz_mem, req_scalar, gpu_used;
-    DevBuf<int32_t> num_pods, cnt, cnt_total, tp, fcount, size, out_node;
+    // elements of one scenario's slice: node-indexed, classes (csum / fbits / ocache rows), constraint tables, out_node, VG requested
+    size_t nodes = 1, ncl = 1, tabw = 1, regw = 1, pods = 1, vn = 1;
+    NodeState state;
+    DevBuf<int32_t> tp, fcount, size, out_node;
     DevBuf<long long> csum;
     DevBuf<uint8_t> fbits, hard_reg;
     DevBuf<unsigned long long> ocache, clk;
@@ -235,14 +284,14 @@ struct simon_ctx {
     DevBuf<uint32_t> d_mv_hreg, d_mv_slots;
     DevBuf<int2> d_mv_hs;
     DevBuf<SmvGpu> d_mv_gpu;
-    // migration plans (simon_moves_plan): plan-owned copies of the dynamic columns of the single-scenario state, the steps and the
-    // control words.  have_live: the single-scenario state holds a placement (a schedule, resume, replay or drain rebuild since the
+    // migration plans (simon_moves_plan): plan-owned copies of the single-scenario node state, placement and GPU slot words, the steps
+    // and control words.  have_live: the single-scenario state holds a placement (a schedule, resume, replay or drain rebuild since the
     // last pod upload or reset); pl_valid: the plan columns hold the last plan's end state
     bool have_live = false, pl_valid = false;
-    DevBuf<int64_t> d_pl_req_mcpu, d_pl_req_mem, d_pl_req_eph, d_pl_nz_mcpu, d_pl_nz_mem, d_pl_req_scalar, d_pl_gpu_used;
-    DevBuf<int32_t> d_pl_num_pods, d_pl_cnt, d_pl_cnt_total, d_pl_place;
-    DevBuf<uint32_t> d_pl_slots, d_pl_ctl;
-    DevBuf<simon_plan_step> d_pl_steps;
+    NodeState pl_state;
+    DevBuf<int32_t> pl_place;
+    DevBuf<uint32_t> pl_slots, pl_ctl;
+    DevBuf<simon_plan_step> pl_steps;
     uint32_t n_pin_fast = 0;           // pods marked for the pinned-run fast path (-4 in the device copy of pod_fixed_node)
     std::vector<uint8_t> bypass;        // per pod: never reaches the scheduler in a single-scenario run (pre-bound or absent)
     // resumed runs (simon_schedule_resume): per pod the uploaded pod_fixed_node and guard (what its prefix entry is checked against),
@@ -315,10 +364,7 @@ SkScenario fill_scen(const ScenPool &s, uint32_t i, uint32_t n_active, bool iden
     o.order = identity ? nullptr : s.order.p + nn;
     o.rank_of = identity ? nullptr : s.rank_of.p + nn;
     o.n_active = n_active;
-    o.req_mcpu = s.req_mcpu.p + nn; o.req_mem = s.req_mem.p + nn; o.req_eph = s.req_eph.p + nn;
-    o.nz_mcpu = s.nz_mcpu.p + nn; o.nz_mem = s.nz_mem.p + nn;
-    o.req_scalar = s.req_scalar.p + i * s.scal; o.gpu_used = s.gpu_used.p + nn * SIMON_MAX_GPU_DEV;
-    o.num_pods = s.num_pods.p + nn; o.cnt = s.cnt.p + i * s.cntw; o.cnt_total = s.cnt_total.p + i * s.nct;
+    s.state.slice(i, o);
     o.tp = s.tp.p + i * s.tabw; o.fcount = s.fcount.p + i * s.tabw; o.size = s.size.p + (size_t)i * SK_MAX_SOFT;
     o.hard_reg = s.hard_reg.p + i * s.regw;
     o.csum = s.csum.p + i * s.ncl * SK_CSUM_W; o.fbits = s.fbits.p + nn * s.ncl; o.ocache = s.ocache.p + nn * s.ncl;
@@ -341,11 +387,7 @@ cudaError_t bcast(simon_ctx *ctx, const T *src, size_t len, uint32_t n, T *dst) 
 int clear_pool(simon_ctx *ctx, ScenPool &s) {
     cudaStream_t st = ctx->stream;
     const size_t n = s.n, nn = n * s.nodes;
-    CU(cudaMemsetAsync(s.req_mcpu.p, 0, 8 * nn, st)); CU(cudaMemsetAsync(s.req_mem.p, 0, 8 * nn, st));
-    CU(cudaMemsetAsync(s.req_eph.p, 0, 8 * nn, st)); CU(cudaMemsetAsync(s.nz_mcpu.p, 0, 8 * nn, st));
-    CU(cudaMemsetAsync(s.nz_mem.p, 0, 8 * nn, st)); CU(cudaMemsetAsync(s.req_scalar.p, 0, 8 * n * s.scal, st));
-    CU(cudaMemsetAsync(s.gpu_used.p, 0, 8 * nn * SIMON_MAX_GPU_DEV, st)); CU(cudaMemsetAsync(s.num_pods.p, 0, 4 * nn, st));
-    CU(cudaMemsetAsync(s.cnt.p, 0, 4 * n * s.cntw, st)); CU(cudaMemsetAsync(s.cnt_total.p, 0, 4 * n * s.nct, st));
+    CU(s.state.clear(st));
     // the own-score cache is keyed by the node's pod count, which restarts with the state
     CU(cudaMemsetAsync(s.ocache.p, 0, 8 * nn * s.ncl, st));
     // the stored feasible-set summaries (and the feasibility bits they are exact for) describe the node set and order of
@@ -358,37 +400,41 @@ int clear_pool(simon_ctx *ctx, ScenPool &s) {
     return SIMON_OK;
 }
 
-// Size every column of `s` for n scenarios of the current uploads (DevBuf keeps the capacity), without clearing it.  single: the pool
-// of single runs, with their per-pod outputs and its one SkScenario (every node) uploaded; else a batch pool, with node lists and
-// results, and with out_node [n][P] unless pod_outputs is false (drain batches keep their per-pod outputs elsewhere).
-int size_pool(simon_ctx *ctx, ScenPool &s, uint32_t n, bool single, bool pod_outputs = true) {
+// Shape `s` for n scenarios of the current uploads, then f(column, elements of one scenario) for every per-scenario column; out_node
+// holds one element unless pod_outputs (drain batches keep their per-pod outputs elsewhere)
+template <typename F>
+cudaError_t pool_columns(const simon_ctx *ctx, ScenPool &s, uint32_t n, bool single, bool pod_outputs, F &&f) {
     s.n = n;
-    s.nodes = std::max(1u, ctx->N); s.scal = (size_t)(ctx->K ? ctx->K : 1) * s.nodes;
-    s.cntw = std::max<uint64_t>(1, ctx->cnt_words); s.nct = std::max(1u, ctx->n_counters); s.ncl = std::max(1u, ctx->n_classes);
+    s.state.shape(n, ctx->N, ctx->K, ctx->cnt_words, ctx->n_counters);
+    s.nodes = std::max(1u, ctx->N); s.ncl = std::max(1u, ctx->n_classes);
     s.tabw = (size_t)SK_MAX_SOFT * ctx->max_dom; s.regw = (size_t)SK_MAX_HARD * ctx->max_dom; s.pods = pod_outputs ? std::max(1u, ctx->n_pods) : 1;
     s.vn = std::max<size_t>(1, (size_t)ctx->V * ctx->N);
-    const size_t nn = (size_t)n * s.nodes;
-    CU(s.req_mcpu.alloc(nn)); CU(s.req_mem.alloc(nn)); CU(s.req_eph.alloc(nn)); CU(s.nz_mcpu.alloc(nn)); CU(s.nz_mem.alloc(nn));
-    CU(s.req_scalar.alloc(n * s.scal)); CU(s.gpu_used.alloc(nn * SIMON_MAX_GPU_DEV)); CU(s.num_pods.alloc(nn));
-    CU(s.cnt.alloc(n * s.cntw)); CU(s.cnt_total.alloc(n * s.nct));
-    CU(s.tp.alloc(n * s.tabw)); CU(s.fcount.alloc(n * s.tabw)); CU(s.size.alloc((size_t)n * SK_MAX_SOFT)); CU(s.hard_reg.alloc(n * s.regw));
-    CU(s.csum.alloc(n * s.ncl * SK_CSUM_W)); CU(s.fbits.alloc(nn * s.ncl)); CU(s.ocache.alloc(nn * s.ncl));
-    CU(s.out_node.alloc(n * s.pods)); CU(s.counters.alloc(2ull * n)); CU(s.clk.alloc(2ull * n)); CU(s.scen.alloc(n));
+    cudaError_t e = s.state.each(s.state, true, [&](auto &c, auto &, uint64_t k) { return f(c, k); });
+    auto col = [&](auto &c, size_t count) { if (e == cudaSuccess) e = f(c, count); };
+    col(s.tp, s.tabw); col(s.fcount, s.tabw); col(s.size, SK_MAX_SOFT); col(s.hard_reg, s.regw);
+    col(s.csum, s.ncl * SK_CSUM_W); col(s.fbits, s.nodes * s.ncl); col(s.ocache, s.nodes * s.ncl);
+    col(s.out_node, s.pods); col(s.counters, 2); col(s.clk, 2); col(s.scen, 1);
+    if (!single) { col(s.order, s.nodes); col(s.rank_of, s.nodes); col(s.results, 1); }
+    if (!single && ctx->have_storage) col(s.local_results, 1);
+    if (ctx->have_storage) { col(s.vg_req, s.vn); col(s.local_raw, s.nodes); }
+    if (ctx->have_devices) col(s.dev_alloc, s.nodes);
+    return e;
+}
+
+// Size every column of `s` for n scenarios (pool_columns; DevBuf keeps the capacity), without clearing it.  single: the pool of single
+// runs, with their per-pod outputs and its one SkScenario (every node) uploaded; else a batch pool.
+int size_pool(simon_ctx *ctx, ScenPool &s, uint32_t n, bool single, bool pod_outputs = true) {
+    CU(pool_columns(ctx, s, n, single, pod_outputs, [&](auto &c, size_t k) { return c.alloc(n * k); }));
     if (single) {
         if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(s.out_score.alloc(ctx->n_pods));
         CU(s.out_gpu.alloc(ctx->n_pods));
         CU(s.fail_counts.alloc((size_t)ctx->max_fail * SIMON_N_FAIL_CODES)); CU(s.fail_pod.alloc(ctx->max_fail));
         // fbits are cleared here for single runs and never for batches: the kernel reads them only under a valid csum record
-        CU(cudaMemsetAsync(s.fbits.p, 0, nn * s.ncl, ctx->stream));
+        CU(cudaMemsetAsync(s.fbits.p, 0, (size_t)n * s.nodes * s.ncl, ctx->stream));
         const SkScenario sc = fill_scen(s, 0, ctx->N, true);
         CU(cudaMemcpyAsync(s.scen.p, &sc, sizeof(sc), cudaMemcpyHostToDevice, ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));        // `sc` leaves scope
-    } else {
-        CU(s.order.alloc(nn)); CU(s.rank_of.alloc(nn)); CU(s.results.alloc(n));
-        if (ctx->have_storage) CU(s.local_results.alloc(n));
     }
-    if (ctx->have_storage) { CU(s.vg_req.alloc(n * s.vn)); CU(s.local_raw.alloc(nn)); }
-    if (ctx->have_devices) CU(s.dev_alloc.alloc(nn));
     return SIMON_OK;
 }
 
@@ -734,6 +780,50 @@ int rebuild_prefix(simon_ctx *ctx, const SkParams &P, const int32_t *prefix_node
     return SIMON_OK;
 }
 
+// Before a run on the single-scenario pool: clear its failure records and counters; arm the dump in P if its pod is in [first, first + count)
+cudaError_t single_begin(simon_ctx *ctx, SkParams &P, uint32_t first = 0, uint32_t count = 0) {
+    cudaStream_t st = ctx->stream;
+    cudaError_t e = cudaMemsetAsync(ctx->single.fail_counts.p, 0, 4ull * ctx->max_fail * SIMON_N_FAIL_CODES, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ctx->single.counters.p, 0, 8, st);
+    if (e == cudaSuccess && ctx->dump_pod >= first && ctx->dump_pod < first + count) {
+        P.dump_pod = ctx->dump_pod; P.dump_total = ctx->d_dump_total.p; P.dump_code = ctx->d_dump_code.p;
+        e = cudaMemsetAsync(ctx->d_dump_total.p, 0xff, 8ull * std::max(1u, ctx->N), st);     // -1: node not scored (infeasible)
+        if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_dump_code.p, 0, 4ull * std::max(1u, ctx->N), st);
+    }
+    return e;
+}
+
+// After a run on the single-scenario pool: its device time, failure count, per-pod results of [first, first + count), failure records
+int single_end(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_node, int64_t *out_score, uint32_t *out_fail_counts,
+               uint32_t *out_fail_pod, uint32_t max_fail, uint32_t *out_n_fail) {
+    cudaError_t e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    ctx->have_live = true;
+    CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    const ScenPool &S = ctx->single;
+    uint32_t counters[2] = {0, 0};
+    CU(cudaMemcpy(counters, S.counters.p, 8, cudaMemcpyDeviceToHost));
+    if (out_n_fail) *out_n_fail = counters[0];
+    if (out_node && count) CU(cudaMemcpy(out_node, S.out_node.p + first, 4ull * count, cudaMemcpyDeviceToHost));
+    if (out_score && S.out_score.p && count) CU(cudaMemcpy(out_score, S.out_score.p + first, 8ull * count, cudaMemcpyDeviceToHost));
+    uint32_t nf = std::min(std::min(counters[0], max_fail), ctx->max_fail);
+    if (nf && out_fail_counts) CU(cudaMemcpy(out_fail_counts, S.fail_counts.p, 4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
+    if (nf && out_fail_pod) CU(cudaMemcpy(out_fail_pod, S.fail_pod.p, 4ull * nf, cudaMemcpyDeviceToHost));
+    return SIMON_OK;
+}
+
+// A batch's node lists (scenario_lists) on the device and its SkScenario array in h; all N nodes in index order need no node list
+cudaError_t batch_scenarios(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, std::vector<SkScenario> &h) {
+    const uint32_t N = ctx->N;
+    const ScenPool &B = ctx->batch;
+    h.resize(n);
+    for (uint32_t i = 0; i < n; i++)
+        h[i] = fill_scen(B, i, scen[i].n_nodes, scen[i].n_nodes == N && std::is_sorted(scen[i].nodes, scen[i].nodes + N));
+    const size_t bytes = 4ull * n * std::max(1u, N);
+    const cudaError_t e = cudaMemcpyAsync(B.order.p, B.h_order.data(), bytes, cudaMemcpyHostToDevice, ctx->stream);
+    return e != cudaSuccess ? e : cudaMemcpyAsync(B.rank_of.p, B.h_rank.data(), bytes, cudaMemcpyHostToDevice, ctx->stream);
+}
+
 }  // namespace
 
 extern "C" {
@@ -1043,37 +1133,17 @@ int simon_schedule(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_
     CU(cudaSetDevice(ctx->device));
     ctx->last_launch = simon_launch_info{};
     if (count == 0) { if (out_n_fail) *out_n_fail = 0; return SIMON_OK; }
-    cudaStream_t st = ctx->stream;
-    const ScenPool &S = ctx->single;
     uint32_t CS, TPB, NPT;
     size_t smem;
     int rc = choose_geometry(ctx, ctx->N, CS, TPB, NPT, smem);
     if (rc) return rc;
     SkParams P;
-    fill_params(ctx, S, P);
+    fill_params(ctx, ctx->single, P);
     P.first = first; P.count = count; P.max_fail = ctx->max_fail; P.npt = NPT;
-    CU(cudaMemsetAsync(S.fail_counts.p, 0, 4ull * ctx->max_fail * SIMON_N_FAIL_CODES, st));
-    CU(cudaMemsetAsync(S.counters.p, 0, 8, st));
-    if (ctx->dump_pod >= first && ctx->dump_pod < first + count) {
-        P.dump_pod = ctx->dump_pod; P.dump_total = ctx->d_dump_total.p; P.dump_code = ctx->d_dump_code.p;
-        CU(cudaMemsetAsync(ctx->d_dump_total.p, 0xff, 8ull * std::max(1u, ctx->N), st));     // -1: node not scored (infeasible)
-        CU(cudaMemsetAsync(ctx->d_dump_code.p, 0, 4ull * std::max(1u, ctx->N), st));
-    }
+    CU(single_begin(ctx, P, first, count));
     rc = launch_range(ctx, P, CS, TPB, smem, first, count, true);
     if (rc) return rc;
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
-    ctx->have_live = true;
-    CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
-    uint32_t counters[2] = {0, 0};
-    CU(cudaMemcpy(counters, S.counters.p, 8, cudaMemcpyDeviceToHost));
-    if (out_n_fail) *out_n_fail = counters[0];
-    if (out_node) CU(cudaMemcpy(out_node, S.out_node.p + first, 4ull * count, cudaMemcpyDeviceToHost));
-    if (out_score && S.out_score.p) CU(cudaMemcpy(out_score, S.out_score.p + first, 8ull * count, cudaMemcpyDeviceToHost));
-    uint32_t nf = std::min(std::min(counters[0], max_fail), ctx->max_fail);
-    if (nf && out_fail_counts) CU(cudaMemcpy(out_fail_counts, S.fail_counts.p, 4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
-    if (nf && out_fail_pod) CU(cudaMemcpy(out_fail_pod, S.fail_pod.p, 4ull * nf, cudaMemcpyDeviceToHost));
-    return SIMON_OK;
+    return single_end(ctx, first, count, out_node, out_score, out_fail_counts, out_fail_pod, max_fail, out_n_fail);
 }
 
 int simon_schedule_resume(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n_prefix, int32_t *out_node, int64_t *out_score,
@@ -1098,13 +1168,7 @@ int simon_schedule_resume(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n
     const uint32_t first = n_prefix, count = ctx->n_pods - n_prefix;
     rc = clear_pool(ctx, S);
     if (rc) return rc;
-    CU(cudaMemsetAsync(S.fail_counts.p, 0, 4ull * ctx->max_fail * SIMON_N_FAIL_CODES, st));
-    CU(cudaMemsetAsync(S.counters.p, 0, 8, st));
-    if (ctx->dump_pod >= first && ctx->dump_pod < first + count) {
-        P.dump_pod = ctx->dump_pod; P.dump_total = ctx->d_dump_total.p; P.dump_code = ctx->d_dump_code.p;
-        CU(cudaMemsetAsync(ctx->d_dump_total.p, 0xff, 8ull * std::max(1u, ctx->N), st));     // -1: node not scored (infeasible)
-        CU(cudaMemsetAsync(ctx->d_dump_code.p, 0, 4ull * std::max(1u, ctx->N), st));
-    }
+    CU(single_begin(ctx, P, first, count));
     CU(cudaEventRecord(ctx->ev0, st));
     rc = rebuild_prefix(ctx, P, prefix_node, n_prefix);
     if (rc) return rc;
@@ -1113,19 +1177,7 @@ int simon_schedule_resume(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n
         if (rc) return rc;
     }
     CU(cudaEventRecord(ctx->ev1, st));
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
-    ctx->have_live = true;
-    CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
-    uint32_t counters[2] = {0, 0};
-    CU(cudaMemcpy(counters, S.counters.p, 8, cudaMemcpyDeviceToHost));
-    if (out_n_fail) *out_n_fail = counters[0];
-    if (out_node && ctx->n_pods) CU(cudaMemcpy(out_node, S.out_node.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost));
-    if (out_score && S.out_score.p && ctx->n_pods) CU(cudaMemcpy(out_score, S.out_score.p, 8ull * ctx->n_pods, cudaMemcpyDeviceToHost));
-    uint32_t nf = std::min(std::min(counters[0], max_fail), ctx->max_fail);
-    if (nf && out_fail_counts) CU(cudaMemcpy(out_fail_counts, S.fail_counts.p, 4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
-    if (nf && out_fail_pod) CU(cudaMemcpy(out_fail_pod, S.fail_pod.p, 4ull * nf, cudaMemcpyDeviceToHost));
-    return SIMON_OK;
+    return single_end(ctx, 0, ctx->n_pods, out_node, out_score, out_fail_counts, out_fail_pod, max_fail, out_n_fail);
 }
 
 int simon_replay(simon_ctx *ctx, uint32_t steps, float *out_ms_total) {
@@ -1146,8 +1198,7 @@ int simon_replay(simon_ctx *ctx, uint32_t steps, float *out_ms_total) {
     for (uint32_t s = 0; s < steps; s++) {
         rc = clear_pool(ctx, S);
         if (rc) return rc;
-        CU(cudaMemsetAsync(S.fail_counts.p, 0, 4ull * ctx->max_fail * SIMON_N_FAIL_CODES, st));
-        CU(cudaMemsetAsync(S.counters.p, 0, 8, st));
+        CU(single_begin(ctx, P));
         rc = launch_range(ctx, P, CS, TPB, smem, 0, ctx->n_pods, false);
         if (rc) return rc;
     }
@@ -1180,14 +1231,8 @@ int simon_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *req_mem, in
                          int64_t *nz_mem, int32_t *num_pods) {
     if (!ctx || !ctx->have_pods) return SIMON_ERR_STATE;
     CU(cudaSetDevice(ctx->device));
-    const uint32_t N = ctx->N;
-    const ScenPool &S = ctx->single;
-    if (req_mcpu) CU(cudaMemcpy(req_mcpu, S.req_mcpu.p, 8ull * N, cudaMemcpyDeviceToHost));
-    if (req_mem) CU(cudaMemcpy(req_mem, S.req_mem.p, 8ull * N, cudaMemcpyDeviceToHost));
-    if (req_eph) CU(cudaMemcpy(req_eph, S.req_eph.p, 8ull * N, cudaMemcpyDeviceToHost));
-    if (nz_mcpu) CU(cudaMemcpy(nz_mcpu, S.nz_mcpu.p, 8ull * N, cudaMemcpyDeviceToHost));
-    if (nz_mem) CU(cudaMemcpy(nz_mem, S.nz_mem.p, 8ull * N, cudaMemcpyDeviceToHost));
-    if (num_pods) CU(cudaMemcpy(num_pods, S.num_pods.p, 4ull * N, cudaMemcpyDeviceToHost));
+    void *const dst[NodeState::COLS] = {req_mcpu, req_mem, req_eph, nz_mcpu, nz_mem, num_pods};
+    CU(ctx->single.state.download(dst));
     return SIMON_OK;
 }
 
@@ -1222,7 +1267,7 @@ static int scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n,
     ctx->last_launch = simon_launch_info{};
     cudaStream_t st = ctx->stream;
     if (n == 0) return SIMON_OK;
-    const uint32_t N = ctx->N, N1 = std::max(1u, N);
+    const uint32_t N = ctx->N;
     ScenPool &B = ctx->batch;
     const bool local = out_local != nullptr;
     if (local) B.n_storage = 0;         // the slices are overwritten below
@@ -1234,12 +1279,9 @@ static int scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n,
     // starts from the uploaded VG requested values and device masks ----
     rc = alloc_pool(ctx, B, n, false);
     if (rc) return rc;
-    CU(cudaMemcpyAsync(B.order.p, B.h_order.data(), 4ull * n * N1, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(B.rank_of.p, B.h_rank.data(), 4ull * n * N1, cudaMemcpyHostToDevice, st));
+    std::vector<SkScenario> h;
+    CU(batch_scenarios(ctx, scen, n, h));
     CU(cudaMemsetAsync(B.counters.p, 0, 8ull * n, st)); CU(cudaMemsetAsync(B.clk.p, 0, 16ull * n, st));
-    std::vector<SkScenario> h(n);
-    for (uint32_t i = 0; i < n; i++)     // all N nodes in index order (distinct, so sorted) need no node list
-        h[i] = fill_scen(B, i, scen[i].n_nodes, scen[i].n_nodes == N && std::is_sorted(scen[i].nodes, scen[i].nodes + N));
     CU(B.scen.upload(h.data(), n, st));
     uint32_t CS, TPB, NPT;
     size_t smem;
@@ -1302,15 +1344,9 @@ int simon_scenarios_storage_download(simon_ctx *ctx, uint32_t scenario, int64_t 
 // its per-node arrays in global memory (the node arrays of one cluster per scenario).  Engine.drain_run keeps the margin for them by
 // sizing a batch to a fraction of the free memory.
 static uint64_t drain_scenario_bytes(const simon_ctx *ctx) {
-    const uint64_t nodes = std::max(1u, ctx->N), scal = (uint64_t)(ctx->K ? ctx->K : 1) * nodes, cntw = std::max<uint64_t>(1, ctx->cnt_words);
-    const uint64_t nct = std::max(1u, ctx->n_counters), ncl = std::max(1u, ctx->n_classes);
-    const uint64_t tabw = (uint64_t)SK_MAX_SOFT * ctx->max_dom, regw = (uint64_t)SK_MAX_HARD * ctx->max_dom;
-    uint64_t b = 8 * nodes * 5 + 8 * scal + 8 * nodes * SIMON_MAX_GPU_DEV + 4 * nodes + 4 * cntw + 4 * nct;   // requests .. counter totals
-    b += 4 * tabw * 2 + 4 * SK_MAX_SOFT + regw;                                                                 // tp, fcount, size, hard_reg
-    b += 8 * ncl * SK_CSUM_W + nodes * ncl + 8 * nodes * ncl;                                                   // csum, fbits, ocache
-    b += 4 + 8 + 16 + sizeof(SkScenario) + 4 * nodes * 2 + sizeof(simon_scenario_result);                       // out_node .. results
-    if (ctx->have_storage) b += sizeof(simon_scenario_local_result) + 8 * std::max<uint64_t>(1, (uint64_t)ctx->V * ctx->N) + 4 * nodes;
-    if (ctx->have_devices) b += 4 * nodes;
+    ScenPool shape;         // shaped, never allocated
+    uint64_t b = 0;
+    pool_columns(ctx, shape, 1, false, false, [&](auto &c, size_t k) { b += k * sizeof(*c.p); return cudaSuccess; });
     return b;
 }
 
@@ -1405,11 +1441,9 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
     CU(ctx->d_dr_node.alloc(n_ev)); CU(ctx->d_dr_gpu.alloc(n_ev));
     if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(ctx->d_dr_score.alloc(n_ev));
     CU(ctx->d_dr_fail_counts.alloc((size_t)n * ctx->dr_max * SIMON_N_FAIL_CODES)); CU(ctx->d_dr_fail_pod.alloc((size_t)n * ctx->dr_max));
-    CU(cudaMemcpyAsync(B.order.p, B.h_order.data(), 4ull * n * N1, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(B.rank_of.p, B.h_rank.data(), 4ull * n * N1, cudaMemcpyHostToDevice, st));
-    std::vector<SkScenario> h(n);
+    std::vector<SkScenario> h;
+    CU(batch_scenarios(ctx, remain, n, h));
     for (uint32_t i = 0; i < n; i++) {
-        h[i] = fill_scen(B, i, remain[i].n_nodes, remain[i].n_nodes == N && std::is_sorted(remain[i].nodes, remain[i].nodes + N));
         h[i].out_node = ctx->d_dr_node.p; h[i].out_gpu = ctx->d_dr_gpu.p;
         h[i].out_score = (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) ? ctx->d_dr_score.p : nullptr;
         h[i].fail_counts = ctx->d_dr_fail_counts.p + (size_t)i * ctx->dr_max * SIMON_N_FAIL_CODES;
@@ -1425,21 +1459,15 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
     fill_params(ctx, S, Ps);
     rc = clear_pool(ctx, S);
     if (rc) return rc;
-    CU(cudaMemsetAsync(S.fail_counts.p, 0, 4ull * ctx->max_fail * SIMON_N_FAIL_CODES, st));
-    CU(cudaMemsetAsync(S.counters.p, 0, 8, st));
+    CU(single_begin(ctx, Ps));
     rc = rebuild_prefix(ctx, Ps, placed, P);
     if (rc) return rc;
     CU(cudaMemsetAsync(B.csum.p, 0, 8 * n * B.ncl * SK_CSUM_W, st));
     CU(cudaMemsetAsync(B.ocache.p, 0, 8 * n * B.nodes * B.ncl, st));
     CU(cudaMemsetAsync(B.counters.p, 0, 8ull * n, st)); CU(cudaMemsetAsync(B.clk.p, 0, 16ull * n, st));
     CU(cudaMemsetAsync(ctx->d_dr_fail_counts.p, 0, 4ull * n * ctx->dr_max * SIMON_N_FAIL_CODES, st));
-    CU(bcast(ctx, S.req_mcpu.p, S.nodes, n, B.req_mcpu.p)); CU(bcast(ctx, S.req_mem.p, S.nodes, n, B.req_mem.p));
-    CU(bcast(ctx, S.req_eph.p, S.nodes, n, B.req_eph.p)); CU(bcast(ctx, S.nz_mcpu.p, S.nodes, n, B.nz_mcpu.p));
-    CU(bcast(ctx, S.nz_mem.p, S.nodes, n, B.nz_mem.p)); CU(bcast(ctx, S.num_pods.p, S.nodes, n, B.num_pods.p));
-    CU(bcast(ctx, S.req_scalar.p, S.scal, n, B.req_scalar.p));
-    CU(bcast(ctx, S.gpu_used.p, S.nodes * SIMON_MAX_GPU_DEV, n, B.gpu_used.p));
-    CU(bcast(ctx, S.cnt.p, S.cntw, n, B.cnt.p)); CU(bcast(ctx, S.cnt_total.p, S.nct, n, B.cnt_total.p));
-    ctx->launches += 10;
+    // every slot = the live state, one broadcast per column
+    CU(B.state.each(S.state, true, [&](auto &b, auto &s, uint64_t k) { ctx->launches++; return bcast(ctx, s.p, k, n, b.p); }));
     SkParams Pb;
     fill_params(ctx, B, Pb);
     if (!pairs.empty()) {
@@ -1535,9 +1563,8 @@ int simon_gpu_slots_download(simon_ctx *ctx, uint32_t first, uint32_t count, uin
 int simon_state_download_ext(simon_ctx *ctx, int64_t *req_scalar, int64_t *gpu_used) {
     if (!ctx || !ctx->have_pods) return SIMON_ERR_STATE;
     CU(cudaSetDevice(ctx->device));
-    const uint32_t N = ctx->N;
-    if (req_scalar && ctx->K) CU(cudaMemcpy(req_scalar, ctx->single.req_scalar.p, 8ull * ctx->K * N, cudaMemcpyDeviceToHost));
-    if (gpu_used) CU(cudaMemcpy(gpu_used, ctx->single.gpu_used.p, 8ull * SIMON_MAX_GPU_DEV * N, cudaMemcpyDeviceToHost));
+    void *const dst[NodeState::COLS] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, req_scalar, gpu_used};
+    CU(ctx->single.state.download(dst));
     return SIMON_OK;
 }
 
@@ -1711,50 +1738,68 @@ static int moves_scope_refresh(simon_ctx *ctx) {
     return SIMON_OK;
 }
 
-static int moves_launch(simon_ctx *ctx, bool record) {
+// The move kernel's parameters for the uploaded move list, under the current scope, on copy 0 of node state s with that placement
+static SmvParams moves_params(const simon_ctx *ctx, const NodeState &s, const int32_t *placement, uint32_t move_base) {
+    SmvParams P;
+    memset(&P, 0, sizeof(P));
+    P.N = ctx->N; P.K = ctx->K; P.WT = ctx->WT; P.T = ctx->T; P.n_pods = ctx->n_pods; P.n_moves = ctx->mv_n; P.use_scache = ctx->use_scache;
+    P.nodes = ctx->d_mv_nodes.p; P.alloc_scalar = ctx->d_alloc_scalar.p; P.req_scalar = s.req_scalar.p; P.node_flags = ctx->d_node_flags.p;
+    P.label_bits = ctx->d_label_bits.p; P.taint_hard = ctx->d_taint_hard.p; P.topo_dom = ctx->d_topo_dom.p; P.pods = ctx->d_mv_pods.p;
+    P.class_off = ctx->d_class_off.p; P.class_blob = ctx->d_class_blob.p; P.classes = ctx->d_mv_classes.p; P.pod_class = ctx->d_pod_class.p; P.placement = placement;
+    P.cnt = s.cnt.p; P.cnt_total = s.cnt_total.p; P.scache = ctx->d_scache.p; P.moves = ctx->d_moves.p;
+    P.out_gain = ctx->d_mv_gain.p; P.out_code = ctx->d_mv_code.p; P.best_per_pod = ctx->d_mv_best_pod.p; P.best_global = ctx->d_mv_best.p;
+    P.hist = ctx->d_mv_hist.p; P.move_base = move_base;
+    P.scope = ctx->mv_scope; P.gpu = ctx->d_mv_gpu.p; P.hs = ctx->d_mv_hs.p; P.hreg = ctx->d_mv_hreg.p;
+    P.out_slots = (ctx->mv_scope & SIMON_MOVES_SCOPE_GPU_SHARE) ? ctx->d_mv_slots.p : nullptr;
+    return P;
+}
+
+// Enqueue the packed records of copy 0 of node state s with that placement: SmvNode / SmvPod, and SmvGpu when gpu (GPU share scored).
+// Only the SmvGpu pack is counted in simon_launch_count here; simon_moves_plan counts the other, simon_moves_run never has.
+static void moves_pack(simon_ctx *ctx, const NodeState &s, const int32_t *placement, bool gpu) {
     cudaStream_t st = ctx->stream;
-    const uint32_t N = ctx->N, n = ctx->mv_n, scope = ctx->mv_scope;
-    const bool scoped = ctx->mv_scoped;
-    const ScenPool &S = ctx->single;
-    if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && n) CU(ctx->d_mv_slots.alloc(n));
-    if (record) CU(cudaEventRecord(ctx->ev0, st));
-    if (scoped && (scope & SIMON_MOVES_SCOPE_GPU_SHARE) && N) {
-        CU(ctx->d_mv_gpu.alloc(N));
+    const uint32_t N = ctx->N;
+    if (gpu) {
         simon_moves_pack_gpu<<<(N + 255) / 256, 256, 0, st>>>(N, ctx->d_gpu_count.p, ctx->d_gpu_dev_mem.p, ctx->d_gpu_total_mem.p,
-                                                               S.gpu_used.p, ctx->d_mv_gpu.p);
+                                                               s.gpu_used.p, ctx->d_mv_gpu.p);
         ctx->launches++;
     }
-    if (scoped && ctx->mv_n_prep) {
-        simon_moves_hard_prep<<<ctx->mv_n_prep, 256, 0, st>>>(N, ctx->use_scache, ctx->d_scache.p, ctx->d_label_bits.p, ctx->d_topo_dom.p,
-                                                              ctx->d_topo_ndom.p, ctx->d_class_off.p, ctx->d_class_blob.p, S.cnt.p,
+    simon_moves_pack<<<std::max(std::max(1u, (N + 255) / 256), std::min(1184u, (ctx->n_pods + 255) / 256)), 256, 0, st>>>(N, ctx->T, ctx->d_alloc_mcpu.p, ctx->d_alloc_mem.p, ctx->d_alloc_eph.p, ctx->d_alloc_pods.p,
+                                                                     ctx->d_topo_dom.p, s.req_mcpu.p, s.req_mem.p, s.req_eph.p,
+                                                                     s.nz_mcpu.p, s.nz_mem.p, s.num_pods.p, ctx->d_mv_nodes.p,
+                                                                     ctx->d_mv_best_pod.p, ctx->n_pods, ctx->d_mv_best.p, ctx->d_mv_hist.p,
+                                                                     ctx->d_pod_class.p, placement, ctx->d_mv_classes.p, ctx->d_mv_pods.p);
+}
+
+// Enqueue one scoring pass with P (moves_params): the hard-spread prep when the scope admits hard classes, then the move kernel
+static void moves_score(simon_ctx *ctx, const SmvParams &P) {
+    cudaStream_t st = ctx->stream;
+    if (ctx->mv_scoped && ctx->mv_n_prep) {
+        simon_moves_hard_prep<<<ctx->mv_n_prep, 256, 0, st>>>(ctx->N, ctx->use_scache, ctx->d_scache.p, ctx->d_label_bits.p, ctx->d_topo_dom.p,
+                                                              ctx->d_topo_ndom.p, ctx->d_class_off.p, ctx->d_class_blob.p, P.cnt,
                                                               ctx->d_mv_prep.p, ctx->d_mv_hreg.p, ctx->d_mv_hs.p);
         ctx->launches++;
     }
-    if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && !scoped && n) CU(cudaMemsetAsync(ctx->d_mv_slots.p, 0, 4ull * n, st));
-    simon_moves_pack<<<std::max(std::max(1u, (N + 255) / 256), std::min(1184u, (ctx->n_pods + 255) / 256)), 256, 0, st>>>(N, ctx->T, ctx->d_alloc_mcpu.p, ctx->d_alloc_mem.p, ctx->d_alloc_eph.p, ctx->d_alloc_pods.p,
-                                                                     ctx->d_topo_dom.p, S.req_mcpu.p, S.req_mem.p, S.req_eph.p,
-                                                                     S.nz_mcpu.p, S.nz_mem.p, S.num_pods.p, ctx->d_mv_nodes.p,
-                                                                     ctx->d_mv_best_pod.p, ctx->n_pods, ctx->d_mv_best.p, ctx->d_mv_hist.p,
-                                                                     ctx->d_pod_class.p, S.out_node.p, ctx->d_mv_classes.p, ctx->d_mv_pods.p);
-    SmvParams P;
-    memset(&P, 0, sizeof(P));
-    P.N = N; P.K = ctx->K; P.WT = ctx->WT; P.T = ctx->T; P.n_pods = ctx->n_pods; P.n_moves = n; P.use_scache = ctx->use_scache;
-    P.nodes = ctx->d_mv_nodes.p; P.alloc_scalar = ctx->d_alloc_scalar.p; P.req_scalar = S.req_scalar.p; P.node_flags = ctx->d_node_flags.p;
-    P.label_bits = ctx->d_label_bits.p; P.taint_hard = ctx->d_taint_hard.p; P.topo_dom = ctx->d_topo_dom.p;
-    P.pods = ctx->d_mv_pods.p;
-    P.class_off = ctx->d_class_off.p; P.class_blob = ctx->d_class_blob.p; P.classes = ctx->d_mv_classes.p; P.pod_class = ctx->d_pod_class.p; P.placement = S.out_node.p;
-    P.cnt = S.cnt.p; P.cnt_total = S.cnt_total.p; P.scache = ctx->d_scache.p; P.moves = ctx->d_moves.p;
-    P.out_gain = ctx->d_mv_gain.p; P.out_code = ctx->d_mv_code.p; P.best_per_pod = ctx->d_mv_best_pod.p; P.best_global = ctx->d_mv_best.p;
-    P.hist = ctx->d_mv_hist.p; P.move_base = ctx->mv_base;
-    P.scope = scope; P.gpu = ctx->d_mv_gpu.p; P.hs = ctx->d_mv_hs.p; P.hreg = ctx->d_mv_hreg.p;
-    P.out_slots = (scope & SIMON_MOVES_SCOPE_GPU_SHARE) ? ctx->d_mv_slots.p : nullptr;
-    if (n) {
+    if (P.n_moves) {
         // 4 resident CTAs per SM (64 registers, a few spills), two rounds of them
-        const uint32_t grid = std::min<uint32_t>((n + 255) / 256, (uint32_t)ctx->sms * 4u * 2u);
-        if (scoped) simon_moves_kernel<4, true><<<grid, 256, 0, st>>>(P);
+        const uint32_t grid = std::min<uint32_t>((P.n_moves + 255) / 256, (uint32_t)ctx->sms * 4u * 2u);
+        if (ctx->mv_scoped) simon_moves_kernel<4, true><<<grid, 256, 0, st>>>(P);
         else simon_moves_kernel<4, false><<<grid, 256, 0, st>>>(P);
         ctx->launches++;
     }
+}
+
+static int moves_launch(simon_ctx *ctx, bool record) {
+    cudaStream_t st = ctx->stream;
+    const uint32_t N = ctx->N, n = ctx->mv_n, scope = ctx->mv_scope;
+    const bool gpu = ctx->mv_scoped && (scope & SIMON_MOVES_SCOPE_GPU_SHARE) && N;
+    const ScenPool &S = ctx->single;
+    if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && n) CU(ctx->d_mv_slots.alloc(n));
+    if (gpu) CU(ctx->d_mv_gpu.alloc(N));
+    if (record) CU(cudaEventRecord(ctx->ev0, st));
+    if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && !ctx->mv_scoped && n) CU(cudaMemsetAsync(ctx->d_mv_slots.p, 0, 4ull * n, st));
+    moves_pack(ctx, S.state, S.out_node.p, gpu);
+    moves_score(ctx, moves_params(ctx, S.state, S.out_node.p, ctx->mv_base));
     if (record) CU(cudaEventRecord(ctx->ev1, st));
     CU(cudaGetLastError());
     return SIMON_OK;
@@ -1896,91 +1941,50 @@ int simon_moves_plan(simon_ctx *ctx, uint32_t max_moves, int32_t min_gain, simon
     ctx->mv_ran = false;            // the per-move slots are overwritten
     ctx->pl_valid = false;
     cudaStream_t st = ctx->stream;
-    const ScenPool &S = ctx->single;
+    ScenPool &S = ctx->single;
+    NodeState &pl = ctx->pl_state;
     const uint32_t N = ctx->N, P = ctx->n_pods, n = ctx->mv_n, scope = ctx->mv_scope;
-    const bool scoped = ctx->mv_scoped, gpu = scoped && (scope & SIMON_MOVES_SCOPE_GPU_SHARE) && N;
-    const size_t nn = S.nodes, P1 = std::max(1u, P);
+    const bool gpu = ctx->mv_scoped && (scope & SIMON_MOVES_SCOPE_GPU_SHARE) && N;
+    const size_t P1 = std::max(1u, P);
     const uint32_t cap = (uint32_t)std::min<uint64_t>(max_moves, P1);
-    CU(ctx->d_pl_req_mcpu.alloc(nn)); CU(ctx->d_pl_req_mem.alloc(nn)); CU(ctx->d_pl_req_eph.alloc(nn));
-    CU(ctx->d_pl_nz_mcpu.alloc(nn)); CU(ctx->d_pl_nz_mem.alloc(nn)); CU(ctx->d_pl_num_pods.alloc(nn));
-    CU(ctx->d_pl_req_scalar.alloc(S.scal)); CU(ctx->d_pl_gpu_used.alloc(nn * SIMON_MAX_GPU_DEV));
-    CU(ctx->d_pl_cnt.alloc(S.cntw)); CU(ctx->d_pl_cnt_total.alloc(S.nct));
-    CU(ctx->d_pl_place.alloc(P1)); CU(ctx->d_pl_slots.alloc(P1)); CU(ctx->d_pl_ctl.alloc(4)); CU(ctx->d_pl_steps.alloc(cap));
+    pl.shape(1, N, ctx->K, ctx->cnt_words, ctx->n_counters);
+    CU(pl.alloc());
+    CU(ctx->pl_place.alloc(P1)); CU(ctx->pl_slots.alloc(P1)); CU(ctx->pl_ctl.alloc(4)); CU(ctx->pl_steps.alloc(cap));
     if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && n) CU(ctx->d_mv_slots.alloc(n));
     if (gpu) CU(ctx->d_mv_gpu.alloc(N));
     CU(cudaEventRecord(ctx->ev0, st));
-    CU(cudaMemcpyAsync(ctx->d_pl_req_mcpu.p, S.req_mcpu.p, 8 * nn, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pl_req_mem.p, S.req_mem.p, 8 * nn, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pl_req_eph.p, S.req_eph.p, 8 * nn, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pl_nz_mcpu.p, S.nz_mcpu.p, 8 * nn, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pl_nz_mem.p, S.nz_mem.p, 8 * nn, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pl_num_pods.p, S.num_pods.p, 4 * nn, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pl_req_scalar.p, S.req_scalar.p, 8 * S.scal, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pl_gpu_used.p, S.gpu_used.p, 8 * nn * SIMON_MAX_GPU_DEV, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pl_cnt.p, S.cnt.p, 4 * S.cntw, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pl_cnt_total.p, S.cnt_total.p, 4 * S.nct, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pl_place.p, S.out_node.p, 4 * P1, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(ctx->d_pl_slots.p, S.out_gpu.p, 4 * P1, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemsetAsync(ctx->d_pl_ctl.p, 0, 16, st));
+    CU(pl.copy(S.state, st));
+    CU(cudaMemcpyAsync(ctx->pl_place.p, S.out_node.p, 4 * P1, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(ctx->pl_slots.p, S.out_gpu.p, 4 * P1, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemsetAsync(ctx->pl_ctl.p, 0, 16, st));
     // ---- setup: the packed records of the plan state, once ----
-    if (gpu) {
-        simon_moves_pack_gpu<<<(N + 255) / 256, 256, 0, st>>>(N, ctx->d_gpu_count.p, ctx->d_gpu_dev_mem.p, ctx->d_gpu_total_mem.p,
-                                                               ctx->d_pl_gpu_used.p, ctx->d_mv_gpu.p);
-        ctx->launches++;
-    }
-    simon_moves_pack<<<std::max(std::max(1u, (N + 255) / 256), std::min(1184u, (P + 255) / 256)), 256, 0, st>>>(N, ctx->T, ctx->d_alloc_mcpu.p, ctx->d_alloc_mem.p, ctx->d_alloc_eph.p, ctx->d_alloc_pods.p,
-                                                                 ctx->d_topo_dom.p, ctx->d_pl_req_mcpu.p, ctx->d_pl_req_mem.p, ctx->d_pl_req_eph.p,
-                                                                 ctx->d_pl_nz_mcpu.p, ctx->d_pl_nz_mem.p, ctx->d_pl_num_pods.p, ctx->d_mv_nodes.p,
-                                                                 ctx->d_mv_best_pod.p, P, ctx->d_mv_best.p, ctx->d_mv_hist.p,
-                                                                 ctx->d_pod_class.p, ctx->d_pl_place.p, ctx->d_mv_classes.p, ctx->d_mv_pods.p);
-    simon_moves_plan_setup<<<std::max(1u, std::min(1184u, (P + 255) / 256)), 256, 0, st>>>(P, ctx->d_pl_slots.p, ctx->d_mv_pods.p, ctx->d_pl_ctl.p);
-    ctx->launches += 2;
+    moves_pack(ctx, pl, ctx->pl_place.p, gpu);
+    simon_moves_plan_setup<<<std::max(1u, std::min(1184u, (P + 255) / 256)), 256, 0, st>>>(P, ctx->pl_slots.p, ctx->d_mv_pods.p, ctx->pl_ctl.p);
+    ctx->launches += 2;             // the pack and the setup
     CU(cudaGetLastError());
-    SmvParams M;
-    memset(&M, 0, sizeof(M));
-    M.N = N; M.K = ctx->K; M.WT = ctx->WT; M.T = ctx->T; M.n_pods = P; M.n_moves = n; M.use_scache = ctx->use_scache;
-    M.nodes = ctx->d_mv_nodes.p; M.alloc_scalar = ctx->d_alloc_scalar.p; M.req_scalar = ctx->d_pl_req_scalar.p; M.node_flags = ctx->d_node_flags.p;
-    M.label_bits = ctx->d_label_bits.p; M.taint_hard = ctx->d_taint_hard.p; M.topo_dom = ctx->d_topo_dom.p;
-    M.pods = ctx->d_mv_pods.p;
-    M.class_off = ctx->d_class_off.p; M.class_blob = ctx->d_class_blob.p; M.classes = ctx->d_mv_classes.p; M.pod_class = ctx->d_pod_class.p;
-    M.placement = ctx->d_pl_place.p;
-    M.cnt = ctx->d_pl_cnt.p; M.cnt_total = ctx->d_pl_cnt_total.p; M.scache = ctx->d_scache.p; M.moves = ctx->d_moves.p;
-    M.out_gain = ctx->d_mv_gain.p; M.out_code = ctx->d_mv_code.p; M.best_per_pod = ctx->d_mv_best_pod.p; M.best_global = ctx->d_mv_best.p;
-    M.hist = ctx->d_mv_hist.p; M.move_base = 0;
-    M.scope = scope; M.gpu = ctx->d_mv_gpu.p; M.hs = ctx->d_mv_hs.p; M.hreg = ctx->d_mv_hreg.p;
-    M.out_slots = (scope & SIMON_MOVES_SCOPE_GPU_SHARE) ? ctx->d_mv_slots.p : nullptr;
+    const SmvParams M = moves_params(ctx, pl, ctx->pl_place.p, 0);
     SkParams Pk;
     fill_params(ctx, S, Pk);
     SmvPlan Q;
     memset(&Q, 0, sizeof(Q));
     Q.max_moves = max_moves; Q.min_gain = min_gain;
-    Q.req_mcpu = ctx->d_pl_req_mcpu.p; Q.req_mem = ctx->d_pl_req_mem.p; Q.req_eph = ctx->d_pl_req_eph.p;
-    Q.nz_mcpu = ctx->d_pl_nz_mcpu.p; Q.nz_mem = ctx->d_pl_nz_mem.p; Q.req_scalar = ctx->d_pl_req_scalar.p; Q.gpu_used = ctx->d_pl_gpu_used.p;
-    Q.num_pods = ctx->d_pl_num_pods.p; Q.cnt = ctx->d_pl_cnt.p; Q.cnt_total = ctx->d_pl_cnt_total.p; Q.place = ctx->d_pl_place.p;
-    Q.slots = ctx->d_pl_slots.p; Q.moves = ctx->d_moves.p; Q.mv_slots = M.out_slots;
+    pl.slice(0, Q);
+    Q.place = ctx->pl_place.p; Q.slots = ctx->pl_slots.p; Q.moves = ctx->d_moves.p; Q.mv_slots = M.out_slots;
     Q.best_global = ctx->d_mv_best.p; Q.hist = ctx->d_mv_hist.p; Q.nodes = ctx->d_mv_nodes.p; Q.gpu = gpu ? ctx->d_mv_gpu.p : nullptr;
-    Q.pods = ctx->d_mv_pods.p; Q.steps = ctx->d_pl_steps.p; Q.ctl = ctx->d_pl_ctl.p;
+    Q.pods = ctx->d_mv_pods.p; Q.steps = ctx->pl_steps.p; Q.ctl = ctx->pl_ctl.p;
     // ---- steps: [hard prep] + scoring + apply, in chunks of growing length ----
-    const uint32_t grid = std::min<uint32_t>((n + 255) / 256, (uint32_t)ctx->sms * 4u * 2u);
     const uint64_t limit = std::min<uint64_t>(max_moves, (uint64_t)P + 1);     // after P steps every pod has moved: the next pass stops
     uint32_t ctl[4] = {0, 0, 0, 0};
     uint64_t enq = 0;
     for (uint32_t chunk = 4; enq < limit && !ctl[1]; chunk = std::min(chunk * 2, 64u)) {
         const uint64_t end = std::min<uint64_t>(limit, enq + chunk);
         for (; enq < end; enq++) {
-            if (scoped && ctx->mv_n_prep)
-                simon_moves_hard_prep<<<ctx->mv_n_prep, 256, 0, st>>>(N, ctx->use_scache, ctx->d_scache.p, ctx->d_label_bits.p, ctx->d_topo_dom.p,
-                                                                      ctx->d_topo_ndom.p, ctx->d_class_off.p, ctx->d_class_blob.p, ctx->d_pl_cnt.p,
-                                                                      ctx->d_mv_prep.p, ctx->d_mv_hreg.p, ctx->d_mv_hs.p);
-            if (n) {
-                if (scoped) simon_moves_kernel<4, true><<<grid, 256, 0, st>>>(M);
-                else simon_moves_kernel<4, false><<<grid, 256, 0, st>>>(M);
-            }
+            moves_score(ctx, M);
             simon_moves_plan_apply<<<1, 32, 0, st>>>(Pk, Q);
-            ctx->launches += (scoped && ctx->mv_n_prep ? 1 : 0) + (n ? 1 : 0) + 1;
+            ctx->launches++;
         }
         CU(cudaGetLastError());
-        CU(cudaMemcpyAsync(ctl, ctx->d_pl_ctl.p, 16, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(ctl, ctx->pl_ctl.p, 16, cudaMemcpyDeviceToHost, st));
         cudaError_t e = cudaStreamSynchronize(st);
         if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "move plan failed: %s", cudaGetErrorString(e));
     }
@@ -1991,7 +1995,7 @@ int simon_moves_plan(simon_ctx *ctx, uint32_t max_moves, int32_t min_gain, simon
         return fail(ctx, SIMON_ERR_CUDA, "move plan: inconsistent state at step %u (%s)", ctl[0],
                     ctl[2] == SMV_PLAN_ERR_SLOTS ? "Reserve on the target differs from the scored GPU slots" : "a count of the source node went negative");
     if (!ctl[1]) return fail(ctx, SIMON_ERR_CUDA, "move plan: no stop after %llu steps", (unsigned long long)limit);
-    if (ctl[0]) CU(cudaMemcpy(out_steps, ctx->d_pl_steps.p, sizeof(simon_plan_step) * ctl[0], cudaMemcpyDeviceToHost));
+    if (ctl[0]) CU(cudaMemcpy(out_steps, ctx->pl_steps.p, sizeof(simon_plan_step) * ctl[0], cudaMemcpyDeviceToHost));
     memset(out, 0, sizeof(*out));
     out->n_steps = ctl[0]; out->stop_reason = ctl[1]; out->n_excluded = ctl[3]; out->kernel_ms = ctx->last_ms;
     ctx->pl_valid = true;
@@ -2002,8 +2006,8 @@ int simon_moves_plan_download(simon_ctx *ctx, int32_t *placement, uint32_t *gpu_
     if (!ctx) return SIMON_ERR_INVALID;
     if (!ctx->pl_valid) return fail(ctx, SIMON_ERR_STATE, "no simon_moves_plan since the last upload");
     CU(cudaSetDevice(ctx->device));
-    if (placement && ctx->n_pods) CU(cudaMemcpy(placement, ctx->d_pl_place.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost));
-    if (gpu_slots && ctx->n_pods) CU(cudaMemcpy(gpu_slots, ctx->d_pl_slots.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost));
+    if (placement && ctx->n_pods) CU(cudaMemcpy(placement, ctx->pl_place.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost));
+    if (gpu_slots && ctx->n_pods) CU(cudaMemcpy(gpu_slots, ctx->pl_slots.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
@@ -2012,15 +2016,8 @@ int simon_moves_plan_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *
     if (!ctx) return SIMON_ERR_INVALID;
     if (!ctx->pl_valid) return fail(ctx, SIMON_ERR_STATE, "no simon_moves_plan since the last upload");
     CU(cudaSetDevice(ctx->device));
-    const uint64_t N = ctx->N;
-    if (req_mcpu) CU(cudaMemcpy(req_mcpu, ctx->d_pl_req_mcpu.p, 8 * N, cudaMemcpyDeviceToHost));
-    if (req_mem) CU(cudaMemcpy(req_mem, ctx->d_pl_req_mem.p, 8 * N, cudaMemcpyDeviceToHost));
-    if (req_eph) CU(cudaMemcpy(req_eph, ctx->d_pl_req_eph.p, 8 * N, cudaMemcpyDeviceToHost));
-    if (nz_mcpu) CU(cudaMemcpy(nz_mcpu, ctx->d_pl_nz_mcpu.p, 8 * N, cudaMemcpyDeviceToHost));
-    if (nz_mem) CU(cudaMemcpy(nz_mem, ctx->d_pl_nz_mem.p, 8 * N, cudaMemcpyDeviceToHost));
-    if (num_pods) CU(cudaMemcpy(num_pods, ctx->d_pl_num_pods.p, 4 * N, cudaMemcpyDeviceToHost));
-    if (req_scalar && ctx->K) CU(cudaMemcpy(req_scalar, ctx->d_pl_req_scalar.p, 8 * ctx->K * N, cudaMemcpyDeviceToHost));
-    if (gpu_used) CU(cudaMemcpy(gpu_used, ctx->d_pl_gpu_used.p, 8 * SIMON_MAX_GPU_DEV * N, cudaMemcpyDeviceToHost));
+    void *const dst[NodeState::COLS] = {req_mcpu, req_mem, req_eph, nz_mcpu, nz_mem, num_pods, req_scalar, gpu_used};
+    CU(ctx->pl_state.download(dst));
     return SIMON_OK;
 }
 

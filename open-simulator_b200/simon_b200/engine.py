@@ -261,11 +261,20 @@ class Engine:
                     node_slots=li.node_slots, n_scenarios=li.n_scenarios, large=bool(li.large), local=bool(li.local),
                     smem_bytes=int(li.smem_bytes))
 
+    def _state(self, download, cols: slice = slice(0, 8)):
+        """The node state through `download` (simon_state_download, simon_state_download_ext or simon_moves_plan_state_download),
+        called with the host arrays of columns `cols` of (req_mcpu, req_mem, req_eph, nz_mcpu, nz_mem, num_pods, req_scalar [K][N],
+        gpu_used [8][N]): -> (state() dict, state_ext() dict)."""
+        N, K = self.c.n_nodes, int(self.c.snap_dims["n_scalars"])
+        N1 = max(N, 1)
+        arrs = [np.zeros(N1, np.int64) for _ in range(5)] + [np.zeros(N1, np.int32), np.zeros((max(K, 1), N1), np.int64),
+                                                             np.zeros((8, N1), np.int64)]
+        self._check(download(self.h, *[a.ctypes.data for a in arrs[cols]]))
+        return (dict(zip(["req_mcpu", "req_mem", "req_eph", "nz_mcpu", "nz_mem", "num_pods"], [a[:N] for a in arrs[:6]])),
+                dict(req_scalar=arrs[6][:K, :N], gpu_used=arrs[7][:, :N]))
+
     def state(self):
-        N = self.c.n_nodes
-        arrs = [np.zeros(N, np.int64) for _ in range(5)] + [np.zeros(N, np.int32)]
-        self._check(lib().simon_state_download(self.h, *[a.ctypes.data for a in arrs]))
-        return dict(zip(["req_mcpu", "req_mem", "req_eph", "nz_mcpu", "nz_mem", "num_pods"], arrs))
+        return self._state(lib().simon_state_download, slice(0, 6))[0]
 
     def storage_state(self) -> np.ndarray:
         """Open-Local VG requested after scheduling, [V][N]."""
@@ -297,11 +306,7 @@ class Engine:
         return out
 
     def state_ext(self):
-        N, K = self.c.n_nodes, int(self.c.snap_dims["n_scalars"])
-        rs = np.zeros((max(K, 1), max(N, 1)), np.int64)
-        gu = np.zeros((8, max(N, 1)), np.int64)
-        self._check(lib().simon_state_download_ext(self.h, rs.ctypes.data, gu.ctypes.data))
-        return dict(req_scalar=rs[:K, :N], gpu_used=gu[:, :N])
+        return self._state(lib().simon_state_download_ext, slice(6, 8))[1]
 
     def dump_pod(self, pod: int, placed: Optional[np.ndarray] = None):
         """From the EMPTY state, schedule up to and including `pod`; return (out_node of the range, per-node totals,
@@ -380,13 +385,7 @@ class Engine:
 
     def moves_plan_state(self):
         """After moves_plan: the plan's end state as (state(), state_ext()) dicts."""
-        N, K = self.c.n_nodes, int(self.c.snap_dims["n_scalars"])
-        arrs = [np.zeros(max(N, 1), np.int64) for _ in range(5)] + [np.zeros(max(N, 1), np.int32)]
-        rs = np.zeros((max(K, 1), max(N, 1)), np.int64)
-        gu = np.zeros((8, max(N, 1)), np.int64)
-        self._check(lib().simon_moves_plan_state_download(self.h, *[a.ctypes.data for a in arrs], rs.ctypes.data, gu.ctypes.data))
-        st = dict(zip(["req_mcpu", "req_mem", "req_eph", "nz_mcpu", "nz_mem", "num_pods"], [a[:N] for a in arrs]))
-        return st, dict(req_scalar=rs[:K, :N], gpu_used=gu[:, :N])
+        return self._state(lib().simon_moves_plan_state_download)
 
     def run_scenarios(self, scenarios: List[np.ndarray], want_nodes: bool = False):
         """scenarios: list of uint32 arrays (active node indices in scenario order)."""
@@ -398,15 +397,19 @@ class Engine:
         annotated nodes after the run (satisfyResourceSetting's MaxVG input)."""
         return self._run_scenarios(scenarios, want_nodes, True)
 
+    @staticmethod
+    def _scenario_array(node_lists):
+        """(SimonScenario array over node_lists, the uint32 arrays it points into: keep them alive for the call)."""
+        arr = (abi.SimonScenario * len(node_lists))()
+        keep = [np.ascontiguousarray(nodes, dtype=np.uint32) for nodes in node_lists]
+        for s, a in zip(arr, keep):
+            s.n_nodes = len(a)
+            s.nodes = a.ctypes.data if len(a) else None
+        return arr, keep
+
     def _run_scenarios(self, scenarios, want_nodes, local):
         n = len(scenarios)
-        arr = (abi.SimonScenario * n)()
-        keep = []
-        for i, nodes in enumerate(scenarios):
-            a = np.ascontiguousarray(nodes, dtype=np.uint32)
-            keep.append(a)
-            arr[i].n_nodes = len(a)
-            arr[i].nodes = a.ctypes.data
+        arr, keep = self._scenario_array(scenarios)
         res = (abi.SimonScenarioResult * n)()
         P = self.c.pods_dims["n_pods"]
         out_node = np.full((n, P), -9, np.int32) if want_nodes else None
@@ -461,13 +464,7 @@ class Engine:
         for b in range(0, n, chunk):
             part = remain_lists[b:b + chunk]
             m = len(part)
-            arr = (abi.SimonScenario * m)()
-            keep = []
-            for i, nodes in enumerate(part):
-                a = np.ascontiguousarray(nodes, dtype=np.uint32)
-                keep.append(a)
-                arr[i].n_nodes = len(a)
-                arr[i].nodes = a.ctypes.data if len(a) else None
+            arr, keep = self._scenario_array(part)
             res = (abi.SimonDrainResult * m)()
             self._check(L.simon_drain_run(self.h, pl.ctypes.data, arr, m, res))
             su, pm = C.c_float(0), C.c_float(0)
