@@ -14,6 +14,7 @@
 
 #include "simon_kernel.cu"   // single translation unit: kernel + host API
 #include "simon_moves.cu"    // candidate-move scoring kernels (config 5)
+#include "simon_pdb.cuh"     // PodDisruptionBudget counts and marks (drains, move runs, plans): kernels in simon_pdb.cu
 
 namespace {
 
@@ -336,6 +337,15 @@ struct simon_ctx {
     DevBuf<int64_t> d_dr_score;
     DevBuf<uint2> d_dr_pairs;
     float dr_setup_ms = 0.f, dr_place_ms = 0.f;
+    // PodDisruptionBudgets (simon_pdbs_upload; n_pdbs 0: no table): the pod -> PDB CSR (also on the host, for drains), the PDB -> pod
+    // CSR and the desired counts; d_pdb_rem holds `allowed` of the last computation, and a plan's remaining budgets; d_pdb_ctl the
+    // plan's step watch (seen steps, PDBs that reached 0, blocked pods), d_pdb_hit the ids of those PDBs
+    uint32_t n_pdbs = 0, pdb_max_per_pod = 0, pdb_max_members = 0;
+    std::vector<uint32_t> h_pdb_off, h_pdb_ids;
+    DevBuf<uint32_t> d_pdb_off, d_pdb_ids, d_pdb_moff, d_pdb_members, d_pdb_ctl, d_pdb_hit;
+    DevBuf<int32_t> d_pdb_desired, d_pdb_rem;
+    // per drain of the last batch: its violated PDBs, ascending, and their evicted members (CSR dr_voff)
+    std::vector<uint32_t> dr_voff, dr_vpdb, dr_vcnt;
 };
 
 namespace {
@@ -824,6 +834,20 @@ cudaError_t batch_scenarios(simon_ctx *ctx, const simon_scenario *scen, uint32_t
     return e != cudaSuccess ? e : cudaMemcpyAsync(B.rank_of.p, B.h_rank.data(), bytes, cudaMemcpyHostToDevice, ctx->stream);
 }
 
+// With a PDB table: enqueue allowed[j] = max(0, placed members of j - desired[j]) on `placement` into d_pdb_rem
+cudaError_t pdb_allowed(simon_ctx *ctx, const int32_t *placement) {
+    ctx->launches += 2;
+    return simon_pdb_launch_allowed(ctx->stream, ctx->sms * 4u, ctx->n_pods, placement, ctx->d_pdb_off.p, ctx->d_pdb_ids.p, ctx->n_pdbs,
+                                    ctx->d_pdb_desired.p, ctx->d_pdb_rem.p);
+}
+
+// With a PDB table: after the pack of SmvPod records, the pods of PDBs without budget (d_pdb_rem <= 0) become never movable
+cudaError_t pdb_mark(simon_ctx *ctx, uint32_t *blocked) {
+    ctx->launches++;
+    return simon_pdb_launch_mark(ctx->stream, ctx->sms * 4u, ctx->n_pods, ctx->d_pdb_off.p, ctx->d_pdb_ids.p, ctx->d_pdb_rem.p,
+                                 ctx->d_mv_pods.p, blocked);
+}
+
 }  // namespace
 
 extern "C" {
@@ -897,6 +921,7 @@ int simon_snapshot_upload(simon_ctx *ctx, const simon_snapshot *s) {
     ctx->batch.n_storage = 0;
     ctx->dr_n = 0;
     ctx->have_live = ctx->pl_valid = false;
+    ctx->n_pdbs = 0;
     return SIMON_OK;
 }
 
@@ -910,6 +935,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     ctx->batch.n_storage = 0;
     ctx->dr_n = 0;
     ctx->have_live = ctx->pl_valid = false;
+    ctx->n_pdbs = 0;                    // the PDB table is per pod: a new pod set needs its own upload
     ctx->n_classes = p->n_classes; ctx->n_pods = p->n_pods; ctx->n_counters = p->n_counters;
     // validate classes; derive limits
     uint32_t max_words = SCW_HDR_WORDS, emax = 0;
@@ -1487,19 +1513,45 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
     CU(cudaGetLastError());
     std::vector<simon_scenario_result> res(n);
     CU(cudaMemcpyAsync(res.data(), B.results.p, sizeof(simon_scenario_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    // with a PDB table: `allowed` on the rebuilt live state, read at the same synchronisation
+    std::vector<int32_t> allowed(ctx->n_pdbs);
+    if (ctx->n_pdbs) {
+        CU(pdb_allowed(ctx, S.out_node.p));
+        CU(cudaMemcpyAsync(allowed.data(), ctx->d_pdb_rem.p, 4ull * ctx->n_pdbs, cudaMemcpyDeviceToHost, st));
+    }
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
     ctx->have_live = true;
     CU(cudaEventElapsedTime(&ctx->dr_setup_ms, ctx->ev0, ctx->evm));
     CU(cudaEventElapsedTime(&ctx->dr_place_ms, ctx->evm, ctx->ev1));
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    // violated PDBs per drain: its evicted members per PDB (filterPodsWithPDBViolation's count) above `allowed`
+    ctx->dr_voff.assign(1, 0u); ctx->dr_vpdb.clear(); ctx->dr_vcnt.clear();
+    {
+        std::vector<uint32_t> cnt(ctx->n_pdbs, 0u), touched;
+        for (uint32_t i = 0; i < n && ctx->n_pdbs; i++) {
+            for (uint32_t k = ctx->dr_off[i]; k < ctx->dr_off[i + 1]; k++) {
+                const uint32_t q = ctx->dr_pods[k];
+                for (uint32_t u = ctx->h_pdb_off[q]; u < ctx->h_pdb_off[q + 1]; u++)
+                    if (!cnt[ctx->h_pdb_ids[u]]++) touched.push_back(ctx->h_pdb_ids[u]);
+            }
+            std::sort(touched.begin(), touched.end());
+            for (uint32_t j : touched) {
+                if ((int64_t)cnt[j] > (int64_t)allowed[j]) { ctx->dr_vpdb.push_back(j); ctx->dr_vcnt.push_back(cnt[j]); }
+                cnt[j] = 0;
+            }
+            touched.clear();
+            ctx->dr_voff.push_back((uint32_t)ctx->dr_vpdb.size());
+        }
+        if (!ctx->n_pdbs) ctx->dr_voff.assign(n + 1, 0u);
+    }
     ctx->dr_nfail.resize(n);
     for (uint32_t i = 0; i < n; i++) {
         simon_drain_result &o = out[i];
         o.n_evicted = ctx->dr_off[i + 1] - ctx->dr_off[i];
         o.n_placed = res[i].n_scheduled; o.n_unscheduled = res[i].n_unscheduled;
         o.n_blocked = ctx->dr_boff[i + 1] - ctx->dr_boff[i];
-        o.n_vanished = n_vanished[i]; o.reserved = 0;
+        o.n_vanished = n_vanished[i]; o.n_pdb_violated = ctx->dr_voff[i + 1] - ctx->dr_voff[i];
         o.req_mcpu = res[i].req_mcpu; o.alloc_mcpu = res[i].alloc_mcpu; o.req_mem = res[i].req_mem; o.alloc_mem = res[i].alloc_mem;
         ctx->dr_nfail[i] = res[i].n_unscheduled;
     }
@@ -1535,6 +1587,76 @@ extern "C" int simon_drain_download(simon_ctx *ctx, uint32_t scenario, uint32_t 
         CU(cudaMemcpy(fail_counts, ctx->d_dr_fail_counts.p + (size_t)scenario * ctx->dr_max * SIMON_N_FAIL_CODES,
                       4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
     if (fail_pod && nf) CU(cudaMemcpy(fail_pod, ctx->d_dr_fail_pod.p + (size_t)scenario * ctx->dr_max, 4ull * nf, cudaMemcpyDeviceToHost));
+    return SIMON_OK;
+}
+
+extern "C" int simon_drain_pdb_download(simon_ctx *ctx, uint32_t scenario, uint32_t *pdb, uint32_t *evicted) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->dr_n) return fail(ctx, SIMON_ERR_STATE, "no simon_drain_run batch since the last upload");
+    if (scenario >= ctx->dr_n) return fail(ctx, SIMON_ERR_INVALID, "drain %u of a batch of %u", scenario, ctx->dr_n);
+    const uint32_t b = ctx->dr_voff[scenario], e = ctx->dr_voff[scenario + 1];
+    if (pdb) std::copy(ctx->dr_vpdb.begin() + b, ctx->dr_vpdb.begin() + e, pdb);
+    if (evicted) std::copy(ctx->dr_vcnt.begin() + b, ctx->dr_vcnt.begin() + e, evicted);
+    return SIMON_OK;
+}
+
+// ---- PodDisruptionBudgets ----------------------------------------------------------------------------------------------------------
+extern "C" int simon_pdbs_upload(simon_ctx *ctx, const simon_pdbs *t) {
+    if (!ctx || !t) return SIMON_ERR_INVALID;
+    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_pdbs_upload before simon_pods_upload");
+    const uint32_t P = ctx->n_pods, J = t->n_pdbs;
+    if (J == 0) { ctx->n_pdbs = 0; return SIMON_OK; }
+    // ---- refusals before any device work ----
+    if (t->n_pods != P) return fail(ctx, SIMON_ERR_INVALID, "simon_pdbs_upload: n_pods %u, the pod set has %u", t->n_pods, P);
+    if (!t->pod_off || !t->desired) return fail(ctx, SIMON_ERR_INVALID, "simon_pdbs_upload: NULL pod_off or desired");
+    if (t->pod_off[0] != 0) return fail(ctx, SIMON_ERR_INVALID, "simon_pdbs_upload: pod_off[0] is %u, not 0", t->pod_off[0]);
+    for (uint32_t q = 0; q < P; q++)
+        if (t->pod_off[q + 1] < t->pod_off[q]) return fail(ctx, SIMON_ERR_INVALID, "simon_pdbs_upload: pod_off is not monotone at pod %u", q);
+    const uint32_t E = t->pod_off[P];
+    if (E && !t->pod_pdb) return fail(ctx, SIMON_ERR_INVALID, "simon_pdbs_upload: NULL pod_pdb");
+    uint32_t max_per_pod = 0;
+    std::vector<uint32_t> moff(J + 1, 0u);
+    for (uint32_t q = 0; q < P; q++) {
+        max_per_pod = std::max(max_per_pod, t->pod_off[q + 1] - t->pod_off[q]);
+        for (uint32_t k = t->pod_off[q]; k < t->pod_off[q + 1]; k++) {
+            const uint32_t j = t->pod_pdb[k];
+            if (j >= J) return fail(ctx, SIMON_ERR_INVALID, "simon_pdbs_upload: pod %u names PDB %u of %u", q, j, J);
+            if (k > t->pod_off[q] && j <= t->pod_pdb[k - 1])
+                return fail(ctx, SIMON_ERR_INVALID, "simon_pdbs_upload: the PDBs of pod %u are not ascending (PDB %u repeated or out of order)", q, j);
+            moff[j + 1]++;
+        }
+    }
+    for (uint32_t j = 0; j < J; j++)
+        if (t->desired[j] < 0) return fail(ctx, SIMON_ERR_INVALID, "simon_pdbs_upload: PDB %u has desired %d < 0", j, t->desired[j]);
+    // ---- the inverse CSR (members in pod order), then the uploads ----
+    uint32_t max_members = 0;
+    for (uint32_t j = 0; j < J; j++) { max_members = std::max(max_members, moff[j + 1]); moff[j + 1] += moff[j]; }
+    std::vector<uint32_t> members(std::max(1u, E)), cur(moff.begin(), moff.end() - 1);
+    for (uint32_t q = 0; q < P; q++)
+        for (uint32_t k = t->pod_off[q]; k < t->pod_off[q + 1]; k++) members[cur[t->pod_pdb[k]]++] = q;
+    CU(cudaSetDevice(ctx->device));
+    cudaStream_t st = ctx->stream;
+    ctx->h_pdb_off.assign(t->pod_off, t->pod_off + P + 1);
+    ctx->h_pdb_ids.assign(t->pod_pdb, t->pod_pdb + E);
+    CU(ctx->d_pdb_off.upload(t->pod_off, P + 1, st)); CU(ctx->d_pdb_ids.upload(t->pod_pdb, E, st));
+    CU(ctx->d_pdb_moff.upload(moff.data(), J + 1, st)); CU(ctx->d_pdb_members.upload(members.data(), E, st));
+    CU(ctx->d_pdb_desired.upload(t->desired, J, st)); CU(ctx->d_pdb_rem.alloc(J));
+    CU(ctx->d_pdb_ctl.alloc(4)); CU(ctx->d_pdb_hit.alloc(std::max(1u, max_per_pod)));
+    CU(cudaStreamSynchronize(st));       // the host vectors leave scope
+    ctx->n_pdbs = J; ctx->pdb_max_per_pod = max_per_pod; ctx->pdb_max_members = max_members;
+    return SIMON_OK;
+}
+
+extern "C" int simon_pdbs_allowed(simon_ctx *ctx, int32_t *allowed) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->have_live) return fail(ctx, SIMON_ERR_STATE, "simon_pdbs_allowed: no placement since the last pod upload or reset");
+    if (!ctx->n_pdbs) return SIMON_OK;
+    if (!allowed) return fail(ctx, SIMON_ERR_INVALID, "simon_pdbs_allowed: NULL allowed");
+    CU(cudaSetDevice(ctx->device));
+    CU(pdb_allowed(ctx, ctx->single.out_node.p));
+    CU(cudaMemcpyAsync(allowed, ctx->d_pdb_rem.p, 4ull * ctx->n_pdbs, cudaMemcpyDeviceToHost, ctx->stream));
+    cudaError_t e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "PDB count failed: %s", cudaGetErrorString(e));
     return SIMON_OK;
 }
 
@@ -1799,6 +1921,10 @@ static int moves_launch(simon_ctx *ctx, bool record) {
     if (record) CU(cudaEventRecord(ctx->ev0, st));
     if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && !ctx->mv_scoped && n) CU(cudaMemsetAsync(ctx->d_mv_slots.p, 0, 4ull * n, st));
     moves_pack(ctx, S.state, S.out_node.p, gpu);
+    if (ctx->n_pdbs) {                  // pods of PDBs with no disruption allowed on the live placement do not move
+        CU(pdb_allowed(ctx, S.out_node.p));
+        CU(pdb_mark(ctx, nullptr));
+    }
     moves_score(ctx, moves_params(ctx, S.state, S.out_node.p, ctx->mv_base));
     if (record) CU(cudaEventRecord(ctx->ev1, st));
     CU(cudaGetLastError());
@@ -1962,6 +2088,13 @@ int simon_moves_plan(simon_ctx *ctx, uint32_t max_moves, int32_t min_gain, simon
     simon_moves_plan_setup<<<std::max(1u, std::min(1184u, (P + 255) / 256)), 256, 0, st>>>(P, ctx->pl_slots.p, ctx->d_mv_pods.p, ctx->pl_ctl.p);
     ctx->launches += 2;             // the pack and the setup
     CU(cudaGetLastError());
+    // with a PDB table: remaining = allowed on the live placement; the pods of PDBs without budget are marked and counted
+    const uint32_t n_pdbs = ctx->n_pdbs;
+    if (n_pdbs) {
+        CU(cudaMemsetAsync(ctx->d_pdb_ctl.p, 0, 16, st));
+        CU(pdb_allowed(ctx, ctx->pl_place.p));
+        CU(pdb_mark(ctx, ctx->d_pdb_ctl.p + 2));
+    }
     const SmvParams M = moves_params(ctx, pl, ctx->pl_place.p, 0);
     SkParams Pk;
     fill_params(ctx, S, Pk);
@@ -1982,6 +2115,12 @@ int simon_moves_plan(simon_ctx *ctx, uint32_t max_moves, int32_t min_gain, simon
             moves_score(ctx, M);
             simon_moves_plan_apply<<<1, 32, 0, st>>>(Pk, Q);
             ctx->launches++;
+            if (n_pdbs) {               // the step's PDB spending, and the members of PDBs it used up
+                CU(simon_pdb_launch_step(st, ctx->sms * 4u, ctx->pl_ctl.p, ctx->pl_steps.p, ctx->d_pdb_off.p, ctx->d_pdb_ids.p,
+                                         ctx->d_pdb_rem.p, ctx->d_pdb_ctl.p, ctx->d_pdb_hit.p, ctx->pdb_max_members, ctx->d_pdb_moff.p,
+                                         ctx->d_pdb_members.p, ctx->d_mv_pods.p));
+                ctx->launches += 2;
+            }
         }
         CU(cudaGetLastError());
         CU(cudaMemcpyAsync(ctl, ctx->pl_ctl.p, 16, cudaMemcpyDeviceToHost, st));
@@ -1996,8 +2135,10 @@ int simon_moves_plan(simon_ctx *ctx, uint32_t max_moves, int32_t min_gain, simon
                     ctl[2] == SMV_PLAN_ERR_SLOTS ? "Reserve on the target differs from the scored GPU slots" : "a count of the source node went negative");
     if (!ctl[1]) return fail(ctx, SIMON_ERR_CUDA, "move plan: no stop after %llu steps", (unsigned long long)limit);
     if (ctl[0]) CU(cudaMemcpy(out_steps, ctx->pl_steps.p, sizeof(simon_plan_step) * ctl[0], cudaMemcpyDeviceToHost));
+    uint32_t pctl[4] = {0, 0, 0, 0};
+    if (n_pdbs) CU(cudaMemcpy(pctl, ctx->d_pdb_ctl.p, 16, cudaMemcpyDeviceToHost));
     memset(out, 0, sizeof(*out));
-    out->n_steps = ctl[0]; out->stop_reason = ctl[1]; out->n_excluded = ctl[3]; out->kernel_ms = ctx->last_ms;
+    out->n_steps = ctl[0]; out->stop_reason = ctl[1]; out->n_excluded = ctl[3]; out->n_pdb_blocked = pctl[2]; out->kernel_ms = ctx->last_ms;
     ctx->pl_valid = true;
     return SIMON_OK;
 }

@@ -42,22 +42,7 @@ struct __align__(32) SmvClass {
                                                          //           | scope bits the class needs:2 | never movable:1 | n_hard:4 | n_ports, bit 5 (32 ports: SK_MAX_ENT)
 };
 static_assert(sizeof(SmvClass) == 64, "SmvClass layout");
-// per-pod record built by the pack kernel of every launch: everything a move needs to know about its pod in ONE 16-byte load,
-// so that the class header, the static verdict record and both node records can be fetched in parallel afterwards
-struct __align__(16) SmvPod {
-    int32_t cls, node;      // class, current node (or < 0)
-    uint32_t sig, bits;     // static signature and SmvClass::bits of the class
-};
-#define SMC_NOT_MOVABLE (1u << 8)
-#define SMC_HAS_SCALAR (1u << 9)
-#define SMC_NPORTS(b) ((((b) >> 10) & 31u) | (((b) >> 24) & 32u))   // bits 10..14 and 29: 0..63 (a class has at most SK_MAX_ENT = 32)
-#define SMC_NFILT(b) (((b) >> 15) & 63u)
-#define SMC_OWN_INC (1u << 21)
-#define SMC_NEED(b) (((b) >> 22) & 3u)   // SIMON_MOVES_SCOPE_* bits that admit a not-movable class (GPU share, hard spread)
-#define SMC_NEED_GPU (1u << 22)
-#define SMC_NEED_HARD (1u << 23)
-#define SMC_NEVER (1u << 24)             // pinned (DaemonSet) or Open-Local class: not movable under any scope
-#define SMC_NHARD(b) (((b) >> 25) & 15u)
+#include "simon_moves.cuh"       // SmvPod and the SMC_* class bits (shared with simon_pdb.cu)
 #define SMV_MAX_HARD 8                   // == SK_MAX_HARD: stride of the per-class rows of SmvParams::hs
 
 // free memory per GPU-share device of a node (-1 past gpu_count) and its total gpu-mem: AllocateGpuId's input

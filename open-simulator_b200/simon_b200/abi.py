@@ -57,7 +57,7 @@ class SimonScenarioResult(C.Structure):
 
 class SimonDrainResult(C.Structure):
     _fields_ = [("n_evicted", C.c_uint32), ("n_placed", C.c_uint32), ("n_unscheduled", C.c_uint32), ("n_blocked", C.c_uint32),
-                ("n_vanished", C.c_uint32), ("reserved", C.c_uint32),
+                ("n_vanished", C.c_uint32), ("n_pdb_violated", C.c_uint32),
                 ("req_mcpu", C.c_int64), ("alloc_mcpu", C.c_int64), ("req_mem", C.c_int64), ("alloc_mem", C.c_int64)]
 
 
@@ -120,8 +120,20 @@ PLAN_STEP_DTYPE = np.dtype([("move", np.uint32), ("pod", np.uint32), ("from", np
 
 
 class SimonMovesPlanResult(C.Structure):
-    _fields_ = [("n_steps", C.c_uint32), ("stop_reason", C.c_uint32), ("n_excluded", C.c_uint32), ("reserved", C.c_uint32),
+    _fields_ = [("n_steps", C.c_uint32), ("stop_reason", C.c_uint32), ("n_excluded", C.c_uint32), ("n_pdb_blocked", C.c_uint32),
                 ("kernel_ms", C.c_float), ("reserved2", C.c_uint32)]
+
+
+class SimonPdbs(C.Structure):
+    _fields_ = [("n_pdbs", C.c_uint32), ("n_pods", C.c_uint32), ("pod_off", C.c_void_p), ("pod_pdb", C.c_void_p), ("desired", C.c_void_p)]
+
+
+def marshal_pdbs(t):
+    """disruption.PdbTables -> (SimonPdbs, arrays that must outlive the upload call)."""
+    keep = [np.ascontiguousarray(a, dtype=d) for a, d in ((t.pod_off, np.uint32), (t.pod_pdb, np.uint32), (t.desired, np.int32))]
+    keep = [a if a.size else np.zeros(1, a.dtype) for a in keep]
+    s = SimonPdbs(len(t.desired), len(t.pod_off) - 1, *[a.ctypes.data for a in keep])
+    return s, keep
 
 
 _SNAP_DTYPES = {

@@ -27,7 +27,8 @@ EXPORTS = ["simon_gpu_version", "simon_ctx_create", "simon_ctx_destroy", "simon_
            "simon_storage_upload", "simon_storage_state_download", "simon_devices_upload", "simon_devices_state_download",
            "simon_scenarios_run_local", "simon_scenarios_storage_download", "simon_moves_set_scope", "simon_moves_gpu_slots_download",
            "simon_schedule_resume", "simon_last_launch", "simon_drain_run", "simon_drain_download", "simon_drain_times",
-           "simon_drain_budget", "simon_moves_plan", "simon_moves_plan_download", "simon_moves_plan_state_download"]
+           "simon_drain_budget", "simon_moves_plan", "simon_moves_plan_download", "simon_moves_plan_state_download",
+           "simon_pdbs_upload", "simon_pdbs_allowed", "simon_drain_pdb_download"]
 
 
 class EngineUnavailable(RuntimeError):
@@ -122,6 +123,12 @@ def lib():
         L.simon_moves_plan_download.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.simon_moves_plan_state_download.restype = C.c_int
         L.simon_moves_plan_state_download.argtypes = [C.c_void_p] + [C.c_void_p] * 8
+        L.simon_pdbs_upload.restype = C.c_int
+        L.simon_pdbs_upload.argtypes = [C.c_void_p, C.c_void_p]
+        L.simon_pdbs_allowed.restype = C.c_int
+        L.simon_pdbs_allowed.argtypes = [C.c_void_p, C.c_void_p]
+        L.simon_drain_pdb_download.restype = C.c_int
+        L.simon_drain_pdb_download.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     except AttributeError:
         if not os.environ.get("SIMON_GPU_LIB"):       # an experiment library may lack the newer entry points; the shipped one may not
             raise
@@ -373,7 +380,7 @@ class Engine:
         res = abi.SimonMovesPlanResult()
         self._check(lib().simon_moves_plan(self.h, max_moves, min_gain, steps.ctypes.data, C.byref(res)))
         return dict(steps=steps[:res.n_steps].copy(), stop_reason=int(res.stop_reason), excluded=int(res.n_excluded),
-                    kernel_ms=float(res.kernel_ms))
+                    pdb_blocked=int(res.n_pdb_blocked), kernel_ms=float(res.kernel_ms))
 
     def moves_plan_download(self):
         """After moves_plan: (placement [P] int32, GPU slot words [P] uint32) of the plan's end state."""
@@ -434,6 +441,24 @@ class Engine:
         self._check(lib().simon_scenarios_storage_download(self.h, i, vg.ctypes.data, None if dev is None else dev.ctypes.data))
         return vg[:V * N].reshape(V, N), None if dev is None else dev[:N]
 
+    # ---- PodDisruptionBudgets (simon_pdbs_upload) ----
+    def pdbs_upload(self, tables):
+        """Upload disruption.PdbTables of this pod list (None or no PDB: clear the table).  Later drains, move runs and plans honour
+        them; a new pod upload drops them."""
+        if tables is None:
+            self.pdbs, self._pdbs_keep = abi.SimonPdbs(0, self.c.pods_dims["n_pods"], None, None, None), []
+        else:
+            self.pdbs, self._pdbs_keep = abi.marshal_pdbs(tables)
+        self.n_pdbs = int(self.pdbs.n_pdbs)
+        self._check(lib().simon_pdbs_upload(self.h, C.byref(self.pdbs)))
+
+    def pdbs_allowed(self) -> np.ndarray:
+        """Per uploaded PDB: the disruptions it allows on the live placement, max(0, placed members - desired)."""
+        n = getattr(self, "n_pdbs", 0)
+        a = np.zeros(max(n, 1), np.int32)
+        self._check(lib().simon_pdbs_allowed(self.h, a.ctypes.data))
+        return a[:n]
+
     # ---- node drains (simon_drain_run) ----
     # share of the memory simon_drain_budget reports that one batch's pooled state may take: the rest is the margin for what the
     # per-scenario bytes do not count (per-evicted-pod outputs, failure records, the large-cluster variant's node arrays)
@@ -450,9 +475,10 @@ class Engine:
         nodes that remain, in their nodeTree.list() order.  The list runs in batches (chunks) sized so that one batch's pooled state
         fits the device: chunk scenarios of simon_drain_budget's per-scenario bytes in DRAIN_MEM_FRACTION of what it reports free
         (chunk: an explicit batch size).  Returns one dict per drain: n_evicted, n_placed, n_unscheduled, n_blocked, n_vanished and
-        the sums req_mcpu / alloc_mcpu / req_mem / alloc_mem over the remaining nodes; with detail also evicted (pod indices in
-        pod order), node (per evicted pod, -1 unschedulable), gpu_slots, score, blocked, fail_counts [n_unscheduled][24] and
-        fail_pod.  self.last_drain: chunks, scenario_bytes, setup_ms / place_ms (device time summed over the batches)."""
+        the sums req_mcpu / alloc_mcpu / req_mem / alloc_mem over the remaining nodes, and n_pdb_violated (with a PDB table); with
+        detail also evicted (pod indices in pod order), node (per evicted pod, -1 unschedulable), gpu_slots, score, blocked,
+        fail_counts [n_unscheduled][24], fail_pod, and pdb_violated / pdb_evicted (the violated PDBs ascending, their evicted
+        members).  self.last_drain: chunks, scenario_bytes, setup_ms / place_ms (device time summed over the batches)."""
         L = lib()
         pl = np.ascontiguousarray(placed, dtype=np.int32)
         n = len(remain_lists)
@@ -475,7 +501,8 @@ class Engine:
             info["launches"].append(self.last_launch())
             for i, r in enumerate(res):
                 d = dict(n_evicted=r.n_evicted, n_placed=r.n_placed, n_unscheduled=r.n_unscheduled, n_blocked=r.n_blocked,
-                         n_vanished=r.n_vanished, req_mcpu=r.req_mcpu, alloc_mcpu=r.alloc_mcpu, req_mem=r.req_mem, alloc_mem=r.alloc_mem)
+                         n_vanished=r.n_vanished, n_pdb_violated=r.n_pdb_violated, req_mcpu=r.req_mcpu, alloc_mcpu=r.alloc_mcpu,
+                         req_mem=r.req_mem, alloc_mem=r.alloc_mem)
                 if detail:
                     ne, nb, nf = r.n_evicted, r.n_blocked, r.n_unscheduled
                     ev = np.zeros(max(ne, 1), np.uint32)
@@ -487,8 +514,12 @@ class Engine:
                     fp = np.zeros(max(nf, 1), np.uint32)
                     self._check(L.simon_drain_download(self.h, i, ev.ctypes.data, node.ctypes.data, slots.ctypes.data, score.ctypes.data,
                                                        blk.ctypes.data, fc.ctypes.data, fp.ctypes.data))
+                    nv = r.n_pdb_violated
+                    vp = np.zeros(max(nv, 1), np.uint32)
+                    vc = np.zeros(max(nv, 1), np.uint32)
+                    self._check(L.simon_drain_pdb_download(self.h, i, vp.ctypes.data, vc.ctypes.data))
                     d.update(evicted=ev[:ne], node=node[:ne], gpu_slots=slots[:ne], score=score[:ne], blocked=blk[:nb],
-                             fail_counts=fc[:nf], fail_pod=fp[:nf])
+                             fail_counts=fc[:nf], fail_pod=fp[:nf], pdb_violated=vp[:nv], pdb_evicted=vc[:nv])
                 out.append(d)
         self.last_drain = info
         return out

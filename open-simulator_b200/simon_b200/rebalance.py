@@ -3,6 +3,10 @@ definition is this project's (include/simon_gpu.h, simon_moves_plan): starting f
 by (gain descending, move index ascending) is applied, then every candidate is scored again on the state it leaves, until max_moves
 migrations are planned or no move gains at least min_gain.  Each pod moves at most once.  Gains, filters and the move scope are those
 of the candidate-move scoring (moves.py).  The whole plan runs on the device; the live state is not changed.
+
+With PodDisruptionBudgets (disruption.py) each PDB starts with the disruptions it allows on the live state; a pod with a PDB at 0 is not
+moved, and each migration spends one unit of every PDB of its pod.  Budgets are not restored within a plan: its migrations are one
+batch of evictions that violates no PDB.
 """
 from __future__ import annotations
 
@@ -36,6 +40,8 @@ class MigrationPlan:
     Excluded: int = 0                # GPU-share pods whose slot word is saturated on a device: never moved
     NodePods: Dict[str, List[str]] = field(default_factory=dict)     # pod names per node after the plan (nodes in index order)
     KernelMs: float = 0.0
+    PdbBlocked: int = 0              # placed pods a PDB without budget on the live state keeps in place
+    PdbExhausted: List[str] = field(default_factory=list)            # PDBs whose budget the plan used up
 
 
 def candidates(compiled: Compiled, placement, sources: Optional[Sequence[int]] = None, targets: Optional[Sequence[int]] = None,
@@ -91,11 +97,20 @@ def _gpu_classes(compiled: Compiled) -> np.ndarray:
     return blob[off[:-1] + SCW_GPU_MEM] > 0
 
 
-def plan(engine, compiled: Compiled, moves: np.ndarray, max_moves: int, min_gain: int = 1, scope: int = 0) -> MigrationPlan:
+def plan(engine, compiled: Compiled, moves: np.ndarray, max_moves: int, min_gain: int = 1, scope: int = 0, pdbs=None) -> MigrationPlan:
     """A migration plan over `moves` (e.g. candidates(...)) on the engine's live state, under the move scope `scope`
-    (abi.MOVES_SCOPE_* bits).  The engine's live state is not changed; its move list and scope are."""
+    (abi.MOVES_SCOPE_* bits); pdbs: disruption.PdbTables of the engine's pod list, uploaded and honoured.  The engine's live state is
+    not changed; its move list, scope and PDB table are."""
+    from . import disruption
     engine.moves_set_scope(scope)
     engine.moves_upload(moves, 0)
+    if pdbs is not None:
+        engine.pdbs_upload(pdbs)
+        allowed = engine.pdbs_allowed()
     r = engine.moves_plan(max_moves, min_gain)
     placement, _ = engine.moves_plan_download()
-    return from_raw(compiled, r["steps"], r["stop_reason"], r["excluded"], placement, r["kernel_ms"])
+    out = from_raw(compiled, r["steps"], r["stop_reason"], r["excluded"], placement, r["kernel_ms"])
+    out.PdbBlocked = r["pdb_blocked"]
+    if pdbs is not None:
+        out.PdbExhausted = [pdbs.names[j] for j in disruption.exhausted(pdbs, allowed, r["steps"]["pod"])]
+    return out

@@ -7,11 +7,13 @@ simon_drain_run):
   * pods of DaemonSets of a removed node vanish with it; pods bound by spec.nodeName and pods with Open-Local volumes block the drain
     (they cannot be recreated elsewhere); every other pod of a removed node is evicted and placed again, in pod-list order, on the
     remaining nodes, on the live state minus the removed nodes' pods;
-  * a drain is drainable when nothing blocks it and every evicted pod finds a node.  PodDisruptionBudgets are not consulted: the
-    result is the end state, not an eviction sequence.
+  * a drain is drainable when nothing blocks it, every evicted pod finds a node and, with PodDisruptionBudgets uploaded
+    (disruption.py, Engine.pdbs_upload), it evicts no more members of any PDB than the PDB allows on the live state.  Vanished and
+    blocked pods do not count against a PDB.  The result is the end state, not an eviction sequence.
 
 ScaleDownPlan sweeps every candidate node alone, orders the drainable ones by utilisation and removes the longest prefix of that order
-whose every prefix drains and meets the satisfyResourceSetting caps (MaxCPU / MaxMemory).
+whose every prefix drains and meets the satisfyResourceSetting caps (MaxCPU / MaxMemory).  With PDBs a prefix that violates one does
+not drain, so the first such prefix ends the plan, and the sweep marks such single-node drains not drainable.
 """
 from __future__ import annotations
 
@@ -45,6 +47,13 @@ class BlockedPod:
 
 
 @dataclass
+class PdbViolation:
+    Name: str                       # "namespace/name"
+    Evicted: int                    # members the drain evicts
+    Allowed: int                    # disruptions the PDB allows on the live state
+
+
+@dataclass
 class DrainResult:
     RemovedNodes: List[str]
     Drainable: bool
@@ -54,6 +63,7 @@ class DrainResult:
     VanishedPods: int = 0
     Occupancy: Dict[str, int] = field(default_factory=dict)  # req_mcpu / alloc_mcpu / req_mem / alloc_mem over the remaining nodes
     CapsOk: bool = True                                       # occupancy_ok under MaxCPU / MaxMemory
+    PdbViolations: List[PdbViolation] = field(default_factory=list)
 
 
 @dataclass
@@ -65,6 +75,7 @@ class NodeSweep:
     Evicted: int
     Unscheduled: int
     Blocked: int
+    PdbViolated: int = 0            # PDBs the drain would violate
 
 
 @dataclass
@@ -181,9 +192,16 @@ def gpu_index(word: int) -> Optional[str]:
     return "-".join(str(d) for d in devs) if devs else None
 
 
+def drainable(r: dict) -> bool:
+    """A drain result of Engine.drain_run: nothing blocked, every evicted pod placed, no PDB violated."""
+    return r["n_blocked"] == 0 and r["n_unscheduled"] == 0 and r.get("n_pdb_violated", 0) == 0
+
+
 def drain_results(compiled: Compiled, placed: np.ndarray, removed_lists: Sequence[Sequence[int]], remain_lists: Sequence[np.ndarray],
-                  raw: Sequence[dict], max_cpu: Optional[int] = None, max_mem: Optional[int] = None) -> List[DrainResult]:
-    """DrainResult per drain from Engine.drain_run(..., detail=True) results."""
+                  raw: Sequence[dict], max_cpu: Optional[int] = None, max_mem: Optional[int] = None, pdbs=None,
+                  allowed: Optional[np.ndarray] = None) -> List[DrainResult]:
+    """DrainResult per drain from Engine.drain_run(..., detail=True) results; pdbs (disruption.PdbTables) and allowed
+    (Engine.pdbs_allowed on the live state) name the violated PDBs."""
     from .simulator import UnscheduledPod, format_fit_error
     if max_cpu is None or max_mem is None:
         max_cpu, max_mem = env_caps()
@@ -195,8 +213,10 @@ def drain_results(compiled: Compiled, placed: np.ndarray, removed_lists: Sequenc
     out = []
     for removed, remain, r in zip(removed_lists, remain_lists, raw):
         active = [int(x) for x in remain]
-        res = DrainResult(RemovedNodes=[names[g] for g in removed], Drainable=r["n_blocked"] == 0 and r["n_unscheduled"] == 0,
-                          VanishedPods=int(r["n_vanished"]))
+        res = DrainResult(RemovedNodes=[names[g] for g in removed], Drainable=drainable(r), VanishedPods=int(r["n_vanished"]))
+        for j, e in zip(r.get("pdb_violated", []), r.get("pdb_evicted", [])):
+            res.PdbViolations.append(PdbViolation(pdbs.names[int(j)] if pdbs is not None else str(int(j)), int(e),
+                                                  int(allowed[int(j)]) if allowed is not None else -1))
         fails = {int(p): j for j, p in enumerate(r["fail_pod"])}
         for q, g, w in zip(r["evicted"].tolist(), r["node"].tolist(), r["gpu_slots"].tolist()):
             res.EvictedPods.append(EvictedPod(recs[q], names[placed[q]], names[g] if g >= 0 else None, gpu_index(w) if g >= 0 else None))
@@ -217,8 +237,8 @@ def drain_results(compiled: Compiled, placed: np.ndarray, removed_lists: Sequenc
 def plan_scale_down(compiled: Compiled, placed: np.ndarray, runner: Callable[[List[np.ndarray]], List[dict]],
                     candidates: Optional[Sequence[int]] = None, max_remove: Optional[int] = None, batch: int = 64,
                     max_cpu: Optional[int] = None, max_mem: Optional[int] = None) -> ScaleDownPlan:
-    """runner(remain_lists) -> per drain a dict with n_blocked, n_unscheduled, n_evicted and the occupancy sums (Engine.drain_run
-    with detail=False).  1. every candidate drained alone, in one run; 2. the drainable ones ordered by utilisation ascending, ties
+    """runner(remain_lists) -> per drain a dict with n_blocked, n_unscheduled, n_evicted, n_pdb_violated and the occupancy sums
+    (Engine.drain_run with detail=False; on an engine with a PDB table the PDBs are honoured).  1. every candidate drained alone, in one run; 2. the drainable ones ordered by utilisation ascending, ties
     in nodeTree order; 3. prefixes k = 1, 2, ... of that order removed together, `batch` consecutive k per run; 4. the plan is the
     largest k such that every prefix up to k drains and meets the caps: the first failing k ends it (no monotonicity is assumed)."""
     if max_cpu is None or max_mem is None:
@@ -232,8 +252,9 @@ def plan_scale_down(compiled: Compiled, placed: np.ndarray, runner: Callable[[Li
     sweep = []
     good = []
     for c, r in zip(cand, sweep_raw):
-        ok = r["n_blocked"] == 0 and r["n_unscheduled"] == 0
-        sweep.append(NodeSweep(names[c], ok, float(util[c]), int(r["n_evicted"]), int(r["n_unscheduled"]), int(r["n_blocked"])))
+        ok = drainable(r)
+        sweep.append(NodeSweep(names[c], ok, float(util[c]), int(r["n_evicted"]), int(r["n_unscheduled"]), int(r["n_blocked"]),
+                               int(r.get("n_pdb_violated", 0))))
         if ok:
             good.append(c)
     good.sort(key=lambda c: (util[c], c))            # compiled index order is nodeTree order
@@ -248,7 +269,7 @@ def plan_scale_down(compiled: Compiled, placed: np.ndarray, runner: Callable[[Li
         raw = runner([order.remaining(good[:j]) for j in ks])
         stop = False
         for j, r in zip(ks, raw):
-            ok = r["n_blocked"] == 0 and r["n_unscheduled"] == 0 and occupancy_ok(r, max_cpu, max_mem)
+            ok = drainable(r) and occupancy_ok(r, max_cpu, max_mem)
             prefixes.append(dict(r, k=j, ok=ok))
             if not ok:
                 stop = True
@@ -262,9 +283,12 @@ def plan_scale_down(compiled: Compiled, placed: np.ndarray, runner: Callable[[Li
 
 # ---- entry points on objects ---------------------------------------------------------------------------------------------------------
 
-def drain(cluster: ResourceTypes, apps: List[AppResource], drains: List[List[str]], *opts) -> List[DrainResult]:
-    """NewSimulator(*opts), RunCluster(PrepareCluster(cluster)), ScheduleApp per app, then DrainNodes(drains)."""
-    from .simulator import NewSimulator, PrepareCluster
+def drain(cluster: ResourceTypes, apps: List[AppResource], drains: List[List[str]], *opts, pdbs: Optional[List[dict]] = None) -> List[DrainResult]:
+    """NewSimulator(*opts), RunCluster(PrepareCluster(cluster)), ScheduleApp per app, then DrainNodes(drains).  pdbs: PDB objects to
+    honour besides the cluster's and the apps' (given, even empty, the session runs WithPodDisruptionBudgets)."""
+    from .simulator import NewSimulator, PrepareCluster, WithPodDisruptionBudgets
+    if pdbs is not None:
+        opts = opts + (WithPodDisruptionBudgets(pdbs),)
     with NewSimulator(*opts) as sim:
         sim.RunCluster(PrepareCluster(cluster))
         for app in apps:

@@ -65,6 +65,8 @@ class SimulatorOptions:
     record_scores: bool = False
     openLocal: bool = False
     openLocalDevices: bool = False
+    pdbs: bool = False
+    extraPdbs: list = field(default_factory=list)
 
 
 Option = Callable[[SimulatorOptions], None]
@@ -98,6 +100,15 @@ def WithOpenLocal(devices: bool = False) -> Option:
     def opt(o):
         o.openLocal = True
         o.openLocalDevices = devices
+    return opt
+
+
+def WithPodDisruptionBudgets(extra: Optional[list] = None) -> Option:
+    """Honour the PodDisruptionBudgets of the cluster and of every app so far (plus `extra` PDB objects) in DrainNodes, PlanScaleDown
+    and PlanMigrations (simon_b200/disruption.py for the definition).  Without it PDBs are not consulted."""
+    def opt(o):
+        o.pdbs = True
+        o.extraPdbs = list(extra or [])
     return opt
 
 
@@ -398,6 +409,7 @@ class Simulator:
         self.scores = np.zeros(0, np.int64)
         self.engine = None
         self.compiled: Optional[Compiled] = None
+        self.pdb_tables = None              # WithPodDisruptionBudgets: disruption.PdbTables of the last call, uploaded to `engine`
         self.last_timing: dict = {}
         # pods of the earlier calls that Open-Gpu-Share / Open-Local rejected everywhere: the per-node detail of such pods is collected
         # for the first MAX_GPU_FAIL_DETAIL of the session, as Simulate collects it for the first of its run
@@ -491,6 +503,12 @@ class Simulator:
             self.engine = None
         eng = Engine(compiled, device=options.device, record_scores=options.record_scores)
         self.engine = eng
+        pdb_tables = None
+        if options.pdbs:
+            from .disruption import compile_pdbs
+            pdb_tables = compile_pdbs(list(self.cluster.PodDisruptionBudgets) + [d for a in self.apps for d in a.Resource.PodDisruptionBudgets] +
+                                      options.extraPdbs, compiled)
+            eng.pdbs_upload(pdb_tables)
         tm["engine_create_upload_s"] = time.perf_counter() - t0
         t0 = time.perf_counter()
         out_node, scores, fail_counts, fail_pod = eng.schedule_resume(self.placements)
@@ -524,6 +542,7 @@ class Simulator:
         self._gpu_failed += len(gpu_failed)
         self._local_failed += local_failed
         self.compiled = compiled
+        self.pdb_tables = pdb_tables
         self.last_timing = tm
         return res
 
@@ -544,7 +563,8 @@ class Simulator:
             removed.append(idx)
         remain = [order.remaining(r) for r in removed]
         raw = eng.drain_run(self.placements, remain, detail=True)
-        return scaledown.drain_results(compiled, self.placements, removed, remain, raw)
+        allowed = eng.pdbs_allowed() if self.pdb_tables is not None else None
+        return scaledown.drain_results(compiled, self.placements, removed, remain, raw, pdbs=self.pdb_tables, allowed=allowed)
 
     def PlanScaleDown(self, candidates: Optional[List[str]] = None, max_remove: Optional[int] = None):
         """scaledown.ScaleDownPlan on the session's live state: candidates (node names; all nodes by default) drained alone, the
@@ -575,7 +595,7 @@ class Simulator:
             if bad:
                 raise ValueError(f"PlanMigrations: no node named {bad[0]!r} among the {what}")
         moves = rebalance.candidates(compiled, self.placements, idx["sources"], idx["targets"])
-        return rebalance.plan(eng, compiled, moves, max_moves, min_gain, move_scope)
+        return rebalance.plan(eng, compiled, moves, max_moves, min_gain, move_scope, pdbs=self.pdb_tables)
 
     def _live(self):
         self._check_open()
