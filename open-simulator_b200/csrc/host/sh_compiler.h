@@ -752,12 +752,15 @@ inline void compile_cluster(const Plan &plan, Compiled &out) {
                 long long w = (wj && wj->truthy()) ? wj->as_int(0) : 0;
                 const J &pref = field_obj(p, "preference");
                 if (w == 0 || is_empty_node_selector_term(pref)) continue;
+                // the API allows 1..100; a negative weight can give a negative normalised score, which the reference's framework
+                // turns into a scheduling error (runtime/framework.go:695-697)
+                if (w < 0) throw CompileError("preferred node affinity weight " + std::to_string(w) + " is negative");
                 cs.prefs.emplace_back(w, compile_term(pref, nullptr));
             }
         }
         // raw NodeAffinity scores are int32 on the device (the reference sums int64, node_affinity.go:77-107): refuse, never narrow
         long long wsum = 0;
-        for (auto &p : cs.prefs) wsum += p.first < 0 ? -p.first : p.first;
+        for (auto &p : cs.prefs) wsum += p.first;
         if (wsum >= (1LL << 31)) throw CompileError("preferred node affinity weights sum to 2^31 or more");
         bool all_pin = pin && !cs.terms.empty();
         if (all_pin)
@@ -861,9 +864,18 @@ inline void compile_cluster(const Plan &plan, Compiled &out) {
                 ent.key = tk ? label_text(*tk) : std::string();
                 const J *ms = t.get("maxSkew");
                 ent.skew = (ms && ms->truthy()) ? ms->as_int(0) : 0;
+                // maxSkew is an int32 in the API and in the device's entry table
+                if (ent.skew > INT32_MAX || ent.skew < INT32_MIN)
+                    throw CompileError("topology spread constraint maxSkew " + std::to_string(ent.skew) + " is outside int32");
                 std::string wu = field_str(t, "whenUnsatisfiable");
                 if (wu == "DoNotSchedule") c.hard.push_back(std::move(ent));
-                else if (wu == "ScheduleAnyway" && !c.pinned) c.soft.push_back(std::move(ent));
+                else if (wu == "ScheduleAnyway" && !c.pinned) {
+                    // maxSkew < 1 can give a raw score of -1 and a normalised score outside [0, 100], a scheduling error in the
+                    // reference; the API requires maxSkew >= 1
+                    if (ent.skew < 1)
+                        throw CompileError("ScheduleAnyway topology spread constraint with maxSkew " + std::to_string(ent.skew) + " < 1");
+                    c.soft.push_back(std::move(ent));
+                }
             }
         } else if (!c.pinned) {
             ReqList sel = default_selector(c);
@@ -1089,8 +1101,17 @@ inline void compile_cluster(const Plan &plan, Compiled &out) {
     out.simon_raw.assign((size_t)n_rows * NC1, 0);
     {
         std::unordered_map<std::string, double> memo;
-        for (size_t r = 0; r < row_reqs.size(); r++)
-            for (uint32_t nc = 0; nc < NC; nc++) out.simon_raw[r * NC1 + nc] = simon_raw_value(*row_reqs[r], nclass_alloc[nc], memo);
+        for (size_t r = 0; r < row_reqs.size(); r++) {
+            size_t n_min = 0;
+            for (uint32_t nc = 0; nc < NC; nc++) {
+                out.simon_raw[r * NC1 + nc] = simon_raw_value(*row_reqs[r], nclass_alloc[nc], memo);
+                n_min += out.simon_raw[r * NC1 + nc] == kMinI64;
+            }
+            // MinInt64 next to any other raw score: the reference's NormalizeScore wraps highest - lowest (simon.go) and the
+            // normalised score can leave [0, 100], a scheduling error there; the engine and the oracle would overflow int64.
+            // Deliberately conservative: the row covers node classes on which the pod may be infeasible (and never normalised).
+            if (n_min > 0 && n_min < NC) throw CompileError("Simon score of MinInt64 on some nodes but not on all: its normalisation overflows int64");
+        }
     }
 
     // ---- extra rows: ImageLocality + 10000 * NodePreferAvoidPods ----
@@ -1260,6 +1281,10 @@ inline void compile_cluster(const Plan &plan, Compiled &out) {
         for (auto &e : L.hard) body.insert(body.end(), e.begin(), e.end());
         put(SCW_OFF_PTS_SOFT);
         w[SCW_N_PTS_SOFT] = (long long)L.soft.size();
+        // the counts part of a raw PodTopologySpread score (pods x constraints x ln(topology size + 2)) must fit int32 on the
+        // device, which keeps raw - sum(maxSkew - 1)
+        if (!L.soft.empty() && (double)P * (double)L.soft.size() * std::log((double)N + 2.0) >= (double)((1LL << 31) - 2))
+            throw CompileError("class " + std::to_string(c.cid) + ": topology spread scores of pod count x constraints can exceed 2^31");
         for (auto &e : L.soft) body.insert(body.end(), e.begin(), e.end());
         put(SCW_OFF_IPA_AFF);
         w[SCW_N_IPA_AFF] = (long long)L.aff.size();

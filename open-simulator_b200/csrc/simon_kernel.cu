@@ -280,6 +280,7 @@ struct ClassState {
     bool have_pred;      // psz[] holds sizes the weights were computed from (prediction or exact)
     int64_t F, n_ign, na_max, tt_max, simon_min, simon_max;
     int64_t nm_na_max, nm_tt_max, nm_simon_min, nm_simon_max;   // normalisers B_SNORM was computed with
+    int64_t pts_off;     // sum of (maxSkew - 1) over the ScheduleAnyway constraints: B_RAW_PTS holds raw - pts_off
     bool snorm_valid;
 };
 
@@ -365,6 +366,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
     C.have_pred = false;
     C.snorm_valid = false;
     C.n_soft = 0;
+    C.pts_off = 0;
     const int64_t *cw = S.blob;
 
     // NodeResourcesFit verdict + LeastAllocated + BalancedAllocation of one node for the current class, with `add` more
@@ -502,7 +504,10 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                 double sfc = (double)VAL(e, idx) * S.soft_w[js] + (double)(ENT(ER_A, e) - 1);
                 score = score + sfc;
             }
-            int64_t raw = (SIMON_OPT & 8) ? (int64_t)score : f2i(score);      // 0 <= score < 2^40: counts x ln(size) + skews
+            // 0 <= score < 2^35: counts x ln(size) + (maxSkew - 1), maxSkew up to 2^31 - 1.  B_RAW_PTS holds the truncated score
+            // less the class constant pts_off = sum(maxSkew - 1): exact, and it fits int32 because the compilers bound the counts
+            // part (pods x soft constraints x ln(nodes + 2) < 2^31 - 2).  P3 adds pts_off back in int64.
+            int64_t raw = ((SIMON_OPT & 8) ? (int64_t)score : f2i(score)) - C.pts_off;
             A32(B_RAW_PTS, idx) = (int32_t)raw;
             unsigned long long er = sk_enc(raw);
             lo = er < lo ? er : lo;
@@ -530,11 +535,15 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
     auto snorm_pass = [&]() {
         const int64_t range = C.simon_max - C.simon_min;
         const bool small = range > 0 && range < (1ll << 24) && C.simon_max < (1ll << 24) && C.simon_min >= 0;
+        const bool na32 = C.na_max <= (int64_t)(UINT32_MAX / 100u);
         #pragma unroll 1
         for (uint32_t s = 0; s < NPT; s++) {
             uint32_t idx = s * TPB + tid;
             if (!(A8(C_NFLAGS, idx) & NF_VALID)) continue;
-            int64_t na = C.na_max == 0 ? A32(B_RAW_NA, idx) : (int64_t)((uint32_t)(100 * A32(B_RAW_NA, idx)) / (uint32_t)C.na_max);
+            // raw NodeAffinity scores are 0 .. 2^31 - 1: 100 x raw fits 32 bits while na_max (>= raw on feasible nodes) does
+            const uint32_t na_raw = (uint32_t)A32(B_RAW_NA, idx);
+            int64_t na = C.na_max == 0 ? (int64_t)na_raw
+                       : na32 ? (int64_t)((100u * na_raw) / (uint32_t)C.na_max) : (int64_t)((100ull * na_raw) / (uint64_t)C.na_max);
             int64_t tt = C.tt_max == 0 ? 100 : 100 - (int64_t)((uint32_t)(100 * A32(B_RAW_TT, idx)) / (uint32_t)C.tt_max);
             int64_t sm;
             if (range == 0) sm = 0;
@@ -851,6 +860,9 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                 for (uint32_t w = tid; w < C.E * 8; w += TPB) S.ent[(w & 7) * SK_MAX_ENT + (w >> 3)] = (int32_t)et[w];
             }
             if (!((SIMON_OPT & 1) && (SIMON_OPT & 16))) __syncthreads();
+            C.pts_off = 0;
+#pragma unroll 1
+            for (uint32_t js = 0; js < C.n_soft; js++) C.pts_off += (int64_t)ENT(ER_A, C.e_soft + js) - 1;
             if (!(SIMON_OPT & 1) && tid < 32) {
                 // compact list of the entries this class increments on commit: entry | topology row << 8 | flags << 16
                 // (lane e looks at entry e; SK_MAX_ENT == 32)
@@ -1368,8 +1380,11 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
         // ---- P3: totals and arg-max (first node in scenario order wins ties) ----
         unsigned long long best = 0;
         const int64_t ipa_diff = ipa_max - ipa_min;
-        const bool pts32 = pts_max > 0 && pts_max < (1 << 23) && pts_min >= 0;
-        const float pts_rinv = pts32 ? 1.0f / (float)pts_max : 0.0f;
+        // pts_min / pts_max range over B_RAW_PTS (raw - pts_off): pmax and pmin are the true extremes, and for a true raw
+        // score r = B_RAW_PTS + pts_off, pmax + pmin - r = pmax + pts_min - B_RAW_PTS
+        const int64_t pmax = pts_max + C.pts_off, pmin = pts_min + C.pts_off;
+        const bool pts32 = pmax > 0 && pmax < (1 << 23) && pmin >= 0;
+        const float pts_rinv = pts32 ? 1.0f / (float)pmax : 0.0f;
         #pragma unroll (NPT_T > 0 ? NPT_T : 1)
         for (uint32_t s = 0; s < NPT; s++) {
             uint32_t idx = s * TPB + tid;
@@ -1380,9 +1395,9 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                 int64_t pts;
                 if (C.n_soft == 0) pts = 100;
                 else if (nf & NF_IGNORED) pts = 0;
-                else if (pts_max == 0) pts = 100;
+                else if (pmax == 0) pts = 100;
                 else if (pts32) {
-                    const uint32_t x = 100u * (uint32_t)(pts_max + pts_min - (int64_t)A32(B_RAW_PTS, idx)), d = (uint32_t)pts_max;
+                    const uint32_t x = 100u * (uint32_t)(pmax + pts_min - (int64_t)A32(B_RAW_PTS, idx)), d = (uint32_t)pmax;
                     if (SIMON_OPT & 64) {
                         // x < 2^31, quotient <= 200: the float estimate is off by < 1, one fix-up step makes it exact
                         uint32_t q = (uint32_t)((float)x * pts_rinv);
@@ -1392,7 +1407,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                         pts = (int64_t)q;
                     } else pts = (int64_t)(x / d);
                 }
-                else pts = (100 * (pts_max + pts_min - (int64_t)A32(B_RAW_PTS, idx))) / pts_max;
+                else pts = (100 * (pmax + pts_min - (int64_t)A32(B_RAW_PTS, idx))) / pmax;
                 int64_t ip = 0;
                 if (C.n_isc && ipa_diff > 0) {
                     const double fr = 100.0 * ((double)((int64_t)A32(B_RAW_IPA, idx) - ipa_min) / (double)ipa_diff);    // in [0, 100]

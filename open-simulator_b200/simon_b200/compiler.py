@@ -23,6 +23,7 @@ from __future__ import annotations
 
 import json
 import marshal
+import math
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Tuple
 
@@ -68,6 +69,11 @@ GPU_COUNT_NAME = "alibabacloud.com/gpu-count"
 GPU_INDEX_NAME = "alibabacloud.com/gpu-index"
 PREFER_AVOID_PODS_ANNOTATION = "scheduler.alpha.kubernetes.io/preferAvoidPods"
 MIN_INT64 = -(1 << 63)
+# largest extra-column score (ImageLocality, NodePreferAvoidPods, extra plugins): the device sums it with up to 500 more in int32
+EXTRA_MAX = (1 << 31) - 1 - 500
+# bound of the counts part of a raw PodTopologySpread score (pods x ScheduleAnyway constraints x ln(topology size + 2)): the
+# device keeps raw - sum(maxSkew - 1) in int32
+PTS_COUNTS_MAX = (1 << 31) - 2
 
 
 class CompileError(ValueError):
@@ -620,13 +626,17 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
                 pref = p.get("preference") or {}
                 if w == 0 or is_empty_node_selector_term(pref):
                     continue
+                # the API allows 1..100; a negative weight can give a negative normalised score, which the reference's
+                # framework turns into a scheduling error (runtime/framework.go:695-697)
+                if w < 0:
+                    raise CompileError(f"preferred node affinity weight {w} is negative")
                 t = _compile_term(pref, _req_atoms, name_to_idx)
                 if t is None:
                     raise CompileError("invalid preferred node affinity term")   # NewPreferredSchedulingTerms errors out
                 prefs.append((w, t))
         # the engine keeps raw NodeAffinity scores as int32 (the reference sums int64, node_affinity.go:77-107): API-valid
         # weights are 1..100, so the sum fits unless the input is not a valid PodSpec - refuse instead of narrowing silently
-        if sum(abs(w) for w, _t in prefs) >= (1 << 31):
+        if sum(w for w, _t in prefs) >= (1 << 31):
             raise CompileError("preferred node affinity weights sum to 2^31 or more")
         c.pinned = pin_name is not None and len(terms) > 0 and all(any(r == (REQ_NODE_IS, -3) for r in t) for t in terms)
         class_sel.append((ns_reqs, has_required, terms, prefs))
@@ -730,9 +740,16 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
             for t in tsc:
                 reqs = label_selector_requirements(t.get("labelSelector"))
                 ent = (t.get("topologyKey", ""), int(t.get("maxSkew") or 0), None if reqs is None else tuple(reqs))
+                # maxSkew is an int32 in the API and in the device's entry table
+                if not -(1 << 31) <= ent[1] < (1 << 31):
+                    raise CompileError(f"topology spread constraint maxSkew {ent[1]} is outside int32")
                 if t.get("whenUnsatisfiable") == "DoNotSchedule":
                     c.hard.append(ent)
                 elif t.get("whenUnsatisfiable") == "ScheduleAnyway" and not c.pinned:
+                    # maxSkew < 1 can give a raw score of -1 and a normalised score outside [0, 100], a scheduling error
+                    # in the reference; the API requires maxSkew >= 1
+                    if ent[1] < 1:
+                        raise CompileError(f"ScheduleAnyway topology spread constraint with maxSkew {ent[1]} < 1")
                     c.soft.append(ent)
         elif not c.pinned:
             sel = default_selector(c)
@@ -918,6 +935,12 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
     for r, reqs in row_reqs.items():
         for nc in range(NC):
             simon_raw[r, nc] = _simon_raw(reqs, nclass_alloc[nc])
+        # MinInt64 next to any other raw score: the reference's NormalizeScore wraps highest - lowest (simon.go) and the
+        # normalised score can leave [0, 100], a scheduling error there; the engine and the oracle would overflow int64.
+        # Deliberately conservative: the row covers node classes on which the pod may be infeasible (and never normalised).
+        row = simon_raw[r, :NC]
+        if (row == MIN_INT64).any() and not (row == MIN_INT64).all():
+            raise CompileError("Simon score of MinInt64 on some nodes but not on all: its normalisation overflows int64")
 
     # ---- extra rows: ImageLocality + 10000 * NodePreferAvoidPods ----
     extra_rows: List[np.ndarray] = []
@@ -938,7 +961,9 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
                     if sc < 0 or sc > 100:
                         raise CompileError(f"plugin {pl.name}: score {sc} outside [0, 100] for node {node_names[i]}")
                     base[i] += w * sc
-            if base.max() >= (1 << 31):
+            # the device adds NodeAffinity + TaintToleration + 2 x Simon (up to 400) and Open-Local (up to 100) to this column
+            # in int32
+            if base.max() > EXTRA_MAX:
                 raise CompileError("extra plugin scores overflow the 32-bit extra column")
             vec = base.astype(np.int32)
         if vec is None:
@@ -1025,6 +1050,8 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
             body.extend(e)
         put(SCW_OFF_PTS_SOFT)
         w[SCW_N_PTS_SOFT] = len(L["soft"])
+        if L["soft"] and len(pods) * len(L["soft"]) * math.log(N + 2 + extra_log) >= PTS_COUNTS_MAX:
+            raise CompileError(f"class {c.cid}: topology spread scores of pod count x constraints can exceed 2^31")
         for e in L["soft"]:
             body.extend(e)
         put(SCW_OFF_IPA_AFF)
