@@ -489,56 +489,28 @@ void fill_params(simon_ctx *ctx, const ScenPool &s, SkParams &P) {
 #define SIMON_AUTO_TPB 320u
 
 typedef void (*sk_kernel_fn)(const SkParams);
+struct sk_variant { sk_kernel_fn fn; const char *name; uint32_t threads, slots; bool prof, big, local, drain; };
+#define SK_VARIANT_ENTRY(name, threads, slots, prof, big, local, drain) {name, #name, threads, slots, prof, big, local, drain},
+const sk_variant sk_variants[] = {SIMON_PLACE_VARIANTS(SK_VARIANT_ENTRY)};
+#undef SK_VARIANT_ENTRY
+
 // The compiled kernel variant for (threads per CTA, node slots per thread) on the context's uploads, which is what launch() runs
-// and what the geometry is sized for.  big: the large-cluster variant; prof: with per-phase clock64 timers.  With Open-Local
-// storage uploaded, the local variants (more registers than the plain ones, runtime node slots per thread, no timers).  drain: the
-// drain-batch variants (simon_drain_run), whatever was uploaded.  nullptr: none.
-sk_kernel_fn kernel_variant(const simon_ctx *ctx, uint32_t TPB, uint32_t npt, bool big, bool prof, bool drain) {
-    if (drain) {            // runtime node slots per thread, no timers, no Open-Local code
-        if (big) return simon_drain_kernel_big;
-        if (TPB > SIMON_MAX_TPB) return nullptr;
-        return TPB <= 256 ? simon_drain_kernel_256 : TPB <= 320 ? simon_drain_kernel_320 : simon_drain_kernel_384;
+// and what the geometry is sized for: the one of the fewest threads that holds TPB, with the unrolled loop for npt slots where
+// there is one and run-time slots otherwise.  big: the large-cluster variant, at any thread count; prof: with per-phase timers
+// (256 and 320 threads only).  With Open-Local storage uploaded, the local variants (no timers).  drain: the drain-batch
+// variants (simon_drain_run), whatever was uploaded.  big and drain ignore prof.  nullptr: none.
+const sk_variant *kernel_variant(const simon_ctx *ctx, uint32_t TPB, uint32_t npt, bool big, bool prof, bool drain) {
+    if (!big && TPB > SIMON_MAX_TPB) return nullptr;
+    const uint32_t threads = TPB <= 256 ? 256 : TPB <= 320 ? 320 : 384;
+    const bool local = ctx->have_storage && !drain;
+    if (big || drain) prof = false;
+    const sk_variant *runtime_slots = nullptr;
+    for (const sk_variant &v : sk_variants) {
+        if (v.big != big || v.drain != drain || v.local != local || v.prof != prof || (!big && v.threads != threads)) continue;
+        if (v.slots == npt) return &v;
+        if (v.slots == 0) runtime_slots = &v;
     }
-    if (big) return ctx->have_storage ? simon_local_kernel_big : simon_place_kernel_big;
-    if (TPB > SIMON_MAX_TPB) return nullptr;
-    if (ctx->have_storage) {
-        if (prof) return nullptr;
-        return TPB <= 256 ? simon_local_kernel_256 : TPB <= 320 ? simon_local_kernel_320 : simon_local_kernel_384;
-    }
-    if (TPB > 320) {
-        if (prof) return nullptr;
-        return npt == 1 ? simon_place_kernel_384_1 : npt == 2 ? simon_place_kernel_384_2 : npt == 3 ? simon_place_kernel_384_3 : simon_place_kernel_384_0;
-    }
-    if (TPB > 256) {
-        if (prof) return npt == 1 ? simon_prof_kernel_320_1 : npt == 2 ? simon_prof_kernel_320_2 : npt == 3 ? simon_prof_kernel_320_3 : npt == 4 ? simon_prof_kernel_320_4 : simon_prof_kernel_320_0;
-        return npt == 1 ? simon_place_kernel_320_1 : npt == 2 ? simon_place_kernel_320_2 : npt == 3 ? simon_place_kernel_320_3 : npt == 4 ? simon_place_kernel_320_4 : simon_place_kernel_320_0;
-    }
-    if (prof) return npt == 1 ? simon_prof_kernel_256_1 : npt == 2 ? simon_prof_kernel_256_2 : npt == 3 ? simon_prof_kernel_256_3 : npt == 4 ? simon_prof_kernel_256_4 : simon_prof_kernel_256_0;
-    return npt == 1 ? simon_place_kernel_256_1 : npt == 2 ? simon_place_kernel_256_2 : npt == 3 ? simon_place_kernel_256_3 : npt == 4 ? simon_place_kernel_256_4 : simon_place_kernel_256_0;
-}
-
-// The symbol of every variant kernel_variant() returns (simon_last_launch)
-#define SK_NAMED(k) {k, #k}
-const struct { sk_kernel_fn fn; const char *name; } kernel_names[] = {
-    SK_NAMED(simon_place_kernel_256_0), SK_NAMED(simon_place_kernel_256_1), SK_NAMED(simon_place_kernel_256_2),
-    SK_NAMED(simon_place_kernel_256_3), SK_NAMED(simon_place_kernel_256_4), SK_NAMED(simon_place_kernel_320_0),
-    SK_NAMED(simon_place_kernel_320_1), SK_NAMED(simon_place_kernel_320_2), SK_NAMED(simon_place_kernel_320_3),
-    SK_NAMED(simon_place_kernel_320_4), SK_NAMED(simon_place_kernel_384_0), SK_NAMED(simon_place_kernel_384_1),
-    SK_NAMED(simon_place_kernel_384_2), SK_NAMED(simon_place_kernel_384_3), SK_NAMED(simon_place_kernel_big),
-    SK_NAMED(simon_local_kernel_256), SK_NAMED(simon_local_kernel_320), SK_NAMED(simon_local_kernel_384),
-    SK_NAMED(simon_local_kernel_big),
-    SK_NAMED(simon_drain_kernel_256), SK_NAMED(simon_drain_kernel_320), SK_NAMED(simon_drain_kernel_384), SK_NAMED(simon_drain_kernel_big),
-    SK_NAMED(simon_prof_kernel_256_0), SK_NAMED(simon_prof_kernel_256_1), SK_NAMED(simon_prof_kernel_256_2),
-    SK_NAMED(simon_prof_kernel_256_3), SK_NAMED(simon_prof_kernel_256_4), SK_NAMED(simon_prof_kernel_320_0),
-    SK_NAMED(simon_prof_kernel_320_1), SK_NAMED(simon_prof_kernel_320_2), SK_NAMED(simon_prof_kernel_320_3),
-    SK_NAMED(simon_prof_kernel_320_4),
-};
-#undef SK_NAMED
-
-const char *kernel_name(sk_kernel_fn fn) {
-    for (const auto &k : kernel_names)
-        if (k.fn == fn) return k.name;
-    return "?";
+    return runtime_slots;
 }
 
 // A launch of fn on `ctas` CTAs in clusters of `cs`, `t` threads and `smem` bytes of shared memory each, with fn's attributes set
@@ -563,12 +535,12 @@ cudaError_t cluster_config(sk_kernel_fn fn, uint32_t ctas, uint32_t cs, uint32_t
 // holds at once, GPC boundaries included (0: not even one; a 16-CTA cluster needs 16 free SMs in one GPC).  The variants with
 // phase timers run in the geometry of the default ones.
 int max_active_clusters(const simon_ctx *ctx, bool big, uint32_t cs, uint32_t t, uint32_t npt, size_t smem, bool drain) {
-    const sk_kernel_fn fn = kernel_variant(ctx, t, npt, big, false, drain);
-    if (!fn) return 0;
+    const sk_variant *v = kernel_variant(ctx, t, npt, big, false, drain);
+    if (!v) return 0;
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute attr;
     int n = 0;
-    if (cluster_config(fn, cs, cs, t, smem, nullptr, cfg, attr) != cudaSuccess || cudaOccupancyMaxActiveClusters(&n, fn, &cfg) != cudaSuccess) {
+    if (cluster_config(v->fn, cs, cs, t, smem, nullptr, cfg, attr) != cudaSuccess || cudaOccupancyMaxActiveClusters(&n, v->fn, &cfg) != cudaSuccess) {
         cudaGetLastError();
         return 0;
     }
@@ -701,8 +673,8 @@ int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t T
     // SIMON_PROFILE=1 selects the variants with per-phase clock64 timers (simon_stats cycles); the default variants
     // carry no timers
     static const bool prof = getenv("SIMON_PROFILE") != nullptr;
-    const sk_kernel_fn fn = kernel_variant(ctx, TPB, P.npt, ctx->big, prof, drain);
-    if (!fn)
+    const sk_variant *v = kernel_variant(ctx, TPB, P.npt, ctx->big, prof, drain);
+    if (!v)
         return fail(ctx, SIMON_ERR_LIMIT, "no kernel variant for %u threads per CTA%s%s", TPB, prof ? " with phase timers" : "",
                     ctx->have_storage ? " and Open-Local storage" : "");
     if (ctx->big) {
@@ -711,14 +683,14 @@ int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t T
     }
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute attr;
-    CU(cluster_config(fn, n_scen * CS, CS, TPB, smem, ctx->stream, cfg, attr));
+    CU(cluster_config(v->fn, n_scen * CS, CS, TPB, smem, ctx->stream, cfg, attr));
     if (record) CU(cudaEventRecord(ctx->ev0, ctx->stream));
-    CU(cudaLaunchKernelEx(&cfg, fn, P));
+    CU(cudaLaunchKernelEx(&cfg, v->fn, P));
     if (record) CU(cudaEventRecord(ctx->ev1, ctx->stream));
     ctx->launches++;
     simon_launch_info &li = ctx->last_launch;
     li = simon_launch_info{};
-    snprintf(li.kernel, sizeof(li.kernel), "%s", kernel_name(fn));
+    snprintf(li.kernel, sizeof(li.kernel), "%s", v->name);
     li.n_nodes = ctx->geom_nodes; li.cluster_ctas = CS; li.threads_per_cta = TPB; li.node_slots = P.npt; li.n_scenarios = n_scen;
     li.large = ctx->big; li.local = ctx->have_storage && !drain; li.smem_bytes = smem;
     return SIMON_OK;

@@ -15,22 +15,6 @@
 // it with a 22-word reduction.
 #include "simon_kernel.cuh"
 
-// Compile-time options of the class switch (each measured on its own on C3):
-//   bit 0  the entry table (int32 rows), the compact commit list and its counter bases come precomputed from the upload
-//          (SkParams::cls_aux) instead of being transposed / compacted by every CTA at every class switch
-//   bit 2  the class switch relies on the release / acquire semantics of barrier.cluster.arrive / .wait instead of a
-//          device-wide __threadfence() before the arrive
-//   bit 1  (removed) log weights from shared-memory windows of the log table: measured slower
-//   bit 3  truncations whose argument is provably in range are plain casts (no Go out-of-range emulation)
-//   bit 7  the leaving class's summary / feasibility bits are stored after barrier.cluster.arrive (per-CTA identical stores)
-//   bit 4  with bit 0: one __syncthreads less in the class switch (nothing is transposed after the header is parsed)
-//   bit 5  the class record's offset is fetched one pod ahead and its length taken as the largest record's (no dependent
-//          global loads at the head of the class switch)
-//   bit 6  the per-node integer divisions of the totals pass by float-reciprocal estimate + exact fix-up
-#ifndef SIMON_OPT
-#define SIMON_OPT 125    // every option on: each was faster on C3 than the build without it
-#endif
-
 // ---- small helpers --------------------------------------------------------------------------------------
 __device__ __forceinline__ int32_t ldcg32(const int32_t *p) { return __ldcg(p); }
 
@@ -55,10 +39,10 @@ __device__ __forceinline__ int64_t div_by(int64_t x, int64_t d, double inv) {
     return q;
 }
 
-// SIMON_PINRUN=0 compiles the run-of-pinned-pods pass out (A/B builds; simon_pods_upload must then not mark pods: SIMON_OPT_NO_PIN_FAST)
-#ifndef SIMON_PINRUN
-#define SIMON_PINRUN 1
-#endif
+// whether a pod exists in the scenario: its guard is -2 (never), -1 (always) or the node whose presence it follows
+__device__ __forceinline__ bool pod_exists(const SkScenario &SC, int64_t guard) {
+    return guard == -2 ? false : (guard >= 0 ? (SC.rank_of ? SC.rank_of[guard] >= 0 : true) : true);
+}
 
 struct ReqCtx {
     const uint64_t *label_bits;
@@ -507,7 +491,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             // 0 <= score < 2^35: counts x ln(size) + (maxSkew - 1), maxSkew up to 2^31 - 1.  B_RAW_PTS holds the truncated score
             // less the class constant pts_off = sum(maxSkew - 1): exact, and it fits int32 because the compilers bound the counts
             // part (pods x soft constraints x ln(nodes + 2) < 2^31 - 2).  P3 adds pts_off back in int64.
-            int64_t raw = ((SIMON_OPT & 8) ? (int64_t)score : f2i(score)) - C.pts_off;
+            int64_t raw = (int64_t)score - C.pts_off;
             A32(B_RAW_PTS, idx) = (int32_t)raw;
             unsigned long long er = sk_enc(raw);
             lo = er < lo ? er : lo;
@@ -530,7 +514,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
     uint32_t i = DRAIN ? P.drain_off[scen_id] : P.first;
     const uint32_t q0 = DRAIN ? (i < end ? P.drain_pods[i] : 0u) : i;
     int32_t nx_cls = P.pod_class[q0], nx_fixed = P.pod_fixed[q0], nx_guard = P.pod_guard[q0];
-    uint64_t nx_off = (SIMON_OPT & 32) ? P.class_off[nx_cls] : 0;
+    uint64_t nx_off = P.class_off[nx_cls];
     // static-normalised part of the total (NodeAffinity + TaintToleration + 2 x Simon + extra) under the current normalisers
     auto snorm_pass = [&]() {
         const int64_t range = C.simon_max - C.simon_min;
@@ -561,15 +545,15 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
         RC.pin = (int32_t)guard;            // pods of pinned classes: the node their REQ_NODE_IS(-3) requirements name
         if (i + 1 < end) {
             const uint32_t q1 = SK_POD(i + 1);
-            nx_cls = P.pod_class[q1]; nx_fixed = P.pod_fixed[q1]; nx_guard = P.pod_guard[q1];
-            if (SIMON_OPT & 32) nx_off = P.class_off[nx_cls];
+            nx_cls = P.pod_class[q1]; nx_fixed = P.pod_fixed[q1]; nx_guard = P.pod_guard[q1]; nx_off = P.class_off[nx_cls];
         }
+        // pod_exists(SC, guard), written out: through the helper the compiler schedules the timer variants differently
         bool exists = true;
         if (guard == -2) exists = false;
         else if (guard >= 0) exists = SC.rank_of ? (SC.rank_of[guard] >= 0) : true;
 
         TICK(0);
-        if (!DRAIN && SIMON_PINRUN && exists && fixed == -4 && i != P.dump_pod) {
+        if (!DRAIN && exists && fixed == -4 && i != P.dump_pod) {
             // ---- run of pinned pods (DaemonSet pods whose dynamic filters are node-local; marked -4 by simon_pods_upload) ----
             // Such a pod can only land on its pin node (every other node fails NodeAffinity at the latest), and whether it does
             // depends on that node alone: NodeUnschedulable, TaintToleration and NodeAffinity of the pin, NodePorts on the node's own
@@ -695,7 +679,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             n_fail += run_f; n_sched += run_s;
             cur_class = -1;
             i = j;
-            if (i < end) { nx_cls = P.pod_class[i]; nx_fixed = P.pod_fixed[i]; nx_guard = P.pod_guard[i]; if (SIMON_OPT & 32) nx_off = P.class_off[nx_cls]; }
+            if (i < end) { nx_cls = P.pod_class[i]; nx_fixed = P.pod_fixed[i]; nx_guard = P.pod_guard[i]; nx_off = P.class_off[nx_cls]; }
             continue;
         }
         if (!DRAIN && (!exists || (fixed != -1 && fixed != -4))) {
@@ -703,16 +687,13 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             uint32_t j = i;
             while (j < end) {
                 int32_t f2 = P.pod_fixed[j];
-                int64_t g2 = P.pod_guard[j];
-                bool ex2 = g2 == -2 ? false : (g2 >= 0 ? (SC.rank_of ? SC.rank_of[g2] >= 0 : true) : true);
-                if (ex2 && (f2 == -1 || f2 == -4)) break;
+                if (pod_exists(SC, P.pod_guard[j]) && (f2 == -1 || f2 == -4)) break;
                 j++;
             }
             #pragma unroll 1
             for (uint32_t q = i; q < j; q++) {
                 int32_t f2 = P.pod_fixed[q];
-                int64_t g2 = P.pod_guard[q];
-                bool ex2 = g2 == -2 ? false : (g2 >= 0 ? (SC.rank_of ? SC.rank_of[g2] >= 0 : true) : true);
+                bool ex2 = pod_exists(SC, P.pod_guard[q]);
                 int32_t res;
                 if (!ex2) res = -3;
                 else if (f2 < 0) res = -2;
@@ -749,7 +730,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             cur_class = -1;
             TICK(1);
             i = j;
-            if (i < end) { nx_cls = P.pod_class[i]; nx_fixed = P.pod_fixed[i]; nx_guard = P.pod_guard[i]; if (SIMON_OPT & 32) nx_off = P.class_off[nx_cls]; }
+            if (i < end) { nx_cls = P.pod_class[i]; nx_fixed = P.pod_fixed[i]; nx_guard = P.pod_guard[i]; nx_off = P.class_off[nx_cls]; }
             continue;
         }
 
@@ -758,14 +739,13 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
         // =================================================================================================
         if (cls != cur_class) {
             st_class++;
-            // remember the summary of the class we leave: it is the prediction for its next visit
             // remember the class we leave: its summary AND the feasibility bits it is exact for.  On the next visit the
             // bits are restored and P1 detects any change against them, exactly as between two pods of one class.
-            auto save_class = [&]() {
+            // The leader stores the summary before the arrive below, whose release orders it for every CTA of the cluster.
+            // (A lambda run in place: as plain code here the compiler allocates the kernel's registers differently.)
+            [&]() {
             if (cur_class >= 0 && C.sum_valid && SC.csum && SC.fbits && !C.any_table && !C.pinned) {
-                // (bit 7: every CTA's thread 0 writes the record - the values are replicated, so the stores are identical - and a CTA
-                //  reads back what its own thread 0 wrote, ordered by __syncthreads: no cluster-scope ordering of these stores is needed)
-                if ((SIMON_OPT & 128) ? tid == 0 : leader) {
+                if (leader) {
                     long long *rec = SC.csum + (uint64_t)cur_class * SK_CSUM_W;
 #pragma unroll
                     for (int js = 0; js < SK_MAX_SOFT; js++) rec[1 + js] = (uint32_t)js < C.n_soft ? psz[js] : 0;
@@ -785,39 +765,30 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                     }
                 }
             }
-            };
-            if (!(SIMON_OPT & 128)) save_class();
+            }();
             TICK(10);
             // the previous commits' counter updates (owner-thread atomics) must be visible before the counters are read:
             // release here, acquire (barrier_wait) only where the first counter is loaded, so that the class blob, entry
-            // table and summary record loads overlap the barrier latency
-            // (SIMON_OPT bit 2: no separate fence - barrier.cluster.arrive is a release and .wait an acquire at cluster scope,
-            //  and every reader of the counters is a thread of this cluster)
-            if (!(SIMON_OPT & 4)) __threadfence();
+            // table and summary record loads overlap the barrier latency.  No fence before the arrive: barrier.cluster.arrive
+            // is a release and .wait an acquire at cluster scope, and every reader of the counters is a thread of this cluster.
             cluster.barrier_arrive();
             __syncthreads();          // every thread of this CTA is done with the previous class's blob and entry table
-            // bit 7: the leaving class's summary and feasibility bits are stored AFTER the arrive, so that its release does not wait
-            // for them (their only readers are this CTA's own threads, a class change later at the earliest)
-            if (SIMON_OPT & 128) save_class();
             TICK(11);
-            // (bit 5: the record's offset came with the pod one iteration ago; copying the largest record's length instead of this
-            //  one's reads into the next record - the upload pads the blob - and saves the dependent loads of the exact length)
-            const int64_t *gw = P.class_blob + ((SIMON_OPT & 32) ? cls_off : P.class_off[cls]);
-            const uint32_t words = (SIMON_OPT & 32) ? P.max_blob_words : (uint32_t)(P.class_off[cls + 1] - P.class_off[cls]);
+            // the record's offset came with the pod one iteration ago; copying the largest record's length instead of this one's
+            // reads into the next record (the upload pads the blob) and saves the dependent loads of the exact length
+            const int64_t *gw = P.class_blob + cls_off;
             #pragma unroll 1
-            for (uint32_t w = tid; w < words; w += TPB) S.blob[w] = gw[w];
+            for (uint32_t w = tid; w < P.max_blob_words; w += TPB) S.blob[w] = gw[w];
             // prediction of the topology sizes from the previous visit of this class (any value is safe: verified)
             if (tid < SK_CSUM_W) S.pred[tid] = SC.csum ? __ldcg(SC.csum + (uint64_t)cls * SK_CSUM_W + tid) : 0;
-            if (SIMON_OPT & 1) {
-                // commit list, counter bases and the int32 entry table as the upload laid them out
-                const uint32_t *ax = P.cls_aux + (uint64_t)cls * SK_AUX_W;
-                #pragma unroll 1
-                for (uint32_t w = tid; w < SK_AUX_W; w += TPB) {
-                    const uint32_t v = __ldg(ax + w);
-                    if (w <= SK_MAX_ENT) S.inc[w] = v;
-                    else if (w < SK_AUX_INCB + 32) S.incb[w - SK_AUX_INCB] = v;
-                    else if (w >= SK_AUX_ENT) S.ent[w - SK_AUX_ENT] = (int32_t)v;
-                }
+            // commit list, counter bases and the int32 entry table as the upload laid them out
+            const uint32_t *ax = P.cls_aux + (uint64_t)cls * SK_AUX_W;
+            #pragma unroll 1
+            for (uint32_t w = tid; w < SK_AUX_W; w += TPB) {
+                const uint32_t v = __ldg(ax + w);
+                if (w <= SK_MAX_ENT) S.inc[w] = v;
+                else if (w < SK_AUX_INCB + 32) S.incb[w - SK_AUX_INCB] = v;
+                else if (w >= SK_AUX_ENT) S.ent[w - SK_AUX_ENT] = (int32_t)v;
             }
             __syncthreads();
             const long long *pred = S.pred;
@@ -853,39 +824,9 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                 long long v = pred[1 + js];
                 psz[js] = (C.have_pred && v >= 0 && v + 2 < (long long)P.n_log) ? (int32_t)v : 0;
             }
-            if (!(SIMON_OPT & 1)) {
-                // the entry table was laid out by the snapshot compiler (SCW_OFF_ENT): 8 words per entry -> 8 rows in smem
-                const int64_t *et = cw + cw[SCW_OFF_ENT];
-#pragma unroll 1
-                for (uint32_t w = tid; w < C.E * 8; w += TPB) S.ent[(w & 7) * SK_MAX_ENT + (w >> 3)] = (int32_t)et[w];
-            }
-            if (!((SIMON_OPT & 1) && (SIMON_OPT & 16))) __syncthreads();
             C.pts_off = 0;
 #pragma unroll 1
             for (uint32_t js = 0; js < C.n_soft; js++) C.pts_off += (int64_t)ENT(ER_A, C.e_soft + js) - 1;
-            if (!(SIMON_OPT & 1) && tid < 32) {
-                // compact list of the entries this class increments on commit: entry | topology row << 8 | flags << 16
-                // (lane e looks at entry e; SK_MAX_ENT == 32)
-                const uint32_t e = tid;
-                uint32_t rec = 0;
-                bool inc = e < C.E && ENT(ER_INC, e) != 0;
-                if (inc) {
-                    const int32_t kind = ENT(ER_KIND, e);
-                    const bool host = kind == EK_SOFT && ENT(ER_B, e);
-                    rec = e | ((host ? 0u : (uint32_t)ENT(ER_T, e)) << 8) | ((kind == EK_SOFT && !host) ? 1u << 16 : 0u) |
-                          (kind == EK_AFF ? 1u << 17 : 0u);
-                }
-                // entries on topology row 0 (the node itself) can only match the winner's own node: they go to the end of the
-                // list and are applied by the owning thread alone; every thread walks the others
-                const bool node_lvl = inc && ((rec >> 8) & 0xff) == 0;
-                const uint32_t m_all = __ballot_sync(0xffffffffu, inc), m_node = __ballot_sync(0xffffffffu, node_lvl);
-                const uint32_t m_dom = m_all & ~m_node, lt = (1u << e) - 1u;
-                if (inc) S.inc[node_lvl ? __popc(m_dom) + __popc(m_node & lt) : __popc(m_dom & lt)] = rec;
-                const uint32_t n_aff_node = __popc(__ballot_sync(0xffffffffu, node_lvl && (rec & (1u << 17))));
-                if (e == 0) S.inc[SK_MAX_ENT] = __popc(m_dom) | (__popc(m_all) << 8) | (n_aff_node << 16);
-                // counter bases of the commit list: fetched once per class switch, not by the committing thread
-                if ((int64_t)e < cw[SCW_N_INC]) S.incb[e] = (uint32_t)P.cnt_off[(cw + cw[SCW_OFF_INC])[3 * e]];
-            }
             // ---- node-static verdicts: from the per-(static signature, node) cache, or computed and cached ----
             // All long-latency loads of up to 4 nodes (cache records, Simon row, first 4 counter values each) are issued back
             // to back before any of them is consumed.  The loads that do not depend on the counters (everything but the
@@ -1398,20 +1339,18 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                 else if (pmax == 0) pts = 100;
                 else if (pts32) {
                     const uint32_t x = 100u * (uint32_t)(pmax + pts_min - (int64_t)A32(B_RAW_PTS, idx)), d = (uint32_t)pmax;
-                    if (SIMON_OPT & 64) {
-                        // x < 2^31, quotient <= 200: the float estimate is off by < 1, one fix-up step makes it exact
-                        uint32_t q = (uint32_t)((float)x * pts_rinv);
-                        const int32_t r = (int32_t)(x - q * d);
-                        if (r < 0) q--;
-                        else if ((uint32_t)r >= d) q++;
-                        pts = (int64_t)q;
-                    } else pts = (int64_t)(x / d);
+                    // x < 2^31, quotient <= 200: the float estimate is off by < 1, one fix-up step makes it exact
+                    uint32_t q = (uint32_t)((float)x * pts_rinv);
+                    const int32_t r = (int32_t)(x - q * d);
+                    if (r < 0) q--;
+                    else if ((uint32_t)r >= d) q++;
+                    pts = (int64_t)q;
                 }
                 else pts = (100 * (pmax + pts_min - (int64_t)A32(B_RAW_PTS, idx))) / pmax;
                 int64_t ip = 0;
                 if (C.n_isc && ipa_diff > 0) {
                     const double fr = 100.0 * ((double)((int64_t)A32(B_RAW_IPA, idx) - ipa_min) / (double)ipa_diff);    // in [0, 100]
-                    ip = (SIMON_OPT & 8) ? (int64_t)fr : f2i(fr);
+                    ip = (int64_t)fr;
                 }
                 total = (int64_t)A32(B_OWN, idx) + (int64_t)A32(B_SNORM, idx) + ip + 2 * pts;
             }
@@ -1592,7 +1531,7 @@ extern "C" __global__ void __launch_bounds__(256) simon_import_kernel(const __gr
     for (uint32_t q = first + blockIdx.x * blockDim.x + threadIdx.x; q < first + count; q += gridDim.x * blockDim.x) {
         const int32_t f2 = placed ? placed[q] : P.pod_fixed[q];
         const int64_t g2 = P.pod_guard[q];
-        const bool ex2 = g2 == -2 ? false : (g2 >= 0 ? (SC.rank_of ? SC.rank_of[g2] >= 0 : true) : true);
+        const bool ex2 = pod_exists(SC, g2);
         int32_t res;
         if (!ex2) res = -3;
         else if (f2 < 0) res = placed ? f2 : -2;
@@ -1746,61 +1685,54 @@ extern "C" __global__ void __launch_bounds__(256) simon_drain_unimport(const __g
     }
 }
 
-// The placement kernel over per-scenario pod lists: one variant per thread count (node slots per thread at run time) and a
-// large-cluster one, none with Open-Local code (an evicted pod has no local volumes: such pods block a drain)
-extern "C" __global__ void __launch_bounds__(256, 1) simon_drain_kernel_256(const __grid_constant__ SkParams P) {
-    simon_place_body<256, 0, false, false, false, true>(P);
-}
-extern "C" __global__ void __launch_bounds__(320, 1) simon_drain_kernel_320(const __grid_constant__ SkParams P) {
-    simon_place_body<320, 0, false, false, false, true>(P);
-}
-extern "C" __global__ void __launch_bounds__(384, 1) simon_drain_kernel_384(const __grid_constant__ SkParams P) {
-    simon_place_body<384, 0, false, false, false, true>(P);
-}
-extern "C" __global__ void __launch_bounds__(320, 1) simon_drain_kernel_big(const __grid_constant__ SkParams P) {
-    simon_place_body<320, 0, false, true, false, true>(P);
-}
+// Every placement-family kernel, declared once: (symbol, threads per CTA at most, node slots per thread (0: counted at run time),
+// per-phase timers, large cluster, Open-Local, drain batch).  The kernels below and the table simon_api.cu's kernel_variant()
+// searches come from this list.
+//   - Unrolled node-slot loops for 1-4 slots at 256 and 320 threads and 1-3 at 384; the run-time slot count past those.
+//   - 384 threads = 12 warps = 3 per SM sub-partition, the same register ceiling (168) as 320 threads: one slot per thread less
+//     where the nodes of a CTA fall between the two (scenario batches on 9-CTA clusters: 3 slots instead of 4).  No timers.
+//   - The large-cluster variants keep per-node arrays in global memory.
+//   - Open-Local: one variant per thread count (run-time slots) and a large-cluster one.
+//   - Drain batches (per-scenario pod lists): the same, with no Open-Local code (an evicted pod has no local volumes: such pods
+//     block a drain).
+#define SIMON_PLACE_VARIANTS(X)                                       \
+    X(simon_place_kernel_256_0,  256, 0, false, false, false, false)  \
+    X(simon_place_kernel_256_1,  256, 1, false, false, false, false)  \
+    X(simon_place_kernel_256_2,  256, 2, false, false, false, false)  \
+    X(simon_place_kernel_256_3,  256, 3, false, false, false, false)  \
+    X(simon_place_kernel_256_4,  256, 4, false, false, false, false)  \
+    X(simon_place_kernel_320_0,  320, 0, false, false, false, false)  \
+    X(simon_place_kernel_320_1,  320, 1, false, false, false, false)  \
+    X(simon_place_kernel_320_2,  320, 2, false, false, false, false)  \
+    X(simon_place_kernel_320_3,  320, 3, false, false, false, false)  \
+    X(simon_place_kernel_320_4,  320, 4, false, false, false, false)  \
+    X(simon_place_kernel_384_0,  384, 0, false, false, false, false)  \
+    X(simon_place_kernel_384_1,  384, 1, false, false, false, false)  \
+    X(simon_place_kernel_384_2,  384, 2, false, false, false, false)  \
+    X(simon_place_kernel_384_3,  384, 3, false, false, false, false)  \
+    X(simon_place_kernel_big,    320, 0, false, true,  false, false)  \
+    X(simon_prof_kernel_256_0,   256, 0, true,  false, false, false)  \
+    X(simon_prof_kernel_256_1,   256, 1, true,  false, false, false)  \
+    X(simon_prof_kernel_256_2,   256, 2, true,  false, false, false)  \
+    X(simon_prof_kernel_256_3,   256, 3, true,  false, false, false)  \
+    X(simon_prof_kernel_256_4,   256, 4, true,  false, false, false)  \
+    X(simon_prof_kernel_320_0,   320, 0, true,  false, false, false)  \
+    X(simon_prof_kernel_320_1,   320, 1, true,  false, false, false)  \
+    X(simon_prof_kernel_320_2,   320, 2, true,  false, false, false)  \
+    X(simon_prof_kernel_320_3,   320, 3, true,  false, false, false)  \
+    X(simon_prof_kernel_320_4,   320, 4, true,  false, false, false)  \
+    X(simon_local_kernel_256,    256, 0, false, false, true,  false)  \
+    X(simon_local_kernel_320,    320, 0, false, false, true,  false)  \
+    X(simon_local_kernel_384,    384, 0, false, false, true,  false)  \
+    X(simon_local_kernel_big,    320, 0, false, true,  true,  false)  \
+    X(simon_drain_kernel_256,    256, 0, false, false, false, true)   \
+    X(simon_drain_kernel_320,    320, 0, false, false, false, true)   \
+    X(simon_drain_kernel_384,    384, 0, false, false, false, true)   \
+    X(simon_drain_kernel_big,    320, 0, false, true,  false, true)
 
-#define SIMON_KERNEL(MAXT, NPTT)                                                                         \
-    extern "C" __global__ void __launch_bounds__(MAXT, 1) simon_place_kernel_##MAXT##_##NPTT(const __grid_constant__ SkParams P) { \
-        simon_place_body<MAXT, NPTT, false>(P);                                                          \
-    }                                                                                                    \
-    extern "C" __global__ void __launch_bounds__(MAXT, 1) simon_prof_kernel_##MAXT##_##NPTT(const __grid_constant__ SkParams P) { \
-        simon_place_body<MAXT, NPTT, true>(P);                                                           \
+#define SK_DEFINE_VARIANT(name, threads, slots, prof, big, local, drain)                                   \
+    extern "C" __global__ void __launch_bounds__(threads, 1) name(const __grid_constant__ SkParams P) { \
+        simon_place_body<threads, slots, prof, big, local, drain>(P);                                    \
     }
-extern "C" __global__ void __launch_bounds__(320, 1) simon_place_kernel_big(const __grid_constant__ SkParams P) {
-    simon_place_body<320, 0, false, true>(P);
-}
-SIMON_KERNEL(256, 0)
-SIMON_KERNEL(256, 1)
-SIMON_KERNEL(256, 2)
-SIMON_KERNEL(256, 3)
-SIMON_KERNEL(256, 4)
-SIMON_KERNEL(320, 0)
-SIMON_KERNEL(320, 1)
-SIMON_KERNEL(320, 2)
-SIMON_KERNEL(320, 3)
-SIMON_KERNEL(320, 4)
-// 384 threads = 12 warps = 3 per SM sub-partition, the same register ceiling (168) as 320 threads: one slot per thread less where the
-// nodes of a CTA fall between the two (scenario batches on 9-CTA clusters: 3 slots instead of 4).  No profiling variants.
-#define SIMON_KERNEL_PLAIN(MAXT, NPTT)                                                                   \
-    extern "C" __global__ void __launch_bounds__(MAXT, 1) simon_place_kernel_##MAXT##_##NPTT(const __grid_constant__ SkParams P) { \
-        simon_place_body<MAXT, NPTT, false>(P);                                                          \
-    }
-SIMON_KERNEL_PLAIN(384, 0)
-SIMON_KERNEL_PLAIN(384, 1)
-SIMON_KERNEL_PLAIN(384, 2)
-SIMON_KERNEL_PLAIN(384, 3)
-// Open-Local: one variant per thread count (node slots per thread at run time) and a large-cluster one
-extern "C" __global__ void __launch_bounds__(256, 1) simon_local_kernel_256(const __grid_constant__ SkParams P) {
-    simon_place_body<256, 0, false, false, true>(P);
-}
-extern "C" __global__ void __launch_bounds__(320, 1) simon_local_kernel_320(const __grid_constant__ SkParams P) {
-    simon_place_body<320, 0, false, false, true>(P);
-}
-extern "C" __global__ void __launch_bounds__(384, 1) simon_local_kernel_384(const __grid_constant__ SkParams P) {
-    simon_place_body<384, 0, false, false, true>(P);
-}
-extern "C" __global__ void __launch_bounds__(320, 1) simon_local_kernel_big(const __grid_constant__ SkParams P) {
-    simon_place_body<320, 0, false, true, true>(P);
-}
+SIMON_PLACE_VARIANTS(SK_DEFINE_VARIANT)
+#undef SK_DEFINE_VARIANT

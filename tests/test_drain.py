@@ -4,17 +4,12 @@ CPU: remaining-node orders against node_tree_list, the classification of a remov
 fake runner, the drain checker (tests/drain_oracle.c) on hand-derived answers.  GPU: every drain kernel variant against the checker,
 drains against the recompile + simon_schedule_resume equivalence that pins the definition, the live state after a drain batch, and
 the session entry points end to end."""
-import os
-import re
-
 import numpy as np
 import pytest
 
 from simon_b200 import objects as O, scaledown, simulator, synth
 from simon_b200.compiler import compile_cluster, node_tree_list
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-KERNEL_SRC = os.path.join(HERE, "..", "open-simulator_b200", "csrc", "simon_kernel.cu")
+from util import compiled_kernels
 
 
 def _compiled(cluster, apps, **kw):
@@ -205,9 +200,8 @@ DRAIN_VARIANTS = {
 }
 
 
-def test_drain_variant_table_names_every_compiled_drain_variant():
-    names = set(re.findall(r"\b(simon_drain_kernel_\w+)\(const", open(KERNEL_SRC).read()))
-    assert set(DRAIN_VARIANTS) == names
+def test_drain_variant_table_names_every_drain_kernel_of_the_variant_list():
+    assert set(DRAIN_VARIANTS) == compiled_kernels("simon_drain_kernel_")
 
 
 # ---- GPU --------------------------------------------------------------------------------------------------------------------

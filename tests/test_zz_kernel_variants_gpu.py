@@ -13,7 +13,6 @@ pods, DaemonSet (pinned) pods, host ports, spread and affinity constraints.  The
 """
 import functools
 import os
-import re
 
 import numpy as np
 import pytest
@@ -21,9 +20,7 @@ import pytest
 from simon_b200 import simulator, synth
 from simon_b200.compiler import compile_cluster
 from test_daemonset_pins import _ds
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-KERNEL_SRC = os.path.join(HERE, "..", "open-simulator_b200", "csrc", "simon_kernel.cu")
+from util import compiled_kernels
 
 # kernel -> (cluster family, [(CTAs per scenario, threads per CTA, force_large)]); the families are built below
 VARIANTS = {
@@ -52,13 +49,10 @@ ENTRIES = [(k, fam, cs, t, big) for k, (fam, geoms) in VARIANTS.items() for cs, 
 
 def compiled_kernel_variants():
     """The placement kernels simon_kernel.cu defines, without the per-phase timer variants (simon_prof_kernel_*)."""
-    src = open(KERNEL_SRC).read()
-    names = {f"simon_place_kernel_{a}_{b}" for a, b in re.findall(r"^SIMON_KERNEL(?:_PLAIN)?\((\d+),\s*(\d+)\)", src, re.M)}
-    names |= set(re.findall(r"\b(simon_(?:place|local)_kernel_\w+)\(const", src))
-    return names
+    return compiled_kernels("simon_place_kernel_") | compiled_kernels("simon_local_kernel_")
 
 
-def test_variant_table_names_every_compiled_variant():
+def test_variant_table_names_every_placement_kernel_of_the_variant_list():
     names = compiled_kernel_variants()
     assert len(names) >= 19 and "simon_place_kernel_big" in names and "simon_local_kernel_big" in names
     assert set(VARIANTS) == names, f"kernels without a test: {sorted(names - set(VARIANTS))}, unknown: {sorted(set(VARIANTS) - names)}"

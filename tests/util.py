@@ -1,4 +1,7 @@
 """Shared helpers for the tests: build a plan + compiled cluster from a synthetic config."""
+import os
+import re
+
 import numpy as np
 
 from simon_b200 import simulator, synth
@@ -10,6 +13,20 @@ def make_case(kind="c3", **kw):
     p = simulator.plan(cluster, apps)
     c = compile_cluster(p.nodes, p.pods, p.ctx)
     return p, c
+
+
+KERNEL_SRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "open-simulator_b200", "csrc", "simon_kernel.cu")
+
+
+def compiled_kernels(prefix):
+    """The kernels named prefix* that simon_kernel.cu defines: the entries of its SIMON_PLACE_VARIANTS list, from which the kernels
+    and the host's variant table are generated, and any kernel defined outside that list."""
+    src = open(KERNEL_SRC).read()
+    m = re.search(r"^#define SIMON_PLACE_VARIANTS\(X\)((?:.*\\\n)*.*)", src, re.M)
+    assert m, "simon_kernel.cu has no SIMON_PLACE_VARIANTS list"
+    names = set(re.findall(r"\bX\((\w+),", m.group(1)))
+    names |= set(re.findall(r"\b(\w+)\(const __grid_constant__", src))
+    return {n for n in names if n.startswith(prefix)}
 
 
 def run_oracle(c):

@@ -1,6 +1,8 @@
 // micro-benchmark: cost of cluster barriers and of the engine's all-reduce primitives on a 16-CTA cluster
+// build (from the repository root):
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/ubench_cluster tools/ubench_cluster.cu
 #include <cstdio>
-#include "sk_experimental.cuh"
+#include "../open-simulator_b200/csrc/simon_kernel.cuh"
 
 extern "C" __global__ void k_sync(long long *out, int iters, int mode) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -18,7 +20,7 @@ extern "C" __global__ void k_sync(long long *out, int iters, int mode) {
     for (int i = 0; i < iters; i++) {
         if (mode == 0) cluster.sync();
         else if (mode == 1) { unsigned long long v[5] = {acc, acc + 1, acc + 2, acc + 3, acc & 1}; const int op[5] = {OP_MINU, OP_MAXU, OP_MINU, OP_MAXU, OP_OR}; sk_allreduce<5>(R, v, op); acc += v[1]; }
-        else if (mode == 2) { unsigned long long v[16]; int op[16]; for (int q = 0; q < 16; q++) { v[q] = acc + q; } const int opc[16] = {0,0,2,2,2,1,1,2,1,2,3,3,3,3,3,3}; sk_allreduce<16>(R, v, opc); acc += v[2]; }
+        else if (mode == 2) { unsigned long long v[16]; for (int q = 0; q < 16; q++) { v[q] = acc + q; } const int opc[16] = {0,0,2,2,2,1,1,2,1,2,3,3,3,3,3,3}; sk_allreduce<16>(R, v, opc); acc += v[2]; }
         else if (mode == 3) { uint32_t who; unsigned long long k = sk_argmax(R, ((acc & 0xffff) << 24) | (0xFFFFFFu - (cluster.block_rank() * blockDim.x + threadIdx.x)), cluster.num_blocks() * blockDim.x, blockDim.x, who); acc += k + sk_wpay(S, who, 0) + sk_wpay(S, who, S.T); }
         else if (mode == 4) __syncthreads();
         else if (mode == 5) { __threadfence(); cluster.sync(); }
@@ -42,20 +44,13 @@ extern "C" __global__ void k_sync(long long *out, int iters, int mode) {
         }
         else if (mode == 12) { uint32_t v[6] = {(uint32_t)acc, (uint32_t)acc + 1, (uint32_t)acc + 2, (uint32_t)acc + 3, (uint32_t)acc & 1, 1u}; const int op[6] = {W_MIN, W_MAX, W_MIN, W_MAX, W_OR, W_SUM}; sk_allreduce_w<6>(R, v, op); acc += v[1] + v[5]; }
         else if (mode == 13) { uint32_t v[22]; for (int q = 0; q < 22; q++) v[q] = (uint32_t)acc + q; const int op[22] = {0,0,2,2,2,1,1,2,1,2,3,3,3,3,3,3,3,3,3,3,3,3}; sk_allreduce_w<22>(R, v, op); acc += v[2] + v[0]; }
-        else if (mode == 14) {  // merged arg-max: key + payload + 7 words in ONE exchange
-            uint32_t who; uint32_t xw[7] = {(uint32_t)acc, (uint32_t)acc + 1, (uint32_t)acc + 2, (uint32_t)acc + 3, (uint32_t)acc & 1, 1u, 0u};
-            const int xop[7] = {W_MIN, W_MAX, W_MIN, W_MAX, W_OR, W_SUM, W_SUM};
-            const uint32_t ct = cluster.num_blocks() * blockDim.x;
-            sk_argmaxx_send<7>(R, ((acc & 0xffff) << 24) | (0xFFFFFFu - (cluster.block_rank() * blockDim.x + threadIdx.x)), ct, blockDim.x, xw, xop);
-            unsigned long long k = sk_argmaxx_wait<7>(R, who, xw, xop); acc += k + sk_wpay(S, who, 0) + xw[1] + xw[5];
-        }
-        else if (mode == 15) {  // what the merged form replaces: allreduce_w<7> followed by the plain arg-max
+        else if (mode == 14) {  // allreduce_w<7> followed by the arg-max
             uint32_t who; uint32_t xw[7] = {(uint32_t)acc, (uint32_t)acc + 1, (uint32_t)acc + 2, (uint32_t)acc + 3, (uint32_t)acc & 1, 1u, 0u};
             const int xop[7] = {W_MIN, W_MAX, W_MIN, W_MAX, W_OR, W_SUM, W_SUM};
             sk_allreduce_w<7>(R, xw, xop);
             unsigned long long k = sk_argmax(R, ((acc & 0xffff) << 24) | (0xFFFFFFu - (cluster.block_rank() * blockDim.x + threadIdx.x)), cluster.num_blocks() * blockDim.x, blockDim.x, who); acc += k + sk_wpay(S, who, 0) + xw[1] + xw[5];
         }
-        else if (mode == 16) {  // allreduce of 6 words with plain DSMEM stores + release/acquire flag polling (no mbarrier / async proxy)
+        else if (mode == 15) {  // allreduce of 6 words with plain DSMEM stores + release/acquire flag polling (no mbarrier / async proxy)
             const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
             const uint32_t CS = cluster.num_blocks(), buf = i & 1;
             uint32_t w[6] = {(uint32_t)acc, (uint32_t)acc + 1, (uint32_t)acc + 2, (uint32_t)acc + 3, (uint32_t)acc & 1, 1u};
@@ -103,8 +98,8 @@ extern "C" __global__ void k_sync(long long *out, int iters, int mode) {
 
 int main() {
     long long *d; cudaMalloc(&d, 64);
-    const char *names[17] = {"cluster.sync", "allreduce<5>", "allreduce<16>", "argmax", "__syncthreads", "threadfence+cluster.sync", "10x redux.max.u32 (dependent)", "10x warp_maxu64 (dependent)", "st.async self + mbar wait", "st.async next CTA + mbar wait", "redux+smem atomicMax+bar", "redux+slots+bar+fold", "allreduce_w<6> (32-bit words)", "allreduce_w<22> (32-bit words)", "merged arg-max + 7 words (1 exchange)", "allreduce_w<7> + arg-max (2 exchanges)", "allreduce 6 words, st.shared::cluster + flag polling"};
-    for (int cs : {1, 2, 4, 8, 16}) for (int tpb : {256, 320}) for (int mode = 0; mode < 17; mode++) {
+    const char *names[16] = {"cluster.sync", "allreduce<5>", "allreduce<16>", "argmax", "__syncthreads", "threadfence+cluster.sync", "10x redux.max.u32 (dependent)", "10x warp_maxu64 (dependent)", "st.async self + mbar wait", "st.async next CTA + mbar wait", "redux+smem atomicMax+bar", "redux+slots+bar+fold", "allreduce_w<6> (32-bit words)", "allreduce_w<22> (32-bit words)", "allreduce_w<7> + arg-max", "allreduce 6 words, st.shared::cluster + flag polling"};
+    for (int cs : {1, 2, 4, 8, 16}) for (int tpb : {256, 320}) for (int mode = 0; mode < 16; mode++) {
         size_t smem = sk_smem_bytes(tpb, 2, 4, 64, cs);
         cudaFuncSetAttribute(k_sync, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         cudaFuncSetAttribute(k_sync, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
