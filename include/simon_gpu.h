@@ -253,6 +253,10 @@ int simon_ctx_create(const simon_ctx_opts *opts, simon_ctx **out);
 void simon_ctx_destroy(simon_ctx *ctx);
 const char *simon_last_error(simon_ctx *ctx);
 
+/* Each upload checks its whole input before it changes the context: a refused upload (SIMON_ERR_INVALID, SIMON_ERR_LIMIT) leaves the
+ * context as it was, and the data uploaded earlier stays usable.  An accepted snapshot upload drops the pod set and everything
+ * uploaded or computed on it; an accepted pod upload drops the storage, device and PDB tables, the live placement, the last drain,
+ * storage batch and plan, and the move list with its last run (the move scope stays). */
 int simon_snapshot_upload(simon_ctx *ctx, const simon_snapshot *snap);
 int simon_pods_upload(simon_ctx *ctx, const simon_podset *pods);
 
@@ -387,6 +391,8 @@ typedef struct simon_moves_result {
     uint32_t reserved;
 } simon_moves_result;
 
+/* A move list indexes the pods and nodes it was uploaded for: a later snapshot or pod upload drops it, and simon_moves_run,
+ * simon_moves_replay and simon_moves_plan answer SIMON_ERR_STATE until the next simon_moves_upload. */
 int simon_moves_upload(simon_ctx *ctx, const simon_move *moves, uint32_t n_moves, uint32_t move_base);
 int simon_moves_run(simon_ctx *ctx, uint32_t k, int32_t *out_gain, uint32_t *out_code, uint64_t *out_best_per_pod,
                     simon_move_rank *out_topk, simon_moves_result *out);

@@ -161,7 +161,6 @@ struct ScenPool {
     std::vector<int32_t> h_rank;
     DevBuf<simon_scenario_result> results;
     DevBuf<simon_scenario_local_result> local_results;
-    uint32_t n_storage = 0;     // scenarios of the last storage batch whose Open-Local slices are kept (0: none since the last upload)
     // Open-Local, with storage uploaded: VG requested [n][V][N], allocated device slots [n][N] (with devices uploaded) and the
     // per-decision raw-score scratch [n][N] (clusters of a batch run concurrently: a shared one would be a race)
     DevBuf<int64_t> vg_req;
@@ -236,116 +235,163 @@ __global__ void simon_scen_reduce(const SkScenario *scen, const int64_t *alloc_m
     }
 }
 
+// What a context holds, one bit per owner of simon_ctx: the data of one upload or of the last run of one kind.  Validity::drop() is
+// the only place that clears a bit, and knows which data is derived from which.  Dropping data does not free its buffers: the
+// next upload of the same shape reuses them (DevBuf).
+enum Data : uint32_t {
+    SNAPSHOT = 1u << 0, POD_SET = 1u << 1, STORAGE = 1u << 2, DEVICES = 1u << 3, PDB_TABLE = 1u << 4,
+    LIVE = 1u << 5,             // the single-scenario pool holds a placement (schedule, resume, replay or a drain's rebuild)
+    MOVE_LIST = 1u << 6, MOVE_RUN = 1u << 7,
+    SCOPE_PREP = 1u << 8,       // what the move scope launches, for the current scope and move-class records
+    STATIC_FILL = 1u << 9,      // the static verdicts of every (signature, node) pair are in the pod set's scache
+    STORAGE_BATCH = 1u << 10, DRAIN_BATCH = 1u << 11, PLAN = 1u << 12,
+};
+
+struct Validity {
+    uint32_t bits = 0;
+    bool has(uint32_t d) const { return (bits & d) == d; }
+    void set(uint32_t d) { bits |= d; }
+    // d and everything derived from it.  Each row lists what is derived from its data directly, after the rows that drop that data.
+    void drop(uint32_t d) {
+        static constexpr uint32_t derived[][2] = {
+            {SNAPSHOT, POD_SET},
+            {POD_SET, STORAGE | PDB_TABLE | LIVE | PLAN | DRAIN_BATCH | MOVE_LIST | SCOPE_PREP | STATIC_FILL},
+            {STORAGE, DEVICES | STORAGE_BATCH | LIVE | SCOPE_PREP},     // SCOPE_PREP: the move-class records exclude local classes
+            {DEVICES, STORAGE_BATCH | LIVE},
+            {MOVE_LIST, MOVE_RUN},
+        };
+        for (const auto &r : derived)
+            if (d & r[0]) d |= r[1];
+        bits &= ~d;
+    }
+};
+
 struct simon_ctx {
     int device = 0, sms = 132;          // sms: the device's multiprocessor count
     uint32_t opt_cluster = 0, opt_threads = 0, opt_flags = 0;
     cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-    float last_ms = 0.f;
-    uint64_t launches = 0;
     std::string err;
-    bool have_snap = false, have_pods = false;
-    // snapshot
-    uint32_t N = 0, K = 0, WL = 0, WT = 0, T = 0, NC = 0, n_log = 0, max_dom = 1;
-    std::vector<uint32_t> topo_ndom;
-    DevBuf<uint32_t> d_topo_ndom, d_node_flags;
-    DevBuf<int64_t> d_alloc_mcpu, d_alloc_mem, d_alloc_eph, d_alloc_scalar, d_gpu_dev_mem, d_gpu_total_mem;
-    DevBuf<int32_t> d_alloc_pods, d_topo_dom, d_node_class, d_gpu_count;
-    DevBuf<uint64_t> d_label_bits, d_taint_hard, d_taint_soft;
-    DevBuf<double> d_log;
-    // pods
-    uint32_t n_classes = 0, n_pods = 0, n_counters = 0, max_blob_words = 0, emax = 0;
-    uint64_t cnt_words = 0;
-    DevBuf<uint64_t> d_class_off, d_cnt_off;
-    DevBuf<int64_t> d_class_blob, d_simon_raw;
-    DevBuf<int32_t> d_pod_class, d_pod_fixed, d_pod_guard, d_extra;
-    DevBuf<uint32_t> d_cls_aux;
-    // debug dump of one pod's per-node totals / filter verdicts (simon_debug_*)
-    uint32_t dump_pod = 0xffffffffu;
-    DevBuf<long long> d_dump_total;
-    DevBuf<int32_t> d_dump_code;
-    // candidate-move scoring (simon_moves_*)
-    DevBuf<uint2> d_moves;
-    DevBuf<int32_t> d_mv_gain;
-    DevBuf<uint32_t> d_mv_code, d_mv_hist, d_mv_topn;
-    DevBuf<unsigned long long> d_mv_best_pod, d_mv_best;
-    DevBuf<uint2> d_mv_topk;
-    DevBuf<SmvNode> d_mv_nodes;
-    DevBuf<SmvClass> d_mv_classes;
-    DevBuf<SmvPod> d_mv_pods;
-    uint32_t mv_n = 0, mv_base = 0;
-    // move scope (simon_moves_set_scope): per class SmvClass::bits on the host, the (class, hard constraint) pairs with their
-    // bitmap offsets, and what the current scope launches (rebuilt when the scope or the classes change)
-    uint32_t mv_scope = 0, mv_last_scope = 0;
-    bool mv_ran = false, mv_scope_dirty = true, mv_scoped = false;
-    std::vector<uint32_t> h_mv_bits;
-    std::vector<uint4> h_mv_pairs;
-    uint32_t mv_n_prep = 0;
-    DevBuf<uint4> d_mv_prep;
-    DevBuf<uint32_t> d_mv_hreg, d_mv_slots;
-    DevBuf<int2> d_mv_hs;
-    DevBuf<SmvGpu> d_mv_gpu;
-    // migration plans (simon_moves_plan): plan-owned copies of the single-scenario node state, placement and GPU slot words, the steps
-    // and control words.  have_live: the single-scenario state holds a placement (a schedule, resume, replay or drain rebuild since the
-    // last pod upload or reset); pl_valid: the plan columns hold the last plan's end state
-    bool have_live = false, pl_valid = false;
-    NodeState pl_state;
-    DevBuf<int32_t> pl_place;
-    DevBuf<uint32_t> pl_slots, pl_ctl;
-    DevBuf<simon_plan_step> pl_steps;
-    uint32_t n_pin_fast = 0;           // pods marked for the pinned-run fast path (-4 in the device copy of pod_fixed_node)
-    std::vector<uint8_t> bypass;        // per pod: never reaches the scheduler in a single-scenario run (pre-bound or absent)
-    // resumed runs (simon_schedule_resume): per pod the uploaded pod_fixed_node and guard (what its prefix entry is checked against),
-    // the prefix on the device and its per-node grouping (counts, offsets, fill cursors, pod list)
-    std::vector<int32_t> h_fixed, h_guard;
-    DevBuf<int32_t> d_prefix;
-    DevBuf<uint32_t> d_rs_cnt, d_rs_off, d_rs_cur, d_rs_list;
-    DevBuf<unsigned char> d_gnode;      // large-cluster variant: per-node arrays in global memory
-    bool big = false;                   // set by choose_geometry for the next launch
-    size_t gnode_stride = 0;
-    uint32_t geom_nodes = 0;            // the node count choose_geometry sized the next launch for
-    simon_launch_info last_launch{};    // what the last scheduling call launched (simon_last_launch)
-    DevBuf<uint32_t> d_sig_class;       // a class per static signature (dense fill of the static verdict cache)
-    bool static_filled = false;
+    Validity valid;
+    struct {
+        uint32_t N = 0, K = 0, WL = 0, WT = 0, T = 0, NC = 0, n_log = 0, max_dom = 1;
+        std::vector<uint32_t> topo_ndom;
+        DevBuf<uint32_t> d_topo_ndom, d_node_flags;
+        DevBuf<int64_t> d_alloc_mcpu, d_alloc_mem, d_alloc_eph, d_alloc_scalar, d_gpu_dev_mem, d_gpu_total_mem;
+        DevBuf<int32_t> d_alloc_pods, d_topo_dom, d_node_class, d_gpu_count;
+        DevBuf<uint64_t> d_label_bits, d_taint_hard, d_taint_soft;
+        DevBuf<double> d_log;
+    } snap;
+    struct {
+        uint32_t n_classes = 0, n_pods = 0, n_counters = 0, max_blob_words = 0, emax = 0;
+        uint64_t cnt_words = 0;
+        DevBuf<uint64_t> d_class_off, d_cnt_off;
+        DevBuf<int64_t> d_class_blob, d_simon_raw;
+        DevBuf<int32_t> d_pod_class, d_pod_fixed, d_pod_guard, d_extra;
+        DevBuf<uint32_t> d_cls_aux;
+        // per pod: the uploaded pod_fixed_node and guard (what a resume prefix entry is checked against), the class, whether it never
+        // reaches the scheduler in a single-scenario run (pre-bound or absent); fixed_dev: pod_fixed_node with the pinned-run marks
+        // (-4) before a storage upload takes its local classes off (d_pod_fixed holds the result)
+        std::vector<int32_t> h_fixed, h_guard, h_class, fixed_dev;
+        std::vector<uint8_t> bypass;
+        DevBuf<uint32_t> d_sig_class;       // a class per static signature (dense fill of the static verdict cache)
+        uint32_t max_fail = 0;
+        DevBuf<unsigned long long> d_stats, d_scache;
+        uint32_t n_sigs = 1, use_scache = 0, simon32 = 0;
+        // debug dump of one pod's per-node totals / filter verdicts (simon_debug_*)
+        uint32_t dump_pod = 0xffffffffu;
+        DevBuf<long long> d_dump_total;
+        DevBuf<int32_t> d_dump_code;
+        // move scoring: the per-class SmvClass records before a storage upload marks its local classes (d_mv_classes and mv_bits, the
+        // records' bits on the host, hold the result), the (class, hard constraint) pairs with their bitmap offsets, and the scratch
+        // of scoped runs sized by the classes
+        std::vector<SmvClass> mv_classes;
+        DevBuf<SmvClass> d_mv_classes;
+        std::vector<uint32_t> mv_bits;
+        std::vector<uint4> mv_pairs;
+        DevBuf<uint32_t> d_mv_hreg;
+        DevBuf<int2> d_mv_hs;
+    } pods;
+    // Open-Local LVM volumes (simon_storage_upload); VG requested [V][N] as uploaded (every scenario starts from it)
+    struct {
+        uint32_t V = 0;
+        DevBuf<int32_t> d_node_n_vg, d_vg_name, d_vol_vg;
+        DevBuf<int64_t> d_vg_cap, d_vg_req0, d_vol_size;
+        DevBuf<uint8_t> d_class_local;
+        DevBuf<uint32_t> d_vol_off;
+        std::vector<uint8_t> h_class_local;
+    } storage;
+    // Open-Local devices (simon_devices_upload); allocated-slot masks [N] as uploaded
+    struct {
+        DevBuf<uint8_t> d_node_n_ssd, d_node_n_hdd;
+        DevBuf<int64_t> d_dev_cap, d_ssd_size, d_hdd_size;
+        DevBuf<uint32_t> d_ssd_off, d_hdd_off, d_dev_alloc0;
+    } devices;
+    // PodDisruptionBudgets (simon_pdbs_upload): n PDBs, the pod -> PDB CSR (also on the host, for drains), the PDB -> pod CSR and the
+    // desired counts; d_rem holds `allowed` of the last computation, and a plan's remaining budgets; d_ctl the plan's step watch (seen
+    // steps, PDBs that reached 0, blocked pods), d_hit the ids of those PDBs
+    struct {
+        uint32_t n = 0, max_per_pod = 0, max_members = 0;
+        std::vector<uint32_t> h_off, h_ids;
+        DevBuf<uint32_t> d_off, d_ids, d_moff, d_members, d_ctl, d_hit;
+        DevBuf<int32_t> d_desired, d_rem;
+    } pdb;
+    // candidate-move scoring (simon_moves_*): the move list and move_base, the move kernel's outputs and scratch, the packed records
+    struct {
+        uint32_t n = 0, base = 0;
+        DevBuf<uint2> d_moves, d_topk;
+        DevBuf<int32_t> d_gain;
+        DevBuf<uint32_t> d_code, d_hist, d_topn, d_slots;
+        DevBuf<unsigned long long> d_best_pod, d_best;
+        DevBuf<SmvNode> d_nodes;
+        DevBuf<SmvPod> d_pods;
+        DevBuf<SmvGpu> d_gpu;
+    } moves;
+    // move scope (simon_moves_set_scope), and what it launches: the scoped kernel iff some class is admitted, the prep pairs of the
+    // admitted hard classes
+    struct {
+        uint32_t bits = 0;
+        bool scoped = false;
+        uint32_t n_prep = 0;
+        DevBuf<uint4> d_prep;
+    } scope;
+    struct { uint32_t scope = 0; } move_run;        // the scope of the last simon_moves_run
+    struct { uint32_t n = 0; } storage_batch;       // scenarios of the last storage batch, whose Open-Local slices the batch pool keeps
+    // the last drain batch (simon_drain_run): n scenarios, per scenario its evicted pods (CSR off / pods, pod order), blocked pods
+    // (boff / blocked) and failures; on the device the evicted pods' nodes, scores, GPU slots and failure records (max rows per
+    // scenario: its largest evictee list); per drain its violated PDBs, ascending, and their evicted members (CSR voff); the device
+    // times of the setup (ev0 .. evm) and the placement (evm .. ev1)
+    struct {
+        uint32_t n = 0, max = 0;
+        std::vector<uint32_t> off, pods, boff, blocked, nfail, voff, vpdb, vcnt;
+        DevBuf<uint32_t> d_pods, d_off, d_gpu, d_fail_counts, d_fail_pod;
+        DevBuf<int32_t> d_node;
+        DevBuf<int64_t> d_score;
+        DevBuf<uint2> d_pairs;
+        float setup_ms = 0.f, place_ms = 0.f;
+    } drain;
+    // the last migration plan (simon_moves_plan): its end state in plan-owned copies of the single-scenario node state, placement and
+    // GPU slot words, the steps and control words
+    struct {
+        NodeState state;
+        DevBuf<int32_t> place;
+        DevBuf<uint32_t> slots, ctl;
+        DevBuf<simon_plan_step> steps;
+    } plan;
     // scenario state: single runs (simon_schedule, simon_replay, ...) and scenario batches
     ScenPool single, batch;
-    uint32_t max_fail = 0;
-    DevBuf<unsigned long long> d_stats, d_scache;
-    uint32_t n_sigs = 1, use_scache = 0, simon32 = 0;
-    // Open-Local LVM volumes (simon_storage_upload); VG requested [V][N] as uploaded (every scenario starts from it)
-    bool have_storage = false;
-    uint32_t V = 0;
-    DevBuf<int32_t> d_node_n_vg, d_vg_name, d_vol_vg;
-    DevBuf<int64_t> d_vg_cap, d_vg_req0, d_vol_size;
-    DevBuf<uint8_t> d_class_local;
-    DevBuf<uint32_t> d_vol_off;
-    std::vector<uint8_t> h_class_local;
-    // Open-Local devices (simon_devices_upload); allocated-slot masks [N] as uploaded
-    bool have_devices = false;
-    DevBuf<uint8_t> d_node_n_ssd, d_node_n_hdd;
-    DevBuf<int64_t> d_dev_cap, d_ssd_size, d_hdd_size;
-    DevBuf<uint32_t> d_ssd_off, d_hdd_off, d_dev_alloc0;
-    // drain batches (simon_drain_run).  The last batch: dr_n scenarios (0: none since the last upload), per scenario its evicted pods (CSR dr_off / dr_pods, pod order),
-    // blocked pods (dr_boff / dr_blocked) and failures; on the device the evicted pods' nodes, scores, GPU slots and failure records
-    // (dr_max rows per scenario: its largest evictee list); the device times of the setup (ev0 .. evm) and the placement (evm .. ev1)
-    std::vector<int32_t> h_class;
-    cudaEvent_t evm = nullptr;
-    uint32_t dr_n = 0, dr_max = 0;
-    std::vector<uint32_t> dr_off, dr_pods, dr_boff, dr_blocked, dr_nfail;
-    DevBuf<uint32_t> d_dr_pods, d_dr_off, d_dr_gpu, d_dr_fail_counts, d_dr_fail_pod;
-    DevBuf<int32_t> d_dr_node;
-    DevBuf<int64_t> d_dr_score;
-    DevBuf<uint2> d_dr_pairs;
-    float dr_setup_ms = 0.f, dr_place_ms = 0.f;
-    // PodDisruptionBudgets (simon_pdbs_upload; n_pdbs 0: no table): the pod -> PDB CSR (also on the host, for drains), the PDB -> pod
-    // CSR and the desired counts; d_pdb_rem holds `allowed` of the last computation, and a plan's remaining budgets; d_pdb_ctl the
-    // plan's step watch (seen steps, PDBs that reached 0, blocked pods), d_pdb_hit the ids of those PDBs
-    uint32_t n_pdbs = 0, pdb_max_per_pod = 0, pdb_max_members = 0;
-    std::vector<uint32_t> h_pdb_off, h_pdb_ids;
-    DevBuf<uint32_t> d_pdb_off, d_pdb_ids, d_pdb_moff, d_pdb_members, d_pdb_ctl, d_pdb_hit;
-    DevBuf<int32_t> d_pdb_desired, d_pdb_rem;
-    // per drain of the last batch: its violated PDBs, ascending, and their evicted members (CSR dr_voff)
-    std::vector<uint32_t> dr_voff, dr_vpdb, dr_vcnt;
+    // launch scratch of no upload: resumed runs' prefix on the device and its per-node grouping (counts, offsets, fill cursors, pod
+    // list); the large-cluster variant's per-node arrays; the geometry choose_geometry sized the next launch for; what the last
+    // scheduling call launched (simon_last_launch); device times and launch count
+    DevBuf<int32_t> d_prefix;
+    DevBuf<uint32_t> d_rs_cnt, d_rs_off, d_rs_cur, d_rs_list;
+    DevBuf<unsigned char> d_gnode;
+    bool big = false;
+    size_t gnode_stride = 0;
+    uint32_t geom_nodes = 0;
+    simon_launch_info last_launch{};
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr, evm = nullptr;
+    float last_ms = 0.f;
+    uint64_t launches = 0;
 };
 
 namespace {
@@ -405,8 +451,8 @@ int clear_pool(simon_ctx *ctx, ScenPool &s) {
     // inherit them (the kernel validates a summary only against flips of nodes it currently owns)
     CU(cudaMemsetAsync(s.csum.p, 0, 8 * n * s.ncl * SK_CSUM_W, st));
     // VG requested and the devices restart from what the node annotations state
-    if (ctx->have_storage) CU(bcast(ctx, ctx->d_vg_req0.p, s.vn, s.n, s.vg_req.p));
-    if (ctx->have_devices) CU(bcast(ctx, ctx->d_dev_alloc0.p, s.nodes, s.n, s.dev_alloc.p));
+    if (ctx->valid.has(STORAGE)) CU(bcast(ctx, ctx->storage.d_vg_req0.p, s.vn, s.n, s.vg_req.p));
+    if (ctx->valid.has(DEVICES)) CU(bcast(ctx, ctx->devices.d_dev_alloc0.p, s.nodes, s.n, s.dev_alloc.p));
     return SIMON_OK;
 }
 
@@ -415,19 +461,19 @@ int clear_pool(simon_ctx *ctx, ScenPool &s) {
 template <typename F>
 cudaError_t pool_columns(const simon_ctx *ctx, ScenPool &s, uint32_t n, bool single, bool pod_outputs, F &&f) {
     s.n = n;
-    s.state.shape(n, ctx->N, ctx->K, ctx->cnt_words, ctx->n_counters);
-    s.nodes = std::max(1u, ctx->N); s.ncl = std::max(1u, ctx->n_classes);
-    s.tabw = (size_t)SK_MAX_SOFT * ctx->max_dom; s.regw = (size_t)SK_MAX_HARD * ctx->max_dom; s.pods = pod_outputs ? std::max(1u, ctx->n_pods) : 1;
-    s.vn = std::max<size_t>(1, (size_t)ctx->V * ctx->N);
+    s.state.shape(n, ctx->snap.N, ctx->snap.K, ctx->pods.cnt_words, ctx->pods.n_counters);
+    s.nodes = std::max(1u, ctx->snap.N); s.ncl = std::max(1u, ctx->pods.n_classes);
+    s.tabw = (size_t)SK_MAX_SOFT * ctx->snap.max_dom; s.regw = (size_t)SK_MAX_HARD * ctx->snap.max_dom; s.pods = pod_outputs ? std::max(1u, ctx->pods.n_pods) : 1;
+    s.vn = std::max<size_t>(1, (size_t)ctx->storage.V * ctx->snap.N);
     cudaError_t e = s.state.each(s.state, true, [&](auto &c, auto &, uint64_t k) { return f(c, k); });
     auto col = [&](auto &c, size_t count) { if (e == cudaSuccess) e = f(c, count); };
     col(s.tp, s.tabw); col(s.fcount, s.tabw); col(s.size, SK_MAX_SOFT); col(s.hard_reg, s.regw);
     col(s.csum, s.ncl * SK_CSUM_W); col(s.fbits, s.nodes * s.ncl); col(s.ocache, s.nodes * s.ncl);
     col(s.out_node, s.pods); col(s.counters, 2); col(s.clk, 2); col(s.scen, 1);
     if (!single) { col(s.order, s.nodes); col(s.rank_of, s.nodes); col(s.results, 1); }
-    if (!single && ctx->have_storage) col(s.local_results, 1);
-    if (ctx->have_storage) { col(s.vg_req, s.vn); col(s.local_raw, s.nodes); }
-    if (ctx->have_devices) col(s.dev_alloc, s.nodes);
+    if (!single && ctx->valid.has(STORAGE)) col(s.local_results, 1);
+    if (ctx->valid.has(STORAGE)) { col(s.vg_req, s.vn); col(s.local_raw, s.nodes); }
+    if (ctx->valid.has(DEVICES)) col(s.dev_alloc, s.nodes);
     return e;
 }
 
@@ -436,12 +482,12 @@ cudaError_t pool_columns(const simon_ctx *ctx, ScenPool &s, uint32_t n, bool sin
 int size_pool(simon_ctx *ctx, ScenPool &s, uint32_t n, bool single, bool pod_outputs = true) {
     CU(pool_columns(ctx, s, n, single, pod_outputs, [&](auto &c, size_t k) { return c.alloc(n * k); }));
     if (single) {
-        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(s.out_score.alloc(ctx->n_pods));
-        CU(s.out_gpu.alloc(ctx->n_pods));
-        CU(s.fail_counts.alloc((size_t)ctx->max_fail * SIMON_N_FAIL_CODES)); CU(s.fail_pod.alloc(ctx->max_fail));
+        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(s.out_score.alloc(ctx->pods.n_pods));
+        CU(s.out_gpu.alloc(ctx->pods.n_pods));
+        CU(s.fail_counts.alloc((size_t)ctx->pods.max_fail * SIMON_N_FAIL_CODES)); CU(s.fail_pod.alloc(ctx->pods.max_fail));
         // fbits are cleared here for single runs and never for batches: the kernel reads them only under a valid csum record
         CU(cudaMemsetAsync(s.fbits.p, 0, (size_t)n * s.nodes * s.ncl, ctx->stream));
-        const SkScenario sc = fill_scen(s, 0, ctx->N, true);
+        const SkScenario sc = fill_scen(s, 0, ctx->snap.N, true);
         CU(cudaMemcpyAsync(s.scen.p, &sc, sizeof(sc), cudaMemcpyHostToDevice, ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));        // `sc` leaves scope
     }
@@ -457,30 +503,30 @@ int alloc_pool(simon_ctx *ctx, ScenPool &s, uint32_t n, bool single) {
 // the launch parameters of the current uploads on pool `s` (its SkScenario array and Open-Local slices)
 void fill_params(simon_ctx *ctx, const ScenPool &s, SkParams &P) {
     memset(&P, 0, sizeof(P));
-    P.N = ctx->N; P.K = ctx->K; P.WL = ctx->WL; P.WT = ctx->WT; P.T = ctx->T; P.NC = ctx->NC; P.n_log = ctx->n_log; P.max_dom = ctx->max_dom;
-    P.topo_ndom = ctx->d_topo_ndom.p; P.alloc_mcpu = ctx->d_alloc_mcpu.p; P.alloc_mem = ctx->d_alloc_mem.p; P.alloc_eph = ctx->d_alloc_eph.p;
-    P.alloc_scalar = ctx->d_alloc_scalar.p; P.alloc_pods = ctx->d_alloc_pods.p; P.node_flags = ctx->d_node_flags.p;
-    P.label_bits = ctx->d_label_bits.p; P.taint_hard = ctx->d_taint_hard.p; P.taint_soft = ctx->d_taint_soft.p;
-    P.topo_dom = ctx->d_topo_dom.p; P.node_class = ctx->d_node_class.p; P.gpu_count = ctx->d_gpu_count.p;
-    P.gpu_dev_mem = ctx->d_gpu_dev_mem.p; P.gpu_total_mem = ctx->d_gpu_total_mem.p; P.log_table = ctx->d_log.p;
-    P.n_classes = ctx->n_classes; P.n_pods = ctx->n_pods; P.n_counters = ctx->n_counters; P.max_blob_words = ctx->max_blob_words;
-    P.class_off = ctx->d_class_off.p; P.class_blob = ctx->d_class_blob.p; P.pod_class = ctx->d_pod_class.p;
-    P.pod_fixed = ctx->d_pod_fixed.p; P.pod_guard = ctx->d_pod_guard.p; P.cnt_off = ctx->d_cnt_off.p;
-    P.simon_raw = ctx->d_simon_raw.p; P.extra_score = ctx->d_extra.p;
-    P.emax = ctx->emax;
-    P.stats = ctx->d_stats.p;
-    P.n_sigs = ctx->n_sigs; P.use_scache = ctx->use_scache; P.simon32 = ctx->simon32; P.scache = ctx->d_scache.p;
-    P.cls_aux = ctx->d_cls_aux.p;
+    P.N = ctx->snap.N; P.K = ctx->snap.K; P.WL = ctx->snap.WL; P.WT = ctx->snap.WT; P.T = ctx->snap.T; P.NC = ctx->snap.NC; P.n_log = ctx->snap.n_log; P.max_dom = ctx->snap.max_dom;
+    P.topo_ndom = ctx->snap.d_topo_ndom.p; P.alloc_mcpu = ctx->snap.d_alloc_mcpu.p; P.alloc_mem = ctx->snap.d_alloc_mem.p; P.alloc_eph = ctx->snap.d_alloc_eph.p;
+    P.alloc_scalar = ctx->snap.d_alloc_scalar.p; P.alloc_pods = ctx->snap.d_alloc_pods.p; P.node_flags = ctx->snap.d_node_flags.p;
+    P.label_bits = ctx->snap.d_label_bits.p; P.taint_hard = ctx->snap.d_taint_hard.p; P.taint_soft = ctx->snap.d_taint_soft.p;
+    P.topo_dom = ctx->snap.d_topo_dom.p; P.node_class = ctx->snap.d_node_class.p; P.gpu_count = ctx->snap.d_gpu_count.p;
+    P.gpu_dev_mem = ctx->snap.d_gpu_dev_mem.p; P.gpu_total_mem = ctx->snap.d_gpu_total_mem.p; P.log_table = ctx->snap.d_log.p;
+    P.n_classes = ctx->pods.n_classes; P.n_pods = ctx->pods.n_pods; P.n_counters = ctx->pods.n_counters; P.max_blob_words = ctx->pods.max_blob_words;
+    P.class_off = ctx->pods.d_class_off.p; P.class_blob = ctx->pods.d_class_blob.p; P.pod_class = ctx->pods.d_pod_class.p;
+    P.pod_fixed = ctx->pods.d_pod_fixed.p; P.pod_guard = ctx->pods.d_pod_guard.p; P.cnt_off = ctx->pods.d_cnt_off.p;
+    P.simon_raw = ctx->pods.d_simon_raw.p; P.extra_score = ctx->pods.d_extra.p;
+    P.emax = ctx->pods.emax;
+    P.stats = ctx->pods.d_stats.p;
+    P.n_sigs = ctx->pods.n_sigs; P.use_scache = ctx->pods.use_scache; P.simon32 = ctx->pods.simon32; P.scache = ctx->pods.d_scache.p;
+    P.cls_aux = ctx->pods.d_cls_aux.p;
     P.dump_pod = 0xffffffffu; P.dump_total = nullptr; P.dump_code = nullptr;
     P.scen = s.scen.p;
-    if (ctx->have_storage) {
-        P.V = ctx->V; P.node_n_vg = ctx->d_node_n_vg.p; P.vg_name = ctx->d_vg_name.p; P.vg_cap = ctx->d_vg_cap.p;
-        P.class_local = ctx->d_class_local.p; P.vol_off = ctx->d_vol_off.p; P.vol_size = ctx->d_vol_size.p; P.vol_vg = ctx->d_vol_vg.p;
+    if (ctx->valid.has(STORAGE)) {
+        P.V = ctx->storage.V; P.node_n_vg = ctx->storage.d_node_n_vg.p; P.vg_name = ctx->storage.d_vg_name.p; P.vg_cap = ctx->storage.d_vg_cap.p;
+        P.class_local = ctx->storage.d_class_local.p; P.vol_off = ctx->storage.d_vol_off.p; P.vol_size = ctx->storage.d_vol_size.p; P.vol_vg = ctx->storage.d_vol_vg.p;
         P.vg_req = s.vg_req.p; P.local_raw = s.local_raw.p; P.vg_req_stride = s.vn; P.node_stride = s.nodes;
     }
-    if (ctx->have_devices) {
-        P.node_n_ssd = ctx->d_node_n_ssd.p; P.node_n_hdd = ctx->d_node_n_hdd.p; P.dev_cap = ctx->d_dev_cap.p;
-        P.ssd_off = ctx->d_ssd_off.p; P.ssd_size = ctx->d_ssd_size.p; P.hdd_off = ctx->d_hdd_off.p; P.hdd_size = ctx->d_hdd_size.p;
+    if (ctx->valid.has(DEVICES)) {
+        P.node_n_ssd = ctx->devices.d_node_n_ssd.p; P.node_n_hdd = ctx->devices.d_node_n_hdd.p; P.dev_cap = ctx->devices.d_dev_cap.p;
+        P.ssd_off = ctx->devices.d_ssd_off.p; P.ssd_size = ctx->devices.d_ssd_size.p; P.hdd_off = ctx->devices.d_hdd_off.p; P.hdd_size = ctx->devices.d_hdd_size.p;
         P.dev_alloc = s.dev_alloc.p;
     }
 }
@@ -502,7 +548,7 @@ const sk_variant sk_variants[] = {SIMON_PLACE_VARIANTS(SK_VARIANT_ENTRY)};
 const sk_variant *kernel_variant(const simon_ctx *ctx, uint32_t TPB, uint32_t npt, bool big, bool prof, bool drain) {
     if (!big && TPB > SIMON_MAX_TPB) return nullptr;
     const uint32_t threads = TPB <= 256 ? 256 : TPB <= 320 ? 320 : 384;
-    const bool local = ctx->have_storage && !drain;
+    const bool local = ctx->valid.has(STORAGE) && !drain;
     if (big || drain) prof = false;
     const sk_variant *runtime_slots = nullptr;
     for (const sk_variant &v : sk_variants) {
@@ -563,12 +609,12 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
         if (cs > SK_MAX_CS) return fail(ctx, SIMON_ERR_LIMIT, "CTAs per scenario must be <= %u (got %u)", (unsigned)SK_MAX_CS, cs);
         if (t > 320) return fail(ctx, SIMON_ERR_LIMIT, "the large-cluster variant runs at most 320 threads per CTA (got %u)", t);
         const uint32_t npt = (n_active + cs * t - 1) / (cs * t);
-        const size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs, false);
+        const size_t b = sk_smem_bytes(npt * t, ctx->snap.T, ctx->pods.emax, ctx->pods.max_blob_words, cs, false);
         if (npt > 64 || b > (size_t)max_smem)
             return fail(ctx, SIMON_ERR_LIMIT, "%u nodes on %u CTAs x %u threads do not fit the large-cluster variant", n_active, cs, t);
         CS = cs; TPB = t; NPT = npt; smem = b;
         ctx->big = true;
-        ctx->gnode_stride = (sk_node_bytes(npt * t, ctx->T, ctx->emax) + 255) & ~(size_t)255;
+        ctx->gnode_stride = (sk_node_bytes(npt * t, ctx->snap.T, ctx->pods.emax) + 255) & ~(size_t)255;
         return SIMON_OK;
     }
     if (n_scen > 1 && !want_cs && !want_t) {
@@ -593,7 +639,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
                 }
             }
             if (npt > 64) continue;
-            const size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs);
+            const size_t b = sk_smem_bytes(npt * t, ctx->snap.T, ctx->pods.emax, ctx->pods.max_blob_words, cs);
             if (b > (size_t)max_smem) continue;
             const int active = max_active_clusters(ctx, false, cs, t, npt, b, drain);
             if (active <= 0) continue;
@@ -622,7 +668,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
             if (n320 < npt_p) { t_p = 320; npt_p = n320; }
             if (n384 < npt_p) { t_p = 384; npt_p = n384; }
         }
-        const size_t b = sk_smem_bytes(npt_p * t_p, ctx->T, ctx->emax, ctx->max_blob_words, cs_p);
+        const size_t b = sk_smem_bytes(npt_p * t_p, ctx->snap.T, ctx->pods.emax, ctx->pods.max_blob_words, cs_p);
         if (npt_p <= 64 && b <= (size_t)max_smem && max_active_clusters(ctx, false, cs_p, t_p, npt_p, b, drain) > 0) {
             CS = cs_p; TPB = t_p; NPT = npt_p; smem = b; return SIMON_OK;
         }
@@ -643,7 +689,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
                 if (t > SIMON_AUTO_TPB) continue; // 320 threads still leave 200 registers/thread; fewer nodes per thread wins
             }
             if (t > SIMON_MAX_TPB) return fail(ctx, SIMON_ERR_LIMIT, "threads per CTA must be <= %u (got %u)", SIMON_MAX_TPB, t);
-            size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs);
+            size_t b = sk_smem_bytes(npt * t, ctx->snap.T, ctx->pods.emax, ctx->pods.max_blob_words, cs);
             if (b <= (size_t)max_smem && (want_cs || max_active_clusters(ctx, false, cs, t, npt, b, drain) > 0)) {
                 CS = cs; TPB = t; NPT = npt; smem = b; return SIMON_OK;
             }
@@ -655,11 +701,11 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
     if (!want_cs && !want_t) {
         const uint32_t cs = 16, t = 320;
         const uint32_t npt = (n_active + cs * t - 1) / (cs * t);
-        const size_t b = sk_smem_bytes(npt * t, ctx->T, ctx->emax, ctx->max_blob_words, cs, false);
+        const size_t b = sk_smem_bytes(npt * t, ctx->snap.T, ctx->pods.emax, ctx->pods.max_blob_words, cs, false);
         if (npt <= 64 && b <= (size_t)max_smem && max_active_clusters(ctx, true, cs, t, npt, b, drain) > 0) {
             CS = cs; TPB = t; NPT = npt; smem = b;
             ctx->big = true;
-            ctx->gnode_stride = (sk_node_bytes(npt * t, ctx->T, ctx->emax) + 255) & ~(size_t)255;
+            ctx->gnode_stride = (sk_node_bytes(npt * t, ctx->snap.T, ctx->pods.emax) + 255) & ~(size_t)255;
             return SIMON_OK;
         }
     }
@@ -676,7 +722,7 @@ int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t T
     const sk_variant *v = kernel_variant(ctx, TPB, P.npt, ctx->big, prof, drain);
     if (!v)
         return fail(ctx, SIMON_ERR_LIMIT, "no kernel variant for %u threads per CTA%s%s", TPB, prof ? " with phase timers" : "",
-                    ctx->have_storage ? " and Open-Local storage" : "");
+                    ctx->valid.has(STORAGE) ? " and Open-Local storage" : "");
     if (ctx->big) {
         CU(ctx->d_gnode.alloc(ctx->gnode_stride * (size_t)n_scen * CS));
         P.gnode = ctx->d_gnode.p; P.gnode_stride = ctx->gnode_stride;
@@ -692,7 +738,7 @@ int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t T
     li = simon_launch_info{};
     snprintf(li.kernel, sizeof(li.kernel), "%s", v->name);
     li.n_nodes = ctx->geom_nodes; li.cluster_ctas = CS; li.threads_per_cta = TPB; li.node_slots = P.npt; li.n_scenarios = n_scen;
-    li.large = ctx->big; li.local = ctx->have_storage && !drain; li.smem_bytes = smem;
+    li.large = ctx->big; li.local = ctx->valid.has(STORAGE) && !drain; li.smem_bytes = smem;
     return SIMON_OK;
 }
 
@@ -700,7 +746,7 @@ int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t T
 // accounted by the parallel import kernel, the rest by the persistent placement kernel.
 int launch_range(simon_ctx *ctx, SkParams &P, uint32_t CS, uint32_t TPB, size_t smem, uint32_t first, uint32_t count, bool record) {
     uint32_t n_pre = 0;
-    while (n_pre < count && ctx->bypass[first + n_pre]) n_pre++;
+    while (n_pre < count && ctx->pods.bypass[first + n_pre]) n_pre++;
     if (n_pre < 256) n_pre = 0;
     if (record) CU(cudaEventRecord(ctx->ev0, ctx->stream));
     if (n_pre) {
@@ -720,11 +766,11 @@ int launch_range(simon_ctx *ctx, SkParams &P, uint32_t CS, uint32_t TPB, size_t 
 
 // simon_schedule_resume's checks of a placed prefix (include/simon_gpu.h), on the host before any device work
 int check_prefix(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n_prefix) {
-    const int32_t N = (int32_t)ctx->N;
+    const int32_t N = (int32_t)ctx->snap.N;
     for (uint32_t i = 0; i < n_prefix; i++) {
-        const int32_t e = prefix_node[i], f = ctx->h_fixed[i], gd = ctx->h_guard[i];
+        const int32_t e = prefix_node[i], f = ctx->pods.h_fixed[i], gd = ctx->pods.h_guard[i];
         if (e < -3 || e >= N) return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u: node %d out of range", i, e);
-        if (ctx->bypass[i]) {
+        if (ctx->pods.bypass[i]) {
             // what the import gives a pod that does not reach the scheduler: absent -3, bound to a node outside the cluster -2
             const int32_t want = gd == -2 ? -3 : (f >= 0 ? f : -2);
             if (e != want) return fail(ctx, SIMON_ERR_INVALID, "prefix pod %u does not reach the scheduler and is reported as %d, not %d", i, want, e);
@@ -748,13 +794,13 @@ int rebuild_prefix(simon_ctx *ctx, const SkParams &P, const int32_t *prefix_node
     simon_import_kernel<<<grid, 256, 0, st>>>(P, 0, n_prefix, ctx->d_prefix.p);
     CU(cudaGetLastError());
     ctx->launches++;
-    const uint32_t N1 = std::max(1u, ctx->N);
+    const uint32_t N1 = std::max(1u, ctx->snap.N);
     CU(ctx->d_rs_cnt.alloc(N1)); CU(ctx->d_rs_off.alloc(N1 + 1)); CU(ctx->d_rs_cur.alloc(N1)); CU(ctx->d_rs_list.alloc(n_prefix));
     CU(cudaMemsetAsync(ctx->d_rs_cnt.p, 0, 4ull * N1, st));
     SkParams R = P;
     R.vg_req_stride = 0; R.node_stride = 0;      // plain CTAs, not one cluster per scenario: every CTA reads slice 0
     simon_resume_count<<<grid, 256, 0, st>>>(R, ctx->d_prefix.p, n_prefix, ctx->d_rs_cnt.p);
-    simon_resume_scan<<<1, 1024, 0, st>>>(ctx->d_rs_cnt.p, ctx->N, ctx->d_rs_off.p, ctx->d_rs_cur.p);
+    simon_resume_scan<<<1, 1024, 0, st>>>(ctx->d_rs_cnt.p, ctx->snap.N, ctx->d_rs_off.p, ctx->d_rs_cur.p);
     simon_resume_fill<<<grid, 256, 0, st>>>(R, ctx->d_prefix.p, n_prefix, ctx->d_rs_cur.p, ctx->d_rs_list.p);
     simon_resume_replay<<<(N1 + 127) / 128, 128, 0, st>>>(R, ctx->d_rs_off.p, ctx->d_rs_list.p);
     CU(cudaGetLastError());
@@ -765,12 +811,12 @@ int rebuild_prefix(simon_ctx *ctx, const SkParams &P, const int32_t *prefix_node
 // Before a run on the single-scenario pool: clear its failure records and counters; arm the dump in P if its pod is in [first, first + count)
 cudaError_t single_begin(simon_ctx *ctx, SkParams &P, uint32_t first = 0, uint32_t count = 0) {
     cudaStream_t st = ctx->stream;
-    cudaError_t e = cudaMemsetAsync(ctx->single.fail_counts.p, 0, 4ull * ctx->max_fail * SIMON_N_FAIL_CODES, st);
+    cudaError_t e = cudaMemsetAsync(ctx->single.fail_counts.p, 0, 4ull * ctx->pods.max_fail * SIMON_N_FAIL_CODES, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(ctx->single.counters.p, 0, 8, st);
-    if (e == cudaSuccess && ctx->dump_pod >= first && ctx->dump_pod < first + count) {
-        P.dump_pod = ctx->dump_pod; P.dump_total = ctx->d_dump_total.p; P.dump_code = ctx->d_dump_code.p;
-        e = cudaMemsetAsync(ctx->d_dump_total.p, 0xff, 8ull * std::max(1u, ctx->N), st);     // -1: node not scored (infeasible)
-        if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_dump_code.p, 0, 4ull * std::max(1u, ctx->N), st);
+    if (e == cudaSuccess && ctx->pods.dump_pod >= first && ctx->pods.dump_pod < first + count) {
+        P.dump_pod = ctx->pods.dump_pod; P.dump_total = ctx->pods.d_dump_total.p; P.dump_code = ctx->pods.d_dump_code.p;
+        e = cudaMemsetAsync(ctx->pods.d_dump_total.p, 0xff, 8ull * std::max(1u, ctx->snap.N), st);     // -1: node not scored (infeasible)
+        if (e == cudaSuccess) e = cudaMemsetAsync(ctx->pods.d_dump_code.p, 0, 4ull * std::max(1u, ctx->snap.N), st);
     }
     return e;
 }
@@ -780,7 +826,7 @@ int single_end(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_node
                uint32_t *out_fail_pod, uint32_t max_fail, uint32_t *out_n_fail) {
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
-    ctx->have_live = true;
+    ctx->valid.set(LIVE);
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     const ScenPool &S = ctx->single;
     uint32_t counters[2] = {0, 0};
@@ -788,7 +834,7 @@ int single_end(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_node
     if (out_n_fail) *out_n_fail = counters[0];
     if (out_node && count) CU(cudaMemcpy(out_node, S.out_node.p + first, 4ull * count, cudaMemcpyDeviceToHost));
     if (out_score && S.out_score.p && count) CU(cudaMemcpy(out_score, S.out_score.p + first, 8ull * count, cudaMemcpyDeviceToHost));
-    uint32_t nf = std::min(std::min(counters[0], max_fail), ctx->max_fail);
+    uint32_t nf = std::min(std::min(counters[0], max_fail), ctx->pods.max_fail);
     if (nf && out_fail_counts) CU(cudaMemcpy(out_fail_counts, S.fail_counts.p, 4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
     if (nf && out_fail_pod) CU(cudaMemcpy(out_fail_pod, S.fail_pod.p, 4ull * nf, cudaMemcpyDeviceToHost));
     return SIMON_OK;
@@ -796,7 +842,7 @@ int single_end(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_node
 
 // A batch's node lists (scenario_lists) on the device and its SkScenario array in h; all N nodes in index order need no node list
 cudaError_t batch_scenarios(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, std::vector<SkScenario> &h) {
-    const uint32_t N = ctx->N;
+    const uint32_t N = ctx->snap.N;
     const ScenPool &B = ctx->batch;
     h.resize(n);
     for (uint32_t i = 0; i < n; i++)
@@ -809,15 +855,15 @@ cudaError_t batch_scenarios(simon_ctx *ctx, const simon_scenario *scen, uint32_t
 // With a PDB table: enqueue allowed[j] = max(0, placed members of j - desired[j]) on `placement` into d_pdb_rem
 cudaError_t pdb_allowed(simon_ctx *ctx, const int32_t *placement) {
     ctx->launches += 2;
-    return simon_pdb_launch_allowed(ctx->stream, ctx->sms * 4u, ctx->n_pods, placement, ctx->d_pdb_off.p, ctx->d_pdb_ids.p, ctx->n_pdbs,
-                                    ctx->d_pdb_desired.p, ctx->d_pdb_rem.p);
+    return simon_pdb_launch_allowed(ctx->stream, ctx->sms * 4u, ctx->pods.n_pods, placement, ctx->pdb.d_off.p, ctx->pdb.d_ids.p, ctx->pdb.n,
+                                    ctx->pdb.d_desired.p, ctx->pdb.d_rem.p);
 }
 
 // With a PDB table: after the pack of SmvPod records, the pods of PDBs without budget (d_pdb_rem <= 0) become never movable
 cudaError_t pdb_mark(simon_ctx *ctx, uint32_t *blocked) {
     ctx->launches++;
-    return simon_pdb_launch_mark(ctx->stream, ctx->sms * 4u, ctx->n_pods, ctx->d_pdb_off.p, ctx->d_pdb_ids.p, ctx->d_pdb_rem.p,
-                                 ctx->d_mv_pods.p, blocked);
+    return simon_pdb_launch_mark(ctx->stream, ctx->sms * 4u, ctx->pods.n_pods, ctx->pdb.d_off.p, ctx->pdb.d_ids.p, ctx->pdb.d_rem.p,
+                                 ctx->moves.d_pods.p, blocked);
 }
 
 }  // namespace
@@ -868,48 +914,55 @@ int simon_snapshot_upload(simon_ctx *ctx, const simon_snapshot *s) {
         return fail(ctx, SIMON_ERR_LIMIT, "snapshot exceeds compiled-in limits");
     if (s->n_nodes >= (1u << 24)) return fail(ctx, SIMON_ERR_LIMIT, "too many nodes");
     CU(cudaSetDevice(ctx->device));
+    ctx->valid.drop(SNAPSHOT);
     cudaStream_t st = ctx->stream;
     const uint32_t N = s->n_nodes;
-    ctx->N = N; ctx->K = s->n_scalars; ctx->WL = s->n_label_words; ctx->WT = s->n_taint_words; ctx->T = s->n_topos;
-    ctx->NC = s->n_node_classes; ctx->n_log = s->n_log;
-    ctx->topo_ndom.assign(s->topo_ndom, s->topo_ndom + s->n_topos);
-    ctx->max_dom = 1;
-    for (uint32_t t = 0; t < s->n_topos; t++) ctx->max_dom = std::max(ctx->max_dom, s->topo_ndom[t]);
-    const uint32_t K1 = ctx->K ? ctx->K : 1;
-    CU(ctx->d_topo_ndom.upload(s->topo_ndom, s->n_topos, st));
-    CU(ctx->d_alloc_mcpu.upload(s->alloc_mcpu, N, st)); CU(ctx->d_alloc_mem.upload(s->alloc_mem, N, st));
-    CU(ctx->d_alloc_eph.upload(s->alloc_eph, N, st)); CU(ctx->d_alloc_scalar.upload(s->alloc_scalar, (size_t)K1 * N, st));
-    CU(ctx->d_alloc_pods.upload(s->alloc_pods, N, st)); CU(ctx->d_node_flags.upload(s->node_flags, N, st));
-    CU(ctx->d_label_bits.upload(s->label_bits, (size_t)ctx->WL * N, st));
-    CU(ctx->d_taint_hard.upload(s->taint_hard, (size_t)ctx->WT * N, st)); CU(ctx->d_taint_soft.upload(s->taint_soft, (size_t)ctx->WT * N, st));
-    CU(ctx->d_topo_dom.upload(s->topo_dom, (size_t)ctx->T * N, st)); CU(ctx->d_node_class.upload(s->node_class, N, st));
-    CU(ctx->d_gpu_count.upload(s->gpu_count, N, st)); CU(ctx->d_gpu_dev_mem.upload(s->gpu_dev_mem, N, st));
-    CU(ctx->d_gpu_total_mem.upload(s->gpu_total_mem, N, st)); CU(ctx->d_log.upload(s->log_table, s->n_log, st));
+    ctx->snap.N = N; ctx->snap.K = s->n_scalars; ctx->snap.WL = s->n_label_words; ctx->snap.WT = s->n_taint_words; ctx->snap.T = s->n_topos;
+    ctx->snap.NC = s->n_node_classes; ctx->snap.n_log = s->n_log;
+    ctx->snap.topo_ndom.assign(s->topo_ndom, s->topo_ndom + s->n_topos);
+    ctx->snap.max_dom = 1;
+    for (uint32_t t = 0; t < s->n_topos; t++) ctx->snap.max_dom = std::max(ctx->snap.max_dom, s->topo_ndom[t]);
+    const uint32_t K1 = ctx->snap.K ? ctx->snap.K : 1;
+    CU(ctx->snap.d_topo_ndom.upload(s->topo_ndom, s->n_topos, st));
+    CU(ctx->snap.d_alloc_mcpu.upload(s->alloc_mcpu, N, st)); CU(ctx->snap.d_alloc_mem.upload(s->alloc_mem, N, st));
+    CU(ctx->snap.d_alloc_eph.upload(s->alloc_eph, N, st)); CU(ctx->snap.d_alloc_scalar.upload(s->alloc_scalar, (size_t)K1 * N, st));
+    CU(ctx->snap.d_alloc_pods.upload(s->alloc_pods, N, st)); CU(ctx->snap.d_node_flags.upload(s->node_flags, N, st));
+    CU(ctx->snap.d_label_bits.upload(s->label_bits, (size_t)ctx->snap.WL * N, st));
+    CU(ctx->snap.d_taint_hard.upload(s->taint_hard, (size_t)ctx->snap.WT * N, st)); CU(ctx->snap.d_taint_soft.upload(s->taint_soft, (size_t)ctx->snap.WT * N, st));
+    CU(ctx->snap.d_topo_dom.upload(s->topo_dom, (size_t)ctx->snap.T * N, st)); CU(ctx->snap.d_node_class.upload(s->node_class, N, st));
+    CU(ctx->snap.d_gpu_count.upload(s->gpu_count, N, st)); CU(ctx->snap.d_gpu_dev_mem.upload(s->gpu_dev_mem, N, st));
+    CU(ctx->snap.d_gpu_total_mem.upload(s->gpu_total_mem, N, st)); CU(ctx->snap.d_log.upload(s->log_table, s->n_log, st));
     CU(cudaStreamSynchronize(st));
-    ctx->have_snap = true;
-    ctx->have_pods = false;
-    ctx->have_storage = false;
-    ctx->have_devices = false;
-    ctx->batch.n_storage = 0;
-    ctx->dr_n = 0;
-    ctx->have_live = ctx->pl_valid = false;
-    ctx->n_pdbs = 0;
+    ctx->valid.set(SNAPSHOT);
+    return SIMON_OK;
+}
+
+// The device copy of pod_fixed_node and the move-class records (with their bits on the host) from the pod set's, with the classes
+// of class_local (nullptr: none) taken off: pods of classes with local storage read the VGs of every node, so they leave the
+// pinned-run fast path (-4) and are never candidates of the move scoring
+static int upload_class_marks(simon_ctx *ctx, const uint8_t *class_local) {
+    auto &ps = ctx->pods;
+    std::vector<int32_t> fixed(ps.fixed_dev);
+    std::vector<SmvClass> mc(ps.mv_classes);
+    for (uint32_t i = 0; i < ps.n_pods && class_local; i++)
+        if (fixed[i] == -4 && class_local[ps.h_class[i]]) fixed[i] = -1;
+    ps.mv_bits.resize(mc.size());
+    for (uint32_t c = 0; c < mc.size(); c++) {
+        if (class_local && c < ps.n_classes && class_local[c]) mc[c].bits |= SMC_NOT_MOVABLE | SMC_NEVER;
+        ps.mv_bits[c] = mc[c].bits;
+    }
+    CU(ps.d_pod_fixed.upload(fixed.data(), ps.n_pods, ctx->stream));
+    CU(ps.d_mv_classes.upload(mc.data(), mc.size(), ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));      // `fixed` and `mc` leave scope
     return SIMON_OK;
 }
 
 int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     if (!ctx || !p) return SIMON_ERR_INVALID;
-    if (!ctx->have_snap) return fail(ctx, SIMON_ERR_STATE, "simon_pods_upload before simon_snapshot_upload");
-    CU(cudaSetDevice(ctx->device));
-    cudaStream_t st = ctx->stream;
-    ctx->have_storage = false;          // the storage tables are per class: a new pod set needs its own upload
-    ctx->have_devices = false;
-    ctx->batch.n_storage = 0;
-    ctx->dr_n = 0;
-    ctx->have_live = ctx->pl_valid = false;
-    ctx->n_pdbs = 0;                    // the PDB table is per pod: a new pod set needs its own upload
-    ctx->n_classes = p->n_classes; ctx->n_pods = p->n_pods; ctx->n_counters = p->n_counters;
-    // validate classes; derive limits
+    if (!ctx->valid.has(SNAPSHOT)) return fail(ctx, SIMON_ERR_STATE, "simon_pods_upload before simon_snapshot_upload");
+    // ---- refusals before any change to the context: class records and limits, pod classes and pins, counters, and the per-class
+    // tables the kernel needs at every class switch, derived once here instead of by every CTA every time: the entry table as int32
+    // rows, the compact list of the entries a commit of the class increments, counter bases ----
     uint32_t max_words = SCW_HDR_WORDS, emax = 0;
     std::vector<int32_t> guard(p->n_pods ? p->n_pods : 1, -1);
     for (uint32_t c = 0; c < p->n_classes; c++) {
@@ -930,28 +983,72 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
         int64_t g = p->class_blob[p->class_off[c] + SCW_GUARD_NODE];
         if (g == -3) {          // per pod: the pin of a DaemonSet pod (simon_podset.pod_pin_node)
             g = p->pod_pin_node ? p->pod_pin_node[i] : -1;
-            if (g >= (int64_t)ctx->N || g < -2) return fail(ctx, SIMON_ERR_INVALID, "pod %u: bad pin node %lld", i, (long long)g);
+            if (g >= (int64_t)ctx->snap.N || g < -2) return fail(ctx, SIMON_ERR_INVALID, "pod %u: bad pin node %lld", i, (long long)g);
         }
         guard[i] = (int32_t)g;
     }
-    ctx->max_blob_words = max_words;
-    ctx->emax = emax;
     std::vector<uint64_t> cnt_off(p->n_counters + 1, 0);
     uint64_t tot = 0;
     for (uint32_t k = 0; k < p->n_counters; k++) {
-        if (p->counter_topo[k] >= ctx->T) return fail(ctx, SIMON_ERR_INVALID, "counter %u: bad topology", k);
+        if (p->counter_topo[k] >= ctx->snap.T) return fail(ctx, SIMON_ERR_INVALID, "counter %u: bad topology", k);
         cnt_off[k] = tot;
-        tot += ctx->topo_ndom[p->counter_topo[k]];
+        tot += ctx->snap.topo_ndom[p->counter_topo[k]];
     }
     cnt_off[p->n_counters] = tot;
-    ctx->cnt_words = tot;
     const uint64_t blob_words = p->class_off[p->n_classes];
-    CU(ctx->d_class_off.upload(p->class_off, p->n_classes + 1, st));
+    if (blob_words >= (1ull << 32)) return fail(ctx, SIMON_ERR_LIMIT, "class records exceed 2^32 words");
+    std::vector<uint32_t> aux((size_t)std::max(1u, p->n_classes) * SK_AUX_W, 0u);
+    for (uint32_t c = 0; c < p->n_classes; c++) {
+        const int64_t *cw = p->class_blob + p->class_off[c];
+        const int64_t *et = cw + cw[SCW_OFF_ENT];
+        const uint32_t E = (uint32_t)(cw[SCW_N_PORTS] + cw[SCW_N_PTS_HARD] + cw[SCW_N_PTS_SOFT] + cw[SCW_N_IPA_AFF] + cw[SCW_N_IPA_ANTI] +
+                                      cw[SCW_N_IPA_EXIST] + cw[SCW_N_IPA_SCORE]);
+        if ((uint64_t)cw[SCW_OFF_ENT] + 8ull * E > p->class_off[c + 1] - p->class_off[c] || (uint32_t)cw[SCW_N_ENT] != E)
+            return fail(ctx, SIMON_ERR_INVALID, "class %u: entry table does not match the list sizes", c);
+        uint32_t *ax = aux.data() + (size_t)c * SK_AUX_W;
+        uint32_t recs[SK_MAX_ENT];
+        bool node_lvl[SK_MAX_ENT], incs[SK_MAX_ENT];
+        uint32_t n_dom = 0, n_all = 0, n_aff_node = 0;
+        for (uint32_t e = 0; e < E; e++) {
+            const int64_t *r = et + 8ull * e;
+            const int32_t kind = (int32_t)r[ER_KIND];
+            const bool host = kind == EK_SOFT && r[ER_B] != 0;
+            incs[e] = r[ER_INC] != 0;
+            // entry | topology row << 8 | flags << 16 (bit 16: domain-level soft constraint, bit 17: required affinity term)
+            recs[e] = e | ((host ? 0u : (uint32_t)r[ER_T]) << 8) | ((kind == EK_SOFT && !host) ? 1u << 16 : 0u) | (kind == EK_AFF ? 1u << 17 : 0u);
+            // entries on topology row 0 (the node itself) can only match the winner's own node: they go to the end of the
+            // list and are applied by the owning thread alone; every thread walks the others
+            node_lvl[e] = incs[e] && ((recs[e] >> 8) & 0xff) == 0;
+            if (incs[e]) { n_all++; if (!node_lvl[e]) n_dom++; else if (recs[e] & (1u << 17)) n_aff_node++; }
+            for (uint32_t q = 0; q < ER_ROWS; q++) ax[SK_AUX_ENT + q * SK_MAX_ENT + e] = (uint32_t)(int32_t)r[q];
+        }
+        uint32_t kd = 0, kn = n_dom;
+        for (uint32_t e = 0; e < E; e++) {
+            if (!incs[e]) continue;
+            if (node_lvl[e]) ax[kn++] = recs[e]; else ax[kd++] = recs[e];
+        }
+        ax[SK_MAX_ENT] = n_dom | (n_all << 8) | (n_aff_node << 16);
+        const int64_t *inc = cw + cw[SCW_OFF_INC];
+        for (uint32_t u = 0; u < 32 && (int64_t)u < cw[SCW_N_INC]; u++) {
+            if (inc[3 * u] < 0 || (uint64_t)inc[3 * u] >= p->n_counters) return fail(ctx, SIMON_ERR_INVALID, "class %u: bad counter in the commit list", c);
+            ax[SK_AUX_INCB + u] = (uint32_t)cnt_off[inc[3 * u]];
+        }
+    }
+    // ---- the upload: the previous pod set and everything derived from it go first ----
+    CU(cudaSetDevice(ctx->device));
+    ctx->valid.drop(POD_SET);
+    cudaStream_t st = ctx->stream;
+    auto &ps = ctx->pods;
+    ps.n_classes = p->n_classes; ps.n_pods = p->n_pods; ps.n_counters = p->n_counters;
+    ps.max_blob_words = max_words;
+    ps.emax = emax;
+    ps.cnt_words = tot;
+    CU(ps.d_class_off.upload(p->class_off, p->n_classes + 1, st));
     {
         // the kernel copies max_blob_words words per class switch regardless of the record's own length: pad the tail
         std::vector<int64_t> padded(blob_words + max_words, 0);
         if (blob_words) memcpy(padded.data(), p->class_blob, 8ull * blob_words);
-        CU(ctx->d_class_blob.upload(padded.data(), padded.size(), st));
+        CU(ps.d_class_blob.upload(padded.data(), padded.size(), st));
         CU(cudaStreamSynchronize(st));
     }
     // Device copy of pod_fixed_node with one more value: -4 = "pinned pod on the fast path".  A pod of a pinned class whose only
@@ -960,8 +1057,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     // that owns the pin node (simon_kernel.cu, "run of pinned pods").  Classes with DoNotSchedule constraints, required pod
     // (anti)affinity of their own or matched by existing pods' anti-affinity, or a GPU-share request read state beyond the
     // node and take the general path.
-    std::vector<int32_t> fixed_dev(p->pod_fixed_node, p->pod_fixed_node + p->n_pods);
-    ctx->n_pin_fast = 0;
+    ps.fixed_dev.assign(p->pod_fixed_node, p->pod_fixed_node + p->n_pods);
     if (!(ctx->opt_flags & SIMON_OPT_NO_PIN_FAST)) {
         std::vector<uint8_t> fast(p->n_classes, 0);
         for (uint32_t c = 0; c < p->n_classes; c++) {
@@ -970,67 +1066,23 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
                       cw[SCW_N_IPA_EXIST] == 0 && cw[SCW_GPU_MEM] == 0 && cw[SCW_GPU_COUNT] == 0 && cw[SCW_NODE_NAME] == -1;
         }
         for (uint32_t i = 0; i < p->n_pods; i++)
-            if (fixed_dev[i] == -1 && guard[i] >= 0 && fast[p->pod_class[i]]) { fixed_dev[i] = -4; ctx->n_pin_fast++; }
+            if (ps.fixed_dev[i] == -1 && guard[i] >= 0 && fast[p->pod_class[i]]) ps.fixed_dev[i] = -4;
     }
-    CU(ctx->d_pod_class.upload(p->pod_class, p->n_pods, st)); CU(ctx->d_pod_fixed.upload(fixed_dev.data(), p->n_pods, st));
+    CU(ps.d_pod_class.upload(p->pod_class, p->n_pods, st));
+    CU(ps.d_pod_guard.upload(guard.data(), p->n_pods, st)); CU(ps.d_cnt_off.upload(cnt_off.data(), cnt_off.size(), st));
+    CU(ps.d_simon_raw.upload(p->simon_raw, (size_t)std::max(1u, p->n_static_rows) * ctx->snap.NC, st));
+    ps.simon32 = 1;
+    for (size_t q = 0; q < (size_t)p->n_static_rows * ctx->snap.NC; q++)
+        if (p->simon_raw[q] < 0 || p->simon_raw[q] >= (1ll << 31)) { ps.simon32 = 0; break; }
+    CU(ps.d_extra.upload(p->extra_score, (size_t)std::max(1u, p->n_extra_rows) * std::max(1u, ctx->snap.N), st));
+    CU(ps.d_cls_aux.upload(aux.data(), aux.size(), st));
     CU(cudaStreamSynchronize(st));
-    CU(ctx->d_pod_guard.upload(guard.data(), p->n_pods, st)); CU(ctx->d_cnt_off.upload(cnt_off.data(), cnt_off.size(), st));
-    CU(ctx->d_simon_raw.upload(p->simon_raw, (size_t)std::max(1u, p->n_static_rows) * ctx->NC, st));
-    ctx->simon32 = 1;
-    for (size_t q = 0; q < (size_t)p->n_static_rows * ctx->NC; q++)
-        if (p->simon_raw[q] < 0 || p->simon_raw[q] >= (1ll << 31)) { ctx->simon32 = 0; break; }
-    CU(ctx->d_extra.upload(p->extra_score, (size_t)std::max(1u, p->n_extra_rows) * std::max(1u, ctx->N), st));
-    if (blob_words >= (1ull << 32)) return fail(ctx, SIMON_ERR_LIMIT, "class records exceed 2^32 words");
-    {
-        // per-class tables the kernel needs at every class switch, derived once here instead of by every CTA every time:
-        // the entry table as int32 rows, the compact list of the entries a commit of the class increments, counter bases
-        std::vector<uint32_t> aux((size_t)std::max(1u, p->n_classes) * SK_AUX_W, 0u);
-        for (uint32_t c = 0; c < p->n_classes; c++) {
-            const int64_t *cw = p->class_blob + p->class_off[c];
-            const int64_t *et = cw + cw[SCW_OFF_ENT];
-            const uint32_t E = (uint32_t)(cw[SCW_N_PORTS] + cw[SCW_N_PTS_HARD] + cw[SCW_N_PTS_SOFT] + cw[SCW_N_IPA_AFF] + cw[SCW_N_IPA_ANTI] +
-                                          cw[SCW_N_IPA_EXIST] + cw[SCW_N_IPA_SCORE]);
-            if ((uint64_t)cw[SCW_OFF_ENT] + 8ull * E > p->class_off[c + 1] - p->class_off[c] || (uint32_t)cw[SCW_N_ENT] != E)
-                return fail(ctx, SIMON_ERR_INVALID, "class %u: entry table does not match the list sizes", c);
-            uint32_t *ax = aux.data() + (size_t)c * SK_AUX_W;
-            uint32_t recs[SK_MAX_ENT];
-            bool node_lvl[SK_MAX_ENT], incs[SK_MAX_ENT];
-            uint32_t n_dom = 0, n_all = 0, n_aff_node = 0;
-            for (uint32_t e = 0; e < E; e++) {
-                const int64_t *r = et + 8ull * e;
-                const int32_t kind = (int32_t)r[ER_KIND];
-                const bool host = kind == EK_SOFT && r[ER_B] != 0;
-                incs[e] = r[ER_INC] != 0;
-                // entry | topology row << 8 | flags << 16 (bit 16: domain-level soft constraint, bit 17: required affinity term)
-                recs[e] = e | ((host ? 0u : (uint32_t)r[ER_T]) << 8) | ((kind == EK_SOFT && !host) ? 1u << 16 : 0u) | (kind == EK_AFF ? 1u << 17 : 0u);
-                // entries on topology row 0 (the node itself) can only match the winner's own node: they go to the end of the
-                // list and are applied by the owning thread alone; every thread walks the others
-                node_lvl[e] = incs[e] && ((recs[e] >> 8) & 0xff) == 0;
-                if (incs[e]) { n_all++; if (!node_lvl[e]) n_dom++; else if (recs[e] & (1u << 17)) n_aff_node++; }
-                for (uint32_t q = 0; q < ER_ROWS; q++) ax[SK_AUX_ENT + q * SK_MAX_ENT + e] = (uint32_t)(int32_t)r[q];
-            }
-            uint32_t kd = 0, kn = n_dom;
-            for (uint32_t e = 0; e < E; e++) {
-                if (!incs[e]) continue;
-                if (node_lvl[e]) ax[kn++] = recs[e]; else ax[kd++] = recs[e];
-            }
-            ax[SK_MAX_ENT] = n_dom | (n_all << 8) | (n_aff_node << 16);
-            const int64_t *inc = cw + cw[SCW_OFF_INC];
-            for (uint32_t u = 0; u < 32 && (int64_t)u < cw[SCW_N_INC]; u++) {
-                if (inc[3 * u] < 0 || (uint64_t)inc[3 * u] >= p->n_counters) return fail(ctx, SIMON_ERR_INVALID, "class %u: bad counter in the commit list", c);
-                ax[SK_AUX_INCB + u] = (uint32_t)cnt_off[inc[3 * u]];
-            }
-        }
-        CU(ctx->d_cls_aux.upload(aux.data(), aux.size(), st));
-        CU(cudaStreamSynchronize(st));
-    }
     {
         // compact per-class header of the move kernel (simon_moves.cu): scoring + Fit inputs and a few counts in 64 bytes
-        std::vector<SmvClass> mc(std::max(1u, p->n_classes));
-        ctx->h_mv_bits.assign(std::max(1u, p->n_classes), 0u);
+        ps.mv_classes.assign(std::max(1u, p->n_classes), SmvClass{});
         for (uint32_t c = 0; c < p->n_classes; c++) {
             const int64_t *cw = p->class_blob + p->class_off[c];
-            SmvClass &k = mc[c];
+            SmvClass &k = ps.mv_classes[c];
             memset(&k, 0, sizeof(k));
             k.score_mcpu = cw[SCW_SCORE_MCPU]; k.score_mem = cw[SCW_SCORE_MEM]; k.nz_mcpu = cw[SCW_NZ_MCPU]; k.nz_mem = cw[SCW_NZ_MEM];
             k.req_mcpu = cw[SCW_REQ_MCPU]; k.req_mem = cw[SCW_REQ_MEM]; k.req_eph = cw[SCW_REQ_EPH];
@@ -1042,7 +1094,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
             if (cw[SCW_N_PTS_HARD] > 0) bits |= SMC_NEED_HARD | ((uint32_t)cw[SCW_N_PTS_HARD] << 25);
             if (cw[SCW_FLAGS] & SIMON_CLS_PINNED) bits |= SMC_NEVER;
             const int64_t *sc = cw + cw[SCW_OFF_SCALARS];
-            for (uint32_t q = 0; q < ctx->K; q++) if (sc[q] != 0) bits |= SMC_HAS_SCALAR;
+            for (uint32_t q = 0; q < ctx->snap.K; q++) if (sc[q] != 0) bits |= SMC_HAS_SCALAR;
             const uint32_t n_filt = (uint32_t)(cw[SCW_N_IPA_AFF] + cw[SCW_N_IPA_ANTI] + cw[SCW_N_IPA_EXIST]);
             bits |= ((uint32_t)cw[SCW_N_PORTS] & 31u) << 10 | ((uint32_t)cw[SCW_N_PORTS] & 32u) << 24;     // SMC_NPORTS
             bits |= (n_filt & 63u) << 15;
@@ -1050,62 +1102,59 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
             const uint32_t E = (uint32_t)cw[SCW_N_ENT];
             for (uint32_t e = 0; e < E; e++) if (et[8ull * e + ER_INC]) bits |= SMC_OWN_INC;
             k.bits = bits;
-            ctx->h_mv_bits[c] = bits;
         }
         // registered-domain bitmaps of the hard constraints, one per (class, constraint), for scoped runs
-        ctx->h_mv_pairs.clear();
+        ps.mv_pairs.clear();
         uint32_t words = 0;
         for (uint32_t c = 0; c < p->n_classes; c++) {
             const int64_t *cw = p->class_blob + p->class_off[c];
             for (uint32_t j = 0; (int64_t)j < cw[SCW_N_PTS_HARD]; j++) {
                 const int64_t t = (cw + cw[SCW_OFF_PTS_HARD])[4 * j + 1];
-                ctx->h_mv_pairs.push_back(make_uint4(c, j, words, 0));
-                words += (ctx->topo_ndom[t] + 31) / 32;
+                ps.mv_pairs.push_back(make_uint4(c, j, words, 0));
+                words += (ctx->snap.topo_ndom[t] + 31) / 32;
             }
         }
-        CU(ctx->d_mv_hreg.alloc(std::max(1u, words)));
-        CU(ctx->d_mv_hs.alloc((size_t)std::max(1u, p->n_classes) * SMV_MAX_HARD));
-        ctx->mv_scope_dirty = true;
+        CU(ps.d_mv_hreg.alloc(std::max(1u, words)));
+        CU(ps.d_mv_hs.alloc((size_t)std::max(1u, p->n_classes) * SMV_MAX_HARD));
         std::vector<uint32_t> sig_class(std::max(1u, p->n_static_sigs), 0u);
         for (uint32_t c = p->n_classes; c-- > 0;) {
             const int64_t sg = (p->class_blob + p->class_off[c])[SCW_STATIC_SIG];
             if (sg >= 0 && (uint64_t)sg < sig_class.size()) sig_class[sg] = c;
         }
-        CU(ctx->d_sig_class.upload(sig_class.data(), sig_class.size(), st));
-        ctx->static_filled = false;
-        CU(ctx->d_mv_classes.upload(mc.data(), mc.size(), st));
-        CU(cudaStreamSynchronize(st));       // `mc` leaves scope
+        CU(ps.d_sig_class.upload(sig_class.data(), sig_class.size(), st));
+        CU(cudaStreamSynchronize(st));       // `sig_class` leaves scope
     }
-    ctx->bypass.assign(std::max(1u, p->n_pods), 0);
-    for (uint32_t i = 0; i < p->n_pods; i++) ctx->bypass[i] = (guard[i] == -2 || p->pod_fixed_node[i] != -1) ? 1 : 0;
-    ctx->h_fixed.assign(p->pod_fixed_node, p->pod_fixed_node + p->n_pods);
-    ctx->h_guard.assign(guard.begin(), guard.begin() + p->n_pods);
-    ctx->h_class.assign(p->pod_class, p->pod_class + p->n_pods);
-    CU(cudaStreamSynchronize(st));
-    ctx->max_fail = std::max(1u, p->n_pods);      // every pod of the list may fail: one histogram row each (96 B)
-    int rc = alloc_pool(ctx, ctx->single, 1, true);
+    ps.bypass.assign(std::max(1u, p->n_pods), 0);
+    for (uint32_t i = 0; i < p->n_pods; i++) ps.bypass[i] = (guard[i] == -2 || p->pod_fixed_node[i] != -1) ? 1 : 0;
+    ps.h_fixed.assign(p->pod_fixed_node, p->pod_fixed_node + p->n_pods);
+    ps.h_guard.assign(guard.begin(), guard.begin() + p->n_pods);
+    ps.h_class.assign(p->pod_class, p->pod_class + p->n_pods);
+    int rc = upload_class_marks(ctx, nullptr);
     if (rc) return rc;
-    ctx->n_sigs = std::max(1u, p->n_static_sigs);
+    ps.max_fail = std::max(1u, p->n_pods);      // every pod of the list may fail: one histogram row each (96 B)
+    rc = alloc_pool(ctx, ctx->single, 1, true);
+    if (rc) return rc;
+    ps.n_sigs = std::max(1u, p->n_static_sigs);
     {
-        size_t words = (size_t)ctx->n_sigs * std::max(1u, ctx->N);
-        ctx->use_scache = words * 8 <= (2ull << 30) ? 1 : 0;      // per-(signature, node) verdict cache, capped at 2 GiB
-        if (!ctx->use_scache) words = 1;
-        CU(ctx->d_scache.alloc(words));
-        CU(cudaMemsetAsync(ctx->d_scache.p, 0, 8ull * words, st));
+        size_t words = (size_t)ps.n_sigs * std::max(1u, ctx->snap.N);
+        ps.use_scache = words * 8 <= (2ull << 30) ? 1 : 0;      // per-(signature, node) verdict cache, capped at 2 GiB
+        if (!ps.use_scache) words = 1;
+        CU(ps.d_scache.alloc(words));
+        CU(cudaMemsetAsync(ps.d_scache.p, 0, 8ull * words, st));
     }
-    CU(ctx->d_dump_total.alloc(std::max(1u, ctx->N))); CU(ctx->d_dump_code.alloc(std::max(1u, ctx->N)));
-    ctx->dump_pod = 0xffffffffu;
-    CU(ctx->d_stats.alloc(32));
-    CU(cudaMemsetAsync(ctx->d_stats.p, 0, 256, st));
+    CU(ps.d_dump_total.alloc(std::max(1u, ctx->snap.N))); CU(ps.d_dump_code.alloc(std::max(1u, ctx->snap.N)));
+    ps.dump_pod = 0xffffffffu;
+    CU(ps.d_stats.alloc(32));
+    CU(cudaMemsetAsync(ps.d_stats.p, 0, 256, st));
     CU(cudaStreamSynchronize(st));
-    ctx->have_pods = true;
+    ctx->valid.set(POD_SET);
     return SIMON_OK;
 }
 
 int simon_state_reset(simon_ctx *ctx) {
-    if (!ctx || !ctx->have_pods) return ctx ? fail(ctx, SIMON_ERR_STATE, "no pods uploaded") : SIMON_ERR_INVALID;
+    if (!ctx || !ctx->valid.has(POD_SET)) return ctx ? fail(ctx, SIMON_ERR_STATE, "no pods uploaded") : SIMON_ERR_INVALID;
     CU(cudaSetDevice(ctx->device));
-    ctx->have_live = false;
+    ctx->valid.drop(LIVE);
     int rc = clear_pool(ctx, ctx->single);
     if (rc) return rc;
     CU(cudaStreamSynchronize(ctx->stream));
@@ -1113,8 +1162,8 @@ int simon_state_reset(simon_ctx *ctx) {
 }
 
 int simon_results_download(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_node, int64_t *out_score) {
-    if (!ctx || !ctx->have_pods) return SIMON_ERR_STATE;
-    if ((uint64_t)first + count > ctx->n_pods) return fail(ctx, SIMON_ERR_INVALID, "range out of bounds");
+    if (!ctx || !ctx->valid.has(POD_SET)) return SIMON_ERR_STATE;
+    if ((uint64_t)first + count > ctx->pods.n_pods) return fail(ctx, SIMON_ERR_INVALID, "range out of bounds");
     CU(cudaSetDevice(ctx->device));
     if (out_node) CU(cudaMemcpyAsync(out_node, ctx->single.out_node.p + first, 4ull * count, cudaMemcpyDeviceToHost, ctx->stream));
     if (out_score && ctx->single.out_score.p)
@@ -1126,18 +1175,18 @@ int simon_results_download(simon_ctx *ctx, uint32_t first, uint32_t count, int32
 int simon_schedule(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_node, int64_t *out_score,
                    uint32_t *out_fail_counts, uint32_t *out_fail_pod, uint32_t max_fail, uint32_t *out_n_fail) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_schedule before uploads");
-    if ((uint64_t)first + count > ctx->n_pods) return fail(ctx, SIMON_ERR_INVALID, "pod range out of bounds");
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_schedule before uploads");
+    if ((uint64_t)first + count > ctx->pods.n_pods) return fail(ctx, SIMON_ERR_INVALID, "pod range out of bounds");
     CU(cudaSetDevice(ctx->device));
     ctx->last_launch = simon_launch_info{};
     if (count == 0) { if (out_n_fail) *out_n_fail = 0; return SIMON_OK; }
     uint32_t CS, TPB, NPT;
     size_t smem;
-    int rc = choose_geometry(ctx, ctx->N, CS, TPB, NPT, smem);
+    int rc = choose_geometry(ctx, ctx->snap.N, CS, TPB, NPT, smem);
     if (rc) return rc;
     SkParams P;
     fill_params(ctx, ctx->single, P);
-    P.first = first; P.count = count; P.max_fail = ctx->max_fail; P.npt = NPT;
+    P.first = first; P.count = count; P.max_fail = ctx->pods.max_fail; P.npt = NPT;
     CU(single_begin(ctx, P, first, count));
     rc = launch_range(ctx, P, CS, TPB, smem, first, count, true);
     if (rc) return rc;
@@ -1147,8 +1196,8 @@ int simon_schedule(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_
 int simon_schedule_resume(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n_prefix, int32_t *out_node, int64_t *out_score,
                           uint32_t *out_fail_counts, uint32_t *out_fail_pod, uint32_t max_fail, uint32_t *out_n_fail) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_schedule_resume before uploads");
-    if (n_prefix > ctx->n_pods) return fail(ctx, SIMON_ERR_INVALID, "prefix of %u pods exceeds the %u uploaded", n_prefix, ctx->n_pods);
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_schedule_resume before uploads");
+    if (n_prefix > ctx->pods.n_pods) return fail(ctx, SIMON_ERR_INVALID, "prefix of %u pods exceeds the %u uploaded", n_prefix, ctx->pods.n_pods);
     if (n_prefix && !prefix_node) return fail(ctx, SIMON_ERR_INVALID, "prefix_node is NULL");
     int rc = check_prefix(ctx, prefix_node, n_prefix);
     if (rc) return rc;
@@ -1158,12 +1207,12 @@ int simon_schedule_resume(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n
     ScenPool &S = ctx->single;
     uint32_t CS, TPB, NPT;
     size_t smem;
-    rc = choose_geometry(ctx, ctx->N, CS, TPB, NPT, smem);
+    rc = choose_geometry(ctx, ctx->snap.N, CS, TPB, NPT, smem);
     if (rc) return rc;
     SkParams P;
     fill_params(ctx, S, P);
-    P.max_fail = ctx->max_fail; P.npt = NPT;
-    const uint32_t first = n_prefix, count = ctx->n_pods - n_prefix;
+    P.max_fail = ctx->pods.max_fail; P.npt = NPT;
+    const uint32_t first = n_prefix, count = ctx->pods.n_pods - n_prefix;
     rc = clear_pool(ctx, S);
     if (rc) return rc;
     CU(single_begin(ctx, P, first, count));
@@ -1175,44 +1224,44 @@ int simon_schedule_resume(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n
         if (rc) return rc;
     }
     CU(cudaEventRecord(ctx->ev1, st));
-    return single_end(ctx, 0, ctx->n_pods, out_node, out_score, out_fail_counts, out_fail_pod, max_fail, out_n_fail);
+    return single_end(ctx, 0, ctx->pods.n_pods, out_node, out_score, out_fail_counts, out_fail_pod, max_fail, out_n_fail);
 }
 
 int simon_replay(simon_ctx *ctx, uint32_t steps, float *out_ms_total) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_replay before uploads");
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_replay before uploads");
     CU(cudaSetDevice(ctx->device));
     ctx->last_launch = simon_launch_info{};
     cudaStream_t st = ctx->stream;
     ScenPool &S = ctx->single;
     uint32_t CS, TPB, NPT;
     size_t smem;
-    int rc = choose_geometry(ctx, ctx->N, CS, TPB, NPT, smem);
+    int rc = choose_geometry(ctx, ctx->snap.N, CS, TPB, NPT, smem);
     if (rc) return rc;
     SkParams P;
     fill_params(ctx, S, P);
-    P.first = 0; P.count = ctx->n_pods; P.max_fail = ctx->max_fail; P.npt = NPT;
+    P.first = 0; P.count = ctx->pods.n_pods; P.max_fail = ctx->pods.max_fail; P.npt = NPT;
     CU(cudaEventRecord(ctx->ev0, st));
     for (uint32_t s = 0; s < steps; s++) {
         rc = clear_pool(ctx, S);
         if (rc) return rc;
         CU(single_begin(ctx, P));
-        rc = launch_range(ctx, P, CS, TPB, smem, 0, ctx->n_pods, false);
+        rc = launch_range(ctx, P, CS, TPB, smem, 0, ctx->pods.n_pods, false);
         if (rc) return rc;
     }
     CU(cudaEventRecord(ctx->ev1, st));
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
-    if (steps) ctx->have_live = true;
+    if (steps) ctx->valid.set(LIVE);
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     if (out_ms_total) *out_ms_total = ctx->last_ms;
     return SIMON_OK;
 }
 
 int simon_stats(simon_ctx *ctx, uint64_t *out8) {
-    if (!ctx || !out8 || !ctx->have_pods) return SIMON_ERR_STATE;
+    if (!ctx || !out8 || !ctx->valid.has(POD_SET)) return SIMON_ERR_STATE;
     CU(cudaSetDevice(ctx->device));
-    CU(cudaMemcpy(out8, ctx->d_stats.p, 256, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(out8, ctx->pods.d_stats.p, 256, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
@@ -1227,7 +1276,7 @@ int simon_last_launch(simon_ctx *ctx, simon_launch_info *out) {
 
 int simon_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *req_mem, int64_t *req_eph, int64_t *nz_mcpu,
                          int64_t *nz_mem, int32_t *num_pods) {
-    if (!ctx || !ctx->have_pods) return SIMON_ERR_STATE;
+    if (!ctx || !ctx->valid.has(POD_SET)) return SIMON_ERR_STATE;
     CU(cudaSetDevice(ctx->device));
     void *const dst[NodeState::COLS] = {req_mcpu, req_mem, req_eph, nz_mcpu, nz_mem, num_pods};
     CU(ctx->single.state.download(dst));
@@ -1237,7 +1286,7 @@ int simon_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *req_mem, in
 // The node lists of a batch into the batch pool's host columns h_order / h_rank (scenario order and its inverse), each checked: at most
 // N nodes, every one in range and listed once.  `what` names a scenario in the messages.
 static int scenario_lists(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, const char *what, uint32_t &max_active) {
-    const uint32_t N = ctx->N, N1 = std::max(1u, N);
+    const uint32_t N = ctx->snap.N, N1 = std::max(1u, N);
     ScenPool &B = ctx->batch;
     max_active = 0;
     B.h_order.assign((size_t)n * N1, 0u);
@@ -1265,10 +1314,10 @@ static int scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n,
     ctx->last_launch = simon_launch_info{};
     cudaStream_t st = ctx->stream;
     if (n == 0) return SIMON_OK;
-    const uint32_t N = ctx->N;
+    const uint32_t N = ctx->snap.N;
     ScenPool &B = ctx->batch;
     const bool local = out_local != nullptr;
-    if (local) B.n_storage = 0;         // the slices are overwritten below
+    if (local) ctx->valid.drop(STORAGE_BATCH);       // the slices are overwritten below
     // ---- node lists: validated on the host, uploaded in ONE copy each (scenario order and its inverse) ----
     uint32_t max_active = 0;
     int rc = scenario_lists(ctx, scen, n, "scenario", max_active);
@@ -1287,50 +1336,53 @@ static int scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n,
     if (rc) return rc;
     SkParams Pm;
     fill_params(ctx, B, Pm);
-    Pm.first = 0; Pm.count = ctx->n_pods; Pm.max_fail = 0; Pm.npt = NPT;
+    Pm.first = 0; Pm.count = ctx->pods.n_pods; Pm.max_fail = 0; Pm.npt = NPT;
     rc = launch(ctx, Pm, n, CS, TPB, smem);
     if (rc) return rc;
     // per-scenario sums over the active nodes on the device; ONE copy of the result structs comes back
-    simon_scen_reduce<<<n, 256, 0, st>>>(B.scen.p, ctx->d_alloc_mcpu.p, ctx->d_alloc_mem.p, B.results.p);
+    simon_scen_reduce<<<n, 256, 0, st>>>(B.scen.p, ctx->snap.d_alloc_mcpu.p, ctx->snap.d_alloc_mem.p, B.results.p);
     CU(cudaGetLastError());
     if (local) {
-        simon_scen_reduce_local<<<n, 256, 0, st>>>(B.scen.p, ctx->d_node_n_vg.p, ctx->d_vg_cap.p, B.vg_req.p, B.vn, N, B.local_results.p);
+        simon_scen_reduce_local<<<n, 256, 0, st>>>(B.scen.p, ctx->storage.d_node_n_vg.p, ctx->storage.d_vg_cap.p, B.vg_req.p, B.vn, N, B.local_results.p);
         CU(cudaGetLastError());
         CU(cudaMemcpyAsync(out_local, B.local_results.p, sizeof(simon_scenario_local_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
     }
     CU(cudaMemcpyAsync(out, B.results.p, sizeof(simon_scenario_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
-    if (out_node) CU(cudaMemcpyAsync(out_node, B.out_node.p, 4ull * n * ctx->n_pods, cudaMemcpyDeviceToHost, st));
+    if (out_node) CU(cudaMemcpyAsync(out_node, B.out_node.p, 4ull * n * ctx->pods.n_pods, cudaMemcpyDeviceToHost, st));
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
-    if (local) B.n_storage = n;
+    if (local) {
+        ctx->storage_batch.n = n;
+        ctx->valid.set(STORAGE_BATCH);
+    }
     return SIMON_OK;
 }
 
 int simon_scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, simon_scenario_result *out, int32_t *out_node) {
     if (!ctx || !scen || !out) return SIMON_ERR_INVALID;
-    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_scenarios_run before uploads");
-    if (ctx->have_storage) return fail(ctx, SIMON_ERR_LIMIT, "scenario batches with Open-Local storage uploaded: use simon_scenarios_run_local");
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_scenarios_run before uploads");
+    if (ctx->valid.has(STORAGE)) return fail(ctx, SIMON_ERR_LIMIT, "scenario batches with Open-Local storage uploaded: use simon_scenarios_run_local");
     return scenarios_run(ctx, scen, n, out, nullptr, out_node);
 }
 
 int simon_scenarios_run_local(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, simon_scenario_result *out,
                               simon_scenario_local_result *out_local, int32_t *out_node) {
     if (!ctx || !scen || !out || !out_local) return SIMON_ERR_INVALID;
-    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_scenarios_run_local before uploads");
-    if (!ctx->have_storage) return fail(ctx, SIMON_ERR_STATE, "simon_scenarios_run_local before simon_storage_upload");
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_scenarios_run_local before uploads");
+    if (!ctx->valid.has(STORAGE)) return fail(ctx, SIMON_ERR_STATE, "simon_scenarios_run_local before simon_storage_upload");
     return scenarios_run(ctx, scen, n, out, out_local, out_node);
 }
 
 int simon_scenarios_storage_download(simon_ctx *ctx, uint32_t scenario, int64_t *vg_requested, uint32_t *dev_alloc) {
     if (!ctx) return SIMON_ERR_INVALID;
     const ScenPool &B = ctx->batch;
-    if (!B.n_storage) return fail(ctx, SIMON_ERR_STATE, "no simon_scenarios_run_local batch since the last upload");
-    if (scenario >= B.n_storage) return fail(ctx, SIMON_ERR_INVALID, "scenario %u of a batch of %u", scenario, B.n_storage);
-    if (dev_alloc && !ctx->have_devices) return fail(ctx, SIMON_ERR_STATE, "no devices uploaded");
+    if (!ctx->valid.has(STORAGE_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_scenarios_run_local batch since the last upload");
+    if (scenario >= ctx->storage_batch.n) return fail(ctx, SIMON_ERR_INVALID, "scenario %u of a batch of %u", scenario, ctx->storage_batch.n);
+    if (dev_alloc && !ctx->valid.has(DEVICES)) return fail(ctx, SIMON_ERR_STATE, "no devices uploaded");
     CU(cudaSetDevice(ctx->device));
-    const uint32_t N = ctx->N;
-    if (vg_requested && ctx->V && N) CU(cudaMemcpy(vg_requested, B.vg_req.p + scenario * B.vn, 8ull * ctx->V * N, cudaMemcpyDeviceToHost));
+    const uint32_t N = ctx->snap.N;
+    if (vg_requested && ctx->storage.V && N) CU(cudaMemcpy(vg_requested, B.vg_req.p + scenario * B.vn, 8ull * ctx->storage.V * N, cudaMemcpyDeviceToHost));
     if (dev_alloc && N) CU(cudaMemcpy(dev_alloc, B.dev_alloc.p + scenario * B.nodes, 4ull * N, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
@@ -1350,7 +1402,7 @@ static uint64_t drain_scenario_bytes(const simon_ctx *ctx) {
 
 extern "C" int simon_drain_budget(simon_ctx *ctx, uint64_t *scenario_bytes, uint64_t *free_bytes) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_drain_budget before uploads");
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_drain_budget before uploads");
     CU(cudaSetDevice(ctx->device));
     const uint64_t per = drain_scenario_bytes(ctx);
     if (scenario_bytes) *scenario_bytes = per;
@@ -1373,9 +1425,9 @@ extern "C" int simon_drain_budget(simon_ctx *ctx, uint64_t *scenario_bytes, uint
 
 extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario *remain, uint32_t n, simon_drain_result *out) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_drain_run before uploads");
-    if ((ctx->n_pods && !placed) || (n && (!remain || !out))) return fail(ctx, SIMON_ERR_INVALID, "simon_drain_run: NULL argument");
-    const uint32_t N = ctx->N, N1 = std::max(1u, N), P = ctx->n_pods;
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_drain_run before uploads");
+    if ((ctx->pods.n_pods && !placed) || (n && (!remain || !out))) return fail(ctx, SIMON_ERR_INVALID, "simon_drain_run: NULL argument");
+    const uint32_t N = ctx->snap.N, N1 = std::max(1u, N), P = ctx->pods.n_pods;
     // ---- refusals before any device work: the live placement as a resume prefix checks it, then the node lists ----
     int rc = check_prefix(ctx, placed, P);
     if (rc) return rc;
@@ -1386,9 +1438,8 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
     if (rc) return rc;
     CU(cudaSetDevice(ctx->device));
     ctx->last_launch = simon_launch_info{};
-    ctx->dr_n = 0;
+    ctx->valid.drop(DRAIN_BATCH | STORAGE_BATCH);     // the batch pool's Open-Local slices are no longer a storage batch's
     ScenPool &S = ctx->single, &B = ctx->batch;
-    B.n_storage = 0;                    // the batch pool's Open-Local slices are no longer a storage batch's
     if (n == 0) return SIMON_OK;
     cudaStream_t st = ctx->stream;
     // ---- per scenario, from the pods each node holds (one CSR): the pods of its removed nodes in pod order, as (scenario, pod)
@@ -1404,10 +1455,10 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
         for (uint32_t q = 0; q < P; q++)
             if (placed[q] >= 0) node_pods[cur[placed[q]]++] = q;
     }
-    ctx->dr_off.assign(1, 0u); ctx->dr_pods.clear(); ctx->dr_boff.assign(1, 0u); ctx->dr_blocked.clear();
+    ctx->drain.off.assign(1, 0u); ctx->drain.pods.clear(); ctx->drain.boff.assign(1, 0u); ctx->drain.blocked.clear();
     std::vector<uint2> pairs;
     std::vector<uint32_t> n_vanished(n, 0u), rm;
-    ctx->dr_max = 0;
+    ctx->drain.max = 0;
     for (uint32_t i = 0; i < n; i++) {
         const int32_t *rank = B.h_rank.data() + (size_t)i * N1;
         rm.clear();
@@ -1416,16 +1467,16 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
         std::sort(rm.begin(), rm.end());
         for (uint32_t q : rm) {
             pairs.push_back(make_uint2(i, q));
-            const int32_t gd = ctx->h_guard[q];
+            const int32_t gd = ctx->pods.h_guard[q];
             if (gd >= 0 && rank[gd] < 0) n_vanished[i]++;
-            else if (ctx->h_fixed[q] >= 0 || (ctx->have_storage && ctx->h_class_local[ctx->h_class[q]])) ctx->dr_blocked.push_back(q);
-            else ctx->dr_pods.push_back(q);
+            else if (ctx->pods.h_fixed[q] >= 0 || (ctx->valid.has(STORAGE) && ctx->storage.h_class_local[ctx->pods.h_class[q]])) ctx->drain.blocked.push_back(q);
+            else ctx->drain.pods.push_back(q);
         }
-        ctx->dr_off.push_back((uint32_t)ctx->dr_pods.size());
-        ctx->dr_boff.push_back((uint32_t)ctx->dr_blocked.size());
-        ctx->dr_max = std::max(ctx->dr_max, ctx->dr_off[i + 1] - ctx->dr_off[i]);
+        ctx->drain.off.push_back((uint32_t)ctx->drain.pods.size());
+        ctx->drain.boff.push_back((uint32_t)ctx->drain.blocked.size());
+        ctx->drain.max = std::max(ctx->drain.max, ctx->drain.off[i + 1] - ctx->drain.off[i]);
     }
-    const size_t n_ev = ctx->dr_pods.size();
+    const size_t n_ev = ctx->drain.pods.size();
     // ---- geometry of the drain variant, the batch pool and the outputs (allocations before the timed work) ----
     uint32_t CS, TPB, NPT;
     size_t smem;
@@ -1433,19 +1484,19 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
     if (rc) return rc;
     rc = size_pool(ctx, B, n, false, false);
     if (rc) return rc;
-    CU(ctx->d_dr_pods.upload(ctx->dr_pods.data(), n_ev, st));
-    CU(ctx->d_dr_off.upload(ctx->dr_off.data(), n + 1, st));
-    CU(ctx->d_dr_pairs.upload(pairs.data(), pairs.size(), st));
-    CU(ctx->d_dr_node.alloc(n_ev)); CU(ctx->d_dr_gpu.alloc(n_ev));
-    if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(ctx->d_dr_score.alloc(n_ev));
-    CU(ctx->d_dr_fail_counts.alloc((size_t)n * ctx->dr_max * SIMON_N_FAIL_CODES)); CU(ctx->d_dr_fail_pod.alloc((size_t)n * ctx->dr_max));
+    CU(ctx->drain.d_pods.upload(ctx->drain.pods.data(), n_ev, st));
+    CU(ctx->drain.d_off.upload(ctx->drain.off.data(), n + 1, st));
+    CU(ctx->drain.d_pairs.upload(pairs.data(), pairs.size(), st));
+    CU(ctx->drain.d_node.alloc(n_ev)); CU(ctx->drain.d_gpu.alloc(n_ev));
+    if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(ctx->drain.d_score.alloc(n_ev));
+    CU(ctx->drain.d_fail_counts.alloc((size_t)n * ctx->drain.max * SIMON_N_FAIL_CODES)); CU(ctx->drain.d_fail_pod.alloc((size_t)n * ctx->drain.max));
     std::vector<SkScenario> h;
     CU(batch_scenarios(ctx, remain, n, h));
     for (uint32_t i = 0; i < n; i++) {
-        h[i].out_node = ctx->d_dr_node.p; h[i].out_gpu = ctx->d_dr_gpu.p;
-        h[i].out_score = (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) ? ctx->d_dr_score.p : nullptr;
-        h[i].fail_counts = ctx->d_dr_fail_counts.p + (size_t)i * ctx->dr_max * SIMON_N_FAIL_CODES;
-        h[i].fail_pod = ctx->d_dr_fail_pod.p + (size_t)i * ctx->dr_max;
+        h[i].out_node = ctx->drain.d_node.p; h[i].out_gpu = ctx->drain.d_gpu.p;
+        h[i].out_score = (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) ? ctx->drain.d_score.p : nullptr;
+        h[i].fail_counts = ctx->drain.d_fail_counts.p + (size_t)i * ctx->drain.max * SIMON_N_FAIL_CODES;
+        h[i].fail_pod = ctx->drain.d_fail_pod.p + (size_t)i * ctx->drain.max;
     }
     CU(B.scen.upload(h.data(), n, st));
     // ---- setup: the live state in the single-scenario pool (the resume's rebuild, its failure records cleared as the resume clears
@@ -1463,121 +1514,123 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
     CU(cudaMemsetAsync(B.csum.p, 0, 8 * n * B.ncl * SK_CSUM_W, st));
     CU(cudaMemsetAsync(B.ocache.p, 0, 8 * n * B.nodes * B.ncl, st));
     CU(cudaMemsetAsync(B.counters.p, 0, 8ull * n, st)); CU(cudaMemsetAsync(B.clk.p, 0, 16ull * n, st));
-    CU(cudaMemsetAsync(ctx->d_dr_fail_counts.p, 0, 4ull * n * ctx->dr_max * SIMON_N_FAIL_CODES, st));
+    CU(cudaMemsetAsync(ctx->drain.d_fail_counts.p, 0, 4ull * n * ctx->drain.max * SIMON_N_FAIL_CODES, st));
     // every slot = the live state, one broadcast per column
     CU(B.state.each(S.state, true, [&](auto &b, auto &s, uint64_t k) { ctx->launches++; return bcast(ctx, s.p, k, n, b.p); }));
     SkParams Pb;
     fill_params(ctx, B, Pb);
     if (!pairs.empty()) {
         const uint32_t grid = (uint32_t)std::min<size_t>((pairs.size() + 255) / 256, (size_t)ctx->sms * 4);
-        simon_drain_unimport<<<grid, 256, 0, st>>>(Pb, ctx->d_prefix.p, ctx->d_dr_pairs.p, (uint32_t)pairs.size());
+        simon_drain_unimport<<<grid, 256, 0, st>>>(Pb, ctx->d_prefix.p, ctx->drain.d_pairs.p, (uint32_t)pairs.size());
         CU(cudaGetLastError());
         ctx->launches++;
     }
     CU(cudaEventRecord(ctx->evm, st));
     // ---- placement of every scenario's evicted pods ----
-    Pb.drain_pods = ctx->d_dr_pods.p; Pb.drain_off = ctx->d_dr_off.p;
-    Pb.first = 0; Pb.count = 0; Pb.max_fail = ctx->dr_max; Pb.npt = NPT;
+    Pb.drain_pods = ctx->drain.d_pods.p; Pb.drain_off = ctx->drain.d_off.p;
+    Pb.first = 0; Pb.count = 0; Pb.max_fail = ctx->drain.max; Pb.npt = NPT;
     rc = launch(ctx, Pb, n, CS, TPB, smem, false, true);
     if (rc) return rc;
     CU(cudaEventRecord(ctx->ev1, st));
-    simon_scen_reduce<<<n, 256, 0, st>>>(B.scen.p, ctx->d_alloc_mcpu.p, ctx->d_alloc_mem.p, B.results.p);
+    simon_scen_reduce<<<n, 256, 0, st>>>(B.scen.p, ctx->snap.d_alloc_mcpu.p, ctx->snap.d_alloc_mem.p, B.results.p);
     CU(cudaGetLastError());
     std::vector<simon_scenario_result> res(n);
     CU(cudaMemcpyAsync(res.data(), B.results.p, sizeof(simon_scenario_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
     // with a PDB table: `allowed` on the rebuilt live state, read at the same synchronisation
-    std::vector<int32_t> allowed(ctx->n_pdbs);
-    if (ctx->n_pdbs) {
+    const uint32_t J = ctx->valid.has(PDB_TABLE) ? ctx->pdb.n : 0;
+    std::vector<int32_t> allowed(J);
+    if (J) {
         CU(pdb_allowed(ctx, S.out_node.p));
-        CU(cudaMemcpyAsync(allowed.data(), ctx->d_pdb_rem.p, 4ull * ctx->n_pdbs, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(allowed.data(), ctx->pdb.d_rem.p, 4ull * J, cudaMemcpyDeviceToHost, st));
     }
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
-    ctx->have_live = true;
-    CU(cudaEventElapsedTime(&ctx->dr_setup_ms, ctx->ev0, ctx->evm));
-    CU(cudaEventElapsedTime(&ctx->dr_place_ms, ctx->evm, ctx->ev1));
+    ctx->valid.set(LIVE);
+    CU(cudaEventElapsedTime(&ctx->drain.setup_ms, ctx->ev0, ctx->evm));
+    CU(cudaEventElapsedTime(&ctx->drain.place_ms, ctx->evm, ctx->ev1));
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     // violated PDBs per drain: its evicted members per PDB (filterPodsWithPDBViolation's count) above `allowed`
-    ctx->dr_voff.assign(1, 0u); ctx->dr_vpdb.clear(); ctx->dr_vcnt.clear();
+    ctx->drain.voff.assign(1, 0u); ctx->drain.vpdb.clear(); ctx->drain.vcnt.clear();
     {
-        std::vector<uint32_t> cnt(ctx->n_pdbs, 0u), touched;
-        for (uint32_t i = 0; i < n && ctx->n_pdbs; i++) {
-            for (uint32_t k = ctx->dr_off[i]; k < ctx->dr_off[i + 1]; k++) {
-                const uint32_t q = ctx->dr_pods[k];
-                for (uint32_t u = ctx->h_pdb_off[q]; u < ctx->h_pdb_off[q + 1]; u++)
-                    if (!cnt[ctx->h_pdb_ids[u]]++) touched.push_back(ctx->h_pdb_ids[u]);
+        std::vector<uint32_t> cnt(J, 0u), touched;
+        for (uint32_t i = 0; i < n && J; i++) {
+            for (uint32_t k = ctx->drain.off[i]; k < ctx->drain.off[i + 1]; k++) {
+                const uint32_t q = ctx->drain.pods[k];
+                for (uint32_t u = ctx->pdb.h_off[q]; u < ctx->pdb.h_off[q + 1]; u++)
+                    if (!cnt[ctx->pdb.h_ids[u]]++) touched.push_back(ctx->pdb.h_ids[u]);
             }
             std::sort(touched.begin(), touched.end());
             for (uint32_t j : touched) {
-                if ((int64_t)cnt[j] > (int64_t)allowed[j]) { ctx->dr_vpdb.push_back(j); ctx->dr_vcnt.push_back(cnt[j]); }
+                if ((int64_t)cnt[j] > (int64_t)allowed[j]) { ctx->drain.vpdb.push_back(j); ctx->drain.vcnt.push_back(cnt[j]); }
                 cnt[j] = 0;
             }
             touched.clear();
-            ctx->dr_voff.push_back((uint32_t)ctx->dr_vpdb.size());
+            ctx->drain.voff.push_back((uint32_t)ctx->drain.vpdb.size());
         }
-        if (!ctx->n_pdbs) ctx->dr_voff.assign(n + 1, 0u);
+        if (!J) ctx->drain.voff.assign(n + 1, 0u);
     }
-    ctx->dr_nfail.resize(n);
+    ctx->drain.nfail.resize(n);
     for (uint32_t i = 0; i < n; i++) {
         simon_drain_result &o = out[i];
-        o.n_evicted = ctx->dr_off[i + 1] - ctx->dr_off[i];
+        o.n_evicted = ctx->drain.off[i + 1] - ctx->drain.off[i];
         o.n_placed = res[i].n_scheduled; o.n_unscheduled = res[i].n_unscheduled;
-        o.n_blocked = ctx->dr_boff[i + 1] - ctx->dr_boff[i];
-        o.n_vanished = n_vanished[i]; o.n_pdb_violated = ctx->dr_voff[i + 1] - ctx->dr_voff[i];
+        o.n_blocked = ctx->drain.boff[i + 1] - ctx->drain.boff[i];
+        o.n_vanished = n_vanished[i]; o.n_pdb_violated = ctx->drain.voff[i + 1] - ctx->drain.voff[i];
         o.req_mcpu = res[i].req_mcpu; o.alloc_mcpu = res[i].alloc_mcpu; o.req_mem = res[i].req_mem; o.alloc_mem = res[i].alloc_mem;
-        ctx->dr_nfail[i] = res[i].n_unscheduled;
+        ctx->drain.nfail[i] = res[i].n_unscheduled;
     }
-    ctx->dr_n = n;
+    ctx->drain.n = n;
+    ctx->valid.set(DRAIN_BATCH);
     return SIMON_OK;
 }
 
 extern "C" int simon_drain_times(simon_ctx *ctx, float *setup_ms, float *place_ms) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (setup_ms) *setup_ms = ctx->dr_setup_ms;
-    if (place_ms) *place_ms = ctx->dr_place_ms;
+    if (setup_ms) *setup_ms = ctx->drain.setup_ms;
+    if (place_ms) *place_ms = ctx->drain.place_ms;
     return SIMON_OK;
 }
 
 extern "C" int simon_drain_download(simon_ctx *ctx, uint32_t scenario, uint32_t *evicted_pod, int32_t *node, uint32_t *gpu_slots,
                                     int64_t *score, uint32_t *blocked_pod, uint32_t *fail_counts, uint32_t *fail_pod) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->dr_n) return fail(ctx, SIMON_ERR_STATE, "no simon_drain_run batch since the last upload");
-    if (scenario >= ctx->dr_n) return fail(ctx, SIMON_ERR_INVALID, "drain %u of a batch of %u", scenario, ctx->dr_n);
+    if (!ctx->valid.has(DRAIN_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_drain_run batch since the last upload");
+    if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "drain %u of a batch of %u", scenario, ctx->drain.n);
     CU(cudaSetDevice(ctx->device));
-    const uint32_t b = ctx->dr_off[scenario], ne = ctx->dr_off[scenario + 1] - b;
-    const uint32_t bb = ctx->dr_boff[scenario], nb = ctx->dr_boff[scenario + 1] - bb;
-    const uint32_t nf = std::min(ctx->dr_nfail[scenario], ctx->dr_max);
-    if (evicted_pod) std::copy(ctx->dr_pods.begin() + b, ctx->dr_pods.begin() + b + ne, evicted_pod);
-    if (blocked_pod) std::copy(ctx->dr_blocked.begin() + bb, ctx->dr_blocked.begin() + bb + nb, blocked_pod);
-    if (node && ne) CU(cudaMemcpy(node, ctx->d_dr_node.p + b, 4ull * ne, cudaMemcpyDeviceToHost));
-    if (gpu_slots && ne) CU(cudaMemcpy(gpu_slots, ctx->d_dr_gpu.p + b, 4ull * ne, cudaMemcpyDeviceToHost));
+    const uint32_t b = ctx->drain.off[scenario], ne = ctx->drain.off[scenario + 1] - b;
+    const uint32_t bb = ctx->drain.boff[scenario], nb = ctx->drain.boff[scenario + 1] - bb;
+    const uint32_t nf = std::min(ctx->drain.nfail[scenario], ctx->drain.max);
+    if (evicted_pod) std::copy(ctx->drain.pods.begin() + b, ctx->drain.pods.begin() + b + ne, evicted_pod);
+    if (blocked_pod) std::copy(ctx->drain.blocked.begin() + bb, ctx->drain.blocked.begin() + bb + nb, blocked_pod);
+    if (node && ne) CU(cudaMemcpy(node, ctx->drain.d_node.p + b, 4ull * ne, cudaMemcpyDeviceToHost));
+    if (gpu_slots && ne) CU(cudaMemcpy(gpu_slots, ctx->drain.d_gpu.p + b, 4ull * ne, cudaMemcpyDeviceToHost));
     if (score && ne) {
-        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(cudaMemcpy(score, ctx->d_dr_score.p + b, 8ull * ne, cudaMemcpyDeviceToHost));
+        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(cudaMemcpy(score, ctx->drain.d_score.p + b, 8ull * ne, cudaMemcpyDeviceToHost));
         else memset(score, 0, 8ull * ne);
     }
     if (fail_counts && nf)
-        CU(cudaMemcpy(fail_counts, ctx->d_dr_fail_counts.p + (size_t)scenario * ctx->dr_max * SIMON_N_FAIL_CODES,
+        CU(cudaMemcpy(fail_counts, ctx->drain.d_fail_counts.p + (size_t)scenario * ctx->drain.max * SIMON_N_FAIL_CODES,
                       4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
-    if (fail_pod && nf) CU(cudaMemcpy(fail_pod, ctx->d_dr_fail_pod.p + (size_t)scenario * ctx->dr_max, 4ull * nf, cudaMemcpyDeviceToHost));
+    if (fail_pod && nf) CU(cudaMemcpy(fail_pod, ctx->drain.d_fail_pod.p + (size_t)scenario * ctx->drain.max, 4ull * nf, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
 extern "C" int simon_drain_pdb_download(simon_ctx *ctx, uint32_t scenario, uint32_t *pdb, uint32_t *evicted) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->dr_n) return fail(ctx, SIMON_ERR_STATE, "no simon_drain_run batch since the last upload");
-    if (scenario >= ctx->dr_n) return fail(ctx, SIMON_ERR_INVALID, "drain %u of a batch of %u", scenario, ctx->dr_n);
-    const uint32_t b = ctx->dr_voff[scenario], e = ctx->dr_voff[scenario + 1];
-    if (pdb) std::copy(ctx->dr_vpdb.begin() + b, ctx->dr_vpdb.begin() + e, pdb);
-    if (evicted) std::copy(ctx->dr_vcnt.begin() + b, ctx->dr_vcnt.begin() + e, evicted);
+    if (!ctx->valid.has(DRAIN_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_drain_run batch since the last upload");
+    if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "drain %u of a batch of %u", scenario, ctx->drain.n);
+    const uint32_t b = ctx->drain.voff[scenario], e = ctx->drain.voff[scenario + 1];
+    if (pdb) std::copy(ctx->drain.vpdb.begin() + b, ctx->drain.vpdb.begin() + e, pdb);
+    if (evicted) std::copy(ctx->drain.vcnt.begin() + b, ctx->drain.vcnt.begin() + e, evicted);
     return SIMON_OK;
 }
 
 // ---- PodDisruptionBudgets ----------------------------------------------------------------------------------------------------------
 extern "C" int simon_pdbs_upload(simon_ctx *ctx, const simon_pdbs *t) {
     if (!ctx || !t) return SIMON_ERR_INVALID;
-    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_pdbs_upload before simon_pods_upload");
-    const uint32_t P = ctx->n_pods, J = t->n_pdbs;
-    if (J == 0) { ctx->n_pdbs = 0; return SIMON_OK; }
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_pdbs_upload before simon_pods_upload");
+    const uint32_t P = ctx->pods.n_pods, J = t->n_pdbs;
+    if (J == 0) { ctx->valid.drop(PDB_TABLE); return SIMON_OK; }
     // ---- refusals before any device work ----
     if (t->n_pods != P) return fail(ctx, SIMON_ERR_INVALID, "simon_pdbs_upload: n_pods %u, the pod set has %u", t->n_pods, P);
     if (!t->pod_off || !t->desired) return fail(ctx, SIMON_ERR_INVALID, "simon_pdbs_upload: NULL pod_off or desired");
@@ -1607,26 +1660,28 @@ extern "C" int simon_pdbs_upload(simon_ctx *ctx, const simon_pdbs *t) {
     for (uint32_t q = 0; q < P; q++)
         for (uint32_t k = t->pod_off[q]; k < t->pod_off[q + 1]; k++) members[cur[t->pod_pdb[k]]++] = q;
     CU(cudaSetDevice(ctx->device));
+    ctx->valid.drop(PDB_TABLE);
     cudaStream_t st = ctx->stream;
-    ctx->h_pdb_off.assign(t->pod_off, t->pod_off + P + 1);
-    ctx->h_pdb_ids.assign(t->pod_pdb, t->pod_pdb + E);
-    CU(ctx->d_pdb_off.upload(t->pod_off, P + 1, st)); CU(ctx->d_pdb_ids.upload(t->pod_pdb, E, st));
-    CU(ctx->d_pdb_moff.upload(moff.data(), J + 1, st)); CU(ctx->d_pdb_members.upload(members.data(), E, st));
-    CU(ctx->d_pdb_desired.upload(t->desired, J, st)); CU(ctx->d_pdb_rem.alloc(J));
-    CU(ctx->d_pdb_ctl.alloc(4)); CU(ctx->d_pdb_hit.alloc(std::max(1u, max_per_pod)));
+    ctx->pdb.h_off.assign(t->pod_off, t->pod_off + P + 1);
+    ctx->pdb.h_ids.assign(t->pod_pdb, t->pod_pdb + E);
+    CU(ctx->pdb.d_off.upload(t->pod_off, P + 1, st)); CU(ctx->pdb.d_ids.upload(t->pod_pdb, E, st));
+    CU(ctx->pdb.d_moff.upload(moff.data(), J + 1, st)); CU(ctx->pdb.d_members.upload(members.data(), E, st));
+    CU(ctx->pdb.d_desired.upload(t->desired, J, st)); CU(ctx->pdb.d_rem.alloc(J));
+    CU(ctx->pdb.d_ctl.alloc(4)); CU(ctx->pdb.d_hit.alloc(std::max(1u, max_per_pod)));
     CU(cudaStreamSynchronize(st));       // the host vectors leave scope
-    ctx->n_pdbs = J; ctx->pdb_max_per_pod = max_per_pod; ctx->pdb_max_members = max_members;
+    ctx->pdb.n = J; ctx->pdb.max_per_pod = max_per_pod; ctx->pdb.max_members = max_members;
+    ctx->valid.set(PDB_TABLE);
     return SIMON_OK;
 }
 
 extern "C" int simon_pdbs_allowed(simon_ctx *ctx, int32_t *allowed) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->have_live) return fail(ctx, SIMON_ERR_STATE, "simon_pdbs_allowed: no placement since the last pod upload or reset");
-    if (!ctx->n_pdbs) return SIMON_OK;
+    if (!ctx->valid.has(LIVE)) return fail(ctx, SIMON_ERR_STATE, "simon_pdbs_allowed: no placement since the last pod upload or reset");
+    if (!ctx->valid.has(PDB_TABLE)) return SIMON_OK;
     if (!allowed) return fail(ctx, SIMON_ERR_INVALID, "simon_pdbs_allowed: NULL allowed");
     CU(cudaSetDevice(ctx->device));
     CU(pdb_allowed(ctx, ctx->single.out_node.p));
-    CU(cudaMemcpyAsync(allowed, ctx->d_pdb_rem.p, 4ull * ctx->n_pdbs, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(allowed, ctx->pdb.d_rem.p, 4ull * ctx->pdb.n, cudaMemcpyDeviceToHost, ctx->stream));
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "PDB count failed: %s", cudaGetErrorString(e));
     return SIMON_OK;
@@ -1634,28 +1689,28 @@ extern "C" int simon_pdbs_allowed(simon_ctx *ctx, int32_t *allowed) {
 
 int simon_debug_set_dump_pod(simon_ctx *ctx, uint32_t pod) {
     if (!ctx) return SIMON_ERR_INVALID;
-    ctx->dump_pod = pod;
+    ctx->pods.dump_pod = pod;
     return SIMON_OK;
 }
 
 int simon_debug_dump_read(simon_ctx *ctx, int64_t *out_total, int32_t *out_code) {
-    if (!ctx || !ctx->have_pods) return SIMON_ERR_STATE;
+    if (!ctx || !ctx->valid.has(POD_SET)) return SIMON_ERR_STATE;
     CU(cudaSetDevice(ctx->device));
-    if (out_total) CU(cudaMemcpy(out_total, ctx->d_dump_total.p, 8ull * ctx->N, cudaMemcpyDeviceToHost));
-    if (out_code) CU(cudaMemcpy(out_code, ctx->d_dump_code.p, 4ull * ctx->N, cudaMemcpyDeviceToHost));
+    if (out_total) CU(cudaMemcpy(out_total, ctx->pods.d_dump_total.p, 8ull * ctx->snap.N, cudaMemcpyDeviceToHost));
+    if (out_code) CU(cudaMemcpy(out_code, ctx->pods.d_dump_code.p, 4ull * ctx->snap.N, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
 int simon_gpu_slots_download(simon_ctx *ctx, uint32_t first, uint32_t count, uint32_t *out_slots) {
-    if (!ctx || !ctx->have_pods || !out_slots) return SIMON_ERR_STATE;
-    if ((uint64_t)first + count > ctx->n_pods) return fail(ctx, SIMON_ERR_INVALID, "range out of bounds");
+    if (!ctx || !ctx->valid.has(POD_SET) || !out_slots) return SIMON_ERR_STATE;
+    if ((uint64_t)first + count > ctx->pods.n_pods) return fail(ctx, SIMON_ERR_INVALID, "range out of bounds");
     CU(cudaSetDevice(ctx->device));
     CU(cudaMemcpy(out_slots, ctx->single.out_gpu.p + first, 4ull * count, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
 int simon_state_download_ext(simon_ctx *ctx, int64_t *req_scalar, int64_t *gpu_used) {
-    if (!ctx || !ctx->have_pods) return SIMON_ERR_STATE;
+    if (!ctx || !ctx->valid.has(POD_SET)) return SIMON_ERR_STATE;
     CU(cudaSetDevice(ctx->device));
     void *const dst[NodeState::COLS] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, req_scalar, gpu_used};
     CU(ctx->single.state.download(dst));
@@ -1664,10 +1719,8 @@ int simon_state_download_ext(simon_ctx *ctx, int64_t *req_scalar, int64_t *gpu_u
 
 int simon_storage_upload(simon_ctx *ctx, const simon_storage *sg) {
     if (!ctx || !sg) return SIMON_ERR_INVALID;
-    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_storage_upload before simon_pods_upload");
-    ctx->have_devices = false;          // device tables belong to the storage upload they followed
-    ctx->batch.n_storage = 0;           // and so does the state of the last storage batch
-    const uint32_t N = ctx->N, V = sg->n_vgs, C = ctx->n_classes;
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_storage_upload before simon_pods_upload");
+    const uint32_t N = ctx->snap.N, V = sg->n_vgs, C = ctx->pods.n_classes;
     if (sg->n_classes != C) return fail(ctx, SIMON_ERR_INVALID, "storage table has %u classes, the pod set %u", sg->n_classes, C);
     if (V > SIMON_MAX_VGS) return fail(ctx, SIMON_ERR_LIMIT, "more than %d VGs per node", SIMON_MAX_VGS);
     if (!sg->node_n_vg || !sg->class_local || !sg->vol_off || (V && N && (!sg->vg_capacity || !sg->vg_requested || !sg->vg_name)))
@@ -1692,64 +1745,44 @@ int simon_storage_upload(simon_ctx *ctx, const simon_storage *sg) {
         if (sg->vol_vg[q] < -1) return fail(ctx, SIMON_ERR_INVALID, "volume %u: VG name id must be >= -1", q);
     }
     CU(cudaSetDevice(ctx->device));
+    ctx->valid.drop(STORAGE);
     cudaStream_t st = ctx->stream;
     const size_t VN = std::max<size_t>(1, (size_t)V * N);
     std::vector<int64_t> zero64(VN, 0);
     std::vector<int32_t> zero32(VN, 0);
-    CU(ctx->d_node_n_vg.upload(sg->node_n_vg, std::max(1u, N), st));
-    CU(ctx->d_vg_cap.upload(V && N ? sg->vg_capacity : zero64.data(), VN, st));
-    CU(ctx->d_vg_req0.upload(V && N ? sg->vg_requested : zero64.data(), VN, st));
-    CU(ctx->d_vg_name.upload(V && N ? sg->vg_name : zero32.data(), VN, st));
-    CU(ctx->d_class_local.upload(sg->class_local, std::max(1u, C), st));
-    CU(ctx->d_vol_off.upload(sg->vol_off, C + 1, st));
+    CU(ctx->storage.d_node_n_vg.upload(sg->node_n_vg, std::max(1u, N), st));
+    CU(ctx->storage.d_vg_cap.upload(V && N ? sg->vg_capacity : zero64.data(), VN, st));
+    CU(ctx->storage.d_vg_req0.upload(V && N ? sg->vg_requested : zero64.data(), VN, st));
+    CU(ctx->storage.d_vg_name.upload(V && N ? sg->vg_name : zero32.data(), VN, st));
+    CU(ctx->storage.d_class_local.upload(sg->class_local, std::max(1u, C), st));
+    CU(ctx->storage.d_vol_off.upload(sg->vol_off, C + 1, st));
     std::vector<int64_t> vs(sg->vol_size, sg->vol_size + n_vol); vs.push_back(0);
     std::vector<int32_t> vv(sg->vol_vg, sg->vol_vg + n_vol); vv.push_back(0);
-    CU(ctx->d_vol_size.upload(vs.data(), vs.size(), st)); CU(ctx->d_vol_vg.upload(vv.data(), vv.size(), st));
-    // pods of classes with local storage read the VGs of every node: off the pinned-run fast path (-4) ...
-    if (ctx->n_pin_fast) {
-        std::vector<int32_t> fixed(ctx->n_pods), cls(ctx->n_pods);
-        CU(cudaMemcpyAsync(fixed.data(), ctx->d_pod_fixed.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost, st));
-        CU(cudaMemcpyAsync(cls.data(), ctx->d_pod_class.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
-        for (uint32_t i = 0; i < ctx->n_pods; i++)
-            if (fixed[i] == -4 && sg->class_local[cls[i]]) { fixed[i] = -1; ctx->n_pin_fast--; }
-        CU(ctx->d_pod_fixed.upload(fixed.data(), ctx->n_pods, st));
-        CU(cudaStreamSynchronize(st));      // `fixed` leaves scope
-    }
-    // ... and not candidates of the move scoring
-    {
-        std::vector<SmvClass> mc(std::max(1u, C));
-        CU(cudaMemcpyAsync(mc.data(), ctx->d_mv_classes.p, sizeof(SmvClass) * mc.size(), cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
-        for (uint32_t c = 0; c < C; c++)
-            if (sg->class_local[c]) { mc[c].bits |= SMC_NOT_MOVABLE | SMC_NEVER; ctx->h_mv_bits[c] = mc[c].bits; }
-        ctx->mv_scope_dirty = true;
-        CU(ctx->d_mv_classes.upload(mc.data(), mc.size(), st));
-        CU(cudaStreamSynchronize(st));      // `mc` leaves scope
-    }
-    ctx->V = V;
-    ctx->h_class_local.assign(sg->class_local, sg->class_local + C);
-    ctx->have_storage = true;
-    ctx->have_live = false;
-    int rc = alloc_pool(ctx, ctx->single, 1, true);
+    CU(ctx->storage.d_vol_size.upload(vs.data(), vs.size(), st)); CU(ctx->storage.d_vol_vg.upload(vv.data(), vv.size(), st));
+    ctx->storage.V = V;
+    ctx->storage.h_class_local.assign(sg->class_local, sg->class_local + C);
+    int rc = upload_class_marks(ctx, sg->class_local);
     if (rc) return rc;
+    // the single-scenario pool gains the VG columns, and starts from the uploaded VG requested values
+    ctx->valid.set(STORAGE);
+    rc = alloc_pool(ctx, ctx->single, 1, true);
+    if (rc) { ctx->valid.drop(STORAGE); return rc; }
     CU(cudaStreamSynchronize(st));
     return SIMON_OK;
 }
 
 int simon_storage_state_download(simon_ctx *ctx, int64_t *vg_requested) {
     if (!ctx || !vg_requested) return SIMON_ERR_INVALID;
-    if (!ctx->have_storage) return fail(ctx, SIMON_ERR_STATE, "no storage uploaded");
+    if (!ctx->valid.has(STORAGE)) return fail(ctx, SIMON_ERR_STATE, "no storage uploaded");
     CU(cudaSetDevice(ctx->device));
-    if (ctx->V && ctx->N) CU(cudaMemcpy(vg_requested, ctx->single.vg_req.p, 8ull * ctx->V * ctx->N, cudaMemcpyDeviceToHost));
+    if (ctx->storage.V && ctx->snap.N) CU(cudaMemcpy(vg_requested, ctx->single.vg_req.p, 8ull * ctx->storage.V * ctx->snap.N, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
 int simon_devices_upload(simon_ctx *ctx, const simon_devices *dv) {
     if (!ctx || !dv) return SIMON_ERR_INVALID;
-    if (!ctx->have_storage) return fail(ctx, SIMON_ERR_STATE, "simon_devices_upload before simon_storage_upload");
-    ctx->batch.n_storage = 0;           // the last storage batch ran on the device tables this upload replaces
-    const uint32_t N = ctx->N, D = dv->n_slots, C = ctx->n_classes;
+    if (!ctx->valid.has(STORAGE)) return fail(ctx, SIMON_ERR_STATE, "simon_devices_upload before simon_storage_upload");
+    const uint32_t N = ctx->snap.N, D = dv->n_slots, C = ctx->pods.n_classes;
     if (dv->n_classes != C) return fail(ctx, SIMON_ERR_INVALID, "device table has %u classes, the pod set %u", dv->n_classes, C);
     if (D > SIMON_MAX_DEVS) return fail(ctx, SIMON_ERR_LIMIT, "more than %d devices per node", SIMON_MAX_DEVS);
     if (!dv->node_n_ssd || !dv->node_n_hdd || !dv->dev_alloc || !dv->ssd_off || !dv->hdd_off || (D && N && !dv->dev_capacity))
@@ -1779,56 +1812,57 @@ int simon_devices_upload(simon_ctx *ctx, const simon_devices *dv) {
     for (uint32_t c = 0; c < C; c++) {
         const uint32_t n = (dv->ssd_off[c + 1] - dv->ssd_off[c]) + (dv->hdd_off[c + 1] - dv->hdd_off[c]);
         if (n > SIMON_MAX_DEV_VOLS) return fail(ctx, SIMON_ERR_LIMIT, "class %u: more than %d device volumes", c, SIMON_MAX_DEV_VOLS);
-        if (n && !ctx->h_class_local[c]) return fail(ctx, SIMON_ERR_INVALID, "class %u: device volumes without the local flag", c);
+        if (n && !ctx->storage.h_class_local[c]) return fail(ctx, SIMON_ERR_INVALID, "class %u: device volumes without the local flag", c);
     }
     CU(cudaSetDevice(ctx->device));
+    ctx->valid.drop(DEVICES);
     cudaStream_t st = ctx->stream;
     const size_t DN = std::max<size_t>(1, (size_t)D * N);
     std::vector<int64_t> zero64(DN, 0);
-    CU(ctx->d_node_n_ssd.upload(dv->node_n_ssd, std::max(1u, N), st));
-    CU(ctx->d_node_n_hdd.upload(dv->node_n_hdd, std::max(1u, N), st));
-    CU(ctx->d_dev_cap.upload(D && N ? dv->dev_capacity : zero64.data(), DN, st));
-    CU(ctx->d_dev_alloc0.upload(dv->dev_alloc, std::max(1u, N), st));
-    CU(ctx->d_ssd_off.upload(dv->ssd_off, C + 1, st));
-    CU(ctx->d_hdd_off.upload(dv->hdd_off, C + 1, st));
+    CU(ctx->devices.d_node_n_ssd.upload(dv->node_n_ssd, std::max(1u, N), st));
+    CU(ctx->devices.d_node_n_hdd.upload(dv->node_n_hdd, std::max(1u, N), st));
+    CU(ctx->devices.d_dev_cap.upload(D && N ? dv->dev_capacity : zero64.data(), DN, st));
+    CU(ctx->devices.d_dev_alloc0.upload(dv->dev_alloc, std::max(1u, N), st));
+    CU(ctx->devices.d_ssd_off.upload(dv->ssd_off, C + 1, st));
+    CU(ctx->devices.d_hdd_off.upload(dv->hdd_off, C + 1, st));
     std::vector<int64_t> ss(dv->ssd_size, dv->ssd_size + (C ? dv->ssd_off[C] : 0)); ss.push_back(0);
     std::vector<int64_t> hs(dv->hdd_size, dv->hdd_size + (C ? dv->hdd_off[C] : 0)); hs.push_back(0);
-    CU(ctx->d_ssd_size.upload(ss.data(), ss.size(), st)); CU(ctx->d_hdd_size.upload(hs.data(), hs.size(), st));
-    ctx->have_devices = true;
-    ctx->have_live = false;
-    int rc = alloc_pool(ctx, ctx->single, 1, true);
-    if (rc) return rc;
+    CU(ctx->devices.d_ssd_size.upload(ss.data(), ss.size(), st)); CU(ctx->devices.d_hdd_size.upload(hs.data(), hs.size(), st));
+    // the single-scenario pool gains the device column, and starts from the uploaded allocated-slot masks
+    ctx->valid.set(DEVICES);
+    const int rc = alloc_pool(ctx, ctx->single, 1, true);
+    if (rc) { ctx->valid.drop(DEVICES); return rc; }
     CU(cudaStreamSynchronize(st));      // `ss` / `hs` leave scope
     return SIMON_OK;
 }
 
 int simon_devices_state_download(simon_ctx *ctx, uint32_t *alloc_mask) {
     if (!ctx || !alloc_mask) return SIMON_ERR_INVALID;
-    if (!ctx->have_devices) return fail(ctx, SIMON_ERR_STATE, "no devices uploaded");
+    if (!ctx->valid.has(DEVICES)) return fail(ctx, SIMON_ERR_STATE, "no devices uploaded");
     CU(cudaSetDevice(ctx->device));
-    if (ctx->N) CU(cudaMemcpy(alloc_mask, ctx->single.dev_alloc.p, 4ull * ctx->N, cudaMemcpyDeviceToHost));
+    if (ctx->snap.N) CU(cudaMemcpy(alloc_mask, ctx->single.dev_alloc.p, 4ull * ctx->snap.N, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
 // ---- candidate-move scoring (config 5) ------------------------------------------------------------------------------
 // What the current scope launches: the scoped kernel iff some class is admitted, and the prep pairs of the admitted hard classes
 static int moves_scope_refresh(simon_ctx *ctx) {
-    if (!ctx->mv_scope_dirty) return SIMON_OK;
-    const uint32_t scope = ctx->mv_scope;
+    if (ctx->valid.has(SCOPE_PREP)) return SIMON_OK;
+    const uint32_t scope = ctx->scope.bits;
     auto admitted = [&](uint32_t c) {
-        const uint32_t b = ctx->h_mv_bits[c];
+        const uint32_t b = ctx->pods.mv_bits[c];
         return scope && (b & SMC_NOT_MOVABLE) && !(b & SMC_NEVER) && !(SMC_NEED(b) & ~scope);
     };
-    ctx->mv_scoped = false;
-    for (uint32_t c = 0; c < ctx->n_classes; c++) ctx->mv_scoped |= admitted(c);
+    ctx->scope.scoped = false;
+    for (uint32_t c = 0; c < ctx->pods.n_classes; c++) ctx->scope.scoped |= admitted(c);
     std::vector<uint4> prep;
-    for (const uint4 &q : ctx->h_mv_pairs) if (admitted(q.x)) prep.push_back(q);
-    ctx->mv_n_prep = (uint32_t)prep.size();
+    for (const uint4 &q : ctx->pods.mv_pairs) if (admitted(q.x)) prep.push_back(q);
+    ctx->scope.n_prep = (uint32_t)prep.size();
     if (!prep.empty()) {
-        CU(ctx->d_mv_prep.upload(prep.data(), prep.size(), ctx->stream));
+        CU(ctx->scope.d_prep.upload(prep.data(), prep.size(), ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));      // `prep` leaves scope
     }
-    ctx->mv_scope_dirty = false;
+    ctx->valid.set(SCOPE_PREP);
     return SIMON_OK;
 }
 
@@ -1836,15 +1870,15 @@ static int moves_scope_refresh(simon_ctx *ctx) {
 static SmvParams moves_params(const simon_ctx *ctx, const NodeState &s, const int32_t *placement, uint32_t move_base) {
     SmvParams P;
     memset(&P, 0, sizeof(P));
-    P.N = ctx->N; P.K = ctx->K; P.WT = ctx->WT; P.T = ctx->T; P.n_pods = ctx->n_pods; P.n_moves = ctx->mv_n; P.use_scache = ctx->use_scache;
-    P.nodes = ctx->d_mv_nodes.p; P.alloc_scalar = ctx->d_alloc_scalar.p; P.req_scalar = s.req_scalar.p; P.node_flags = ctx->d_node_flags.p;
-    P.label_bits = ctx->d_label_bits.p; P.taint_hard = ctx->d_taint_hard.p; P.topo_dom = ctx->d_topo_dom.p; P.pods = ctx->d_mv_pods.p;
-    P.class_off = ctx->d_class_off.p; P.class_blob = ctx->d_class_blob.p; P.classes = ctx->d_mv_classes.p; P.pod_class = ctx->d_pod_class.p; P.placement = placement;
-    P.cnt = s.cnt.p; P.cnt_total = s.cnt_total.p; P.scache = ctx->d_scache.p; P.moves = ctx->d_moves.p;
-    P.out_gain = ctx->d_mv_gain.p; P.out_code = ctx->d_mv_code.p; P.best_per_pod = ctx->d_mv_best_pod.p; P.best_global = ctx->d_mv_best.p;
-    P.hist = ctx->d_mv_hist.p; P.move_base = move_base;
-    P.scope = ctx->mv_scope; P.gpu = ctx->d_mv_gpu.p; P.hs = ctx->d_mv_hs.p; P.hreg = ctx->d_mv_hreg.p;
-    P.out_slots = (ctx->mv_scope & SIMON_MOVES_SCOPE_GPU_SHARE) ? ctx->d_mv_slots.p : nullptr;
+    P.N = ctx->snap.N; P.K = ctx->snap.K; P.WT = ctx->snap.WT; P.T = ctx->snap.T; P.n_pods = ctx->pods.n_pods; P.n_moves = ctx->moves.n; P.use_scache = ctx->pods.use_scache;
+    P.nodes = ctx->moves.d_nodes.p; P.alloc_scalar = ctx->snap.d_alloc_scalar.p; P.req_scalar = s.req_scalar.p; P.node_flags = ctx->snap.d_node_flags.p;
+    P.label_bits = ctx->snap.d_label_bits.p; P.taint_hard = ctx->snap.d_taint_hard.p; P.topo_dom = ctx->snap.d_topo_dom.p; P.pods = ctx->moves.d_pods.p;
+    P.class_off = ctx->pods.d_class_off.p; P.class_blob = ctx->pods.d_class_blob.p; P.classes = ctx->pods.d_mv_classes.p; P.pod_class = ctx->pods.d_pod_class.p; P.placement = placement;
+    P.cnt = s.cnt.p; P.cnt_total = s.cnt_total.p; P.scache = ctx->pods.d_scache.p; P.moves = ctx->moves.d_moves.p;
+    P.out_gain = ctx->moves.d_gain.p; P.out_code = ctx->moves.d_code.p; P.best_per_pod = ctx->moves.d_best_pod.p; P.best_global = ctx->moves.d_best.p;
+    P.hist = ctx->moves.d_hist.p; P.move_base = move_base;
+    P.scope = ctx->scope.bits; P.gpu = ctx->moves.d_gpu.p; P.hs = ctx->pods.d_mv_hs.p; P.hreg = ctx->pods.d_mv_hreg.p;
+    P.out_slots = (ctx->scope.bits & SIMON_MOVES_SCOPE_GPU_SHARE) ? ctx->moves.d_slots.p : nullptr;
     return P;
 }
 
@@ -1852,32 +1886,32 @@ static SmvParams moves_params(const simon_ctx *ctx, const NodeState &s, const in
 // Only the SmvGpu pack is counted in simon_launch_count here; simon_moves_plan counts the other, simon_moves_run never has.
 static void moves_pack(simon_ctx *ctx, const NodeState &s, const int32_t *placement, bool gpu) {
     cudaStream_t st = ctx->stream;
-    const uint32_t N = ctx->N;
+    const uint32_t N = ctx->snap.N;
     if (gpu) {
-        simon_moves_pack_gpu<<<(N + 255) / 256, 256, 0, st>>>(N, ctx->d_gpu_count.p, ctx->d_gpu_dev_mem.p, ctx->d_gpu_total_mem.p,
-                                                               s.gpu_used.p, ctx->d_mv_gpu.p);
+        simon_moves_pack_gpu<<<(N + 255) / 256, 256, 0, st>>>(N, ctx->snap.d_gpu_count.p, ctx->snap.d_gpu_dev_mem.p, ctx->snap.d_gpu_total_mem.p,
+                                                               s.gpu_used.p, ctx->moves.d_gpu.p);
         ctx->launches++;
     }
-    simon_moves_pack<<<std::max(std::max(1u, (N + 255) / 256), std::min(1184u, (ctx->n_pods + 255) / 256)), 256, 0, st>>>(N, ctx->T, ctx->d_alloc_mcpu.p, ctx->d_alloc_mem.p, ctx->d_alloc_eph.p, ctx->d_alloc_pods.p,
-                                                                     ctx->d_topo_dom.p, s.req_mcpu.p, s.req_mem.p, s.req_eph.p,
-                                                                     s.nz_mcpu.p, s.nz_mem.p, s.num_pods.p, ctx->d_mv_nodes.p,
-                                                                     ctx->d_mv_best_pod.p, ctx->n_pods, ctx->d_mv_best.p, ctx->d_mv_hist.p,
-                                                                     ctx->d_pod_class.p, placement, ctx->d_mv_classes.p, ctx->d_mv_pods.p);
+    simon_moves_pack<<<std::max(std::max(1u, (N + 255) / 256), std::min(1184u, (ctx->pods.n_pods + 255) / 256)), 256, 0, st>>>(N, ctx->snap.T, ctx->snap.d_alloc_mcpu.p, ctx->snap.d_alloc_mem.p, ctx->snap.d_alloc_eph.p, ctx->snap.d_alloc_pods.p,
+                                                                     ctx->snap.d_topo_dom.p, s.req_mcpu.p, s.req_mem.p, s.req_eph.p,
+                                                                     s.nz_mcpu.p, s.nz_mem.p, s.num_pods.p, ctx->moves.d_nodes.p,
+                                                                     ctx->moves.d_best_pod.p, ctx->pods.n_pods, ctx->moves.d_best.p, ctx->moves.d_hist.p,
+                                                                     ctx->pods.d_pod_class.p, placement, ctx->pods.d_mv_classes.p, ctx->moves.d_pods.p);
 }
 
 // Enqueue one scoring pass with P (moves_params): the hard-spread prep when the scope admits hard classes, then the move kernel
 static void moves_score(simon_ctx *ctx, const SmvParams &P) {
     cudaStream_t st = ctx->stream;
-    if (ctx->mv_scoped && ctx->mv_n_prep) {
-        simon_moves_hard_prep<<<ctx->mv_n_prep, 256, 0, st>>>(ctx->N, ctx->use_scache, ctx->d_scache.p, ctx->d_label_bits.p, ctx->d_topo_dom.p,
-                                                              ctx->d_topo_ndom.p, ctx->d_class_off.p, ctx->d_class_blob.p, P.cnt,
-                                                              ctx->d_mv_prep.p, ctx->d_mv_hreg.p, ctx->d_mv_hs.p);
+    if (ctx->scope.scoped && ctx->scope.n_prep) {
+        simon_moves_hard_prep<<<ctx->scope.n_prep, 256, 0, st>>>(ctx->snap.N, ctx->pods.use_scache, ctx->pods.d_scache.p, ctx->snap.d_label_bits.p, ctx->snap.d_topo_dom.p,
+                                                              ctx->snap.d_topo_ndom.p, ctx->pods.d_class_off.p, ctx->pods.d_class_blob.p, P.cnt,
+                                                              ctx->scope.d_prep.p, ctx->pods.d_mv_hreg.p, ctx->pods.d_mv_hs.p);
         ctx->launches++;
     }
     if (P.n_moves) {
         // 4 resident CTAs per SM (64 registers, a few spills), two rounds of them
         const uint32_t grid = std::min<uint32_t>((P.n_moves + 255) / 256, (uint32_t)ctx->sms * 4u * 2u);
-        if (ctx->mv_scoped) simon_moves_kernel<4, true><<<grid, 256, 0, st>>>(P);
+        if (ctx->scope.scoped) simon_moves_kernel<4, true><<<grid, 256, 0, st>>>(P);
         else simon_moves_kernel<4, false><<<grid, 256, 0, st>>>(P);
         ctx->launches++;
     }
@@ -1885,19 +1919,19 @@ static void moves_score(simon_ctx *ctx, const SmvParams &P) {
 
 static int moves_launch(simon_ctx *ctx, bool record) {
     cudaStream_t st = ctx->stream;
-    const uint32_t N = ctx->N, n = ctx->mv_n, scope = ctx->mv_scope;
-    const bool gpu = ctx->mv_scoped && (scope & SIMON_MOVES_SCOPE_GPU_SHARE) && N;
+    const uint32_t N = ctx->snap.N, n = ctx->moves.n, scope = ctx->scope.bits;
+    const bool gpu = ctx->scope.scoped && (scope & SIMON_MOVES_SCOPE_GPU_SHARE) && N;
     const ScenPool &S = ctx->single;
-    if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && n) CU(ctx->d_mv_slots.alloc(n));
-    if (gpu) CU(ctx->d_mv_gpu.alloc(N));
+    if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && n) CU(ctx->moves.d_slots.alloc(n));
+    if (gpu) CU(ctx->moves.d_gpu.alloc(N));
     if (record) CU(cudaEventRecord(ctx->ev0, st));
-    if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && !ctx->mv_scoped && n) CU(cudaMemsetAsync(ctx->d_mv_slots.p, 0, 4ull * n, st));
+    if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && !ctx->scope.scoped && n) CU(cudaMemsetAsync(ctx->moves.d_slots.p, 0, 4ull * n, st));
     moves_pack(ctx, S.state, S.out_node.p, gpu);
-    if (ctx->n_pdbs) {                  // pods of PDBs with no disruption allowed on the live placement do not move
+    if (ctx->valid.has(PDB_TABLE)) {   // pods of PDBs with no disruption allowed on the live placement do not move
         CU(pdb_allowed(ctx, S.out_node.p));
         CU(pdb_mark(ctx, nullptr));
     }
-    moves_score(ctx, moves_params(ctx, S.state, S.out_node.p, ctx->mv_base));
+    moves_score(ctx, moves_params(ctx, S.state, S.out_node.p, ctx->moves.base));
     if (record) CU(cudaEventRecord(ctx->ev1, st));
     CU(cudaGetLastError());
     return SIMON_OK;
@@ -1905,43 +1939,45 @@ static int moves_launch(simon_ctx *ctx, bool record) {
 
 int simon_moves_upload(simon_ctx *ctx, const simon_move *moves, uint32_t n_moves, uint32_t move_base) {
     if (!ctx || (!moves && n_moves)) return SIMON_ERR_INVALID;
-    if (!ctx->have_pods) return fail(ctx, SIMON_ERR_STATE, "simon_moves_upload before uploads");
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_moves_upload before uploads");
     CU(cudaSetDevice(ctx->device));
+    ctx->valid.drop(MOVE_LIST);
     static_assert(sizeof(simon_move) == sizeof(uint2), "simon_move layout");
-    CU(ctx->d_moves.upload(reinterpret_cast<const uint2 *>(moves), n_moves, ctx->stream));
-    CU(ctx->d_mv_gain.alloc(n_moves)); CU(ctx->d_mv_code.alloc(n_moves)); CU(ctx->d_mv_hist.alloc(SMV_NBINS)); CU(ctx->d_mv_topn.alloc(2));
-    CU(ctx->d_mv_best_pod.alloc(std::max(1u, ctx->n_pods))); CU(ctx->d_mv_best.alloc(1)); CU(ctx->d_mv_nodes.alloc(std::max(1u, ctx->N)));
-    CU(ctx->d_mv_pods.alloc(std::max(1u, ctx->n_pods)));
-    ctx->mv_n = n_moves; ctx->mv_base = move_base; ctx->mv_ran = false;
-    if (!ctx->static_filled && ctx->use_scache && ctx->N && ctx->n_classes) {
+    CU(ctx->moves.d_moves.upload(reinterpret_cast<const uint2 *>(moves), n_moves, ctx->stream));
+    CU(ctx->moves.d_gain.alloc(n_moves)); CU(ctx->moves.d_code.alloc(n_moves)); CU(ctx->moves.d_hist.alloc(SMV_NBINS)); CU(ctx->moves.d_topn.alloc(2));
+    CU(ctx->moves.d_best_pod.alloc(std::max(1u, ctx->pods.n_pods))); CU(ctx->moves.d_best.alloc(1)); CU(ctx->moves.d_nodes.alloc(std::max(1u, ctx->snap.N)));
+    CU(ctx->moves.d_pods.alloc(std::max(1u, ctx->pods.n_pods)));
+    ctx->moves.n = n_moves; ctx->moves.base = move_base;
+    if (!ctx->valid.has(STATIC_FILL) && ctx->pods.use_scache && ctx->snap.N && ctx->pods.n_classes) {
         // once per uploaded pod list: the static verdicts of every (signature, node) pair, densely
         SkParams Pm;
         fill_params(ctx, ctx->single, Pm);
-        simon_static_fill<<<ctx->sms * 8, 256, 0, ctx->stream>>>(Pm, ctx->d_sig_class.p, ctx->n_sigs);
+        simon_static_fill<<<ctx->sms * 8, 256, 0, ctx->stream>>>(Pm, ctx->pods.d_sig_class.p, ctx->pods.n_sigs);
         CU(cudaGetLastError());
         ctx->launches++;
-        ctx->static_filled = true;
+        ctx->valid.set(STATIC_FILL);
     }
     CU(cudaStreamSynchronize(ctx->stream));
+    ctx->valid.set(MOVE_LIST);
     return SIMON_OK;
 }
 
 int simon_moves_run(simon_ctx *ctx, uint32_t k, int32_t *out_gain, uint32_t *out_code, uint64_t *out_best_per_pod,
                     simon_move_rank *out_topk, simon_moves_result *out) {
     if (!ctx || !out) return SIMON_ERR_INVALID;
-    if (!ctx->have_pods || !ctx->d_moves.p) return fail(ctx, SIMON_ERR_STATE, "simon_moves_run before simon_moves_upload");
+    if (!ctx->valid.has(MOVE_LIST)) return fail(ctx, SIMON_ERR_STATE, "simon_moves_run before simon_moves_upload");
     CU(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
-    const uint32_t n = ctx->mv_n;
-    ctx->mv_ran = false;
+    const uint32_t n = ctx->moves.n;
+    ctx->valid.drop(MOVE_RUN);
     int rc = moves_scope_refresh(ctx);
     if (rc) return rc;
     rc = moves_launch(ctx, true);
     if (rc) return rc;
     uint32_t hist[SMV_NBINS];
     unsigned long long best = 0;
-    CU(cudaMemcpyAsync(hist, ctx->d_mv_hist.p, sizeof(hist), cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(&best, ctx->d_mv_best.p, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(hist, ctx->moves.d_hist.p, sizeof(hist), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(&best, ctx->moves.d_best.p, 8, cudaMemcpyDeviceToHost, st));
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "move kernel failed: %s", cudaGetErrorString(e));
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
@@ -1959,11 +1995,11 @@ int simon_moves_run(simon_ctx *ctx, uint32_t k, int32_t *out_gain, uint32_t *out
             if (cum + hist[b] >= kk) { thr = b - 200; n_gt = (uint32_t)cum; need_eq = kk - (uint32_t)cum; break; }
             cum += hist[b];
         }
-        CU(ctx->d_mv_topk.alloc(2ull * kk));
-        simon_moves_collect<<<1, 1024, 0, st>>>(n, ctx->d_mv_gain.p, ctx->d_mv_code.p, thr, need_eq, kk, ctx->mv_base, ctx->d_mv_topk.p, ctx->d_mv_topn.p);
+        CU(ctx->moves.d_topk.alloc(2ull * kk));
+        simon_moves_collect<<<1, 1024, 0, st>>>(n, ctx->moves.d_gain.p, ctx->moves.d_code.p, thr, need_eq, kk, ctx->moves.base, ctx->moves.d_topk.p, ctx->moves.d_topn.p);
         CU(cudaGetLastError());
         std::vector<uint2> tk(2ull * kk);
-        CU(cudaMemcpyAsync(tk.data(), ctx->d_mv_topk.p, 16ull * kk, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(tk.data(), ctx->moves.d_topk.p, 16ull * kk, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
         std::vector<simon_move_rank> r;
         for (uint32_t q = 0; q < n_gt; q++) r.push_back({tk[q].x, (int32_t)tk[q].y});
@@ -1972,41 +2008,41 @@ int simon_moves_run(simon_ctx *ctx, uint32_t k, int32_t *out_gain, uint32_t *out
         for (uint32_t q = 0; q < kk; q++) out_topk[q] = r[q];
         out->n_topk = kk;
     }
-    if (out_gain && n) CU(cudaMemcpyAsync(out_gain, ctx->d_mv_gain.p, 4ull * n, cudaMemcpyDeviceToHost, st));
-    if (out_code && n) CU(cudaMemcpyAsync(out_code, ctx->d_mv_code.p, 4ull * n, cudaMemcpyDeviceToHost, st));
-    if (out_best_per_pod && ctx->n_pods) CU(cudaMemcpyAsync(out_best_per_pod, ctx->d_mv_best_pod.p, 8ull * ctx->n_pods, cudaMemcpyDeviceToHost, st));
+    if (out_gain && n) CU(cudaMemcpyAsync(out_gain, ctx->moves.d_gain.p, 4ull * n, cudaMemcpyDeviceToHost, st));
+    if (out_code && n) CU(cudaMemcpyAsync(out_code, ctx->moves.d_code.p, 4ull * n, cudaMemcpyDeviceToHost, st));
+    if (out_best_per_pod && ctx->pods.n_pods) CU(cudaMemcpyAsync(out_best_per_pod, ctx->moves.d_best_pod.p, 8ull * ctx->pods.n_pods, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    ctx->mv_ran = true;
-    ctx->mv_last_scope = ctx->mv_scope;
+    ctx->valid.set(MOVE_RUN);
+    ctx->move_run.scope = ctx->scope.bits;
     return SIMON_OK;
 }
 
 int simon_moves_set_scope(simon_ctx *ctx, uint32_t scope) {
     if (!ctx) return SIMON_ERR_INVALID;
     if (scope & ~(SIMON_MOVES_SCOPE_GPU_SHARE | SIMON_MOVES_SCOPE_HARD_SPREAD)) return fail(ctx, SIMON_ERR_INVALID, "unknown move scope bits 0x%x", scope);
-    if (scope != ctx->mv_scope) ctx->mv_scope_dirty = true;
-    ctx->mv_scope = scope;
+    if (scope != ctx->scope.bits) ctx->valid.drop(SCOPE_PREP);
+    ctx->scope.bits = scope;
     return SIMON_OK;
 }
 
 int simon_moves_gpu_slots_download(simon_ctx *ctx, uint32_t first, uint32_t count, uint32_t *out_slots) {
     if (!ctx || (!out_slots && count)) return SIMON_ERR_INVALID;
-    if (!ctx->mv_ran || !(ctx->mv_last_scope & SIMON_MOVES_SCOPE_GPU_SHARE))
+    if (!ctx->valid.has(MOVE_RUN) || !(ctx->move_run.scope & SIMON_MOVES_SCOPE_GPU_SHARE))
         return fail(ctx, SIMON_ERR_STATE, "no simon_moves_run with GPU share in its scope since the last simon_moves_upload");
-    if ((uint64_t)first + count > ctx->mv_n) return fail(ctx, SIMON_ERR_INVALID, "range out of bounds");
+    if ((uint64_t)first + count > ctx->moves.n) return fail(ctx, SIMON_ERR_INVALID, "range out of bounds");
     CU(cudaSetDevice(ctx->device));
-    if (count) CU(cudaMemcpy(out_slots, ctx->d_mv_slots.p + first, 4ull * count, cudaMemcpyDeviceToHost));
+    if (count) CU(cudaMemcpy(out_slots, ctx->moves.d_slots.p + first, 4ull * count, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
 int simon_moves_replay(simon_ctx *ctx, uint32_t steps, float *out_ms_total) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->have_pods || !ctx->d_moves.p) return fail(ctx, SIMON_ERR_STATE, "simon_moves_replay before simon_moves_upload");
+    if (!ctx->valid.has(MOVE_LIST)) return fail(ctx, SIMON_ERR_STATE, "simon_moves_replay before simon_moves_upload");
     CU(cudaSetDevice(ctx->device));
     cudaStream_t st = ctx->stream;
     int rc0 = moves_scope_refresh(ctx);
     if (rc0) return rc0;
-    ctx->mv_ran = false;        // the slots of the last simon_moves_run may be overwritten
+    ctx->valid.drop(MOVE_RUN);          // the slots of the last simon_moves_run may be overwritten
     CU(cudaEventRecord(ctx->ev0, st));
     for (uint32_t s = 0; s < steps; s++) {
         int rc = moves_launch(ctx, false);
@@ -2030,53 +2066,52 @@ int simon_moves_plan(simon_ctx *ctx, uint32_t max_moves, int32_t min_gain, simon
     if (max_moves == 0) return fail(ctx, SIMON_ERR_INVALID, "simon_moves_plan: max_moves must be at least 1");
     if (!out_steps) return fail(ctx, SIMON_ERR_INVALID, "simon_moves_plan: out_steps is NULL");
     if (min_gain < 1 || min_gain > 200) return fail(ctx, SIMON_ERR_INVALID, "simon_moves_plan: min_gain %d outside [1, 200]", min_gain);
-    if (!ctx->have_pods || !ctx->d_moves.p) return fail(ctx, SIMON_ERR_STATE, "simon_moves_plan before simon_moves_upload");
-    if (ctx->mv_base != 0) return fail(ctx, SIMON_ERR_INVALID, "simon_moves_plan: the move list was uploaded with move_base %u, not 0", ctx->mv_base);
-    if (!ctx->have_live) return fail(ctx, SIMON_ERR_STATE, "simon_moves_plan: no placement since the last pod upload or reset");
+    if (!ctx->valid.has(MOVE_LIST)) return fail(ctx, SIMON_ERR_STATE, "simon_moves_plan before simon_moves_upload");
+    if (ctx->moves.base != 0) return fail(ctx, SIMON_ERR_INVALID, "simon_moves_plan: the move list was uploaded with move_base %u, not 0", ctx->moves.base);
+    if (!ctx->valid.has(LIVE)) return fail(ctx, SIMON_ERR_STATE, "simon_moves_plan: no placement since the last pod upload or reset");
     CU(cudaSetDevice(ctx->device));
     int rc = moves_scope_refresh(ctx);
     if (rc) return rc;
-    ctx->mv_ran = false;            // the per-move slots are overwritten
-    ctx->pl_valid = false;
+    ctx->valid.drop(MOVE_RUN | PLAN);   // the per-move slots are overwritten
     cudaStream_t st = ctx->stream;
     ScenPool &S = ctx->single;
-    NodeState &pl = ctx->pl_state;
-    const uint32_t N = ctx->N, P = ctx->n_pods, n = ctx->mv_n, scope = ctx->mv_scope;
-    const bool gpu = ctx->mv_scoped && (scope & SIMON_MOVES_SCOPE_GPU_SHARE) && N;
+    NodeState &pl = ctx->plan.state;
+    const uint32_t N = ctx->snap.N, P = ctx->pods.n_pods, n = ctx->moves.n, scope = ctx->scope.bits;
+    const bool gpu = ctx->scope.scoped && (scope & SIMON_MOVES_SCOPE_GPU_SHARE) && N;
     const size_t P1 = std::max(1u, P);
     const uint32_t cap = (uint32_t)std::min<uint64_t>(max_moves, P1);
-    pl.shape(1, N, ctx->K, ctx->cnt_words, ctx->n_counters);
+    pl.shape(1, N, ctx->snap.K, ctx->pods.cnt_words, ctx->pods.n_counters);
     CU(pl.alloc());
-    CU(ctx->pl_place.alloc(P1)); CU(ctx->pl_slots.alloc(P1)); CU(ctx->pl_ctl.alloc(4)); CU(ctx->pl_steps.alloc(cap));
-    if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && n) CU(ctx->d_mv_slots.alloc(n));
-    if (gpu) CU(ctx->d_mv_gpu.alloc(N));
+    CU(ctx->plan.place.alloc(P1)); CU(ctx->plan.slots.alloc(P1)); CU(ctx->plan.ctl.alloc(4)); CU(ctx->plan.steps.alloc(cap));
+    if ((scope & SIMON_MOVES_SCOPE_GPU_SHARE) && n) CU(ctx->moves.d_slots.alloc(n));
+    if (gpu) CU(ctx->moves.d_gpu.alloc(N));
     CU(cudaEventRecord(ctx->ev0, st));
     CU(pl.copy(S.state, st));
-    CU(cudaMemcpyAsync(ctx->pl_place.p, S.out_node.p, 4 * P1, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemcpyAsync(ctx->pl_slots.p, S.out_gpu.p, 4 * P1, cudaMemcpyDeviceToDevice, st));
-    CU(cudaMemsetAsync(ctx->pl_ctl.p, 0, 16, st));
+    CU(cudaMemcpyAsync(ctx->plan.place.p, S.out_node.p, 4 * P1, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemcpyAsync(ctx->plan.slots.p, S.out_gpu.p, 4 * P1, cudaMemcpyDeviceToDevice, st));
+    CU(cudaMemsetAsync(ctx->plan.ctl.p, 0, 16, st));
     // ---- setup: the packed records of the plan state, once ----
-    moves_pack(ctx, pl, ctx->pl_place.p, gpu);
-    simon_moves_plan_setup<<<std::max(1u, std::min(1184u, (P + 255) / 256)), 256, 0, st>>>(P, ctx->pl_slots.p, ctx->d_mv_pods.p, ctx->pl_ctl.p);
+    moves_pack(ctx, pl, ctx->plan.place.p, gpu);
+    simon_moves_plan_setup<<<std::max(1u, std::min(1184u, (P + 255) / 256)), 256, 0, st>>>(P, ctx->plan.slots.p, ctx->moves.d_pods.p, ctx->plan.ctl.p);
     ctx->launches += 2;             // the pack and the setup
     CU(cudaGetLastError());
     // with a PDB table: remaining = allowed on the live placement; the pods of PDBs without budget are marked and counted
-    const uint32_t n_pdbs = ctx->n_pdbs;
-    if (n_pdbs) {
-        CU(cudaMemsetAsync(ctx->d_pdb_ctl.p, 0, 16, st));
-        CU(pdb_allowed(ctx, ctx->pl_place.p));
-        CU(pdb_mark(ctx, ctx->d_pdb_ctl.p + 2));
+    const bool pdbs = ctx->valid.has(PDB_TABLE);
+    if (pdbs) {
+        CU(cudaMemsetAsync(ctx->pdb.d_ctl.p, 0, 16, st));
+        CU(pdb_allowed(ctx, ctx->plan.place.p));
+        CU(pdb_mark(ctx, ctx->pdb.d_ctl.p + 2));
     }
-    const SmvParams M = moves_params(ctx, pl, ctx->pl_place.p, 0);
+    const SmvParams M = moves_params(ctx, pl, ctx->plan.place.p, 0);
     SkParams Pk;
     fill_params(ctx, S, Pk);
     SmvPlan Q;
     memset(&Q, 0, sizeof(Q));
     Q.max_moves = max_moves; Q.min_gain = min_gain;
     pl.slice(0, Q);
-    Q.place = ctx->pl_place.p; Q.slots = ctx->pl_slots.p; Q.moves = ctx->d_moves.p; Q.mv_slots = M.out_slots;
-    Q.best_global = ctx->d_mv_best.p; Q.hist = ctx->d_mv_hist.p; Q.nodes = ctx->d_mv_nodes.p; Q.gpu = gpu ? ctx->d_mv_gpu.p : nullptr;
-    Q.pods = ctx->d_mv_pods.p; Q.steps = ctx->pl_steps.p; Q.ctl = ctx->pl_ctl.p;
+    Q.place = ctx->plan.place.p; Q.slots = ctx->plan.slots.p; Q.moves = ctx->moves.d_moves.p; Q.mv_slots = M.out_slots;
+    Q.best_global = ctx->moves.d_best.p; Q.hist = ctx->moves.d_hist.p; Q.nodes = ctx->moves.d_nodes.p; Q.gpu = gpu ? ctx->moves.d_gpu.p : nullptr;
+    Q.pods = ctx->moves.d_pods.p; Q.steps = ctx->plan.steps.p; Q.ctl = ctx->plan.ctl.p;
     // ---- steps: [hard prep] + scoring + apply, in chunks of growing length ----
     const uint64_t limit = std::min<uint64_t>(max_moves, (uint64_t)P + 1);     // after P steps every pod has moved: the next pass stops
     uint32_t ctl[4] = {0, 0, 0, 0};
@@ -2087,15 +2122,15 @@ int simon_moves_plan(simon_ctx *ctx, uint32_t max_moves, int32_t min_gain, simon
             moves_score(ctx, M);
             simon_moves_plan_apply<<<1, 32, 0, st>>>(Pk, Q);
             ctx->launches++;
-            if (n_pdbs) {               // the step's PDB spending, and the members of PDBs it used up
-                CU(simon_pdb_launch_step(st, ctx->sms * 4u, ctx->pl_ctl.p, ctx->pl_steps.p, ctx->d_pdb_off.p, ctx->d_pdb_ids.p,
-                                         ctx->d_pdb_rem.p, ctx->d_pdb_ctl.p, ctx->d_pdb_hit.p, ctx->pdb_max_members, ctx->d_pdb_moff.p,
-                                         ctx->d_pdb_members.p, ctx->d_mv_pods.p));
+            if (pdbs) {               // the step's PDB spending, and the members of PDBs it used up
+                CU(simon_pdb_launch_step(st, ctx->sms * 4u, ctx->plan.ctl.p, ctx->plan.steps.p, ctx->pdb.d_off.p, ctx->pdb.d_ids.p,
+                                         ctx->pdb.d_rem.p, ctx->pdb.d_ctl.p, ctx->pdb.d_hit.p, ctx->pdb.max_members, ctx->pdb.d_moff.p,
+                                         ctx->pdb.d_members.p, ctx->moves.d_pods.p));
                 ctx->launches += 2;
             }
         }
         CU(cudaGetLastError());
-        CU(cudaMemcpyAsync(ctl, ctx->pl_ctl.p, 16, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(ctl, ctx->plan.ctl.p, 16, cudaMemcpyDeviceToHost, st));
         cudaError_t e = cudaStreamSynchronize(st);
         if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "move plan failed: %s", cudaGetErrorString(e));
     }
@@ -2106,31 +2141,31 @@ int simon_moves_plan(simon_ctx *ctx, uint32_t max_moves, int32_t min_gain, simon
         return fail(ctx, SIMON_ERR_CUDA, "move plan: inconsistent state at step %u (%s)", ctl[0],
                     ctl[2] == SMV_PLAN_ERR_SLOTS ? "Reserve on the target differs from the scored GPU slots" : "a count of the source node went negative");
     if (!ctl[1]) return fail(ctx, SIMON_ERR_CUDA, "move plan: no stop after %llu steps", (unsigned long long)limit);
-    if (ctl[0]) CU(cudaMemcpy(out_steps, ctx->pl_steps.p, sizeof(simon_plan_step) * ctl[0], cudaMemcpyDeviceToHost));
+    if (ctl[0]) CU(cudaMemcpy(out_steps, ctx->plan.steps.p, sizeof(simon_plan_step) * ctl[0], cudaMemcpyDeviceToHost));
     uint32_t pctl[4] = {0, 0, 0, 0};
-    if (n_pdbs) CU(cudaMemcpy(pctl, ctx->d_pdb_ctl.p, 16, cudaMemcpyDeviceToHost));
+    if (pdbs) CU(cudaMemcpy(pctl, ctx->pdb.d_ctl.p, 16, cudaMemcpyDeviceToHost));
     memset(out, 0, sizeof(*out));
     out->n_steps = ctl[0]; out->stop_reason = ctl[1]; out->n_excluded = ctl[3]; out->n_pdb_blocked = pctl[2]; out->kernel_ms = ctx->last_ms;
-    ctx->pl_valid = true;
+    ctx->valid.set(PLAN);
     return SIMON_OK;
 }
 
 int simon_moves_plan_download(simon_ctx *ctx, int32_t *placement, uint32_t *gpu_slots) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->pl_valid) return fail(ctx, SIMON_ERR_STATE, "no simon_moves_plan since the last upload");
+    if (!ctx->valid.has(PLAN)) return fail(ctx, SIMON_ERR_STATE, "no simon_moves_plan since the last upload");
     CU(cudaSetDevice(ctx->device));
-    if (placement && ctx->n_pods) CU(cudaMemcpy(placement, ctx->pl_place.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost));
-    if (gpu_slots && ctx->n_pods) CU(cudaMemcpy(gpu_slots, ctx->pl_slots.p, 4ull * ctx->n_pods, cudaMemcpyDeviceToHost));
+    if (placement && ctx->pods.n_pods) CU(cudaMemcpy(placement, ctx->plan.place.p, 4ull * ctx->pods.n_pods, cudaMemcpyDeviceToHost));
+    if (gpu_slots && ctx->pods.n_pods) CU(cudaMemcpy(gpu_slots, ctx->plan.slots.p, 4ull * ctx->pods.n_pods, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
 int simon_moves_plan_state_download(simon_ctx *ctx, int64_t *req_mcpu, int64_t *req_mem, int64_t *req_eph, int64_t *nz_mcpu,
                                     int64_t *nz_mem, int32_t *num_pods, int64_t *req_scalar, int64_t *gpu_used) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->pl_valid) return fail(ctx, SIMON_ERR_STATE, "no simon_moves_plan since the last upload");
+    if (!ctx->valid.has(PLAN)) return fail(ctx, SIMON_ERR_STATE, "no simon_moves_plan since the last upload");
     CU(cudaSetDevice(ctx->device));
     void *const dst[NodeState::COLS] = {req_mcpu, req_mem, req_eph, nz_mcpu, nz_mem, num_pods, req_scalar, gpu_used};
-    CU(ctx->pl_state.download(dst));
+    CU(ctx->plan.state.download(dst));
     return SIMON_OK;
 }
 
