@@ -1,14 +1,60 @@
-"""ctypes mirror of include/simon_gpu.h (structs + marshalling of a Compiled cluster)."""
+"""The one Python copy of include/simon_gpu.h: its constants (header names without the SIMON_ prefix), ctypes mirrors of its structs,
+the signature of every entry point, and the marshalling of a Compiled cluster.  tests/test_abi.py checks all of it against the
+header."""
 from __future__ import annotations
 
 import ctypes as C
 
 import numpy as np
 
+ABI_VERSION = 3
+
+# ---- limits ----
+MAX_SCALARS = 8
+MAX_GPU_DEV = 8
+MAX_GPU_SLOTS = 64      # alibabacloud.com/gpu-count of a GPU-share pod
+MAX_LABEL_WORDS = 16
+MAX_TAINT_WORDS = 4
+MAX_TOPOS = 8
+MAX_VGS = 8             # Open-Local VGs per node
+MAX_VOLS = 8            # Open-Local LVM PVCs per class
+MAX_DEVS = 16           # Open-Local SSD + HDD devices per node
+MAX_DEV_VOLS = 8        # Open-Local SSD + HDD PVCs per class
 N_FAIL_CODES = 24
+
+NODE_UNSCHEDULABLE = 1
+NODE_HAS_LABELS = 2
+
+# ---- pod class records: word indices (enum simon_class_word), flags, node-selection requirement ops ----
+(SCW_REQ_MCPU, SCW_REQ_MEM, SCW_REQ_EPH, SCW_NZ_MCPU, SCW_NZ_MEM, SCW_SCORE_MCPU, SCW_SCORE_MEM, SCW_GPU_MEM,
+ SCW_GPU_COUNT, SCW_FLAGS, SCW_NODE_NAME, SCW_STATIC_ROW, SCW_EXTRA_ROW, SCW_GUARD_NODE, SCW_STATIC_SIG, SCW_OFF_SCALARS, SCW_OFF_TOL, SCW_OFF_SEL,
+ SCW_OFF_PREF, SCW_N_PREF, SCW_OFF_PORTS, SCW_N_PORTS, SCW_OFF_PTS_HARD, SCW_N_PTS_HARD, SCW_OFF_PTS_SOFT,
+ SCW_N_PTS_SOFT, SCW_OFF_IPA_AFF, SCW_N_IPA_AFF, SCW_OFF_IPA_ANTI, SCW_N_IPA_ANTI, SCW_OFF_IPA_EXIST,
+ SCW_N_IPA_EXIST, SCW_OFF_IPA_SCORE, SCW_N_IPA_SCORE, SCW_OFF_INC, SCW_N_INC, SCW_OFF_ENT, SCW_N_ENT, SCW_ANY_TABLE,
+ SCW_ELIG_SIG, SCW_HDR_WORDS) = range(41)
+CLS_HAS_REQUEST = 1
+CLS_TOL_UNSCHED = 2
+CLS_IPA_SELF_MATCH = 4
+CLS_SIMON_NOREQ = 8
+CLS_PINNED = 16            # node-selection programs refer to the pod's own pin node (REQ_NODE_IS payload -3): DaemonSet pods
+REQ_ANY, REQ_NONE, REQ_NODE_IS, REQ_NODE_ISNOT = 1, 2, 3, 4
+
+# ---- failure histogram columns (enum simon_fail_code); a filter verdict is a bitmask of (1 << code) ----
+SFC_STATIC, SFC_PORTS, SFC_TOO_MANY_PODS, SFC_CPU, SFC_MEM, SFC_EPH, SFC_SCALAR0 = range(7)     # SFC_SCALAR0 + k: scalar resource k
+SFC_PTS_MISSING, SFC_PTS_SKEW, SFC_IPA_AFF, SFC_IPA_ANTI, SFC_IPA_EXIST, SFC_GPU, SFC_LOCAL = range(14, 21)
+
+# simon_ctx_opts.flags
 OPT_RECORD_SCORES = 1
 OPT_NO_PIN_FAST = 2
 OPT_FORCE_LARGE = 4
+
+# move codes other than filter verdicts, and the bias of the per-pod best-move key
+MOVE_NOOP, MOVE_NOT_PLACED, MOVE_NOT_MOVABLE, MOVE_BAD_INDEX = 1 << 24, 1 << 25, 1 << 26, 1 << 27
+MOVE_GAIN_BIAS = 1000
+# simon_moves_set_scope: admit GPU-share classes / classes with DoNotSchedule spread constraints as move candidates
+MOVES_SCOPE_GPU_SHARE, MOVES_SCOPE_HARD_SPREAD = 1, 2
+# simon_moves_plan stop reasons
+PLAN_STOP_NO_MOVE, PLAN_STOP_MAX_MOVES = 1, 2
 
 
 class SimonSnapshot(C.Structure):
@@ -102,19 +148,7 @@ def marshal_devices(st):
     return s, keep
 
 
-MOVE_NOOP, MOVE_NOT_PLACED, MOVE_NOT_MOVABLE, MOVE_BAD_INDEX = 1 << 24, 1 << 25, 1 << 26, 1 << 27
-MOVE_GAIN_BIAS = 1000
-# simon_moves_set_scope: admit GPU-share classes / classes with DoNotSchedule spread constraints as move candidates
-MOVES_SCOPE_GPU_SHARE, MOVES_SCOPE_HARD_SPREAD = 1, 2
-# simon_moves_plan stop reasons
-PLAN_STOP_NO_MOVE, PLAN_STOP_MAX_MOVES = 1, 2
-
-
-class SimonPlanStep(C.Structure):
-    _fields_ = [("move", C.c_uint32), ("pod", C.c_uint32), ("from_", C.c_int32), ("to", C.c_int32), ("gain", C.c_int32),
-                ("gpu_slots", C.c_uint32)]
-
-
+# simon_plan_step, as the structured array Engine.moves_plan passes
 PLAN_STEP_DTYPE = np.dtype([("move", np.uint32), ("pod", np.uint32), ("from", np.int32), ("to", np.int32), ("gain", np.int32),
                             ("gpu_slots", np.uint32)])
 
@@ -174,3 +208,73 @@ def marshal(compiled):
         keep.append(a)
         setattr(pods, k, ptr(a))
     return snap, pods, keep
+
+
+# ---- entry points: name -> (restype, argtypes), in the header's order; structs and arrays are passed as c_void_p ----
+_P, _I, _U32, _I32, _PP = C.c_void_p, C.c_int, C.c_uint32, C.c_int32, C.POINTER(C.c_void_p)
+_PF, _PU64 = C.POINTER(C.c_float), C.POINTER(C.c_uint64)
+SIGNATURES = {
+    "simon_gpu_version": (_I, []),
+    "simon_ctx_create": (_I, [_P, _PP]),
+    "simon_ctx_destroy": (None, [_P]),
+    "simon_last_error": (C.c_char_p, [_P]),
+    "simon_snapshot_upload": (_I, [_P, _P]),
+    "simon_pods_upload": (_I, [_P, _P]),
+    "simon_state_reset": (_I, [_P]),
+    "simon_schedule": (_I, [_P, _U32, _U32, _P, _P, _P, _P, _U32, _P]),
+    "simon_schedule_resume": (_I, [_P, _P, _U32, _P, _P, _P, _P, _U32, _P]),
+    "simon_results_download": (_I, [_P, _U32, _U32, _P, _P]),
+    "simon_replay": (_I, [_P, _U32, _PF]),
+    "simon_stats": (_I, [_P, _P]),
+    "simon_last_kernel_ms": (C.c_float, [_P]),
+    "simon_launch_count": (C.c_uint64, [_P]),
+    "simon_last_launch": (_I, [_P, _P]),
+    "simon_state_download": (_I, [_P] * 7),
+    "simon_scenarios_run": (_I, [_P, _P, _U32, _P, _P]),
+    "simon_gpu_slots_download": (_I, [_P, _U32, _U32, _P]),
+    "simon_state_download_ext": (_I, [_P, _P, _P]),
+    "simon_debug_set_dump_pod": (_I, [_P, _U32]),
+    "simon_debug_dump_read": (_I, [_P, _P, _P]),
+    "simon_moves_upload": (_I, [_P, _P, _U32, _U32]),
+    "simon_moves_run": (_I, [_P, _U32, _P, _P, _P, _P, _P]),
+    "simon_moves_replay": (_I, [_P, _U32, _PF]),
+    "simon_moves_set_scope": (_I, [_P, _U32]),
+    "simon_moves_gpu_slots_download": (_I, [_P, _U32, _U32, _P]),
+    "simon_moves_plan": (_I, [_P, _U32, _I32, _P, _P]),
+    "simon_moves_plan_download": (_I, [_P, _P, _P]),
+    "simon_moves_plan_state_download": (_I, [_P] * 9),
+    "simon_storage_upload": (_I, [_P, _P]),
+    "simon_storage_state_download": (_I, [_P, _P]),
+    "simon_devices_upload": (_I, [_P, _P]),
+    "simon_devices_state_download": (_I, [_P, _P]),
+    "simon_scenarios_run_local": (_I, [_P, _P, _U32, _P, _P, _P]),
+    "simon_scenarios_storage_download": (_I, [_P, _U32, _P, _P]),
+    "simon_drain_run": (_I, [_P, _P, _P, _U32, _P]),
+    "simon_drain_download": (_I, [_P, _U32] + [_P] * 7),
+    "simon_drain_pdb_download": (_I, [_P, _U32, _P, _P]),
+    "simon_drain_times": (_I, [_P, _PF, _PF]),
+    "simon_drain_budget": (_I, [_P, _PU64, _PU64]),
+    "simon_pdbs_upload": (_I, [_P, _P]),
+    "simon_pdbs_allowed": (_I, [_P, _P]),
+    "simon_host_go118_sort": (_I, [_P, _U32, _P]),
+    "simon_host_last_error": (C.c_char_p, []),
+    "simon_host_compile": (_I, [C.c_char_p, C.c_uint64, _PP]),
+    "simon_host_plan_free": (None, [_P]),
+    "simon_host_plan_columns": (_I, [_P, _P, _P]),
+    "simon_host_plan_describe": (C.c_char_p, [_P]),
+    "simon_host_simulate": (_I, [C.c_char_p, C.c_uint64, _P, _PP, _PU64]),
+    "simon_host_free": (None, [_P]),
+    "simon_host_capacity_search": (_I, [C.c_char_p, C.c_uint64, _P, _PP, _PU64]),
+    "simon_host_plan_fit_error": (_I, [_P, _U32, _P, _PP]),
+    "simon_host_quantity_probe": (_I, [C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_double)]),
+}
+
+
+def bind(L: C.CDLL, partial: bool = False) -> C.CDLL:
+    """Give each entry point of SIGNATURES its restype and argtypes on the loaded library L.  partial: skip the ones L does not export
+    (an experiment library, or a build of the host side alone); the shipped library exports every one."""
+    for name, (restype, argtypes) in SIGNATURES.items():
+        f = getattr(L, name, None) if partial else getattr(L, name)
+        if f is not None:
+            f.restype, f.argtypes = restype, argtypes
+    return L

@@ -30,6 +30,15 @@ from typing import Dict, List, Optional, Tuple
 import numpy as np
 
 from . import objects as O
+# the format constants of include/simon_gpu.h
+from .abi import (CLS_HAS_REQUEST, CLS_IPA_SELF_MATCH, CLS_PINNED, CLS_SIMON_NOREQ, CLS_TOL_UNSCHED, MAX_GPU_DEV, MAX_GPU_SLOTS,  # noqa: F401
+                  MAX_LABEL_WORDS, MAX_SCALARS, MAX_TAINT_WORDS, MAX_TOPOS, NODE_HAS_LABELS, NODE_UNSCHEDULABLE, REQ_ANY, REQ_NODE_IS,
+                  REQ_NODE_ISNOT, REQ_NONE, SCW_ANY_TABLE, SCW_ELIG_SIG, SCW_EXTRA_ROW, SCW_FLAGS, SCW_GPU_COUNT, SCW_GPU_MEM,
+                  SCW_GUARD_NODE, SCW_HDR_WORDS, SCW_N_ENT, SCW_N_INC, SCW_N_IPA_AFF, SCW_N_IPA_ANTI, SCW_N_IPA_EXIST, SCW_N_IPA_SCORE,
+                  SCW_N_PORTS, SCW_N_PREF, SCW_N_PTS_HARD, SCW_N_PTS_SOFT, SCW_NODE_NAME, SCW_NZ_MCPU, SCW_NZ_MEM, SCW_OFF_ENT,
+                  SCW_OFF_INC, SCW_OFF_IPA_AFF, SCW_OFF_IPA_ANTI, SCW_OFF_IPA_EXIST, SCW_OFF_IPA_SCORE, SCW_OFF_PORTS, SCW_OFF_PREF,
+                  SCW_OFF_PTS_HARD, SCW_OFF_PTS_SOFT, SCW_OFF_SCALARS, SCW_OFF_SEL, SCW_OFF_TOL, SCW_REQ_EPH, SCW_REQ_MCPU,
+                  SCW_REQ_MEM, SCW_SCORE_MCPU, SCW_SCORE_MEM, SCW_STATIC_ROW, SCW_STATIC_SIG)
 from .gomath import log_table
 from .objects import Obj
 from .quantity import Quantity
@@ -37,28 +46,6 @@ from .selectors import (SelectorError, _parse_int64, is_empty_node_selector_term
                         node_selector_term_requirements, requirements_match, toleration_tolerates_taint)
 from .workloads import PodRec, PodTemplate
 
-# ---- format constants: keep in sync with include/simon_gpu.h ----
-MAX_SCALARS = 8
-MAX_GPU_DEV = 8
-MAX_GPU_SLOTS = 64      # alibabacloud.com/gpu-count of a GPU-share pod
-MAX_LABEL_WORDS = 16
-MAX_TAINT_WORDS = 4
-MAX_TOPOS = 8
-N_FAIL_CODES = 24
-NODE_UNSCHEDULABLE = 1
-NODE_HAS_LABELS = 2
-(SCW_REQ_MCPU, SCW_REQ_MEM, SCW_REQ_EPH, SCW_NZ_MCPU, SCW_NZ_MEM, SCW_SCORE_MCPU, SCW_SCORE_MEM, SCW_GPU_MEM,
- SCW_GPU_COUNT, SCW_FLAGS, SCW_NODE_NAME, SCW_STATIC_ROW, SCW_EXTRA_ROW, SCW_GUARD_NODE, SCW_STATIC_SIG, SCW_OFF_SCALARS, SCW_OFF_TOL, SCW_OFF_SEL,
- SCW_OFF_PREF, SCW_N_PREF, SCW_OFF_PORTS, SCW_N_PORTS, SCW_OFF_PTS_HARD, SCW_N_PTS_HARD, SCW_OFF_PTS_SOFT,
- SCW_N_PTS_SOFT, SCW_OFF_IPA_AFF, SCW_N_IPA_AFF, SCW_OFF_IPA_ANTI, SCW_N_IPA_ANTI, SCW_OFF_IPA_EXIST,
- SCW_N_IPA_EXIST, SCW_OFF_IPA_SCORE, SCW_N_IPA_SCORE, SCW_OFF_INC, SCW_N_INC, SCW_OFF_ENT, SCW_N_ENT, SCW_ANY_TABLE,
- SCW_ELIG_SIG, SCW_HDR_WORDS) = range(41)
-CLS_HAS_REQUEST = 1
-CLS_TOL_UNSCHED = 2
-CLS_IPA_SELF_MATCH = 4
-CLS_SIMON_NOREQ = 8
-CLS_PINNED = 16            # node-selection programs refer to the pod's own pin node (REQ_NODE_IS payload -3): DaemonSet pods
-REQ_ANY, REQ_NONE, REQ_NODE_IS, REQ_NODE_ISNOT = 1, 2, 3, 4
 EK_PORT, EK_HARD, EK_SOFT, EK_AFF, EK_ANTI, EK_EXIST, EK_SCORE = range(7)
 SK_MAXW = 6      # domain-bitmask words the engine reduces per decision (csrc/simon_kernel.cuh)
 

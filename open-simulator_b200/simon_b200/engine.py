@@ -17,18 +17,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SIMON_GPU_LIB") or os.path.join(_HERE, "libsimon_gpu.so")    # the override is for kernel experiments
 _LIB = None
 
-EXPORTS = ["simon_gpu_version", "simon_ctx_create", "simon_ctx_destroy", "simon_last_error", "simon_snapshot_upload",
-           "simon_pods_upload", "simon_state_reset", "simon_schedule", "simon_results_download", "simon_last_kernel_ms",
-           "simon_launch_count", "simon_state_download", "simon_scenarios_run", "simon_replay", "simon_stats",
-           "simon_gpu_slots_download", "simon_state_download_ext", "simon_debug_set_dump_pod", "simon_debug_dump_read",
-           "simon_moves_upload", "simon_moves_run", "simon_moves_replay", "simon_host_go118_sort",
-           "simon_host_last_error", "simon_host_compile", "simon_host_plan_free", "simon_host_plan_columns", "simon_host_plan_describe",
-           "simon_host_simulate", "simon_host_free", "simon_host_quantity_probe", "simon_host_plan_fit_error", "simon_host_capacity_search",
-           "simon_storage_upload", "simon_storage_state_download", "simon_devices_upload", "simon_devices_state_download",
-           "simon_scenarios_run_local", "simon_scenarios_storage_download", "simon_moves_set_scope", "simon_moves_gpu_slots_download",
-           "simon_schedule_resume", "simon_last_launch", "simon_drain_run", "simon_drain_download", "simon_drain_times",
-           "simon_drain_budget", "simon_moves_plan", "simon_moves_plan_download", "simon_moves_plan_state_download",
-           "simon_pdbs_upload", "simon_pdbs_allowed", "simon_drain_pdb_download"]
+EXPORTS = list(abi.SIGNATURES)       # every entry point of include/simon_gpu.h
 
 
 class EngineUnavailable(RuntimeError):
@@ -41,99 +30,9 @@ def lib():
         return _LIB
     if not os.path.exists(LIB_PATH):
         raise EngineUnavailable(f"{LIB_PATH} not built: run __graft_entry__.build() (nvcc, sm_90a)")
-    L = C.CDLL(LIB_PATH)
-    L.simon_gpu_version.restype = C.c_int
-    L.simon_ctx_create.restype = C.c_int
-    L.simon_ctx_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-    L.simon_ctx_destroy.argtypes = [C.c_void_p]
-    L.simon_last_error.restype = C.c_char_p
-    L.simon_last_error.argtypes = [C.c_void_p]
-    L.simon_snapshot_upload.restype = C.c_int
-    L.simon_snapshot_upload.argtypes = [C.c_void_p, C.c_void_p]
-    L.simon_pods_upload.restype = C.c_int
-    L.simon_pods_upload.argtypes = [C.c_void_p, C.c_void_p]
-    L.simon_state_reset.restype = C.c_int
-    L.simon_state_reset.argtypes = [C.c_void_p]
-    L.simon_schedule.restype = C.c_int
-    L.simon_schedule.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                 C.c_uint32, C.c_void_p]
-    L.simon_results_download.restype = C.c_int
-    L.simon_results_download.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]
-    L.simon_replay.restype = C.c_int
-    L.simon_replay.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_float)]
-    L.simon_stats.restype = C.c_int
-    L.simon_stats.argtypes = [C.c_void_p, C.c_void_p]
-    L.simon_last_kernel_ms.restype = C.c_float
-    L.simon_last_kernel_ms.argtypes = [C.c_void_p]
-    L.simon_launch_count.restype = C.c_uint64
-    L.simon_launch_count.argtypes = [C.c_void_p]
-    L.simon_state_download.restype = C.c_int
-    L.simon_state_download.argtypes = [C.c_void_p] + [C.c_void_p] * 6
-    L.simon_scenarios_run.restype = C.c_int
-    L.simon_scenarios_run.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
-    try:
-        L.simon_gpu_slots_download.restype = C.c_int
-        L.simon_gpu_slots_download.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
-        L.simon_state_download_ext.restype = C.c_int
-        L.simon_state_download_ext.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.simon_debug_set_dump_pod.restype = C.c_int
-        L.simon_debug_set_dump_pod.argtypes = [C.c_void_p, C.c_uint32]
-        L.simon_debug_dump_read.restype = C.c_int
-        L.simon_debug_dump_read.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.simon_moves_upload.restype = C.c_int
-        L.simon_moves_upload.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32]
-        L.simon_moves_run.restype = C.c_int
-        L.simon_moves_run.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.simon_moves_replay.restype = C.c_int
-        L.simon_moves_replay.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_float)]
-        L.simon_host_go118_sort.restype = C.c_int
-        L.simon_host_go118_sort.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
-        L.simon_storage_upload.restype = C.c_int
-        L.simon_storage_upload.argtypes = [C.c_void_p, C.c_void_p]
-        L.simon_storage_state_download.restype = C.c_int
-        L.simon_storage_state_download.argtypes = [C.c_void_p, C.c_void_p]
-        L.simon_devices_upload.restype = C.c_int
-        L.simon_devices_upload.argtypes = [C.c_void_p, C.c_void_p]
-        L.simon_devices_state_download.restype = C.c_int
-        L.simon_devices_state_download.argtypes = [C.c_void_p, C.c_void_p]
-        L.simon_scenarios_run_local.restype = C.c_int
-        L.simon_scenarios_run_local.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.simon_scenarios_storage_download.restype = C.c_int
-        L.simon_scenarios_storage_download.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
-        L.simon_moves_set_scope.restype = C.c_int
-        L.simon_moves_set_scope.argtypes = [C.c_void_p, C.c_uint32]
-        L.simon_moves_gpu_slots_download.restype = C.c_int
-        L.simon_moves_gpu_slots_download.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
-        L.simon_schedule_resume.restype = C.c_int
-        L.simon_schedule_resume.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                            C.c_uint32, C.c_void_p]
-        L.simon_last_launch.restype = C.c_int
-        L.simon_last_launch.argtypes = [C.c_void_p, C.c_void_p]
-        L.simon_drain_run.restype = C.c_int
-        L.simon_drain_run.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
-        L.simon_drain_download.restype = C.c_int
-        L.simon_drain_download.argtypes = [C.c_void_p, C.c_uint32] + [C.c_void_p] * 7
-        L.simon_drain_times.restype = C.c_int
-        L.simon_drain_times.argtypes = [C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_float)]
-        L.simon_drain_budget.restype = C.c_int
-        L.simon_drain_budget.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
-        L.simon_moves_plan.restype = C.c_int
-        L.simon_moves_plan.argtypes = [C.c_void_p, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p]
-        L.simon_moves_plan_download.restype = C.c_int
-        L.simon_moves_plan_download.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.simon_moves_plan_state_download.restype = C.c_int
-        L.simon_moves_plan_state_download.argtypes = [C.c_void_p] + [C.c_void_p] * 8
-        L.simon_pdbs_upload.restype = C.c_int
-        L.simon_pdbs_upload.argtypes = [C.c_void_p, C.c_void_p]
-        L.simon_pdbs_allowed.restype = C.c_int
-        L.simon_pdbs_allowed.argtypes = [C.c_void_p, C.c_void_p]
-        L.simon_drain_pdb_download.restype = C.c_int
-        L.simon_drain_pdb_download.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
-    except AttributeError:
-        if not os.environ.get("SIMON_GPU_LIB"):       # an experiment library may lack the newer entry points; the shipped one may not
-            raise
-    _LIB = L
-    return L
+    # an experiment library may lack the newer entry points; the shipped one may not
+    _LIB = abi.bind(C.CDLL(LIB_PATH), partial=bool(os.environ.get("SIMON_GPU_LIB")))
+    return _LIB
 
 
 class Engine:

@@ -30,25 +30,11 @@ def lib():
         return _LIB
     path = os.environ.get("SIMON_HOST_LIB")
     if path:
-        L = C.CDLL(path)
+        _LIB = abi.bind(C.CDLL(path), partial=True)
     else:
         from .engine import lib as _engine_lib
-        L = _engine_lib()
-    L.simon_host_last_error.restype = C.c_char_p
-    L.simon_host_compile.restype = C.c_int
-    L.simon_host_compile.argtypes = [C.c_char_p, C.c_uint64, C.POINTER(C.c_void_p)]
-    L.simon_host_plan_free.argtypes = [C.c_void_p]
-    L.simon_host_plan_columns.restype = C.c_int
-    L.simon_host_plan_columns.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-    L.simon_host_plan_describe.restype = C.c_char_p
-    L.simon_host_plan_describe.argtypes = [C.c_void_p]
-    L.simon_host_simulate.restype = C.c_int
-    L.simon_host_simulate.argtypes = [C.c_char_p, C.c_uint64, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
-    L.simon_host_free.argtypes = [C.c_void_p]
-    L.simon_host_capacity_search.restype = C.c_int
-    L.simon_host_capacity_search.argtypes = [C.c_char_p, C.c_uint64, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
-    _LIB = L
-    return L
+        _LIB = _engine_lib()
+    return _LIB
 
 
 class NativeHostError(RuntimeError):

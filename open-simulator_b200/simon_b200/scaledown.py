@@ -22,6 +22,7 @@ from typing import Callable, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
+from . import abi
 from .capacity import env_caps, occupancy_ok
 from .compiler import SCW_GUARD_NODE, SCW_REQ_MCPU, SCW_REQ_MEM, Compiled, get_zone_key
 from .objects import AppResource, ResourceTypes
@@ -222,7 +223,7 @@ def drain_results(compiled: Compiled, placed: np.ndarray, removed_lists: Sequenc
             res.EvictedPods.append(EvictedPod(recs[q], names[placed[q]], names[g] if g >= 0 else None, gpu_index(w) if g >= 0 else None))
             if g < 0:
                 j = fails.get(q)
-                counts = r["fail_counts"][j] if j is not None else np.zeros(24, np.uint32)
+                counts = r["fail_counts"][j] if j is not None else np.zeros(abi.N_FAIL_CODES, np.uint32)
                 res.UnscheduledPods.append(UnscheduledPod(recs[q], format_fit_error(compiled, recs[q], counts, active=active, static_memo=memo)))
         for q in r["blocked"].tolist():
             res.BlockedPods.append(BlockedPod(recs[q], names[placed[q]], BLOCK_NODE_NAME if fixed[q] >= 0 else BLOCK_LOCAL_STORAGE))

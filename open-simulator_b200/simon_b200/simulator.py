@@ -24,7 +24,7 @@ from typing import Callable, List, Optional, Tuple
 
 import numpy as np
 
-from . import objects as O
+from . import abi, objects as O
 from .algo import order_app_pods
 from .compiler import ClusterContext, Compiled, compile_cluster
 from .objects import AppResource, Obj, ResourceTypes
@@ -145,13 +145,14 @@ def _plan(cluster: ResourceTypes, apps: List[AppResource]) -> Plan:
 
 # Failure reason strings of the in-tree plugins (status.Reasons() histogram: generic_scheduler.go:72-90)
 _DYNAMIC_REASONS = {
-    1: ["node(s) didn't have free ports for the requested pod ports"],
-    2: ["Too many pods"], 3: ["Insufficient cpu"], 4: ["Insufficient memory"], 5: ["Insufficient ephemeral-storage"],
-    14: ["node(s) didn't match pod topology spread constraints (missing required label)"],
-    15: ["node(s) didn't match pod topology spread constraints"],
-    16: ["node(s) didn't match pod affinity/anti-affinity", "node(s) didn't match pod affinity rules"],
-    17: ["node(s) didn't match pod affinity/anti-affinity", "node(s) didn't match pod anti-affinity rules"],
-    18: ["node(s) didn't match pod affinity/anti-affinity", "node(s) didn't satisfy existing pods anti-affinity rules"],
+    abi.SFC_PORTS: ["node(s) didn't have free ports for the requested pod ports"],
+    abi.SFC_TOO_MANY_PODS: ["Too many pods"], abi.SFC_CPU: ["Insufficient cpu"], abi.SFC_MEM: ["Insufficient memory"],
+    abi.SFC_EPH: ["Insufficient ephemeral-storage"],
+    abi.SFC_PTS_MISSING: ["node(s) didn't match pod topology spread constraints (missing required label)"],
+    abi.SFC_PTS_SKEW: ["node(s) didn't match pod topology spread constraints"],
+    abi.SFC_IPA_AFF: ["node(s) didn't match pod affinity/anti-affinity", "node(s) didn't match pod affinity rules"],
+    abi.SFC_IPA_ANTI: ["node(s) didn't match pod affinity/anti-affinity", "node(s) didn't match pod anti-affinity rules"],
+    abi.SFC_IPA_EXIST: ["node(s) didn't match pod affinity/anti-affinity", "node(s) didn't satisfy existing pods anti-affinity rules"],
 }
 
 
@@ -205,22 +206,24 @@ def format_fit_error(compiled: Compiled, rec: PodRec, counts: np.ndarray, active
             for s in strs:
                 reasons[s] = reasons.get(s, 0) + c
     for k, nm in enumerate(compiled.scalar_names):
-        c = int(counts[6 + k])
+        c = int(counts[abi.SFC_SCALAR0 + k])
         if c:
             reasons["Insufficient " + nm] = reasons.get("Insufficient " + nm, 0) + c
-    if int(counts[19]):
-        if gpu_nodes is not None and len(gpu_nodes) == int(counts[19]):
+    n_gpu = int(counts[abi.SFC_GPU])
+    n_local = int(counts[abi.SFC_LOCAL]) if len(counts) > abi.SFC_LOCAL else 0
+    if n_gpu:
+        if gpu_nodes is not None and len(gpu_nodes) == n_gpu:
             for nm in gpu_nodes:
                 reasons["Node:" + nm] = reasons.get("Node:" + nm, 0) + 1
         else:       # node list not collected (more failing GPU pods than the re-evaluation budget): counts only
-            reasons["Node:<%d nodes rejected by Open-Gpu-Share>" % int(counts[19])] = int(counts[19])
-    if len(counts) > 20 and int(counts[20]):
-        if local_reasons is not None and len(local_reasons) == int(counts[20]):
+            reasons["Node:<%d nodes rejected by Open-Gpu-Share>" % n_gpu] = n_gpu
+    if n_local:
+        if local_reasons is not None and len(local_reasons) == n_local:
             for r in local_reasons:
                 if r:
                     reasons[r] = reasons.get(r, 0) + 1
         else:       # per-node texts not collected: counts only
-            reasons["<%d nodes rejected by Open-Local>" % int(counts[20])] = int(counts[20])
+            reasons["<%d nodes rejected by Open-Local>" % n_local] = n_local
     total = len(idxs)
     parts = sorted(f"{v} {k}" for k, v in reasons.items())
     msg = f"0/{total} nodes are available: {', '.join(parts)}."
@@ -245,7 +248,7 @@ def build_result(compiled: Compiled, p: Plan, out_node: np.ndarray, fail_counts,
             lists[n].append(rec)
         elif n == -1 and i >= first_listed:
             j = fail_idx.get(i)
-            counts = fail_counts[j] if j is not None and j < len(fail_counts) else np.zeros(24, np.uint32)
+            counts = fail_counts[j] if j is not None and j < len(fail_counts) else np.zeros(abi.N_FAIL_CODES, np.uint32)
             res.UnscheduledPods.append(UnscheduledPod(rec, format_fit_error(compiled, rec, counts, gpu_nodes=(gpu_fail_nodes or {}).get(i),
                                                                               static_memo=static_memo,
                                                                               local_reasons=(local_fail_reasons or {}).get(i))))
@@ -308,8 +311,8 @@ def _simulate(cluster: ResourceTypes, apps: List[AppResource], *opts: Option) ->
         t0 = time.perf_counter()
         # Open-Gpu-Share's failure reason names the node, so the histogram needs the node LIST of such pods, not a count:
         # re-evaluate those pods with the per-node verdict dump (a bounded number of them - each costs a partial re-run)
-        gpu_bit = 1 << 19
-        todo = [int(pod) for j, pod in enumerate(fail_pod) if j < len(fail_counts) and int(fail_counts[j][19]) > 0][:MAX_GPU_FAIL_DETAIL]
+        gpu_bit = 1 << abi.SFC_GPU
+        todo = [int(pod) for j, pod in enumerate(fail_pod) if j < len(fail_counts) and int(fail_counts[j][abi.SFC_GPU]) > 0][:MAX_GPU_FAIL_DETAIL]
         for pod in todo:
             _o, _t, code = eng.dump_pod(pod)
             gpu_fail_nodes[pod] = [compiled.node_names[g] for g in np.nonzero(code & gpu_bit)[0]]
@@ -341,7 +344,7 @@ def _bound_by_scheduler(compiled: Compiled, out_node: np.ndarray):
 def _local_fail_reasons(eng, compiled: Compiled, out_node: np.ndarray, fail_counts, fail_pod, limit: int = MAX_GPU_FAIL_DETAIL) -> dict:
     from .storage import StorageReplay
     pod_class = compiled.pods["pod_class"]
-    todo = sorted(int(pod) for j, pod in enumerate(fail_pod) if j < len(fail_counts) and int(fail_counts[j][20]) > 0)[:limit]
+    todo = sorted(int(pod) for j, pod in enumerate(fail_pod) if j < len(fail_counts) and int(fail_counts[j][abi.SFC_LOCAL]) > 0)[:limit]
     if not todo:
         return {}
     codes = {pod: eng.dump_pod(pod)[2] for pod in todo}
@@ -354,7 +357,7 @@ def _local_fail_reasons(eng, compiled: Compiled, out_node: np.ndarray, fail_coun
             rep.bind(int(pod_class[nxt[0]]), nxt[1])
             nxt = next(bound, None)
         cls = int(pod_class[pod])
-        out[pod] = [rep.reason(cls, g) for g in np.nonzero(codes[pod] & (1 << 20))[0].tolist()]
+        out[pod] = [rep.reason(cls, g) for g in np.nonzero(codes[pod] & (1 << abi.SFC_LOCAL))[0].tolist()]
     return out
 
 
@@ -519,14 +522,14 @@ class Simulator:
         # the failure details of this call's pods, as Simulate collects them; each per-node verdict dump rebuilds the state before
         # the pod from this call's placements instead of placing the pods before it again
         resumed = _ResumedDump(eng, out_node)
-        gpu_bit = 1 << 19
+        gpu_bit = 1 << abi.SFC_GPU
         gpu_fail_nodes = {}
-        gpu_failed = [int(pod) for j, pod in enumerate(fail_pod) if j < len(fail_counts) and int(fail_counts[j][19]) > 0]
+        gpu_failed = [int(pod) for j, pod in enumerate(fail_pod) if j < len(fail_counts) and int(fail_counts[j][abi.SFC_GPU]) > 0]
         for pod in gpu_failed[:max(0, MAX_GPU_FAIL_DETAIL - self._gpu_failed)]:
             code = resumed.dump_pod(pod)[2]
             gpu_fail_nodes[pod] = [compiled.node_names[g] for g in np.nonzero(code & gpu_bit)[0]]
         local_fail_reasons = {}
-        local_failed = sum(1 for j in range(min(len(fail_pod), len(fail_counts))) if int(fail_counts[j][20]) > 0)
+        local_failed = sum(1 for j in range(min(len(fail_pod), len(fail_counts))) if int(fail_counts[j][abi.SFC_LOCAL]) > 0)
         if compiled.storage is not None:
             local_fail_reasons = _local_fail_reasons(resumed, compiled, out_node, fail_counts, fail_pod,
                                                      limit=max(0, MAX_GPU_FAIL_DETAIL - self._local_failed))

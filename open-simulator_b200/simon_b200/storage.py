@@ -25,12 +25,9 @@ from typing import Dict, List, Optional, Tuple
 import numpy as np
 
 from . import objects as O
+from .abi import MAX_DEV_VOLS, MAX_DEVS, MAX_VGS, MAX_VOLS
 
 LVM_SC = ("open-local-lvm", "yoda-lvm-default")      # pkg/utils/utils.go:603 (OpenLocalSCNameLVM, YodaSCNameLVM)
-MAX_VGS = 8           # include/simon_gpu.h SIMON_MAX_VGS
-MAX_VOLS = 8          # SIMON_MAX_VOLS
-MAX_DEVS = 16         # SIMON_MAX_DEVS: SSD + HDD devices per node
-MAX_DEV_VOLS = 8      # SIMON_MAX_DEV_VOLS: SSD + HDD PVCs per class
 MEDIA = ("ssd", "hdd")     # OL/types.go:72-73, in the order ProcessDevicePVC takes them
 INT64_MIN = -(1 << 63)
 

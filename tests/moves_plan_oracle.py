@@ -3,37 +3,16 @@ oracle.binding.Oracle: plan(o, moves, placement, slots, max_moves, min_gain, sco
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-from moves_scope_oracle import CFLAGS
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(_HERE)
-_LIB = None
-
-
-def build() -> str:
-    so = os.path.join(ROOT, "build", "libmoves_plan_oracle.so")
-    srcs = [os.path.join(_HERE, "moves_plan_oracle.c"), os.path.join(_HERE, "moves_scope_oracle.c"),
-            os.path.join(ROOT, "oracle", "simon_oracle.c"), os.path.join(ROOT, "include", "simon_gpu.h")]
-    if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(s) for s in srcs):
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-o", so, srcs[0], "-lm"])
-    return so
+from checkers import load_checker
 
 
 def lib():
-    global _LIB
-    if _LIB is None:
-        L = C.CDLL(build())
-        L.simon_oracle_moves_plan.restype = C.c_int
-        L.simon_oracle_moves_plan.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32] + [C.c_void_p] * 4 + [C.c_uint32, C.c_int32] + \
-            [C.c_void_p] * 4
-        _LIB = L
-    return _LIB
+    return load_checker("moves_plan_oracle", {
+        "simon_oracle_moves_plan": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32] + [C.c_void_p] * 4 + [C.c_uint32, C.c_int32] +
+                                    [C.c_void_p] * 4)})
 
 
 STEP_FIELDS = ("move", "pod", "from", "to", "gain", "gpu_slots")

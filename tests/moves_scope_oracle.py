@@ -3,36 +3,16 @@ oracle.binding.Oracle: moves_score(o, moves, placement, scope) and gpu_used(o)."
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(_HERE)
-_LIB = None
-CFLAGS = ["-O2", "-fPIC", "-shared", "-std=c11", "-D_GNU_SOURCE", "-pthread", "-Wall", "-Wextra", "-ffp-contract=off", "-fno-fast-math"]
-
-
-def build() -> str:
-    so = os.path.join(ROOT, "build", "libmoves_scope_oracle.so")
-    srcs = [os.path.join(_HERE, "moves_scope_oracle.c"), os.path.join(ROOT, "oracle", "simon_oracle.c"),
-            os.path.join(ROOT, "include", "simon_gpu.h")]
-    if not os.path.exists(so) or os.path.getmtime(so) < max(os.path.getmtime(s) for s in srcs):
-        os.makedirs(os.path.dirname(so), exist_ok=True)
-        subprocess.check_call([os.environ.get("CC", "gcc")] + CFLAGS + ["-o", so, srcs[0], "-lm"])
-    return so
+from checkers import load_checker
 
 
 def lib():
-    global _LIB
-    if _LIB is None:
-        L = C.CDLL(build())
-        L.simon_oracle_moves_score_scoped.restype = C.c_int
-        L.simon_oracle_moves_score_scoped.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32] + [C.c_void_p] * 6
-        L.simon_oracle_gpu_used.argtypes = [C.c_void_p, C.c_void_p]
-        _LIB = L
-    return _LIB
+    return load_checker("moves_scope_oracle", {
+        "simon_oracle_moves_score_scoped": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint32] + [C.c_void_p] * 6),
+        "simon_oracle_gpu_used": (None, [C.c_void_p, C.c_void_p])})
 
 
 def moves_score(o, moves, placement, scope: int = 0, class_local=None):

@@ -19,11 +19,11 @@ import numpy as np
 import pytest
 
 from simon_b200 import native_host, objects as O, simulator, synth
+from simon_b200.abi import SFC_SCALAR0
 from simon_b200.compiler import (CompileError, SCW_N_ENT, SCW_N_INC, SCW_N_IPA_AFF, SCW_N_IPA_ANTI, SCW_N_IPA_EXIST,
                                  SCW_N_IPA_SCORE, SCW_N_PORTS, SCW_N_PTS_HARD, SCW_N_PTS_SOFT, compile_cluster)
 from util import run_oracle, run_pyref
 
-SFC_SCALAR0, SFC_GPU = 6, 19        # include/simon_gpu.h simon_fail_code
 R = "requiredDuringSchedulingIgnoredDuringExecution"
 P = "preferredDuringSchedulingIgnoredDuringExecution"
 
@@ -411,8 +411,6 @@ def test_native_fit_error_equals_python_at_the_limit(name):
     cluster, apps = BUILDERS[name]()
     p, c = compiled(cluster, apps)
     L = native_host.lib()
-    L.simon_host_plan_fit_error.restype = C.c_int
-    L.simon_host_plan_fit_error.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_void_p)]
     req = native_host.request_json(cluster, apps)
     h = C.c_void_p()
     assert L.simon_host_compile(req, len(req), C.byref(h)) == 0

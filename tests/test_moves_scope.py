@@ -5,11 +5,11 @@ import numpy as np
 import pytest
 
 import moves_scope_oracle as MS
+from simon_b200.abi import SFC_GPU, SFC_PTS_MISSING, SFC_PTS_SKEW, SFC_STATIC
 from util import make_case
 
 GI = 1 << 30
 GPU, HARD = 1, 2
-SFC_STATIC, SFC_PTS_MISSING, SFC_PTS_SKEW, SFC_GPU = 0, 14, 15, 19     # include/simon_gpu.h simon_fail_code
 # the four clusters of test_moves.py's GPU parity test
 CASES = [
     ("mix", dict(seed_no=103, n_nodes=95, n_workloads=40, max_replicas=7), 30000),

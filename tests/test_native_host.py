@@ -21,7 +21,7 @@ import pytest
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.join(HERE, "golden"))
 
-from simon_b200 import native_host, simulator, synth  # noqa: E402
+from simon_b200 import abi, native_host, simulator, synth  # noqa: E402
 from simon_b200.compiler import compile_cluster  # noqa: E402
 from simon_b200.objects import AppResource, ResourceTypes  # noqa: E402
 
@@ -92,8 +92,6 @@ def test_native_quantity_matches_the_python_restatement(text):
     from simon_b200.quantity import Quantity
     q = Quantity.parse(text)
     L = native_host.lib()
-    L.simon_host_quantity_probe.restype = C.c_int
-    L.simon_host_quantity_probe.argtypes = [C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_double)]
     v, m, a = C.c_int64(0), C.c_int64(0), C.c_double(0)
     want_v, want_m = q.int_value(), q.milli_value()
     assert L.simon_host_quantity_probe(text.encode(), None, None, C.byref(a)) == 0, L.simon_host_last_error()
@@ -112,8 +110,6 @@ def test_native_quantity_rejects_what_the_python_restatement_rejects(text):
     with pytest.raises(QuantityError):
         Quantity.parse(text)
     L = native_host.lib()
-    L.simon_host_quantity_probe.restype = C.c_int
-    L.simon_host_quantity_probe.argtypes = [C.c_char_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_double)]
     v = C.c_int64(0)
     assert L.simon_host_quantity_probe(text.encode(), C.byref(v), None, None) != 0
 
@@ -224,8 +220,6 @@ def test_native_failure_messages_match_the_python_mirror(seed):
     p = simulator.plan(cluster, apps)
     c = compile_cluster(p.nodes, p.pods, p.ctx)
     L = native_host.lib()
-    L.simon_host_plan_fit_error.restype = C.c_int
-    L.simon_host_plan_fit_error.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_void_p)]
     req = native_host.request_json(cluster, apps)
     h = C.c_void_p()
     assert L.simon_host_compile(req, len(req), C.byref(h)) == 0
@@ -233,7 +227,7 @@ def test_native_failure_messages_match_the_python_mirror(seed):
         counts = np.zeros(24, np.uint32)
         counts[[1, 2, 3, 4, 5, 14, 15, 16, 17, 18]] = [1, 2, 3, 4, 5, 6, 7, 8, 9, 10]
         for k in range(len(c.scalar_names)):
-            counts[6 + k] = 11 + k
+            counts[abi.SFC_SCALAR0 + k] = 11 + k
         seen = set()
         for i, rec in enumerate(p.pods):
             if id(rec.tmpl) in seen:

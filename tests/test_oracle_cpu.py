@@ -77,19 +77,6 @@ def test_duplicate_taints_are_rejected():
         compile_cluster(p.nodes, p.pods, p.ctx)
 
 
-def test_abi_library_exports():
-    """The C-ABI library loads and exports every symbol include/simon_gpu.h declares (no compute calls)."""
-    import os, re
-    from simon_b200 import engine
-    hdr = open(os.path.join(os.path.dirname(__file__), "..", "include", "simon_gpu.h")).read()
-    declared = set(re.findall(r"^(?:int|void|float|uint64_t|const char \*)\s*(simon_[a-z0-9_]+)\s*\(", hdr, re.M))
-    L = engine.lib()
-    for name in declared:
-        assert hasattr(L, name), name
-    assert set(engine.EXPORTS) == declared
-    assert L.simon_gpu_version() == 3
-
-
 def test_open_local_pods_are_refused_at_compile_time():
     """A StatefulSet whose volumeClaimTemplates use an open-local storage class would be filtered / scored / reserved by
     the Open-Local plugin (pkg/simulator/plugin/open-local.go:51-138), which this engine does not implement: refuse."""

@@ -57,8 +57,9 @@ with Engine(c, device=0) as eng:
 # bitmap word and counter at the target 8, at the source 8) + per GPU filter evaluated 100 (device record 96, slot output 4)
 code = runs[SCOPE]["code"]
 cls = c.pods["pod_class"][mv[:, 0]]
-after_fit = (code == 0) | ((code & ((3 << 14) | (7 << 16) | (1 << 19))) != 0)
-reach_gpu = gpu_cls[cls] & ((code == 0) | (code == (1 << 19)))
+gpu_code = 1 << abi.SFC_GPU
+after_fit = (code == 0) | ((code & ((3 << abi.SFC_PTS_MISSING) | (7 << abi.SFC_IPA_AFF) | gpu_code)) != 0)
+reach_gpu = gpu_cls[cls] & ((code == 0) | (code == gpu_code))
 alg = 280 * a.moves + 88 * int(n_hard[cls][after_fit].sum()) + 100 * int(reach_gpu.sum())
 for scope, name in ((0, "unscoped"), (SCOPE, "scoped  ")):
     ms = np.array(res[scope])
