@@ -229,6 +229,9 @@ typedef struct simon_ctx_opts {
 #define SIMON_OPT_FORCE_LARGE 4u     /* run the large-cluster variant (per-node arrays in global memory) at any cluster size, on
                                         cluster_ctas x threads_per_cta when given (threads <= 320), else 16 x 320; a geometry that does
                                         not fit is SIMON_ERR_LIMIT (same results; for verification) */
+#define SIMON_OPT_NO_STATIC_CACHE 8u /* keep no per-(static signature, node) verdict cache: the placement and move kernels evaluate
+                                        every static verdict where they need it, as they do when the cache would pass its 2 GiB cap
+                                        (same results; for verification) */
 
 /* One what-if scenario of the capacity-planning search (pkg/apply/apply.go:203-259):
  * the uploaded snapshot holds the base nodes plus a pool of candidate new nodes; a scenario

@@ -1137,7 +1137,8 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     ps.n_sigs = std::max(1u, p->n_static_sigs);
     {
         size_t words = (size_t)ps.n_sigs * std::max(1u, ctx->snap.N);
-        ps.use_scache = words * 8 <= (2ull << 30) ? 1 : 0;      // per-(signature, node) verdict cache, capped at 2 GiB
+        // per-(signature, node) verdict cache, capped at 2 GiB
+        ps.use_scache = words * 8 <= (2ull << 30) && !(ctx->opt_flags & SIMON_OPT_NO_STATIC_CACHE) ? 1 : 0;
         if (!ps.use_scache) words = 1;
         CU(ps.d_scache.alloc(words));
         CU(cudaMemsetAsync(ps.d_scache.p, 0, 8ull * words, st));

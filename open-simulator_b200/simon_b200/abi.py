@@ -47,6 +47,7 @@ SFC_PTS_MISSING, SFC_PTS_SKEW, SFC_IPA_AFF, SFC_IPA_ANTI, SFC_IPA_EXIST, SFC_GPU
 OPT_RECORD_SCORES = 1
 OPT_NO_PIN_FAST = 2
 OPT_FORCE_LARGE = 4
+OPT_NO_STATIC_CACHE = 8
 
 # move codes other than filter verdicts, and the bias of the per-pod best-move key
 MOVE_NOOP, MOVE_NOT_PLACED, MOVE_NOT_MOVABLE, MOVE_BAD_INDEX = 1 << 24, 1 << 25, 1 << 26, 1 << 27

@@ -39,15 +39,17 @@ class Engine:
     """One device context holding one compiled cluster (snapshot + ordered pod list)."""
 
     def __init__(self, compiled, device: int = 0, record_scores: bool = False, cluster_ctas: int = 0,
-                 threads_per_cta: int = 0, pin_fast: bool = True, force_large: bool = False):
+                 threads_per_cta: int = 0, pin_fast: bool = True, force_large: bool = False, static_cache: bool = True):
         L = lib()
         self.c = compiled
         self.h = C.c_void_p()
         # pin_fast=False: DaemonSet pods take the general one-decision-at-a-time path (SIMON_OPT_NO_PIN_FAST; same results)
         # force_large=True: the large-cluster kernel variant at any size (SIMON_OPT_FORCE_LARGE; same results)
+        # static_cache=False: no static verdict cache, every verdict evaluated where it is needed, as past the cache's 2 GiB cap
+        # (SIMON_OPT_NO_STATIC_CACHE; same results)
         opts = abi.SimonCtxOpts(device, cluster_ctas, threads_per_cta,
                                 (abi.OPT_RECORD_SCORES if record_scores else 0) | (0 if pin_fast else abi.OPT_NO_PIN_FAST) |
-                                (abi.OPT_FORCE_LARGE if force_large else 0))
+                                (abi.OPT_FORCE_LARGE if force_large else 0) | (0 if static_cache else abi.OPT_NO_STATIC_CACHE))
         rc = L.simon_ctx_create(C.byref(opts), C.byref(self.h))
         if rc != 0 or not self.h:
             raise EngineUnavailable(f"simon_ctx_create failed (rc={rc}): no usable CUDA device {device}; "

@@ -398,9 +398,9 @@ def test_move_scoring_marks_pdb_blocked_pods():
             np.testing.assert_array_equal(b["gain"][keep], a["gain"][keep])
 
 
-def _engine_plan(c, mv, t, max_moves, scope=0, min_gain=1):
+def _engine_plan(c, mv, t, max_moves, scope=0, min_gain=1, static_cache=True):
     from simon_b200.engine import Engine
-    with Engine(c, device=0) as eng:
+    with Engine(c, device=0, static_cache=static_cache) as eng:
         out = eng.schedule()[0]
         eng.moves_set_scope(scope)
         eng.moves_upload(mv, 0)
@@ -418,10 +418,10 @@ def _steps(r):
     return np.stack([s["move"], s["pod"], s["from"], s["to"], s["gain"], s["gpu_slots"]], 1).astype(np.int64) if len(s) else np.zeros((0, 6), np.int64)
 
 
-def _plan_vs_checker(c, mv, t, max_moves, scope=0, rebuild=True):
+def _plan_vs_checker(c, mv, t, max_moves, scope=0, rebuild=True, static_cache=True):
     from oracle.binding import Oracle
     from simon_b200.engine import Engine
-    out, allowed, r, pl, sl, st = _engine_plan(c, mv, t, max_moves, scope)
+    out, allowed, r, pl, sl, st = _engine_plan(c, mv, t, max_moves, scope, static_cache=static_cache)
     np.testing.assert_array_equal(allowed, t.allowed(out))
     o = Oracle(c)
     assert np.array_equal(o.schedule()[0], out)
@@ -446,7 +446,7 @@ def _plan_vs_checker(c, mv, t, max_moves, scope=0, rebuild=True):
         moved = got[:, 1]
         fixed[moved] = np.where(fixed[moved] >= 0, pl[moved], fixed[moved])
         c2.pods["pod_fixed_node"] = fixed
-        with Engine(c2, device=0) as eng:
+        with Engine(c2, device=0, static_cache=static_cache) as eng:
             eng.schedule_resume(pl)
             s2 = eng.state()
         for k in s2:

@@ -180,7 +180,7 @@ def _steps(r):
     return np.stack([s["move"], s["pod"], s["from"], s["to"], s["gain"], s["gpu_slots"]], 1).astype(np.int64) if len(s) else np.zeros((0, 6), np.int64)
 
 
-def _engine_vs_checker(c, mv, max_moves, min_gain=1, scope=0, class_local=None, rebuild=False):
+def _engine_vs_checker(c, mv, max_moves, min_gain=1, scope=0, class_local=None, rebuild=False, static_cache=True):
     """The engine's plan equals the checker's, step by step and in the end state; the live state is untouched; with rebuild, the end
     placement resumed on a fresh context gives the plan's end state, and after NO_MOVE no unmoved pod has a qualifying move there."""
     from simon_b200.engine import Engine
@@ -188,7 +188,7 @@ def _engine_vs_checker(c, mv, max_moves, min_gain=1, scope=0, class_local=None, 
         ref = _checker(c, mv, max_moves, min_gain, scope)
     else:
         # the C oracle has no Open-Local: its state is the engine's placement, every placed pod pre-bound where the engine put it
-        with Engine(c, device=0) as eng:
+        with Engine(c, device=0, static_cache=static_cache) as eng:
             live = eng.schedule()[0]
             assert not eng.gpu_slot_words().any()
         cf = copy.copy(c)
@@ -200,7 +200,7 @@ def _engine_vs_checker(c, mv, max_moves, min_gain=1, scope=0, class_local=None, 
         ref = MP.plan(o, mv, live, np.zeros(len(live), np.uint32), max_moves, min_gain, scope, class_local=class_local)
         o.close()
         ref["live"] = live
-    with Engine(c, device=0) as eng:
+    with Engine(c, device=0, static_cache=static_cache) as eng:
         out = eng.schedule()[0]
         np.testing.assert_array_equal(out, ref["live"])
         eng.moves_set_scope(scope)
@@ -230,11 +230,11 @@ def _engine_vs_checker(c, mv, max_moves, min_gain=1, scope=0, class_local=None, 
         np.testing.assert_array_equal(before[3][k], after[3][k])
     assert before[3]["topk"] == after[3]["topk"] and before[3]["best_key"] == after[3]["best_key"]
     if rebuild:
-        _independent_rebuild(c, r, pl, st, ext, mv, min_gain, scope)
+        _independent_rebuild(c, r, pl, st, ext, mv, min_gain, scope, static_cache)
     return r
 
 
-def _independent_rebuild(c, r, pl, st, ext, mv, min_gain, scope):
+def _independent_rebuild(c, r, pl, st, ext, mv, min_gain, scope, static_cache=True):
     from simon_b200.engine import Engine
     c2 = copy.copy(c)
     c2.pods = dict(c.pods)
@@ -242,7 +242,7 @@ def _independent_rebuild(c, r, pl, st, ext, mv, min_gain, scope):
     moved = _steps(r)[:, 1]
     fixed[moved] = np.where(fixed[moved] >= 0, pl[moved], fixed[moved])     # a moved pre-bound pod is bound to its new node
     c2.pods["pod_fixed_node"] = fixed
-    with Engine(c2, device=0) as eng:
+    with Engine(c2, device=0, static_cache=static_cache) as eng:
         eng.schedule_resume(pl)
         st2, ext2 = eng.state(), eng.state_ext()
         for k in st:

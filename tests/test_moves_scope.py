@@ -310,11 +310,11 @@ def _stage_of(code):
 
 # ---------------------------------------------------------------------------------------------------------------- GPU ----
 
-def _engine_vs_checker(c, o, out, mv, scope, class_local=None):
+def _engine_vs_checker(c, o, out, mv, scope, class_local=None, static_cache=True):
     from simon_b200 import moves as M
     from simon_b200.engine import Engine
     gain, code, slots = MS.moves_score(o, mv, out, scope, class_local=class_local)
-    with Engine(c, device=0) as eng:
+    with Engine(c, device=0, static_cache=static_cache) as eng:
         np.testing.assert_array_equal(eng.schedule()[0], out)
         eng.moves_set_scope(scope)
         eng.moves_upload(mv, 0)

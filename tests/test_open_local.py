@@ -352,13 +352,22 @@ def check_restated_open_local(c, out, score, final):
     with different raw Open-Local scores."""
     import ctypes
     from oracle.binding import Oracle
-    from simon_b200.storage import StorageReplay, lvm_place, normalize_scores
-    st = c.storage
     orc = Oracle(c)
     orc.enable_dump()
-    P = c.pods_dims["n_pods"]
-    fixed = np.ctypeslib.as_array((ctypes.c_int32 * P).from_address(orc.pods.pod_fixed_node))
+    # the oracle reads c's own pod_fixed_node array: it is restored afterwards, so that c can be checked again
+    fixed = np.ctypeslib.as_array((ctypes.c_int32 * c.pods_dims["n_pods"]).from_address(orc.pods.pod_fixed_node))
     orig = fixed.copy()
+    try:
+        return _restated_open_local_pods(c, out, score, final, orc, fixed, orig)
+    finally:
+        fixed[:] = orig
+        orc.close()
+
+
+def _restated_open_local_pods(c, out, score, final, orc, fixed, orig):
+    from simon_b200.storage import StorageReplay, lvm_place, normalize_scores
+    st = c.storage
+    P = c.pods_dims["n_pods"]
     rep = StorageReplay(st, c.node_names)
     pod_class = c.pods["pod_class"]
     multi = 0
@@ -398,7 +407,6 @@ def check_restated_open_local(c, out, score, final):
                 multi += 1
         if st.class_local[cls]:
             rep.bind(cls, int(out[i]))
-    orc.close()
     assert np.array_equal(final, rep.requested())
     return multi
 
