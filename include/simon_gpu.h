@@ -57,6 +57,7 @@ extern "C" {
 #define SIMON_MAX_TAINT_WORDS 4
 #define SIMON_MAX_TOPOS 8
 #define SIMON_N_FAIL_CODES 24
+#define SIMON_SOFT_SIZE0_WOFF 6 /* entry-table bitmask word offset past the engine's domain bitmask: the entry counts no domain */
 
 typedef enum simon_status {
     SIMON_OK = 0,
@@ -144,12 +145,17 @@ enum simon_class_word {
     SCW_N_IPA_SCORE,
     SCW_OFF_INC,        /* counters this class's pods increment when placed, 3 words each: counter, topo, sig:
                            sig = -1, or a class id: increment only if the node is eligible for THAT class
-                           (passes its node selection program and carries all its soft topology keys) */
+                           (passes its node selection program and carries all its soft topology keys).  A counter
+                           appears m times when m of its selectors match the class (spread constraints of one class
+                           on one topology key share one summed counter), so a pod adds m to it */
     SCW_N_INC,
     SCW_OFF_ENT,        /* engine entry table, 8 words per entry in the order ports, hard, soft, aff, anti, exist, score:
-                           kind, counter, topo, a (maxSkew | weight), b (selfMatch | is_hostname), inc (this class's pods
-                           increment the counter), bitmask word offset (-1: table method), offset of the counter in the
-                           engine's counter array (prefix sum of topo_ndom over counter ids) */
+                           kind, counter, topo, a (maxSkew | weight), b (selfMatch | is_hostname), inc (how many times this
+                           class's pods increment the counter: its multiplicity in the commit list, 0: never), bitmask word
+                           offset (-1: table method; SIMON_SOFT_SIZE0_WOFF: a ScheduleAnyway constraint on a non-hostname
+                           key that an earlier constraint of the class already uses, whose topology size is 0,
+                           podtopologyspread/scoring.go:85-99), offset of the counter in the engine's counter array
+                           (prefix sum of topo_ndom over counter ids) */
     SCW_N_ENT,
     SCW_ANY_TABLE,      /* some soft constraint's topology is too large for the per-decision domain bitmask */
     SCW_ELIG_SIG,       /* representative class id of this class's own spreading-eligibility signature (the `sig`

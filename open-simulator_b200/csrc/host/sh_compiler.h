@@ -477,6 +477,7 @@ struct PerClass {
     std::vector<long long> ports;
     std::vector<std::array<long long, 4>> hard;
     std::vector<std::array<long long, 5>> soft;
+    std::vector<long long> soft_mult;      // per soft constraint: the largest multiplicity of a class in its counter
     std::vector<std::array<long long, 2>> aff, anti, exist;
     std::map<std::pair<long long, long long>, long long> score;
     int self = 0;
@@ -1029,17 +1030,33 @@ inline void compile_cluster(const Plan &plan, Compiled &out) {
                 if (p.ip == "0.0.0.0" || pu.first.ip == "0.0.0.0" || pu.first.ip == p.ip) chk.insert(counter(pu.second, 0));
             }
         L.ports.assign(chk.begin(), chk.end());
+        // PodTopologySpread counts are kept per topology PAIR, so the constraints of one kind on one key see the sum of their
+        // selectors' matches (filtering.go:215-265 TpPairToMatchNum; scoring.go:57-105 TopologyPairToPodCounts, hostname
+        // excepted: scoring.go:195-198 counts per constraint on the node): they share one counter over the summed member
+        // lists, sorted, with a class repeated once per selector it matches
+        auto summed = [&](const std::vector<Spread> &list, const std::string &key) {
+            std::vector<int> S;
+            for (auto &e : list)
+                if (e.key == key) { const std::vector<int> &m = members(Clauses{{&own_ns, &e.reqs}}); S.insert(S.end(), m.begin(), m.end()); }
+            std::sort(S.begin(), S.end());
+            return S;
+        };
         for (auto &e : c.hard) {
-            const std::vector<int> &S = members(Clauses{{&own_ns, &e.reqs}});
             long long selfm = requirements_match(e.reqs, *c.labels) ? 1 : 0, t = topo_id(e.key);
-            L.hard.push_back({counter(S, t), t, e.skew, selfm});
+            L.hard.push_back({counter(summed(c.hard, e.key), t), t, e.skew, selfm});
         }
         for (auto &e : c.soft) {
-            const std::vector<int> &S = members(Clauses{{&own_ns, &e.reqs}});
             long long host = e.key == LABEL_HOSTNAME ? 1 : 0, t = topo_id(e.key);
+            const std::vector<int> S = host ? members(Clauses{{&own_ns, &e.reqs}}) : summed(c.soft, e.key);
             long long domk = host ? -1 : counter(S, t, elig_sig(c));
             long long nodek = counter(S, 0);
             L.soft.push_back({nodek, t, e.skew, host, domk});
+            long long mult = S.empty() ? 1 : 0;
+            for (size_t i = 0, j; i < S.size(); i = j) {
+                for (j = i; j < S.size() && S[j] == S[i]; j++) {}
+                mult = std::max<long long>(mult, (long long)(j - i));
+            }
+            L.soft_mult.push_back(mult);
         }
         if (!c.aff_req.empty()) {
             Clauses cl;
@@ -1282,8 +1299,10 @@ inline void compile_cluster(const Plan &plan, Compiled &out) {
         put(SCW_OFF_PTS_SOFT);
         w[SCW_N_PTS_SOFT] = (long long)L.soft.size();
         // the counts part of a raw PodTopologySpread score (pods x constraints x ln(topology size + 2)) must fit int32 on the
-        // device, which keeps raw - sum(maxSkew - 1)
-        if (!L.soft.empty() && (double)P * (double)L.soft.size() * std::log((double)N + 2.0) >= (double)((1LL << 31) - 2))
+        // device, which keeps raw - sum(maxSkew - 1); a pod adds up to its class's multiplicity in a summed counter
+        long long n_soft_counts = 0;
+        for (long long m : L.soft_mult) n_soft_counts += m;
+        if (!L.soft.empty() && (double)P * (double)n_soft_counts * std::log((double)N + 2.0) >= (double)((1LL << 31) - 2))
             throw CompileError("class " + std::to_string(c.cid) + ": topology spread scores of pod count x constraints can exceed 2^31");
         for (auto &e : L.soft) body.insert(body.end(), e.begin(), e.end());
         put(SCW_OFF_IPA_AFF);
@@ -1315,8 +1334,8 @@ inline void compile_cluster(const Plan &plan, Compiled &out) {
         // engine entry table: one 8-word row per list entry (kind, counter, topo, a, b, inc, bitmask word offset, counter base)
         put(SCW_OFF_ENT);
         std::vector<std::array<long long, 8>> ent;
-        std::set<std::pair<long long, long long>> inc_set;
-        for (auto &e : inc) inc_set.insert({e[0], e[1]});
+        std::map<std::pair<long long, long long>, long long> inc_mult;
+        for (auto &e : inc) inc_mult[{e[0], e[1]}]++;
         for (long long kid : L.ports) ent.push_back({EK_PORT, kid, 0, 0, 0, 0, 0, 0});
         for (auto &e : L.hard) ent.push_back({EK_HARD, e[0], e[1], e[2], e[3], 0, 0, 0});
         for (auto &e : L.soft) ent.push_back({EK_SOFT, e[3] ? e[0] : e[4], e[1], e[2], e[3], 0, 0, 0});
@@ -1325,12 +1344,18 @@ inline void compile_cluster(const Plan &plan, Compiled &out) {
         for (auto &e : ex) ent.push_back({EK_EXIST, e[0], e[1], 0, 0, 0, 0, 0});
         for (auto &kv : L.score) ent.push_back({EK_SCORE, kv.first.first, kv.first.second, kv.second, 0, 0, 0, 0});
         long long woff = 0, any_table = 0;
+        std::set<long long> soft_topos;
         for (auto &r : ent) {
             long long kind = r[0], kid = r[1], t = r[2], b = r[4];
             long long tk = (kind == EK_SOFT && b) ? 0 : t;
-            r[5] = inc_set.count({kid, tk}) ? 1 : 0;
+            auto im = inc_mult.find({kid, tk});
+            r[5] = im == inc_mult.end() ? 0 : im->second;
             long long wo = -1;
-            if (kind == EK_SOFT && !b) {
+            if (kind == EK_SOFT && !b && soft_topos.count(t)) {
+                // topoSize grows only for the constraint that creates a pair (scoring.go:85-99): a later one on the same key gets 0
+                wo = SIMON_SOFT_SIZE0_WOFF;
+            } else if (kind == EK_SOFT && !b) {
+                soft_topos.insert(t);
                 long long nw = ((long long)out.topo_ndom[(size_t)t] + 63) / 64;
                 if (woff + nw <= SK_MAXW) { wo = woff; woff += nw; }
                 else any_table = 1;

@@ -1007,26 +1007,31 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
             return fail(ctx, SIMON_ERR_INVALID, "class %u: entry table does not match the list sizes", c);
         uint32_t *ax = aux.data() + (size_t)c * SK_AUX_W;
         uint32_t recs[SK_MAX_ENT];
-        bool node_lvl[SK_MAX_ENT], incs[SK_MAX_ENT];
+        bool node_lvl[SK_MAX_ENT];
+        uint32_t incs[SK_MAX_ENT];
         uint32_t n_dom = 0, n_all = 0, n_aff_node = 0;
         for (uint32_t e = 0; e < E; e++) {
             const int64_t *r = et + 8ull * e;
             const int32_t kind = (int32_t)r[ER_KIND];
             const bool host = kind == EK_SOFT && r[ER_B] != 0;
-            incs[e] = r[ER_INC] != 0;
+            // a commit adds the class's multiplicity in the entry's counter: the record is listed that many times
+            if (r[ER_INC] < 0 || r[ER_INC] > SK_MAX_ENT) return fail(ctx, SIMON_ERR_INVALID, "class %u: bad increment count", c);
+            incs[e] = (uint32_t)r[ER_INC];
             // entry | topology row << 8 | flags << 16 (bit 16: domain-level soft constraint, bit 17: required affinity term)
             recs[e] = e | ((host ? 0u : (uint32_t)r[ER_T]) << 8) | ((kind == EK_SOFT && !host) ? 1u << 16 : 0u) | (kind == EK_AFF ? 1u << 17 : 0u);
             // entries on topology row 0 (the node itself) can only match the winner's own node: they go to the end of the
             // list and are applied by the owning thread alone; every thread walks the others
             node_lvl[e] = incs[e] && ((recs[e] >> 8) & 0xff) == 0;
-            if (incs[e]) { n_all++; if (!node_lvl[e]) n_dom++; else if (recs[e] & (1u << 17)) n_aff_node++; }
+            if (incs[e]) { n_all += incs[e]; if (!node_lvl[e]) n_dom += incs[e]; else if (recs[e] & (1u << 17)) n_aff_node += incs[e]; }
             for (uint32_t q = 0; q < ER_ROWS; q++) ax[SK_AUX_ENT + q * SK_MAX_ENT + e] = (uint32_t)(int32_t)r[q];
         }
+        if (n_all > SK_MAX_ENT)
+            return fail(ctx, SIMON_ERR_LIMIT, "class %u: a commit increments %u cached entry values, more than the engine limit (%d)", c, n_all, SK_MAX_ENT);
         uint32_t kd = 0, kn = n_dom;
-        for (uint32_t e = 0; e < E; e++) {
-            if (!incs[e]) continue;
-            if (node_lvl[e]) ax[kn++] = recs[e]; else ax[kd++] = recs[e];
-        }
+        for (uint32_t e = 0; e < E; e++)
+            for (uint32_t m = 0; m < incs[e]; m++) {
+                if (node_lvl[e]) ax[kn++] = recs[e]; else ax[kd++] = recs[e];
+            }
         ax[SK_MAX_ENT] = n_dom | (n_all << 8) | (n_aff_node << 16);
         const int64_t *inc = cw + cw[SCW_OFF_INC];
         for (uint32_t u = 0; u < 32 && (int64_t)u < cw[SCW_N_INC]; u++) {

@@ -23,6 +23,8 @@ namespace cg = cooperative_groups;
 #define SK_MAX_SOFT 8
 #define SK_MAX_CS 16
 #define SK_MAXW 6           // domain-bitmask words available per decision
+// a soft entry whose word offset is SK_MAXW or more sets no bit and counts no domain: topology size 0
+static_assert(SIMON_SOFT_SIZE0_WOFF >= SK_MAXW, "the size-0 word offset must lie past the domain bitmask");
 #define SK_NV 16            // max values per all-reduce
 #define SK_PLW 5            // payload: up to 10 int32 packed in 5 u64 (T domains + flags); only (T + 2) / 2 of them are sent
 #define SK_MAX_WARPS 16     // threads per CTA <= 512 (the shipped variants use <= 320)

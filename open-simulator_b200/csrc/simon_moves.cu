@@ -326,11 +326,12 @@ __global__ void __launch_bounds__(256, MINB) simon_moves_kernel(const __grid_con
                 if (st_code) code = 1u << SFC_STATIC;
                 if (code == SMV_OK && need_ent && !cw) cw = P.class_blob + __ldg(P.class_off + cls);
                 const int64_t *et = need_ent && cw ? cw + cw[SCW_OFF_ENT] : nullptr;
-                // counter value of entry e at b's domain with p's own contribution (made from node a) removed
+                // counter value of entry e at b's domain with p's own contribution (made from node a: its multiplicity in the
+                // counter) removed
                 auto val_at = [&](uint32_t e, int32_t d) -> int32_t {
                     const int64_t *r = et + 8ull * e;
                     int32_t v = __ldg(P.cnt + (uint32_t)r[ER_BASE] + (uint32_t)d);
-                    if (r[ER_INC] && smv_dom(P, na, (uint32_t)a, r[ER_T]) == d) v -= 1;
+                    if (r[ER_INC] && smv_dom(P, na, (uint32_t)a, r[ER_T]) == d) v -= (int32_t)r[ER_INC];
                     return v;
                 };
                 // ---- NodePorts
@@ -356,7 +357,7 @@ __global__ void __launch_bounds__(256, MINB) simon_moves_kernel(const __grid_con
                 }
                 // ---- PodTopologySpread, DoNotSchedule constraints (filtering.go:276-328) with p removed: b's count loses p's own
                 // count if p's sits at b's domain (val_at), and the minimum over the registered domains becomes
-                // min(min, cnt[dom_a] - 1) when p's count sits at a registered dom_a
+                // min(min, cnt[dom_a] - m) when p's count m (its class's multiplicity in the counter) sits at a registered dom_a
                 if (SCOPED && code == SMV_OK && n_hard) {
                     const int2 *hs = P.hs + (uint64_t)cls * SMV_MAX_HARD;
 #pragma unroll 1
@@ -372,7 +373,7 @@ __global__ void __launch_bounds__(256, MINB) simon_moves_kernel(const __grid_con
                         if (r[ER_INC]) {
                             const int32_t da = smv_dom(P, na, (uint32_t)a, t);
                             if (da >= 0 && ((__ldg(reg + (da >> 5)) >> (da & 31)) & 1u))
-                                mn = min(mn, __ldg(P.cnt + (uint32_t)r[ER_BASE] + (uint32_t)da) - 1);
+                                mn = min(mn, __ldg(P.cnt + (uint32_t)r[ER_BASE] + (uint32_t)da) - (int32_t)r[ER_INC]);
                         }
                         if ((int64_t)match + r[ER_B] - (int64_t)mn > r[ER_A]) { code = 1u << SFC_PTS_SKEW; break; }
                     }

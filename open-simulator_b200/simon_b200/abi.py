@@ -21,6 +21,7 @@ MAX_VOLS = 8            # Open-Local LVM PVCs per class
 MAX_DEVS = 16           # Open-Local SSD + HDD devices per node
 MAX_DEV_VOLS = 8        # Open-Local SSD + HDD PVCs per class
 N_FAIL_CODES = 24
+SOFT_SIZE0_WOFF = 6     # entry-table word offset of a later same-key ScheduleAnyway constraint: topology size 0
 
 NODE_UNSCHEDULABLE = 1
 NODE_HAS_LABELS = 2

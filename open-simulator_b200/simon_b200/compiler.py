@@ -38,7 +38,7 @@ from .abi import (CLS_HAS_REQUEST, CLS_IPA_SELF_MATCH, CLS_PINNED, CLS_SIMON_NOR
                   SCW_N_PORTS, SCW_N_PREF, SCW_N_PTS_HARD, SCW_N_PTS_SOFT, SCW_NODE_NAME, SCW_NZ_MCPU, SCW_NZ_MEM, SCW_OFF_ENT,
                   SCW_OFF_INC, SCW_OFF_IPA_AFF, SCW_OFF_IPA_ANTI, SCW_OFF_IPA_EXIST, SCW_OFF_IPA_SCORE, SCW_OFF_PORTS, SCW_OFF_PREF,
                   SCW_OFF_PTS_HARD, SCW_OFF_PTS_SOFT, SCW_OFF_SCALARS, SCW_OFF_SEL, SCW_OFF_TOL, SCW_REQ_EPH, SCW_REQ_MCPU,
-                  SCW_REQ_MEM, SCW_SCORE_MCPU, SCW_SCORE_MEM, SCW_STATIC_ROW, SCW_STATIC_SIG)
+                  SCW_REQ_MEM, SCW_SCORE_MCPU, SCW_SCORE_MEM, SCW_STATIC_ROW, SCW_STATIC_SIG, SOFT_SIZE0_WOFF)
 from .gomath import log_table
 from .objects import Obj
 from .quantity import Quantity
@@ -813,7 +813,9 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
         group_cache[key] = got
         return got
 
-    counters = _Interner()   # (frozenset S, topo, eligibility signature class | None)
+    # (member classes S, topo, eligibility signature class | None); S is a frozenset, or (see _summed) a sorted tuple with a
+    # class repeated once per selector of a summed counter that it matches
+    counters = _Interner()
 
     def counter(S: frozenset, t: int, sig=None) -> int:
         return counters.get((S, t, sig))
@@ -848,7 +850,7 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
             port_users.setdefault(p, []).append(c.cid)
 
     for c in classes:
-        L = {"ports": [], "hard": [], "soft": [], "aff": [], "anti": [], "exist": [], "score": {}, "self": 0}
+        L = {"ports": [], "hard": [], "soft": [], "soft_mult": [], "aff": [], "anti": [], "exist": [], "score": {}, "self": 0}
         # host ports (HostPortInfo.CheckConflict, types.go:784-814)
         chk = set()
         for (ip, proto, port) in c.ports:
@@ -858,15 +860,25 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
                 if ip == "0.0.0.0" or ip2 == "0.0.0.0" or ip2 == ip:
                     chk.add(counter(frozenset(users), 0))
         L["ports"] = sorted(chk)
+        # PodTopologySpread counts are kept per topology PAIR, so the constraints of one kind on one key see the sum of their
+        # selectors' matches (filtering.go:215-265 TpPairToMatchNum; scoring.go:57-105 TopologyPairToPodCounts, hostname
+        # excepted: scoring.go:195-198 counts per constraint on the node): they share one counter over the summed member sets
+        hard_sets: Dict[str, list] = {}
+        for (key, _skew, reqs) in c.hard:
+            hard_sets.setdefault(key, []).append(members(((frozenset([c.namespace]), reqs),)))
+        soft_sets: Dict[str, list] = {}
+        for (key, _skew, reqs) in c.soft:
+            if key != O.LABEL_HOSTNAME:
+                soft_sets.setdefault(key, []).append(members(((frozenset([c.namespace]), reqs),)))
         for (key, skew, reqs) in c.hard:
-            S = members(((frozenset([c.namespace]), reqs),))
             selfm = 1 if requirements_match(reqs, c.labels) else 0
-            L["hard"].append((counter(S, topo.ids[key]), topo.ids[key], skew, selfm))
+            L["hard"].append((counter(_summed(hard_sets[key]), topo.ids[key]), topo.ids[key], skew, selfm))
         for (key, skew, reqs) in c.soft:
-            S = members(((frozenset([c.namespace]), reqs),))
             host = 1 if key == O.LABEL_HOSTNAME else 0
+            S = members(((frozenset([c.namespace]), reqs),)) if host else _summed(soft_sets[key])
             domk = -1 if host else counter(S, topo.ids[key], elig_sig(c))
             L["soft"].append((counter(S, 0), topo.ids[key], skew, host, domk))
+            L["soft_mult"].append(_max_multiplicity(S))
         if c.aff_req:
             clauses = tuple((ns, reqs) for (ns, reqs, _k) in c.aff_req)
             S = members(clauses)
@@ -1037,7 +1049,8 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
             body.extend(e)
         put(SCW_OFF_PTS_SOFT)
         w[SCW_N_PTS_SOFT] = len(L["soft"])
-        if L["soft"] and len(pods) * len(L["soft"]) * math.log(N + 2 + extra_log) >= PTS_COUNTS_MAX:
+        # a pod adds up to its class's multiplicity in a summed counter: the bound counts every constraint that many times
+        if L["soft"] and len(pods) * sum(L["soft_mult"]) * math.log(N + 2 + extra_log) >= PTS_COUNTS_MAX:
             raise CompileError(f"class {c.cid}: topology spread scores of pod count x constraints can exceed 2^31")
         for e in L["soft"]:
             body.extend(e)
@@ -1070,7 +1083,9 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
         # engine entry table: one 8-word row per list entry (kind, counter, topo, a, b, inc, bitmask word offset, counter base)
         put(SCW_OFF_ENT)
         ent_rows = []
-        inc_set = {(kid, t) for (kid, t, _sig) in inc_lists[c.cid]}
+        inc_mult: Dict[Tuple[int, int], int] = {}
+        for (kid, t, _sig) in inc_lists[c.cid]:
+            inc_mult[(kid, t)] = inc_mult.get((kid, t), 0) + 1
         for kid in L["ports"]:
             ent_rows.append([EK_PORT, kid, 0, 0, 0])
         for (kid, t, skew, selfm) in L["hard"]:
@@ -1087,12 +1102,17 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
             ent_rows.append([EK_SCORE, kid, t, wt, 0])
         woff = 0
         any_table = 0
+        soft_topos = set()
         for r in ent_rows:
             kind, kid, t, a, b = r
             tk = 0 if (kind == EK_SOFT and b) else t
-            inc = 1 if (kid, tk) in inc_set else 0
+            inc = inc_mult.get((kid, tk), 0)
             wo = -1
-            if kind == EK_SOFT and not b:
+            if kind == EK_SOFT and not b and t in soft_topos:
+                # topoSize grows only for the constraint that creates a pair (scoring.go:85-99): a later one on the same key gets 0
+                wo = SOFT_SIZE0_WOFF
+            elif kind == EK_SOFT and not b:
+                soft_topos.add(t)
                 nw = (int(topo_ndom[t]) + 63) // 64
                 if woff + nw <= SK_MAXW:
                     wo = woff
@@ -1138,6 +1158,28 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
 
 def _i64(x: int) -> int:
     return x - (1 << 64) if x >= (1 << 63) else x
+
+
+def _summed(sets: List[frozenset]):
+    """Member set of the counter that sums the matches of several selectors on one key: the frozenset of the classes when none
+    is in two of the sets (so a lone constraint keeps its plain counter), else the sorted tuple of the classes with each class
+    repeated once per set it is in.  Either way iterating it yields a class as many times as a pod of it adds to the count."""
+    if len(sets) == 1:
+        return sets[0]
+    mult: Dict[int, int] = {}
+    for s in sets:
+        for cid in s:
+            mult[cid] = mult.get(cid, 0) + 1
+    if all(m == 1 for m in mult.values()):
+        return frozenset(mult)
+    return tuple(sorted(cid for cid, m in mult.items() for _ in range(m)))
+
+
+def _max_multiplicity(S) -> int:
+    """How many times the class most often repeated in a counter's member set (see _summed) is in it; 1 for a frozenset."""
+    if isinstance(S, frozenset):
+        return 1
+    return max([S.count(cid) for cid in set(S)] or [1])
 
 
 def _compile_term(term: Obj, req_atoms, name_to_idx, pin_name: Optional[str] = None):

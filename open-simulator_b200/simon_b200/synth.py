@@ -523,6 +523,82 @@ def make_mix(seed_no: int = 100, n_nodes: int = 40, n_workloads: int = 30, max_r
     return cluster, [app]
 
 
+SAME_KEY_SELECTORS = [{"matchLabels": {"a": "x"}}, {"matchLabels": {"b": "y"}}, {"matchLabels": {"a": "x", "b": "y"}},
+                      {"matchExpressions": [{"key": "a", "operator": "In", "values": ["x", "y"]}]},
+                      {"matchExpressions": [{"key": "b", "operator": "Exists"}]}]
+
+
+def make_same_key(seed_no: int = 1, n_nodes: int = 24, n_workloads: int = 14, max_replicas: int = 6):
+    """Clusters whose workloads carry 2-4 PodTopologySpread constraints on ONE topology key (hostname, zone or a custom rack
+    key): all DoNotSchedule, all ScheduleAnyway, or both kinds on the key.  The selectors are disjoint, overlapping (a pod labelled
+    a=x, b=y matches two or three of them) or identical with another maxSkew.  The reference sums the counts of such constraints per
+    topology pair.  Around them: nodes without the zone or rack label, a nodeSelector that restricts eligibility, a constraint on a
+    second key, pre-bound pods labelled for the selectors, bare pods, and a DaemonSet with two zone constraints."""
+    rng = SplitMix64(SEED_BASE + 0x3000 + seed_no)
+    cluster = ResourceTypes()
+    zone_key, host_key, rack_key = "topology.kubernetes.io/zone", "kubernetes.io/hostname", "example.com/rack"
+    node_names = []
+    for i in range(n_nodes):
+        name = f"node-{i:03d}"
+        node_names.append(name)
+        labels = {"pool": rng.pick(["a", "b"])}
+        if not rng.chance(15):
+            labels[rack_key] = f"rack-{rng.below(4)}"
+        n = _node(name, 64 if i % 7 == 3 else rng.pick([4, 8, 16]), f"zone-{i % 3}", "", 100, labels, pods=rng.pick([8, 16, 110]))
+        if rng.chance(10):
+            del n["metadata"]["labels"][zone_key]
+        cluster.Nodes.append(n)
+
+    def labelled():
+        return {"a": rng.pick(["x", "y"]), "b": rng.pick(["y", "z"])}
+
+    for i in range(n_nodes):
+        if rng.chance(25):
+            cluster.Pods.append({"apiVersion": "v1", "kind": "Pod",
+                                 "metadata": {"name": f"running-{i:03d}", "namespace": "default", "labels": labelled()},
+                                 "spec": {"nodeName": node_names[i],
+                                          "containers": [{"name": "c", "image": "registry.local/sys:v1",
+                                                          "resources": {"requests": {"cpu": "250m", "memory": "256Mi"}}}]}})
+    app = AppResource("same-key", ResourceTypes())
+    for w in range(n_workloads):
+        name = f"wl-{w:03d}"
+        key = rng.pick([host_key, zone_key, zone_key, rack_key])
+        mode = rng.below(3)          # 0: DoNotSchedule, 1: ScheduleAnyway, 2: both kinds on the key
+        cons = []
+        for j in range(2 + rng.below(3)):
+            when = ("DoNotSchedule", "ScheduleAnyway")[j % 2] if mode == 2 else ("DoNotSchedule", "ScheduleAnyway")[mode]
+            same = [x for x in cons if x["whenUnsatisfiable"] == when]
+            sel = dict(same[-1]["labelSelector"]) if same and rng.chance(25) else rng.pick(SAME_KEY_SELECTORS)
+            # a DoNotSchedule maxSkew of 0 is a valid filter that no domain at or above the minimum passes
+            skew = 0 if when == "DoNotSchedule" and rng.chance(8) else 1 + rng.below(3)
+            cons.append({"maxSkew": skew, "topologyKey": key, "whenUnsatisfiable": when, "labelSelector": sel})
+        if rng.chance(20):
+            cons.append({"maxSkew": 2, "topologyKey": rng.pick([k for k in (host_key, zone_key, rack_key) if k != key]),
+                         "whenUnsatisfiable": rng.pick(["DoNotSchedule", "ScheduleAnyway"]), "labelSelector": rng.pick(SAME_KEY_SELECTORS)})
+        cont = {"name": "c", "image": f"registry.local/{name}:v1",
+                "resources": {"requests": {"cpu": f"{_log_uniform(rng, 100, 3000, 50)}m", "memory": f"{_log_uniform(rng, 128, 4096, 64)}Mi"}}}
+        spec = {"containers": [cont], "topologySpreadConstraints": cons}
+        if rng.chance(20):
+            spec["nodeSelector"] = {"pool": "a"}
+        labels = dict(labelled(), app=name)
+        if rng.chance(25):
+            app.Resource.Pods.append({"apiVersion": "v1", "kind": "Pod", "metadata": {"name": name, "namespace": "default", "labels": labels},
+                                      "spec": spec})
+        else:
+            app.Resource.Deployments.append({"apiVersion": "apps/v1", "kind": "Deployment", "metadata": {"name": name, "namespace": "default"},
+                                             "spec": {"replicas": 1 + rng.below(max_replicas), "selector": {"matchLabels": {"app": name}},
+                                                      "template": {"metadata": {"labels": labels}, "spec": spec}}})
+    ds_cons = [{"maxSkew": 3, "topologyKey": zone_key, "whenUnsatisfiable": "DoNotSchedule", "labelSelector": sel}
+               for sel in SAME_KEY_SELECTORS[:2]]
+    app.Resource.DaemonSets.append({"apiVersion": "apps/v1", "kind": "DaemonSet", "metadata": {"name": "agent", "namespace": "default"},
+                                    "spec": {"selector": {"matchLabels": {"app": "agent"}},
+                                             "template": {"metadata": {"labels": {"app": "agent", "a": "x", "b": "y"}},
+                                                          "spec": {"containers": [{"name": "a", "image": "registry.local/agent:v1",
+                                                                                   "resources": {"requests": {"cpu": "50m", "memory": "64Mi"}}}],
+                                                                   "topologySpreadConstraints": ds_cons}}}})
+    return cluster, [app]
+
+
 class LiveSnapshot:
     """A compiled cluster whose pod list is a set of RUNNING pods (spec.nodeName set): what importing a live cluster yields.
     Same arrays as compiler.Compiled as far as Engine / Oracle are concerned."""

@@ -633,6 +633,10 @@ static int64_t schedule_one(simon_oracle *o, uint32_t cls, int64_t *out_score, u
                 for (uint32_t d = 0; d < nd; d++) reg[d] |= pr[d];
             }
             for (uint32_t d = 0; d < nd; d++) size += reg[d];
+            /* topoSize[j] grows only when constraint j creates the pair (scoring.go:85-99): a later constraint on a key an
+             * earlier one already has gets 0, which the compiler marks in the entry table's word offset */
+            const int64_t *ent = cw + cw[SCW_OFF_ENT] + 8 * (c->n_ports + c->n_hard + j);
+            if (ent[6] == SIMON_SOFT_SIZE0_WOFF) size = 0;
             run_stage(c, ST_SOFTTP);
             memset(tp, 0, sizeof(int64_t) * nd);
             for (int t2 = 0; t2 < T; t2++) {
@@ -857,13 +861,15 @@ int simon_oracle_gpu_slots(simon_oracle *o, uint32_t first, uint32_t count, uint
     return SIMON_OK;
 }
 
-/* does a pod of the class with commit list `inc` (n entries of {counter, topology, sig}), sitting on node a, contribute
- * one count to counter k (keyed on topology t) at domain d?  (what commit() added for it and RemovePod takes back) */
+/* how many counts does a pod of the class with commit list `inc` (n entries of {counter, topology, sig}), sitting on node a,
+ * contribute to counter k (keyed on topology t) at domain d?  One per time the list names k: a summed spread counter is named
+ * once per selector of the key that the class matches.  (what commit() added for it and RemovePod takes back) */
 static int32_t own_inc(const simon_oracle *o, const int64_t *inc, int64_t n, int64_t k, int64_t t, uint32_t a, int32_t d) {
+    if (dom_of(o, t, a) != d) return 0;
+    int32_t m = 0;
     for (int64_t i = 0; i < n; i++)
-        if (inc[3 * i] == k && inc[3 * i + 1] == t && inc[3 * i + 2] < 0)
-            return dom_of(o, t, a) == d ? 1 : 0;
-    return 0;
+        if (inc[3 * i] == k && inc[3 * i + 1] == t && inc[3 * i + 2] < 0) m++;
+    return m;
 }
 
 /* ---------------------------------------------------------------------------------------------------------------

@@ -126,6 +126,13 @@ def test_native_columns_match_python_on_random_feature_mixes(seed):
                                  with_images=bool(seed % 3 == 0))) == []
 
 
+@pytest.mark.parametrize("seed", [1, 2, 3, 4, 5, 6, 7, 8])
+def test_native_columns_match_python_on_same_key_spread(seed):
+    """Spread constraints of one kind sharing a topology key (synth.make_same_key): the summed counters, the commit lists that
+    name a counter once per matching selector, the entry tables' increment counts and size-0 marks are the same in both compilers."""
+    assert _diff(*synth.make_same_key(seed_no=seed)) == []
+
+
 def test_native_columns_match_python_on_the_plugin_kats():
     import kat_plugins
     for name, kat in kat_plugins.CASES.items():
@@ -196,11 +203,15 @@ def test_native_refusals_match_the_python_compiler():
     assert "spec.containers" in e.value.msg
 
 
-@pytest.mark.parametrize("seed", [5, 101, 104, 107, 110, 113])
+@pytest.mark.parametrize("seed", [5, 101, 104, 107, 110, 113, "same-key-2", "same-key-5"])
 def test_native_failure_messages_match_the_python_mirror(seed):
-    """FitError text for every pod of a mixed cluster (taints, node selectors / affinity incl. matchFields, cordoned nodes), with an
-    empty and with a synthetic dynamic histogram: simon_host_plan_fit_error == simulator.format_fit_error."""
-    cluster, apps = synth.make_mix(seed_no=seed, n_nodes=40, n_workloads=25, max_replicas=3)
+    """FitError text for every pod of a mixed cluster (taints, node selectors / affinity incl. matchFields, cordoned nodes) or of a
+    cluster with spread constraints sharing a key, with an empty and with a synthetic dynamic histogram:
+    simon_host_plan_fit_error == simulator.format_fit_error."""
+    if isinstance(seed, str):
+        cluster, apps = synth.make_same_key(seed_no=int(seed.rsplit("-", 1)[1]))
+    else:
+        cluster, apps = synth.make_mix(seed_no=seed, n_nodes=40, n_workloads=25, max_replicas=3)
     cluster.Nodes[3].setdefault("spec", {})["unschedulable"] = True
     names = [n["metadata"]["name"] for n in cluster.Nodes]
     base = {"containers": [{"name": "c", "image": "x", "resources": {"requests": {"cpu": "100m"}}}]}

@@ -9,7 +9,7 @@ from simon_b200.compiler import compile_cluster
 
 
 def make_case(kind="c3", **kw):
-    cluster, apps = {"c3": synth.make_c3, "c2": synth.make_c2, "mix": synth.make_mix}[kind](**kw)
+    cluster, apps = {"c3": synth.make_c3, "c2": synth.make_c2, "mix": synth.make_mix, "same_key": synth.make_same_key}[kind](**kw)
     p = simulator.plan(cluster, apps)
     c = compile_cluster(p.nodes, p.pods, p.ctx)
     return p, c
@@ -61,6 +61,63 @@ def run_pyref(p, c):
     ref = PyRef(c.node_objs, services=p.ctx.services, replicasets=p.ctx.replicasets, statefulsets=p.ctx.statefulsets,
                 creation_order=c.node_orig_index)
     return np.array(ref.run([x.tmpl.pod for x in p.pods], [x.node_name for x in p.pods]), dtype=np.int32)
+
+
+def _sfc_of(reason: str, scalar_names) -> int:
+    from simon_b200 import abi
+    fixed = {"static": abi.SFC_STATIC, "ports": abi.SFC_PORTS, "Too many pods": abi.SFC_TOO_MANY_PODS, "Insufficient cpu": abi.SFC_CPU,
+             "Insufficient memory": abi.SFC_MEM, "Insufficient ephemeral-storage": abi.SFC_EPH, "pts-missing": abi.SFC_PTS_MISSING,
+             "pts-skew": abi.SFC_PTS_SKEW, "ipa-aff": abi.SFC_IPA_AFF, "ipa-anti": abi.SFC_IPA_ANTI, "ipa-exist": abi.SFC_IPA_EXIST,
+             "gpu": abi.SFC_GPU}
+    if reason in fixed:
+        return fixed[reason]
+    assert reason.startswith("Insufficient "), reason
+    return abi.SFC_SCALAR0 + list(scalar_names).index(reason[len("Insufficient "):])
+
+
+def pyref_walk(p, c):
+    """PyRef.schedule_one pod by pod, as PyRef.run commits: -> (node [P], winning total [P], feasible node count [P], failure
+    histogram [P][N_FAIL_CODES] in simon_fail_code columns).  Pods bound by spec.nodeName get their node, total 0 and no failure."""
+    from oracle.pyref import PyRef
+    from simon_b200 import abi
+    ref = PyRef(c.node_objs, services=p.ctx.services, replicasets=p.ctx.replicasets, statefulsets=p.ctx.statefulsets,
+                creation_order=c.node_orig_index)
+    P = len(p.pods)
+    node, total, feas = np.full(P, -1, np.int32), np.zeros(P, np.int64), np.zeros(P, np.int64)
+    hist = np.zeros((P, abi.N_FAIL_CODES), np.uint32)
+    for i, rec in enumerate(p.pods):
+        pod = rec.tmpl.pod
+        if rec.node_name:
+            ns = ref.by_name.get(rec.node_name)
+            if ns is None:
+                node[i] = -2
+            else:
+                ref.commit(pod, ns, reserve_gpu=False)
+                node[i] = ref.nodes.index(ns)
+            continue
+        detail: dict = {}
+        idx, best, h = ref.schedule_one(pod, detail)
+        node[i], feas[i] = idx, len(detail)
+        if idx >= 0:
+            total[i] = best
+            ref.commit(pod, ref.nodes[idx])
+        for reason, n in h.items():
+            hist[i, _sfc_of(reason, c.scalar_names)] += n
+    return node, total, feas, hist
+
+
+def assert_matches_walk(walk, out, score, fail_counts, fail_pod, what=""):
+    """A run's nodes, winning totals (pods with one feasible node are not scored: the engine and the oracle record 0) and per-pod
+    failure histograms equal pyref_walk's."""
+    node, total, feas, hist = walk
+    bad = np.nonzero(out != node)[0]
+    assert len(bad) == 0, f"{what}: {len(bad)} placements differ, first pods {bad[:6]}: got {out[bad[:6]]} pyref {node[bad[:6]]}"
+    scored = (node >= 0) & (feas > 1)
+    bad = np.nonzero(scored & (score != total))[0]
+    assert len(bad) == 0, f"{what}: totals differ at pods {bad[:6]}: got {score[bad[:6]]} pyref {total[bad[:6]]}"
+    failed = np.nonzero(node == -1)[0]
+    np.testing.assert_array_equal(np.asarray(fail_pod), failed, err_msg=f"{what}: failing pods")
+    np.testing.assert_array_equal(np.asarray(fail_counts), hist[failed], err_msg=f"{what}: failure histograms")
 
 
 class CompiledArrays:
