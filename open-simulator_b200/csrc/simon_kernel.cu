@@ -402,6 +402,18 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
         A32(B_OWN, idx) = own;
     };
 
+    // the Open-Local and GPU-share filters of one node (classes with CLS_LOCAL / SK_CLS_GPU); returns the reason bit or 0
+    auto device_filter = [&](uint32_t idx) -> uint32_t {
+        uint32_t g = (uint32_t)A32(B_NODE_G, idx);
+        if ((C.cflags & CLS_LOCAL) && sk_slice(P.local_raw, P.node_stride)[g] < 0) return 1u << SFC_LOCAL;
+        if (C.cflags & SK_CLS_GPU) {
+            int slots[64];
+            int64_t total = P.gpu_total_mem ? P.gpu_total_mem[g] : 0;
+            if (total < cw[SCW_GPU_MEM] || gpu_allocate(P, SC, cw[SCW_GPU_MEM], cw[SCW_GPU_COUNT], g, slots) == 0) return 1u << SFC_GPU;
+        }
+        return 0;
+    };
+
     // filters on cached state; returns the reason bitmask (0 = feasible). hard_min: global minima of hard constraints.
     auto filter_node = [&](uint32_t idx, uint8_t nf, const int32_t *hard_min, bool want_reasons) -> uint32_t {
         if (nf & NF_STATIC_FAIL) return 1u << SFC_STATIC;
@@ -454,16 +466,66 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
         #pragma unroll 1
         for (uint32_t e = C.e_exist; e < C.e_isc; e++)
             if (DOM(ENT(ER_T, e), idx) >= 0 && VAL(e, idx) > 0) return 1u << SFC_IPA_EXIST;
-        if (C.cflags & (CLS_LOCAL | SK_CLS_GPU)) {
-            uint32_t g = (uint32_t)A32(B_NODE_G, idx);
-            if ((C.cflags & CLS_LOCAL) && sk_slice(P.local_raw, P.node_stride)[g] < 0) return 1u << SFC_LOCAL;
-            if (C.cflags & SK_CLS_GPU) {
-                int slots[64];
-                int64_t total = P.gpu_total_mem ? P.gpu_total_mem[g] : 0;
-                if (total < cw[SCW_GPU_MEM] || gpu_allocate(P, SC, cw[SCW_GPU_MEM], cw[SCW_GPU_COUNT], g, slots) == 0) return 1u << SFC_GPU;
+        return (C.cflags & (CLS_LOCAL | SK_CLS_GPU)) ? device_filter(idx) : 0u;
+    };
+
+    // filter_node's verdict (feasible or not) of every slot of this thread at once, for the unrolled-slot variants: bit s is
+    // set when slot s is valid and passes every filter.  Entry outside, slots inside: an entry's row is read once and the
+    // shared-memory loads of all slots issue back to back.  Feasibility is the AND of the filters, so the order they are
+    // evaluated in does not change it; the first failure reason comes from filter_node alone.
+    auto filter_slots = [&](const int32_t *hard_min) -> uint32_t {
+        uint32_t ok = 0;
+#pragma unroll
+        for (uint32_t s = 0; s < (uint32_t)NPT_T; s++)
+            if ((A8(C_NFLAGS, s * TPB + tid) & (NF_VALID | NF_STATIC_FAIL | NF_FIT_OK)) == (NF_VALID | NF_FIT_OK)) ok |= 1u << s;
+        #pragma unroll 1
+        for (uint32_t e = 0; e < C.n_ports && ok; e++)
+#pragma unroll
+            for (uint32_t s = 0; s < (uint32_t)NPT_T; s++)
+                if (VAL(e, s * TPB + tid) > 0) ok &= ~(1u << s);
+        #pragma unroll 1
+        for (uint32_t jh = 0; jh < C.n_hard && ok; jh++) {
+            const uint32_t e = C.e_hard + jh;
+            const int32_t t = ENT(ER_T, e);
+            const int64_t b = (int64_t)ENT(ER_B, e) - (int64_t)hard_min[jh], a = ENT(ER_A, e);
+#pragma unroll
+            for (uint32_t s = 0; s < (uint32_t)NPT_T; s++) {
+                const uint32_t idx = s * TPB + tid;
+                int64_t match = (A8(C_REGBITS, idx) >> jh) & 1 ? VAL(e, idx) : 0;
+                if (DOM(t, idx) < 0 || match + b > a) ok &= ~(1u << s);
             }
         }
-        return 0;
+        if (C.n_aff && ok) {
+            uint32_t missing = 0, pods_exist = ok;
+            #pragma unroll 1
+            for (uint32_t e = C.e_aff; e < C.e_anti; e++) {
+                const int32_t t = ENT(ER_T, e);
+#pragma unroll
+                for (uint32_t s = 0; s < (uint32_t)NPT_T; s++) {
+                    const uint32_t idx = s * TPB + tid;
+                    if (DOM(t, idx) < 0) missing |= 1u << s;
+                    if (VAL(e, idx) <= 0) pods_exist &= ~(1u << s);
+                }
+            }
+            ok &= ~missing;
+            if (!(C.aff_total == 0 && (C.cflags & SIMON_CLS_IPA_SELF_MATCH))) ok &= pods_exist;
+        }
+        // required anti-affinity of the pod, then that of the pods already placed
+        #pragma unroll 1
+        for (uint32_t e = C.e_anti; e < C.e_isc && ok; e++) {
+            const int32_t t = ENT(ER_T, e);
+#pragma unroll
+            for (uint32_t s = 0; s < (uint32_t)NPT_T; s++) {
+                const uint32_t idx = s * TPB + tid;
+                if (DOM(t, idx) >= 0 && VAL(e, idx) > 0) ok &= ~(1u << s);
+            }
+        }
+        if (C.cflags & (CLS_LOCAL | SK_CLS_GPU)) {
+#pragma unroll
+            for (uint32_t s = 0; s < (uint32_t)NPT_T; s++)
+                if (((ok >> s) & 1) && device_filter(s * TPB + tid)) ok &= ~(1u << s);
+        }
+        return ok;
     };
 
     // PodTopologySpread raw scores with the current weights (scoring.go:175-208); returns local (min, max) encoded
@@ -476,18 +538,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
         lo = sk_enc(INT64_MAX);
         hi = sk_enc(0);
         if (C.n_soft == 0) return;
-        #pragma unroll (NPT_T > 0 ? NPT_T : 1)
-        for (uint32_t s = 0; s < NPT; s++) {
-            uint32_t idx = s * TPB + tid;
-            uint8_t nf = A8(C_NFLAGS, idx);
-            if ((nf & (NF_FEASIBLE | NF_IGNORED)) != NF_FEASIBLE) continue;
-            double score = 0.0;
-            #pragma unroll 1
-            for (uint32_t js = 0; js < C.n_soft; js++) {
-                uint32_t e = C.e_soft + js;
-                double sfc = (double)VAL(e, idx) * S.soft_w[js] + (double)(ENT(ER_A, e) - 1);
-                score = score + sfc;
-            }
+        auto pts_node = [&](uint32_t idx, double score) {
             // 0 <= score < 2^35: counts x ln(size) + (maxSkew - 1), maxSkew up to 2^31 - 1.  B_RAW_PTS holds the truncated score
             // less the class constant pts_off = sum(maxSkew - 1): exact, and it fits int32 because the compilers bound the counts
             // part (pods x soft constraints x ln(nodes + 2) < 2^31 - 2).  P3 adds pts_off back in int64.
@@ -496,6 +547,45 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             unsigned long long er = sk_enc(raw);
             lo = er < lo ? er : lo;
             hi = er > hi ? er : hi;
+        };
+        if constexpr (NPT_T > 0 && NPT_T % 2 == 0) {
+            // 2 and 4 unrolled slots: constraint outside, a pair of slots inside (a weight and a row are read once per
+            // constraint and pair).  Each slot's sum is taken in constraint order, as in the slot-outer loop below, so every
+            // node's score is the same double.  At 3 slots this form spills, so odd slot counts keep the slot-outer loop.
+#pragma unroll
+            for (uint32_t s0 = 0; s0 < (uint32_t)NPT_T; s0 += 2) {
+                double sc[2] = {0.0, 0.0};
+                #pragma unroll 1
+                for (uint32_t js = 0; js < C.n_soft; js++) {
+                    const uint32_t e = C.e_soft + js;
+                    const double w = S.soft_w[js], a = (double)(ENT(ER_A, e) - 1);
+#pragma unroll
+                    for (uint32_t u = 0; u < 2; u++) {
+                        double sfc = (double)VAL(e, (s0 + u) * TPB + tid) * w + a;
+                        sc[u] = sc[u] + sfc;
+                    }
+                }
+#pragma unroll
+                for (uint32_t u = 0; u < 2; u++) {
+                    const uint32_t idx = (s0 + u) * TPB + tid;
+                    if ((A8(C_NFLAGS, idx) & (NF_FEASIBLE | NF_IGNORED)) == NF_FEASIBLE) pts_node(idx, sc[u]);
+                }
+            }
+        } else {
+            #pragma unroll (NPT_T > 0 ? NPT_T : 1)
+            for (uint32_t s = 0; s < NPT; s++) {
+                uint32_t idx = s * TPB + tid;
+                uint8_t nf = A8(C_NFLAGS, idx);
+                if ((nf & (NF_FEASIBLE | NF_IGNORED)) != NF_FEASIBLE) continue;
+                double score = 0.0;
+                #pragma unroll 1
+                for (uint32_t js = 0; js < C.n_soft; js++) {
+                    uint32_t e = C.e_soft + js;
+                    double sfc = (double)VAL(e, idx) * S.soft_w[js] + (double)(ENT(ER_A, e) - 1);
+                    score = score + sfc;
+                }
+                pts_node(idx, score);
+            }
         }
     };
 
@@ -1056,12 +1146,14 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
         uint32_t my_nf = 0;
         int32_t my_dc = 0;                  // net change of the counted (feasible, not ignored) set seen by this thread
         int64_t ipa_lo = 0, ipa_hi = 0;     // min/max of raw InterPodAffinity scores (initialised to 0: scoring.go:255)
+        uint32_t feas_mask = 0;
+        if constexpr (NPT_T > 0) feas_mask = filter_slots(hard_min);
         #pragma unroll (NPT_T > 0 ? NPT_T : 1)
         for (uint32_t s = 0; s < NPT; s++) {
             uint32_t idx = s * TPB + tid;
             uint8_t nf = A8(C_NFLAGS, idx);
             if (!(nf & NF_VALID)) continue;
-            bool feas = filter_node(idx, nf, hard_min, false) == 0;
+            bool feas = NPT_T > 0 ? ((feas_mask >> s) & 1) != 0 : filter_node(idx, nf, hard_min, false) == 0;
             if (feas != ((nf & NF_FEASIBLE) != 0)) {
                 my_fl |= 1u; my_nf++;
                 if (!feas && s * CT + gtid == last_win_r)
