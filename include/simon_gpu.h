@@ -563,9 +563,11 @@ typedef struct simon_scenario_local_result {
 } simon_scenario_local_result;
 int simon_scenarios_run_local(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, simon_scenario_result *out,
                               simon_scenario_local_result *out_local, int32_t *out_node);
-/* Scenario `scenario` of the last simon_scenarios_run_local batch: its final VG requested [V][N] and, if dev_alloc is not NULL, its
- * allocated device slots [N] (SIMON_ERR_STATE without a simon_devices_upload); node-indexed like the snapshot, inactive nodes keep
- * the uploaded values.  SIMON_ERR_STATE if no such batch ran since the last snapshot, pod, storage or device upload. */
+/* Scenario `scenario` of the last simon_scenarios_run_local or simon_drain_run_local batch: its final VG requested [V][N] and, if
+ * dev_alloc is not NULL, its allocated device slots [N] (SIMON_ERR_STATE without a simon_devices_upload); node-indexed like the
+ * snapshot.  Inactive nodes keep the values the scenario started from: the uploaded ones in a scenario batch, the live ones (the
+ * state `placed` leaves) on a drain's removed nodes.  SIMON_ERR_STATE if no such batch ran since the last snapshot, pod, storage or
+ * device upload, or if a simon_drain_run batch ran after it (it reuses the batch pool). */
 int simon_scenarios_storage_download(simon_ctx *ctx, uint32_t scenario, int64_t *vg_requested, uint32_t *dev_alloc);
 
 /* ---- node drains and cluster scale-down (the reference's third use case, README.md:16 "Pods Migration: scaling down cluster,
@@ -592,8 +594,8 @@ int simon_scenarios_storage_download(simon_ctx *ctx, uint32_t scenario, int64_t 
  * each scenario places its own evicted pods.  out[i] holds drain i's counts and the sums over its remaining nodes after the placement
  * (satisfyResourceSetting's inputs, as simon_scenario_result).  With Open-Local storage uploaded the same kernels run: evicted pods have
  * no volumes, and a class without volumes scores 0 and passes Open-Local's filter everywhere.  The batch pool is reused, so
- * simon_scenarios_storage_download refuses after a drain batch.  simon_last_kernel_ms is the device time of setup + placement,
- * simon_drain_times splits it.
+ * simon_scenarios_storage_download refuses after a simon_drain_run batch.  simon_last_kernel_ms is the device time of setup +
+ * placement, simon_drain_times splits it.
  * SIMON_ERR_INVALID with a message, before any device work: `placed` fails the resume prefix checks, a drain leaves no node, lists a node
  * twice or a node out of range.  Not all pods placed (-1 entries) is not an error. */
 typedef struct simon_drain_result {
@@ -607,6 +609,24 @@ typedef struct simon_drain_result {
     int64_t req_mem, alloc_mem;
 } simon_drain_result;
 int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario *remain, uint32_t n, simon_drain_result *out);
+/* simon_drain_run_local: drains on a cluster with Open-Local storage that move the pods with local volumes instead of being blocked by
+ * them (an opt-in; simon_drain_run keeps blocking them).  After a simon_storage_upload (else SIMON_ERR_STATE); simon_devices_upload is
+ * optional.  Everything above holds, except that a pod of a class with Open-Local volumes (simon_storage.class_local) on a removed node
+ * is evicted, not blocked, unless it is bound by spec.nodeName: it is placed again with the other evicted pods, in pod-list order,
+ * through the full path including Open-Local's Filter, Score and Bind (LVM volumes and, with devices uploaded, exclusive devices) on
+ * the remaining nodes.  Its volumes are provisioned again on the new node at the same sizes; their data is not carried over, and the
+ * removed node's VGs and devices go away with the node.  This answers whether the volumes fit elsewhere, not how to migrate data.
+ * Each scenario starts from the live VG requested values and device masks (the state `placed` leaves, as the resume's rebuild
+ * replays Bind), so the equivalence above holds with storage: the cluster compiled without D with Open-Local storage (and devices
+ * when they are uploaded), resumed the same way, gives the same nodes, GPU slots, final VG requested and device masks on every
+ * remaining node.  With a PDB table, evicted pods with volumes count against their PDBs like any other evicted pod.
+ * out_local[i] holds drain i's Open-Local sums after the placement, as simon_scenarios_run_local's: VG requested and VG capacity over
+ * the remaining nodes that carry the simon/node-local-storage annotation (satisfyResourceSetting's MaxVG input,
+ * pkg/apply/apply.go:746-772).  simon_drain_download, simon_drain_pdb_download and simon_drain_times serve the batch as they serve
+ * simon_drain_run's, and simon_scenarios_storage_download gives each drain's final VG requested and device masks.
+ * SIMON_ERR_INVALID for a NULL out_local; the other refusals are simon_drain_run's. */
+int simon_drain_run_local(simon_ctx *ctx, const int32_t *placed, const simon_scenario *remain, uint32_t n, simon_drain_result *out,
+                          simon_scenario_local_result *out_local);
 /* Drain `scenario` of the last simon_drain_run batch, each pointer may be NULL: its evicted pods in pod order [n_evicted], the node each
  * landed on or -1, its GPU-share slots (simon_gpu_slots_download's format), its winning total score (0 without SIMON_OPT_RECORD_SCORES
  * or with a single feasible node); its blocked pods [n_blocked]; and the failure histogram [n_unscheduled][SIMON_N_FAIL_CODES] and pod

@@ -535,6 +535,10 @@ void fill_params(simon_ctx *ctx, const ScenPool &s, SkParams &P) {
 #define SIMON_AUTO_TPB 320u
 
 typedef void (*sk_kernel_fn)(const SkParams);
+// The kernel family a launch runs, an argument of kernel_variant / max_active_clusters / choose_geometry / launch (never context
+// state, so no other call can launch a drain kernel): the placement variants (the local ones with storage uploaded), the drain-batch
+// variants without Open-Local code (simon_drain_run), or those with it (simon_drain_run_local)
+enum Family { PLACE, DRAIN, DRAIN_LOCAL };
 struct sk_variant { sk_kernel_fn fn; const char *name; uint32_t threads, slots; bool prof, big, local, drain; };
 #define SK_VARIANT_ENTRY(name, threads, slots, prof, big, local, drain) {name, #name, threads, slots, prof, big, local, drain},
 const sk_variant sk_variants[] = {SIMON_PLACE_VARIANTS(SK_VARIANT_ENTRY)};
@@ -543,12 +547,14 @@ const sk_variant sk_variants[] = {SIMON_PLACE_VARIANTS(SK_VARIANT_ENTRY)};
 // The compiled kernel variant for (threads per CTA, node slots per thread) on the context's uploads, which is what launch() runs
 // and what the geometry is sized for: the one of the fewest threads that holds TPB, with the unrolled loop for npt slots where
 // there is one and run-time slots otherwise.  big: the large-cluster variant, at any thread count; prof: with per-phase timers
-// (256 and 320 threads only).  With Open-Local storage uploaded, the local variants (no timers).  drain: the drain-batch
-// variants (simon_drain_run), whatever was uploaded.  big and drain ignore prof.  nullptr: none.
-const sk_variant *kernel_variant(const simon_ctx *ctx, uint32_t TPB, uint32_t npt, bool big, bool prof, bool drain) {
+// (256 and 320 threads only).  PLACE: with Open-Local storage uploaded, the local variants (no timers).  DRAIN: the drain-batch
+// variants without Open-Local code (simon_drain_run), whatever was uploaded; DRAIN_LOCAL: those with it (simon_drain_run_local).  big
+// and the drain families ignore prof.  nullptr: none.
+const sk_variant *kernel_variant(const simon_ctx *ctx, uint32_t TPB, uint32_t npt, bool big, bool prof, Family fam) {
     if (!big && TPB > SIMON_MAX_TPB) return nullptr;
     const uint32_t threads = TPB <= 256 ? 256 : TPB <= 320 ? 320 : 384;
-    const bool local = ctx->valid.has(STORAGE) && !drain;
+    const bool drain = fam != PLACE;
+    const bool local = fam == DRAIN_LOCAL || (fam == PLACE && ctx->valid.has(STORAGE));
     if (big || drain) prof = false;
     const sk_variant *runtime_slots = nullptr;
     for (const sk_variant &v : sk_variants) {
@@ -580,8 +586,8 @@ cudaError_t cluster_config(sk_kernel_fn fn, uint32_t ctas, uint32_t cs, uint32_t
 // Clusters of `cs` CTAs x `t` threads x `npt` node slots with `smem` bytes each of the variant for that shape that the device
 // holds at once, GPC boundaries included (0: not even one; a 16-CTA cluster needs 16 free SMs in one GPC).  The variants with
 // phase timers run in the geometry of the default ones.
-int max_active_clusters(const simon_ctx *ctx, bool big, uint32_t cs, uint32_t t, uint32_t npt, size_t smem, bool drain) {
-    const sk_variant *v = kernel_variant(ctx, t, npt, big, false, drain);
+int max_active_clusters(const simon_ctx *ctx, bool big, uint32_t cs, uint32_t t, uint32_t npt, size_t smem, Family fam) {
+    const sk_variant *v = kernel_variant(ctx, t, npt, big, false, fam);
     if (!v) return 0;
     cudaLaunchConfig_t cfg;
     cudaLaunchAttribute attr;
@@ -593,9 +599,9 @@ int max_active_clusters(const simon_ctx *ctx, bool big, uint32_t cs, uint32_t t,
     return n;
 }
 
-// choose cluster size / threads / nodes-per-thread for n_active nodes, for the variants launch(..., drain) runs
+// choose cluster size / threads / nodes-per-thread for n_active nodes, for the variants of family `fam` (what launch(..., fam) runs)
 int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &TPB, uint32_t &NPT, size_t &smem, uint32_t n_scen = 1,
-                    bool drain = false) {
+                    Family fam = PLACE) {
     int max_smem = 0;
     cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device);
     const uint32_t cs_opts[5] = {16, 8, 4, 2, 1};
@@ -641,7 +647,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
             if (npt > 64) continue;
             const size_t b = sk_smem_bytes(npt * t, ctx->snap.T, ctx->pods.emax, ctx->pods.max_blob_words, cs);
             if (b > (size_t)max_smem) continue;
-            const int active = max_active_clusters(ctx, false, cs, t, npt, b, drain);
+            const int active = max_active_clusters(ctx, false, cs, t, npt, b, fam);
             if (active <= 0) continue;
             const uint32_t waves = (n_scen + (uint32_t)active - 1) / (uint32_t)active;
             const double cost = waves * (265.0 + 196.0 * npt + (t > 320 ? 18.0 : 0.0) + 5.0 * cs);
@@ -669,7 +675,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
             if (n384 < npt_p) { t_p = 384; npt_p = n384; }
         }
         const size_t b = sk_smem_bytes(npt_p * t_p, ctx->snap.T, ctx->pods.emax, ctx->pods.max_blob_words, cs_p);
-        if (npt_p <= 64 && b <= (size_t)max_smem && max_active_clusters(ctx, false, cs_p, t_p, npt_p, b, drain) > 0) {
+        if (npt_p <= 64 && b <= (size_t)max_smem && max_active_clusters(ctx, false, cs_p, t_p, npt_p, b, fam) > 0) {
             CS = cs_p; TPB = t_p; NPT = npt_p; smem = b; return SIMON_OK;
         }
     }
@@ -690,7 +696,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
             }
             if (t > SIMON_MAX_TPB) return fail(ctx, SIMON_ERR_LIMIT, "threads per CTA must be <= %u (got %u)", SIMON_MAX_TPB, t);
             size_t b = sk_smem_bytes(npt * t, ctx->snap.T, ctx->pods.emax, ctx->pods.max_blob_words, cs);
-            if (b <= (size_t)max_smem && (want_cs || max_active_clusters(ctx, false, cs, t, npt, b, drain) > 0)) {
+            if (b <= (size_t)max_smem && (want_cs || max_active_clusters(ctx, false, cs, t, npt, b, fam) > 0)) {
                 CS = cs; TPB = t; NPT = npt; smem = b; return SIMON_OK;
             }
             if (want_t) break;
@@ -702,7 +708,7 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
         const uint32_t cs = 16, t = 320;
         const uint32_t npt = (n_active + cs * t - 1) / (cs * t);
         const size_t b = sk_smem_bytes(npt * t, ctx->snap.T, ctx->pods.emax, ctx->pods.max_blob_words, cs, false);
-        if (npt <= 64 && b <= (size_t)max_smem && max_active_clusters(ctx, true, cs, t, npt, b, drain) > 0) {
+        if (npt <= 64 && b <= (size_t)max_smem && max_active_clusters(ctx, true, cs, t, npt, b, fam) > 0) {
             CS = cs; TPB = t; NPT = npt; smem = b;
             ctx->big = true;
             ctx->gnode_stride = (sk_node_bytes(npt * t, ctx->snap.T, ctx->pods.emax) + 255) & ~(size_t)255;
@@ -714,15 +720,15 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
 
 static_assert(sizeof(SkScenario) % 8 == 0, "SkScenario is copied in 8-byte words");
 
-// drain: a drain-batch variant (P carries drain_pods / drain_off)
-int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t TPB, size_t smem, bool record = true, bool drain = false) {
+// fam DRAIN / DRAIN_LOCAL: a drain-batch variant (P carries drain_pods / drain_off)
+int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t TPB, size_t smem, bool record = true, Family fam = PLACE) {
     // SIMON_PROFILE=1 selects the variants with per-phase clock64 timers (simon_stats cycles); the default variants
     // carry no timers
     static const bool prof = getenv("SIMON_PROFILE") != nullptr;
-    const sk_variant *v = kernel_variant(ctx, TPB, P.npt, ctx->big, prof, drain);
+    const sk_variant *v = kernel_variant(ctx, TPB, P.npt, ctx->big, prof, fam);
     if (!v)
         return fail(ctx, SIMON_ERR_LIMIT, "no kernel variant for %u threads per CTA%s%s", TPB, prof ? " with phase timers" : "",
-                    ctx->valid.has(STORAGE) ? " and Open-Local storage" : "");
+                    (fam == DRAIN_LOCAL || (fam == PLACE && ctx->valid.has(STORAGE))) ? " and Open-Local storage" : "");
     if (ctx->big) {
         CU(ctx->d_gnode.alloc(ctx->gnode_stride * (size_t)n_scen * CS));
         P.gnode = ctx->d_gnode.p; P.gnode_stride = ctx->gnode_stride;
@@ -738,7 +744,7 @@ int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t T
     li = simon_launch_info{};
     snprintf(li.kernel, sizeof(li.kernel), "%s", v->name);
     li.n_nodes = ctx->geom_nodes; li.cluster_ctas = CS; li.threads_per_cta = TPB; li.node_slots = P.npt; li.n_scenarios = n_scen;
-    li.large = ctx->big; li.local = ctx->valid.has(STORAGE) && !drain; li.smem_bytes = smem;
+    li.large = ctx->big; li.local = v->local; li.smem_bytes = smem;
     return SIMON_OK;
 }
 
@@ -1383,7 +1389,8 @@ int simon_scenarios_run_local(simon_ctx *ctx, const simon_scenario *scen, uint32
 int simon_scenarios_storage_download(simon_ctx *ctx, uint32_t scenario, int64_t *vg_requested, uint32_t *dev_alloc) {
     if (!ctx) return SIMON_ERR_INVALID;
     const ScenPool &B = ctx->batch;
-    if (!ctx->valid.has(STORAGE_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_scenarios_run_local batch since the last upload");
+    if (!ctx->valid.has(STORAGE_BATCH))
+        return fail(ctx, SIMON_ERR_STATE, "no simon_scenarios_run_local or simon_drain_run_local batch since the last upload");
     if (scenario >= ctx->storage_batch.n) return fail(ctx, SIMON_ERR_INVALID, "scenario %u of a batch of %u", scenario, ctx->storage_batch.n);
     if (dev_alloc && !ctx->valid.has(DEVICES)) return fail(ctx, SIMON_ERR_STATE, "no devices uploaded");
     CU(cudaSetDevice(ctx->device));
@@ -1429,10 +1436,14 @@ extern "C" int simon_drain_budget(simon_ctx *ctx, uint64_t *scenario_bytes, uint
     return SIMON_OK;
 }
 
-extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario *remain, uint32_t n, simon_drain_result *out) {
-    if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_drain_run before uploads");
-    if ((ctx->pods.n_pods && !placed) || (n && (!remain || !out))) return fail(ctx, SIMON_ERR_INVALID, "simon_drain_run: NULL argument");
+// simon_drain_run and simon_drain_run_local (out_local != nullptr: pods with Open-Local volumes are evicted, not blocked, and each
+// scenario carries its own Open-Local state, the live one to start with)
+static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario *remain, uint32_t n, simon_drain_result *out,
+                     simon_scenario_local_result *out_local) {
+    const bool local = out_local != nullptr;
+    const char *what = local ? "simon_drain_run_local" : "simon_drain_run";
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "%s before uploads", what);
+    if ((ctx->pods.n_pods && !placed) || (n && (!remain || !out))) return fail(ctx, SIMON_ERR_INVALID, "%s: NULL argument", what);
     const uint32_t N = ctx->snap.N, N1 = std::max(1u, N), P = ctx->pods.n_pods;
     // ---- refusals before any device work: the live placement as a resume prefix checks it, then the node lists ----
     int rc = check_prefix(ctx, placed, P);
@@ -1449,8 +1460,8 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
     if (n == 0) return SIMON_OK;
     cudaStream_t st = ctx->stream;
     // ---- per scenario, from the pods each node holds (one CSR): the pods of its removed nodes in pod order, as (scenario, pod)
-    // pairs for the un-import, and split into vanished (DaemonSet pods of a removed node), blocked (bound by spec.nodeName or with
-    // Open-Local volumes) and evicted pods ----
+    // pairs for the un-import, and split into vanished (DaemonSet pods of a removed node), blocked (bound by spec.nodeName, or with
+    // Open-Local volumes unless local) and evicted pods ----
     std::vector<uint32_t> node_off(N1 + 1, 0u), node_pods;
     for (uint32_t q = 0; q < P; q++)
         if (placed[q] >= 0) node_off[placed[q] + 1]++;
@@ -1475,7 +1486,8 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
             pairs.push_back(make_uint2(i, q));
             const int32_t gd = ctx->pods.h_guard[q];
             if (gd >= 0 && rank[gd] < 0) n_vanished[i]++;
-            else if (ctx->pods.h_fixed[q] >= 0 || (ctx->valid.has(STORAGE) && ctx->storage.h_class_local[ctx->pods.h_class[q]])) ctx->drain.blocked.push_back(q);
+            else if (ctx->pods.h_fixed[q] >= 0 || (!local && ctx->valid.has(STORAGE) && ctx->storage.h_class_local[ctx->pods.h_class[q]]))
+                ctx->drain.blocked.push_back(q);
             else ctx->drain.pods.push_back(q);
         }
         ctx->drain.off.push_back((uint32_t)ctx->drain.pods.size());
@@ -1486,7 +1498,8 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
     // ---- geometry of the drain variant, the batch pool and the outputs (allocations before the timed work) ----
     uint32_t CS, TPB, NPT;
     size_t smem;
-    rc = choose_geometry(ctx, max_active, CS, TPB, NPT, smem, n, true);
+    const Family fam = local ? DRAIN_LOCAL : DRAIN;
+    rc = choose_geometry(ctx, max_active, CS, TPB, NPT, smem, n, fam);
     if (rc) return rc;
     rc = size_pool(ctx, B, n, false, false);
     if (rc) return rc;
@@ -1508,7 +1521,8 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
     // ---- setup: the live state in the single-scenario pool (the resume's rebuild, its failure records cleared as the resume clears
     // them), copied into every slot, minus what each scenario's removed nodes' pods contributed to the counters.  Of the batch pool
     // only what the copies do not overwrite is cleared: the per-class summaries and own-score caches, the counters and failure
-    // records ----
+    // records.  local: the live Open-Local state (the rebuild's Bind replay) is copied too; the removed nodes' VGs and devices stay as
+    // they are, since those nodes are inactive ----
     CU(cudaEventRecord(ctx->ev0, st));
     SkParams Ps;
     fill_params(ctx, S, Ps);
@@ -1523,6 +1537,11 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
     CU(cudaMemsetAsync(ctx->drain.d_fail_counts.p, 0, 4ull * n * ctx->drain.max * SIMON_N_FAIL_CODES, st));
     // every slot = the live state, one broadcast per column
     CU(B.state.each(S.state, true, [&](auto &b, auto &s, uint64_t k) { ctx->launches++; return bcast(ctx, s.p, k, n, b.p); }));
+    if (local) {
+        CU(bcast(ctx, S.vg_req.p, B.vn, n, B.vg_req.p));
+        ctx->launches++;
+        if (ctx->valid.has(DEVICES)) { CU(bcast(ctx, S.dev_alloc.p, B.nodes, n, B.dev_alloc.p)); ctx->launches++; }
+    }
     SkParams Pb;
     fill_params(ctx, B, Pb);
     if (!pairs.empty()) {
@@ -1535,11 +1554,16 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
     // ---- placement of every scenario's evicted pods ----
     Pb.drain_pods = ctx->drain.d_pods.p; Pb.drain_off = ctx->drain.d_off.p;
     Pb.first = 0; Pb.count = 0; Pb.max_fail = ctx->drain.max; Pb.npt = NPT;
-    rc = launch(ctx, Pb, n, CS, TPB, smem, false, true);
+    rc = launch(ctx, Pb, n, CS, TPB, smem, false, fam);
     if (rc) return rc;
     CU(cudaEventRecord(ctx->ev1, st));
     simon_scen_reduce<<<n, 256, 0, st>>>(B.scen.p, ctx->snap.d_alloc_mcpu.p, ctx->snap.d_alloc_mem.p, B.results.p);
     CU(cudaGetLastError());
+    if (local) {
+        simon_scen_reduce_local<<<n, 256, 0, st>>>(B.scen.p, ctx->storage.d_node_n_vg.p, ctx->storage.d_vg_cap.p, B.vg_req.p, B.vn, N, B.local_results.p);
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(out_local, B.local_results.p, sizeof(simon_scenario_local_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    }
     std::vector<simon_scenario_result> res(n);
     CU(cudaMemcpyAsync(res.data(), B.results.p, sizeof(simon_scenario_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
     // with a PDB table: `allowed` on the rebuilt live state, read at the same synchronisation
@@ -1587,7 +1611,24 @@ extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simo
     }
     ctx->drain.n = n;
     ctx->valid.set(DRAIN_BATCH);
+    if (local) {
+        ctx->storage_batch.n = n;           // simon_scenarios_storage_download serves this batch
+        ctx->valid.set(STORAGE_BATCH);
+    }
     return SIMON_OK;
+}
+
+extern "C" int simon_drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario *remain, uint32_t n, simon_drain_result *out) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    return drain_run(ctx, placed, remain, n, out, nullptr);
+}
+
+extern "C" int simon_drain_run_local(simon_ctx *ctx, const int32_t *placed, const simon_scenario *remain, uint32_t n, simon_drain_result *out,
+                                     simon_scenario_local_result *out_local) {
+    if (!ctx || !out_local) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_drain_run_local before uploads");
+    if (!ctx->valid.has(STORAGE)) return fail(ctx, SIMON_ERR_STATE, "simon_drain_run_local before simon_storage_upload");
+    return drain_run(ctx, placed, remain, n, out, out_local);
 }
 
 extern "C" int simon_drain_times(simon_ctx *ctx, float *setup_ms, float *place_ms) {

@@ -272,7 +272,9 @@ struct ClassState {
 // LOCAL: the variants launched when Open-Local storage was uploaded (simon_storage_upload); every other run uses variants whose
 // code has none of it
 // DRAIN: the drain-batch variants (simon_drain_run): each scenario places its own list of evicted pods (SkParams::drain_pods) on the
-// live state; an evicted pod is scheduler-placed and exists, so the pinned-run and bypass blocks are compiled out
+// live state; an evicted pod is scheduler-placed and exists, so the pinned-run and bypass blocks are compiled out.  LOCAL and DRAIN
+// together (simon_drain_run_local): the Open-Local code reads the pod's class only (never its index), and its VG / device / scratch
+// slices are the cluster's (sk_slice), which is the drain's scenario: a drain launch has one cluster per scenario, as a batch does
 template <int MAXT, int NPT_T, bool PROF, bool BIG = false, bool LOCAL = false, bool DRAIN = false>
 __device__ __forceinline__ void simon_place_body(const SkParams &P) {
     constexpr uint32_t CLS_LOCAL = LOCAL ? SK_CLS_LOCAL : 0u;
@@ -1785,8 +1787,9 @@ extern "C" __global__ void __launch_bounds__(256) simon_drain_unimport(const __g
 //     where the nodes of a CTA fall between the two (scenario batches on 9-CTA clusters: 3 slots instead of 4).  No timers.
 //   - The large-cluster variants keep per-node arrays in global memory.
 //   - Open-Local: one variant per thread count (run-time slots) and a large-cluster one.
-//   - Drain batches (per-scenario pod lists): the same, with no Open-Local code (an evicted pod has no local volumes: such pods
-//     block a drain).
+//   - Drain batches (per-scenario pod lists): the same, with no Open-Local code (by default a pod with local volumes blocks a drain,
+//     so no evicted pod has any).
+//   - Drain batches that evict pods with Open-Local volumes (simon_drain_run_local): the same again, with the Open-Local code.
 #define SIMON_PLACE_VARIANTS(X)                                       \
     X(simon_place_kernel_256_0,  256, 0, false, false, false, false)  \
     X(simon_place_kernel_256_1,  256, 1, false, false, false, false)  \
@@ -1820,7 +1823,11 @@ extern "C" __global__ void __launch_bounds__(256) simon_drain_unimport(const __g
     X(simon_drain_kernel_256,    256, 0, false, false, false, true)   \
     X(simon_drain_kernel_320,    320, 0, false, false, false, true)   \
     X(simon_drain_kernel_384,    384, 0, false, false, false, true)   \
-    X(simon_drain_kernel_big,    320, 0, false, true,  false, true)
+    X(simon_drain_kernel_big,    320, 0, false, true,  false, true)   \
+    X(simon_drain_local_kernel_256, 256, 0, false, false, true, true)  \
+    X(simon_drain_local_kernel_320, 320, 0, false, false, true, true)  \
+    X(simon_drain_local_kernel_384, 384, 0, false, false, true, true)  \
+    X(simon_drain_local_kernel_big, 320, 0, false, true,  true, true)
 
 #define SK_DEFINE_VARIANT(name, threads, slots, prof, big, local, drain)                                   \
     extern "C" __global__ void __launch_bounds__(threads, 1) name(const __grid_constant__ SkParams P) { \

@@ -252,6 +252,7 @@ SIGNATURES = {
     "simon_scenarios_run_local": (_I, [_P, _P, _U32, _P, _P, _P]),
     "simon_scenarios_storage_download": (_I, [_P, _U32, _P, _P]),
     "simon_drain_run": (_I, [_P, _P, _P, _U32, _P]),
+    "simon_drain_run_local": (_I, [_P, _P, _P, _U32, _P, _P]),
     "simon_drain_download": (_I, [_P, _U32] + [_P] * 7),
     "simon_drain_pdb_download": (_I, [_P, _U32, _P, _P]),
     "simon_drain_times": (_I, [_P, _PF, _PF]),

@@ -334,8 +334,9 @@ class Engine:
         return out, out_node
 
     def scenario_storage_state(self, i: int):
-        """Scenario i of the last run_scenarios_local batch: (VG requested [V][N], allocated device slot masks [N] or None without
-        devices), node-indexed like the snapshot."""
+        """Scenario i of the last run_scenarios_local batch, or drain i of the last batch (chunk) of the last
+        drain_run(..., local=True): (VG requested [V][N], allocated device slot masks [N] or None without devices), node-indexed like
+        the snapshot.  A drain's removed nodes keep their live values."""
         V, N = self.c.storage.n_vgs, self.c.n_nodes
         vg = np.zeros(max(V * N, 1), np.int64)
         dev = np.zeros(max(N, 1), np.uint32) if self.c.storage.devices else None
@@ -371,7 +372,7 @@ class Engine:
         self._check(lib().simon_drain_budget(self.h, C.byref(per), C.byref(free)))
         return int(per.value), int(free.value)
 
-    def drain_run(self, placed, remain_lists: List[np.ndarray], detail: bool = True, chunk: Optional[int] = None):
+    def drain_run(self, placed, remain_lists: List[np.ndarray], detail: bool = True, chunk: Optional[int] = None, local: bool = False):
         """Drains on the live state `placed` (out_node of a full placement of the pod list): each entry of remain_lists lists the
         nodes that remain, in their nodeTree.list() order.  The list runs in batches (chunks) sized so that one batch's pooled state
         fits the device: chunk scenarios of simon_drain_budget's per-scenario bytes in DRAIN_MEM_FRACTION of what it reports free
@@ -379,7 +380,11 @@ class Engine:
         the sums req_mcpu / alloc_mcpu / req_mem / alloc_mem over the remaining nodes, and n_pdb_violated (with a PDB table); with
         detail also evicted (pod indices in pod order), node (per evicted pod, -1 unschedulable), gpu_slots, score, blocked,
         fail_counts [n_unscheduled][24], fail_pod, and pdb_violated / pdb_evicted (the violated PDBs ascending, their evicted
-        members).  self.last_drain: chunks, scenario_bytes, setup_ms / place_ms (device time summed over the batches)."""
+        members).  self.last_drain: chunks, scenario_bytes, setup_ms / place_ms (device time summed over the batches).
+        local=True (a cluster compiled with open_local=True): simon_drain_run_local, so pods with Open-Local volumes are evicted and
+        provisioned again on the remaining nodes instead of blocking the drain, and every result also carries vg_requested /
+        vg_capacity, the VG sums over the remaining annotated nodes after the placement (satisfyResourceSetting's MaxVG input);
+        scenario_storage_state(i) then describes drain i of the last chunk."""
         L = lib()
         pl = np.ascontiguousarray(placed, dtype=np.int32)
         n = len(remain_lists)
@@ -393,7 +398,11 @@ class Engine:
             m = len(part)
             arr, keep = self._scenario_array(part)
             res = (abi.SimonDrainResult * m)()
-            self._check(L.simon_drain_run(self.h, pl.ctypes.data, arr, m, res))
+            if local:
+                loc = (abi.SimonScenarioLocalResult * m)()
+                self._check(L.simon_drain_run_local(self.h, pl.ctypes.data, arr, m, res, loc))
+            else:
+                self._check(L.simon_drain_run(self.h, pl.ctypes.data, arr, m, res))
             su, pm = C.c_float(0), C.c_float(0)
             self._check(L.simon_drain_times(self.h, C.byref(su), C.byref(pm)))
             info["chunks"] += 1
@@ -404,6 +413,8 @@ class Engine:
                 d = dict(n_evicted=r.n_evicted, n_placed=r.n_placed, n_unscheduled=r.n_unscheduled, n_blocked=r.n_blocked,
                          n_vanished=r.n_vanished, n_pdb_violated=r.n_pdb_violated, req_mcpu=r.req_mcpu, alloc_mcpu=r.alloc_mcpu,
                          req_mem=r.req_mem, alloc_mem=r.alloc_mem)
+                if local:
+                    d["vg_requested"], d["vg_capacity"] = int(loc[i].vg_requested), int(loc[i].vg_capacity)
                 if detail:
                     ne, nb, nf = r.n_evicted, r.n_blocked, r.n_unscheduled
                     ev = np.zeros(max(ne, 1), np.uint32)

@@ -11,9 +11,16 @@ simon_drain_run):
     (disruption.py, Engine.pdbs_upload), it evicts no more members of any PDB than the PDB allows on the live state.  Vanished and
     blocked pods do not count against a PDB.  The result is the end state, not an eviction sequence.
 
+With local volumes (local_volumes=True, on a cluster compiled with open_local=True; Engine.drain_run(..., local=True)) pods with
+Open-Local volumes are evicted instead of blocking: they are placed again with the other evicted pods, through Open-Local's Filter,
+Score and Bind on the remaining nodes, and their volumes are provisioned again there at the same sizes.  Their data is not carried
+over, and the removed nodes' VGs and devices go with them: this answers whether the volumes fit elsewhere, not how to move the data.
+Such drains also carry the VG sums of the remaining annotated nodes, and the MaxVG cap applies to them.
+
 ScaleDownPlan sweeps every candidate node alone, orders the drainable ones by utilisation and removes the longest prefix of that order
-whose every prefix drains and meets the satisfyResourceSetting caps (MaxCPU / MaxMemory).  With PDBs a prefix that violates one does
-not drain, so the first such prefix ends the plan, and the sweep marks such single-node drains not drainable.
+whose every prefix drains and meets the satisfyResourceSetting caps (MaxCPU / MaxMemory, and MaxVG for drains with VG sums).  With
+PDBs a prefix that violates one does not drain, so the first such prefix ends the plan, and the sweep marks such single-node drains
+not drainable.
 """
 from __future__ import annotations
 
@@ -23,7 +30,7 @@ from typing import Callable, Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import abi
-from .capacity import env_caps, occupancy_ok
+from .capacity import env_caps, env_vg_cap, occupancy_ok
 from .compiler import SCW_GUARD_NODE, SCW_REQ_MCPU, SCW_REQ_MEM, Compiled, get_zone_key
 from .objects import AppResource, ResourceTypes
 from .workloads import PodRec
@@ -144,8 +151,10 @@ def pod_guard(compiled: Compiled) -> np.ndarray:
     return g
 
 
-def classify(compiled: Compiled, placed: np.ndarray, removed: Sequence[int]) -> Tuple[List[int], List[Tuple[int, str]], List[int]]:
-    """The pods of the removed nodes in pod order: (evicted, blocked as (pod, reason), vanished)."""
+def classify(compiled: Compiled, placed: np.ndarray, removed: Sequence[int], local_volumes: bool = False
+             ) -> Tuple[List[int], List[Tuple[int, str]], List[int]]:
+    """The pods of the removed nodes in pod order: (evicted, blocked as (pod, reason), vanished).  local_volumes: pods with
+    Open-Local volumes are evicted instead of blocked (Engine.drain_run(..., local=True))."""
     placed = np.asarray(placed)
     rm = np.zeros(compiled.n_nodes, bool)
     rm[np.asarray(list(removed), dtype=np.int64)] = True
@@ -159,7 +168,7 @@ def classify(compiled: Compiled, placed: np.ndarray, removed: Sequence[int]) -> 
             va.append(q)
         elif fixed[q] >= 0:
             bl.append((q, BLOCK_NODE_NAME))
-        elif local is not None and local[int(cls[q])]:
+        elif local is not None and local[int(cls[q])] and not local_volumes:
             bl.append((q, BLOCK_LOCAL_STORAGE))
         else:
             ev.append(q)
@@ -200,9 +209,10 @@ def drainable(r: dict) -> bool:
 
 def drain_results(compiled: Compiled, placed: np.ndarray, removed_lists: Sequence[Sequence[int]], remain_lists: Sequence[np.ndarray],
                   raw: Sequence[dict], max_cpu: Optional[int] = None, max_mem: Optional[int] = None, pdbs=None,
-                  allowed: Optional[np.ndarray] = None) -> List[DrainResult]:
+                  allowed: Optional[np.ndarray] = None, max_vg: Optional[int] = None) -> List[DrainResult]:
     """DrainResult per drain from Engine.drain_run(..., detail=True) results; pdbs (disruption.PdbTables) and allowed
-    (Engine.pdbs_allowed on the live state) name the violated PDBs."""
+    (Engine.pdbs_allowed on the live state) name the violated PDBs.  Results of drains with local volumes carry the VG sums: they go
+    into Occupancy (vg_requested / vg_capacity) and CapsOk applies max_vg to them (default: env_vg_cap())."""
     from .simulator import UnscheduledPod, format_fit_error
     if max_cpu is None or max_mem is None:
         max_cpu, max_mem = env_caps()
@@ -228,7 +238,13 @@ def drain_results(compiled: Compiled, placed: np.ndarray, removed_lists: Sequenc
         for q in r["blocked"].tolist():
             res.BlockedPods.append(BlockedPod(recs[q], names[placed[q]], BLOCK_NODE_NAME if fixed[q] >= 0 else BLOCK_LOCAL_STORAGE))
         res.Occupancy = {k: int(r[k]) for k in ("req_mcpu", "alloc_mcpu", "req_mem", "alloc_mem")}
-        res.CapsOk = occupancy_ok(res.Occupancy, max_cpu, max_mem)
+        if "vg_capacity" in r:
+            if max_vg is None:
+                max_vg = env_vg_cap()
+            res.Occupancy.update(vg_requested=int(r["vg_requested"]), vg_capacity=int(r["vg_capacity"]))
+            res.CapsOk = occupancy_ok(res.Occupancy, max_cpu, max_mem, max_vg)
+        else:
+            res.CapsOk = occupancy_ok(res.Occupancy, max_cpu, max_mem)
         out.append(res)
     return out
 
@@ -237,13 +253,23 @@ def drain_results(compiled: Compiled, placed: np.ndarray, removed_lists: Sequenc
 
 def plan_scale_down(compiled: Compiled, placed: np.ndarray, runner: Callable[[List[np.ndarray]], List[dict]],
                     candidates: Optional[Sequence[int]] = None, max_remove: Optional[int] = None, batch: int = 64,
-                    max_cpu: Optional[int] = None, max_mem: Optional[int] = None) -> ScaleDownPlan:
+                    max_cpu: Optional[int] = None, max_mem: Optional[int] = None, max_vg: Optional[int] = None) -> ScaleDownPlan:
     """runner(remain_lists) -> per drain a dict with n_blocked, n_unscheduled, n_evicted, n_pdb_violated and the occupancy sums
     (Engine.drain_run with detail=False; on an engine with a PDB table the PDBs are honoured).  1. every candidate drained alone, in one run; 2. the drainable ones ordered by utilisation ascending, ties
     in nodeTree order; 3. prefixes k = 1, 2, ... of that order removed together, `batch` consecutive k per run; 4. the plan is the
-    largest k such that every prefix up to k drains and meets the caps: the first failing k ends it (no monotonicity is assumed)."""
+    largest k such that every prefix up to k drains and meets the caps: the first failing k ends it (no monotonicity is assumed).
+    max_vg (default env_vg_cap(), read at the first result with VG sums) applies to results that carry the VG sums (drains with local
+    volumes) and is ignored for the others."""
     if max_cpu is None or max_mem is None:
         max_cpu, max_mem = env_caps()
+
+    def caps_ok(r):
+        nonlocal max_vg
+        if "vg_capacity" not in r:
+            return occupancy_ok(r, max_cpu, max_mem)
+        if max_vg is None:
+            max_vg = env_vg_cap()
+        return occupancy_ok(r, max_cpu, max_mem, max_vg)
     names = compiled.node_names
     n = compiled.n_nodes
     cand = list(range(n)) if candidates is None else list(dict.fromkeys(int(c) for c in candidates))     # repeats dropped, order kept
@@ -270,7 +296,7 @@ def plan_scale_down(compiled: Compiled, placed: np.ndarray, runner: Callable[[Li
         raw = runner([order.remaining(good[:j]) for j in ks])
         stop = False
         for j, r in zip(ks, raw):
-            ok = drainable(r) and occupancy_ok(r, max_cpu, max_mem)
+            ok = drainable(r) and caps_ok(r)
             prefixes.append(dict(r, k=j, ok=ok))
             if not ok:
                 stop = True
@@ -284,9 +310,11 @@ def plan_scale_down(compiled: Compiled, placed: np.ndarray, runner: Callable[[Li
 
 # ---- entry points on objects ---------------------------------------------------------------------------------------------------------
 
-def drain(cluster: ResourceTypes, apps: List[AppResource], drains: List[List[str]], *opts, pdbs: Optional[List[dict]] = None) -> List[DrainResult]:
-    """NewSimulator(*opts), RunCluster(PrepareCluster(cluster)), ScheduleApp per app, then DrainNodes(drains).  pdbs: PDB objects to
-    honour besides the cluster's and the apps' (given, even empty, the session runs WithPodDisruptionBudgets)."""
+def drain(cluster: ResourceTypes, apps: List[AppResource], drains: List[List[str]], *opts, pdbs: Optional[List[dict]] = None,
+          local_volumes: bool = False) -> List[DrainResult]:
+    """NewSimulator(*opts), RunCluster(PrepareCluster(cluster)), ScheduleApp per app, then DrainNodes(drains, local_volumes).  pdbs: PDB
+    objects to honour besides the cluster's and the apps' (given, even empty, the session runs WithPodDisruptionBudgets);
+    local_volumes needs WithOpenLocal among opts."""
     from .simulator import NewSimulator, PrepareCluster, WithPodDisruptionBudgets
     if pdbs is not None:
         opts = opts + (WithPodDisruptionBudgets(pdbs),)
@@ -294,4 +322,4 @@ def drain(cluster: ResourceTypes, apps: List[AppResource], drains: List[List[str
         sim.RunCluster(PrepareCluster(cluster))
         for app in apps:
             sim.ScheduleApp(app)
-        return sim.DrainNodes(drains)
+        return sim.DrainNodes(drains, local_volumes=local_volumes)

@@ -551,10 +551,13 @@ class Simulator:
 
 
     # ---- node drains and scale-down (this project's extension: the reference names the use case, README.md:16, without code) ----
-    def DrainNodes(self, drains: List[List[str]]):
+    def DrainNodes(self, drains: List[List[str]], local_volumes: bool = False):
         """Each entry names nodes to remove together; per entry a scaledown.DrainResult on the session's live state (the last
-        call's placements and compiled cluster, on its device context: no new compile)."""
+        call's placements and compiled cluster, on its device context: no new compile).  local_volumes (a session WithOpenLocal):
+        pods with Open-Local volumes are evicted and their volumes provisioned again on the remaining nodes instead of blocking the
+        drain (their data is not carried over); the results then carry the VG sums and CapsOk applies MaxVG."""
         from . import scaledown
+        self._check_local_volumes(local_volumes, "DrainNodes")
         eng, compiled = self._live()
         order = scaledown.NodeOrder(compiled)
         removed = []
@@ -565,21 +568,24 @@ class Simulator:
                 raise ValueError(f"DrainNodes: no node named {bad[0]!r}")
             removed.append(idx)
         remain = [order.remaining(r) for r in removed]
-        raw = eng.drain_run(self.placements, remain, detail=True)
+        raw = eng.drain_run(self.placements, remain, detail=True, local=local_volumes)
         allowed = eng.pdbs_allowed() if self.pdb_tables is not None else None
         return scaledown.drain_results(compiled, self.placements, removed, remain, raw, pdbs=self.pdb_tables, allowed=allowed)
 
-    def PlanScaleDown(self, candidates: Optional[List[str]] = None, max_remove: Optional[int] = None):
+    def PlanScaleDown(self, candidates: Optional[List[str]] = None, max_remove: Optional[int] = None, local_volumes: bool = False):
         """scaledown.ScaleDownPlan on the session's live state: candidates (node names; all nodes by default) drained alone, the
-        drainable ones ordered by utilisation, and the longest prefix of that order whose every prefix drains within the caps."""
+        drainable ones ordered by utilisation, and the longest prefix of that order whose every prefix drains within the caps.
+        local_volumes: the drains move pods with Open-Local volumes (DrainNodes), and MaxVG joins the caps."""
         from . import scaledown
+        self._check_local_volumes(local_volumes, "PlanScaleDown")
         eng, compiled = self._live()
         cand = None
         if candidates is not None:
             cand = [compiled.node_index(nm) for nm in candidates]
             if any(g < 0 for g in cand):
                 raise ValueError("PlanScaleDown: a candidate names no node of the cluster")
-        return scaledown.plan_scale_down(compiled, self.placements, lambda rl: eng.drain_run(self.placements, rl, detail=False),
+        return scaledown.plan_scale_down(compiled, self.placements,
+                                         lambda rl: eng.drain_run(self.placements, rl, detail=False, local=local_volumes),
                                          candidates=cand, max_remove=max_remove)
 
     def PlanMigrations(self, sources: Optional[List[str]] = None, targets: Optional[List[str]] = None, max_moves: int = 100,
@@ -599,6 +605,10 @@ class Simulator:
                 raise ValueError(f"PlanMigrations: no node named {bad[0]!r} among the {what}")
         moves = rebalance.candidates(compiled, self.placements, idx["sources"], idx["targets"])
         return rebalance.plan(eng, compiled, moves, max_moves, min_gain, move_scope, pdbs=self.pdb_tables)
+
+    def _check_local_volumes(self, local_volumes: bool, what: str):
+        if local_volumes and not self.options.openLocal:
+            raise ValueError(f"{what}: local_volumes=True needs a session WithOpenLocal (without it no pod has Open-Local volumes)")
 
     def _live(self):
         self._check_open()
