@@ -44,16 +44,35 @@ def lib():
         _LIB.simon_oracle_moves_score.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _LIB.simon_oracle_set_threads.restype = C.c_int
         _LIB.simon_oracle_set_threads.argtypes = [C.c_void_p, C.c_int]
+        _LIB.simon_oracle_set_storage.restype = C.c_int
+        _LIB.simon_oracle_set_storage.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        _LIB.simon_oracle_storage_state.restype = C.c_int
+        _LIB.simon_oracle_storage_state.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     return _LIB
 
 
 class Oracle:
-    def __init__(self, compiled, threads: int = 1):
+    def __init__(self, compiled, threads: int = 1, open_local: bool = False):
+        """open_local: run Open-Local (Filter, Score, Bind) on the storage tables of a cluster compiled with open_local=True,
+        and with its devices when it was compiled with local_devices=True; without it the oracle has no Open-Local."""
         self.c = compiled
         self.snap, self.pods, self._keep = abi.marshal(compiled)
         self.h = lib().simon_oracle_create(C.byref(self.snap), C.byref(self.pods))
         if not self.h:
             raise MemoryError("simon_oracle_create failed")
+        self.open_local = open_local
+        if open_local:
+            st = compiled.storage
+            if st is None:
+                raise ValueError("Oracle(open_local=True) needs a cluster compiled with open_local=True")
+            # the oracle reads these arrays for its whole life: they are kept with it
+            self.storage, self._storage_keep = abi.marshal_storage(st)
+            self.devices, self._devices_keep = abi.marshal_devices(st) if st.devices else (None, [])
+            rc = lib().simon_oracle_set_storage(self.h, C.byref(self.storage),
+                                                C.byref(self.devices) if self.devices is not None else None)
+            if rc != 0:
+                self.close()
+                raise RuntimeError(f"simon_oracle_set_storage rc={rc}")
         self.threads = 1
         if threads > 1:
             self.set_threads(threads)
@@ -144,3 +163,15 @@ class Oracle:
         if rc != 0:
             raise RuntimeError(f"simon_oracle_gpu_slots rc={rc}")
         return a[:count]
+
+    def storage_state(self):
+        """Open-Local state (Oracle(open_local=True)): (VG requested [V][N], allocated device slot masks [N] or None without
+        devices), as Engine.storage_state / Engine.device_state report them."""
+        st = self.c.storage
+        V, N = st.n_vgs, self.c.n_nodes
+        vg = np.zeros(max(V * N, 1), np.int64)
+        dev = np.zeros(max(N, 1), np.uint32)
+        rc = lib().simon_oracle_storage_state(self.h, vg.ctypes.data, dev.ctypes.data)
+        if rc != 0:
+            raise RuntimeError(f"simon_oracle_storage_state rc={rc}")
+        return vg[:V * N].reshape(V, N), (dev[:N] if st.devices else None)

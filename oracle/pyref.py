@@ -14,13 +14,16 @@ Followed code (paths relative to the reference tree, PL = vendor/k8s.io/kubernet
   PL/nodeunschedulable, nodename, tainttoleration, nodeaffinity, nodeports, noderesources (fit, least, balanced),
   PL/podtopologyspread (filtering.go, scoring.go, common.go), PL/interpodaffinity (filtering.go, scoring.go),
   PL/helper (normalize_score.go, spread.go, node_affinity.go), pkg/simulator/plugin/simon.go, open-gpu-share.go
-It reuses the product's Quantity / go_log restatements (simon_b200.quantity, simon_b200.gomath).
+  and, opted in per instance, pkg/simulator/plugin/open-local.go:51-254 (Filter, Score, NormalizeScore, Bind)
+It reuses the product's Quantity / go_log restatements (simon_b200.quantity, simon_b200.gomath) and, for Open-Local, the
+object-level plugin restatement of simon_b200.storage (node annotations, pod volumes, the VG and device choice, the scores).
 """
 from __future__ import annotations
 
 import math
 from typing import Dict, List, Optional, Tuple
 
+from simon_b200 import storage as OL
 from simon_b200.gomath import go_log
 from simon_b200.quantity import Quantity
 
@@ -341,11 +344,23 @@ def _gpu_allocate(ns: NodeState, mem, num):
 
 
 class PyRef:
-    """Schedules pods one at a time over dict objects. nodes must already be in snapshot (nodeTree.list) order."""
+    """Schedules pods one at a time over dict objects. nodes must already be in snapshot (nodeTree.list) order.
+    open_local: None (no Open-Local plugin), or (storage classes, devices): run Open-Local with those StorageClass objects, and
+    place SSD / HDD volumes on the nodes' devices when devices is true."""
 
-    def __init__(self, nodes: List[dict], services=None, replicasets=None, statefulsets=None, creation_order=None):
+    def __init__(self, nodes: List[dict], services=None, replicasets=None, statefulsets=None, creation_order=None,
+                 open_local=None):
         self.nodes = [NodeState(n) for n in nodes]
         self.by_name = {n.name: n for n in self.nodes}
+        self.open_local = open_local is not None
+        if self.open_local:
+            scs, self.local_devices = open_local
+            self.sc_params = OL.storage_class_params(list(scs or []))
+            for ns in self.nodes:
+                st = OL.parse_node_storage(ns.node, self.local_devices)     # GetNodeCache: None without the annotation
+                ns.has_storage = st is not None
+                ns.vgs = [list(v) for v in (st.vgs or [])] if st is not None else None
+                ns.devs = [dict(d) for d in (st.devices or [])] if st is not None else None
         # ImageLocality: the scheduler cache summarises a node's images when the node is ADDED (cache.go:673-697), in
         # node creation order (creation_order[i] = original index of snapshot node i), and never refreshes the summary
         order = sorted(range(len(nodes)), key=(lambda i: creation_order[i]) if creation_order is not None else (lambda i: i))
@@ -422,12 +437,50 @@ class PyRef:
         ns.nz_mem += n0m
         for p in _ports(spec):
             ns.ports.add(p)
+        if reserve_gpu and self.open_local:
+            self.local_bind(pod, ns)
         mem, num = _gpu_req(pod)
         if mem > 0 and reserve_gpu:
             slots = _gpu_allocate(ns, mem, num)
             for d in slots or []:
                 ns.gpu_used[d] += mem
         ns.pods.append(pod)
+
+    # -- Open-Local (pkg/simulator/plugin/open-local.go)
+    def pod_volumes(self, pod) -> Optional[OL.ClassVolumes]:
+        """GetPodLocalPVCs of the pod, None when Open-Local is off or the pod requests no local volume."""
+        if not self.open_local:
+            return None
+        cv = OL.pod_volumes(pod, self.sc_params, self.local_devices)
+        return cv if cv.local else None
+
+    @staticmethod
+    def local_place(cv: OL.ClassVolumes, ns: NodeState):
+        """Filter (open-local.go:51-92) on the node's current annotation -> (fits, LVM units, chosen devices, raw Score
+        (:94-138): ScoreLVMVolume + ScoreDeviceVolume with the all-dropped MinInt64, Go int64)."""
+        if not ns.has_storage:
+            return False, [], [], 0
+        err, units, s1 = OL.lvm_place(ns.name, ns.vgs, cv.lvm)
+        if err is not None:
+            return False, [], [], 0
+        err, chosen, s2 = OL.device_place(ns.name, ns.devs, cv.ssd, cv.hdd)
+        if err is not None:
+            return False, [], [], 0
+        raw = OL.raw_score(cv, s1 + s2)
+        return True, units, chosen, raw
+
+    def local_bind(self, pod, ns: NodeState):
+        """Bind (open-local.go:175-254): the VGs and devices the Filter's choice took.  Skipped without the annotation."""
+        cv = self.pod_volumes(pod)
+        if cv is None or not ns.has_storage:
+            return
+        fits, units, chosen, _raw = self.local_place(cv, ns)
+        if not fits:
+            return
+        for i, size in units:
+            ns.vgs[i][2] += size
+        for i in chosen:
+            ns.devs[i]["isAllocated"] = True
 
     def schedule_one(self, pod, detail: Optional[dict] = None):
         """-> (node index or -1, total score, fail reasons histogram)."""
@@ -478,6 +531,8 @@ class PyRef:
                         anti_map[(key, str(n.labels[key]))] = anti_map.get((key, str(n.labels[key])), 0) + 1
         self_match_all = bool(aff_terms) and all(_pod_matches(pod, nsset, reqs) for (nsset, reqs, _k) in aff_terms)
 
+        cv_local = self.pod_volumes(pod)
+        local_raw: Dict[int, int] = {}
         codes = []
         reasons_all = []
         for i, n in enumerate(nodes):
@@ -540,6 +595,12 @@ class PyRef:
                     if exist_map.get((k, str(v)), 0) > 0:
                         reasons = ["ipa-exist"]
                         break
+            if not reasons and cv_local is not None:      # Open-Local: after InterPodAffinity, before GPU share (utils.go:334-343)
+                ok, _u, _d, raw = self.local_place(cv_local, n)
+                if not ok:
+                    reasons = ["local"]
+                else:
+                    local_raw[i] = raw
             if not reasons and gmem > 0:
                 if n.gpu_total < gmem or _gpu_allocate(n, gmem, gnum) is None:
                     reasons = ["gpu"]
@@ -652,6 +713,8 @@ class PyRef:
         s_max = max(raw[i]["simon"] for i in feas)
         ip_min = min([0] + [raw[i]["ipa"] for i in feas])
         ip_max = max([0] + [raw[i]["ipa"] for i in feas])
+        # Open-Local NormalizeScore over the feasible nodes (open-local.go:146-171), weight 1; 0 for pods without volumes
+        local_norm = dict(zip(feas, OL.normalize_scores([local_raw[i] for i in feas]))) if cv_local is not None else {}
         pts_vals = [raw[i]["pts"] for i in feas if i not in ignored]
         pts_min = min(pts_vals) if pts_vals else MAXI64
         pts_max = max([0] + pts_vals)
@@ -680,9 +743,10 @@ class PyRef:
             else:
                 pts = (100 * (pts_max + pts_min - r["pts"])) // pts_max
             ex = self.image_locality(pod, i) + 10000 * self.prefer_avoid(pod, n)
-            total = ba + la + ip + na + 2 * pts + tt + 2 * sm + ex
+            ol = local_norm.get(i, 0)
+            total = ba + la + ip + na + 2 * pts + tt + 2 * sm + ex + ol
             if detail is not None:
-                detail[i] = dict(ba=ba, la=la, ip=ip, na=na, pts=pts, tt=tt, sm=sm, ex=ex, total=total)
+                detail[i] = dict(ba=ba, la=la, ip=ip, na=na, pts=pts, tt=tt, sm=sm, ex=ex, ol=ol, total=total)
             if best is None or total > best:
                 best, best_i = total, i
         return best_i, best, {}

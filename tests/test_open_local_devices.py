@@ -312,16 +312,28 @@ def test_engine_matches_cpu_port_with_restated_devices(seed, n_nodes, n_pods):
     ScoreDevice and NormalizeScore come on top from the state the engine's earlier Binds left (storage.py).  The nodes share one
     allocatable shape and the pods are bare, so every other score plugin gives the same per-node score whatever the feasible set
     is.  Some placements must be decided by differing device scores."""
-    from oracle.binding import Oracle
     from simon_b200.engine import Engine
-    from simon_b200.storage import lvm_place, normalize_scores
-    rng = np.random.default_rng(seed)
-    nodes, pods = _random_cluster(rng, n_nodes, n_pods)
-    c = compile_cluster(nodes, pods, open_local=True, storage_classes=SCS, local_devices=True)
-    st = c.storage
+    c = restated_cluster(seed, n_nodes, n_pods)
     with Engine(c, record_scores=True) as eng:
         out, score, _fc, _fp = eng.schedule()
         final_dev = eng.device_state()
+    assert check_restated_devices(c, out, score, final_dev) > 0
+
+
+def restated_cluster(seed, n_nodes, n_pods):
+    """The cluster of _random_cluster(seed) compiled with Open-Local and its devices."""
+    rng = np.random.default_rng(seed)
+    nodes, pods = _random_cluster(rng, n_nodes, n_pods)
+    return compile_cluster(nodes, pods, open_local=True, storage_classes=SCS, local_devices=True)
+
+
+def check_restated_devices(c, out, score, final_dev):
+    """The composition above, pod by pod, for a run of a cluster of restated_cluster: out / score are its placements and recorded
+    winning scores, final_dev its device masks.  Returns the number of decisions with several feasible nodes whose device scores
+    differ."""
+    from oracle.binding import Oracle
+    from simon_b200.storage import lvm_place, normalize_scores
+    st = c.storage
     orc = Oracle(c)
     orc.enable_dump()
     P = c.pods_dims["n_pods"]
@@ -367,7 +379,7 @@ def test_engine_matches_cpu_port_with_restated_devices(seed, n_nodes, n_pods):
             rep.bind(cls, int(out[i]))
     orc.close()
     assert np.array_equal(final_dev, rep.alloc_masks())
-    assert by_device > 0
+    return by_device
 
 
 @pytest.mark.gpu

@@ -228,8 +228,9 @@ def test_variant_matrix_exercised_the_flip_paths():
 @pytest.mark.parametrize("kernel,fam,cs,t,big", [e for e in ENTRIES if e[1].startswith("local")],
                          ids=[f"{k[6:]}-{cs}x{t}" for k, fam, cs, t, big in ENTRIES if fam.startswith("local")])
 def test_open_local_variant_matches_restated_composition(kernel, fam, cs, t, big):
-    """Open-Local has no C oracle: the CPU oracle plus storage.py's Filter, ScoreLVM, NormalizeScore and Bind, pod by pod
-    (test_open_local.check_restated_open_local), at a geometry that launches the variant."""
+    """The storage-less CPU oracle plus storage.py's Filter, ScoreLVM, NormalizeScore and Bind, pod by pod
+    (test_open_local.check_restated_open_local), at a geometry that launches the variant: a check independent of the oracle's own
+    Open-Local, which test_zz_open_local_oracle_gpu.py compares every variant with on mixed clusters."""
     from test_open_local import check_restated_open_local
     c = family(fam)
     with _engine(c, cs, t, big, record_scores=True) as eng:

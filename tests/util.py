@@ -68,20 +68,23 @@ def _sfc_of(reason: str, scalar_names) -> int:
     fixed = {"static": abi.SFC_STATIC, "ports": abi.SFC_PORTS, "Too many pods": abi.SFC_TOO_MANY_PODS, "Insufficient cpu": abi.SFC_CPU,
              "Insufficient memory": abi.SFC_MEM, "Insufficient ephemeral-storage": abi.SFC_EPH, "pts-missing": abi.SFC_PTS_MISSING,
              "pts-skew": abi.SFC_PTS_SKEW, "ipa-aff": abi.SFC_IPA_AFF, "ipa-anti": abi.SFC_IPA_ANTI, "ipa-exist": abi.SFC_IPA_EXIST,
-             "gpu": abi.SFC_GPU}
+             "gpu": abi.SFC_GPU, "local": abi.SFC_LOCAL}
     if reason in fixed:
         return fixed[reason]
     assert reason.startswith("Insufficient "), reason
     return abi.SFC_SCALAR0 + list(scalar_names).index(reason[len("Insufficient "):])
 
 
-def pyref_walk(p, c):
+def pyref_walk(p, c, open_local=None, ref_out=None):
     """PyRef.schedule_one pod by pod, as PyRef.run commits: -> (node [P], winning total [P], feasible node count [P], failure
-    histogram [P][N_FAIL_CODES] in simon_fail_code columns).  Pods bound by spec.nodeName get their node, total 0 and no failure."""
+    histogram [P][N_FAIL_CODES] in simon_fail_code columns).  Pods bound by spec.nodeName get their node, total 0 and no failure.
+    open_local: PyRef's Open-Local setting, (storage classes, devices).  ref_out: a list that receives the PyRef afterwards."""
     from oracle.pyref import PyRef
     from simon_b200 import abi
     ref = PyRef(c.node_objs, services=p.ctx.services, replicasets=p.ctx.replicasets, statefulsets=p.ctx.statefulsets,
-                creation_order=c.node_orig_index)
+                creation_order=c.node_orig_index, open_local=open_local)
+    if ref_out is not None:
+        ref_out.append(ref)
     P = len(p.pods)
     node, total, feas = np.full(P, -1, np.int32), np.zeros(P, np.int64), np.zeros(P, np.int64)
     hist = np.zeros((P, abi.N_FAIL_CODES), np.uint32)
