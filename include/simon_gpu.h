@@ -563,7 +563,8 @@ typedef struct simon_scenario_local_result {
 } simon_scenario_local_result;
 int simon_scenarios_run_local(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, simon_scenario_result *out,
                               simon_scenario_local_result *out_local, int32_t *out_node);
-/* Scenario `scenario` of the last simon_scenarios_run_local or simon_drain_run_local batch: its final VG requested [V][N] and, if
+/* Scenario `scenario` of the last simon_scenarios_run_local or simon_drain_run_local batch, or probe `scenario` of the last simon_probe_run
+ * batch on a context with storage: its final VG requested [V][N] and, if
  * dev_alloc is not NULL, its allocated device slots [N] (SIMON_ERR_STATE without a simon_devices_upload); node-indexed like the
  * snapshot.  Inactive nodes keep the values the scenario started from: the uploaded ones in a scenario batch, the live ones (the
  * state `placed` leaves) on a drain's removed nodes.  SIMON_ERR_STATE if no such batch ran since the last snapshot, pod, storage or
@@ -641,8 +642,57 @@ int simon_drain_times(simon_ctx *ctx, float *setup_ms, float *place_ms);
 /* Sizing of drain batches: device bytes one scenario holds in the batch pool (they grow with nodes x pod classes), and the bytes a
  * batch may use now (free device memory + the stream-ordered pool's cached blocks + the batch pool's current columns).  Not in the
  * per-scenario bytes, since they depend on the drains: 16 B per evicted pod of the batch, 100 B x the batch's largest evicted-pod list
- * per scenario (failure records), and the large-cluster variant's per-node arrays when it runs; a caller leaves a margin for them. */
+ * per scenario (failure records), and the large-cluster variant's per-node arrays when it runs; a caller leaves a margin for them.
+ * The per-scenario bytes size probe batches (simon_probe_run) too: a probe holds one batch-pool slot, and its outputs take 16 B per
+ * replica of its max_replicas plus one failure record. */
 int simon_drain_budget(simon_ctx *ctx, uint64_t *scenario_bytes, uint64_t *free_bytes);
+
+/* ---- scheduling headroom (the reference's first use case, README.md:14 capacity planning, asked of the running cluster; it has no
+ * code for it, so the definition is this library's) -------------------------------------------------------------------------------
+ * The live state is placed[n_pods], checked as simon_drain_run checks it.  A probe (pod q, max_replicas R >= 1) asks how many more
+ * replicas of pod q fit the live cluster: replicas of q are placed one at a time through the full filter -> score -> select ->
+ * Reserve / Bind path on all nodes, each on the state the ones before it leave (requests, non-zero requests, pod counts, the class
+ * counters spread and inter-pod (anti-)affinity read, GPU-share device memory and, with Open-Local, VGs and devices).  The probe stops at
+ * the first replica that does not fit (SIMON_PROBE_STOP_UNSCHEDULABLE, n_placed = the replicas placed before it): a failed decision
+ * commits nothing, so every later replica would fail the same way.  Or it stops after R replicas (SIMON_PROBE_STOP_MAX_REPLICAS).
+ * q must reach the scheduler: not bound by spec.nodeName, existing, and not of a pinned (DaemonSet) class.  Its own live result does
+ * not matter: a replica is a new pod of q's class, so the live pods of q's workload count against its anti-affinity and spread.
+ * Equivalently: probe (q, R) places what compiling the pod list with R copies of q appended and resuming with `placed` as the prefix
+ * (simon_schedule_resume) places; the first n_placed copies land on the probe's nodes with the same GPU slots, final VG requested and
+ * device masks, and copy n_placed + 1 (if n_placed < R) fails with the probe's failure histogram.
+ * Precondition: the class tables of q's class must stay within their int32 bounds for n_pods + R pods (the compiler's per-class pod
+ * limit); the library trusts the uploaded tables here as it does for every class table.
+ *
+ * simon_probe_run runs n probes as one batch, each independently from the live state: it is rebuilt from `placed` into the
+ * single-scenario state (as simon_drain_run rebuilds it: afterwards the single-scenario downloads describe `placed`) and copied into
+ * every probe's slot of the batch pool.  The probe kernels with Open-Local code run when storage is uploaded and some probe pod's class
+ * has Open-Local volumes; otherwise those without it (a class without volumes passes Open-Local's filter and scores 0).  out[i] holds
+ * probe i's outcome and the sums over all nodes after its replicas, as simon_scenario_result's.  out_local (NULL, or n entries; needs a
+ * simon_storage_upload, else SIMON_ERR_STATE) gets each probe's VG sums as simon_scenarios_run_local's, and after a batch on a context
+ * with storage simon_scenarios_storage_download gives each probe's final VG requested and device masks.  A probe batch and a drain batch
+ * share the batch pool: after a probe batch simon_drain_download refuses, and after a drain batch simon_probe_download does.
+ * simon_last_kernel_ms is the device time of setup + placement, simon_probe_times splits it.
+ * SIMON_ERR_INVALID with a message, before any device work: `placed` fails the prefix checks, a probe pod is out of range, does not
+ * reach the scheduler or has a pinned class, or max_replicas is 0.  SIMON_ERR_LIMIT: the per-replica outputs do not fit the device. */
+typedef struct simon_probe {
+    uint32_t pod;
+    uint32_t max_replicas;
+} simon_probe;
+#define SIMON_PROBE_STOP_UNSCHEDULABLE 1u
+#define SIMON_PROBE_STOP_MAX_REPLICAS  2u
+typedef struct simon_probe_result {
+    uint32_t n_placed, stop_reason;
+    int64_t req_mcpu, alloc_mcpu, req_mem, alloc_mem;   /* over all nodes after the replicas (simon_scen_reduce) */
+} simon_probe_result;
+int simon_probe_run(simon_ctx *ctx, const int32_t *placed, const simon_probe *probes, uint32_t n, simon_probe_result *out,
+                    simon_scenario_local_result *out_local /* may be NULL */);
+/* Probe `probe` of the last simon_probe_run batch, any pointer may be NULL: the node of each replica [n_placed], its GPU slot word
+ * [n_placed] (simon_gpu_slots_download's format), its winning total score [n_placed] (0 without SIMON_OPT_RECORD_SCORES or with a
+ * single feasible node), and the failure histogram [SIMON_N_FAIL_CODES] of the replica that stopped it (zeros on MaxReplicas).
+ * SIMON_ERR_STATE if no probe batch ran since the last snapshot or pod upload, or a drain batch ran after it. */
+int simon_probe_download(simon_ctx *ctx, uint32_t probe, int32_t *node, uint32_t *gpu_slots, int64_t *score, uint32_t *fail_counts);
+/* Device time of the last simon_probe_run: setup (rebuild, copies into the slots) and placement, ms. */
+int simon_probe_times(simon_ctx *ctx, float *setup_ms, float *place_ms);
 
 /* ---- PodDisruptionBudgets in drains, move scoring and migration plans (this library's reading; the reference carries PDBs in
  * ResourceTypes.PodDisruptionBudgets, pkg/simulator/core.go:48, and creates them, simulator.go:261-262, 374-376) ----------------------

@@ -244,7 +244,7 @@ enum Data : uint32_t {
     MOVE_LIST = 1u << 6, MOVE_RUN = 1u << 7,
     SCOPE_PREP = 1u << 8,       // what the move scope launches, for the current scope and move-class records
     STATIC_FILL = 1u << 9,      // the static verdicts of every (signature, node) pair are in the pod set's scache
-    STORAGE_BATCH = 1u << 10, DRAIN_BATCH = 1u << 11, PLAN = 1u << 12,
+    STORAGE_BATCH = 1u << 10, DRAIN_BATCH = 1u << 11, PLAN = 1u << 12, PROBE_BATCH = 1u << 13,
 };
 
 struct Validity {
@@ -255,7 +255,7 @@ struct Validity {
     void drop(uint32_t d) {
         static constexpr uint32_t derived[][2] = {
             {SNAPSHOT, POD_SET},
-            {POD_SET, STORAGE | PDB_TABLE | LIVE | PLAN | DRAIN_BATCH | MOVE_LIST | SCOPE_PREP | STATIC_FILL},
+            {POD_SET, STORAGE | PDB_TABLE | LIVE | PLAN | DRAIN_BATCH | PROBE_BATCH | MOVE_LIST | SCOPE_PREP | STATIC_FILL},
             {STORAGE, DEVICES | STORAGE_BATCH | LIVE | SCOPE_PREP},     // SCOPE_PREP: the move-class records exclude local classes
             {DEVICES, STORAGE_BATCH | LIVE},
             {MOVE_LIST, MOVE_RUN},
@@ -369,6 +369,16 @@ struct simon_ctx {
         DevBuf<uint2> d_pairs;
         float setup_ms = 0.f, place_ms = 0.f;
     } drain;
+    // the last probe batch (simon_probe_run): n probes, each one's output positions (CSR off, max_replicas apart) and replicas placed; on
+    // the device the probe pods, the offsets, the replicas' nodes, scores and GPU slots, and one failure record per probe
+    struct {
+        uint32_t n = 0;
+        std::vector<uint32_t> off, placed;
+        DevBuf<uint32_t> d_pod, d_off, d_gpu, d_fail_counts, d_fail_pod;
+        DevBuf<int32_t> d_node;
+        DevBuf<int64_t> d_score;
+        float setup_ms = 0.f, place_ms = 0.f;
+    } probe;
     // the last migration plan (simon_moves_plan): its end state in plan-owned copies of the single-scenario node state, placement and
     // GPU slot words, the steps and control words
     struct {
@@ -537,10 +547,11 @@ void fill_params(simon_ctx *ctx, const ScenPool &s, SkParams &P) {
 typedef void (*sk_kernel_fn)(const SkParams);
 // The kernel family a launch runs, an argument of kernel_variant / max_active_clusters / choose_geometry / launch (never context
 // state, so no other call can launch a drain kernel): the placement variants (the local ones with storage uploaded), the drain-batch
-// variants without Open-Local code (simon_drain_run), or those with it (simon_drain_run_local)
-enum Family { PLACE, DRAIN, DRAIN_LOCAL };
-struct sk_variant { sk_kernel_fn fn; const char *name; uint32_t threads, slots; bool prof, big, local, drain; };
-#define SK_VARIANT_ENTRY(name, threads, slots, prof, big, local, drain) {name, #name, threads, slots, prof, big, local, drain},
+// variants without Open-Local code (simon_drain_run), or those with it (simon_drain_run_local), and the same two of the headroom-probe
+// variants (simon_probe_run)
+enum Family { PLACE, DRAIN, DRAIN_LOCAL, PROBE, PROBE_LOCAL };
+struct sk_variant { sk_kernel_fn fn; const char *name; uint32_t threads, slots; bool prof, big, local, drain, probe; };
+#define SK_VARIANT_ENTRY(name, threads, slots, prof, big, local, drain, probe) {name, #name, threads, slots, prof, big, local, drain, probe},
 const sk_variant sk_variants[] = {SIMON_PLACE_VARIANTS(SK_VARIANT_ENTRY)};
 #undef SK_VARIANT_ENTRY
 
@@ -548,17 +559,18 @@ const sk_variant sk_variants[] = {SIMON_PLACE_VARIANTS(SK_VARIANT_ENTRY)};
 // and what the geometry is sized for: the one of the fewest threads that holds TPB, with the unrolled loop for npt slots where
 // there is one and run-time slots otherwise.  big: the large-cluster variant, at any thread count; prof: with per-phase timers
 // (256 and 320 threads only).  PLACE: with Open-Local storage uploaded, the local variants (no timers).  DRAIN: the drain-batch
-// variants without Open-Local code (simon_drain_run), whatever was uploaded; DRAIN_LOCAL: those with it (simon_drain_run_local).  big
-// and the drain families ignore prof.  nullptr: none.
+// variants without Open-Local code (simon_drain_run), whatever was uploaded; DRAIN_LOCAL: those with it (simon_drain_run_local); PROBE
+// and PROBE_LOCAL likewise for probe batches.  big and the drain and probe families ignore prof.  nullptr: none.
 const sk_variant *kernel_variant(const simon_ctx *ctx, uint32_t TPB, uint32_t npt, bool big, bool prof, Family fam) {
     if (!big && TPB > SIMON_MAX_TPB) return nullptr;
     const uint32_t threads = TPB <= 256 ? 256 : TPB <= 320 ? 320 : 384;
-    const bool drain = fam != PLACE;
-    const bool local = fam == DRAIN_LOCAL || (fam == PLACE && ctx->valid.has(STORAGE));
-    if (big || drain) prof = false;
+    const bool drain = fam == DRAIN || fam == DRAIN_LOCAL, probe = fam == PROBE || fam == PROBE_LOCAL;
+    const bool local = fam == DRAIN_LOCAL || fam == PROBE_LOCAL || (fam == PLACE && ctx->valid.has(STORAGE));
+    if (big || drain || probe) prof = false;
     const sk_variant *runtime_slots = nullptr;
     for (const sk_variant &v : sk_variants) {
-        if (v.big != big || v.drain != drain || v.local != local || v.prof != prof || (!big && v.threads != threads)) continue;
+        if (v.big != big || v.drain != drain || v.probe != probe || v.local != local || v.prof != prof || (!big && v.threads != threads))
+            continue;
         if (v.slots == npt) return &v;
         if (v.slots == 0) runtime_slots = &v;
     }
@@ -720,7 +732,8 @@ int choose_geometry(simon_ctx *ctx, uint32_t n_active, uint32_t &CS, uint32_t &T
 
 static_assert(sizeof(SkScenario) % 8 == 0, "SkScenario is copied in 8-byte words");
 
-// fam DRAIN / DRAIN_LOCAL: a drain-batch variant (P carries drain_pods / drain_off)
+// fam DRAIN / DRAIN_LOCAL: a drain-batch variant (P carries drain_pods / drain_off); PROBE / PROBE_LOCAL: a probe-batch variant (P
+// carries probe_pod / probe_off)
 int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t TPB, size_t smem, bool record = true, Family fam = PLACE) {
     // SIMON_PROFILE=1 selects the variants with per-phase clock64 timers (simon_stats cycles); the default variants
     // carry no timers
@@ -728,7 +741,7 @@ int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t T
     const sk_variant *v = kernel_variant(ctx, TPB, P.npt, ctx->big, prof, fam);
     if (!v)
         return fail(ctx, SIMON_ERR_LIMIT, "no kernel variant for %u threads per CTA%s%s", TPB, prof ? " with phase timers" : "",
-                    (fam == DRAIN_LOCAL || (fam == PLACE && ctx->valid.has(STORAGE))) ? " and Open-Local storage" : "");
+                    (fam == DRAIN_LOCAL || fam == PROBE_LOCAL || (fam == PLACE && ctx->valid.has(STORAGE))) ? " and Open-Local storage" : "");
     if (ctx->big) {
         CU(ctx->d_gnode.alloc(ctx->gnode_stride * (size_t)n_scen * CS));
         P.gnode = ctx->d_gnode.p; P.gnode_stride = ctx->gnode_stride;
@@ -1390,7 +1403,7 @@ int simon_scenarios_storage_download(simon_ctx *ctx, uint32_t scenario, int64_t 
     if (!ctx) return SIMON_ERR_INVALID;
     const ScenPool &B = ctx->batch;
     if (!ctx->valid.has(STORAGE_BATCH))
-        return fail(ctx, SIMON_ERR_STATE, "no simon_scenarios_run_local or simon_drain_run_local batch since the last upload");
+        return fail(ctx, SIMON_ERR_STATE, "no simon_scenarios_run_local, simon_drain_run_local or simon_probe_run batch with storage since the last upload");
     if (scenario >= ctx->storage_batch.n) return fail(ctx, SIMON_ERR_INVALID, "scenario %u of a batch of %u", scenario, ctx->storage_batch.n);
     if (dev_alloc && !ctx->valid.has(DEVICES)) return fail(ctx, SIMON_ERR_STATE, "no devices uploaded");
     CU(cudaSetDevice(ctx->device));
@@ -1436,6 +1449,57 @@ extern "C" int simon_drain_budget(simon_ctx *ctx, uint64_t *scenario_bytes, uint
     return SIMON_OK;
 }
 
+// The setup drain and probe batches share, enqueued once their refusals and allocations are done: the live state `placed` leaves,
+// rebuilt into the single-scenario pool (the resume's rebuild, its failure records cleared as the resume clears them) and copied into
+// each of the n slots of the batch pool, one broadcast per column.  Of the batch pool only what the copies do not overwrite is cleared:
+// the per-class summaries and own-score caches, the counters and clocks, and the batch's failure records (fail_words words at
+// fail_counts).  local: the live Open-Local state (the rebuild's Bind replay) is copied too.  ctx->ev0 is recorded before it; Pb gets the
+// batch pool's launch parameters.
+static int live_batch_setup(simon_ctx *ctx, const int32_t *placed, uint32_t n, bool local, uint32_t *fail_counts, size_t fail_words,
+                            SkParams &Pb) {
+    ScenPool &S = ctx->single, &B = ctx->batch;
+    cudaStream_t st = ctx->stream;
+    CU(cudaEventRecord(ctx->ev0, st));
+    SkParams Ps;
+    fill_params(ctx, S, Ps);
+    int rc = clear_pool(ctx, S);
+    if (rc) return rc;
+    CU(single_begin(ctx, Ps));
+    rc = rebuild_prefix(ctx, Ps, placed, ctx->pods.n_pods);
+    if (rc) return rc;
+    CU(cudaMemsetAsync(B.csum.p, 0, 8 * n * B.ncl * SK_CSUM_W, st));
+    CU(cudaMemsetAsync(B.ocache.p, 0, 8 * n * B.nodes * B.ncl, st));
+    CU(cudaMemsetAsync(B.counters.p, 0, 8ull * n, st)); CU(cudaMemsetAsync(B.clk.p, 0, 16ull * n, st));
+    CU(cudaMemsetAsync(fail_counts, 0, 4ull * fail_words, st));
+    CU(B.state.each(S.state, true, [&](auto &b, auto &s, uint64_t k) { ctx->launches++; return bcast(ctx, s.p, k, n, b.p); }));
+    if (local) {
+        CU(bcast(ctx, S.vg_req.p, B.vn, n, B.vg_req.p));
+        ctx->launches++;
+        if (ctx->valid.has(DEVICES)) { CU(bcast(ctx, S.dev_alloc.p, B.nodes, n, B.dev_alloc.p)); ctx->launches++; }
+    }
+    fill_params(ctx, B, Pb);
+    return SIMON_OK;
+}
+
+// After a drain or probe batch's launch: each scenario's sums over its active nodes (simon_scen_reduce) into res and, local, its VG sums
+// into out_local, copied back on the stream (the caller synchronises)
+static int live_batch_reduce(simon_ctx *ctx, uint32_t n, bool local, std::vector<simon_scenario_result> &res,
+                             simon_scenario_local_result *out_local) {
+    ScenPool &B = ctx->batch;
+    cudaStream_t st = ctx->stream;
+    simon_scen_reduce<<<n, 256, 0, st>>>(B.scen.p, ctx->snap.d_alloc_mcpu.p, ctx->snap.d_alloc_mem.p, B.results.p);
+    CU(cudaGetLastError());
+    if (local) {
+        simon_scen_reduce_local<<<n, 256, 0, st>>>(B.scen.p, ctx->storage.d_node_n_vg.p, ctx->storage.d_vg_cap.p, B.vg_req.p, B.vn, ctx->snap.N,
+                                                   B.local_results.p);
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(out_local, B.local_results.p, sizeof(simon_scenario_local_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    }
+    res.resize(n);
+    CU(cudaMemcpyAsync(res.data(), B.results.p, sizeof(simon_scenario_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    return SIMON_OK;
+}
+
 // simon_drain_run and simon_drain_run_local (out_local != nullptr: pods with Open-Local volumes are evicted, not blocked, and each
 // scenario carries its own Open-Local state, the live one to start with)
 static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario *remain, uint32_t n, simon_drain_result *out,
@@ -1455,7 +1519,8 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
     if (rc) return rc;
     CU(cudaSetDevice(ctx->device));
     ctx->last_launch = simon_launch_info{};
-    ctx->valid.drop(DRAIN_BATCH | STORAGE_BATCH);     // the batch pool's Open-Local slices are no longer a storage batch's
+    // the batch pool is no longer a probe batch's, nor are its Open-Local slices a storage batch's
+    ctx->valid.drop(DRAIN_BATCH | PROBE_BATCH | STORAGE_BATCH);
     ScenPool &S = ctx->single, &B = ctx->batch;
     if (n == 0) return SIMON_OK;
     cudaStream_t st = ctx->stream;
@@ -1518,32 +1583,11 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
         h[i].fail_pod = ctx->drain.d_fail_pod.p + (size_t)i * ctx->drain.max;
     }
     CU(B.scen.upload(h.data(), n, st));
-    // ---- setup: the live state in the single-scenario pool (the resume's rebuild, its failure records cleared as the resume clears
-    // them), copied into every slot, minus what each scenario's removed nodes' pods contributed to the counters.  Of the batch pool
-    // only what the copies do not overwrite is cleared: the per-class summaries and own-score caches, the counters and failure
-    // records.  local: the live Open-Local state (the rebuild's Bind replay) is copied too; the removed nodes' VGs and devices stay as
-    // they are, since those nodes are inactive ----
-    CU(cudaEventRecord(ctx->ev0, st));
-    SkParams Ps;
-    fill_params(ctx, S, Ps);
-    rc = clear_pool(ctx, S);
-    if (rc) return rc;
-    CU(single_begin(ctx, Ps));
-    rc = rebuild_prefix(ctx, Ps, placed, P);
-    if (rc) return rc;
-    CU(cudaMemsetAsync(B.csum.p, 0, 8 * n * B.ncl * SK_CSUM_W, st));
-    CU(cudaMemsetAsync(B.ocache.p, 0, 8 * n * B.nodes * B.ncl, st));
-    CU(cudaMemsetAsync(B.counters.p, 0, 8ull * n, st)); CU(cudaMemsetAsync(B.clk.p, 0, 16ull * n, st));
-    CU(cudaMemsetAsync(ctx->drain.d_fail_counts.p, 0, 4ull * n * ctx->drain.max * SIMON_N_FAIL_CODES, st));
-    // every slot = the live state, one broadcast per column
-    CU(B.state.each(S.state, true, [&](auto &b, auto &s, uint64_t k) { ctx->launches++; return bcast(ctx, s.p, k, n, b.p); }));
-    if (local) {
-        CU(bcast(ctx, S.vg_req.p, B.vn, n, B.vg_req.p));
-        ctx->launches++;
-        if (ctx->valid.has(DEVICES)) { CU(bcast(ctx, S.dev_alloc.p, B.nodes, n, B.dev_alloc.p)); ctx->launches++; }
-    }
+    // ---- setup: the live state in every slot (live_batch_setup), minus what each scenario's removed nodes' pods contributed to the
+    // counters.  local: the removed nodes' VGs and devices keep their live values, since those nodes are inactive ----
     SkParams Pb;
-    fill_params(ctx, B, Pb);
+    rc = live_batch_setup(ctx, placed, n, local, ctx->drain.d_fail_counts.p, (size_t)n * ctx->drain.max * SIMON_N_FAIL_CODES, Pb);
+    if (rc) return rc;
     if (!pairs.empty()) {
         const uint32_t grid = (uint32_t)std::min<size_t>((pairs.size() + 255) / 256, (size_t)ctx->sms * 4);
         simon_drain_unimport<<<grid, 256, 0, st>>>(Pb, ctx->d_prefix.p, ctx->drain.d_pairs.p, (uint32_t)pairs.size());
@@ -1557,15 +1601,9 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
     rc = launch(ctx, Pb, n, CS, TPB, smem, false, fam);
     if (rc) return rc;
     CU(cudaEventRecord(ctx->ev1, st));
-    simon_scen_reduce<<<n, 256, 0, st>>>(B.scen.p, ctx->snap.d_alloc_mcpu.p, ctx->snap.d_alloc_mem.p, B.results.p);
-    CU(cudaGetLastError());
-    if (local) {
-        simon_scen_reduce_local<<<n, 256, 0, st>>>(B.scen.p, ctx->storage.d_node_n_vg.p, ctx->storage.d_vg_cap.p, B.vg_req.p, B.vn, N, B.local_results.p);
-        CU(cudaGetLastError());
-        CU(cudaMemcpyAsync(out_local, B.local_results.p, sizeof(simon_scenario_local_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
-    }
-    std::vector<simon_scenario_result> res(n);
-    CU(cudaMemcpyAsync(res.data(), B.results.p, sizeof(simon_scenario_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    std::vector<simon_scenario_result> res;
+    rc = live_batch_reduce(ctx, n, local, res, out_local);
+    if (rc) return rc;
     // with a PDB table: `allowed` on the rebuilt live state, read at the same synchronisation
     const uint32_t J = ctx->valid.has(PDB_TABLE) ? ctx->pdb.n : 0;
     std::vector<int32_t> allowed(J);
@@ -1641,7 +1679,7 @@ extern "C" int simon_drain_times(simon_ctx *ctx, float *setup_ms, float *place_m
 extern "C" int simon_drain_download(simon_ctx *ctx, uint32_t scenario, uint32_t *evicted_pod, int32_t *node, uint32_t *gpu_slots,
                                     int64_t *score, uint32_t *blocked_pod, uint32_t *fail_counts, uint32_t *fail_pod) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->valid.has(DRAIN_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_drain_run batch since the last upload");
+    if (!ctx->valid.has(DRAIN_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_drain_run batch since the last upload, or a probe batch after it");
     if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "drain %u of a batch of %u", scenario, ctx->drain.n);
     CU(cudaSetDevice(ctx->device));
     const uint32_t b = ctx->drain.off[scenario], ne = ctx->drain.off[scenario + 1] - b;
@@ -1664,11 +1702,146 @@ extern "C" int simon_drain_download(simon_ctx *ctx, uint32_t scenario, uint32_t 
 
 extern "C" int simon_drain_pdb_download(simon_ctx *ctx, uint32_t scenario, uint32_t *pdb, uint32_t *evicted) {
     if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->valid.has(DRAIN_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_drain_run batch since the last upload");
+    if (!ctx->valid.has(DRAIN_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_drain_run batch since the last upload, or a probe batch after it");
     if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "drain %u of a batch of %u", scenario, ctx->drain.n);
     const uint32_t b = ctx->drain.voff[scenario], e = ctx->drain.voff[scenario + 1];
     if (pdb) std::copy(ctx->drain.vpdb.begin() + b, ctx->drain.vpdb.begin() + e, pdb);
     if (evicted) std::copy(ctx->drain.vcnt.begin() + b, ctx->drain.vcnt.begin() + e, evicted);
+    return SIMON_OK;
+}
+
+// ---- headroom probes ------------------------------------------------------------------------------------------------------------
+extern "C" int simon_probe_run(simon_ctx *ctx, const int32_t *placed, const simon_probe *probes, uint32_t n, simon_probe_result *out,
+                               simon_scenario_local_result *out_local) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_probe_run before uploads");
+    const uint32_t N = ctx->snap.N, P = ctx->pods.n_pods;
+    if ((P && !placed) || (n && (!probes || !out))) return fail(ctx, SIMON_ERR_INVALID, "simon_probe_run: NULL argument");
+    // ---- refusals before any device work: the live placement as a resume prefix checks it, then the probes ----
+    int rc = check_prefix(ctx, placed, P);
+    if (rc) return rc;
+    uint64_t total = 0;
+    bool any_local = false;
+    for (uint32_t i = 0; i < n; i++) {
+        const uint32_t q = probes[i].pod;
+        if (q >= P) return fail(ctx, SIMON_ERR_INVALID, "probe %u: pod %u out of range (%u pods)", i, q, P);
+        if (ctx->pods.h_fixed[q] != -1) return fail(ctx, SIMON_ERR_INVALID, "probe %u: pod %u does not reach the scheduler (bound by spec.nodeName)", i, q);
+        if (ctx->pods.h_guard[q] == -2) return fail(ctx, SIMON_ERR_INVALID, "probe %u: pod %u does not reach the scheduler (it does not exist)", i, q);
+        if (ctx->pods.h_guard[q] >= 0) return fail(ctx, SIMON_ERR_INVALID, "probe %u: pod %u has a pinned class (a DaemonSet pod)", i, q);
+        if (probes[i].max_replicas == 0) return fail(ctx, SIMON_ERR_INVALID, "probe %u: max_replicas is 0", i);
+        total += probes[i].max_replicas;
+        any_local |= ctx->valid.has(STORAGE) && ctx->storage.h_class_local[ctx->pods.h_class[q]];
+    }
+    if (out_local && !ctx->valid.has(STORAGE)) return fail(ctx, SIMON_ERR_STATE, "simon_probe_run: out_local without simon_storage_upload");
+    CU(cudaSetDevice(ctx->device));
+    {
+        // the per-replica outputs (node, GPU slots, score: 16 B per replica) and one failure record per probe
+        size_t fr = 0, tot = 0;
+        CU(cudaMemGetInfo(&fr, &tot));
+        const uint64_t held = 16ull * ctx->probe.d_node.cap;
+        const uint64_t need = 16ull * total + (4ull * SIMON_N_FAIL_CODES + 16) * n;
+        if (total >= (1ull << 32) || need > (uint64_t)fr + held)
+            return fail(ctx, SIMON_ERR_LIMIT, "simon_probe_run: outputs of %llu replicas (%llu bytes) do not fit the device (%llu bytes free)",
+                        (unsigned long long)total, (unsigned long long)need, (unsigned long long)fr);
+    }
+    ctx->last_launch = simon_launch_info{};
+    // the batch pool is no longer a drain batch's, nor are its Open-Local slices another storage batch's
+    ctx->valid.drop(DRAIN_BATCH | PROBE_BATCH | STORAGE_BATCH);
+    if (n == 0) return SIMON_OK;
+    cudaStream_t st = ctx->stream;
+    ScenPool &B = ctx->batch;
+    const bool storage = ctx->valid.has(STORAGE);
+    // ---- geometry, the batch pool and the outputs (allocations before the timed work): every probe runs on all nodes in index order,
+    // the order of the live run ----
+    uint32_t CS, TPB, NPT;
+    size_t smem;
+    const Family fam = any_local ? PROBE_LOCAL : PROBE;
+    rc = choose_geometry(ctx, N, CS, TPB, NPT, smem, n, fam);
+    if (rc) return rc;
+    rc = size_pool(ctx, B, n, false, false);
+    if (rc) return rc;
+    std::vector<uint32_t> pods(n);
+    ctx->probe.off.assign(n + 1, 0u);
+    for (uint32_t i = 0; i < n; i++) {
+        pods[i] = probes[i].pod;
+        ctx->probe.off[i + 1] = ctx->probe.off[i] + probes[i].max_replicas;
+    }
+    CU(ctx->probe.d_pod.upload(pods.data(), n, st));
+    CU(ctx->probe.d_off.upload(ctx->probe.off.data(), n + 1, st));
+    CU(ctx->probe.d_node.alloc(total)); CU(ctx->probe.d_gpu.alloc(total));
+    if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(ctx->probe.d_score.alloc(total));
+    CU(ctx->probe.d_fail_counts.alloc((size_t)n * SIMON_N_FAIL_CODES)); CU(ctx->probe.d_fail_pod.alloc(n));
+    std::vector<SkScenario> h(n);
+    for (uint32_t i = 0; i < n; i++) {
+        h[i] = fill_scen(B, i, N, true);
+        h[i].out_node = ctx->probe.d_node.p; h[i].out_gpu = ctx->probe.d_gpu.p;
+        h[i].out_score = (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) ? ctx->probe.d_score.p : nullptr;
+        h[i].fail_counts = ctx->probe.d_fail_counts.p + (size_t)i * SIMON_N_FAIL_CODES;
+        h[i].fail_pod = ctx->probe.d_fail_pod.p + i;
+    }
+    CU(B.scen.upload(h.data(), n, st));
+    // ---- setup: the live state in every slot, with its Open-Local state when storage is uploaded (live_batch_setup) ----
+    SkParams Pb;
+    rc = live_batch_setup(ctx, placed, n, storage, ctx->probe.d_fail_counts.p, (size_t)n * SIMON_N_FAIL_CODES, Pb);
+    if (rc) return rc;
+    CU(cudaEventRecord(ctx->evm, st));
+    // ---- placement of every probe's replicas, one failure record each ----
+    Pb.probe_pod = ctx->probe.d_pod.p; Pb.probe_off = ctx->probe.d_off.p;
+    Pb.first = 0; Pb.count = 0; Pb.max_fail = 1; Pb.npt = NPT;
+    rc = launch(ctx, Pb, n, CS, TPB, smem, false, fam);
+    if (rc) return rc;
+    CU(cudaEventRecord(ctx->ev1, st));
+    std::vector<simon_scenario_result> res;
+    rc = live_batch_reduce(ctx, n, out_local != nullptr, res, out_local);
+    if (rc) return rc;
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    ctx->valid.set(LIVE);
+    CU(cudaEventElapsedTime(&ctx->probe.setup_ms, ctx->ev0, ctx->evm));
+    CU(cudaEventElapsedTime(&ctx->probe.place_ms, ctx->evm, ctx->ev1));
+    CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    ctx->probe.placed.resize(n);
+    for (uint32_t i = 0; i < n; i++) {
+        simon_probe_result &o = out[i];
+        o.n_placed = res[i].n_scheduled;
+        o.stop_reason = res[i].n_unscheduled ? SIMON_PROBE_STOP_UNSCHEDULABLE : SIMON_PROBE_STOP_MAX_REPLICAS;
+        o.req_mcpu = res[i].req_mcpu; o.alloc_mcpu = res[i].alloc_mcpu; o.req_mem = res[i].req_mem; o.alloc_mem = res[i].alloc_mem;
+        ctx->probe.placed[i] = o.n_placed;
+    }
+    ctx->probe.n = n;
+    ctx->valid.set(PROBE_BATCH);
+    if (storage) {
+        ctx->storage_batch.n = n;           // simon_scenarios_storage_download serves this batch
+        ctx->valid.set(STORAGE_BATCH);
+    }
+    return SIMON_OK;
+}
+
+extern "C" int simon_probe_download(simon_ctx *ctx, uint32_t probe, int32_t *node, uint32_t *gpu_slots, int64_t *score, uint32_t *fail_counts) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(PROBE_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_probe_run batch since the last upload, or a drain batch after it");
+    if (probe >= ctx->probe.n) return fail(ctx, SIMON_ERR_INVALID, "probe %u of a batch of %u", probe, ctx->probe.n);
+    CU(cudaSetDevice(ctx->device));
+    const uint32_t b = ctx->probe.off[probe], k = ctx->probe.placed[probe];
+    const bool stopped = k < ctx->probe.off[probe + 1] - b;          // Unschedulable: its failure record was written
+    if (node && k) CU(cudaMemcpy(node, ctx->probe.d_node.p + b, 4ull * k, cudaMemcpyDeviceToHost));
+    if (gpu_slots && k) CU(cudaMemcpy(gpu_slots, ctx->probe.d_gpu.p + b, 4ull * k, cudaMemcpyDeviceToHost));
+    if (score && k) {
+        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(cudaMemcpy(score, ctx->probe.d_score.p + b, 8ull * k, cudaMemcpyDeviceToHost));
+        else memset(score, 0, 8ull * k);
+    }
+    if (fail_counts) {
+        if (stopped) CU(cudaMemcpy(fail_counts, ctx->probe.d_fail_counts.p + (size_t)probe * SIMON_N_FAIL_CODES, 4ull * SIMON_N_FAIL_CODES,
+                                   cudaMemcpyDeviceToHost));
+        else memset(fail_counts, 0, 4ull * SIMON_N_FAIL_CODES);
+    }
+    return SIMON_OK;
+}
+
+extern "C" int simon_probe_times(simon_ctx *ctx, float *setup_ms, float *place_ms) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (setup_ms) *setup_ms = ctx->probe.setup_ms;
+    if (place_ms) *place_ms = ctx->probe.place_ms;
     return SIMON_OK;
 }
 

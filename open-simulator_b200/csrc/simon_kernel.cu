@@ -275,9 +275,14 @@ struct ClassState {
 // live state; an evicted pod is scheduler-placed and exists, so the pinned-run and bypass blocks are compiled out.  LOCAL and DRAIN
 // together (simon_drain_run_local): the Open-Local code reads the pod's class only (never its index), and its VG / device / scratch
 // slices are the cluster's (sk_slice), which is the drain's scenario: a drain launch has one cluster per scenario, as a batch does
-template <int MAXT, int NPT_T, bool PROF, bool BIG = false, bool LOCAL = false, bool DRAIN = false>
+// PROBE: the headroom-probe variants (simon_probe_run): scenario s places replicas of one pod (SkParams::probe_pod[s]) on the live
+// state, one position of its output range each, until one does not fit.  A probe pod reaches the scheduler and is not pinned, so
+// the pinned-run and bypass blocks are compiled out as under DRAIN.  The stop is taken inside the C.F == 0 branch, which every thread
+// of the cluster takes at the same iteration (see there).  LOCAL and PROBE together: as LOCAL and DRAIN
+template <int MAXT, int NPT_T, bool PROF, bool BIG = false, bool LOCAL = false, bool DRAIN = false, bool PROBE = false>
 __device__ __forceinline__ void simon_place_body(const SkParams &P) {
     constexpr uint32_t CLS_LOCAL = LOCAL ? SK_CLS_LOCAL : 0u;
+    constexpr bool LIST = DRAIN || PROBE;      // the scenario's own pod stream, every pod of it scheduler-placed
     extern __shared__ __align__(16) unsigned char smem_raw[];
     cg::cluster_group cluster = cg::this_cluster();
     const uint32_t CS = cluster.num_blocks();
@@ -600,11 +605,12 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             if ((uint32_t)js < C.n_soft) S.soft_w[js] = __ldg(&P.log_table[psz[js] + 2]);
     };
 
-    // i runs over pod indices, or under DRAIN over positions in drain_pods (SK_POD: the pod at position x)
-#define SK_POD(x) (DRAIN ? P.drain_pods[x] : (x))
-    const uint32_t end = DRAIN ? P.drain_off[scen_id + 1] : P.first + P.count;
-    uint32_t i = DRAIN ? P.drain_off[scen_id] : P.first;
-    const uint32_t q0 = DRAIN ? (i < end ? P.drain_pods[i] : 0u) : i;
+    // i runs over pod indices, under DRAIN over positions in drain_pods, under PROBE over the scenario's output positions (SK_POD:
+    // the pod at position x)
+#define SK_POD(x) (PROBE ? P.probe_pod[scen_id] : DRAIN ? P.drain_pods[x] : (x))
+    const uint32_t end = LIST ? P.drain_off[scen_id + 1] : P.first + P.count;
+    uint32_t i = LIST ? P.drain_off[scen_id] : P.first;
+    const uint32_t q0 = LIST ? (i < end ? SK_POD(i) : 0u) : i;
     int32_t nx_cls = P.pod_class[q0], nx_fixed = P.pod_fixed[q0], nx_guard = P.pod_guard[q0];
     uint64_t nx_off = P.class_off[nx_cls];
     // static-normalised part of the total (NodeAffinity + TaintToleration + 2 x Simon + extra) under the current normalisers
@@ -645,7 +651,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
         else if (guard >= 0) exists = SC.rank_of ? (SC.rank_of[guard] >= 0) : true;
 
         TICK(0);
-        if (!DRAIN && exists && fixed == -4 && i != P.dump_pod) {
+        if (!LIST && exists && fixed == -4 && i != P.dump_pod) {
             // ---- run of pinned pods (DaemonSet pods whose dynamic filters are node-local; marked -4 by simon_pods_upload) ----
             // Such a pod can only land on its pin node (every other node fails NodeAffinity at the latest), and whether it does
             // depends on that node alone: NodeUnschedulable, TaintToleration and NodeAffinity of the pin, NodePorts on the node's own
@@ -774,7 +780,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             if (i < end) { nx_cls = P.pod_class[i]; nx_fixed = P.pod_fixed[i]; nx_guard = P.pod_guard[i]; nx_off = P.class_off[nx_cls]; }
             continue;
         }
-        if (!DRAIN && (!exists || (fixed != -1 && fixed != -4))) {
+        if (!LIST && (!exists || (fixed != -1 && fixed != -4))) {
             // ---- batch of pods that bypass scheduling (spec.nodeName preset) or do not exist in this scenario ----
             uint32_t j = i;
             while (j < end) {
@@ -1408,6 +1414,12 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             }
             if (leader) { SC.out_node[i] = -1; if (SC.out_score) SC.out_score[i] = 0; if (SC.out_gpu) SC.out_gpu[i] = 0; }
             n_fail++;
+            // PROBE: a failed decision commits nothing, so every later replica of the same pod would fail the same way.  The stop is
+            // uniform across the cluster: C.F is the same in every thread of it, being either the W_SUM all-reduce result sw[0] of
+            // the full summary, or a value derived only from all-reduced words (the single-flip path's C.F - 1 under the reduced
+            // qv / pv, the restore from the csum record every CTA reads alike), and this branch already holds no barrier of its own
+            // that only some threads would reach.  Every thread leaves the loop here and meets the others at the final cluster.sync.
+            if (PROBE) break;
             i++;
             continue;
         }
@@ -1790,48 +1802,57 @@ extern "C" __global__ void __launch_bounds__(256) simon_drain_unimport(const __g
 //   - Drain batches (per-scenario pod lists): the same, with no Open-Local code (by default a pod with local volumes blocks a drain,
 //     so no evicted pod has any).
 //   - Drain batches that evict pods with Open-Local volumes (simon_drain_run_local): the same again, with the Open-Local code.
-#define SIMON_PLACE_VARIANTS(X)                                       \
-    X(simon_place_kernel_256_0,  256, 0, false, false, false, false)  \
-    X(simon_place_kernel_256_1,  256, 1, false, false, false, false)  \
-    X(simon_place_kernel_256_2,  256, 2, false, false, false, false)  \
-    X(simon_place_kernel_256_3,  256, 3, false, false, false, false)  \
-    X(simon_place_kernel_256_4,  256, 4, false, false, false, false)  \
-    X(simon_place_kernel_320_0,  320, 0, false, false, false, false)  \
-    X(simon_place_kernel_320_1,  320, 1, false, false, false, false)  \
-    X(simon_place_kernel_320_2,  320, 2, false, false, false, false)  \
-    X(simon_place_kernel_320_3,  320, 3, false, false, false, false)  \
-    X(simon_place_kernel_320_4,  320, 4, false, false, false, false)  \
-    X(simon_place_kernel_384_0,  384, 0, false, false, false, false)  \
-    X(simon_place_kernel_384_1,  384, 1, false, false, false, false)  \
-    X(simon_place_kernel_384_2,  384, 2, false, false, false, false)  \
-    X(simon_place_kernel_384_3,  384, 3, false, false, false, false)  \
-    X(simon_place_kernel_big,    320, 0, false, true,  false, false)  \
-    X(simon_prof_kernel_256_0,   256, 0, true,  false, false, false)  \
-    X(simon_prof_kernel_256_1,   256, 1, true,  false, false, false)  \
-    X(simon_prof_kernel_256_2,   256, 2, true,  false, false, false)  \
-    X(simon_prof_kernel_256_3,   256, 3, true,  false, false, false)  \
-    X(simon_prof_kernel_256_4,   256, 4, true,  false, false, false)  \
-    X(simon_prof_kernel_320_0,   320, 0, true,  false, false, false)  \
-    X(simon_prof_kernel_320_1,   320, 1, true,  false, false, false)  \
-    X(simon_prof_kernel_320_2,   320, 2, true,  false, false, false)  \
-    X(simon_prof_kernel_320_3,   320, 3, true,  false, false, false)  \
-    X(simon_prof_kernel_320_4,   320, 4, true,  false, false, false)  \
-    X(simon_local_kernel_256,    256, 0, false, false, true,  false)  \
-    X(simon_local_kernel_320,    320, 0, false, false, true,  false)  \
-    X(simon_local_kernel_384,    384, 0, false, false, true,  false)  \
-    X(simon_local_kernel_big,    320, 0, false, true,  true,  false)  \
-    X(simon_drain_kernel_256,    256, 0, false, false, false, true)   \
-    X(simon_drain_kernel_320,    320, 0, false, false, false, true)   \
-    X(simon_drain_kernel_384,    384, 0, false, false, false, true)   \
-    X(simon_drain_kernel_big,    320, 0, false, true,  false, true)   \
-    X(simon_drain_local_kernel_256, 256, 0, false, false, true, true)  \
-    X(simon_drain_local_kernel_320, 320, 0, false, false, true, true)  \
-    X(simon_drain_local_kernel_384, 384, 0, false, false, true, true)  \
-    X(simon_drain_local_kernel_big, 320, 0, false, true,  true, true)
+//   - Headroom probes (simon_probe_run): the same two, without and with the Open-Local code.
+#define SIMON_PLACE_VARIANTS(X)                                               \
+    X(simon_place_kernel_256_0,  256, 0, false, false, false, false, false)   \
+    X(simon_place_kernel_256_1,  256, 1, false, false, false, false, false)   \
+    X(simon_place_kernel_256_2,  256, 2, false, false, false, false, false)   \
+    X(simon_place_kernel_256_3,  256, 3, false, false, false, false, false)   \
+    X(simon_place_kernel_256_4,  256, 4, false, false, false, false, false)   \
+    X(simon_place_kernel_320_0,  320, 0, false, false, false, false, false)   \
+    X(simon_place_kernel_320_1,  320, 1, false, false, false, false, false)   \
+    X(simon_place_kernel_320_2,  320, 2, false, false, false, false, false)   \
+    X(simon_place_kernel_320_3,  320, 3, false, false, false, false, false)   \
+    X(simon_place_kernel_320_4,  320, 4, false, false, false, false, false)   \
+    X(simon_place_kernel_384_0,  384, 0, false, false, false, false, false)   \
+    X(simon_place_kernel_384_1,  384, 1, false, false, false, false, false)   \
+    X(simon_place_kernel_384_2,  384, 2, false, false, false, false, false)   \
+    X(simon_place_kernel_384_3,  384, 3, false, false, false, false, false)   \
+    X(simon_place_kernel_big,    320, 0, false, true,  false, false, false)   \
+    X(simon_prof_kernel_256_0,   256, 0, true,  false, false, false, false)   \
+    X(simon_prof_kernel_256_1,   256, 1, true,  false, false, false, false)   \
+    X(simon_prof_kernel_256_2,   256, 2, true,  false, false, false, false)   \
+    X(simon_prof_kernel_256_3,   256, 3, true,  false, false, false, false)   \
+    X(simon_prof_kernel_256_4,   256, 4, true,  false, false, false, false)   \
+    X(simon_prof_kernel_320_0,   320, 0, true,  false, false, false, false)   \
+    X(simon_prof_kernel_320_1,   320, 1, true,  false, false, false, false)   \
+    X(simon_prof_kernel_320_2,   320, 2, true,  false, false, false, false)   \
+    X(simon_prof_kernel_320_3,   320, 3, true,  false, false, false, false)   \
+    X(simon_prof_kernel_320_4,   320, 4, true,  false, false, false, false)   \
+    X(simon_local_kernel_256,    256, 0, false, false, true,  false, false)   \
+    X(simon_local_kernel_320,    320, 0, false, false, true,  false, false)   \
+    X(simon_local_kernel_384,    384, 0, false, false, true,  false, false)   \
+    X(simon_local_kernel_big,    320, 0, false, true,  true,  false, false)   \
+    X(simon_drain_kernel_256,    256, 0, false, false, false, true, false)    \
+    X(simon_drain_kernel_320,    320, 0, false, false, false, true, false)    \
+    X(simon_drain_kernel_384,    384, 0, false, false, false, true, false)    \
+    X(simon_drain_kernel_big,    320, 0, false, true,  false, true, false)    \
+    X(simon_drain_local_kernel_256, 256, 0, false, false, true, true, false)  \
+    X(simon_drain_local_kernel_320, 320, 0, false, false, true, true, false)  \
+    X(simon_drain_local_kernel_384, 384, 0, false, false, true, true, false)  \
+    X(simon_drain_local_kernel_big, 320, 0, false, true,  true, true, false)  \
+    X(simon_probe_kernel_256,    256, 0, false, false, false, false, true)    \
+    X(simon_probe_kernel_320,    320, 0, false, false, false, false, true)    \
+    X(simon_probe_kernel_384,    384, 0, false, false, false, false, true)    \
+    X(simon_probe_kernel_big,    320, 0, false, true,  false, false, true)    \
+    X(simon_probe_local_kernel_256, 256, 0, false, false, true, false, true)  \
+    X(simon_probe_local_kernel_320, 320, 0, false, false, true, false, true)  \
+    X(simon_probe_local_kernel_384, 384, 0, false, false, true, false, true)  \
+    X(simon_probe_local_kernel_big, 320, 0, false, true,  true, false, true)
 
-#define SK_DEFINE_VARIANT(name, threads, slots, prof, big, local, drain)                                   \
+#define SK_DEFINE_VARIANT(name, threads, slots, prof, big, local, drain, probe)                            \
     extern "C" __global__ void __launch_bounds__(threads, 1) name(const __grid_constant__ SkParams P) { \
-        simon_place_body<threads, slots, prof, big, local, drain>(P);                                    \
+        simon_place_body<threads, slots, prof, big, local, drain, probe>(P);                             \
     }
 SIMON_PLACE_VARIANTS(SK_DEFINE_VARIANT)
 #undef SK_DEFINE_VARIANT

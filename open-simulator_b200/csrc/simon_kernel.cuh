@@ -131,8 +131,11 @@ struct SkParams {
     // launch is one cluster: it reads slice 0)
     uint64_t vg_req_stride, node_stride;
     // drain batches (simon_drain_kernel_*): scenario s places pods drain_pods[drain_off[s] .. drain_off[s + 1]) (pod indices, in
-    // pod-list order); the per-pod outputs of SkScenario are indexed by the position in drain_pods, not by the pod
-    const uint32_t *drain_pods, *drain_off;
+    // pod-list order); the per-pod outputs of SkScenario are indexed by the position in drain_pods, not by the pod.
+    // probe batches (simon_probe_kernel_*): scenario s places replicas of pod probe_pod[s] at positions probe_off[s] .. probe_off[s + 1)
+    // of the per-pod outputs, and stops at the first one that does not fit
+    union { const uint32_t *drain_pods; const uint32_t *probe_pod; };
+    union { const uint32_t *drain_off; const uint32_t *probe_off; };
 };
 
 // the index of this thread-block cluster in the (1-D) grid: the scenario of the launch (blockIdx.x / cluster size)

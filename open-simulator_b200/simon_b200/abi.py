@@ -57,6 +57,8 @@ MOVE_GAIN_BIAS = 1000
 MOVES_SCOPE_GPU_SHARE, MOVES_SCOPE_HARD_SPREAD = 1, 2
 # simon_moves_plan stop reasons
 PLAN_STOP_NO_MOVE, PLAN_STOP_MAX_MOVES = 1, 2
+# simon_probe_run stop reasons
+PROBE_STOP_UNSCHEDULABLE, PROBE_STOP_MAX_REPLICAS = 1, 2
 
 
 class SimonSnapshot(C.Structure):
@@ -111,6 +113,15 @@ class SimonDrainResult(C.Structure):
 
 class SimonScenarioLocalResult(C.Structure):
     _fields_ = [("vg_requested", C.c_int64), ("vg_capacity", C.c_int64), ("reserved", C.c_uint64)]
+
+
+class SimonProbe(C.Structure):
+    _fields_ = [("pod", C.c_uint32), ("max_replicas", C.c_uint32)]
+
+
+class SimonProbeResult(C.Structure):
+    _fields_ = [("n_placed", C.c_uint32), ("stop_reason", C.c_uint32),
+                ("req_mcpu", C.c_int64), ("alloc_mcpu", C.c_int64), ("req_mem", C.c_int64), ("alloc_mem", C.c_int64)]
 
 
 class SimonMovesResult(C.Structure):
@@ -257,6 +268,9 @@ SIGNATURES = {
     "simon_drain_pdb_download": (_I, [_P, _U32, _P, _P]),
     "simon_drain_times": (_I, [_P, _PF, _PF]),
     "simon_drain_budget": (_I, [_P, _PU64, _PU64]),
+    "simon_probe_run": (_I, [_P, _P, _P, _U32, _P, _P]),
+    "simon_probe_download": (_I, [_P, _U32, _P, _P, _P, _P]),
+    "simon_probe_times": (_I, [_P, _PF, _PF]),
     "simon_pdbs_upload": (_I, [_P, _P]),
     "simon_pdbs_allowed": (_I, [_P, _P]),
     "simon_host_go118_sort": (_I, [_P, _U32, _P]),

@@ -63,6 +63,34 @@ EXTRA_MAX = (1 << 31) - 1 - 500
 PTS_COUNTS_MAX = (1 << 31) - 2
 
 
+# Compiled.class_pod_limit of a class no pod-count bound applies to
+POD_LIMIT_NONE = (1 << 62)
+
+
+def _soft_bound_ok(n_pods: int, mult: int, log_n: float) -> bool:
+    """The ScheduleAnyway spread bound for a list of n_pods pods: pods x summed multiplicity x ln(topology size + 2) stays in int32."""
+    return n_pods * mult * log_n < PTS_COUNTS_MAX
+
+
+def _ipa_bound_ok(n_pods: int, weights: int) -> bool:
+    """The InterPodAffinity bound for a list of n_pods pods: sum |weight| x pods stays in int32."""
+    return weights * max(1, n_pods) < (1 << 31)
+
+
+def _largest_ok(ok, lo: int) -> int:
+    """The largest n >= lo with ok(n), for a predicate that holds at lo and, once false, stays false (POD_LIMIT_NONE if it holds
+    that far)."""
+    hi = max(lo, 1)
+    while ok(hi):
+        if hi >= POD_LIMIT_NONE:
+            return POD_LIMIT_NONE
+        lo, hi = hi, min(2 * hi, POD_LIMIT_NONE)
+    while hi - lo > 1:                     # ok(lo), not ok(hi)
+        mid = (lo + hi) // 2
+        lo, hi = (mid, hi) if ok(mid) else (lo, mid)
+    return lo
+
+
 class CompileError(ValueError):
     pass
 
@@ -171,6 +199,9 @@ class Compiled:
     counters: List[Tuple[frozenset, int]]
     pod_recs: List[PodRec]
     storage: Optional[object] = None      # storage.StorageTables when compiled with open_local=True
+    # per class: the largest pod-list length for which the int32 bounds of its tables (ScheduleAnyway spread, InterPodAffinity scores)
+    # still hold, at least n_pods; a headroom probe that appends R replicas of a class needs n_pods + R within it
+    class_pod_limit: Optional[List[int]] = None
 
     def node_index(self, name: str) -> int:
         if not hasattr(self, "_nidx"):
@@ -984,6 +1015,7 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
     blob: List[int] = []
     class_off = [0]
     static_sigs = _Interner()
+    class_pod_limit = [POD_LIMIT_NONE] * len(classes)
     for c in classes:
         L = per_class[c.cid]
         w = [0] * SCW_HDR_WORDS
@@ -1050,8 +1082,11 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
         put(SCW_OFF_PTS_SOFT)
         w[SCW_N_PTS_SOFT] = len(L["soft"])
         # a pod adds up to its class's multiplicity in a summed counter: the bound counts every constraint that many times
-        if L["soft"] and len(pods) * sum(L["soft_mult"]) * math.log(N + 2 + extra_log) >= PTS_COUNTS_MAX:
+        soft_mult, soft_log = sum(L["soft_mult"]), math.log(N + 2 + extra_log)
+        if L["soft"] and not _soft_bound_ok(len(pods), soft_mult, soft_log):
             raise CompileError(f"class {c.cid}: topology spread scores of pod count x constraints can exceed 2^31")
+        if L["soft"]:
+            class_pod_limit[c.cid] = _largest_ok(lambda n: _soft_bound_ok(n, soft_mult, soft_log), len(pods))
         for e in L["soft"]:
             body.extend(e)
         put(SCW_OFF_IPA_AFF)
@@ -1072,8 +1107,11 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
         w[SCW_N_IPA_SCORE] = len(sc)
         # raw InterPodAffinity scores (sum of weight x matching pods, scoring.go:224-243) are kept as int32 on the device:
         # bound them by the number of pods of the list
-        if sum(abs(v) for _k, v in sc) * max(1, len(pods)) >= (1 << 31):
+        ipa_w = sum(abs(v) for _k, v in sc)
+        if not _ipa_bound_ok(len(pods), ipa_w):
             raise CompileError(f"class {c.cid}: inter-pod affinity weights x pod count can exceed 2^31")
+        if ipa_w:
+            class_pod_limit[c.cid] = min(class_pod_limit[c.cid], _largest_ok(lambda n: _ipa_bound_ok(n, ipa_w), len(pods)))
         for (kid, t), wt in sc:
             body.extend((kid, t, wt))
         put(SCW_OFF_INC)
@@ -1153,7 +1191,7 @@ def _compile_cluster(nodes: List[Obj], pods: List[PodRec], ctx: Optional[Cluster
     pods_dims = {"n_classes": C, "n_pods": len(pods), "n_counters": n_counters, "n_static_sigs": max(1, len(static_sigs.items)),
                  "n_static_rows": simon_raw.shape[0], "n_extra_rows": len(extra_rows)}
     return Compiled(N, node_names, order, snodes, snap, snap_dims, podset, pods_dims, classes, scalar_names,
-                    list(taint_ids.items), list(topo.items), list(counters.items), list(pods))
+                    list(taint_ids.items), list(topo.items), list(counters.items), list(pods), class_pod_limit=class_pod_limit)
 
 
 def _i64(x: int) -> int:

@@ -435,3 +435,64 @@ class Engine:
                 out.append(d)
         self.last_drain = info
         return out
+
+    # ---- headroom probes (simon_probe_run) ----
+    def probe_run(self, placed, probes, detail: bool = True, chunk: Optional[int] = None):
+        """Headroom probes on the live state `placed` (out_node of a full placement of the pod list): each entry of probes is (pod,
+        max_replicas), and places replicas of that pod one at a time on the state the ones before it leave, until one does not fit or
+        max_replicas are placed.  The list runs in batches sized as drain_run sizes them (chunk: an explicit batch size).  Refused
+        before any device work: n_pods + max_replicas past compiled.class_pod_limit of the pod's class (the int32 bounds of its
+        tables).  Returns one dict per probe: n_placed, stop_reason (abi.PROBE_STOP_*) and the sums req_mcpu / alloc_mcpu / req_mem /
+        alloc_mem over all nodes after the replicas, vg_requested / vg_capacity on a cluster compiled with open_local=True; with
+        detail also node and gpu_slots and score per replica [n_placed] and fail_counts [24], the histogram of the replica that stopped
+        it (zeros on MaxReplicas).  self.last_probe: chunks, scenario_bytes, setup_ms / place_ms (device time summed over the batches),
+        launches.  scenario_storage_state(i) then describes probe i of the last chunk."""
+        L = lib()
+        pl = np.ascontiguousarray(placed, dtype=np.int32)
+        probes = [(int(q), int(r)) for q, r in probes]
+        P = self.c.pods_dims["n_pods"]
+        limit = self.c.class_pod_limit
+        cls = self.c.pods["pod_class"]
+        for i, (q, r) in enumerate(probes):
+            if limit is not None and 0 <= q < P and r > 0 and P + r > limit[int(cls[q])]:
+                raise RuntimeError(f"probe {i}: {P} pods + {r} replicas of pod {q} exceed its class's int32 bounds "
+                                   f"({limit[int(cls[q])]} pods)")
+        local = getattr(self.c, "storage", None) is not None
+        n = len(probes)
+        per, free = self.drain_budget()
+        if chunk is None:
+            chunk = max(1, int(free * self.DRAIN_MEM_FRACTION) // max(per, 1))
+        out = []
+        info = dict(chunks=0, scenario_bytes=per, chunk=chunk, setup_ms=0.0, place_ms=0.0, launches=[])
+        for b in range(0, max(n, 1), chunk):
+            part = probes[b:b + chunk]
+            m = len(part)
+            arr = (abi.SimonProbe * max(m, 1))(*[abi.SimonProbe(q, r) for q, r in part])
+            res = (abi.SimonProbeResult * max(m, 1))()
+            loc = (abi.SimonScenarioLocalResult * max(m, 1))() if local else None
+            self._check(L.simon_probe_run(self.h, pl.ctypes.data, arr, m, res, loc))
+            if m == 0:
+                break
+            su, pm = C.c_float(0), C.c_float(0)
+            self._check(L.simon_probe_times(self.h, C.byref(su), C.byref(pm)))
+            info["chunks"] += 1
+            info["setup_ms"] += float(su.value)
+            info["place_ms"] += float(pm.value)
+            info["launches"].append(self.last_launch())
+            for i in range(m):
+                r = res[i]
+                d = dict(n_placed=r.n_placed, stop_reason=r.stop_reason, req_mcpu=r.req_mcpu, alloc_mcpu=r.alloc_mcpu,
+                         req_mem=r.req_mem, alloc_mem=r.alloc_mem)
+                if local:
+                    d["vg_requested"], d["vg_capacity"] = int(loc[i].vg_requested), int(loc[i].vg_capacity)
+                if detail:
+                    k = r.n_placed
+                    node = np.zeros(max(k, 1), np.int32)
+                    slots = np.zeros(max(k, 1), np.uint32)
+                    score = np.zeros(max(k, 1), np.int64)
+                    fc = np.zeros(abi.N_FAIL_CODES, np.uint32)
+                    self._check(L.simon_probe_download(self.h, i, node.ctypes.data, slots.ctypes.data, score.ctypes.data, fc.ctypes.data))
+                    d.update(node=node[:k], gpu_slots=slots[:k], score=score[:k], fail_counts=fc)
+                out.append(d)
+        self.last_probe = info
+        return out

@@ -606,6 +606,58 @@ class Simulator:
         moves = rebalance.candidates(compiled, self.placements, idx["sources"], idx["targets"])
         return rebalance.plan(eng, compiled, moves, max_moves, min_gain, move_scope, pdbs=self.pdb_tables)
 
+    # ---- scheduling headroom (this project's extension of the capacity-planning use case, README.md:14, to the live cluster) ----
+    def Headroom(self, probes: list, max_replicas: Optional[int] = None):
+        """Per entry a headroom.HeadroomResult: how many more replicas of a pod fit the session's live state, one at a time, until one
+        does not fit or max_replicas are placed (default: the cluster's free pod slots, which no probe can exceed).  An entry is a
+        workload reference "Kind/namespace/name" of the cluster or apps (its first pod is the probe pod; the live context runs it, no
+        recompile), or a Pod object used as a template: made valid as MakeValidPodByPod does and appended after the session's pods as
+        a pending pod, the list compiled on a device context of its own with the live placements as the prefix.  The session's engine,
+        compiled cluster and placements are not changed."""
+        from . import headroom
+        from .engine import Engine
+        eng, compiled = self._live()
+        if max_replicas is None:
+            max_replicas = max(1, headroom.free_pod_slots(compiled, self.placements))
+        if max_replicas < 1:
+            raise ValueError(f"Headroom: max_replicas must be at least 1 (got {max_replicas})")
+        refs = [(i, e) for i, e in enumerate(probes) if isinstance(e, str)]
+        tmpls = [(i, e) for i, e in enumerate(probes) if not isinstance(e, str)]
+        out: List = [None] * len(probes)
+        live = [(ref, q, max_replicas) for (_i, ref), q in zip(refs, headroom.workload_pods(compiled, [e for _i, e in refs]))]
+        guard = headroom.pod_guard(compiled)
+        for label, q, r in live:
+            headroom.check_probe(compiled, q, r, label, guard)
+        recs = []
+        for _i, pod in tmpls:
+            if ((pod.get("spec") or {}).get("nodeName") or ""):
+                raise ValueError(f"Headroom: template pod {O.name_of(pod)!r} sets spec.nodeName: it never reaches the scheduler")
+            recs.append(make_valid_pod_by_pod(pod))
+        if tmpls:
+            # the session's pod list plus the templates as pending pods, checked in full before any device work
+            p = self._plan()
+            storage_classes = None
+            if self.options.openLocal:
+                storage_classes = list(self.cluster.StorageClasss) + [sc for a in self.apps for sc in a.Resource.StorageClasss]
+            c2 = compile_cluster(p.nodes, p.pods + recs, p.ctx, extra_plugins=self._extra_plugins or None, open_local=self.options.openLocal,
+                                 storage_classes=storage_classes, local_devices=self.options.openLocalDevices)
+            n0 = len(p.pods)
+            extra = [(f"Pod/{r.tmpl.workload_namespace}/{r.name}", n0 + j, max_replicas) for j, r in enumerate(recs)]
+            for label, q, r in extra:
+                headroom.check_probe(c2, q, r, label)
+        self.last_headroom = []             # Engine.last_probe of each batch list this call ran (live context, then templates)
+        if live:
+            for (i, _e), res in zip(refs, headroom.run(eng, compiled, self.placements, live)):
+                out[i] = res
+            self.last_headroom.append(eng.last_probe)
+        if tmpls:
+            placed2 = np.concatenate([self.placements, np.full(len(recs), -1, np.int32)])
+            with Engine(c2, device=self.options.device) as eng2:
+                for (i, _e), res in zip(tmpls, headroom.run(eng2, c2, placed2, extra)):
+                    out[i] = res
+                self.last_headroom.append(eng2.last_probe)
+        return out
+
     def _check_local_volumes(self, local_volumes: bool, what: str):
         if local_volumes and not self.options.openLocal:
             raise ValueError(f"{what}: local_volumes=True needs a session WithOpenLocal (without it no pod has Open-Local volumes)")
