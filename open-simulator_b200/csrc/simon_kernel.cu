@@ -1201,16 +1201,17 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             // steady state: the summary is exact unless some node flipped feasibility since it was taken
             pts_pass(plo, phi);
             TICK(15);
-            // 6 words: the spread / affinity ranges, the flip flags and (net change of the counted set << 16) + flipped nodes
-            // (a scenario holds at most ~15,000 nodes, so both fields of the last word fit 16 bits)
-            uint32_t pv[7] = {e32(plo), e32(phi), w_enc((int32_t)ipa_lo), w_enc((int32_t)ipa_hi), my_fl, ((uint32_t)my_dc << 16) + my_nf, 0u};
+            // 6 words: the spread / affinity ranges, the flip flags and the flip word (net change of the counted set, flipped
+            // nodes: 16 / 16 bits in the shared-memory variants, 20 bits of flip count in the large one, simon_flip_word.h)
+            using FW = SkFlipWord<BIG>;
+            uint32_t pv[7] = {e32(plo), e32(phi), w_enc((int32_t)ipa_lo), w_enc((int32_t)ipa_hi), my_fl, FW::enc(my_dc, my_nf), 0u};
             {
                 const int pop[6] = {W_MIN, W_MAX, W_MIN, W_MAX, W_OR, W_SUM};
                 uint32_t (&pv6)[6] = reinterpret_cast<uint32_t (&)[6]>(pv);
                 sk_allreduce_w<6>(R, pv6, pop);
                 const uint32_t packed = pv[5];
-                pv[6] = packed & 0xffffu;
-                pv[5] = (uint32_t)((int32_t)(packed - pv[6]) >> 16);
+                pv[6] = FW::nf(packed);
+                pv[5] = (uint32_t)FW::dc(packed, pv[6]);
             }
             pts_min = w_dec(pv[0]); pts_max = w_dec(pv[1]); ipa_min = w_dec(pv[2]); ipa_max = w_dec(pv[3]);
             if (pv[4] & 1u) {

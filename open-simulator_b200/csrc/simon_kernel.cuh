@@ -15,6 +15,7 @@
 #include <stdint.h>
 
 #include "../../include/simon_gpu.h"
+#include "simon_flip_word.h"
 
 namespace cg = cooperative_groups;
 

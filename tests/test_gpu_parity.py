@@ -123,16 +123,20 @@ def test_full_size_c3_properties():
 
 
 def _cmp(c):
+    """Placements, every scheduled pod's score (zeros included: a pod with one feasible node is not scored), failure records
+    and state() against the oracle."""
     (ref, rscore, rfc, rfp), rstate = run_oracle(c)
     with _engine(c) as eng:
         out, score, fc, fp = eng.schedule()
         st = eng.state()
+        li = eng.last_launch()
     np.testing.assert_array_equal(out, ref)
+    np.testing.assert_array_equal(score[ref >= 0], rscore[ref >= 0])
     np.testing.assert_array_equal(fp, rfp)
     np.testing.assert_array_equal(fc, rfc)
     for k in rstate:
         np.testing.assert_array_equal(st[k], rstate[k], err_msg=k)
-    return out
+    return out, li
 
 
 def test_edge_empty_pod_list():
@@ -141,18 +145,18 @@ def test_edge_empty_pod_list():
     cluster, apps = synth.make_c2(n_nodes=5, n_workloads=0, replicas=1)
     p = simulator.plan(cluster, apps)
     c = compile_cluster(p.nodes, p.pods, p.ctx)
-    assert len(_cmp(c)) == 0
+    assert len(_cmp(c)[0]) == 0
 
 
 def test_edge_single_node_fills_up():
     p, c = make_case("c2", n_nodes=1, n_workloads=3, replicas=50, seed_no=2)
-    out = _cmp(c)
+    out = _cmp(c)[0]
     assert (out == 0).sum() > 0 and (out == -1).sum() > 0        # F == 1 short-circuit, then "Insufficient ..." for the rest
 
 
 def test_edge_no_nodes():
     p, c = make_case("c2", n_nodes=0, n_workloads=2, replicas=2, seed_no=2)
-    out = _cmp(c)
+    out = _cmp(c)[0]
     assert (out == -1).all()
 
 
@@ -170,10 +174,11 @@ def test_edge_zero_count_and_tail_calls():
 
 def test_large_cluster_variant_40k_nodes():
     """A scenario that does not fit the cluster's shared memory (40,000 nodes; round 1 refused it) runs on the large-cluster
-    variant - the same kernel with its per-node arrays in global memory - and reproduces the oracle bit for bit."""
+    variant - the same kernel with its per-node arrays in global memory - and reproduces the oracle bit for bit, scores included."""
     p, c = make_case("c3", n_nodes=40000, n_workloads=60, replicas=20, n_apps=2, seed_no=7)
-    out = _cmp(c)
+    out, li = _cmp(c)
     assert (out >= 0).sum() > 1000
+    assert li["large"] and li["node_slots"] == 8, li
 
 
 def test_limit_too_many_nodes_is_an_error_not_a_fallback():
