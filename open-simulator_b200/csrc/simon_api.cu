@@ -560,13 +560,13 @@ const sk_variant sk_variants[] = {SIMON_PLACE_VARIANTS(SK_VARIANT_ENTRY)};
 // there is one and run-time slots otherwise.  big: the large-cluster variant, at any thread count; prof: with per-phase timers
 // (256 and 320 threads only).  PLACE: with Open-Local storage uploaded, the local variants (no timers).  DRAIN: the drain-batch
 // variants without Open-Local code (simon_drain_run), whatever was uploaded; DRAIN_LOCAL: those with it (simon_drain_run_local); PROBE
-// and PROBE_LOCAL likewise for probe batches.  big and the drain and probe families ignore prof.  nullptr: none.
+// and PROBE_LOCAL likewise for probe batches.  Where no variant with timers exists (big, 384 threads, the local, drain and probe
+// families), prof falls back to the variant without them, which last_launch() names.  nullptr: none.
 const sk_variant *kernel_variant(const simon_ctx *ctx, uint32_t TPB, uint32_t npt, bool big, bool prof, Family fam) {
     if (!big && TPB > SIMON_MAX_TPB) return nullptr;
     const uint32_t threads = TPB <= 256 ? 256 : TPB <= 320 ? 320 : 384;
     const bool drain = fam == DRAIN || fam == DRAIN_LOCAL, probe = fam == PROBE || fam == PROBE_LOCAL;
     const bool local = fam == DRAIN_LOCAL || fam == PROBE_LOCAL || (fam == PLACE && ctx->valid.has(STORAGE));
-    if (big || drain || probe) prof = false;
     const sk_variant *runtime_slots = nullptr;
     for (const sk_variant &v : sk_variants) {
         if (v.big != big || v.drain != drain || v.probe != probe || v.local != local || v.prof != prof || (!big && v.threads != threads))
@@ -574,6 +574,7 @@ const sk_variant *kernel_variant(const simon_ctx *ctx, uint32_t TPB, uint32_t np
         if (v.slots == npt) return &v;
         if (v.slots == 0) runtime_slots = &v;
     }
+    if (!runtime_slots && prof) return kernel_variant(ctx, TPB, npt, big, false, fam);
     return runtime_slots;
 }
 
@@ -736,11 +737,11 @@ static_assert(sizeof(SkScenario) % 8 == 0, "SkScenario is copied in 8-byte words
 // carries probe_pod / probe_off)
 int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t TPB, size_t smem, bool record = true, Family fam = PLACE) {
     // SIMON_PROFILE=1 selects the variants with per-phase clock64 timers (simon_stats cycles); the default variants
-    // carry no timers
+    // carry no timers.  A shape or family without a timer variant runs the default one (last_launch().kernel names it)
     static const bool prof = getenv("SIMON_PROFILE") != nullptr;
     const sk_variant *v = kernel_variant(ctx, TPB, P.npt, ctx->big, prof, fam);
     if (!v)
-        return fail(ctx, SIMON_ERR_LIMIT, "no kernel variant for %u threads per CTA%s%s", TPB, prof ? " with phase timers" : "",
+        return fail(ctx, SIMON_ERR_LIMIT, "no kernel variant for %u threads per CTA%s", TPB,
                     (fam == DRAIN_LOCAL || fam == PROBE_LOCAL || (fam == PLACE && ctx->valid.has(STORAGE))) ? " and Open-Local storage" : "");
     if (ctx->big) {
         CU(ctx->d_gnode.alloc(ctx->gnode_stride * (size_t)n_scen * CS));
