@@ -369,6 +369,48 @@ int simon_state_download_ext(simon_ctx *ctx, int64_t *req_scalar, int64_t *gpu_u
 int simon_debug_set_dump_pod(simon_ctx *ctx, uint32_t pod);
 int simon_debug_dump_read(simon_ctx *ctx, int64_t *out_total, int32_t *out_code);
 
+/* ---- explained placement decisions (klog V(10) of prioritizeNodes, generic_scheduler.go:502-506, 558-562) ----------------------
+ * An explained pod is a pod of the uploaded list in the set of simon_explain_set.  Every later simon_schedule or
+ * simon_schedule_resume call that places it decides it exactly as without the set, and also writes one record for it:
+ *   node      its out_node (-1 unschedulable, -2 / -3 or its node for a pod that never reaches the scheduler);
+ *             SIMON_EXPLAIN_NOT_RUN while no call has covered the pod (the pods of a resume prefix are not run: a resume writes the
+ *             marker into their records)
+ *   feasible  F, the number of nodes that pass every filter
+ *   rejected  for each simon_fail_code, the number of active nodes whose filter verdict carries it (the FitError histogram; for an
+ *             unschedulable pod it equals that pod's out_fail_counts row)
+ *   n_top     min(top_k, F): the entries of the pod's simon_explain_node rows that are filled
+ * and top_k simon_explain_node rows: the best feasible nodes by total descending, ties to the earlier node in scenario (nodeTree)
+ * order (the scheduler's arg-max: row 0 is the placed node and its total is out_score).  words[] are the per-node terms in the order of
+ * the oracle's detail: [0] BalancedAllocation [1] LeastAllocated [2] InterPodAffinity [3] NodeAffinity [4] PodTopologySpread before
+ * its weight of 2 [5] TaintToleration [6] Simon (= Open-Gpu-Share; each has weight 1) [7] the static row (ImageLocality +
+ * NodePreferAvoidPods x 10000 + the host-side extra score plugins, already weighted) [8] total [9] Open-Local.  With F == 1 nothing
+ * is scored (generic_scheduler.go:159-165): the one row holds the node with all words 0.
+ * Scenario batches, drains, probes, moves and plans ignore the set; a call whose range holds no explained pod launches what it
+ * launches without one. */
+#define SIMON_EXPLAIN_MAX_TOP 16
+#define SIMON_EXPLAIN_WORDS 10
+#define SIMON_EXPLAIN_NOT_RUN (-4)
+typedef struct simon_explain_record {
+    int32_t node;
+    uint32_t feasible;
+    uint32_t n_top;
+    uint32_t reserved;
+    uint32_t rejected[24];              /* SIMON_N_FAIL_CODES */
+} simon_explain_record;
+typedef struct simon_explain_node {
+    int32_t node;
+    uint32_t reserved;
+    int64_t words[10];                  /* SIMON_EXPLAIN_WORDS */
+} simon_explain_node;
+/* Set the explained pods: pods[n] strictly ascending pod indices < n_pods, 1 <= top_k <= SIMON_EXPLAIN_MAX_TOP; n = 0 clears the set.
+ * Needs a pod upload (SIMON_ERR_STATE); an accepted pod upload drops the set.  SIMON_ERR_INVALID with a message, before any device
+ * work, leaving the context as it was: pods NULL with n > 0, not strictly ascending or out of range, top_k out of range.  Every record
+ * starts as SIMON_EXPLAIN_NOT_RUN. */
+int simon_explain_set(simon_ctx *ctx, const uint32_t *pods, uint32_t n, uint32_t top_k);
+/* Records [first, first + count) of the set (in the order of `pods`) and their nodes [count][top_k]; either pointer may be NULL.
+ * SIMON_ERR_STATE without a set, SIMON_ERR_INVALID past its end. */
+int simon_explain_download(simon_ctx *ctx, uint32_t first, uint32_t count, simon_explain_record *records, simon_explain_node *nodes);
+
 /* ---- candidate-move scoring for defragmentation / rebalancing (BASELINE config 5) ----------------------------------
  * The reference names the use case (README.md:16) and provides the primitive, NodeInfo.RemovePod
  * (K8S/framework/types.go:539-585); it has no implementation of the scoring itself, so the definition is this library's:

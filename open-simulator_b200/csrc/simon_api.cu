@@ -245,6 +245,7 @@ enum Data : uint32_t {
     SCOPE_PREP = 1u << 8,       // what the move scope launches, for the current scope and move-class records
     STATIC_FILL = 1u << 9,      // the static verdicts of every (signature, node) pair are in the pod set's scache
     STORAGE_BATCH = 1u << 10, DRAIN_BATCH = 1u << 11, PLAN = 1u << 12, PROBE_BATCH = 1u << 13,
+    EXPLAIN_SET = 1u << 14,     // simon_explain_set's pods, records and device tables
 };
 
 struct Validity {
@@ -255,7 +256,7 @@ struct Validity {
     void drop(uint32_t d) {
         static constexpr uint32_t derived[][2] = {
             {SNAPSHOT, POD_SET},
-            {POD_SET, STORAGE | PDB_TABLE | LIVE | PLAN | DRAIN_BATCH | PROBE_BATCH | MOVE_LIST | SCOPE_PREP | STATIC_FILL},
+            {POD_SET, STORAGE | PDB_TABLE | LIVE | PLAN | DRAIN_BATCH | PROBE_BATCH | MOVE_LIST | SCOPE_PREP | STATIC_FILL | EXPLAIN_SET},
             {STORAGE, DEVICES | STORAGE_BATCH | LIVE | SCOPE_PREP},     // SCOPE_PREP: the move-class records exclude local classes
             {DEVICES, STORAGE_BATCH | LIVE},
             {MOVE_LIST, MOVE_RUN},
@@ -291,7 +292,7 @@ struct simon_ctx {
         // per pod: the uploaded pod_fixed_node and guard (what a resume prefix entry is checked against), the class, whether it never
         // reaches the scheduler in a single-scenario run (pre-bound or absent); fixed_dev: pod_fixed_node with the pinned-run marks
         // (-4) before a storage upload takes its local classes off (d_pod_fixed holds the result)
-        std::vector<int32_t> h_fixed, h_guard, h_class, fixed_dev;
+        std::vector<int32_t> h_fixed, h_guard, h_class, fixed_dev, fixed_cur;     // fixed_cur: what d_pod_fixed holds
         std::vector<uint8_t> bypass;
         DevBuf<uint32_t> d_sig_class;       // a class per static signature (dense fill of the static verdict cache)
         uint32_t max_fail = 0;
@@ -387,6 +388,19 @@ struct simon_ctx {
         DevBuf<uint32_t> slots, ctl;
         DevBuf<simon_plan_step> steps;
     } plan;
+    // explained pods (simon_explain_set): the pods, top_k, each record's initial value (SIMON_EXPLAIN_NOT_RUN); on the device the
+    // SkExplain tables, the records, their node rows and the per-node scratch
+    struct {
+        std::vector<uint32_t> pods;
+        uint32_t top_k = 0;
+        std::vector<simon_explain_record> h_init;
+        DevBuf<int32_t> d_slot, d_fixed;      // d_fixed: the pod_fixed of explained launches (explain_fixed)
+        DevBuf<simon_explain_record> d_rec;
+        DevBuf<simon_explain_node> d_nodes;
+        DevBuf<long long> d_total;
+        DevBuf<int2> d_pts_ipa;
+        DevBuf<SkExplain> d_x;
+    } explain;
     // scenario state: single runs (simon_schedule, simon_replay, ...) and scenario batches
     ScenPool single, batch;
     // launch scratch of no upload: resumed runs' prefix on the device and its per-node grouping (counts, offsets, fill cursors, pod
@@ -549,9 +563,10 @@ typedef void (*sk_kernel_fn)(const SkParams);
 // state, so no other call can launch a drain kernel): the placement variants (the local ones with storage uploaded), the drain-batch
 // variants without Open-Local code (simon_drain_run), or those with it (simon_drain_run_local), and the same two of the headroom-probe
 // variants (simon_probe_run)
-enum Family { PLACE, DRAIN, DRAIN_LOCAL, PROBE, PROBE_LOCAL };
-struct sk_variant { sk_kernel_fn fn; const char *name; uint32_t threads, slots; bool prof, big, local, drain, probe; };
-#define SK_VARIANT_ENTRY(name, threads, slots, prof, big, local, drain, probe) {name, #name, threads, slots, prof, big, local, drain, probe},
+// EXPLAIN: the explained-decision variants of a single run whose range holds an explained pod (the local ones with storage uploaded)
+enum Family { PLACE, DRAIN, DRAIN_LOCAL, PROBE, PROBE_LOCAL, EXPLAIN };
+struct sk_variant { sk_kernel_fn fn; const char *name; uint32_t threads, slots; bool prof, big, local, drain, probe, explain; };
+#define SK_VARIANT_ENTRY(name, threads, slots, prof, big, local, drain, probe, explain) {name, #name, threads, slots, prof, big, local, drain, probe, explain},
 const sk_variant sk_variants[] = {SIMON_PLACE_VARIANTS(SK_VARIANT_ENTRY)};
 #undef SK_VARIANT_ENTRY
 
@@ -565,11 +580,12 @@ const sk_variant sk_variants[] = {SIMON_PLACE_VARIANTS(SK_VARIANT_ENTRY)};
 const sk_variant *kernel_variant(const simon_ctx *ctx, uint32_t TPB, uint32_t npt, bool big, bool prof, Family fam) {
     if (!big && TPB > SIMON_MAX_TPB) return nullptr;
     const uint32_t threads = TPB <= 256 ? 256 : TPB <= 320 ? 320 : 384;
-    const bool drain = fam == DRAIN || fam == DRAIN_LOCAL, probe = fam == PROBE || fam == PROBE_LOCAL;
-    const bool local = fam == DRAIN_LOCAL || fam == PROBE_LOCAL || (fam == PLACE && ctx->valid.has(STORAGE));
+    const bool drain = fam == DRAIN || fam == DRAIN_LOCAL, probe = fam == PROBE || fam == PROBE_LOCAL, explain = fam == EXPLAIN;
+    const bool local = fam == DRAIN_LOCAL || fam == PROBE_LOCAL || ((fam == PLACE || explain) && ctx->valid.has(STORAGE));
     const sk_variant *runtime_slots = nullptr;
     for (const sk_variant &v : sk_variants) {
-        if (v.big != big || v.drain != drain || v.probe != probe || v.local != local || v.prof != prof || (!big && v.threads != threads))
+        if (v.big != big || v.drain != drain || v.probe != probe || v.explain != explain || v.local != local || v.prof != prof ||
+            (!big && v.threads != threads))
             continue;
         if (v.slots == npt) return &v;
         if (v.slots == 0) runtime_slots = &v;
@@ -742,7 +758,7 @@ int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t T
     const sk_variant *v = kernel_variant(ctx, TPB, P.npt, ctx->big, prof, fam);
     if (!v)
         return fail(ctx, SIMON_ERR_LIMIT, "no kernel variant for %u threads per CTA%s", TPB,
-                    (fam == DRAIN_LOCAL || fam == PROBE_LOCAL || (fam == PLACE && ctx->valid.has(STORAGE))) ? " and Open-Local storage" : "");
+                    (fam == DRAIN_LOCAL || fam == PROBE_LOCAL || ((fam == PLACE || fam == EXPLAIN) && ctx->valid.has(STORAGE))) ? " and Open-Local storage" : "");
     if (ctx->big) {
         CU(ctx->d_gnode.alloc(ctx->gnode_stride * (size_t)n_scen * CS));
         P.gnode = ctx->d_gnode.p; P.gnode_stride = ctx->gnode_stride;
@@ -762,11 +778,26 @@ int launch(simon_ctx *ctx, SkParams &P, uint32_t n_scen, uint32_t CS, uint32_t T
     return SIMON_OK;
 }
 
+// The explained pods of the set in [first, first + count): the set's records [lo, hi) (it is ascending)
+void explain_range(const simon_ctx *ctx, uint32_t first, uint32_t count, uint32_t &lo, uint32_t &hi) {
+    const std::vector<uint32_t> &v = ctx->explain.pods;
+    lo = hi = 0;
+    if (!ctx->valid.has(EXPLAIN_SET)) return;
+    lo = (uint32_t)(std::lower_bound(v.begin(), v.end(), first) - v.begin());
+    hi = (uint32_t)(std::lower_bound(v.begin(), v.end(), first + count) - v.begin());
+}
+
 // Place pods [first, first + count) of the single scenario: a long leading run of pods that bypass the scheduler is
-// accounted by the parallel import kernel, the rest by the persistent placement kernel.
-int launch_range(simon_ctx *ctx, SkParams &P, uint32_t CS, uint32_t TPB, size_t smem, uint32_t first, uint32_t count, bool record) {
+// accounted by the parallel import kernel, the rest by the persistent placement kernel.  explain: the run honours the explained-pod
+// set (simon_schedule, simon_schedule_resume): when the range holds an explained pod, the placement kernel is an explained-decision
+// variant and the leading run stops before the first explained pod, whose record the kernel writes.
+int launch_range(simon_ctx *ctx, SkParams &P, uint32_t CS, uint32_t TPB, size_t smem, uint32_t first, uint32_t count, bool record,
+                 bool explain = false) {
+    uint32_t lo = 0, hi = 0;
+    if (explain) explain_range(ctx, first, count, lo, hi);
+    const uint32_t pre_end = hi > lo ? ctx->explain.pods[lo] - first : count;
     uint32_t n_pre = 0;
-    while (n_pre < count && ctx->pods.bypass[first + n_pre]) n_pre++;
+    while (n_pre < pre_end && ctx->pods.bypass[first + n_pre]) n_pre++;
     if (n_pre < 256) n_pre = 0;
     if (record) CU(cudaEventRecord(ctx->ev0, ctx->stream));
     if (n_pre) {
@@ -777,7 +808,19 @@ int launch_range(simon_ctx *ctx, SkParams &P, uint32_t CS, uint32_t TPB, size_t 
     }
     if (count > n_pre) {
         P.first = first + n_pre; P.count = count - n_pre;
-        int rc = launch(ctx, P, 1, CS, TPB, smem, false);
+        Family fam = PLACE;
+        if (hi > lo) {
+            // the records of this range start empty (their node rows zero, the reason counts 0) and the kernel fills them
+            cudaStream_t st = ctx->stream;
+            CU(cudaMemcpyAsync(ctx->explain.d_rec.p + lo, ctx->explain.h_init.data() + lo, sizeof(simon_explain_record) * (hi - lo),
+                               cudaMemcpyHostToDevice, st));
+            CU(cudaMemsetAsync(ctx->explain.d_nodes.p + (size_t)lo * ctx->explain.top_k, 0,
+                               sizeof(simon_explain_node) * (size_t)(hi - lo) * ctx->explain.top_k, st));
+            P.pod_fixed = ctx->explain.d_fixed.p;      // explained pods leave pinned runs (explain_fixed)
+            P.explain = ctx->explain.d_x.p;
+            fam = EXPLAIN;
+        }
+        int rc = launch(ctx, P, 1, CS, TPB, smem, false, fam);
         if (rc) return rc;
     }
     if (record) CU(cudaEventRecord(ctx->ev1, ctx->stream));
@@ -960,6 +1003,8 @@ int simon_snapshot_upload(simon_ctx *ctx, const simon_snapshot *s) {
 // The device copy of pod_fixed_node and the move-class records (with their bits on the host) from the pod set's, with the classes
 // of class_local (nullptr: none) taken off: pods of classes with local storage read the VGs of every node, so they leave the
 // pinned-run fast path (-4) and are never candidates of the move scoring
+static int explain_fixed(simon_ctx *ctx);
+
 static int upload_class_marks(simon_ctx *ctx, const uint8_t *class_local) {
     auto &ps = ctx->pods;
     std::vector<int32_t> fixed(ps.fixed_dev);
@@ -974,7 +1019,8 @@ static int upload_class_marks(simon_ctx *ctx, const uint8_t *class_local) {
     CU(ps.d_pod_fixed.upload(fixed.data(), ps.n_pods, ctx->stream));
     CU(ps.d_mv_classes.upload(mc.data(), mc.size(), ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));      // `fixed` and `mc` leave scope
-    return SIMON_OK;
+    ps.fixed_cur = std::move(fixed);
+    return ctx->valid.has(EXPLAIN_SET) ? explain_fixed(ctx) : SIMON_OK;
 }
 
 int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
@@ -1214,7 +1260,7 @@ int simon_schedule(simon_ctx *ctx, uint32_t first, uint32_t count, int32_t *out_
     fill_params(ctx, ctx->single, P);
     P.first = first; P.count = count; P.max_fail = ctx->pods.max_fail; P.npt = NPT;
     CU(single_begin(ctx, P, first, count));
-    rc = launch_range(ctx, P, CS, TPB, smem, first, count, true);
+    rc = launch_range(ctx, P, CS, TPB, smem, first, count, true, true);
     if (rc) return rc;
     return single_end(ctx, first, count, out_node, out_score, out_fail_counts, out_fail_pod, max_fail, out_n_fail);
 }
@@ -1242,11 +1288,17 @@ int simon_schedule_resume(simon_ctx *ctx, const int32_t *prefix_node, uint32_t n
     rc = clear_pool(ctx, S);
     if (rc) return rc;
     CU(single_begin(ctx, P, first, count));
+    if (ctx->valid.has(EXPLAIN_SET)) {
+        // the prefix's pods are not run: their records go back to SIMON_EXPLAIN_NOT_RUN (the rest is reset by launch_range)
+        uint32_t lo, hi;
+        explain_range(ctx, first, count, lo, hi);
+        if (lo) CU(cudaMemcpyAsync(ctx->explain.d_rec.p, ctx->explain.h_init.data(), sizeof(simon_explain_record) * lo, cudaMemcpyHostToDevice, st));
+    }
     CU(cudaEventRecord(ctx->ev0, st));
     rc = rebuild_prefix(ctx, P, prefix_node, n_prefix);
     if (rc) return rc;
     if (count) {
-        rc = launch_range(ctx, P, CS, TPB, smem, first, count, false);
+        rc = launch_range(ctx, P, CS, TPB, smem, first, count, false, true);
         if (rc) return rc;
     }
     CU(cudaEventRecord(ctx->ev1, st));
@@ -1919,6 +1971,67 @@ int simon_debug_dump_read(simon_ctx *ctx, int64_t *out_total, int32_t *out_code)
     CU(cudaSetDevice(ctx->device));
     if (out_total) CU(cudaMemcpy(out_total, ctx->pods.d_dump_total.p, 8ull * ctx->snap.N, cudaMemcpyDeviceToHost));
     if (out_code) CU(cudaMemcpy(out_code, ctx->pods.d_dump_code.p, 4ull * ctx->snap.N, cudaMemcpyDeviceToHost));
+    return SIMON_OK;
+}
+
+// The pod_fixed of launches that hold explained pods: d_pod_fixed with the explained pods marked -1 (a pod the scheduler places)
+// instead of -4 (a pod of a pinned run), so that they leave pinned runs as the debug dump pod does.  Built when the set is set and
+// again when a storage upload changes the marks.
+static int explain_fixed(simon_ctx *ctx) {
+    std::vector<int32_t> fx(ctx->pods.fixed_cur);
+    for (uint32_t q : ctx->explain.pods)
+        if (fx[q] == -4) fx[q] = -1;
+    CU(ctx->explain.d_fixed.upload(fx.data(), fx.size(), ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));      // `fx` leaves scope
+    return SIMON_OK;
+}
+
+int simon_explain_set(simon_ctx *ctx, const uint32_t *pods, uint32_t n, uint32_t top_k) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_explain_set before a pod upload");
+    const uint32_t P = ctx->pods.n_pods;
+    if (n == 0) { ctx->valid.drop(EXPLAIN_SET); ctx->explain.pods.clear(); return SIMON_OK; }
+    if (!pods) return fail(ctx, SIMON_ERR_INVALID, "simon_explain_set: pods is NULL");
+    if (top_k < 1 || top_k > SIMON_EXPLAIN_MAX_TOP) return fail(ctx, SIMON_ERR_INVALID, "simon_explain_set: top_k %u outside [1, %u]", top_k, SIMON_EXPLAIN_MAX_TOP);
+    for (uint32_t i = 0; i < n; i++) {
+        if (pods[i] >= P) return fail(ctx, SIMON_ERR_INVALID, "simon_explain_set: pod %u out of range (%u pods)", pods[i], P);
+        if (i && pods[i] <= pods[i - 1]) return fail(ctx, SIMON_ERR_INVALID, "simon_explain_set: pods not strictly ascending at entry %u", i);
+    }
+    CU(cudaSetDevice(ctx->device));
+    ctx->valid.drop(EXPLAIN_SET);
+    auto &X = ctx->explain;
+    cudaStream_t st = ctx->stream;
+    const uint32_t N1 = std::max(1u, ctx->snap.N);
+    std::vector<int32_t> slot(std::max(1u, P), -1);
+    for (uint32_t i = 0; i < n; i++) slot[pods[i]] = (int32_t)i;
+    simon_explain_record init{};
+    init.node = SIMON_EXPLAIN_NOT_RUN;
+    X.h_init.assign(n, init);
+    CU(X.d_slot.upload(slot.data(), slot.size(), st));
+    CU(X.d_rec.upload(X.h_init.data(), n, st));
+    CU(X.d_nodes.alloc((size_t)n * top_k));
+    CU(cudaMemsetAsync(X.d_nodes.p, 0, sizeof(simon_explain_node) * (size_t)n * top_k, st));
+    CU(X.d_total.alloc(N1)); CU(X.d_pts_ipa.alloc(N1));
+    SkExplain x{X.d_slot.p, X.d_rec.p, X.d_nodes.p, X.d_total.p, X.d_pts_ipa.p, top_k, 0};
+    CU(X.d_x.upload(&x, 1, st));
+    CU(cudaStreamSynchronize(st));      // `slot` and `x` leave scope
+    X.pods.assign(pods, pods + n);
+    X.top_k = top_k;
+    const int rc = explain_fixed(ctx);
+    if (rc) return rc;
+    ctx->valid.set(EXPLAIN_SET);
+    return SIMON_OK;
+}
+
+int simon_explain_download(simon_ctx *ctx, uint32_t first, uint32_t count, simon_explain_record *records, simon_explain_node *nodes) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(EXPLAIN_SET)) return fail(ctx, SIMON_ERR_STATE, "no explained-pod set");
+    const auto &X = ctx->explain;
+    if ((uint64_t)first + count > X.pods.size()) return fail(ctx, SIMON_ERR_INVALID, "records [%u, %u + %u) past the set of %zu", first, first, count, X.pods.size());
+    if (!count) return SIMON_OK;
+    CU(cudaSetDevice(ctx->device));
+    if (records) CU(cudaMemcpy(records, X.d_rec.p + first, sizeof(simon_explain_record) * count, cudaMemcpyDeviceToHost));
+    if (nodes) CU(cudaMemcpy(nodes, X.d_nodes.p + (size_t)first * X.top_k, sizeof(simon_explain_node) * (size_t)count * X.top_k, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 

@@ -279,10 +279,16 @@ struct ClassState {
 // state, one position of its output range each, until one does not fit.  A probe pod reaches the scheduler and is not pinned, so
 // the pinned-run and bypass blocks are compiled out as under DRAIN.  The stop is taken inside the C.F == 0 branch, which every thread
 // of the cluster takes at the same iteration (see there).  LOCAL and PROBE together: as LOCAL and DRAIN
-template <int MAXT, int NPT_T, bool PROF, bool BIG = false, bool LOCAL = false, bool DRAIN = false, bool PROBE = false>
+// EXPLAIN: the variants of single-scenario runs whose range holds an explained pod (simon_explain_set, SkParams::explain).  Such a pod
+// is decided as in every other variant; in addition its decision writes the filter-reason histogram of every node, and after the
+// arg-max, top_k - 1 further cluster arg-max rounds below the previous key find the next best nodes, whose owners write their plugin
+// terms.  Explained pods leave pinned runs, as the debug dump pod does: the launch's pod_fixed marks them -1 instead of -4.
+template <int MAXT, int NPT_T, bool PROF, bool BIG = false, bool LOCAL = false, bool DRAIN = false, bool PROBE = false, bool EXPLAIN = false>
 __device__ __forceinline__ void simon_place_body(const SkParams &P) {
     constexpr uint32_t CLS_LOCAL = LOCAL ? SK_CLS_LOCAL : 0u;
     constexpr bool LIST = DRAIN || PROBE;      // the scenario's own pod stream, every pod of it scheduler-placed
+    static_assert(!(EXPLAIN && (LIST || PROF)), "explained decisions are single-scenario runs without timers");
+    const SkExplain *const X = EXPLAIN ? P.explain : nullptr;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     cg::cluster_group cluster = cg::this_cluster();
     const uint32_t CS = cluster.num_blocks();
@@ -362,7 +368,8 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
 
     // NodeResourcesFit verdict + LeastAllocated + BalancedAllocation of one node for the current class, with `add` more
     // pods of this class already on the node (add = 0: the node as it is; add = 1: as it will be after winning this pod).
-    auto own_core = [&](uint32_t idx, int64_t add, bool &fit_out, int32_t &own_out) {
+    // parts != nullptr (explained decisions): also parts[0] = BalancedAllocation, parts[1] = LeastAllocated
+    auto own_core = [&](uint32_t idx, int64_t add, bool &fit_out, int32_t &own_out, int64_t *parts = nullptr) {
         bool fit = !(A32(B_NUM_PODS, idx) + (int32_t)add + 1 > A32(B_ALLOC_PODS, idx));
         const int64_t capc = A64(A_ALLOC_MCPU, idx), capm = A64(A_ALLOC_MEM, idx);
         if (fit && (C.cflags & SIMON_CLS_HAS_REQUEST)) {
@@ -398,6 +405,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
             }
             ba = (int64_t)fl;
         }
+        if (parts) { parts[0] = ba; parts[1] = la; }
         fit_out = fit;
         own_out = (int32_t)(la + ba);
     };
@@ -614,6 +622,19 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
     int32_t nx_cls = P.pod_class[q0], nx_fixed = P.pod_fixed[q0], nx_guard = P.pod_guard[q0];
     uint64_t nx_off = P.class_off[nx_cls];
     // static-normalised part of the total (NodeAffinity + TaintToleration + 2 x Simon + extra) under the current normalisers
+    // NodeAffinity, TaintToleration and Simon of node idx under the current normalisers, declared as na, tt, sm (range, small, na32: as
+    // snorm_pass sets them).  Written as statements in place, not as a call: snorm_pass compiles to the same code as before explained
+    // decisions existed, which a lambda call does not.
+#define SK_SNORM_TERMS(idx, range, small, na32)                                                                                      \
+    /* raw NodeAffinity scores are 0 .. 2^31 - 1: 100 x raw fits 32 bits while na_max (>= raw on feasible nodes) does */               \
+    const uint32_t na_raw = (uint32_t)A32(B_RAW_NA, idx);                                                                            \
+    int64_t na = C.na_max == 0 ? (int64_t)na_raw                                                                                     \
+               : na32 ? (int64_t)((100u * na_raw) / (uint32_t)C.na_max) : (int64_t)((100ull * na_raw) / (uint64_t)C.na_max);      \
+    int64_t tt = C.tt_max == 0 ? 100 : 100 - (int64_t)((uint32_t)(100 * A32(B_RAW_TT, idx)) / (uint32_t)C.tt_max);                 \
+    int64_t sm;                                                                                                                      \
+    if (range == 0) sm = 0;                                                                                                          \
+    else if (small) sm = (int64_t)((uint32_t)((uint32_t)(A64(A_SIMON, idx) - C.simon_min) * 100u) / (uint32_t)range);              \
+    else sm = ((A64(A_SIMON, idx) - C.simon_min) * 100) / range
     auto snorm_pass = [&]() {
         const int64_t range = C.simon_max - C.simon_min;
         const bool small = range > 0 && range < (1ll << 24) && C.simon_max < (1ll << 24) && C.simon_min >= 0;
@@ -622,15 +643,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
         for (uint32_t s = 0; s < NPT; s++) {
             uint32_t idx = s * TPB + tid;
             if (!(A8(C_NFLAGS, idx) & NF_VALID)) continue;
-            // raw NodeAffinity scores are 0 .. 2^31 - 1: 100 x raw fits 32 bits while na_max (>= raw on feasible nodes) does
-            const uint32_t na_raw = (uint32_t)A32(B_RAW_NA, idx);
-            int64_t na = C.na_max == 0 ? (int64_t)na_raw
-                       : na32 ? (int64_t)((100u * na_raw) / (uint32_t)C.na_max) : (int64_t)((100ull * na_raw) / (uint64_t)C.na_max);
-            int64_t tt = C.tt_max == 0 ? 100 : 100 - (int64_t)((uint32_t)(100 * A32(B_RAW_TT, idx)) / (uint32_t)C.tt_max);
-            int64_t sm;
-            if (range == 0) sm = 0;
-            else if (small) sm = (int64_t)((uint32_t)((uint32_t)(A64(A_SIMON, idx) - C.simon_min) * 100u) / (uint32_t)range);
-            else sm = ((A64(A_SIMON, idx) - C.simon_min) * 100) / range;
+            SK_SNORM_TERMS(idx, range, small, na32);
             A32(B_SNORM, idx) = (int32_t)(na + tt + 2 * sm + (int64_t)A32(B_EXTRA, idx));
         }
         C.nm_na_max = C.na_max; C.nm_tt_max = C.tt_max; C.nm_simon_min = C.simon_min; C.nm_simon_max = C.simon_max;
@@ -640,6 +653,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
         const int32_t cls = nx_cls, fixed = nx_fixed;
         const uint64_t cls_off = nx_off;
         const int64_t guard = nx_guard;
+        const int32_t xslot = EXPLAIN ? X->slot[i] : -1;     // the pod's explain record, -1: not explained
         RC.pin = (int32_t)guard;            // pods of pinned classes: the node their REQ_NODE_IS(-3) requirements name
         if (i + 1 < end) {
             const uint32_t q1 = SK_POD(i + 1);
@@ -824,6 +838,10 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                     }
                 }
                 if (leader) { SC.out_node[q] = res; if (SC.out_score) SC.out_score[q] = 0; if (SC.out_gpu) SC.out_gpu[q] = 0; }
+                if constexpr (EXPLAIN) {
+                    const int32_t xq = X->slot[q];
+                    if (leader && xq >= 0) { X->rec[xq].node = res; X->rec[xq].feasible = 0; X->rec[xq].n_top = 0; }
+                }
             }
             cur_class = -1;
             TICK(1);
@@ -1400,6 +1418,34 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                 if (nf & NF_VALID) P.dump_code[(uint32_t)A32(B_NODE_G, idx)] = (int32_t)filter_node(idx, nf, hard_min, true);
             }
         }
+        if constexpr (EXPLAIN) {
+            if (xslot >= 0) {
+                // ---- explained: the histogram of per-node failure reasons for every decision, and F ----
+                uint32_t h[SIMON_N_FAIL_CODES];
+#pragma unroll
+                for (int b = 0; b < SIMON_N_FAIL_CODES; b++) h[b] = 0;
+                #pragma unroll 1
+                for (uint32_t s = 0; s < NPT; s++) {
+                    uint32_t idx = s * TPB + tid;
+                    uint8_t nf = A8(C_NFLAGS, idx);
+                    if (!(nf & NF_VALID) || (nf & NF_FEASIBLE)) continue;
+                    const uint32_t rs = filter_node(idx, nf, hard_min, true);
+#pragma unroll
+                    for (int b = 0; b < SIMON_N_FAIL_CODES; b++) h[b] += (rs >> b) & 1u;
+                }
+                simon_explain_record &xr = X->rec[xslot];
+#pragma unroll
+                for (int b = 0; b < SIMON_N_FAIL_CODES; b++) {
+                    const uint32_t c = __reduce_add_sync(0xffffffffu, h[b]);
+                    if ((tid & 31) == 0 && c) atomicAdd(&xr.rejected[b], c);
+                }
+                if (leader) {
+                    xr.feasible = (uint32_t)C.F;
+                    xr.n_top = (uint32_t)(C.F < (int64_t)X->top_k ? C.F : (int64_t)X->top_k);
+                    if (C.F == 0) xr.node = -1;
+                }
+            }
+        }
         if (C.F == 0) {
             // ---- unschedulable: histogram of per-node failure reasons (FitError, generic_scheduler.go:72-90) ----
             if (n_fail < P.max_fail && SC.fail_counts) {
@@ -1460,8 +1506,17 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                     ip = (int64_t)fr;
                 }
                 total = (int64_t)A32(B_OWN, idx) + (int64_t)A32(B_SNORM, idx) + ip + 2 * pts;
+                if constexpr (EXPLAIN) {
+                    if (xslot >= 0) X->pts_ipa[(uint32_t)A32(B_NODE_G, idx)] = make_int2((int32_t)pts, (int32_t)ip);
+                }
             }
             if (!PROF && i == P.dump_pod && P.dump_total) P.dump_total[(uint32_t)A32(B_NODE_G, idx)] = total;
+            if constexpr (EXPLAIN) {
+                if (xslot >= 0) {
+                    const uint32_t g = (uint32_t)A32(B_NODE_G, idx);
+                    X->total[g] = total;
+                }
+            }
             uint32_t r = s * CT + gtid;
             unsigned long long key = ((unsigned long long)(total + 1) << 24) | (unsigned long long)(0xFFFFFFu - r);
             best = key > best ? key : best;
@@ -1505,6 +1560,64 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
         const bool own_thread = win_g == gtid;
         const uint32_t own_idx = (win_r / CT) * TPB + tid;
         if (tid < T) S.lastdom[tid] = sk_wpay(S, who, tid);
+        // explained decisions: the rounds below reuse the inbox that holds the winner's message, so the commit fold reads the winner's
+        // domains from S.lastdom (the same words; the __syncthreads at the end of the block orders them).  No variable of this block
+        // lives outside it: one did change the code of the variants without it.
+        if constexpr (EXPLAIN) {
+            if (xslot >= 0) {
+                // ---- explained: the best min(top_k, F) feasible nodes, on the state before the commit.  The owner of each writes its
+                //      terms: the split sums of B_OWN (own_core) and B_SNORM (SK_SNORM_TERMS), the P3 terms stored above, Open-Local's
+                //      normalised score ----
+                simon_explain_node *const xn = X->nodes + (uint64_t)xslot * X->top_k;
+                const int64_t range = C.simon_max - C.simon_min;
+                const bool small = range > 0 && range < (1ll << 24) && C.simon_max < (1ll << 24) && C.simon_min >= 0;
+                const bool na32 = C.na_max <= (int64_t)(UINT32_MAX / 100u);
+                auto explain_row = [&](uint32_t idx, simon_explain_node &row, bool first) {
+                    const uint32_t g = (uint32_t)A32(B_NODE_G, idx);
+                    int64_t w[SIMON_EXPLAIN_WORDS];
+#pragma unroll
+                    for (int q = 0; q < SIMON_EXPLAIN_WORDS; q++) w[q] = 0;
+                    if (C.F > 1) {
+                        bool fit;
+                        int32_t own;
+                        own_core(idx, 0, fit, own, w);
+                        const int2 pi = X->pts_ipa[g];
+                        w[2] = pi.y; w[4] = pi.x;
+                        SK_SNORM_TERMS(idx, range, small, na32);
+                        w[3] = na; w[5] = tt; w[6] = sm;
+                        w[7] = A32(B_EXTRA, idx);
+                        w[8] = X->total[g];
+                        if (C.cflags & CLS_LOCAL) w[9] = sk_slice(P.local_raw, P.node_stride)[g];
+                    }
+                    row.node = (int32_t)g;
+#pragma unroll
+                    for (int q = 0; q < SIMON_EXPLAIN_WORDS; q++) row.words[q] = w[q];
+                    if (first) X->rec[xslot].node = (int32_t)g;
+                };
+                if (own_thread) explain_row(own_idx, xn[0], true);
+                const uint32_t n_top = (uint32_t)(C.F < (int64_t)X->top_k ? C.F : (int64_t)X->top_k);
+                unsigned long long prev = best;
+                #pragma unroll 1
+                for (uint32_t k = 1; k < n_top; k++) {
+                    unsigned long long mine = 0;
+                    #pragma unroll 1
+                    for (uint32_t s = 0; s < NPT; s++) {
+                        const uint32_t idx = s * TPB + tid;
+                        if (!(A8(C_NFLAGS, idx) & NF_FEASIBLE)) continue;
+                        const unsigned long long key = ((unsigned long long)(X->total[(uint32_t)A32(B_NODE_G, idx)] + 1) << 24) |
+                                                       (unsigned long long)(0xFFFFFFu - (s * CT + gtid));
+                        if (key < prev && key > mine) mine = key;
+                    }
+                    unsigned long long v[1] = {mine};
+                    const int vop[1] = {OP_MAXU};
+                    sk_allreduce<1>(R, v, vop);
+                    prev = v[0];
+                    const uint32_t r = 0xFFFFFFu - (uint32_t)(prev & 0xFFFFFFu);
+                    if (r % CT == gtid) explain_row((r / CT) * TPB + tid, xn[k], false);
+                }
+                __syncthreads();
+            }
+        }
         if (win_g / TPB == crank) {
             const uint32_t own_tid = win_g % TPB, own_warp = own_tid >> 5, nwarp_cta = (TPB + 31) >> 5;
             const uint32_t help_warp = own_warp + 1 < nwarp_cta ? own_warp + 1 : 0;
@@ -1582,7 +1695,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                 if (trow != cur_row) {
                     cur_row = trow;
                     match = 0;
-                    const int32_t wd = sk_wpay(S, who, trow);
+                    const int32_t wd = EXPLAIN && xslot >= 0 ? S.lastdom[trow] : sk_wpay(S, who, trow);
                     if (wd >= 0) {
                         #pragma unroll (NPT_T > 0 ? NPT_T : 1)
                         for (uint32_t s = 0; s < NPT; s++) {
@@ -1592,7 +1705,7 @@ __device__ __forceinline__ void simon_place_body(const SkParams &P) {
                     }
                 }
                 if ((rec & (1u << 16)) && win_ignored) continue;
-                if (rec & (1u << 17)) { if (sk_wpay(S, who, trow) >= 0) C.aff_total += 1; }
+                if (rec & (1u << 17)) { if ((EXPLAIN && xslot >= 0 ? S.lastdom[trow] : sk_wpay(S, who, trow)) >= 0) C.aff_total += 1; }
                 if (!match) continue;
                 #pragma unroll (NPT_T > 0 ? NPT_T : 1)
                 for (uint32_t s = 0; s < NPT; s++)
@@ -1793,7 +1906,7 @@ extern "C" __global__ void __launch_bounds__(256) simon_drain_unimport(const __g
 }
 
 // Every placement-family kernel, declared once: (symbol, threads per CTA at most, node slots per thread (0: counted at run time),
-// per-phase timers, large cluster, Open-Local, drain batch).  The kernels below and the table simon_api.cu's kernel_variant()
+// per-phase timers, large cluster, Open-Local, drain batch, probe batch, explained decisions).  The kernels below and the table simon_api.cu's kernel_variant()
 // searches come from this list.
 //   - Unrolled node-slot loops for 1-4 slots at 256 and 320 threads and 1-3 at 384; the run-time slot count past those.
 //   - 384 threads = 12 warps = 3 per SM sub-partition, the same register ceiling (168) as 320 threads: one slot per thread less
@@ -1804,56 +1917,65 @@ extern "C" __global__ void __launch_bounds__(256) simon_drain_unimport(const __g
 //     so no evicted pod has any).
 //   - Drain batches that evict pods with Open-Local volumes (simon_drain_run_local): the same again, with the Open-Local code.
 //   - Headroom probes (simon_probe_run): the same two, without and with the Open-Local code.
-#define SIMON_PLACE_VARIANTS(X)                                               \
-    X(simon_place_kernel_256_0,  256, 0, false, false, false, false, false)   \
-    X(simon_place_kernel_256_1,  256, 1, false, false, false, false, false)   \
-    X(simon_place_kernel_256_2,  256, 2, false, false, false, false, false)   \
-    X(simon_place_kernel_256_3,  256, 3, false, false, false, false, false)   \
-    X(simon_place_kernel_256_4,  256, 4, false, false, false, false, false)   \
-    X(simon_place_kernel_320_0,  320, 0, false, false, false, false, false)   \
-    X(simon_place_kernel_320_1,  320, 1, false, false, false, false, false)   \
-    X(simon_place_kernel_320_2,  320, 2, false, false, false, false, false)   \
-    X(simon_place_kernel_320_3,  320, 3, false, false, false, false, false)   \
-    X(simon_place_kernel_320_4,  320, 4, false, false, false, false, false)   \
-    X(simon_place_kernel_384_0,  384, 0, false, false, false, false, false)   \
-    X(simon_place_kernel_384_1,  384, 1, false, false, false, false, false)   \
-    X(simon_place_kernel_384_2,  384, 2, false, false, false, false, false)   \
-    X(simon_place_kernel_384_3,  384, 3, false, false, false, false, false)   \
-    X(simon_place_kernel_big,    320, 0, false, true,  false, false, false)   \
-    X(simon_prof_kernel_256_0,   256, 0, true,  false, false, false, false)   \
-    X(simon_prof_kernel_256_1,   256, 1, true,  false, false, false, false)   \
-    X(simon_prof_kernel_256_2,   256, 2, true,  false, false, false, false)   \
-    X(simon_prof_kernel_256_3,   256, 3, true,  false, false, false, false)   \
-    X(simon_prof_kernel_256_4,   256, 4, true,  false, false, false, false)   \
-    X(simon_prof_kernel_320_0,   320, 0, true,  false, false, false, false)   \
-    X(simon_prof_kernel_320_1,   320, 1, true,  false, false, false, false)   \
-    X(simon_prof_kernel_320_2,   320, 2, true,  false, false, false, false)   \
-    X(simon_prof_kernel_320_3,   320, 3, true,  false, false, false, false)   \
-    X(simon_prof_kernel_320_4,   320, 4, true,  false, false, false, false)   \
-    X(simon_local_kernel_256,    256, 0, false, false, true,  false, false)   \
-    X(simon_local_kernel_320,    320, 0, false, false, true,  false, false)   \
-    X(simon_local_kernel_384,    384, 0, false, false, true,  false, false)   \
-    X(simon_local_kernel_big,    320, 0, false, true,  true,  false, false)   \
-    X(simon_drain_kernel_256,    256, 0, false, false, false, true, false)    \
-    X(simon_drain_kernel_320,    320, 0, false, false, false, true, false)    \
-    X(simon_drain_kernel_384,    384, 0, false, false, false, true, false)    \
-    X(simon_drain_kernel_big,    320, 0, false, true,  false, true, false)    \
-    X(simon_drain_local_kernel_256, 256, 0, false, false, true, true, false)  \
-    X(simon_drain_local_kernel_320, 320, 0, false, false, true, true, false)  \
-    X(simon_drain_local_kernel_384, 384, 0, false, false, true, true, false)  \
-    X(simon_drain_local_kernel_big, 320, 0, false, true,  true, true, false)  \
-    X(simon_probe_kernel_256,    256, 0, false, false, false, false, true)    \
-    X(simon_probe_kernel_320,    320, 0, false, false, false, false, true)    \
-    X(simon_probe_kernel_384,    384, 0, false, false, false, false, true)    \
-    X(simon_probe_kernel_big,    320, 0, false, true,  false, false, true)    \
-    X(simon_probe_local_kernel_256, 256, 0, false, false, true, false, true)  \
-    X(simon_probe_local_kernel_320, 320, 0, false, false, true, false, true)  \
-    X(simon_probe_local_kernel_384, 384, 0, false, false, true, false, true)  \
-    X(simon_probe_local_kernel_big, 320, 0, false, true,  true, false, true)
+//   - Explained decisions (simon_explain_set): single runs whose range holds an explained pod, the same two.
+#define SIMON_PLACE_VARIANTS(X)                                                       \
+    X(simon_place_kernel_256_0,  256, 0, false, false, false, false, false, false)    \
+    X(simon_place_kernel_256_1,  256, 1, false, false, false, false, false, false)    \
+    X(simon_place_kernel_256_2,  256, 2, false, false, false, false, false, false)    \
+    X(simon_place_kernel_256_3,  256, 3, false, false, false, false, false, false)    \
+    X(simon_place_kernel_256_4,  256, 4, false, false, false, false, false, false)    \
+    X(simon_place_kernel_320_0,  320, 0, false, false, false, false, false, false)    \
+    X(simon_place_kernel_320_1,  320, 1, false, false, false, false, false, false)    \
+    X(simon_place_kernel_320_2,  320, 2, false, false, false, false, false, false)    \
+    X(simon_place_kernel_320_3,  320, 3, false, false, false, false, false, false)    \
+    X(simon_place_kernel_320_4,  320, 4, false, false, false, false, false, false)    \
+    X(simon_place_kernel_384_0,  384, 0, false, false, false, false, false, false)    \
+    X(simon_place_kernel_384_1,  384, 1, false, false, false, false, false, false)    \
+    X(simon_place_kernel_384_2,  384, 2, false, false, false, false, false, false)    \
+    X(simon_place_kernel_384_3,  384, 3, false, false, false, false, false, false)    \
+    X(simon_place_kernel_big,    320, 0, false, true,  false, false, false, false)    \
+    X(simon_prof_kernel_256_0,   256, 0, true,  false, false, false, false, false)    \
+    X(simon_prof_kernel_256_1,   256, 1, true,  false, false, false, false, false)    \
+    X(simon_prof_kernel_256_2,   256, 2, true,  false, false, false, false, false)    \
+    X(simon_prof_kernel_256_3,   256, 3, true,  false, false, false, false, false)    \
+    X(simon_prof_kernel_256_4,   256, 4, true,  false, false, false, false, false)    \
+    X(simon_prof_kernel_320_0,   320, 0, true,  false, false, false, false, false)    \
+    X(simon_prof_kernel_320_1,   320, 1, true,  false, false, false, false, false)    \
+    X(simon_prof_kernel_320_2,   320, 2, true,  false, false, false, false, false)    \
+    X(simon_prof_kernel_320_3,   320, 3, true,  false, false, false, false, false)    \
+    X(simon_prof_kernel_320_4,   320, 4, true,  false, false, false, false, false)    \
+    X(simon_local_kernel_256,    256, 0, false, false, true,  false, false, false)    \
+    X(simon_local_kernel_320,    320, 0, false, false, true,  false, false, false)    \
+    X(simon_local_kernel_384,    384, 0, false, false, true,  false, false, false)    \
+    X(simon_local_kernel_big,    320, 0, false, true,  true,  false, false, false)    \
+    X(simon_drain_kernel_256,    256, 0, false, false, false, true, false, false)     \
+    X(simon_drain_kernel_320,    320, 0, false, false, false, true, false, false)     \
+    X(simon_drain_kernel_384,    384, 0, false, false, false, true, false, false)     \
+    X(simon_drain_kernel_big,    320, 0, false, true,  false, true, false, false)     \
+    X(simon_drain_local_kernel_256, 256, 0, false, false, true, true, false, false)   \
+    X(simon_drain_local_kernel_320, 320, 0, false, false, true, true, false, false)   \
+    X(simon_drain_local_kernel_384, 384, 0, false, false, true, true, false, false)   \
+    X(simon_drain_local_kernel_big, 320, 0, false, true,  true, true, false, false)   \
+    X(simon_probe_kernel_256,    256, 0, false, false, false, false, true, false)     \
+    X(simon_probe_kernel_320,    320, 0, false, false, false, false, true, false)     \
+    X(simon_probe_kernel_384,    384, 0, false, false, false, false, true, false)     \
+    X(simon_probe_kernel_big,    320, 0, false, true,  false, false, true, false)     \
+    X(simon_probe_local_kernel_256, 256, 0, false, false, true, false, true, false)   \
+    X(simon_probe_local_kernel_320, 320, 0, false, false, true, false, true, false)   \
+    X(simon_probe_local_kernel_384, 384, 0, false, false, true, false, true, false)   \
+    X(simon_probe_local_kernel_big, 320, 0, false, true,  true, false, true, false)   \
+    X(simon_explain_kernel_256,  256, 0, false, false, false, false, false, true)     \
+    X(simon_explain_kernel_320,  320, 0, false, false, false, false, false, true)     \
+    X(simon_explain_kernel_384,  384, 0, false, false, false, false, false, true)     \
+    X(simon_explain_kernel_big,  320, 0, false, true,  false, false, false, true)     \
+    X(simon_explain_local_kernel_256, 256, 0, false, false, true, false, false, true) \
+    X(simon_explain_local_kernel_320, 320, 0, false, false, true, false, false, true) \
+    X(simon_explain_local_kernel_384, 384, 0, false, false, true, false, false, true) \
+    X(simon_explain_local_kernel_big, 320, 0, false, true,  true, false, false, true)
 
-#define SK_DEFINE_VARIANT(name, threads, slots, prof, big, local, drain, probe)                            \
+#define SK_DEFINE_VARIANT(name, threads, slots, prof, big, local, drain, probe, explain)                   \
     extern "C" __global__ void __launch_bounds__(threads, 1) name(const __grid_constant__ SkParams P) { \
-        simon_place_body<threads, slots, prof, big, local, drain, probe>(P);                             \
+        simon_place_body<threads, slots, prof, big, local, drain, probe, explain>(P);                    \
     }
 SIMON_PLACE_VARIANTS(SK_DEFINE_VARIANT)
 #undef SK_DEFINE_VARIANT

@@ -135,8 +135,21 @@ struct SkParams {
     // pod-list order); the per-pod outputs of SkScenario are indexed by the position in drain_pods, not by the pod.
     // probe batches (simon_probe_kernel_*): scenario s places replicas of pod probe_pod[s] at positions probe_off[s] .. probe_off[s + 1)
     // of the per-pod outputs, and stops at the first one that does not fit
-    union { const uint32_t *drain_pods; const uint32_t *probe_pod; };
+    // explained decisions (simon_explain_kernel_*, single-scenario runs, where drain / probe lists are unused): the set's tables
+    union { const uint32_t *drain_pods; const uint32_t *probe_pod; const struct SkExplain *explain; };
     union { const uint32_t *drain_off; const uint32_t *probe_off; };
+};
+
+// The explained-pod set of simon_explain_set on the device: slot[pod] = the pod's record (-1: not explained), its records and
+// [record][top_k] node rows, and per node the last explained decision's total and its (PodTopologySpread, InterPodAffinity) scores,
+// written and read by the node's owning thread only
+struct SkExplain {
+    const int32_t *slot;
+    simon_explain_record *rec;
+    simon_explain_node *nodes;
+    long long *total;          // [N]
+    int2 *pts_ipa;             // [N]
+    uint32_t top_k, pad;
 };
 
 // the index of this thread-block cluster in the (1-D) grid: the scenario of the launch (blockIdx.x / cluster size)

@@ -59,6 +59,10 @@ MOVES_SCOPE_GPU_SHARE, MOVES_SCOPE_HARD_SPREAD = 1, 2
 PLAN_STOP_NO_MOVE, PLAN_STOP_MAX_MOVES = 1, 2
 # simon_probe_run stop reasons
 PROBE_STOP_UNSCHEDULABLE, PROBE_STOP_MAX_REPLICAS = 1, 2
+# explained decisions (simon_explain_set): largest top_k, words per listed node, the record node of a pod no call has covered
+EXPLAIN_MAX_TOP = 16
+EXPLAIN_WORDS = 10
+EXPLAIN_NOT_RUN = -4
 
 
 class SimonSnapshot(C.Structure):
@@ -161,6 +165,20 @@ def marshal_devices(st):
     return s, keep
 
 
+class SimonExplainRecord(C.Structure):
+    _fields_ = [("node", C.c_int32), ("feasible", C.c_uint32), ("n_top", C.c_uint32), ("reserved", C.c_uint32),
+                ("rejected", C.c_uint32 * N_FAIL_CODES)]
+
+
+class SimonExplainNode(C.Structure):
+    _fields_ = [("node", C.c_int32), ("reserved", C.c_uint32), ("words", C.c_int64 * EXPLAIN_WORDS)]
+
+
+# the same two as the structured arrays Engine.explanations returns
+EXPLAIN_RECORD_DTYPE = np.dtype(SimonExplainRecord)
+EXPLAIN_NODE_DTYPE = np.dtype(SimonExplainNode)
+
+
 # simon_plan_step, as the structured array Engine.moves_plan passes
 PLAN_STEP_DTYPE = np.dtype([("move", np.uint32), ("pod", np.uint32), ("from", np.int32), ("to", np.int32), ("gain", np.int32),
                             ("gpu_slots", np.uint32)])
@@ -248,6 +266,8 @@ SIGNATURES = {
     "simon_state_download_ext": (_I, [_P, _P, _P]),
     "simon_debug_set_dump_pod": (_I, [_P, _U32]),
     "simon_debug_dump_read": (_I, [_P, _P, _P]),
+    "simon_explain_set": (_I, [_P, _P, _U32, _U32]),
+    "simon_explain_download": (_I, [_P, _U32, _U32, _P, _P]),
     "simon_moves_upload": (_I, [_P, _P, _U32, _U32]),
     "simon_moves_run": (_I, [_P, _U32, _P, _P, _P, _P, _P]),
     "simon_moves_replay": (_I, [_P, _U32, _PF]),

@@ -91,8 +91,29 @@ class Engine:
     def reset(self):
         self._check(lib().simon_state_reset(self.h))
 
-    def schedule(self, first: int = 0, count: Optional[int] = None, max_fail: Optional[int] = None, download: bool = True):
-        """Place pods [first, first+count). Returns (out_node, out_score, fail_counts, fail_pod)."""
+    def explain_set(self, pods, top_k: int = 3):
+        """simon_explain_set: later schedule / schedule_resume calls also explain these pods (ascending pod indices; [] clears the
+        set), listing the best top_k feasible nodes of each; explanations() reads the records."""
+        a = np.ascontiguousarray(pods, dtype=np.uint32)
+        self._check(lib().simon_explain_set(self.h, a.ctypes.data if len(a) else None, len(a), int(top_k)))
+        self._explain = (len(a), int(top_k))
+
+    def explanations(self):
+        """The explained pods' records of the set, in its order: (records [n] of abi.EXPLAIN_RECORD_DTYPE, nodes [n][top_k] of
+        abi.EXPLAIN_NODE_DTYPE); only the first records["n_top"] nodes of a record are filled."""
+        n, k = getattr(self, "_explain", (0, 0))
+        rec = np.zeros(max(n, 1), abi.EXPLAIN_RECORD_DTYPE)
+        nodes = np.zeros((max(n, 1), max(k, 1)), abi.EXPLAIN_NODE_DTYPE)
+        if n:
+            self._check(lib().simon_explain_download(self.h, 0, n, rec.ctypes.data, nodes.ctypes.data))
+        return rec[:n], nodes[:n, :k]
+
+    def schedule(self, first: int = 0, count: Optional[int] = None, max_fail: Optional[int] = None, download: bool = True,
+                 explain=None, top_k: int = 3):
+        """Place pods [first, first+count). Returns (out_node, out_score, fail_counts, fail_pod).  explain: set the explained pods
+        first (explain_set(explain, top_k)); None keeps the set as it is."""
+        if explain is not None:
+            self.explain_set(explain, top_k)
         P = self.c.pods_dims["n_pods"]
         count = P - first if count is None else count
         max_fail = count if max_fail is None else max_fail
@@ -110,10 +131,12 @@ class Engine:
         nf = min(n_fail.value, max_fail)
         return out_node, out_score, fail_counts[:nf], fail_pod[:nf]
 
-    def schedule_resume(self, prefix_node, max_fail: Optional[int] = None):
+    def schedule_resume(self, prefix_node, max_fail: Optional[int] = None, explain=None, top_k: int = 3):
         """simon_schedule_resume: rebuild the state pods [0, len(prefix_node)) leave at the nodes an earlier call gave them (its
         out_node), then place the rest.  Returns (out_node, out_score, fail_counts, fail_pod) over ALL pods; the scores of the prefix
-        pods are 0 (not recomputed) and the failures are those of the placed rest only."""
+        pods are 0 (not recomputed) and the failures are those of the placed rest only.  explain: as schedule's."""
+        if explain is not None:
+            self.explain_set(explain, top_k)
         P = self.c.pods_dims["n_pods"]
         prefix = np.ascontiguousarray(prefix_node, dtype=np.int32)
         n_prefix = len(prefix)

@@ -199,6 +199,18 @@ def format_fit_error(compiled: Compiled, rec: PodRec, counts: np.ndarray, active
         static = _static_reasons(compiled, rec, idxs)
         if static_memo is not None:
             static_memo[mkey] = static
+    reasons = fit_reasons(compiled, counts, static, gpu_nodes, local_reasons)
+    total = len(idxs)
+    parts = sorted(f"{v} {k}" for k, v in reasons.items())
+    msg = f"0/{total} nodes are available: {', '.join(parts)}."
+    ns = rec.tmpl.namespace
+    return f"failed to schedule pod ({ns}/{rec.name}): Unschedulable: {msg}"
+
+
+def fit_reasons(compiled: Compiled, counts: np.ndarray, static: dict, gpu_nodes: Optional[List[str]] = None,
+                local_reasons: Optional[List[Optional[str]]] = None) -> dict:
+    """The FitError reason texts -> node counts of a failure histogram `counts` [SIMON_N_FAIL_CODES], whose node-static bin is
+    `static` (_static_reasons)."""
     reasons = dict(static)
     for code, strs in _DYNAMIC_REASONS.items():
         c = int(counts[code])
@@ -224,11 +236,7 @@ def format_fit_error(compiled: Compiled, rec: PodRec, counts: np.ndarray, active
                     reasons[r] = reasons.get(r, 0) + 1
         else:       # per-node texts not collected: counts only
             reasons["<%d nodes rejected by Open-Local>" % n_local] = n_local
-    total = len(idxs)
-    parts = sorted(f"{v} {k}" for k, v in reasons.items())
-    msg = f"0/{total} nodes are available: {', '.join(parts)}."
-    ns = rec.tmpl.namespace
-    return f"failed to schedule pod ({ns}/{rec.name}): Unschedulable: {msg}"
+    return reasons
 
 
 def build_result(compiled: Compiled, p: Plan, out_node: np.ndarray, fail_counts, fail_pod, gpu_fail_nodes=None,
@@ -656,6 +664,62 @@ class Simulator:
                 for (i, _e), res in zip(tmpls, headroom.run(eng2, c2, placed2, extra)):
                     out[i] = res
                 self.last_headroom.append(eng2.last_probe)
+        return out
+
+    def Explain(self, entries: list, top: int = 3):
+        """Per entry an explain.Explanation: why the pod goes where it goes on the session's state - its node, the feasible count, the
+        best `top` feasible nodes with each score plugin's weighted points, and the FitError reasons of the other nodes.  An entry is
+        a pod of the session ("namespace/name" as its results name it), explained on the state just before it: the live context re-runs
+        schedule_resume(placements[:i0]) from the first such pod i0 with the pods explained, and the re-run must reproduce the
+        session's placements and GPU slots from i0 on.  Or a Pod object, explained on the live state as if it came alone: made valid as
+        MakeValidPodByPod does and appended after the session's pods (one compile per call; spec.nodeName is refused), one resume per
+        template with the earlier templates' entries -1.  The session's placements, slots and scores are not changed."""
+        from . import explain
+        from .engine import Engine
+        eng, compiled = self._live()
+        out: List = [None] * len(entries)
+        idx = explain.pod_index(compiled)
+        live = [(i, e) for i, e in enumerate(entries) if isinstance(e, str)]
+        tmpls = [(i, e) for i, e in enumerate(entries) if not isinstance(e, str)]
+        for _i, e in live:
+            if e not in idx:
+                raise ValueError(f"Explain: {e!r} is not a pod of the session")
+        recs = []
+        for _i, pod in tmpls:
+            if ((pod.get("spec") or {}).get("nodeName") or ""):
+                raise ValueError(f"Explain: template pod {O.name_of(pod)!r} sets spec.nodeName: it never reaches the scheduler")
+            recs.append(make_valid_pod_by_pod(pod))
+        plugins = self._extra_plugins or None
+        if live:
+            pods = sorted({idx[e] for _i, e in live})
+            i0 = pods[0]
+            eng.explain_set(pods, top)
+            try:
+                got = eng.schedule_resume(self.placements[:i0], max_fail=0)[0]
+                slots = eng.gpu_slot_words()
+                if not (np.array_equal(got, self.placements) and np.array_equal(slots[i0:], self.gpu_slots[i0:])):
+                    raise RuntimeError("Explain: the re-run from the first explained pod did not reproduce the session's placements")
+                rec, nodes = eng.explanations()
+            finally:
+                eng.explain_set([])
+            at = {q: j for j, q in enumerate(pods)}
+            for i, e in live:
+                j = at[idx[e]]
+                out[i] = explain.build(compiled, idx[e], rec[j], nodes[j], plugins)
+        if tmpls:
+            p = self._plan()
+            storage_classes = None
+            if self.options.openLocal:
+                storage_classes = list(self.cluster.StorageClasss) + [sc for a in self.apps for sc in a.Resource.StorageClasss]
+            c2 = compile_cluster(p.nodes, p.pods + recs, p.ctx, extra_plugins=plugins, open_local=self.options.openLocal,
+                                 storage_classes=storage_classes, local_devices=self.options.openLocalDevices)
+            n0 = len(p.pods)
+            with Engine(c2, device=self.options.device) as eng2:
+                for j, (i, _e) in enumerate(tmpls):
+                    eng2.explain_set([n0 + j], top)
+                    eng2.schedule_resume(np.concatenate([self.placements, np.full(j, -1, np.int32)]), max_fail=0)
+                    rec, nodes = eng2.explanations()
+                    out[i] = explain.build(c2, n0 + j, rec[0], nodes[0], plugins)
         return out
 
     def _check_local_volumes(self, local_volumes: bool, what: str):
