@@ -606,7 +606,7 @@ typedef struct simon_scenario_local_result {
 int simon_scenarios_run_local(simon_ctx *ctx, const simon_scenario *scen, uint32_t n, simon_scenario_result *out,
                               simon_scenario_local_result *out_local, int32_t *out_node);
 /* Scenario `scenario` of the last simon_scenarios_run_local or simon_drain_run_local batch, or probe `scenario` of the last simon_probe_run
- * batch on a context with storage: its final VG requested [V][N] and, if
+ * batch or scenario `scenario` of the last simon_grow_run batch on a context with storage: its final VG requested [V][N] and, if
  * dev_alloc is not NULL, its allocated device slots [N] (SIMON_ERR_STATE without a simon_devices_upload); node-indexed like the
  * snapshot.  Inactive nodes keep the values the scenario started from: the uploaded ones in a scenario batch, the live ones (the
  * state `placed` leaves) on a drain's removed nodes.  SIMON_ERR_STATE if no such batch ran since the last snapshot, pod, storage or
@@ -735,6 +735,48 @@ int simon_probe_run(simon_ctx *ctx, const int32_t *placed, const simon_probe *pr
 int simon_probe_download(simon_ctx *ctx, uint32_t probe, int32_t *node, uint32_t *gpu_slots, int64_t *score, uint32_t *fail_counts);
 /* Device time of the last simon_probe_run: setup (rebuild, copies into the slots) and placement, ms. */
 int simon_probe_times(simon_ctx *ctx, float *setup_ms, float *place_ms);
+
+/* ---- nodes to add to the live cluster (the reference's second use case, README.md:15: "determine whether the applications can be
+ * deployed successfully at one time ... in the running kubernetes cluster. If the cluster size does not meet the resource requirements
+ * of applications, plan out the number of nodes to add"; the reference runs `simon apply` on a kubeConfig cluster) ---------------------
+ * A grow batch runs on a compiled superset cluster: the nodes are the running cluster's nodes plus a pool of candidate new nodes, and
+ * the pod list is a prefix [0, n_prefix) holding the running cluster's pods followed by a pending tail [n_prefix, n_pods): the DaemonSet
+ * pods of the pool nodes (each guarded by its node) and the new apps' pods.  The live state is placed[n_prefix], the out_node entries of
+ * the prefix as a placement reported them, checked as simon_schedule_resume checks a prefix.  Each scenario is a simon_scenario that
+ * lists its active nodes (the running nodes plus its pool nodes) in its own nodeTree.list() order.  For each scenario, from the live state
+ * (requests, non-zero requests, pod counts, the class counters, GPU-share device memory and, with Open-Local, VGs and devices), the tail
+ * pods are placed in pod order through the full filter -> score -> select -> Reserve / Bind path on the active nodes only.  A tail pod
+ * whose guard node is inactive does not exist in that scenario (-3), as in scenario batches; a tail pod bound by spec.nodeName is
+ * accounted on its node as there.  Prefix pods stay where they are, and prefix pods with -1 stay pending and are not retried.
+ * Equivalently: the scenario places what compiling its active nodes with the pod list filtered to the pods that exist there (order
+ * kept) and resuming with `placed` (remapped to the new node indices) as the prefix (simon_schedule_resume) places: the same tail nodes,
+ * GPU slots, scores, failure histograms, final VG requested and device masks.
+ *
+ * simon_grow_run runs n scenarios as one batch: the live state is rebuilt from placed[n_prefix] into the single-scenario state (as
+ * simon_drain_run rebuilds it: afterwards the single-scenario downloads describe the prefix) and copied into every scenario's slot of
+ * the batch pool; then each scenario places the tail with the scenario-batch placement kernels.  out[i] holds scenario i's counts over
+ * its existing tail pods that reach the scheduler (n_scheduled, n_unscheduled) and the sums over its active nodes after the placement
+ * (satisfyResourceSetting's inputs).  With Open-Local storage uploaded the placement kernels with Open-Local code run and each scenario
+ * starts from the live VG requested values and device masks; out_local (NULL, or n entries; needs a simon_storage_upload, else
+ * SIMON_ERR_STATE) gets each scenario's VG sums as simon_scenarios_run_local's, and after a batch on a context with storage
+ * simon_scenarios_storage_download gives each scenario's final VG requested and device masks.  Grow, drain and probe batches share the
+ * batch pool: after a grow batch simon_drain_download and simon_probe_download refuse, and after a drain or probe batch
+ * simon_grow_download does.  simon_last_kernel_ms is the device time of setup + placement, simon_grow_times splits it.
+ * Every scenario must list every node that holds a placed prefix pod: the live state counts those pods, and nothing takes them out.
+ * SIMON_ERR_INVALID with a message, before any device work: n_prefix above n_pods, `placed` fails the prefix checks, a scenario has no
+ * node, lists a node twice or a node out of range, or leaves out a node that holds a placed prefix pod.  SIMON_ERR_LIMIT: the
+ * per-tail-pod outputs do not fit the device. */
+int simon_grow_run(simon_ctx *ctx, const int32_t *placed, uint32_t n_prefix, const simon_scenario *scen, uint32_t n,
+                   simon_scenario_result *out, simon_scenario_local_result *out_local /* may be NULL */);
+/* Scenario `scenario` of the last simon_grow_run batch, any pointer may be NULL: per tail pod [n_pods - n_prefix] the node it landed on
+ * (-1 unschedulable, -2 bound to an inactive node, -3 it does not exist in the scenario), its GPU slot word (simon_gpu_slots_download's
+ * format) and its winning total score (0 without SIMON_OPT_RECORD_SCORES or with a single feasible node); and the failure histogram
+ * [n_unscheduled][SIMON_N_FAIL_CODES] and pod index of each unscheduled tail pod in order of failure.  SIMON_ERR_STATE if no grow batch
+ * ran since the last snapshot or pod upload, or a drain or probe batch ran after it. */
+int simon_grow_download(simon_ctx *ctx, uint32_t scenario, int32_t *node, uint32_t *gpu_slots, int64_t *score, uint32_t *fail_counts,
+                        uint32_t *fail_pod);
+/* Device time of the last simon_grow_run: setup (rebuild, copies into the slots) and placement, ms. */
+int simon_grow_times(simon_ctx *ctx, float *setup_ms, float *place_ms);
 
 /* ---- PodDisruptionBudgets in drains, move scoring and migration plans (this library's reading; the reference carries PDBs in
  * ResourceTypes.PodDisruptionBudgets, pkg/simulator/core.go:48, and creates them, simulator.go:261-262, 374-376) ----------------------

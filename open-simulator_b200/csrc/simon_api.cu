@@ -246,6 +246,7 @@ enum Data : uint32_t {
     STATIC_FILL = 1u << 9,      // the static verdicts of every (signature, node) pair are in the pod set's scache
     STORAGE_BATCH = 1u << 10, DRAIN_BATCH = 1u << 11, PLAN = 1u << 12, PROBE_BATCH = 1u << 13,
     EXPLAIN_SET = 1u << 14,     // simon_explain_set's pods, records and device tables
+    GROW_BATCH = 1u << 15,
 };
 
 struct Validity {
@@ -256,7 +257,7 @@ struct Validity {
     void drop(uint32_t d) {
         static constexpr uint32_t derived[][2] = {
             {SNAPSHOT, POD_SET},
-            {POD_SET, STORAGE | PDB_TABLE | LIVE | PLAN | DRAIN_BATCH | PROBE_BATCH | MOVE_LIST | SCOPE_PREP | STATIC_FILL | EXPLAIN_SET},
+            {POD_SET, STORAGE | PDB_TABLE | LIVE | PLAN | DRAIN_BATCH | PROBE_BATCH | GROW_BATCH | MOVE_LIST | SCOPE_PREP | STATIC_FILL | EXPLAIN_SET},
             {STORAGE, DEVICES | STORAGE_BATCH | LIVE | SCOPE_PREP},     // SCOPE_PREP: the move-class records exclude local classes
             {DEVICES, STORAGE_BATCH | LIVE},
             {MOVE_LIST, MOVE_RUN},
@@ -380,6 +381,17 @@ struct simon_ctx {
         DevBuf<int64_t> d_score;
         float setup_ms = 0.f, place_ms = 0.f;
     } probe;
+    // the last grow batch (simon_grow_run): n scenarios placing the tail [n_prefix, n_prefix + tail) of the pod list, each one's
+    // unscheduled tail pods; on the device the tail's nodes, GPU slots and scores (scenario i's pod q at i * tail + q: n * tail +
+    // n_prefix entries) and tail failure records per scenario
+    struct {
+        uint32_t n = 0, n_prefix = 0, tail = 0;
+        std::vector<uint32_t> nfail;
+        DevBuf<uint32_t> d_gpu, d_fail_counts, d_fail_pod;
+        DevBuf<int32_t> d_node;
+        DevBuf<int64_t> d_score;
+        float setup_ms = 0.f, place_ms = 0.f;
+    } grow;
     // the last migration plan (simon_moves_plan): its end state in plan-owned copies of the single-scenario node state, placement and
     // GPU slot words, the steps and control words
     struct {
@@ -1456,7 +1468,7 @@ int simon_scenarios_storage_download(simon_ctx *ctx, uint32_t scenario, int64_t 
     if (!ctx) return SIMON_ERR_INVALID;
     const ScenPool &B = ctx->batch;
     if (!ctx->valid.has(STORAGE_BATCH))
-        return fail(ctx, SIMON_ERR_STATE, "no simon_scenarios_run_local, simon_drain_run_local or simon_probe_run batch with storage since the last upload");
+        return fail(ctx, SIMON_ERR_STATE, "no simon_scenarios_run_local, simon_drain_run_local, simon_probe_run or simon_grow_run batch with storage since the last upload");
     if (scenario >= ctx->storage_batch.n) return fail(ctx, SIMON_ERR_INVALID, "scenario %u of a batch of %u", scenario, ctx->storage_batch.n);
     if (dev_alloc && !ctx->valid.has(DEVICES)) return fail(ctx, SIMON_ERR_STATE, "no devices uploaded");
     CU(cudaSetDevice(ctx->device));
@@ -1502,14 +1514,14 @@ extern "C" int simon_drain_budget(simon_ctx *ctx, uint64_t *scenario_bytes, uint
     return SIMON_OK;
 }
 
-// The setup drain and probe batches share, enqueued once their refusals and allocations are done: the live state `placed` leaves,
-// rebuilt into the single-scenario pool (the resume's rebuild, its failure records cleared as the resume clears them) and copied into
+// The setup drain, probe and grow batches share, enqueued once their refusals and allocations are done: the live state that pods
+// [0, n_prefix) leave at `placed`, rebuilt into the single-scenario pool (the resume's rebuild, its failure records cleared as the resume clears them) and copied into
 // each of the n slots of the batch pool, one broadcast per column.  Of the batch pool only what the copies do not overwrite is cleared:
 // the per-class summaries and own-score caches, the counters and clocks, and the batch's failure records (fail_words words at
 // fail_counts).  local: the live Open-Local state (the rebuild's Bind replay) is copied too.  ctx->ev0 is recorded before it; Pb gets the
 // batch pool's launch parameters.
-static int live_batch_setup(simon_ctx *ctx, const int32_t *placed, uint32_t n, bool local, uint32_t *fail_counts, size_t fail_words,
-                            SkParams &Pb) {
+static int live_batch_setup(simon_ctx *ctx, const int32_t *placed, uint32_t n_prefix, uint32_t n, bool local, uint32_t *fail_counts,
+                            size_t fail_words, SkParams &Pb) {
     ScenPool &S = ctx->single, &B = ctx->batch;
     cudaStream_t st = ctx->stream;
     CU(cudaEventRecord(ctx->ev0, st));
@@ -1518,7 +1530,7 @@ static int live_batch_setup(simon_ctx *ctx, const int32_t *placed, uint32_t n, b
     int rc = clear_pool(ctx, S);
     if (rc) return rc;
     CU(single_begin(ctx, Ps));
-    rc = rebuild_prefix(ctx, Ps, placed, ctx->pods.n_pods);
+    rc = rebuild_prefix(ctx, Ps, placed, n_prefix);
     if (rc) return rc;
     CU(cudaMemsetAsync(B.csum.p, 0, 8 * n * B.ncl * SK_CSUM_W, st));
     CU(cudaMemsetAsync(B.ocache.p, 0, 8 * n * B.nodes * B.ncl, st));
@@ -1534,7 +1546,7 @@ static int live_batch_setup(simon_ctx *ctx, const int32_t *placed, uint32_t n, b
     return SIMON_OK;
 }
 
-// After a drain or probe batch's launch: each scenario's sums over its active nodes (simon_scen_reduce) into res and, local, its VG sums
+// After a drain, probe or grow batch's launch: each scenario's sums over its active nodes (simon_scen_reduce) into res and, local, its VG sums
 // into out_local, copied back on the stream (the caller synchronises)
 static int live_batch_reduce(simon_ctx *ctx, uint32_t n, bool local, std::vector<simon_scenario_result> &res,
                              simon_scenario_local_result *out_local) {
@@ -1572,8 +1584,8 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
     if (rc) return rc;
     CU(cudaSetDevice(ctx->device));
     ctx->last_launch = simon_launch_info{};
-    // the batch pool is no longer a probe batch's, nor are its Open-Local slices a storage batch's
-    ctx->valid.drop(DRAIN_BATCH | PROBE_BATCH | STORAGE_BATCH);
+    // the batch pool is no longer a probe or grow batch's, nor are its Open-Local slices a storage batch's
+    ctx->valid.drop(DRAIN_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
     ScenPool &S = ctx->single, &B = ctx->batch;
     if (n == 0) return SIMON_OK;
     cudaStream_t st = ctx->stream;
@@ -1639,7 +1651,7 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
     // ---- setup: the live state in every slot (live_batch_setup), minus what each scenario's removed nodes' pods contributed to the
     // counters.  local: the removed nodes' VGs and devices keep their live values, since those nodes are inactive ----
     SkParams Pb;
-    rc = live_batch_setup(ctx, placed, n, local, ctx->drain.d_fail_counts.p, (size_t)n * ctx->drain.max * SIMON_N_FAIL_CODES, Pb);
+    rc = live_batch_setup(ctx, placed, P, n, local, ctx->drain.d_fail_counts.p, (size_t)n * ctx->drain.max * SIMON_N_FAIL_CODES, Pb);
     if (rc) return rc;
     if (!pairs.empty()) {
         const uint32_t grid = (uint32_t)std::min<size_t>((pairs.size() + 255) / 256, (size_t)ctx->sms * 4);
@@ -1798,8 +1810,8 @@ extern "C" int simon_probe_run(simon_ctx *ctx, const int32_t *placed, const simo
                         (unsigned long long)total, (unsigned long long)need, (unsigned long long)fr);
     }
     ctx->last_launch = simon_launch_info{};
-    // the batch pool is no longer a drain batch's, nor are its Open-Local slices another storage batch's
-    ctx->valid.drop(DRAIN_BATCH | PROBE_BATCH | STORAGE_BATCH);
+    // the batch pool is no longer a drain or grow batch's, nor are its Open-Local slices another storage batch's
+    ctx->valid.drop(DRAIN_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
     if (n == 0) return SIMON_OK;
     cudaStream_t st = ctx->stream;
     ScenPool &B = ctx->batch;
@@ -1835,7 +1847,7 @@ extern "C" int simon_probe_run(simon_ctx *ctx, const int32_t *placed, const simo
     CU(B.scen.upload(h.data(), n, st));
     // ---- setup: the live state in every slot, with its Open-Local state when storage is uploaded (live_batch_setup) ----
     SkParams Pb;
-    rc = live_batch_setup(ctx, placed, n, storage, ctx->probe.d_fail_counts.p, (size_t)n * SIMON_N_FAIL_CODES, Pb);
+    rc = live_batch_setup(ctx, placed, P, n, storage, ctx->probe.d_fail_counts.p, (size_t)n * SIMON_N_FAIL_CODES, Pb);
     if (rc) return rc;
     CU(cudaEventRecord(ctx->evm, st));
     // ---- placement of every probe's replicas, one failure record each ----
@@ -1895,6 +1907,144 @@ extern "C" int simon_probe_times(simon_ctx *ctx, float *setup_ms, float *place_m
     if (!ctx) return SIMON_ERR_INVALID;
     if (setup_ms) *setup_ms = ctx->probe.setup_ms;
     if (place_ms) *place_ms = ctx->probe.place_ms;
+    return SIMON_OK;
+}
+
+// ---- grow batches ---------------------------------------------------------------------------------------------------------------
+// The batch placement variants (family PLACE) run from the broadcast live state with P.first = n_prefix: the body already starts
+// there for resumed single runs, and every per-scenario column it reads is in the slot the setup filled.  The per-pod outputs are
+// indexed by pod, so scenario i's are based at i * tail in arrays of n * tail + n_prefix entries: pod q of the tail lands at
+// i * tail + q, inside the array and after scenario i - 1's last pod.
+extern "C" int simon_grow_run(simon_ctx *ctx, const int32_t *placed, uint32_t n_prefix, const simon_scenario *scen, uint32_t n,
+                              simon_scenario_result *out, simon_scenario_local_result *out_local) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_grow_run before uploads");
+    const uint32_t P = ctx->pods.n_pods;
+    // ---- refusals before any device work: the prefix, then the node lists ----
+    if (n_prefix > P) return fail(ctx, SIMON_ERR_INVALID, "simon_grow_run: n_prefix %u above the %u pods", n_prefix, P);
+    if ((n_prefix && !placed) || (n && (!scen || !out))) return fail(ctx, SIMON_ERR_INVALID, "simon_grow_run: NULL argument");
+    int rc = check_prefix(ctx, placed, n_prefix);
+    if (rc) return rc;
+    for (uint32_t i = 0; i < n; i++)
+        if (scen[i].n_nodes == 0) return fail(ctx, SIMON_ERR_INVALID, "grow scenario %u has no node", i);
+    uint32_t max_active = 0;
+    rc = scenario_lists(ctx, scen, n, "grow scenario", max_active);
+    if (rc) return rc;
+    {
+        // the live state counts every placed prefix pod on its node: a scenario without that node would keep them there
+        const uint32_t N1 = std::max(1u, ctx->snap.N);
+        std::vector<uint8_t> held(N1, 0);
+        std::vector<uint32_t> nodes;
+        for (uint32_t q = 0; q < n_prefix; q++)
+            if (placed[q] >= 0 && !held[placed[q]]) { held[placed[q]] = 1; nodes.push_back((uint32_t)placed[q]); }
+        for (uint32_t i = 0; i < n; i++) {
+            const int32_t *rank = ctx->batch.h_rank.data() + (size_t)i * N1;
+            for (uint32_t g : nodes)
+                if (rank[g] < 0) return fail(ctx, SIMON_ERR_INVALID, "grow scenario %u leaves out node %u, which holds a placed prefix pod", i, g);
+        }
+    }
+    if (out_local && !ctx->valid.has(STORAGE)) return fail(ctx, SIMON_ERR_STATE, "simon_grow_run: out_local without simon_storage_upload");
+    const uint32_t T = P - n_prefix;
+    CU(cudaSetDevice(ctx->device));
+    {
+        // the per-tail-pod outputs (node, GPU slots, score: 16 B per pod and scenario) and one failure record per tail pod and scenario
+        size_t fr = 0, tot = 0;
+        CU(cudaMemGetInfo(&fr, &tot));
+        const uint64_t cells = (uint64_t)n * T + n_prefix;
+        const uint64_t held = 16ull * ctx->grow.d_node.cap + (4ull * SIMON_N_FAIL_CODES + 4) * ctx->grow.d_fail_pod.cap;
+        const uint64_t need = 16ull * cells + (4ull * SIMON_N_FAIL_CODES + 4) * n * T;
+        if (cells >= (1ull << 32) || need > (uint64_t)fr + held)
+            return fail(ctx, SIMON_ERR_LIMIT, "simon_grow_run: outputs of %u scenarios x %u tail pods (%llu bytes) do not fit the device (%llu bytes free)",
+                        n, T, (unsigned long long)need, (unsigned long long)fr);
+    }
+    ctx->last_launch = simon_launch_info{};
+    // the batch pool is no longer a drain or probe batch's, nor are its Open-Local slices another storage batch's
+    ctx->valid.drop(DRAIN_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
+    if (n == 0) return SIMON_OK;
+    cudaStream_t st = ctx->stream;
+    ScenPool &B = ctx->batch;
+    const bool storage = ctx->valid.has(STORAGE);
+    // ---- geometry of the batch placement variants, the batch pool and the outputs (allocations before the timed work) ----
+    uint32_t CS, TPB, NPT;
+    size_t smem;
+    rc = choose_geometry(ctx, max_active, CS, TPB, NPT, smem, n);
+    if (rc) return rc;
+    rc = size_pool(ctx, B, n, false, false);
+    if (rc) return rc;
+    const size_t cells = (size_t)n * T + n_prefix, rows = std::max<size_t>(1, (size_t)n * T);
+    const bool scores = ctx->opt_flags & SIMON_OPT_RECORD_SCORES;
+    CU(ctx->grow.d_node.alloc(cells)); CU(ctx->grow.d_gpu.alloc(cells));
+    if (scores) CU(ctx->grow.d_score.alloc(cells));
+    CU(ctx->grow.d_fail_counts.alloc(rows * SIMON_N_FAIL_CODES)); CU(ctx->grow.d_fail_pod.alloc(rows));
+    std::vector<SkScenario> h;
+    CU(batch_scenarios(ctx, scen, n, h));
+    for (uint32_t i = 0; i < n; i++) {
+        const size_t base = (size_t)i * T;
+        h[i].out_node = ctx->grow.d_node.p + base; h[i].out_gpu = ctx->grow.d_gpu.p + base;
+        h[i].out_score = scores ? ctx->grow.d_score.p + base : nullptr;
+        h[i].fail_counts = ctx->grow.d_fail_counts.p + base * SIMON_N_FAIL_CODES;
+        h[i].fail_pod = ctx->grow.d_fail_pod.p + base;
+    }
+    CU(B.scen.upload(h.data(), n, st));
+    // ---- setup: the live state of the prefix in every slot, with its Open-Local state when storage is uploaded ----
+    SkParams Pb;
+    rc = live_batch_setup(ctx, placed, n_prefix, n, storage, ctx->grow.d_fail_counts.p, rows * SIMON_N_FAIL_CODES, Pb);
+    if (rc) return rc;
+    CU(cudaEventRecord(ctx->evm, st));
+    // ---- placement of every scenario's tail, on its active nodes ----
+    if (T) {
+        Pb.first = n_prefix; Pb.count = T; Pb.max_fail = T; Pb.npt = NPT;
+        rc = launch(ctx, Pb, n, CS, TPB, smem, false);
+        if (rc) return rc;
+    }
+    CU(cudaEventRecord(ctx->ev1, st));
+    std::vector<simon_scenario_result> res;
+    rc = live_batch_reduce(ctx, n, out_local != nullptr, res, out_local);
+    if (rc) return rc;
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    ctx->valid.set(LIVE);
+    CU(cudaEventElapsedTime(&ctx->grow.setup_ms, ctx->ev0, ctx->evm));
+    CU(cudaEventElapsedTime(&ctx->grow.place_ms, ctx->evm, ctx->ev1));
+    CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    ctx->grow.nfail.resize(n);
+    for (uint32_t i = 0; i < n; i++) {
+        out[i] = res[i];
+        ctx->grow.nfail[i] = res[i].n_unscheduled;
+    }
+    ctx->grow.n = n; ctx->grow.n_prefix = n_prefix; ctx->grow.tail = T;
+    ctx->valid.set(GROW_BATCH);
+    if (storage) {
+        ctx->storage_batch.n = n;           // simon_scenarios_storage_download serves this batch
+        ctx->valid.set(STORAGE_BATCH);
+    }
+    return SIMON_OK;
+}
+
+extern "C" int simon_grow_download(simon_ctx *ctx, uint32_t scenario, int32_t *node, uint32_t *gpu_slots, int64_t *score,
+                                   uint32_t *fail_counts, uint32_t *fail_pod) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(GROW_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_grow_run batch since the last upload, or a drain or probe batch after it");
+    if (scenario >= ctx->grow.n) return fail(ctx, SIMON_ERR_INVALID, "grow scenario %u of a batch of %u", scenario, ctx->grow.n);
+    CU(cudaSetDevice(ctx->device));
+    const uint32_t T = ctx->grow.tail, nf = std::min(ctx->grow.nfail[scenario], T);
+    const size_t at = (size_t)scenario * T + ctx->grow.n_prefix, base = (size_t)scenario * T;
+    if (node && T) CU(cudaMemcpy(node, ctx->grow.d_node.p + at, 4ull * T, cudaMemcpyDeviceToHost));
+    if (gpu_slots && T) CU(cudaMemcpy(gpu_slots, ctx->grow.d_gpu.p + at, 4ull * T, cudaMemcpyDeviceToHost));
+    if (score && T) {
+        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(cudaMemcpy(score, ctx->grow.d_score.p + at, 8ull * T, cudaMemcpyDeviceToHost));
+        else memset(score, 0, 8ull * T);
+    }
+    if (fail_counts && nf)
+        CU(cudaMemcpy(fail_counts, ctx->grow.d_fail_counts.p + base * SIMON_N_FAIL_CODES, 4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
+    if (fail_pod && nf) CU(cudaMemcpy(fail_pod, ctx->grow.d_fail_pod.p + base, 4ull * nf, cudaMemcpyDeviceToHost));
+    return SIMON_OK;
+}
+
+extern "C" int simon_grow_times(simon_ctx *ctx, float *setup_ms, float *place_ms) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (setup_ms) *setup_ms = ctx->grow.setup_ms;
+    if (place_ms) *place_ms = ctx->grow.place_ms;
     return SIMON_OK;
 }
 

@@ -291,6 +291,9 @@ SIGNATURES = {
     "simon_probe_run": (_I, [_P, _P, _P, _U32, _P, _P]),
     "simon_probe_download": (_I, [_P, _U32, _P, _P, _P, _P]),
     "simon_probe_times": (_I, [_P, _PF, _PF]),
+    "simon_grow_run": (_I, [_P, _P, _U32, _P, _U32, _P, _P]),
+    "simon_grow_download": (_I, [_P, _U32] + [_P] * 5),
+    "simon_grow_times": (_I, [_P, _PF, _PF]),
     "simon_pdbs_upload": (_I, [_P, _P]),
     "simon_pdbs_allowed": (_I, [_P, _P]),
     "simon_host_go118_sort": (_I, [_P, _U32, _P]),

@@ -100,38 +100,16 @@ def auto_add_nodes(cluster: ResourceTypes, apps: List[AppResource], new_node, ru
     if open_local:
         keys += ("vg_requested", "vg_capacity")
 
-    def evaluate(klist):
-        todo = [by_k[k] for k in klist if k not in per_k]
+    def evaluate(pairs):
+        todo = [by_k[k] for _s, k in pairs if k not in per_k]
         for sc, res in zip(todo, runner(ss, todo)):
             per_k[sc.k] = {q: int(res[q]) for q in keys}
 
-    def ok(k):
+    def ok(_s, k):
         r = per_k[k]
         return r["n_unscheduled"] == 0 and capacity.occupancy_ok(r, max_cpu, max_mem, max_vg)
 
-    rounds = 0
-    if method == "sweep" or not specs:
-        evaluate(ks if specs else [0])
-        rounds = 1
-        best = next((k for k in sorted(per_k) if ok(k)), -1)
-    else:
-        evaluate([0, kmax])
-        rounds = 1
-        if ok(0):
-            best = 0
-        elif not ok(kmax):
-            best = -1
-        else:
-            lo, hi = 0, kmax                   # invariant: lo infeasible, hi feasible
-            while hi - lo > 1:
-                mid = (lo + hi) // 2
-                evaluate([mid])
-                rounds += 1
-                if ok(mid):
-                    hi = mid
-                else:
-                    lo = mid
-            best = hi
+    (best,), rounds = capacity.search_min_k(1, kmax, method if specs else "sweep", evaluate, ok)
     return ApplyResult(best, per_k[0]["n_unscheduled"] if 0 in per_k else -1, len(per_k), rounds, per_k)
 
 

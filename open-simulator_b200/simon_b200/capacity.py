@@ -55,15 +55,7 @@ def build_scenarios(cluster: ResourceTypes, apps: List[AppResource], specs: Sequ
     annotation (make_valid_node_by_node keeps annotations, like NewFakeNodes), so each copy adds the spec's VGs and devices."""
     kmax = max(ks) if len(ks) else 0
     base = list(cluster.Nodes)
-    pool: List[Tuple[int, int, Obj]] = []
-    for si, spec in enumerate(specs):
-        work = deep_copy(spec)
-        for i in range(kmax):
-            # NewFakeNodes mutates its template across iterations (pkg/utils/utils.go:890-899); names are
-            # simon-<rand5> in the reference, simon-<spec>-<ordinal> here
-            n = make_valid_node_by_node(work, f"{O.NEW_NODE_NAME_PREFIX}-{si:02d}-{i:05d}")
-            n["metadata"]["labels"][O.LABEL_NEW_NODE] = ""
-            pool.append((si, i, deep_copy(n)))
+    pool = pool_nodes(specs, kmax)
     nodes = base + [n for (_s, _i, n) in pool]
     # pod list over the superset (DaemonSet pods are generated per node and guarded by it)
     pods: List[PodRec] = get_valid_pod_exclude_daemonset(cluster)
@@ -77,19 +69,40 @@ def build_scenarios(cluster: ResourceTypes, apps: List[AppResource], specs: Sequ
                          statefulsets=list(cluster.StatefulSets))
     storage_classes = list(cluster.StorageClasss) + [sc for a in apps for sc in a.Resource.StorageClasss] if open_local else None
     compiled = compile_cluster(nodes, pods, ctx, open_local=open_local, storage_classes=storage_classes, local_devices=local_devices)
+    nb = len(base)
+    scenarios = scenario_nodes(compiled, nodes, nb, kmax, len(specs), ks)
+    return ScenarioSet(compiled, scenarios, pods, nb)
+
+
+def pool_nodes(specs: Sequence[Obj], kmax: int) -> List[Tuple[int, int, Obj]]:
+    """The candidate pool of a superset: (spec, ordinal, node) for kmax copies of every spec, spec by spec."""
+    pool: List[Tuple[int, int, Obj]] = []
+    for si, spec in enumerate(specs):
+        work = deep_copy(spec)
+        for i in range(kmax):
+            # NewFakeNodes mutates its template across iterations (pkg/utils/utils.go:890-899); names are
+            # simon-<rand5> in the reference, simon-<spec>-<ordinal> here
+            n = make_valid_node_by_node(work, f"{O.NEW_NODE_NAME_PREFIX}-{si:02d}-{i:05d}")
+            n["metadata"]["labels"][O.LABEL_NEW_NODE] = ""
+            pool.append((si, i, deep_copy(n)))
+    return pool
+
+
+def scenario_nodes(compiled: Compiled, nodes: List[Obj], nb: int, kmax: int, n_specs: int, ks: Sequence[int]) -> List[Scenario]:
+    """One Scenario per (spec, k in ks), spec by spec: the nb base nodes plus the first k pool copies of the spec (nodes = base +
+    pool_nodes(specs, kmax), compiled as `compiled`), in the scenario's own nodeTree.list() order as compiled node indices."""
     orig_to_compiled = np.zeros(len(nodes), np.int64)
     for ci, oi in enumerate(compiled.node_orig_index):
         orig_to_compiled[oi] = ci
     scenarios: List[Scenario] = []
-    nb = len(base)
-    for si in range(len(specs)):
+    for si in range(n_specs):
         for k in ks:
             members = list(range(nb)) + [nb + si * kmax + i for i in range(k)]
             sub = [nodes[m] for m in members]
             order = node_tree_list(sub)                      # positions within `members`
             act = np.array([orig_to_compiled[members[o]] for o in order], dtype=np.uint32)
             scenarios.append(Scenario(len(scenarios), si, k, act))
-    return ScenarioSet(compiled, scenarios, pods, nb)
+    return scenarios
 
 
 def occupancy_ok(res: Dict[str, int], max_cpu: int = 100, max_mem: int = 100, max_vg: int = 100) -> bool:
@@ -180,6 +193,43 @@ def search(ss: ScenarioSet, runner: Runner, rank: int = 0, world: int = 1, all_r
         local_best = min(local_best, scenario_key(sc, res, max_cpu, max_mem, max_vg))
     best = all_reduce_min(local_best) if all_reduce_min is not None else local_best
     return best, by_sid
+
+
+def search_min_k(n_specs: int, kmax: int, method: str, evaluate: Callable[[List[Tuple[int, int]]], None],
+                 ok: Callable[[int, int], bool]) -> Tuple[List[int], int]:
+    """The add-node search over k in [0, kmax] for each of n_specs specs: evaluate(pairs) runs the (spec, k) pairs given (one batch per
+    call), ok(spec, k) tells whether an evaluated pair is feasible.  "sweep": every pair in one batch.  Otherwise bisection, valid
+    because feasibility is monotone in k for one spec: (s, 0) and (s, kmax) of every spec in one batch, then one batch per round with
+    the midpoint of every spec still open.  Returns (per spec the minimal feasible k or -1, rounds)."""
+    ks = range(kmax + 1)
+    if method == "sweep":
+        evaluate([(s, k) for s in range(n_specs) for k in ks])
+        return [next((k for k in ks if ok(s, k)), -1) for s in range(n_specs)], 1
+    evaluate([(s, k) for s in range(n_specs) for k in sorted({0, kmax})])
+    rounds = 1
+    best: List[Optional[int]] = []
+    bounds: Dict[int, List[int]] = {}
+    for s in range(n_specs):
+        if ok(s, 0):
+            best.append(0)
+        elif not ok(s, kmax):
+            best.append(-1)
+        else:
+            best.append(None)
+            bounds[s] = [0, kmax]                   # invariant: lo infeasible, hi feasible
+    while True:
+        for s, (lo, hi) in list(bounds.items()):
+            if hi - lo <= 1:
+                best[s] = hi
+                del bounds[s]
+        if not bounds:
+            break
+        mids = {s: (lo + hi) // 2 for s, (lo, hi) in bounds.items()}
+        evaluate(list(mids.items()))
+        rounds += 1
+        for s, mid in mids.items():
+            bounds[s][1 if ok(s, mid) else 0] = mid
+    return [int(b) for b in best], rounds
 
 
 def decode_key(key: int):

@@ -519,3 +519,58 @@ class Engine:
                 out.append(d)
         self.last_probe = info
         return out
+
+    # ---- grow batches (simon_grow_run) ----
+    def grow_run(self, placed, n_prefix: int, scenarios: List[np.ndarray], detail: bool = True, chunk: Optional[int] = None):
+        """Grow scenarios on the live state placed[:n_prefix] (out_node of the prefix pods): each entry of scenarios lists its active
+        nodes in their nodeTree.list() order, and places the tail pods [n_prefix, n_pods) on them from the live state.  The list runs
+        in batches sized as drain_run sizes them, where one scenario also holds its per-tail-pod outputs and failure records (16 + 4 x 24 + 4
+        = 116 bytes per tail pod); chunk: an explicit batch size.  Returns one dict per scenario: n_scheduled / n_unscheduled over its
+        existing tail pods that reach the scheduler and the sums req_mcpu / alloc_mcpu / req_mem / alloc_mem over its active nodes,
+        vg_requested / vg_capacity on a cluster compiled with open_local=True; with detail also node, gpu_slots and score per tail pod
+        [n_pods - n_prefix] (node -3: the pod does not exist in the scenario), and fail_counts [n_unscheduled][24] and fail_pod.
+        self.last_grow: chunks, scenario_bytes, setup_ms / place_ms (device time summed over the batches), launches.
+        scenario_storage_state(i) then describes scenario i of the last chunk."""
+        L = lib()
+        pl = np.ascontiguousarray(np.asarray(placed)[:n_prefix], dtype=np.int32)
+        P = self.c.pods_dims["n_pods"]
+        T = max(P - int(n_prefix), 0)
+        local = getattr(self.c, "storage", None) is not None
+        n = len(scenarios)
+        per, free = self.drain_budget()
+        per += (16 + 4 * abi.N_FAIL_CODES + 4) * T
+        if chunk is None:
+            chunk = max(1, int(free * self.DRAIN_MEM_FRACTION) // max(per, 1))
+        out = []
+        info = dict(chunks=0, scenario_bytes=per, chunk=chunk, setup_ms=0.0, place_ms=0.0, launches=[])
+        for b in range(0, n, chunk):
+            part = scenarios[b:b + chunk]
+            m = len(part)
+            arr, keep = self._scenario_array(part)
+            res = (abi.SimonScenarioResult * m)()
+            loc = (abi.SimonScenarioLocalResult * m)() if local else None
+            self._check(L.simon_grow_run(self.h, pl.ctypes.data if n_prefix else None, int(n_prefix), arr, m, res, loc))
+            su, pm = C.c_float(0), C.c_float(0)
+            self._check(L.simon_grow_times(self.h, C.byref(su), C.byref(pm)))
+            info["chunks"] += 1
+            info["setup_ms"] += float(su.value)
+            info["place_ms"] += float(pm.value)
+            info["launches"].append(self.last_launch())
+            for i, r in enumerate(res):
+                d = dict(n_unscheduled=r.n_unscheduled, n_scheduled=r.n_scheduled, req_mcpu=r.req_mcpu, alloc_mcpu=r.alloc_mcpu,
+                         req_mem=r.req_mem, alloc_mem=r.alloc_mem)
+                if local:
+                    d["vg_requested"], d["vg_capacity"] = int(loc[i].vg_requested), int(loc[i].vg_capacity)
+                if detail:
+                    nf = r.n_unscheduled
+                    node = np.zeros(max(T, 1), np.int32)
+                    slots = np.zeros(max(T, 1), np.uint32)
+                    score = np.zeros(max(T, 1), np.int64)
+                    fc = np.zeros((max(nf, 1), abi.N_FAIL_CODES), np.uint32)
+                    fp = np.zeros(max(nf, 1), np.uint32)
+                    self._check(L.simon_grow_download(self.h, i, node.ctypes.data, slots.ctypes.data, score.ctypes.data, fc.ctypes.data,
+                                                      fp.ctypes.data))
+                    d.update(node=node[:T], gpu_slots=slots[:T], score=score[:T], fail_counts=fc[:nf], fail_pod=fp[:nf])
+                out.append(d)
+        self.last_grow = info
+        return out

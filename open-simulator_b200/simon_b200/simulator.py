@@ -666,6 +666,39 @@ class Simulator:
                 self.last_headroom.append(eng2.last_probe)
         return out
 
+    # ---- nodes to add for new apps (the reference's second use case, README.md:15, on the session's live state) ----
+    def PlanAddNodes(self, apps: List[AppResource], new_nodes: List[Obj], kmax: int = 64, method: str = "sweep",
+                     max_cpu: Optional[int] = None, max_mem: Optional[int] = None, max_vg: Optional[int] = None):
+        """grow.AddNodesPlan: per candidate spec of new_nodes, how many copies must join the running cluster before `apps` fit (the
+        minimal k in [0, kmax]; 0 if they fit already, -1 if none does), with every evaluated k's counts and occupancy, the overall best
+        (spec, k), and at each spec's chosen k (kmax when none fits) each new pod's node and gpu-index and the UnscheduledPods.  The
+        session's pods stay where they are with their GPU-share devices and Open-Local volumes; only the new pods (the apps', and the
+        DaemonSet pods of the cluster and earlier apps on the new nodes) are placed.  method "sweep" runs every k in one device batch,
+        "bisect" halves [0, kmax] per spec.  max_cpu / max_mem / max_vg: satisfyResourceSetting's caps (default: the environment).
+        The superset (the session's nodes plus kmax copies of every spec) is compiled once and runs on a device context of its own;
+        the session's engine, compiled cluster and placements are not changed."""
+        from . import grow
+        from .engine import Engine
+        self._live()
+        if kmax < 0:
+            raise ValueError(f"PlanAddNodes: kmax must be at least 0 (got {kmax})")
+        for n in new_nodes:
+            if not isinstance(n, dict) or n.get("kind") != "Node":
+                raise ValueError(f"PlanAddNodes: new_nodes holds {type(n).__name__} {O.name_of(n) if isinstance(n, dict) else n!r}, not a Node")
+        if method not in grow.METHODS:
+            raise ValueError(f"PlanAddNodes: unknown method {method!r} (one of {', '.join(grow.METHODS)})")
+        import time
+        t0 = time.perf_counter()
+        gs = grow.build(self, apps, new_nodes, kmax)
+        tm = {"compile_s": time.perf_counter() - t0}
+        t0 = time.perf_counter()
+        with Engine(gs.compiled, device=self.options.device, record_scores=self.options.record_scores) as eng:
+            res = grow.plan(eng, gs, [O.name_of(n) for n in new_nodes], method, max_cpu, max_mem, max_vg)
+            self.last_grow = eng.last_grow_batches
+        tm["plan_s"] = time.perf_counter() - t0
+        self.last_grow_timing = tm
+        return res
+
     def Explain(self, entries: list, top: int = 3):
         """Per entry an explain.Explanation: why the pod goes where it goes on the session's state - its node, the feasible count, the
         best `top` feasible nodes with each score plugin's weighted points, and the FitError reasons of the other nodes.  An entry is
