@@ -689,6 +689,44 @@ int simon_drain_times(simon_ctx *ctx, float *setup_ms, float *place_ms);
  * replica of its max_replicas plus one failure record. */
 int simon_drain_budget(simon_ctx *ctx, uint64_t *scenario_bytes, uint64_t *free_bytes);
 
+/* ---- rolling node maintenance: drains in waves, each wave starting from the state the waves before it leave (this library's
+ * definition, built on the drains above) ------------------------------------------------------------------------------------------
+ * A wave base is a single-scenario state plus its placement: for every pod its node (out_node's format) and its GPU slot word
+ * (simon_gpu_slots_download's format).  The single-scenario pool holds it; the library keeps a host mirror of the placement.
+ *   simon_wave_begin   makes the first base: the live state rebuilt from placed[n_pods] exactly as simon_drain_run rebuilds it (placed
+ *                      is checked the same way).
+ *   simon_wave_run     a wave batch: n drains (remain[i] lists the nodes that remain, as for simon_drain_run) whose scenarios start from
+ *                      the base, with no rebuild.  The base is copied into every slot, the pods of each scenario's removed nodes are
+ *                      taken out of its counters at the nodes the base gives them, and the evicted pods are placed in pod order by the
+ *                      drain kernels.  Vanished, blocked and evicted pods are classified as simon_drain_run classifies them, and PDB
+ *                      `allowed` is computed on the base placement.  Drain i's results equal those of simon_drain_run(base placement,
+ *                      remain[i]) from a live state equal to the base.  simon_drain_download, simon_drain_pdb_download and
+ *                      simon_drain_times serve the batch as they serve a drain batch.
+ *   simon_wave_commit  scenario `scenario` of the last wave batch becomes the next base: (1) its slot's dynamic state is copied into the
+ *                      base; (2) its evicted pods' nodes and GPU slot words are written into the base placement, on the device and in
+ *                      the mirror; (3) its removed nodes return: each one's requests, non-zero requests, pod count, scalars and GPU-share
+ *                      memory per device are reset to an empty node's, then its DaemonSet pods (guarded to it and placed there in the
+ *                      base) are added back in pod order, with the requests and counter increments the import adds and Reserve for the
+ *                      GPU-share ones that went through the scheduler, as the resume's replay does on an empty node (their slot words
+ *                      are rewritten).  The per-class summaries and own-score caches are cleared by the next wave batch's setup.
+ *                      SIMON_ERR_INVALID before any device work for a scenario out of range, or one with an unscheduled evicted pod,
+ *                      a blocked pod or a violated PDB.  No other scenario of that batch may be committed afterwards.
+ * Open-Local: there is no wave variant.  Pods with Open-Local volumes block a wave as they block simon_drain_run, and the base's VG and
+ * device state never changes.  The wave calls leave the single-scenario pool holding the base, not the live state: simon_moves_plan and
+ * simon_pdbs_allowed refuse (SIMON_ERR_STATE) until a call that rebuilds or places into the pool.  Any upload, and any call that
+ * rebuilds or places into the single-scenario pool (simon_schedule, simon_schedule_resume, simon_replay, simon_state_reset, a drain,
+ * probe or grow batch), drops the base.  Wave, drain, probe, grow and scenario batches share the batch pool: any of them drops the last
+ * wave batch, and a wave batch drops the others' results as a drain batch does.
+ * SIMON_ERR_STATE: simon_wave_run, simon_wave_commit or simon_wave_download without a base, or simon_wave_commit without a wave batch
+ * since the base last changed.  simon_wave_run's other refusals are simon_drain_run's (a drain that leaves no node, a bad node list). */
+int simon_wave_begin(simon_ctx *ctx, const int32_t *placed);
+int simon_wave_run(simon_ctx *ctx, const simon_scenario *remain, uint32_t n, simon_drain_result *out);
+int simon_wave_commit(simon_ctx *ctx, uint32_t scenario);
+/* The current base placement: per pod its node [n_pods] and GPU slot word [n_pods]; either pointer may be NULL. */
+int simon_wave_download(simon_ctx *ctx, int32_t *placed, uint32_t *gpu_slots);
+/* Device time of the last wave batch (setup: copies into the slots and counter removal; placement) and of the last commit, ms. */
+int simon_wave_times(simon_ctx *ctx, float *setup_ms, float *place_ms, float *commit_ms);
+
 /* ---- scheduling headroom (the reference's first use case, README.md:14 capacity planning, asked of the running cluster; it has no
  * code for it, so the definition is this library's) -------------------------------------------------------------------------------
  * The live state is placed[n_pods], checked as simon_drain_run checks it.  A probe (pod q, max_replicas R >= 1) asks how many more

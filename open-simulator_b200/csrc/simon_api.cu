@@ -247,6 +247,8 @@ enum Data : uint32_t {
     STORAGE_BATCH = 1u << 10, DRAIN_BATCH = 1u << 11, PLAN = 1u << 12, PROBE_BATCH = 1u << 13,
     EXPLAIN_SET = 1u << 14,     // simon_explain_set's pods, records and device tables
     GROW_BATCH = 1u << 15,
+    WAVE_BASE = 1u << 16,       // the single-scenario pool holds a wave base (simon_wave_begin, simon_wave_commit) and wave.place / slots mirror it
+    WAVE_BATCH = 1u << 17,      // the last drain batch is a wave batch from the current base (simon_wave_run)
 };
 
 struct Validity {
@@ -257,10 +259,11 @@ struct Validity {
     void drop(uint32_t d) {
         static constexpr uint32_t derived[][2] = {
             {SNAPSHOT, POD_SET},
-            {POD_SET, STORAGE | PDB_TABLE | LIVE | PLAN | DRAIN_BATCH | PROBE_BATCH | GROW_BATCH | MOVE_LIST | SCOPE_PREP | STATIC_FILL | EXPLAIN_SET},
-            {STORAGE, DEVICES | STORAGE_BATCH | LIVE | SCOPE_PREP},     // SCOPE_PREP: the move-class records exclude local classes
-            {DEVICES, STORAGE_BATCH | LIVE},
+            {POD_SET, STORAGE | PDB_TABLE | LIVE | WAVE_BASE | PLAN | DRAIN_BATCH | PROBE_BATCH | GROW_BATCH | MOVE_LIST | SCOPE_PREP | STATIC_FILL | EXPLAIN_SET},
+            {STORAGE, DEVICES | STORAGE_BATCH | LIVE | WAVE_BASE | SCOPE_PREP},     // SCOPE_PREP: the move-class records exclude local classes
+            {DEVICES, STORAGE_BATCH | LIVE | WAVE_BASE},
             {MOVE_LIST, MOVE_RUN},
+            {WAVE_BASE, WAVE_BATCH},
         };
         for (const auto &r : derived)
             if (d & r[0]) d |= r[1];
@@ -392,6 +395,15 @@ struct simon_ctx {
         DevBuf<int64_t> d_score;
         float setup_ms = 0.f, place_ms = 0.f;
     } grow;
+    // the wave base (simon_wave_begin): the single-scenario pool's state and its per-pod results (out_node, out_gpu) are the base, and
+    // place / slots their host mirror; of the last wave batch, each scenario's removed nodes (CSR roff / removed, index order) and
+    // vanished pods (CSR voff / vanished, pod order), which return with them; on the device the returned nodes and their pods (CSR) of the last commit, and its device time
+    struct {
+        std::vector<int32_t> place;
+        std::vector<uint32_t> slots, voff, vanished, roff, removed;
+        DevBuf<uint32_t> d_nodes, d_off, d_pods;
+        float commit_ms = 0.f;
+    } wave;
     // the last migration plan (simon_moves_plan): its end state in plan-owned copies of the single-scenario node state, placement and
     // GPU slot words, the steps and control words
     struct {
@@ -885,6 +897,7 @@ int rebuild_prefix(simon_ctx *ctx, const SkParams &P, const int32_t *prefix_node
 
 // Before a run on the single-scenario pool: clear its failure records and counters; arm the dump in P if its pod is in [first, first + count)
 cudaError_t single_begin(simon_ctx *ctx, SkParams &P, uint32_t first = 0, uint32_t count = 0) {
+    ctx->valid.drop(WAVE_BASE);         // the run overwrites the pool that holds it
     cudaStream_t st = ctx->stream;
     cudaError_t e = cudaMemsetAsync(ctx->single.fail_counts.p, 0, 4ull * ctx->pods.max_fail * SIMON_N_FAIL_CODES, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(ctx->single.counters.p, 0, 8, st);
@@ -1238,7 +1251,7 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
 int simon_state_reset(simon_ctx *ctx) {
     if (!ctx || !ctx->valid.has(POD_SET)) return ctx ? fail(ctx, SIMON_ERR_STATE, "no pods uploaded") : SIMON_ERR_INVALID;
     CU(cudaSetDevice(ctx->device));
-    ctx->valid.drop(LIVE);
+    ctx->valid.drop(LIVE | WAVE_BASE);
     int rc = clear_pool(ctx, ctx->single);
     if (rc) return rc;
     CU(cudaStreamSynchronize(ctx->stream));
@@ -1408,6 +1421,7 @@ static int scenarios_run(simon_ctx *ctx, const simon_scenario *scen, uint32_t n,
     ScenPool &B = ctx->batch;
     const bool local = out_local != nullptr;
     if (local) ctx->valid.drop(STORAGE_BATCH);       // the slices are overwritten below
+    ctx->valid.drop(WAVE_BATCH);                    // and so are the slots a wave commit copies from
     // ---- node lists: validated on the host, uploaded in ONE copy each (scenario order and its inverse) ----
     uint32_t max_active = 0;
     int rc = scenario_lists(ctx, scen, n, "scenario", max_active);
@@ -1514,6 +1528,25 @@ extern "C" int simon_drain_budget(simon_ctx *ctx, uint64_t *scenario_bytes, uint
     return SIMON_OK;
 }
 
+// The single-scenario state copied into each of the n slots of the batch pool, one broadcast per column, and what the copies do not
+// overwrite cleared (live_batch_setup below).  A wave batch's whole setup: its single-scenario state is the wave base.
+static int batch_from_single(simon_ctx *ctx, uint32_t n, bool local, uint32_t *fail_counts, size_t fail_words, SkParams &Pb) {
+    ScenPool &S = ctx->single, &B = ctx->batch;
+    cudaStream_t st = ctx->stream;
+    CU(cudaMemsetAsync(B.csum.p, 0, 8 * n * B.ncl * SK_CSUM_W, st));
+    CU(cudaMemsetAsync(B.ocache.p, 0, 8 * n * B.nodes * B.ncl, st));
+    CU(cudaMemsetAsync(B.counters.p, 0, 8ull * n, st)); CU(cudaMemsetAsync(B.clk.p, 0, 16ull * n, st));
+    CU(cudaMemsetAsync(fail_counts, 0, 4ull * fail_words, st));
+    CU(B.state.each(S.state, true, [&](auto &b, auto &s, uint64_t k) { ctx->launches++; return bcast(ctx, s.p, k, n, b.p); }));
+    if (local) {
+        CU(bcast(ctx, S.vg_req.p, B.vn, n, B.vg_req.p));
+        ctx->launches++;
+        if (ctx->valid.has(DEVICES)) { CU(bcast(ctx, S.dev_alloc.p, B.nodes, n, B.dev_alloc.p)); ctx->launches++; }
+    }
+    fill_params(ctx, B, Pb);
+    return SIMON_OK;
+}
+
 // The setup drain, probe and grow batches share, enqueued once their refusals and allocations are done: the live state that pods
 // [0, n_prefix) leave at `placed`, rebuilt into the single-scenario pool (the resume's rebuild, its failure records cleared as the resume clears them) and copied into
 // each of the n slots of the batch pool, one broadcast per column.  Of the batch pool only what the copies do not overwrite is cleared:
@@ -1532,18 +1565,7 @@ static int live_batch_setup(simon_ctx *ctx, const int32_t *placed, uint32_t n_pr
     CU(single_begin(ctx, Ps));
     rc = rebuild_prefix(ctx, Ps, placed, n_prefix);
     if (rc) return rc;
-    CU(cudaMemsetAsync(B.csum.p, 0, 8 * n * B.ncl * SK_CSUM_W, st));
-    CU(cudaMemsetAsync(B.ocache.p, 0, 8 * n * B.nodes * B.ncl, st));
-    CU(cudaMemsetAsync(B.counters.p, 0, 8ull * n, st)); CU(cudaMemsetAsync(B.clk.p, 0, 16ull * n, st));
-    CU(cudaMemsetAsync(fail_counts, 0, 4ull * fail_words, st));
-    CU(B.state.each(S.state, true, [&](auto &b, auto &s, uint64_t k) { ctx->launches++; return bcast(ctx, s.p, k, n, b.p); }));
-    if (local) {
-        CU(bcast(ctx, S.vg_req.p, B.vn, n, B.vg_req.p));
-        ctx->launches++;
-        if (ctx->valid.has(DEVICES)) { CU(bcast(ctx, S.dev_alloc.p, B.nodes, n, B.dev_alloc.p)); ctx->launches++; }
-    }
-    fill_params(ctx, B, Pb);
-    return SIMON_OK;
+    return batch_from_single(ctx, n, local, fail_counts, fail_words, Pb);
 }
 
 // After a drain, probe or grow batch's launch: each scenario's sums over its active nodes (simon_scen_reduce) into res and, local, its VG sums
@@ -1566,16 +1588,18 @@ static int live_batch_reduce(simon_ctx *ctx, uint32_t n, bool local, std::vector
 }
 
 // simon_drain_run and simon_drain_run_local (out_local != nullptr: pods with Open-Local volumes are evicted, not blocked, and each
-// scenario carries its own Open-Local state, the live one to start with)
+// scenario carries its own Open-Local state, the live one to start with).  wave (simon_wave_run): the scenarios start from the wave
+// base, which `placed` mirrors, instead of a state rebuilt from `placed`, and each one's vanished pods are kept for a commit.
 static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario *remain, uint32_t n, simon_drain_result *out,
-                     simon_scenario_local_result *out_local) {
+                     simon_scenario_local_result *out_local, bool wave = false) {
     const bool local = out_local != nullptr;
-    const char *what = local ? "simon_drain_run_local" : "simon_drain_run";
+    const char *what = wave ? "simon_wave_run" : local ? "simon_drain_run_local" : "simon_drain_run";
     if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "%s before uploads", what);
     if ((ctx->pods.n_pods && !placed) || (n && (!remain || !out))) return fail(ctx, SIMON_ERR_INVALID, "%s: NULL argument", what);
     const uint32_t N = ctx->snap.N, N1 = std::max(1u, N), P = ctx->pods.n_pods;
-    // ---- refusals before any device work: the live placement as a resume prefix checks it, then the node lists ----
-    int rc = check_prefix(ctx, placed, P);
+    // ---- refusals before any device work: the live placement as a resume prefix checks it (a wave base was checked when it began),
+    // then the node lists ----
+    int rc = wave ? SIMON_OK : check_prefix(ctx, placed, P);
     if (rc) return rc;
     for (uint32_t i = 0; i < n; i++)
         if (remain[i].n_nodes == 0) return fail(ctx, SIMON_ERR_INVALID, "drain %u leaves no node", i);
@@ -1585,7 +1609,7 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
     CU(cudaSetDevice(ctx->device));
     ctx->last_launch = simon_launch_info{};
     // the batch pool is no longer a probe or grow batch's, nor are its Open-Local slices a storage batch's
-    ctx->valid.drop(DRAIN_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
+    ctx->valid.drop(DRAIN_BATCH | WAVE_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
     ScenPool &S = ctx->single, &B = ctx->batch;
     if (n == 0) return SIMON_OK;
     cudaStream_t st = ctx->stream;
@@ -1606,22 +1630,30 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
     std::vector<uint2> pairs;
     std::vector<uint32_t> n_vanished(n, 0u), rm;
     ctx->drain.max = 0;
+    ctx->wave.voff.assign(1, 0u); ctx->wave.vanished.clear(); ctx->wave.roff.assign(1, 0u); ctx->wave.removed.clear();
     for (uint32_t i = 0; i < n; i++) {
         const int32_t *rank = B.h_rank.data() + (size_t)i * N1;
         rm.clear();
         for (uint32_t g = 0; g < N; g++)
-            if (rank[g] < 0) rm.insert(rm.end(), node_pods.begin() + node_off[g], node_pods.begin() + node_off[g + 1]);
+            if (rank[g] < 0) {
+                rm.insert(rm.end(), node_pods.begin() + node_off[g], node_pods.begin() + node_off[g + 1]);
+                if (wave) ctx->wave.removed.push_back(g);
+            }
+        ctx->wave.roff.push_back((uint32_t)ctx->wave.removed.size());
         std::sort(rm.begin(), rm.end());
         for (uint32_t q : rm) {
             pairs.push_back(make_uint2(i, q));
             const int32_t gd = ctx->pods.h_guard[q];
-            if (gd >= 0 && rank[gd] < 0) n_vanished[i]++;
-            else if (ctx->pods.h_fixed[q] >= 0 || (!local && ctx->valid.has(STORAGE) && ctx->storage.h_class_local[ctx->pods.h_class[q]]))
+            if (gd >= 0 && rank[gd] < 0) {
+                n_vanished[i]++;
+                if (wave) ctx->wave.vanished.push_back(q);
+            } else if (ctx->pods.h_fixed[q] >= 0 || (!local && ctx->valid.has(STORAGE) && ctx->storage.h_class_local[ctx->pods.h_class[q]]))
                 ctx->drain.blocked.push_back(q);
             else ctx->drain.pods.push_back(q);
         }
         ctx->drain.off.push_back((uint32_t)ctx->drain.pods.size());
         ctx->drain.boff.push_back((uint32_t)ctx->drain.blocked.size());
+        ctx->wave.voff.push_back((uint32_t)ctx->wave.vanished.size());
         ctx->drain.max = std::max(ctx->drain.max, ctx->drain.off[i + 1] - ctx->drain.off[i]);
     }
     const size_t n_ev = ctx->drain.pods.size();
@@ -1648,14 +1680,21 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
         h[i].fail_pod = ctx->drain.d_fail_pod.p + (size_t)i * ctx->drain.max;
     }
     CU(B.scen.upload(h.data(), n, st));
-    // ---- setup: the live state in every slot (live_batch_setup), minus what each scenario's removed nodes' pods contributed to the
-    // counters.  local: the removed nodes' VGs and devices keep their live values, since those nodes are inactive ----
+    // ---- setup: the live state in every slot (live_batch_setup; a wave: the base, batch_from_single), minus what each scenario's
+    // removed nodes' pods contributed to the counters, at their nodes in that state.  local: the removed nodes' VGs and devices keep
+    // their live values, since those nodes are inactive ----
     SkParams Pb;
-    rc = live_batch_setup(ctx, placed, P, n, local, ctx->drain.d_fail_counts.p, (size_t)n * ctx->drain.max * SIMON_N_FAIL_CODES, Pb);
+    const size_t fail_words = (size_t)n * ctx->drain.max * SIMON_N_FAIL_CODES;
+    if (wave) {
+        CU(cudaEventRecord(ctx->ev0, st));
+        rc = batch_from_single(ctx, n, false, ctx->drain.d_fail_counts.p, fail_words, Pb);
+    } else {
+        rc = live_batch_setup(ctx, placed, P, n, local, ctx->drain.d_fail_counts.p, fail_words, Pb);
+    }
     if (rc) return rc;
     if (!pairs.empty()) {
         const uint32_t grid = (uint32_t)std::min<size_t>((pairs.size() + 255) / 256, (size_t)ctx->sms * 4);
-        simon_drain_unimport<<<grid, 256, 0, st>>>(Pb, ctx->d_prefix.p, ctx->drain.d_pairs.p, (uint32_t)pairs.size());
+        simon_drain_unimport<<<grid, 256, 0, st>>>(Pb, wave ? S.out_node.p : ctx->d_prefix.p, ctx->drain.d_pairs.p, (uint32_t)pairs.size());
         CU(cudaGetLastError());
         ctx->launches++;
     }
@@ -1669,7 +1708,7 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
     std::vector<simon_scenario_result> res;
     rc = live_batch_reduce(ctx, n, local, res, out_local);
     if (rc) return rc;
-    // with a PDB table: `allowed` on the rebuilt live state, read at the same synchronisation
+    // with a PDB table: `allowed` on the rebuilt live state (a wave: the base), read at the same synchronisation
     const uint32_t J = ctx->valid.has(PDB_TABLE) ? ctx->pdb.n : 0;
     std::vector<int32_t> allowed(J);
     if (J) {
@@ -1678,7 +1717,7 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
     }
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
-    ctx->valid.set(LIVE);
+    if (!wave) ctx->valid.set(LIVE);
     CU(cudaEventElapsedTime(&ctx->drain.setup_ms, ctx->ev0, ctx->evm));
     CU(cudaEventElapsedTime(&ctx->drain.place_ms, ctx->evm, ctx->ev1));
     CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
@@ -1713,7 +1752,7 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
         ctx->drain.nfail[i] = res[i].n_unscheduled;
     }
     ctx->drain.n = n;
-    ctx->valid.set(DRAIN_BATCH);
+    ctx->valid.set(DRAIN_BATCH | (wave ? WAVE_BATCH : 0u));
     if (local) {
         ctx->storage_batch.n = n;           // simon_scenarios_storage_download serves this batch
         ctx->valid.set(STORAGE_BATCH);
@@ -1775,6 +1814,124 @@ extern "C" int simon_drain_pdb_download(simon_ctx *ctx, uint32_t scenario, uint3
     return SIMON_OK;
 }
 
+// ---- rolling maintenance waves ------------------------------------------------------------------------------------------------
+extern "C" int simon_wave_begin(simon_ctx *ctx, const int32_t *placed) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_begin before uploads");
+    const uint32_t P = ctx->pods.n_pods;
+    if (P && !placed) return fail(ctx, SIMON_ERR_INVALID, "simon_wave_begin: NULL argument");
+    int rc = check_prefix(ctx, placed, P);
+    if (rc) return rc;
+    CU(cudaSetDevice(ctx->device));
+    ScenPool &S = ctx->single;
+    cudaStream_t st = ctx->stream;
+    SkParams Ps;
+    fill_params(ctx, S, Ps);
+    rc = clear_pool(ctx, S);
+    if (rc) return rc;
+    CU(single_begin(ctx, Ps));          // drops the base and the last wave batch
+    rc = rebuild_prefix(ctx, Ps, placed, P);
+    if (rc) return rc;
+    ctx->wave.place.assign(placed, placed + P);
+    ctx->wave.slots.assign(P, 0u);
+    if (P) CU(cudaMemcpyAsync(ctx->wave.slots.data(), S.out_gpu.p, 4ull * P, cudaMemcpyDeviceToHost, st));
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    ctx->valid.drop(LIVE);
+    ctx->valid.set(WAVE_BASE);
+    return SIMON_OK;
+}
+
+extern "C" int simon_wave_run(simon_ctx *ctx, const simon_scenario *remain, uint32_t n, simon_drain_result *out) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(WAVE_BASE)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_run without a wave base (simon_wave_begin)");
+    return drain_run(ctx, ctx->wave.place.data(), remain, n, out, nullptr, true);
+}
+
+extern "C" int simon_wave_commit(simon_ctx *ctx, uint32_t scenario) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(WAVE_BASE)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_commit without a wave base (simon_wave_begin)");
+    if (!ctx->valid.has(WAVE_BATCH)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_commit: no simon_wave_run batch since the base changed");
+    if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u of a batch of %u", scenario, ctx->drain.n);
+    const uint32_t s = scenario;
+    if (ctx->drain.nfail[s]) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u leaves %u evicted pods unscheduled", s, ctx->drain.nfail[s]);
+    if (ctx->drain.boff[s + 1] > ctx->drain.boff[s])
+        return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u has %u blocked pods", s, ctx->drain.boff[s + 1] - ctx->drain.boff[s]);
+    if (ctx->drain.voff[s + 1] > ctx->drain.voff[s])
+        return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u violates %u PDBs", s, ctx->drain.voff[s + 1] - ctx->drain.voff[s]);
+    CU(cudaSetDevice(ctx->device));
+    ScenPool &S = ctx->single, &B = ctx->batch;
+    cudaStream_t st = ctx->stream;
+    const uint32_t N1 = std::max(1u, ctx->snap.N);
+    // ---- on the host: the evicted pods' new nodes; the returned nodes (the scenario's removed ones) and
+    // their DaemonSet pods (its vanished pods), grouped by node, pod order kept ----
+    const uint32_t b = ctx->drain.off[s], ne = ctx->drain.off[s + 1] - b;
+    std::vector<int32_t> node(ne);
+    if (ne) CU(cudaMemcpy(node.data(), ctx->drain.d_node.p + b, 4ull * ne, cudaMemcpyDeviceToHost));
+    std::vector<uint32_t> nodes(ctx->wave.removed.begin() + ctx->wave.roff[s], ctx->wave.removed.begin() + ctx->wave.roff[s + 1]);
+    std::vector<uint32_t> off(1, 0u), pods;
+    {
+        std::vector<uint32_t> cnt(N1, 0u), at(N1, 0u);
+        for (uint32_t k = ctx->wave.voff[s]; k < ctx->wave.voff[s + 1]; k++) cnt[ctx->wave.place[ctx->wave.vanished[k]]]++;
+        for (uint32_t g : nodes) { at[g] = off.back(); off.push_back(off.back() + cnt[g]); }
+        pods.resize(off.back());
+        for (uint32_t k = ctx->wave.voff[s]; k < ctx->wave.voff[s + 1]; k++) {
+            const uint32_t q = ctx->wave.vanished[k];
+            pods[at[ctx->wave.place[q]]++] = q;
+        }
+    }
+    // ---- on the device, timed: the slot's state into the base, the scatter, the return ----
+    CU(ctx->wave.d_nodes.upload(nodes.data(), nodes.size(), st));
+    CU(ctx->wave.d_off.upload(off.data(), off.size(), st));
+    CU(ctx->wave.d_pods.upload(pods.data(), pods.size(), st));
+    CU(cudaEventRecord(ctx->ev0, st));
+    CU(S.state.each(B.state, true, [&](auto &d, auto &c, uint64_t k) {
+        return cudaMemcpyAsync(d.p, c.p + (size_t)s * k, k * sizeof(*d.p), cudaMemcpyDeviceToDevice, st);
+    }));
+    if (ne) {
+        const uint32_t grid = std::min<uint32_t>((ne + 255) / 256, (uint32_t)ctx->sms * 4);
+        simon_wave_scatter<<<grid, 256, 0, st>>>(ctx->drain.d_pods.p + b, ctx->drain.d_node.p + b, ctx->drain.d_gpu.p + b, ne, S.out_node.p,
+                                                 S.out_gpu.p);
+        CU(cudaGetLastError());
+        ctx->launches++;
+    }
+    if (!nodes.empty()) {
+        SkParams Ps;
+        fill_params(ctx, S, Ps);
+        simon_wave_return<<<((uint32_t)nodes.size() + 127) / 128, 128, 0, st>>>(Ps, ctx->wave.d_nodes.p, ctx->wave.d_off.p, ctx->wave.d_pods.p,
+                                                                                 (uint32_t)nodes.size());
+        CU(cudaGetLastError());
+        ctx->launches++;
+    }
+    CU(cudaEventRecord(ctx->ev1, st));
+    // the mirror's slot words: the evicted pods' and the returned DaemonSet pods' changed
+    if (ctx->pods.n_pods) CU(cudaMemcpyAsync(ctx->wave.slots.data(), S.out_gpu.p, 4ull * ctx->pods.n_pods, cudaMemcpyDeviceToHost, st));
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    CU(cudaEventElapsedTime(&ctx->wave.commit_ms, ctx->ev0, ctx->ev1));
+    ctx->last_ms = ctx->wave.commit_ms;
+    for (uint32_t i = 0; i < ne; i++) ctx->wave.place[ctx->drain.pods[b + i]] = node[i];
+    // the batch's slots describe the old base: no other scenario of it may be committed
+    ctx->valid.drop(WAVE_BATCH);
+    return SIMON_OK;
+}
+
+extern "C" int simon_wave_download(simon_ctx *ctx, int32_t *placed, uint32_t *gpu_slots) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(WAVE_BASE)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_download without a wave base (simon_wave_begin)");
+    if (placed) std::copy(ctx->wave.place.begin(), ctx->wave.place.end(), placed);
+    if (gpu_slots) std::copy(ctx->wave.slots.begin(), ctx->wave.slots.end(), gpu_slots);
+    return SIMON_OK;
+}
+
+extern "C" int simon_wave_times(simon_ctx *ctx, float *setup_ms, float *place_ms, float *commit_ms) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (setup_ms) *setup_ms = ctx->drain.setup_ms;
+    if (place_ms) *place_ms = ctx->drain.place_ms;
+    if (commit_ms) *commit_ms = ctx->wave.commit_ms;
+    return SIMON_OK;
+}
+
 // ---- headroom probes ------------------------------------------------------------------------------------------------------------
 extern "C" int simon_probe_run(simon_ctx *ctx, const int32_t *placed, const simon_probe *probes, uint32_t n, simon_probe_result *out,
                                simon_scenario_local_result *out_local) {
@@ -1811,7 +1968,7 @@ extern "C" int simon_probe_run(simon_ctx *ctx, const int32_t *placed, const simo
     }
     ctx->last_launch = simon_launch_info{};
     // the batch pool is no longer a drain or grow batch's, nor are its Open-Local slices another storage batch's
-    ctx->valid.drop(DRAIN_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
+    ctx->valid.drop(DRAIN_BATCH | WAVE_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
     if (n == 0) return SIMON_OK;
     cudaStream_t st = ctx->stream;
     ScenPool &B = ctx->batch;
@@ -1959,7 +2116,7 @@ extern "C" int simon_grow_run(simon_ctx *ctx, const int32_t *placed, uint32_t n_
     }
     ctx->last_launch = simon_launch_info{};
     // the batch pool is no longer a drain or probe batch's, nor are its Open-Local slices another storage batch's
-    ctx->valid.drop(DRAIN_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
+    ctx->valid.drop(DRAIN_BATCH | WAVE_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
     if (n == 0) return SIMON_OK;
     cudaStream_t st = ctx->stream;
     ScenPool &B = ctx->batch;

@@ -1905,6 +1905,53 @@ extern "C" __global__ void __launch_bounds__(256) simon_drain_unimport(const __g
     }
 }
 
+// ---- wave commits (simon_wave_commit) ----------------------------------------------------------------------------------------------
+// The committed scenario's evicted pods into the base placement: pod pods[i] now sits on node[i] with GPU slot word gpu[i].
+extern "C" __global__ void __launch_bounds__(256) simon_wave_scatter(const uint32_t *pods, const int32_t *node, const uint32_t *gpu, uint32_t n,
+                                                                     int32_t *place, uint32_t *slots) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        place[pods[i]] = node[i];
+        slots[pods[i]] = gpu[i];
+    }
+}
+
+// The committed scenario's removed nodes return to the base (the single scenario of P): one thread per node nodes[t], whose dynamic
+// state is reset to an empty node's, then its DaemonSet pods pods[off[t] .. off[t + 1]) (pod order) are added back: the sums and
+// counter increments as simon_import_kernel adds them (written out here, so that the import kernel stays as it is; the node's own
+// sums need no atomics, the counters are shared between nodes), and Reserve of the GPU-share pods that went through the scheduler
+// with gpu_reserve, as simon_resume_replay does on an empty node.  Each pod's GPU slot word in the base is rewritten.
+extern "C" __global__ void __launch_bounds__(128) simon_wave_return(const __grid_constant__ SkParams P, const uint32_t *nodes, const uint32_t *off,
+                                                                    const uint32_t *pods, uint32_t n) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const SkScenario &SC = P.scen[0];
+    const ReqCtx RC{P.label_bits, P.N, -1};
+    const uint32_t N = P.N, K = P.K, g = nodes[t];
+    SC.req_mcpu[g] = 0; SC.req_mem[g] = 0; SC.req_eph[g] = 0; SC.nz_mcpu[g] = 0; SC.nz_mem[g] = 0; SC.num_pods[g] = 0;
+    for (uint32_t k = 0; k < K; k++) SC.req_scalar[(uint64_t)k * N + g] = 0;
+    for (uint32_t d = 0; d < SIMON_MAX_GPU_DEV; d++) SC.gpu_used[(uint64_t)d * N + g] = 0;
+    #pragma unroll 1
+    for (uint32_t i = off[t]; i < off[t + 1]; i++) {
+        const uint32_t q = pods[i];
+        const int64_t *cw = P.class_blob + P.class_off[P.pod_class[q]];
+        SC.req_mcpu[g] += cw[SCW_REQ_MCPU]; SC.req_mem[g] += cw[SCW_REQ_MEM]; SC.req_eph[g] += cw[SCW_REQ_EPH];
+        SC.nz_mcpu[g] += cw[SCW_NZ_MCPU]; SC.nz_mem[g] += cw[SCW_NZ_MEM]; SC.num_pods[g] += 1;
+        const int64_t *sc = cw + cw[SCW_OFF_SCALARS];
+        for (uint32_t k = 0; k < K; k++) SC.req_scalar[(uint64_t)k * N + g] += sc[k];
+        const int64_t *inc = cw + cw[SCW_OFF_INC];
+        for (int64_t u = 0; u < cw[SCW_N_INC]; u++) {
+            const int64_t k = inc[3 * u], tp = inc[3 * u + 1], sig = inc[3 * u + 2];
+            const int32_t d = P.topo_dom[(uint64_t)tp * N + g];
+            if (d < 0) continue;
+            if (sig >= 0 && !elig_eval(P, sig, RC, g)) continue;
+            atomicAdd(&SC.cnt[P.cnt_off[k] + d], 1);
+            atomicAdd(&SC.cnt_total[k], 1);
+        }
+        const int32_t f = P.pod_fixed[q];
+        SC.out_gpu[q] = (f == -1 || f == -4) && cw[SCW_GPU_MEM] > 0 ? gpu_reserve(P, SC, cw, g) : 0u;
+    }
+}
+
 // Every placement-family kernel, declared once: (symbol, threads per CTA at most, node slots per thread (0: counted at run time),
 // per-phase timers, large cluster, Open-Local, drain batch, probe batch, explained decisions).  The kernels below and the table simon_api.cu's kernel_variant()
 // searches come from this list.

@@ -288,6 +288,11 @@ SIGNATURES = {
     "simon_drain_pdb_download": (_I, [_P, _U32, _P, _P]),
     "simon_drain_times": (_I, [_P, _PF, _PF]),
     "simon_drain_budget": (_I, [_P, _PU64, _PU64]),
+    "simon_wave_begin": (_I, [_P, _P]),
+    "simon_wave_run": (_I, [_P, _P, _U32, _P]),
+    "simon_wave_commit": (_I, [_P, _U32]),
+    "simon_wave_download": (_I, [_P, _P, _P]),
+    "simon_wave_times": (_I, [_P, _PF, _PF, _PF]),
     "simon_probe_run": (_I, [_P, _P, _P, _U32, _P, _P]),
     "simon_probe_download": (_I, [_P, _U32, _P, _P, _P, _P]),
     "simon_probe_times": (_I, [_P, _PF, _PF]),

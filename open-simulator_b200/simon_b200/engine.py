@@ -432,32 +432,94 @@ class Engine:
             info["setup_ms"] += float(su.value)
             info["place_ms"] += float(pm.value)
             info["launches"].append(self.last_launch())
-            for i, r in enumerate(res):
-                d = dict(n_evicted=r.n_evicted, n_placed=r.n_placed, n_unscheduled=r.n_unscheduled, n_blocked=r.n_blocked,
-                         n_vanished=r.n_vanished, n_pdb_violated=r.n_pdb_violated, req_mcpu=r.req_mcpu, alloc_mcpu=r.alloc_mcpu,
-                         req_mem=r.req_mem, alloc_mem=r.alloc_mem)
-                if local:
-                    d["vg_requested"], d["vg_capacity"] = int(loc[i].vg_requested), int(loc[i].vg_capacity)
-                if detail:
-                    ne, nb, nf = r.n_evicted, r.n_blocked, r.n_unscheduled
-                    ev = np.zeros(max(ne, 1), np.uint32)
-                    node = np.zeros(max(ne, 1), np.int32)
-                    slots = np.zeros(max(ne, 1), np.uint32)
-                    score = np.zeros(max(ne, 1), np.int64)
-                    blk = np.zeros(max(nb, 1), np.uint32)
-                    fc = np.zeros((max(nf, 1), abi.N_FAIL_CODES), np.uint32)
-                    fp = np.zeros(max(nf, 1), np.uint32)
-                    self._check(L.simon_drain_download(self.h, i, ev.ctypes.data, node.ctypes.data, slots.ctypes.data, score.ctypes.data,
-                                                       blk.ctypes.data, fc.ctypes.data, fp.ctypes.data))
-                    nv = r.n_pdb_violated
-                    vp = np.zeros(max(nv, 1), np.uint32)
-                    vc = np.zeros(max(nv, 1), np.uint32)
-                    self._check(L.simon_drain_pdb_download(self.h, i, vp.ctypes.data, vc.ctypes.data))
-                    d.update(evicted=ev[:ne], node=node[:ne], gpu_slots=slots[:ne], score=score[:ne], blocked=blk[:nb],
-                             fail_counts=fc[:nf], fail_pod=fp[:nf], pdb_violated=vp[:nv], pdb_evicted=vc[:nv])
-                out.append(d)
+            out.extend(self._drain_results(res, loc if local else None, detail))
         self.last_drain = info
         return out
+
+    def _drain_results(self, res, loc, detail: bool) -> List[dict]:
+        """The dicts drain_run returns, of the last drain or wave batch's results `res` (and Open-Local sums `loc`, or None)."""
+        L = lib()
+        out = []
+        for i, r in enumerate(res):
+            d = dict(n_evicted=r.n_evicted, n_placed=r.n_placed, n_unscheduled=r.n_unscheduled, n_blocked=r.n_blocked,
+                     n_vanished=r.n_vanished, n_pdb_violated=r.n_pdb_violated, req_mcpu=r.req_mcpu, alloc_mcpu=r.alloc_mcpu,
+                     req_mem=r.req_mem, alloc_mem=r.alloc_mem)
+            if loc is not None:
+                d["vg_requested"], d["vg_capacity"] = int(loc[i].vg_requested), int(loc[i].vg_capacity)
+            if detail:
+                ne, nb, nf = r.n_evicted, r.n_blocked, r.n_unscheduled
+                ev = np.zeros(max(ne, 1), np.uint32)
+                node = np.zeros(max(ne, 1), np.int32)
+                slots = np.zeros(max(ne, 1), np.uint32)
+                score = np.zeros(max(ne, 1), np.int64)
+                blk = np.zeros(max(nb, 1), np.uint32)
+                fc = np.zeros((max(nf, 1), abi.N_FAIL_CODES), np.uint32)
+                fp = np.zeros(max(nf, 1), np.uint32)
+                self._check(L.simon_drain_download(self.h, i, ev.ctypes.data, node.ctypes.data, slots.ctypes.data, score.ctypes.data,
+                                                   blk.ctypes.data, fc.ctypes.data, fp.ctypes.data))
+                nv = r.n_pdb_violated
+                vp = np.zeros(max(nv, 1), np.uint32)
+                vc = np.zeros(max(nv, 1), np.uint32)
+                self._check(L.simon_drain_pdb_download(self.h, i, vp.ctypes.data, vc.ctypes.data))
+                d.update(evicted=ev[:ne], node=node[:ne], gpu_slots=slots[:ne], score=score[:ne], blocked=blk[:nb],
+                         fail_counts=fc[:nf], fail_pod=fp[:nf], pdb_violated=vp[:nv], pdb_evicted=vc[:nv])
+            out.append(d)
+        return out
+
+    # ---- rolling maintenance waves (simon_wave_*) ----
+    def wave_begin(self, placed):
+        """simon_wave_begin: the wave base is the live state `placed` (out_node of a full placement of the pod list) leaves."""
+        pl = np.ascontiguousarray(placed, dtype=np.int32)
+        self._check(lib().simon_wave_begin(self.h, pl.ctypes.data))
+        self._wave = None
+        self.last_wave = dict(batches=0, setup_ms=0.0, place_ms=0.0, commits=0, commit_ms=0.0, launches=[])
+
+    def wave_run(self, remain_lists: List[np.ndarray], detail: bool = True, chunk: Optional[int] = None) -> List[dict]:
+        """Drains from the wave base, one dict per entry of remain_lists as drain_run returns them; in batches sized as drain_run
+        sizes them (chunk: an explicit batch size).  self.last_wave sums the device times of every batch and commit since wave_begin."""
+        L = lib()
+        n = len(remain_lists)
+        if chunk is None:
+            per, free = self.drain_budget()
+            chunk = max(1, int(free * self.DRAIN_MEM_FRACTION) // max(per, 1))
+        out = []
+        for b in range(0, n, chunk):
+            part = remain_lists[b:b + chunk]
+            arr, keep = self._scenario_array(part)
+            res = (abi.SimonDrainResult * len(part))()
+            self._check(L.simon_wave_run(self.h, arr, len(part), res))
+            self._wave = (list(remain_lists), b, len(part))
+            su, pm, cm = C.c_float(0), C.c_float(0), C.c_float(0)
+            self._check(L.simon_wave_times(self.h, C.byref(su), C.byref(pm), C.byref(cm)))
+            self.last_wave["batches"] += 1
+            self.last_wave["setup_ms"] += float(su.value)
+            self.last_wave["place_ms"] += float(pm.value)
+            self.last_wave["launches"].append(self.last_launch())
+            out.extend(self._drain_results(res, None, detail))
+        return out
+
+    def wave_commit(self, i: int):
+        """simon_wave_commit of entry i of the last wave_run's remain_lists: it becomes the next base.  When entry i was not in the last
+        batch it is run again alone first."""
+        lists, b, m = self._wave if self._wave is not None else (None, 0, 0)
+        if lists is not None and not b <= i < b + m:
+            self.wave_run([lists[i]], detail=False, chunk=1)
+            self._wave = (lists, i, 1)
+            b = i
+        self._check(lib().simon_wave_commit(self.h, i - b))
+        self._wave = None
+        cm = C.c_float(0)
+        self._check(lib().simon_wave_times(self.h, None, None, C.byref(cm)))
+        self.last_wave["commits"] += 1
+        self.last_wave["commit_ms"] += float(cm.value)
+
+    def wave_placement(self):
+        """The wave base's placement: (node per pod, GPU slot word per pod)."""
+        P = self.c.pods_dims["n_pods"]
+        pl = np.zeros(max(P, 1), np.int32)
+        sl = np.zeros(max(P, 1), np.uint32)
+        self._check(lib().simon_wave_download(self.h, pl.ctypes.data, sl.ctypes.data))
+        return pl[:P], sl[:P]
 
     # ---- headroom probes (simon_probe_run) ----
     def probe_run(self, placed, probes, detail: bool = True, chunk: Optional[int] = None):

@@ -596,6 +596,33 @@ class Simulator:
                                          lambda rl: eng.drain_run(self.placements, rl, detail=False, local=local_volumes),
                                          candidates=cand, max_remove=max_remove)
 
+    def PlanRollingMaintenance(self, nodes: Optional[List[str]] = None, max_unavailable: int = 1, order: str = "utilisation"):
+        """rolling.RollingPlan on the session's live state: `nodes` (all nodes by default) taken out for maintenance in waves of at most
+        max_unavailable and brought back empty apart from their DaemonSet pods, each wave from the state the waves before it leave (the
+        pods they moved stay moved, with their GPU-share devices).  order "utilisation" (live utilisation ascending, ties in nodeTree
+        order) or "given" (as listed).  Each wave is the longest prefix of the remaining nodes whose every prefix drains within the
+        MaxCPU / MaxMemory caps and the PodDisruptionBudgets; a node that cannot go even alone is skipped with its reasons.  Pods with
+        Open-Local volumes block their node (local_volumes is not offered: their volumes would have to move and return with the
+        waves).  Runs on the session's device context; its placements and every later call's answers are unchanged."""
+        from . import rolling
+        eng, compiled = self._live()
+        cand = None
+        if nodes is not None:
+            cand = [compiled.node_index(nm) for nm in nodes]
+            bad = [nm for nm, g in zip(nodes, cand) if g < 0]
+            if bad:
+                raise ValueError(f"PlanRollingMaintenance: no node named {bad[0]!r}")
+        if max_unavailable < 1:
+            raise ValueError(f"PlanRollingMaintenance: max_unavailable must be at least 1 (got {max_unavailable})")
+        if order not in rolling.ORDERS:
+            raise ValueError(f"PlanRollingMaintenance: unknown order {order!r} (one of {', '.join(rolling.ORDERS)})")
+        try:
+            return rolling.plan_rolling(compiled, self.placements, rolling.EngineRunner(eng), cand, order, max_unavailable,
+                                        pdbs=self.pdb_tables)
+        finally:
+            # the context's single-scenario state holds the last wave base: the live state again, for the calls that read it
+            eng.schedule_resume(self.placements)
+
     def PlanMigrations(self, sources: Optional[List[str]] = None, targets: Optional[List[str]] = None, max_moves: int = 100,
                        min_gain: int = 1, move_scope: int = 0):
         """rebalance.MigrationPlan on the session's live state: the pods of the source nodes (all by default) as candidates onto the
