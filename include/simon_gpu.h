@@ -727,6 +727,52 @@ int simon_wave_download(simon_ctx *ctx, int32_t *placed, uint32_t *gpu_slots);
 /* Device time of the last wave batch (setup: copies into the slots and counter removal; placement) and of the last commit, ms. */
 int simon_wave_times(simon_ctx *ctx, float *setup_ms, float *place_ms, float *commit_ms);
 
+/* ---- node-pool replacement: surge waves in which new nodes join while old nodes drain and leave for good (this library's definition,
+ * built on the waves above) ------------------------------------------------------------------------------------------------------------
+ * The cluster is compiled as a superset: the live nodes plus copies of a new node spec that are not yet in the cluster, and the pod list
+ * followed by the copies' DaemonSet pods, pending (-1).  The wave base keeps, per node, whether it is present, absent (not yet joined)
+ * or retired (left for good).  simon_wave_begin is simon_wave_begin_pool with every node present.
+ *   simon_wave_begin_pool  the first base: simon_wave_begin's, with present[n_nodes] (non-zero: present).  SIMON_ERR_INVALID for a pod
+ *                          placed on a node that is not present.
+ *   simon_wave_run_join    a wave batch: scenario i joins the nodes join[i] (absent nodes, each listed in remain[i]) and drains the
+ *                          present nodes missing from remain[i] (the retire set D).  It works as simon_wave_run, with each scenario's
+ *                          pod list [join pods in pod order] + [evicted pods in pod order], placed by the drain kernels on remain[i]
+ *                          after D's pods are taken out; the join pods are the pods whose DaemonSet guard is a node of join[i], and they
+ *                          go through the full filter, score, select and Reserve path.  Equivalently: remain[i] compiled with the pod
+ *                          list [pods that stay, in order] + [join pods] + [evicted pods] and resumed after the first part gives the same
+ *                          nodes, GPU slots and failure histograms (on clusters without GPU share; with it, the wave keeps the devices
+ *                          the base gave).  out[i] counts the evicted pods only; out_join[i] counts the join pods.
+ *                          simon_drain_download, simon_drain_pdb_download and simon_drain_times serve the evicted and blocked pods as
+ *                          for simon_wave_run; simon_wave_join_download serves the join pods.  simon_wave_run refuses as below too.
+ *                          SIMON_ERR_INVALID, before any device work: a joining node out of range, listed twice, not absent or not in
+ *                          remain[i]; a node of remain[i] that is absent and not joining, or retired; a join pod of a class with
+ *                          Open-Local volumes or bound by spec.nodeName; simon_wave_run's refusals.
+ *   simon_wave_commit_retire  scenario `scenario` of the last wave batch becomes the next base: its slot's state is copied into the
+ *                          base; the evicted and join pods' nodes and GPU slot words are written into the base placement, on the
+ *                          device and in the mirror; the joined nodes become present and the drained nodes retired; every
+ *                          DaemonSet pod guarded by a drained node (placed there or pending) is written as -3 (does not exist) into
+ *                          the base placement, and the nodes' requests, non-zero requests, pod counts, scalars and GPU-share memory
+ *                          are reset to an empty node's (the reset of simon_wave_return, launched with no pod to add back: nothing
+ *                          returns).
+ *                          SIMON_ERR_INVALID as simon_wave_commit, and for a scenario with an unscheduled join pod.
+ * simon_wave_commit refuses (SIMON_ERR_INVALID) a scenario of a batch that joined nodes, with or without join pods.  The validity rules of the waves hold. */
+typedef struct simon_join_result {
+    uint32_t n_join;               /* join pods of the scenario */
+    uint32_t n_placed;             /* of them, placed */
+    uint32_t n_unscheduled;        /* of them, unschedulable */
+    uint32_t reserved;
+} simon_join_result;
+int simon_wave_begin_pool(simon_ctx *ctx, const int32_t *placed, const uint8_t *present);
+int simon_wave_run_join(simon_ctx *ctx, const simon_scenario *remain, const simon_scenario *join, uint32_t n, simon_drain_result *out,
+                        simon_join_result *out_join);
+/* Scenario `scenario` of the last simon_wave_run_join batch, each pointer may be NULL: its join pods in pod order [n_join], the node each
+ * landed on or -1, its GPU slot word, its winning score (as simon_drain_download), and the join pods' failure records [n_unscheduled]. */
+int simon_wave_join_download(simon_ctx *ctx, uint32_t scenario, uint32_t *join_pod, int32_t *node, uint32_t *gpu_slots, int64_t *score,
+                             uint32_t *fail_counts, uint32_t *fail_pod);
+int simon_wave_commit_retire(simon_ctx *ctx, uint32_t scenario);
+/* The current base's node states [n_nodes]: 0 absent, 1 present, 2 retired. */
+int simon_wave_presence(simon_ctx *ctx, uint8_t *state);
+
 /* ---- scheduling headroom (the reference's first use case, README.md:14 capacity planning, asked of the running cluster; it has no
  * code for it, so the definition is this library's) -------------------------------------------------------------------------------
  * The live state is placed[n_pods], checked as simon_drain_run checks it.  A probe (pod q, max_replicas R >= 1) asks how many more

@@ -368,6 +368,7 @@ struct simon_ctx {
     struct {
         uint32_t n = 0, max = 0;
         std::vector<uint32_t> off, pods, boff, blocked, nfail, voff, vpdb, vcnt;
+        std::vector<uint32_t> dpos;         // per drain: the device position of its first evicted pod (after a wave batch's join pods)
         DevBuf<uint32_t> d_pods, d_off, d_gpu, d_fail_counts, d_fail_pod;
         DevBuf<int32_t> d_node;
         DevBuf<int64_t> d_score;
@@ -397,11 +398,18 @@ struct simon_ctx {
     } grow;
     // the wave base (simon_wave_begin): the single-scenario pool's state and its per-pod results (out_node, out_gpu) are the base, and
     // place / slots their host mirror; of the last wave batch, each scenario's removed nodes (CSR roff / removed, index order) and
-    // vanished pods (CSR voff / vanished, pod order), which return with them; on the device the returned nodes and their pods (CSR) of the last commit, and its device time
+    // vanished pods (CSR voff / vanished, pod order), which return with them; on the device the returned nodes and their pods (CSR) of the last commit, and its device time.
+    // present: per node 0 absent, 1 present, 2 retired (simon_wave_begin_pool); of the last batch, each scenario's joined nodes (CSR
+    // jnoff / jnodes) and join pods (CSR joff / jpods, pod order, first in the scenario's device list at drain.d_off[i]) with their
+    // unscheduled count; joined: the last batch joined a node
     struct {
         std::vector<int32_t> place;
         std::vector<uint32_t> slots, voff, vanished, roff, removed;
-        DevBuf<uint32_t> d_nodes, d_off, d_pods;
+        std::vector<uint8_t> present;
+        std::vector<uint32_t> jnoff, jnodes, joff, jpods, jfail, dstart;
+        bool joined = false;
+        DevBuf<uint32_t> d_nodes, d_off, d_pods, d_vgpu;
+        DevBuf<int32_t> d_vnode;            // a retiring commit's vanished pods: -3 each (d_vgpu: slot word 0)
         float commit_ms = 0.f;
     } wave;
     // the last migration plan (simon_moves_plan): its end state in plan-owned copies of the single-scenario node state, placement and
@@ -1589,9 +1597,12 @@ static int live_batch_reduce(simon_ctx *ctx, uint32_t n, bool local, std::vector
 
 // simon_drain_run and simon_drain_run_local (out_local != nullptr: pods with Open-Local volumes are evicted, not blocked, and each
 // scenario carries its own Open-Local state, the live one to start with).  wave (simon_wave_run): the scenarios start from the wave
-// base, which `placed` mirrors, instead of a state rebuilt from `placed`, and each one's vanished pods are kept for a commit.
+// base, which `placed` mirrors, instead of a state rebuilt from `placed`, and each one's vanished pods are kept for a commit.  join
+// (simon_wave_run_join): scenario i also joins the nodes join[i]; their DaemonSet pods come first in its device list, and out_join
+// counts them.
 static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario *remain, uint32_t n, simon_drain_result *out,
-                     simon_scenario_local_result *out_local, bool wave = false) {
+                     simon_scenario_local_result *out_local, bool wave = false, const simon_scenario *join = nullptr,
+                     simon_join_result *out_join = nullptr) {
     const bool local = out_local != nullptr;
     const char *what = wave ? "simon_wave_run" : local ? "simon_drain_run_local" : "simon_drain_run";
     if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "%s before uploads", what);
@@ -1606,6 +1617,60 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
     uint32_t max_active = 0;
     rc = scenario_lists(ctx, remain, n, "drain", max_active);
     if (rc) return rc;
+    // ---- a wave: the nodes each scenario joins and the node states of the base, then the join pods (the pods whose DaemonSet guard
+    // joins, pod order) ----
+    ctx->wave.jnoff.assign(1, 0u); ctx->wave.jnodes.clear(); ctx->wave.joff.assign(1, 0u); ctx->wave.jpods.clear();
+    if (wave) {
+        const std::vector<uint8_t> &pr = ctx->wave.present;
+        std::vector<uint8_t> joining(N1, 0u);
+        std::vector<uint32_t> goff, gpods;          // the pods of each DaemonSet guard node (CSR, pod order), built at the first join
+        for (uint32_t i = 0; i < n; i++) {
+            const int32_t *rank = ctx->batch.h_rank.data() + (size_t)i * N1;
+            const uint32_t nj = join ? join[i].n_nodes : 0u, j0 = (uint32_t)ctx->wave.jnodes.size();
+            if (nj && !join[i].nodes) return fail(ctx, SIMON_ERR_INVALID, "wave %u: join nodes is NULL", i);
+            for (uint32_t k = 0; k < nj; k++) {
+                const uint32_t g = join[i].nodes[k];
+                if (g >= N) return fail(ctx, SIMON_ERR_INVALID, "wave %u joins node %u, out of range", i, g);
+                if (joining[g]) return fail(ctx, SIMON_ERR_INVALID, "wave %u joins node %u twice", i, g);
+                if (pr[g] != 0) return fail(ctx, SIMON_ERR_INVALID, "wave %u joins node %u, which is not absent", i, g);
+                if (rank[g] < 0) return fail(ctx, SIMON_ERR_INVALID, "wave %u joins node %u, which is not in its remaining nodes", i, g);
+                joining[g] = 1;
+                ctx->wave.jnodes.push_back(g);
+            }
+            for (uint32_t g = 0; g < N; g++)
+                if (rank[g] >= 0 && !joining[g] && pr[g] != 1)
+                    return fail(ctx, SIMON_ERR_INVALID, pr[g] == 2 ? "wave %u keeps node %u, which is retired"
+                                                                   : "wave %u keeps node %u, which is absent and does not join", i, g);
+            const size_t p0 = ctx->wave.jpods.size();
+            if (nj && goff.empty()) {
+                goff.assign(N1 + 1, 0u);
+                for (uint32_t q = 0; q < P; q++)
+                    if (ctx->pods.h_guard[q] >= 0) goff[ctx->pods.h_guard[q] + 1]++;
+                for (uint32_t g = 0; g < N1; g++) goff[g + 1] += goff[g];
+                gpods.resize(goff[N1]);
+                std::vector<uint32_t> cur(goff.begin(), goff.end() - 1);
+                for (uint32_t q = 0; q < P; q++)
+                    if (ctx->pods.h_guard[q] >= 0) gpods[cur[ctx->pods.h_guard[q]]++] = q;
+            }
+            for (uint32_t k = j0; k < ctx->wave.jnodes.size(); k++) {
+                const uint32_t g = ctx->wave.jnodes[k];
+                joining[g] = 0;
+                ctx->wave.jpods.insert(ctx->wave.jpods.end(), gpods.begin() + goff[g], gpods.begin() + goff[g + 1]);
+            }
+            std::sort(ctx->wave.jpods.begin() + p0, ctx->wave.jpods.end());
+            for (size_t k = p0; k < ctx->wave.jpods.size(); k++) {
+                const uint32_t q = ctx->wave.jpods[k];
+                if (ctx->pods.h_fixed[q] >= 0)
+                    return fail(ctx, SIMON_ERR_INVALID, "wave %u: join pod %u is bound by spec.nodeName", i, q);
+                if (ctx->valid.has(STORAGE) && ctx->storage.h_class_local[ctx->pods.h_class[q]])
+                    return fail(ctx, SIMON_ERR_INVALID, "wave %u: join pod %u has Open-Local volumes", i, q);
+            }
+            ctx->wave.jnoff.push_back((uint32_t)ctx->wave.jnodes.size());
+            ctx->wave.joff.push_back((uint32_t)ctx->wave.jpods.size());
+        }
+    } else {
+        ctx->wave.jnoff.assign(n + 1, 0u); ctx->wave.joff.assign(n + 1, 0u);
+    }
     CU(cudaSetDevice(ctx->device));
     ctx->last_launch = simon_launch_info{};
     // the batch pool is no longer a probe or grow batch's, nor are its Open-Local slices a storage batch's
@@ -1654,9 +1719,20 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
         ctx->drain.off.push_back((uint32_t)ctx->drain.pods.size());
         ctx->drain.boff.push_back((uint32_t)ctx->drain.blocked.size());
         ctx->wave.voff.push_back((uint32_t)ctx->wave.vanished.size());
-        ctx->drain.max = std::max(ctx->drain.max, ctx->drain.off[i + 1] - ctx->drain.off[i]);
     }
-    const size_t n_ev = ctx->drain.pods.size();
+    // ---- the device lists: per scenario its join pods, then its evicted pods; the failure records are sized for both ----
+    ctx->wave.joined = !ctx->wave.jnodes.empty();
+    std::vector<uint32_t> dlist, doff(1, 0u);
+    ctx->drain.dpos.resize(n);
+    for (uint32_t i = 0; i < n; i++) {
+        dlist.insert(dlist.end(), ctx->wave.jpods.begin() + ctx->wave.joff[i], ctx->wave.jpods.begin() + ctx->wave.joff[i + 1]);
+        ctx->drain.dpos[i] = (uint32_t)dlist.size();
+        dlist.insert(dlist.end(), ctx->drain.pods.begin() + ctx->drain.off[i], ctx->drain.pods.begin() + ctx->drain.off[i + 1]);
+        doff.push_back((uint32_t)dlist.size());
+        ctx->drain.max = std::max(ctx->drain.max, doff[i + 1] - doff[i]);
+    }
+    ctx->wave.dstart.assign(doff.begin(), doff.end());
+    const size_t n_ev = dlist.size();
     // ---- geometry of the drain variant, the batch pool and the outputs (allocations before the timed work) ----
     uint32_t CS, TPB, NPT;
     size_t smem;
@@ -1665,8 +1741,8 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
     if (rc) return rc;
     rc = size_pool(ctx, B, n, false, false);
     if (rc) return rc;
-    CU(ctx->drain.d_pods.upload(ctx->drain.pods.data(), n_ev, st));
-    CU(ctx->drain.d_off.upload(ctx->drain.off.data(), n + 1, st));
+    CU(ctx->drain.d_pods.upload(dlist.data(), n_ev, st));
+    CU(ctx->drain.d_off.upload(doff.data(), n + 1, st));
     CU(ctx->drain.d_pairs.upload(pairs.data(), pairs.size(), st));
     CU(ctx->drain.d_node.alloc(n_ev)); CU(ctx->drain.d_gpu.alloc(n_ev));
     if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(ctx->drain.d_score.alloc(n_ev));
@@ -1715,6 +1791,9 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
         CU(pdb_allowed(ctx, S.out_node.p));
         CU(cudaMemcpyAsync(allowed.data(), ctx->pdb.d_rem.p, 4ull * J, cudaMemcpyDeviceToHost, st));
     }
+    // a batch that joins: the join pods' nodes, to count them apart from the evicted pods
+    std::vector<int32_t> jnode(ctx->wave.joined ? n_ev : 0u);
+    if (ctx->wave.joined) CU(cudaMemcpyAsync(jnode.data(), ctx->drain.d_node.p, 4ull * n_ev, cudaMemcpyDeviceToHost, st));
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
     if (!wave) ctx->valid.set(LIVE);
@@ -1742,7 +1821,13 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
         if (!J) ctx->drain.voff.assign(n + 1, 0u);
     }
     ctx->drain.nfail.resize(n);
+    ctx->wave.jfail.assign(n, 0u);
     for (uint32_t i = 0; i < n; i++) {
+        const uint32_t nj = ctx->wave.joff[i + 1] - ctx->wave.joff[i];
+        for (uint32_t k = doff[i]; k < ctx->drain.dpos[i]; k++) ctx->wave.jfail[i] += jnode[k] < 0;
+        if (out_join) out_join[i] = simon_join_result{nj, nj - ctx->wave.jfail[i], ctx->wave.jfail[i], 0u};
+        res[i].n_scheduled -= nj - ctx->wave.jfail[i];
+        res[i].n_unscheduled -= ctx->wave.jfail[i];
         simon_drain_result &o = out[i];
         o.n_evicted = ctx->drain.off[i + 1] - ctx->drain.off[i];
         o.n_placed = res[i].n_scheduled; o.n_unscheduled = res[i].n_unscheduled;
@@ -1786,10 +1871,11 @@ extern "C" int simon_drain_download(simon_ctx *ctx, uint32_t scenario, uint32_t 
     if (!ctx->valid.has(DRAIN_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_drain_run batch since the last upload, or a probe batch after it");
     if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "drain %u of a batch of %u", scenario, ctx->drain.n);
     CU(cudaSetDevice(ctx->device));
-    const uint32_t b = ctx->drain.off[scenario], ne = ctx->drain.off[scenario + 1] - b;
+    // on the device the scenario's evicted pods start at dpos, and their failure records follow those of its join pods
+    const uint32_t h = ctx->drain.off[scenario], ne = ctx->drain.off[scenario + 1] - h, b = ctx->drain.dpos[scenario];
     const uint32_t bb = ctx->drain.boff[scenario], nb = ctx->drain.boff[scenario + 1] - bb;
-    const uint32_t nf = std::min(ctx->drain.nfail[scenario], ctx->drain.max);
-    if (evicted_pod) std::copy(ctx->drain.pods.begin() + b, ctx->drain.pods.begin() + b + ne, evicted_pod);
+    const uint32_t fr = ctx->wave.jfail[scenario], nf = std::min(ctx->drain.nfail[scenario], ctx->drain.max - std::min(fr, ctx->drain.max));
+    if (evicted_pod) std::copy(ctx->drain.pods.begin() + h, ctx->drain.pods.begin() + h + ne, evicted_pod);
     if (blocked_pod) std::copy(ctx->drain.blocked.begin() + bb, ctx->drain.blocked.begin() + bb + nb, blocked_pod);
     if (node && ne) CU(cudaMemcpy(node, ctx->drain.d_node.p + b, 4ull * ne, cudaMemcpyDeviceToHost));
     if (gpu_slots && ne) CU(cudaMemcpy(gpu_slots, ctx->drain.d_gpu.p + b, 4ull * ne, cudaMemcpyDeviceToHost));
@@ -1798,9 +1884,10 @@ extern "C" int simon_drain_download(simon_ctx *ctx, uint32_t scenario, uint32_t 
         else memset(score, 0, 8ull * ne);
     }
     if (fail_counts && nf)
-        CU(cudaMemcpy(fail_counts, ctx->drain.d_fail_counts.p + (size_t)scenario * ctx->drain.max * SIMON_N_FAIL_CODES,
+        CU(cudaMemcpy(fail_counts, ctx->drain.d_fail_counts.p + ((size_t)scenario * ctx->drain.max + fr) * SIMON_N_FAIL_CODES,
                       4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
-    if (fail_pod && nf) CU(cudaMemcpy(fail_pod, ctx->drain.d_fail_pod.p + (size_t)scenario * ctx->drain.max, 4ull * nf, cudaMemcpyDeviceToHost));
+    if (fail_pod && nf)
+        CU(cudaMemcpy(fail_pod, ctx->drain.d_fail_pod.p + (size_t)scenario * ctx->drain.max + fr, 4ull * nf, cudaMemcpyDeviceToHost));
     return SIMON_OK;
 }
 
@@ -1815,13 +1902,20 @@ extern "C" int simon_drain_pdb_download(simon_ctx *ctx, uint32_t scenario, uint3
 }
 
 // ---- rolling maintenance waves ------------------------------------------------------------------------------------------------
-extern "C" int simon_wave_begin(simon_ctx *ctx, const int32_t *placed) {
-    if (!ctx) return SIMON_ERR_INVALID;
+// simon_wave_begin (present == nullptr: every node present) and simon_wave_begin_pool
+static int wave_begin(simon_ctx *ctx, const int32_t *placed, const uint8_t *present) {
     if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_begin before uploads");
-    const uint32_t P = ctx->pods.n_pods;
+    const uint32_t P = ctx->pods.n_pods, N = ctx->snap.N;
     if (P && !placed) return fail(ctx, SIMON_ERR_INVALID, "simon_wave_begin: NULL argument");
     int rc = check_prefix(ctx, placed, P);
     if (rc) return rc;
+    std::vector<uint8_t> pr(N, 1u);
+    if (present) {
+        for (uint32_t g = 0; g < N; g++) pr[g] = present[g] ? 1u : 0u;
+        for (uint32_t q = 0; q < P; q++)
+            if (placed[q] >= 0 && !pr[placed[q]])
+                return fail(ctx, SIMON_ERR_INVALID, "simon_wave_begin_pool: pod %u is placed on node %d, which is not present", q, placed[q]);
+    }
     CU(cudaSetDevice(ctx->device));
     ScenPool &S = ctx->single;
     cudaStream_t st = ctx->stream;
@@ -1833,6 +1927,7 @@ extern "C" int simon_wave_begin(simon_ctx *ctx, const int32_t *placed) {
     rc = rebuild_prefix(ctx, Ps, placed, P);
     if (rc) return rc;
     ctx->wave.place.assign(placed, placed + P);
+    ctx->wave.present.swap(pr);
     ctx->wave.slots.assign(P, 0u);
     if (P) CU(cudaMemcpyAsync(ctx->wave.slots.data(), S.out_gpu.p, 4ull * P, cudaMemcpyDeviceToHost, st));
     const cudaError_t e = cudaStreamSynchronize(st);
@@ -1840,6 +1935,25 @@ extern "C" int simon_wave_begin(simon_ctx *ctx, const int32_t *placed) {
     ctx->valid.drop(LIVE);
     ctx->valid.set(WAVE_BASE);
     return SIMON_OK;
+}
+
+extern "C" int simon_wave_begin(simon_ctx *ctx, const int32_t *placed) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    return wave_begin(ctx, placed, nullptr);
+}
+
+extern "C" int simon_wave_begin_pool(simon_ctx *ctx, const int32_t *placed, const uint8_t *present) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (ctx->snap.N && !present) return fail(ctx, SIMON_ERR_INVALID, "simon_wave_begin_pool: NULL argument");
+    return wave_begin(ctx, placed, present);
+}
+
+extern "C" int simon_wave_run_join(simon_ctx *ctx, const simon_scenario *remain, const simon_scenario *join, uint32_t n, simon_drain_result *out,
+                                   simon_join_result *out_join) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(WAVE_BASE)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_run_join without a wave base (simon_wave_begin)");
+    if (n && (!join || !out_join)) return fail(ctx, SIMON_ERR_INVALID, "simon_wave_run_join: NULL argument");
+    return drain_run(ctx, ctx->wave.place.data(), remain, n, out, nullptr, true, join, out_join);
 }
 
 extern "C" int simon_wave_run(simon_ctx *ctx, const simon_scenario *remain, uint32_t n, simon_drain_result *out) {
@@ -1853,6 +1967,7 @@ extern "C" int simon_wave_commit(simon_ctx *ctx, uint32_t scenario) {
     if (!ctx->valid.has(WAVE_BASE)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_commit without a wave base (simon_wave_begin)");
     if (!ctx->valid.has(WAVE_BATCH)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_commit: no simon_wave_run batch since the base changed");
     if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u of a batch of %u", scenario, ctx->drain.n);
+    if (ctx->wave.joined) return fail(ctx, SIMON_ERR_INVALID, "simon_wave_commit: the last wave batch joined nodes (simon_wave_commit_retire)");
     const uint32_t s = scenario;
     if (ctx->drain.nfail[s]) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u leaves %u evicted pods unscheduled", s, ctx->drain.nfail[s]);
     if (ctx->drain.boff[s + 1] > ctx->drain.boff[s])
@@ -1913,6 +2028,115 @@ extern "C" int simon_wave_commit(simon_ctx *ctx, uint32_t scenario) {
     for (uint32_t i = 0; i < ne; i++) ctx->wave.place[ctx->drain.pods[b + i]] = node[i];
     // the batch's slots describe the old base: no other scenario of it may be committed
     ctx->valid.drop(WAVE_BATCH);
+    return SIMON_OK;
+}
+
+extern "C" int simon_wave_commit_retire(simon_ctx *ctx, uint32_t scenario) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(WAVE_BASE)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_commit_retire without a wave base (simon_wave_begin)");
+    if (!ctx->valid.has(WAVE_BATCH)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_commit_retire: no wave batch since the base changed");
+    if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u of a batch of %u", scenario, ctx->drain.n);
+    const uint32_t s = scenario;
+    if (ctx->drain.nfail[s]) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u leaves %u evicted pods unscheduled", s, ctx->drain.nfail[s]);
+    if (ctx->wave.jfail[s]) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u leaves %u join pods unscheduled", s, ctx->wave.jfail[s]);
+    if (ctx->drain.boff[s + 1] > ctx->drain.boff[s])
+        return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u has %u blocked pods", s, ctx->drain.boff[s + 1] - ctx->drain.boff[s]);
+    if (ctx->drain.voff[s + 1] > ctx->drain.voff[s])
+        return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u violates %u PDBs", s, ctx->drain.voff[s + 1] - ctx->drain.voff[s]);
+    CU(cudaSetDevice(ctx->device));
+    ScenPool &S = ctx->single, &B = ctx->batch;
+    cudaStream_t st = ctx->stream;
+    // ---- on the host: the scenario's device list (join pods, then evicted pods) and their nodes; the retired nodes (the present nodes
+    // it removed) and their DaemonSet pods (its vanished pods), which stop existing ----
+    const uint32_t b = ctx->wave.dstart[s], nl = ctx->wave.dstart[s + 1] - b;
+    std::vector<uint32_t> list(nl);
+    std::vector<int32_t> node(nl);
+    if (nl) {
+        CU(cudaMemcpy(list.data(), ctx->drain.d_pods.p + b, 4ull * nl, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(node.data(), ctx->drain.d_node.p + b, 4ull * nl, cudaMemcpyDeviceToHost));
+    }
+    std::vector<uint32_t> gone;
+    for (uint32_t k = ctx->wave.roff[s]; k < ctx->wave.roff[s + 1]; k++)
+        if (ctx->wave.present[ctx->wave.removed[k]] == 1) gone.push_back(ctx->wave.removed[k]);
+    std::vector<uint32_t> van(ctx->wave.vanished.begin() + ctx->wave.voff[s], ctx->wave.vanished.begin() + ctx->wave.voff[s + 1]);
+    {
+        // the retired nodes' DaemonSet pods that were pending in the base stop existing too
+        std::vector<uint8_t> retiring(std::max(1u, ctx->snap.N), 0u);
+        for (uint32_t g : gone) retiring[g] = 1;
+        for (uint32_t q = 0; q < ctx->pods.n_pods; q++)
+            if (ctx->pods.h_guard[q] >= 0 && retiring[ctx->pods.h_guard[q]] && ctx->wave.place[q] == -1) van.push_back(q);
+    }
+    std::vector<int32_t> van_node(van.size(), -3);
+    std::vector<uint32_t> van_gpu(van.size(), 0u), off(gone.size() + 1, 0u);
+    // ---- on the device, timed: the slot's state into the base, the scatter of the placed pods and of the pods that stop existing, the
+    // retired nodes reset to empty.  The reset reuses simon_wave_return with no pods to add back: its first part is exactly the reset,
+    // and nothing returns ----
+    CU(ctx->wave.d_nodes.upload(gone.data(), gone.size(), st));
+    CU(ctx->wave.d_off.upload(off.data(), off.size(), st));
+    CU(ctx->wave.d_pods.upload(van.data(), van.size(), st));
+    CU(ctx->wave.d_vnode.upload(van_node.data(), van_node.size(), st));
+    CU(ctx->wave.d_vgpu.upload(van_gpu.data(), van_gpu.size(), st));
+    CU(cudaEventRecord(ctx->ev0, st));
+    CU(S.state.each(B.state, true, [&](auto &d, auto &c, uint64_t k) {
+        return cudaMemcpyAsync(d.p, c.p + (size_t)s * k, k * sizeof(*d.p), cudaMemcpyDeviceToDevice, st);
+    }));
+    auto scatter = [&](const uint32_t *pods, const int32_t *nd, const uint32_t *gpu, uint32_t cnt) -> cudaError_t {
+        if (!cnt) return cudaSuccess;
+        const uint32_t grid = std::min<uint32_t>((cnt + 255) / 256, (uint32_t)ctx->sms * 4);
+        simon_wave_scatter<<<grid, 256, 0, st>>>(pods, nd, gpu, cnt, S.out_node.p, S.out_gpu.p);
+        ctx->launches++;
+        return cudaGetLastError();
+    };
+    CU(scatter(ctx->drain.d_pods.p + b, ctx->drain.d_node.p + b, ctx->drain.d_gpu.p + b, nl));
+    CU(scatter(ctx->wave.d_pods.p, ctx->wave.d_vnode.p, ctx->wave.d_vgpu.p, (uint32_t)van.size()));
+    if (!gone.empty()) {
+        SkParams Ps;
+        fill_params(ctx, S, Ps);
+        simon_wave_return<<<((uint32_t)gone.size() + 127) / 128, 128, 0, st>>>(Ps, ctx->wave.d_nodes.p, ctx->wave.d_off.p, ctx->wave.d_pods.p,
+                                                                                (uint32_t)gone.size());
+        CU(cudaGetLastError());
+        ctx->launches++;
+    }
+    CU(cudaEventRecord(ctx->ev1, st));
+    if (ctx->pods.n_pods) CU(cudaMemcpyAsync(ctx->wave.slots.data(), S.out_gpu.p, 4ull * ctx->pods.n_pods, cudaMemcpyDeviceToHost, st));
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    CU(cudaEventElapsedTime(&ctx->wave.commit_ms, ctx->ev0, ctx->ev1));
+    ctx->last_ms = ctx->wave.commit_ms;
+    for (uint32_t k = 0; k < nl; k++) ctx->wave.place[list[k]] = node[k];
+    for (uint32_t q : van) ctx->wave.place[q] = -3;
+    for (uint32_t k = ctx->wave.jnoff[s]; k < ctx->wave.jnoff[s + 1]; k++) ctx->wave.present[ctx->wave.jnodes[k]] = 1;
+    for (uint32_t g : gone) ctx->wave.present[g] = 2;
+    ctx->valid.drop(WAVE_BATCH);
+    return SIMON_OK;
+}
+
+extern "C" int simon_wave_join_download(simon_ctx *ctx, uint32_t scenario, uint32_t *join_pod, int32_t *node, uint32_t *gpu_slots, int64_t *score,
+                                        uint32_t *fail_counts, uint32_t *fail_pod) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(WAVE_BATCH)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_join_download: no wave batch since the base changed");
+    if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u of a batch of %u", scenario, ctx->drain.n);
+    CU(cudaSetDevice(ctx->device));
+    const uint32_t h = ctx->wave.joff[scenario], nj = ctx->wave.joff[scenario + 1] - h, b = ctx->wave.dstart[scenario];
+    const uint32_t nf = std::min(ctx->wave.jfail[scenario], ctx->drain.max);
+    if (join_pod) std::copy(ctx->wave.jpods.begin() + h, ctx->wave.jpods.begin() + h + nj, join_pod);
+    if (node && nj) CU(cudaMemcpy(node, ctx->drain.d_node.p + b, 4ull * nj, cudaMemcpyDeviceToHost));
+    if (gpu_slots && nj) CU(cudaMemcpy(gpu_slots, ctx->drain.d_gpu.p + b, 4ull * nj, cudaMemcpyDeviceToHost));
+    if (score && nj) {
+        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(cudaMemcpy(score, ctx->drain.d_score.p + b, 8ull * nj, cudaMemcpyDeviceToHost));
+        else memset(score, 0, 8ull * nj);
+    }
+    if (fail_counts && nf)
+        CU(cudaMemcpy(fail_counts, ctx->drain.d_fail_counts.p + (size_t)scenario * ctx->drain.max * SIMON_N_FAIL_CODES,
+                      4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
+    if (fail_pod && nf) CU(cudaMemcpy(fail_pod, ctx->drain.d_fail_pod.p + (size_t)scenario * ctx->drain.max, 4ull * nf, cudaMemcpyDeviceToHost));
+    return SIMON_OK;
+}
+
+extern "C" int simon_wave_presence(simon_ctx *ctx, uint8_t *state) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(WAVE_BASE)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_presence without a wave base (simon_wave_begin)");
+    if (state) std::copy(ctx->wave.present.begin(), ctx->wave.present.end(), state);
     return SIMON_OK;
 }
 

@@ -115,6 +115,10 @@ class SimonDrainResult(C.Structure):
                 ("req_mcpu", C.c_int64), ("alloc_mcpu", C.c_int64), ("req_mem", C.c_int64), ("alloc_mem", C.c_int64)]
 
 
+class SimonJoinResult(C.Structure):
+    _fields_ = [("n_join", C.c_uint32), ("n_placed", C.c_uint32), ("n_unscheduled", C.c_uint32), ("reserved", C.c_uint32)]
+
+
 class SimonScenarioLocalResult(C.Structure):
     _fields_ = [("vg_requested", C.c_int64), ("vg_capacity", C.c_int64), ("reserved", C.c_uint64)]
 
@@ -293,6 +297,11 @@ SIGNATURES = {
     "simon_wave_commit": (_I, [_P, _U32]),
     "simon_wave_download": (_I, [_P, _P, _P]),
     "simon_wave_times": (_I, [_P, _PF, _PF, _PF]),
+    "simon_wave_begin_pool": (_I, [_P, _P, _P]),
+    "simon_wave_run_join": (_I, [_P, _P, _P, _U32, _P, _P]),
+    "simon_wave_join_download": (_I, [_P, _U32] + [_P] * 6),
+    "simon_wave_commit_retire": (_I, [_P, _U32]),
+    "simon_wave_presence": (_I, [_P, _P]),
     "simon_probe_run": (_I, [_P, _P, _P, _U32, _P, _P]),
     "simon_probe_download": (_I, [_P, _U32, _P, _P, _P, _P]),
     "simon_probe_times": (_I, [_P, _PF, _PF]),

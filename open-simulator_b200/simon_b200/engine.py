@@ -467,16 +467,26 @@ class Engine:
         return out
 
     # ---- rolling maintenance waves (simon_wave_*) ----
-    def wave_begin(self, placed):
-        """simon_wave_begin: the wave base is the live state `placed` (out_node of a full placement of the pod list) leaves."""
+    def wave_begin(self, placed, present=None):
+        """simon_wave_begin: the wave base is the live state `placed` (out_node of a full placement of the pod list) leaves.
+        present (bool per node): simon_wave_begin_pool, the nodes that are in the cluster; the others are absent until a wave joins
+        them."""
         pl = np.ascontiguousarray(placed, dtype=np.int32)
-        self._check(lib().simon_wave_begin(self.h, pl.ctypes.data))
+        if present is None:
+            self._check(lib().simon_wave_begin(self.h, pl.ctypes.data))
+        else:
+            pr = np.ascontiguousarray(np.asarray(present, dtype=bool).astype(np.uint8))
+            self._check(lib().simon_wave_begin_pool(self.h, pl.ctypes.data, pr.ctypes.data if pr.size else None))
         self._wave = None
         self.last_wave = dict(batches=0, setup_ms=0.0, place_ms=0.0, commits=0, commit_ms=0.0, launches=[])
 
-    def wave_run(self, remain_lists: List[np.ndarray], detail: bool = True, chunk: Optional[int] = None) -> List[dict]:
+    def wave_run(self, remain_lists: List[np.ndarray], joins: Optional[List[np.ndarray]] = None, detail: bool = True,
+                 chunk: Optional[int] = None) -> List[dict]:
         """Drains from the wave base, one dict per entry of remain_lists as drain_run returns them; in batches sized as drain_run
-        sizes them (chunk: an explicit batch size).  self.last_wave sums the device times of every batch and commit since wave_begin."""
+        sizes them (chunk: an explicit batch size).  self.last_wave sums the device times of every batch and commit since wave_begin.
+        joins (simon_wave_run_join): entry i also joins the absent nodes joins[i]; each dict then also carries n_join,
+        n_join_placed, n_join_unscheduled and, with detail, join_pods, join_node, join_gpu_slots, join_score, join_fail_counts and
+        join_fail_pod."""
         L = lib()
         n = len(remain_lists)
         if chunk is None:
@@ -487,26 +497,52 @@ class Engine:
             part = remain_lists[b:b + chunk]
             arr, keep = self._scenario_array(part)
             res = (abi.SimonDrainResult * len(part))()
-            self._check(L.simon_wave_run(self.h, arr, len(part), res))
-            self._wave = (list(remain_lists), b, len(part))
+            if joins is None:
+                self._check(L.simon_wave_run(self.h, arr, len(part), res))
+            else:
+                jarr, jkeep = self._scenario_array(joins[b:b + chunk])
+                jres = (abi.SimonJoinResult * len(part))()
+                self._check(L.simon_wave_run_join(self.h, arr, jarr, len(part), res, jres))
+            self._wave = (list(remain_lists), None if joins is None else list(joins), b, len(part))
             su, pm, cm = C.c_float(0), C.c_float(0), C.c_float(0)
             self._check(L.simon_wave_times(self.h, C.byref(su), C.byref(pm), C.byref(cm)))
             self.last_wave["batches"] += 1
             self.last_wave["setup_ms"] += float(su.value)
             self.last_wave["place_ms"] += float(pm.value)
             self.last_wave["launches"].append(self.last_launch())
-            out.extend(self._drain_results(res, None, detail))
+            part_out = self._drain_results(res, None, detail)
+            if joins is not None:
+                for i, (d, r) in enumerate(zip(part_out, jres)):
+                    d.update(n_join=r.n_join, n_join_placed=r.n_placed, n_join_unscheduled=r.n_unscheduled)
+                    if detail:
+                        d.update(self._join_detail(i, r))
+            out.extend(part_out)
         return out
 
-    def wave_commit(self, i: int):
+    def _join_detail(self, i: int, r) -> dict:
+        """simon_wave_join_download of scenario i of the last wave batch, whose join counts are r."""
+        nj, nf = r.n_join, r.n_unscheduled
+        jp = np.zeros(max(nj, 1), np.uint32)
+        node = np.zeros(max(nj, 1), np.int32)
+        slots = np.zeros(max(nj, 1), np.uint32)
+        score = np.zeros(max(nj, 1), np.int64)
+        fc = np.zeros((max(nf, 1), abi.N_FAIL_CODES), np.uint32)
+        fp = np.zeros(max(nf, 1), np.uint32)
+        self._check(lib().simon_wave_join_download(self.h, i, jp.ctypes.data, node.ctypes.data, slots.ctypes.data, score.ctypes.data,
+                                                   fc.ctypes.data, fp.ctypes.data))
+        return dict(join_pods=jp[:nj], join_node=node[:nj], join_gpu_slots=slots[:nj], join_score=score[:nj], join_fail_counts=fc[:nf],
+                    join_fail_pod=fp[:nf])
+
+    def wave_commit(self, i: int, retire: bool = False):
         """simon_wave_commit of entry i of the last wave_run's remain_lists: it becomes the next base.  When entry i was not in the last
-        batch it is run again alone first."""
-        lists, b, m = self._wave if self._wave is not None else (None, 0, 0)
+        batch it is run again alone first.  retire (simon_wave_commit_retire): its joined nodes become present and its drained nodes
+        leave for good instead of returning."""
+        lists, joins, b, m = self._wave if self._wave is not None else (None, None, 0, 0)
         if lists is not None and not b <= i < b + m:
-            self.wave_run([lists[i]], detail=False, chunk=1)
-            self._wave = (lists, i, 1)
+            self.wave_run([lists[i]], joins=None if joins is None else [joins[i]], detail=False, chunk=1)
+            self._wave = (lists, joins, i, 1)
             b = i
-        self._check(lib().simon_wave_commit(self.h, i - b))
+        self._check((lib().simon_wave_commit_retire if retire else lib().simon_wave_commit)(self.h, i - b))
         self._wave = None
         cm = C.c_float(0)
         self._check(lib().simon_wave_times(self.h, None, None, C.byref(cm)))
@@ -520,6 +556,13 @@ class Engine:
         sl = np.zeros(max(P, 1), np.uint32)
         self._check(lib().simon_wave_download(self.h, pl.ctypes.data, sl.ctypes.data))
         return pl[:P], sl[:P]
+
+    def wave_presence(self) -> np.ndarray:
+        """The wave base's node states: 0 absent, 1 present, 2 retired."""
+        N = self.c.n_nodes
+        st = np.zeros(max(N, 1), np.uint8)
+        self._check(lib().simon_wave_presence(self.h, st.ctypes.data))
+        return st[:N]
 
     # ---- headroom probes (simon_probe_run) ----
     def probe_run(self, placed, probes, detail: bool = True, chunk: Optional[int] = None):

@@ -14,8 +14,10 @@ candidate is skipped with its drain result and not retried.  The plan ends when 
 move (pinned_pods: bound by spec.nodeName, or with Open-Local volumes) fails every drain: it is skipped without a device run, and the
 prefixes past it are not evaluated, which changes no wave.
 
+run_waves is that loop, shared with node-pool replacement (replace.py), whose waves also join new nodes and retire the drained ones.
+
 Left out: pods with Open-Local volumes moving in waves (they block, and the base's VG and device state is never changed), surge
-nodes, retrying skipped nodes, pending pods of the live state (they stay pending and are not retried), sharding over several GPUs,
+nodes (see replace.py), retrying skipped nodes, pending pods of the live state (they stay pending and are not retried), sharding over several GPUs,
 the native host side and a command line.
 """
 from __future__ import annotations
@@ -35,10 +37,12 @@ LAST_NODE_REASON = "no other node would remain"
 
 @dataclass
 class Wave:
-    Nodes: List[str]                                          # taken out together, back at the end of the wave
+    Nodes: List[str]                                          # taken out together, back at the end of the wave (retired: gone for good)
     Evicted: List[scaledown.EvictedPod] = field(default_factory=list)
     PdbEvicted: Dict[str, int] = field(default_factory=dict)  # PDB "namespace/name" -> members the wave evicts
     Occupancy: Dict[str, int] = field(default_factory=dict)   # req_mcpu / alloc_mcpu / req_mem / alloc_mem over the remaining nodes
+    Joined: List[str] = field(default_factory=list)           # node-pool replacement: the new nodes that join first
+    JoinPods: list = field(default_factory=list)              # their DaemonSet pods (grow.NewPod), with their nodes and gpu-index
 
 
 @dataclass
@@ -60,17 +64,18 @@ class RollingPlan:
 
 
 class WaveRunner:
-    """What plan_rolling drives.  begin(placed) makes the first base; run(remain_lists) drains each entry from the base and returns
-    Engine.drain_run(detail=True) dicts; commit(i) makes entry i of the last run the base; placement() -> (node per pod, GPU slot word
-    per pod) of the base."""
+    """What run_waves drives.  begin(placed, present) makes the first base (present: None, or the nodes in the cluster);
+    run(remain_lists, joins) drains each entry from the base, joining the nodes joins[i] first (joins None: no join), and returns
+    Engine.wave_run(detail=True) dicts; commit(i, retire) makes entry i of the last run the base; placement() -> (node per pod, GPU slot
+    word per pod) of the base."""
 
-    def begin(self, placed):
+    def begin(self, placed, present=None):
         raise NotImplementedError
 
-    def run(self, remain_lists):
+    def run(self, remain_lists, joins=None):
         raise NotImplementedError
 
-    def commit(self, i: int):
+    def commit(self, i: int, retire: bool = False):
         raise NotImplementedError
 
     def placement(self):
@@ -83,14 +88,14 @@ class EngineRunner(WaveRunner):
     def __init__(self, eng):
         self.eng = eng
 
-    def begin(self, placed):
-        self.eng.wave_begin(placed)
+    def begin(self, placed, present=None):
+        self.eng.wave_begin(placed, present)
 
-    def run(self, remain_lists):
-        return self.eng.wave_run(remain_lists, detail=True)
+    def run(self, remain_lists, joins=None):
+        return self.eng.wave_run(remain_lists, joins, detail=True)
 
-    def commit(self, i: int):
-        self.eng.wave_commit(i)
+    def commit(self, i: int, retire: bool = False):
+        self.eng.wave_commit(i, retire)
 
     def placement(self):
         return self.eng.wave_placement()
@@ -151,58 +156,120 @@ def plan_rolling(compiled, placed: np.ndarray, runner: WaveRunner, candidates: O
     if max_unavailable < 1:
         raise ValueError(f"max_unavailable must be at least 1 (got {max_unavailable})")
     cand = order_candidates(compiled, placed, candidates, order)
+    plan = RollingPlan(Order=[compiled.node_names[c] for c in cand])
+    runner.begin(placed)
+    plan.Waves, plan.Skipped, plan.MovedPods, _ = run_waves(compiled, placed, runner, cand, max_unavailable, caps, pdbs)
+    plan.FinalPlacement = final_placement(compiled, runner)
+    plan.TotalWaves = len(plan.Waves)
+    return plan
+
+
+def final_placement(compiled, runner: WaveRunner) -> Dict[str, tuple]:
+    """Pod "namespace/name" -> (node or None, gpu-index or None) of the runner's base."""
+    names = compiled.node_names
+    final, slots = runner.placement()
+    out = {}
+    for q, rec in enumerate(compiled.pod_recs):
+        g = int(final[q])
+        out[f"{rec.tmpl.namespace}/{rec.name}"] = (names[g] if g >= 0 else None, scaledown.gpu_index(int(slots[q])) if g >= 0 else None)
+    return out
+
+
+def join_pods(compiled, r: dict) -> list:
+    """The join pods of one wave_run(joins=..., detail=True) dict as grow.NewPod: their nodes (None: unschedulable) and gpu-index."""
+    from .grow import NewPod
+    names, recs = compiled.node_names, compiled.pod_recs
+    return [NewPod(recs[q], names[g] if g >= 0 else None, scaledown.gpu_index(int(w)) if g >= 0 else None)
+            for q, g, w in zip(r["join_pods"].tolist(), r["join_node"].tolist(), r["join_gpu_slots"].tolist())]
+
+
+def join_reasons(compiled, r: dict, remain: np.ndarray) -> List[str]:
+    """The FitError text of each unscheduled join pod of one wave_run(joins=..., detail=True) dict."""
+    from .simulator import format_fit_error
+    recs = compiled.pod_recs
+    active = np.asarray(remain).tolist()
+    memo: dict = {}
+    return [f"new-node pod {recs[q].tmpl.namespace}/{recs[q].name}: "
+            + format_fit_error(compiled, recs[q], r["join_fail_counts"][j], active=active, static_memo=memo)
+            for j, q in enumerate(r["join_fail_pod"].tolist())]
+
+
+def run_waves(compiled, placed: np.ndarray, runner: WaveRunner, cand: List[int], per_wave: int, caps: Optional[tuple], pdbs,
+              present: Optional[np.ndarray] = None, copies: Sequence[int] = (), max_surge: int = 0):
+    """The wave loop on a runner that holds the first base (begin done): each wave evaluates, in one batch, the prefixes of length
+    1 .. min(per_wave, remaining) of the remaining candidates and commits the longest one whose every prefix is committable.  Without
+    `present` (rolling maintenance) the drained nodes return.  With it (node-pool replacement; present: the nodes in the cluster)
+    each wave first joins the next min(max_surge, left) nodes of `copies`, every prefix is evaluated with those joins, a committable
+    prefix also places every join pod, and the drained nodes retire; when no prefix is committable the first candidate is skipped and
+    the wave is tried again with the same joins.  -> (waves, skipped, moved pods, copies never joined)."""
     max_cpu, max_mem = caps if caps is not None else env_caps()
     names = compiled.node_names
     n = compiled.n_nodes
     nodes = scaledown.NodeOrder(compiled)
-    plan = RollingPlan(Order=[names[c] for c in cand])
-    runner.begin(placed)
+    pool = present is not None
+    state = np.array(present, dtype=np.int8) if pool else None          # 0 absent, 1 present, 2 retired
+    left = list(copies)
+    waves: List[Wave] = []
+    skipped: List[SkippedNode] = []
+    moved = 0
     base = np.array(placed, dtype=np.int32)
     remaining = list(cand)
     pinned = pinned_pods(compiled, placed)
     recs = compiled.pod_recs
     while remaining:
-        m = min(max_unavailable, len(remaining), n - 1)
+        join = left[:max_surge] if pool else []
+        out_nodes = np.nonzero(state != 1)[0].tolist() if pool else []       # absent or retired
+        n_in = n - len(out_nodes) + len(join)
+        m = min(per_wave, len(remaining), n_in - 1)
         if m == 0:
-            plan.Skipped += [SkippedNode(names[c], len(plan.Waves), [LAST_NODE_REASON]) for c in remaining]
+            skipped += [SkippedNode(names[c], len(waves), [LAST_NODE_REASON]) for c in remaining]
             break
         if remaining[0] in pinned:
-            plan.Skipped.append(SkippedNode(names[remaining[0]], len(plan.Waves),
-                                            [f"pod {recs[q].tmpl.namespace}/{recs[q].name} {why}" for q, why in pinned[remaining[0]]]))
+            skipped.append(SkippedNode(names[remaining[0]], len(waves),
+                                       [f"pod {recs[q].tmpl.namespace}/{recs[q].name} {why}" for q, why in pinned[remaining[0]]]))
             remaining.pop(0)
             continue
         m = next((j for j in range(1, m) if remaining[j] in pinned), m)       # the prefixes past a pinned node fail
         removed = [remaining[:j] for j in range(1, m + 1)]
-        remain = [nodes.remaining(r) for r in removed]
-        raw = runner.run(remain)
+        if pool:
+            gone = [g for g in out_nodes if g not in set(join)]
+            remain = [nodes.remaining(gone + r) for r in removed]
+            raw = runner.run(remain, [np.asarray(join, np.uint32)] * len(remain))
+        else:
+            remain = [nodes.remaining(r) for r in removed]
+            raw = runner.run(remain)
         k = 0
         for r in raw:
-            if not (scaledown.drainable(r) and occupancy_ok(r, max_cpu, max_mem)):
+            if not (scaledown.drainable(r) and occupancy_ok(r, max_cpu, max_mem) and r.get("n_join_unscheduled", 0) == 0):
                 break
             k += 1
         if k == 0:
             allowed = pdb_allowed(pdbs, base) if pdbs is not None else None
             d = scaledown.drain_results(compiled, base, removed[:1], remain[:1], raw[:1], max_cpu, max_mem, pdbs=pdbs, allowed=allowed)[0]
-            plan.Skipped.append(SkippedNode(names[remaining[0]], len(plan.Waves), _reasons(d), d))
+            why = join_reasons(compiled, raw[0], remain[0]) if pool else []
+            skipped.append(SkippedNode(names[remaining[0]], len(waves), why + _reasons(d), d))
             remaining.pop(0)
             continue
         r = raw[k - 1]
         d = scaledown.drain_results(compiled, base, removed[k - 1:k], remain[k - 1:k], [r], max_cpu, max_mem)[0]
         w = Wave(Nodes=[names[c] for c in removed[k - 1]], Evicted=d.EvictedPods, Occupancy=d.Occupancy)
+        if pool:
+            w.Joined = [names[g] for g in join]
+            w.JoinPods = join_pods(compiled, r)
         if pdbs is not None:
             for q in r["evicted"].tolist():
                 for j in pdbs.pod_pdb[pdbs.pod_off[q]:pdbs.pod_off[q + 1]]:
                     nm = pdbs.names[int(j)]
                     w.PdbEvicted[nm] = w.PdbEvicted.get(nm, 0) + 1
-        runner.commit(k - 1)
+        if pool:
+            runner.commit(k - 1, True)
+            state[join] = 1
+            state[removed[k - 1]] = 2
+            left = left[len(join):]
+        else:
+            runner.commit(k - 1)
         base = np.array(runner.placement()[0], dtype=np.int32)
-        plan.Waves.append(w)
-        plan.MovedPods += len(w.Evicted)
+        waves.append(w)
+        moved += len(w.Evicted)
         remaining = remaining[k:]
-    final, slots = runner.placement()
-    for q, rec in enumerate(compiled.pod_recs):
-        g = int(final[q])
-        plan.FinalPlacement[f"{rec.tmpl.namespace}/{rec.name}"] = (names[g] if g >= 0 else None,
-                                                               scaledown.gpu_index(int(slots[q])) if g >= 0 else None)
-    plan.TotalWaves = len(plan.Waves)
-    return plan
+    return waves, skipped, moved, left

@@ -726,6 +726,57 @@ class Simulator:
         self.last_grow_timing = tm
         return res
 
+    def PlanNodeReplacement(self, nodes: List[str], new_node: Obj, count: Optional[int] = None, max_surge: int = 1,
+                            max_unavailable: int = 0, order: str = "utilisation", kmax: Optional[int] = None):
+        """replace.ReplacementPlan: the old nodes `nodes` replaced by copies of `new_node` in surge waves.  Each wave joins the next
+        min(max_surge, left) copies, then drains the longest prefix (up to max_surge + max_unavailable) of the remaining old nodes whose
+        every prefix is committable (every join and evicted pod placed, the PDBs and the MaxCPU / MaxMemory caps held); the drained nodes
+        leave for good.  An old node that cannot go even alone is skipped with its reasons, and the wave is tried again with the same
+        joins.  Sizing: one batch whose scenario k joins k copies and retires the pool; MinNodes is the least committable k (-1:
+        none up to kmax, default len(nodes)).  The sizing leaves out the old nodes that hold pods which never move (bound by
+        spec.nodeName, or with Open-Local volumes; rolling.pinned_pods): they can never retire, and would make every scenario fail.  count: the copies the plan may join (default MinNodes, or kmax when none).  The superset
+        (the session's nodes plus kmax copies) is compiled once and runs on a device context of its own; the session's engine, compiled
+        cluster and placements are not changed."""
+        from . import grow, rolling
+        from . import replace as node_replace
+        from .engine import Engine
+        _eng, compiled = self._live()
+        cand = [compiled.node_index(nm) for nm in nodes]
+        bad = [nm for nm, g in zip(nodes, cand) if g < 0]
+        if bad:
+            raise ValueError(f"PlanNodeReplacement: no node named {bad[0]!r}")
+        dup = next((nm for i, nm in enumerate(nodes) if nm in nodes[:i]), None)
+        if dup is not None:
+            raise ValueError(f"PlanNodeReplacement: node {dup!r} is listed twice")
+        if not isinstance(new_node, dict) or new_node.get("kind") != "Node":
+            raise ValueError(f"PlanNodeReplacement: new_node is {type(new_node).__name__}, not a Node")
+        if max_surge < 0 or max_unavailable < 0 or max_surge + max_unavailable < 1:
+            raise ValueError(f"PlanNodeReplacement: max_surge + max_unavailable must be at least 1, neither below 0 "
+                             f"(got {max_surge} and {max_unavailable})")
+        if order not in ("utilisation", "given"):
+            raise ValueError(f"PlanNodeReplacement: unknown order {order!r} (one of utilisation, given)")
+        kmax = len(nodes) if kmax is None else int(kmax)
+        if kmax < 0 or (count is not None and not 0 <= count <= kmax):
+            raise ValueError(f"PlanNodeReplacement: need 0 <= count <= kmax (got count {count}, kmax {kmax})")
+        if compiled.n_nodes + kmax > grow.ENGINE_MAX_NODES:
+            raise ValueError(f"PlanNodeReplacement: {compiled.n_nodes} nodes + {kmax} copies exceed the engine's {grow.ENGINE_MAX_NODES}; "
+                             f"lower kmax")
+        import time
+        t0 = time.perf_counter()
+        c, placed, present, pool, copies, pdbs = node_replace.superset(self, [compiled.node_names[g] for g in cand], new_node, kmax)
+        tm = {"compile_s": time.perf_counter() - t0}
+        t0 = time.perf_counter()
+        with Engine(c, device=self.options.device, record_scores=self.options.record_scores) as eng:
+            if pdbs is not None:
+                eng.pdbs_upload(pdbs)
+            plan = node_replace.plan_replacement(c, placed, rolling.EngineRunner(eng), present, pool, copies, count, max_surge, max_unavailable,
+                                            order, pdbs=pdbs)
+            self.last_replace = eng.last_wave
+        tm["plan_s"] = time.perf_counter() - t0
+        self.last_replace_timing = tm
+        plan.Spec = O.name_of(new_node)
+        return plan
+
     def Explain(self, entries: list, top: int = 3):
         """Per entry an explain.Explanation: why the pod goes where it goes on the session's state - its node, the feasible count, the
         best `top` feasible nodes with each score plugin's weighted points, and the FitError reasons of the other nodes.  An entry is
