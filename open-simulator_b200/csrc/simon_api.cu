@@ -361,46 +361,46 @@ struct simon_ctx {
     } scope;
     struct { uint32_t scope = 0; } move_run;        // the scope of the last simon_moves_run
     struct { uint32_t n = 0; } storage_batch;       // scenarios of the last storage batch, whose Open-Local slices the batch pool keeps
-    // the last drain batch (simon_drain_run): n scenarios, per scenario its evicted pods (CSR off / pods, pod order), blocked pods
-    // (boff / blocked) and failures; on the device the evicted pods' nodes, scores, GPU slots and failure records (max rows per
-    // scenario: its largest evictee list); per drain its violated PDBs, ascending, and their evicted members (CSR voff); the device
-    // times of the setup (ev0 .. evm) and the placement (evm .. ev1)
+    // The outputs of the last drain, probe or grow batch, owned by whichever of DRAIN_BATCH, PROBE_BATCH and GROW_BATCH is set
+    // (batch_outputs): n scenarios; on the device the per-pod nodes, GPU slots and scores, scenario i's based at i * stride, and `rows`
+    // failure records per scenario
     struct {
-        uint32_t n = 0, max = 0;
+        uint32_t n = 0, stride = 0, rows = 0;
+        DevBuf<int32_t> d_node;
+        DevBuf<uint32_t> d_gpu, d_fail_counts, d_fail_pod;
+        DevBuf<int64_t> d_score;
+    } bout;
+    // the last drain batch (simon_drain_run): per scenario its evicted pods (CSR off / pods, pod order), blocked pods (boff / blocked)
+    // and failures; the failure rows per scenario (max: its largest device list); on the device the pod lists of the placement (CSR
+    // d_off) and the (scenario, pod) pairs of the un-import; per drain its violated PDBs, ascending, and their evicted members (CSR
+    // voff); the device times of the setup (ev0 .. evm) and the placement (evm .. ev1)
+    struct {
+        uint32_t max = 0;
         std::vector<uint32_t> off, pods, boff, blocked, nfail, voff, vpdb, vcnt;
         std::vector<uint32_t> dpos;         // per drain: the device position of its first evicted pod (after a wave batch's join pods)
-        DevBuf<uint32_t> d_pods, d_off, d_gpu, d_fail_counts, d_fail_pod;
-        DevBuf<int32_t> d_node;
-        DevBuf<int64_t> d_score;
+        DevBuf<uint32_t> d_pods, d_off;
         DevBuf<uint2> d_pairs;
         float setup_ms = 0.f, place_ms = 0.f;
     } drain;
-    // the last probe batch (simon_probe_run): n probes, each one's output positions (CSR off, max_replicas apart) and replicas placed; on
-    // the device the probe pods, the offsets, the replicas' nodes, scores and GPU slots, and one failure record per probe
+    // the last probe batch (simon_probe_run): each probe's output positions (CSR off, max_replicas apart) and replicas placed; on the
+    // device the probe pods and the offsets; one failure record per probe
     struct {
-        uint32_t n = 0;
         std::vector<uint32_t> off, placed;
-        DevBuf<uint32_t> d_pod, d_off, d_gpu, d_fail_counts, d_fail_pod;
-        DevBuf<int32_t> d_node;
-        DevBuf<int64_t> d_score;
+        DevBuf<uint32_t> d_pod, d_off;
         float setup_ms = 0.f, place_ms = 0.f;
     } probe;
-    // the last grow batch (simon_grow_run): n scenarios placing the tail [n_prefix, n_prefix + tail) of the pod list, each one's
-    // unscheduled tail pods; on the device the tail's nodes, GPU slots and scores (scenario i's pod q at i * tail + q: n * tail +
-    // n_prefix entries) and tail failure records per scenario
+    // the last grow batch (simon_grow_run): scenarios placing the tail [n_prefix, n_prefix + tail) of the pod list, each one's
+    // unscheduled tail pods; scenario i's pod q lands at i * tail + q (n * tail + n_prefix outputs), tail failure records per scenario
     struct {
-        uint32_t n = 0, n_prefix = 0, tail = 0;
+        uint32_t n_prefix = 0, tail = 0;
         std::vector<uint32_t> nfail;
-        DevBuf<uint32_t> d_gpu, d_fail_counts, d_fail_pod;
-        DevBuf<int32_t> d_node;
-        DevBuf<int64_t> d_score;
         float setup_ms = 0.f, place_ms = 0.f;
     } grow;
     // the wave base (simon_wave_begin): the single-scenario pool's state and its per-pod results (out_node, out_gpu) are the base, and
     // place / slots their host mirror; of the last wave batch, each scenario's removed nodes (CSR roff / removed, index order) and
     // vanished pods (CSR voff / vanished, pod order), which return with them; on the device the returned nodes and their pods (CSR) of the last commit, and its device time.
     // present: per node 0 absent, 1 present, 2 retired (simon_wave_begin_pool); of the last batch, each scenario's joined nodes (CSR
-    // jnoff / jnodes) and join pods (CSR joff / jpods, pod order, first in the scenario's device list at drain.d_off[i]) with their
+    // jnoff / jnodes) and join pods (CSR joff / jpods, pod order, first in the scenario's device list at dstart[i]) with their
     // unscheduled count; joined: the last batch joined a node
     struct {
         std::vector<int32_t> place;
@@ -1537,14 +1537,15 @@ extern "C" int simon_drain_budget(simon_ctx *ctx, uint64_t *scenario_bytes, uint
 }
 
 // The single-scenario state copied into each of the n slots of the batch pool, one broadcast per column, and what the copies do not
-// overwrite cleared (live_batch_setup below).  A wave batch's whole setup: its single-scenario state is the wave base.
-static int batch_from_single(simon_ctx *ctx, uint32_t n, bool local, uint32_t *fail_counts, size_t fail_words, SkParams &Pb) {
+// overwrite cleared: the per-class summaries and own-score caches, the counters and clocks, and the batch's failure records
+// (batch_outputs).  local: the Open-Local state is copied too.  A wave batch's whole setup: its single-scenario state is the wave base.
+static int batch_from_single(simon_ctx *ctx, uint32_t n, bool local, SkParams &Pb) {
     ScenPool &S = ctx->single, &B = ctx->batch;
     cudaStream_t st = ctx->stream;
     CU(cudaMemsetAsync(B.csum.p, 0, 8 * n * B.ncl * SK_CSUM_W, st));
     CU(cudaMemsetAsync(B.ocache.p, 0, 8 * n * B.nodes * B.ncl, st));
     CU(cudaMemsetAsync(B.counters.p, 0, 8ull * n, st)); CU(cudaMemsetAsync(B.clk.p, 0, 16ull * n, st));
-    CU(cudaMemsetAsync(fail_counts, 0, 4ull * fail_words, st));
+    CU(cudaMemsetAsync(ctx->bout.d_fail_counts.p, 0, 4ull * n * ctx->bout.rows * SIMON_N_FAIL_CODES, st));
     CU(B.state.each(S.state, true, [&](auto &b, auto &s, uint64_t k) { ctx->launches++; return bcast(ctx, s.p, k, n, b.p); }));
     if (local) {
         CU(bcast(ctx, S.vg_req.p, B.vn, n, B.vg_req.p));
@@ -1555,36 +1556,92 @@ static int batch_from_single(simon_ctx *ctx, uint32_t n, bool local, uint32_t *f
     return SIMON_OK;
 }
 
-// The setup drain, probe and grow batches share, enqueued once their refusals and allocations are done: the live state that pods
-// [0, n_prefix) leave at `placed`, rebuilt into the single-scenario pool (the resume's rebuild, its failure records cleared as the resume clears them) and copied into
-// each of the n slots of the batch pool, one broadcast per column.  Of the batch pool only what the copies do not overwrite is cleared:
-// the per-class summaries and own-score caches, the counters and clocks, and the batch's failure records (fail_words words at
-// fail_counts).  local: the live Open-Local state (the rebuild's Bind replay) is copied too.  ctx->ev0 is recorded before it; Pb gets the
-// batch pool's launch parameters.
-static int live_batch_setup(simon_ctx *ctx, const int32_t *placed, uint32_t n_prefix, uint32_t n, bool local, uint32_t *fail_counts,
-                            size_t fail_words, SkParams &Pb) {
-    ScenPool &S = ctx->single, &B = ctx->batch;
-    cudaStream_t st = ctx->stream;
-    CU(cudaEventRecord(ctx->ev0, st));
+// The live state that pods [0, n_prefix) leave at `placed`, rebuilt into the single-scenario pool (the resume's rebuild, its failure
+// records cleared as the resume clears them; it drops the wave base), enqueued on the ctx stream
+static int live_rebuild(simon_ctx *ctx, const int32_t *placed, uint32_t n_prefix) {
+    ScenPool &S = ctx->single;
     SkParams Ps;
     fill_params(ctx, S, Ps);
     int rc = clear_pool(ctx, S);
     if (rc) return rc;
     CU(single_begin(ctx, Ps));
-    rc = rebuild_prefix(ctx, Ps, placed, n_prefix);
-    if (rc) return rc;
-    return batch_from_single(ctx, n, local, fail_counts, fail_words, Pb);
+    return rebuild_prefix(ctx, Ps, placed, n_prefix);
 }
 
-// After a drain, probe or grow batch's launch: each scenario's sums over its active nodes (simon_scen_reduce) into res and, local, its VG sums
-// into out_local, copied back on the stream (the caller synchronises)
-static int live_batch_reduce(simon_ctx *ctx, uint32_t n, bool local, std::vector<simon_scenario_result> &res,
-                             simon_scenario_local_result *out_local) {
+// The setup drain, probe and grow batches share, enqueued once their refusals and allocations are done: the live state that pods
+// [0, n_prefix) leave at `placed` (live_rebuild), copied into each of the n slots of the batch pool (batch_from_single).  local: the live
+// Open-Local state (the rebuild's Bind replay) is copied too.  ctx->ev0 is recorded before it; Pb gets the batch pool's launch parameters.
+static int live_batch_setup(simon_ctx *ctx, const int32_t *placed, uint32_t n_prefix, uint32_t n, bool local, SkParams &Pb) {
+    CU(cudaEventRecord(ctx->ev0, ctx->stream));
+    const int rc = live_rebuild(ctx, placed, n_prefix);
+    return rc ? rc : batch_from_single(ctx, n, local, Pb);
+}
+
+// A drain, probe or grow batch's first step after its refusals: the batch pool, its Open-Local slices and the output block are no
+// longer the last batch's, and no placement kernel of this call has run
+static int batch_begin(simon_ctx *ctx) {
+    CU(cudaSetDevice(ctx->device));
+    ctx->last_launch = simon_launch_info{};
+    ctx->valid.drop(DRAIN_BATCH | WAVE_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
+    return SIMON_OK;
+}
+
+struct Geometry { uint32_t CS = 0, TPB = 0, NPT = 0; size_t smem = 0; };
+
+// The geometry g of family fam for n scenarios of at most n_active nodes, and the batch pool sized for them (without per-pod outputs:
+// those are in the output block)
+static int batch_pool(simon_ctx *ctx, uint32_t n_active, uint32_t n, Family fam, Geometry &g) {
+    const int rc = choose_geometry(ctx, n_active, g.CS, g.TPB, g.NPT, g.smem, n, fam);
+    return rc ? rc : size_pool(ctx, ctx->batch, n, false, false);
+}
+
+// The output block of a batch of n scenarios (ctx->bout): `cells` per-pod outputs (node, GPU slots, scores when recorded), scenario
+// i's based at i * stride, and `rows` failure records per scenario; each SkScenario of h pointed at its slice and uploaded to the batch
+// pool.  Refused when the outputs do not fit the device next to what the block holds (the free memory is asked only when the block
+// must grow); `what` names them in the message.
+static int batch_outputs(simon_ctx *ctx, uint32_t n, uint64_t cells, uint32_t stride, uint32_t rows, std::vector<SkScenario> &h,
+                         const char *what) {
+    auto &o = ctx->bout;
+    size_t fr = 0, tot = 0;
+    const uint64_t rec = 4ull * SIMON_N_FAIL_CODES + 4;          // a failure record: its reason counts and its pod
+    const uint64_t held = 16ull * o.d_node.cap + rec * o.d_fail_pod.cap, need = 16ull * cells + rec * n * rows;
+    const bool grows = cells > o.d_node.cap || (uint64_t)n * rows > o.d_fail_pod.cap;
+    if (grows) CU(cudaMemGetInfo(&fr, &tot));
+    if (cells >= (1ull << 32) || (grows && need > (uint64_t)fr + held))
+        return fail(ctx, SIMON_ERR_LIMIT, "%s (%llu bytes) do not fit the device (%llu bytes free)", what, (unsigned long long)need,
+                    (unsigned long long)fr);
+    const bool scores = ctx->opt_flags & SIMON_OPT_RECORD_SCORES;
+    CU(o.d_node.alloc(cells)); CU(o.d_gpu.alloc(cells));
+    if (scores) CU(o.d_score.alloc(cells));
+    CU(o.d_fail_counts.alloc((size_t)n * rows * SIMON_N_FAIL_CODES)); CU(o.d_fail_pod.alloc((size_t)n * rows));
+    o.n = n; o.stride = stride; o.rows = rows;
+    for (uint32_t i = 0; i < n; i++) {
+        const size_t at = (size_t)i * stride, r = (size_t)i * rows;
+        h[i].out_node = o.d_node.p + at; h[i].out_gpu = o.d_gpu.p + at; h[i].out_score = scores ? o.d_score.p + at : nullptr;
+        h[i].fail_counts = o.d_fail_counts.p + r * SIMON_N_FAIL_CODES; h[i].fail_pod = o.d_fail_pod.p + r;
+    }
+    CU(ctx->batch.scen.upload(h.data(), n, ctx->stream));
+    return SIMON_OK;
+}
+
+// After a batch's setup (timed from ctx->ev0): when `place`, its launch of family fam on geometry g (one failure record per row of the
+// output block), timed from ctx->evm to ctx->ev1; each scenario's sums over its active nodes (simon_scen_reduce) into res and, when
+// out_local is not null, its VG sums into out_local; then the synchronisation and the device times of the setup and the placement.
+// local: the batch pool's Open-Local slices are this batch's, which simon_scenarios_storage_download serves.
+static int batch_place(simon_ctx *ctx, SkParams &Pb, uint32_t n, const Geometry &g, Family fam, bool place, bool local,
+                       std::vector<simon_scenario_result> &res, simon_scenario_local_result *out_local, float &setup_ms, float &place_ms) {
     ScenPool &B = ctx->batch;
     cudaStream_t st = ctx->stream;
+    CU(cudaEventRecord(ctx->evm, st));
+    if (place) {
+        Pb.max_fail = ctx->bout.rows; Pb.npt = g.NPT;
+        const int rc = launch(ctx, Pb, n, g.CS, g.TPB, g.smem, false, fam);
+        if (rc) return rc;
+    }
+    CU(cudaEventRecord(ctx->ev1, st));
     simon_scen_reduce<<<n, 256, 0, st>>>(B.scen.p, ctx->snap.d_alloc_mcpu.p, ctx->snap.d_alloc_mem.p, B.results.p);
     CU(cudaGetLastError());
-    if (local) {
+    if (out_local) {
         simon_scen_reduce_local<<<n, 256, 0, st>>>(B.scen.p, ctx->storage.d_node_n_vg.p, ctx->storage.d_vg_cap.p, B.vg_req.p, B.vn, ctx->snap.N,
                                                    B.local_results.p);
         CU(cudaGetLastError());
@@ -1592,7 +1649,139 @@ static int live_batch_reduce(simon_ctx *ctx, uint32_t n, bool local, std::vector
     }
     res.resize(n);
     CU(cudaMemcpyAsync(res.data(), B.results.p, sizeof(simon_scenario_result) * (size_t)n, cudaMemcpyDeviceToHost, st));
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
+    CU(cudaEventElapsedTime(&setup_ms, ctx->ev0, ctx->evm));
+    CU(cudaEventElapsedTime(&place_ms, ctx->evm, ctx->ev1));
+    CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    if (local) {
+        ctx->storage_batch.n = n;
+        ctx->valid.set(STORAGE_BATCH);
+    }
     return SIMON_OK;
+}
+
+// k per-pod outputs of the last batch from position `at` into whichever of node, gpu_slots and score is not null (scores: zeros when
+// they are not recorded)
+static int batch_download(simon_ctx *ctx, size_t at, uint32_t k, int32_t *node, uint32_t *gpu_slots, int64_t *score) {
+    const auto &o = ctx->bout;
+    if (!k) return SIMON_OK;
+    if (node) CU(cudaMemcpy(node, o.d_node.p + at, 4ull * k, cudaMemcpyDeviceToHost));
+    if (gpu_slots) CU(cudaMemcpy(gpu_slots, o.d_gpu.p + at, 4ull * k, cudaMemcpyDeviceToHost));
+    if (score) {
+        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(cudaMemcpy(score, o.d_score.p + at, 8ull * k, cudaMemcpyDeviceToHost));
+        else memset(score, 0, 8ull * k);
+    }
+    return SIMON_OK;
+}
+
+// nf failure records of the last batch from row r into whichever of fail_counts and fail_pod is not null
+static int batch_fail_download(simon_ctx *ctx, size_t r, uint32_t nf, uint32_t *fail_counts, uint32_t *fail_pod) {
+    const auto &o = ctx->bout;
+    if (fail_counts && nf)
+        CU(cudaMemcpy(fail_counts, o.d_fail_counts.p + r * SIMON_N_FAIL_CODES, 4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
+    if (fail_pod && nf) CU(cudaMemcpy(fail_pod, o.d_fail_pod.p + r, 4ull * nf, cudaMemcpyDeviceToHost));
+    return SIMON_OK;
+}
+
+// A wave batch's joins, checked before any device work: the nodes each scenario joins (CSR wave.jnoff / jnodes; join == nullptr:
+// none), every node it keeps against the node states of the base, and its join pods (CSR wave.joff / jpods: the pods whose DaemonSet
+// guard joins, pod order)
+static int wave_joins(simon_ctx *ctx, const simon_scenario *join, uint32_t n) {
+    const uint32_t N = ctx->snap.N, N1 = std::max(1u, N), P = ctx->pods.n_pods;
+    const std::vector<uint8_t> &pr = ctx->wave.present;
+    ctx->wave.jnoff.assign(1, 0u); ctx->wave.jnodes.clear(); ctx->wave.joff.assign(1, 0u); ctx->wave.jpods.clear();
+    std::vector<uint8_t> joining(N1, 0u);
+    std::vector<uint32_t> goff, gpods;          // the pods of each DaemonSet guard node (CSR, pod order), built at the first join
+    for (uint32_t i = 0; i < n; i++) {
+        const int32_t *rank = ctx->batch.h_rank.data() + (size_t)i * N1;
+        const uint32_t nj = join ? join[i].n_nodes : 0u, j0 = (uint32_t)ctx->wave.jnodes.size();
+        if (nj && !join[i].nodes) return fail(ctx, SIMON_ERR_INVALID, "wave %u: join nodes is NULL", i);
+        for (uint32_t k = 0; k < nj; k++) {
+            const uint32_t g = join[i].nodes[k];
+            if (g >= N) return fail(ctx, SIMON_ERR_INVALID, "wave %u joins node %u, out of range", i, g);
+            if (joining[g]) return fail(ctx, SIMON_ERR_INVALID, "wave %u joins node %u twice", i, g);
+            if (pr[g] != 0) return fail(ctx, SIMON_ERR_INVALID, "wave %u joins node %u, which is not absent", i, g);
+            if (rank[g] < 0) return fail(ctx, SIMON_ERR_INVALID, "wave %u joins node %u, which is not in its remaining nodes", i, g);
+            joining[g] = 1;
+            ctx->wave.jnodes.push_back(g);
+        }
+        for (uint32_t g = 0; g < N; g++)
+            if (rank[g] >= 0 && !joining[g] && pr[g] != 1)
+                return fail(ctx, SIMON_ERR_INVALID, pr[g] == 2 ? "wave %u keeps node %u, which is retired"
+                                                               : "wave %u keeps node %u, which is absent and does not join", i, g);
+        const size_t p0 = ctx->wave.jpods.size();
+        if (nj && goff.empty()) {
+            goff.assign(N1 + 1, 0u);
+            for (uint32_t q = 0; q < P; q++)
+                if (ctx->pods.h_guard[q] >= 0) goff[ctx->pods.h_guard[q] + 1]++;
+            for (uint32_t g = 0; g < N1; g++) goff[g + 1] += goff[g];
+            gpods.resize(goff[N1]);
+            std::vector<uint32_t> cur(goff.begin(), goff.end() - 1);
+            for (uint32_t q = 0; q < P; q++)
+                if (ctx->pods.h_guard[q] >= 0) gpods[cur[ctx->pods.h_guard[q]]++] = q;
+        }
+        for (uint32_t k = j0; k < ctx->wave.jnodes.size(); k++) {
+            const uint32_t g = ctx->wave.jnodes[k];
+            joining[g] = 0;
+            ctx->wave.jpods.insert(ctx->wave.jpods.end(), gpods.begin() + goff[g], gpods.begin() + goff[g + 1]);
+        }
+        std::sort(ctx->wave.jpods.begin() + p0, ctx->wave.jpods.end());
+        for (size_t k = p0; k < ctx->wave.jpods.size(); k++) {
+            const uint32_t q = ctx->wave.jpods[k];
+            if (ctx->pods.h_fixed[q] >= 0)
+                return fail(ctx, SIMON_ERR_INVALID, "wave %u: join pod %u is bound by spec.nodeName", i, q);
+            if (ctx->valid.has(STORAGE) && ctx->storage.h_class_local[ctx->pods.h_class[q]])
+                return fail(ctx, SIMON_ERR_INVALID, "wave %u: join pod %u has Open-Local volumes", i, q);
+        }
+        ctx->wave.jnoff.push_back((uint32_t)ctx->wave.jnodes.size());
+        ctx->wave.joff.push_back((uint32_t)ctx->wave.jpods.size());
+    }
+    return SIMON_OK;
+}
+
+// Per drain, from the pods each node holds at `placed` (one CSR): its removed nodes (CSR wave.roff / removed), and their pods in pod
+// order, as (scenario, pod) pairs for the un-import, split into vanished (DaemonSet pods of a removed node: CSR wave.voff / vanished),
+// blocked (bound by spec.nodeName, or with Open-Local volumes unless local: CSR drain.boff / blocked) and evicted pods (CSR drain.off /
+// pods)
+static void drain_split(simon_ctx *ctx, const int32_t *placed, uint32_t n, bool local, std::vector<uint2> &pairs) {
+    const uint32_t N = ctx->snap.N, N1 = std::max(1u, N), P = ctx->pods.n_pods;
+    std::vector<uint32_t> node_off(N1 + 1, 0u), node_pods;
+    for (uint32_t q = 0; q < P; q++)
+        if (placed[q] >= 0) node_off[placed[q] + 1]++;
+    for (uint32_t g = 0; g < N1; g++) node_off[g + 1] += node_off[g];
+    node_pods.resize(node_off[N1]);
+    {
+        std::vector<uint32_t> cur(node_off.begin(), node_off.end() - 1);
+        for (uint32_t q = 0; q < P; q++)
+            if (placed[q] >= 0) node_pods[cur[placed[q]]++] = q;
+    }
+    ctx->drain.off.assign(1, 0u); ctx->drain.pods.clear(); ctx->drain.boff.assign(1, 0u); ctx->drain.blocked.clear();
+    ctx->wave.voff.assign(1, 0u); ctx->wave.vanished.clear(); ctx->wave.roff.assign(1, 0u); ctx->wave.removed.clear();
+    pairs.clear();
+    std::vector<uint32_t> rm;
+    for (uint32_t i = 0; i < n; i++) {
+        const int32_t *rank = ctx->batch.h_rank.data() + (size_t)i * N1;
+        rm.clear();
+        for (uint32_t g = 0; g < N; g++)
+            if (rank[g] < 0) {
+                rm.insert(rm.end(), node_pods.begin() + node_off[g], node_pods.begin() + node_off[g + 1]);
+                ctx->wave.removed.push_back(g);
+            }
+        ctx->wave.roff.push_back((uint32_t)ctx->wave.removed.size());
+        std::sort(rm.begin(), rm.end());
+        for (uint32_t q : rm) {
+            pairs.push_back(make_uint2(i, q));
+            const int32_t gd = ctx->pods.h_guard[q];
+            if (gd >= 0 && rank[gd] < 0) ctx->wave.vanished.push_back(q);
+            else if (ctx->pods.h_fixed[q] >= 0 || (!local && ctx->valid.has(STORAGE) && ctx->storage.h_class_local[ctx->pods.h_class[q]]))
+                ctx->drain.blocked.push_back(q);
+            else ctx->drain.pods.push_back(q);
+        }
+        ctx->drain.off.push_back((uint32_t)ctx->drain.pods.size());
+        ctx->drain.boff.push_back((uint32_t)ctx->drain.blocked.size());
+        ctx->wave.voff.push_back((uint32_t)ctx->wave.vanished.size());
+    }
 }
 
 // simon_drain_run and simon_drain_run_local (out_local != nullptr: pods with Open-Local volumes are evicted, not blocked, and each
@@ -1607,9 +1796,9 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
     const char *what = wave ? "simon_wave_run" : local ? "simon_drain_run_local" : "simon_drain_run";
     if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "%s before uploads", what);
     if ((ctx->pods.n_pods && !placed) || (n && (!remain || !out))) return fail(ctx, SIMON_ERR_INVALID, "%s: NULL argument", what);
-    const uint32_t N = ctx->snap.N, N1 = std::max(1u, N), P = ctx->pods.n_pods;
+    const uint32_t P = ctx->pods.n_pods;
     // ---- refusals before any device work: the live placement as a resume prefix checks it (a wave base was checked when it began),
-    // then the node lists ----
+    // then the node lists, then a wave's joins ----
     int rc = wave ? SIMON_OK : check_prefix(ctx, placed, P);
     if (rc) return rc;
     for (uint32_t i = 0; i < n; i++)
@@ -1617,113 +1806,23 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
     uint32_t max_active = 0;
     rc = scenario_lists(ctx, remain, n, "drain", max_active);
     if (rc) return rc;
-    // ---- a wave: the nodes each scenario joins and the node states of the base, then the join pods (the pods whose DaemonSet guard
-    // joins, pod order) ----
-    ctx->wave.jnoff.assign(1, 0u); ctx->wave.jnodes.clear(); ctx->wave.joff.assign(1, 0u); ctx->wave.jpods.clear();
     if (wave) {
-        const std::vector<uint8_t> &pr = ctx->wave.present;
-        std::vector<uint8_t> joining(N1, 0u);
-        std::vector<uint32_t> goff, gpods;          // the pods of each DaemonSet guard node (CSR, pod order), built at the first join
-        for (uint32_t i = 0; i < n; i++) {
-            const int32_t *rank = ctx->batch.h_rank.data() + (size_t)i * N1;
-            const uint32_t nj = join ? join[i].n_nodes : 0u, j0 = (uint32_t)ctx->wave.jnodes.size();
-            if (nj && !join[i].nodes) return fail(ctx, SIMON_ERR_INVALID, "wave %u: join nodes is NULL", i);
-            for (uint32_t k = 0; k < nj; k++) {
-                const uint32_t g = join[i].nodes[k];
-                if (g >= N) return fail(ctx, SIMON_ERR_INVALID, "wave %u joins node %u, out of range", i, g);
-                if (joining[g]) return fail(ctx, SIMON_ERR_INVALID, "wave %u joins node %u twice", i, g);
-                if (pr[g] != 0) return fail(ctx, SIMON_ERR_INVALID, "wave %u joins node %u, which is not absent", i, g);
-                if (rank[g] < 0) return fail(ctx, SIMON_ERR_INVALID, "wave %u joins node %u, which is not in its remaining nodes", i, g);
-                joining[g] = 1;
-                ctx->wave.jnodes.push_back(g);
-            }
-            for (uint32_t g = 0; g < N; g++)
-                if (rank[g] >= 0 && !joining[g] && pr[g] != 1)
-                    return fail(ctx, SIMON_ERR_INVALID, pr[g] == 2 ? "wave %u keeps node %u, which is retired"
-                                                                   : "wave %u keeps node %u, which is absent and does not join", i, g);
-            const size_t p0 = ctx->wave.jpods.size();
-            if (nj && goff.empty()) {
-                goff.assign(N1 + 1, 0u);
-                for (uint32_t q = 0; q < P; q++)
-                    if (ctx->pods.h_guard[q] >= 0) goff[ctx->pods.h_guard[q] + 1]++;
-                for (uint32_t g = 0; g < N1; g++) goff[g + 1] += goff[g];
-                gpods.resize(goff[N1]);
-                std::vector<uint32_t> cur(goff.begin(), goff.end() - 1);
-                for (uint32_t q = 0; q < P; q++)
-                    if (ctx->pods.h_guard[q] >= 0) gpods[cur[ctx->pods.h_guard[q]]++] = q;
-            }
-            for (uint32_t k = j0; k < ctx->wave.jnodes.size(); k++) {
-                const uint32_t g = ctx->wave.jnodes[k];
-                joining[g] = 0;
-                ctx->wave.jpods.insert(ctx->wave.jpods.end(), gpods.begin() + goff[g], gpods.begin() + goff[g + 1]);
-            }
-            std::sort(ctx->wave.jpods.begin() + p0, ctx->wave.jpods.end());
-            for (size_t k = p0; k < ctx->wave.jpods.size(); k++) {
-                const uint32_t q = ctx->wave.jpods[k];
-                if (ctx->pods.h_fixed[q] >= 0)
-                    return fail(ctx, SIMON_ERR_INVALID, "wave %u: join pod %u is bound by spec.nodeName", i, q);
-                if (ctx->valid.has(STORAGE) && ctx->storage.h_class_local[ctx->pods.h_class[q]])
-                    return fail(ctx, SIMON_ERR_INVALID, "wave %u: join pod %u has Open-Local volumes", i, q);
-            }
-            ctx->wave.jnoff.push_back((uint32_t)ctx->wave.jnodes.size());
-            ctx->wave.joff.push_back((uint32_t)ctx->wave.jpods.size());
-        }
+        rc = wave_joins(ctx, join, n);
+        if (rc) return rc;
     } else {
-        ctx->wave.jnoff.assign(n + 1, 0u); ctx->wave.joff.assign(n + 1, 0u);
+        ctx->wave.jnoff.assign(n + 1, 0u); ctx->wave.jnodes.clear(); ctx->wave.joff.assign(n + 1, 0u); ctx->wave.jpods.clear();
     }
-    CU(cudaSetDevice(ctx->device));
-    ctx->last_launch = simon_launch_info{};
-    // the batch pool is no longer a probe or grow batch's, nor are its Open-Local slices a storage batch's
-    ctx->valid.drop(DRAIN_BATCH | WAVE_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
-    ScenPool &S = ctx->single, &B = ctx->batch;
-    if (n == 0) return SIMON_OK;
+    rc = batch_begin(ctx);
+    if (rc || n == 0) return rc;
+    ScenPool &S = ctx->single;
     cudaStream_t st = ctx->stream;
-    // ---- per scenario, from the pods each node holds (one CSR): the pods of its removed nodes in pod order, as (scenario, pod)
-    // pairs for the un-import, and split into vanished (DaemonSet pods of a removed node), blocked (bound by spec.nodeName, or with
-    // Open-Local volumes unless local) and evicted pods ----
-    std::vector<uint32_t> node_off(N1 + 1, 0u), node_pods;
-    for (uint32_t q = 0; q < P; q++)
-        if (placed[q] >= 0) node_off[placed[q] + 1]++;
-    for (uint32_t g = 0; g < N1; g++) node_off[g + 1] += node_off[g];
-    node_pods.resize(node_off[N1]);
-    {
-        std::vector<uint32_t> cur(node_off.begin(), node_off.end() - 1);
-        for (uint32_t q = 0; q < P; q++)
-            if (placed[q] >= 0) node_pods[cur[placed[q]]++] = q;
-    }
-    ctx->drain.off.assign(1, 0u); ctx->drain.pods.clear(); ctx->drain.boff.assign(1, 0u); ctx->drain.blocked.clear();
     std::vector<uint2> pairs;
-    std::vector<uint32_t> n_vanished(n, 0u), rm;
-    ctx->drain.max = 0;
-    ctx->wave.voff.assign(1, 0u); ctx->wave.vanished.clear(); ctx->wave.roff.assign(1, 0u); ctx->wave.removed.clear();
-    for (uint32_t i = 0; i < n; i++) {
-        const int32_t *rank = B.h_rank.data() + (size_t)i * N1;
-        rm.clear();
-        for (uint32_t g = 0; g < N; g++)
-            if (rank[g] < 0) {
-                rm.insert(rm.end(), node_pods.begin() + node_off[g], node_pods.begin() + node_off[g + 1]);
-                if (wave) ctx->wave.removed.push_back(g);
-            }
-        ctx->wave.roff.push_back((uint32_t)ctx->wave.removed.size());
-        std::sort(rm.begin(), rm.end());
-        for (uint32_t q : rm) {
-            pairs.push_back(make_uint2(i, q));
-            const int32_t gd = ctx->pods.h_guard[q];
-            if (gd >= 0 && rank[gd] < 0) {
-                n_vanished[i]++;
-                if (wave) ctx->wave.vanished.push_back(q);
-            } else if (ctx->pods.h_fixed[q] >= 0 || (!local && ctx->valid.has(STORAGE) && ctx->storage.h_class_local[ctx->pods.h_class[q]]))
-                ctx->drain.blocked.push_back(q);
-            else ctx->drain.pods.push_back(q);
-        }
-        ctx->drain.off.push_back((uint32_t)ctx->drain.pods.size());
-        ctx->drain.boff.push_back((uint32_t)ctx->drain.blocked.size());
-        ctx->wave.voff.push_back((uint32_t)ctx->wave.vanished.size());
-    }
+    drain_split(ctx, placed, n, local, pairs);
     // ---- the device lists: per scenario its join pods, then its evicted pods; the failure records are sized for both ----
     ctx->wave.joined = !ctx->wave.jnodes.empty();
     std::vector<uint32_t> dlist, doff(1, 0u);
     ctx->drain.dpos.resize(n);
+    ctx->drain.max = 0;
     for (uint32_t i = 0; i < n; i++) {
         dlist.insert(dlist.end(), ctx->wave.jpods.begin() + ctx->wave.joff[i], ctx->wave.jpods.begin() + ctx->wave.joff[i + 1]);
         ctx->drain.dpos[i] = (uint32_t)dlist.size();
@@ -1734,38 +1833,28 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
     ctx->wave.dstart.assign(doff.begin(), doff.end());
     const size_t n_ev = dlist.size();
     // ---- geometry of the drain variant, the batch pool and the outputs (allocations before the timed work) ----
-    uint32_t CS, TPB, NPT;
-    size_t smem;
+    Geometry g;
     const Family fam = local ? DRAIN_LOCAL : DRAIN;
-    rc = choose_geometry(ctx, max_active, CS, TPB, NPT, smem, n, fam);
-    if (rc) return rc;
-    rc = size_pool(ctx, B, n, false, false);
+    rc = batch_pool(ctx, max_active, n, fam, g);
     if (rc) return rc;
     CU(ctx->drain.d_pods.upload(dlist.data(), n_ev, st));
     CU(ctx->drain.d_off.upload(doff.data(), n + 1, st));
     CU(ctx->drain.d_pairs.upload(pairs.data(), pairs.size(), st));
-    CU(ctx->drain.d_node.alloc(n_ev)); CU(ctx->drain.d_gpu.alloc(n_ev));
-    if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(ctx->drain.d_score.alloc(n_ev));
-    CU(ctx->drain.d_fail_counts.alloc((size_t)n * ctx->drain.max * SIMON_N_FAIL_CODES)); CU(ctx->drain.d_fail_pod.alloc((size_t)n * ctx->drain.max));
     std::vector<SkScenario> h;
     CU(batch_scenarios(ctx, remain, n, h));
-    for (uint32_t i = 0; i < n; i++) {
-        h[i].out_node = ctx->drain.d_node.p; h[i].out_gpu = ctx->drain.d_gpu.p;
-        h[i].out_score = (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) ? ctx->drain.d_score.p : nullptr;
-        h[i].fail_counts = ctx->drain.d_fail_counts.p + (size_t)i * ctx->drain.max * SIMON_N_FAIL_CODES;
-        h[i].fail_pod = ctx->drain.d_fail_pod.p + (size_t)i * ctx->drain.max;
-    }
-    CU(B.scen.upload(h.data(), n, st));
+    char outputs[96];
+    snprintf(outputs, sizeof(outputs), "%s: outputs of %zu pods", what, n_ev);
+    rc = batch_outputs(ctx, n, n_ev, 0, ctx->drain.max, h, outputs);
+    if (rc) return rc;
     // ---- setup: the live state in every slot (live_batch_setup; a wave: the base, batch_from_single), minus what each scenario's
     // removed nodes' pods contributed to the counters, at their nodes in that state.  local: the removed nodes' VGs and devices keep
     // their live values, since those nodes are inactive ----
     SkParams Pb;
-    const size_t fail_words = (size_t)n * ctx->drain.max * SIMON_N_FAIL_CODES;
     if (wave) {
         CU(cudaEventRecord(ctx->ev0, st));
-        rc = batch_from_single(ctx, n, false, ctx->drain.d_fail_counts.p, fail_words, Pb);
+        rc = batch_from_single(ctx, n, false, Pb);
     } else {
-        rc = live_batch_setup(ctx, placed, P, n, local, ctx->drain.d_fail_counts.p, fail_words, Pb);
+        rc = live_batch_setup(ctx, placed, P, n, local, Pb);
     }
     if (rc) return rc;
     if (!pairs.empty()) {
@@ -1774,32 +1863,22 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
         CU(cudaGetLastError());
         ctx->launches++;
     }
-    CU(cudaEventRecord(ctx->evm, st));
-    // ---- placement of every scenario's evicted pods ----
+    // ---- placement of every scenario's device list ----
     Pb.drain_pods = ctx->drain.d_pods.p; Pb.drain_off = ctx->drain.d_off.p;
-    Pb.first = 0; Pb.count = 0; Pb.max_fail = ctx->drain.max; Pb.npt = NPT;
-    rc = launch(ctx, Pb, n, CS, TPB, smem, false, fam);
-    if (rc) return rc;
-    CU(cudaEventRecord(ctx->ev1, st));
     std::vector<simon_scenario_result> res;
-    rc = live_batch_reduce(ctx, n, local, res, out_local);
+    rc = batch_place(ctx, Pb, n, g, fam, true, local, res, out_local, ctx->drain.setup_ms, ctx->drain.place_ms);
     if (rc) return rc;
-    // with a PDB table: `allowed` on the rebuilt live state (a wave: the base), read at the same synchronisation
+    if (!wave) ctx->valid.set(LIVE);
+    // with a PDB table: `allowed` on the rebuilt live state (a wave: the base); a batch that joins: the join pods' nodes, to count
+    // them apart from the evicted pods
     const uint32_t J = ctx->valid.has(PDB_TABLE) ? ctx->pdb.n : 0;
-    std::vector<int32_t> allowed(J);
+    std::vector<int32_t> allowed(J), jnode(ctx->wave.joined ? n_ev : 0u);
     if (J) {
         CU(pdb_allowed(ctx, S.out_node.p));
         CU(cudaMemcpyAsync(allowed.data(), ctx->pdb.d_rem.p, 4ull * J, cudaMemcpyDeviceToHost, st));
     }
-    // a batch that joins: the join pods' nodes, to count them apart from the evicted pods
-    std::vector<int32_t> jnode(ctx->wave.joined ? n_ev : 0u);
-    if (ctx->wave.joined) CU(cudaMemcpyAsync(jnode.data(), ctx->drain.d_node.p, 4ull * n_ev, cudaMemcpyDeviceToHost, st));
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
-    if (!wave) ctx->valid.set(LIVE);
-    CU(cudaEventElapsedTime(&ctx->drain.setup_ms, ctx->ev0, ctx->evm));
-    CU(cudaEventElapsedTime(&ctx->drain.place_ms, ctx->evm, ctx->ev1));
-    CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
+    if (ctx->wave.joined) CU(cudaMemcpyAsync(jnode.data(), ctx->bout.d_node.p, 4ull * n_ev, cudaMemcpyDeviceToHost, st));
+    if (J || ctx->wave.joined) CU(cudaStreamSynchronize(st));
     // violated PDBs per drain: its evicted members per PDB (filterPodsWithPDBViolation's count) above `allowed`
     ctx->drain.voff.assign(1, 0u); ctx->drain.vpdb.clear(); ctx->drain.vcnt.clear();
     {
@@ -1832,16 +1911,11 @@ static int drain_run(simon_ctx *ctx, const int32_t *placed, const simon_scenario
         o.n_evicted = ctx->drain.off[i + 1] - ctx->drain.off[i];
         o.n_placed = res[i].n_scheduled; o.n_unscheduled = res[i].n_unscheduled;
         o.n_blocked = ctx->drain.boff[i + 1] - ctx->drain.boff[i];
-        o.n_vanished = n_vanished[i]; o.n_pdb_violated = ctx->drain.voff[i + 1] - ctx->drain.voff[i];
+        o.n_vanished = ctx->wave.voff[i + 1] - ctx->wave.voff[i]; o.n_pdb_violated = ctx->drain.voff[i + 1] - ctx->drain.voff[i];
         o.req_mcpu = res[i].req_mcpu; o.alloc_mcpu = res[i].alloc_mcpu; o.req_mem = res[i].req_mem; o.alloc_mem = res[i].alloc_mem;
         ctx->drain.nfail[i] = res[i].n_unscheduled;
     }
-    ctx->drain.n = n;
     ctx->valid.set(DRAIN_BATCH | (wave ? WAVE_BATCH : 0u));
-    if (local) {
-        ctx->storage_batch.n = n;           // simon_scenarios_storage_download serves this batch
-        ctx->valid.set(STORAGE_BATCH);
-    }
     return SIMON_OK;
 }
 
@@ -1869,32 +1943,22 @@ extern "C" int simon_drain_download(simon_ctx *ctx, uint32_t scenario, uint32_t 
                                     int64_t *score, uint32_t *blocked_pod, uint32_t *fail_counts, uint32_t *fail_pod) {
     if (!ctx) return SIMON_ERR_INVALID;
     if (!ctx->valid.has(DRAIN_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_drain_run batch since the last upload, or a probe batch after it");
-    if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "drain %u of a batch of %u", scenario, ctx->drain.n);
+    if (scenario >= ctx->bout.n) return fail(ctx, SIMON_ERR_INVALID, "drain %u of a batch of %u", scenario, ctx->bout.n);
     CU(cudaSetDevice(ctx->device));
     // on the device the scenario's evicted pods start at dpos, and their failure records follow those of its join pods
-    const uint32_t h = ctx->drain.off[scenario], ne = ctx->drain.off[scenario + 1] - h, b = ctx->drain.dpos[scenario];
+    const uint32_t h = ctx->drain.off[scenario], ne = ctx->drain.off[scenario + 1] - h;
     const uint32_t bb = ctx->drain.boff[scenario], nb = ctx->drain.boff[scenario + 1] - bb;
     const uint32_t fr = ctx->wave.jfail[scenario], nf = std::min(ctx->drain.nfail[scenario], ctx->drain.max - std::min(fr, ctx->drain.max));
     if (evicted_pod) std::copy(ctx->drain.pods.begin() + h, ctx->drain.pods.begin() + h + ne, evicted_pod);
     if (blocked_pod) std::copy(ctx->drain.blocked.begin() + bb, ctx->drain.blocked.begin() + bb + nb, blocked_pod);
-    if (node && ne) CU(cudaMemcpy(node, ctx->drain.d_node.p + b, 4ull * ne, cudaMemcpyDeviceToHost));
-    if (gpu_slots && ne) CU(cudaMemcpy(gpu_slots, ctx->drain.d_gpu.p + b, 4ull * ne, cudaMemcpyDeviceToHost));
-    if (score && ne) {
-        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(cudaMemcpy(score, ctx->drain.d_score.p + b, 8ull * ne, cudaMemcpyDeviceToHost));
-        else memset(score, 0, 8ull * ne);
-    }
-    if (fail_counts && nf)
-        CU(cudaMemcpy(fail_counts, ctx->drain.d_fail_counts.p + ((size_t)scenario * ctx->drain.max + fr) * SIMON_N_FAIL_CODES,
-                      4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
-    if (fail_pod && nf)
-        CU(cudaMemcpy(fail_pod, ctx->drain.d_fail_pod.p + (size_t)scenario * ctx->drain.max + fr, 4ull * nf, cudaMemcpyDeviceToHost));
-    return SIMON_OK;
+    const int rc = batch_download(ctx, ctx->drain.dpos[scenario], ne, node, gpu_slots, score);
+    return rc ? rc : batch_fail_download(ctx, (size_t)scenario * ctx->drain.max + fr, nf, fail_counts, fail_pod);
 }
 
 extern "C" int simon_drain_pdb_download(simon_ctx *ctx, uint32_t scenario, uint32_t *pdb, uint32_t *evicted) {
     if (!ctx) return SIMON_ERR_INVALID;
     if (!ctx->valid.has(DRAIN_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_drain_run batch since the last upload, or a probe batch after it");
-    if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "drain %u of a batch of %u", scenario, ctx->drain.n);
+    if (scenario >= ctx->bout.n) return fail(ctx, SIMON_ERR_INVALID, "drain %u of a batch of %u", scenario, ctx->bout.n);
     const uint32_t b = ctx->drain.voff[scenario], e = ctx->drain.voff[scenario + 1];
     if (pdb) std::copy(ctx->drain.vpdb.begin() + b, ctx->drain.vpdb.begin() + e, pdb);
     if (evicted) std::copy(ctx->drain.vcnt.begin() + b, ctx->drain.vcnt.begin() + e, evicted);
@@ -1919,12 +1983,7 @@ static int wave_begin(simon_ctx *ctx, const int32_t *placed, const uint8_t *pres
     CU(cudaSetDevice(ctx->device));
     ScenPool &S = ctx->single;
     cudaStream_t st = ctx->stream;
-    SkParams Ps;
-    fill_params(ctx, S, Ps);
-    rc = clear_pool(ctx, S);
-    if (rc) return rc;
-    CU(single_begin(ctx, Ps));          // drops the base and the last wave batch
-    rc = rebuild_prefix(ctx, Ps, placed, P);
+    rc = live_rebuild(ctx, placed, P);          // drops the base and the last wave batch
     if (rc) return rc;
     ctx->wave.place.assign(placed, placed + P);
     ctx->wave.present.swap(pr);
@@ -1962,81 +2021,15 @@ extern "C" int simon_wave_run(simon_ctx *ctx, const simon_scenario *remain, uint
     return drain_run(ctx, ctx->wave.place.data(), remain, n, out, nullptr, true);
 }
 
-extern "C" int simon_wave_commit(simon_ctx *ctx, uint32_t scenario) {
-    if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->valid.has(WAVE_BASE)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_commit without a wave base (simon_wave_begin)");
-    if (!ctx->valid.has(WAVE_BATCH)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_commit: no simon_wave_run batch since the base changed");
-    if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u of a batch of %u", scenario, ctx->drain.n);
-    if (ctx->wave.joined) return fail(ctx, SIMON_ERR_INVALID, "simon_wave_commit: the last wave batch joined nodes (simon_wave_commit_retire)");
-    const uint32_t s = scenario;
-    if (ctx->drain.nfail[s]) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u leaves %u evicted pods unscheduled", s, ctx->drain.nfail[s]);
-    if (ctx->drain.boff[s + 1] > ctx->drain.boff[s])
-        return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u has %u blocked pods", s, ctx->drain.boff[s + 1] - ctx->drain.boff[s]);
-    if (ctx->drain.voff[s + 1] > ctx->drain.voff[s])
-        return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u violates %u PDBs", s, ctx->drain.voff[s + 1] - ctx->drain.voff[s]);
-    CU(cudaSetDevice(ctx->device));
-    ScenPool &S = ctx->single, &B = ctx->batch;
-    cudaStream_t st = ctx->stream;
-    const uint32_t N1 = std::max(1u, ctx->snap.N);
-    // ---- on the host: the evicted pods' new nodes; the returned nodes (the scenario's removed ones) and
-    // their DaemonSet pods (its vanished pods), grouped by node, pod order kept ----
-    const uint32_t b = ctx->drain.off[s], ne = ctx->drain.off[s + 1] - b;
-    std::vector<int32_t> node(ne);
-    if (ne) CU(cudaMemcpy(node.data(), ctx->drain.d_node.p + b, 4ull * ne, cudaMemcpyDeviceToHost));
-    std::vector<uint32_t> nodes(ctx->wave.removed.begin() + ctx->wave.roff[s], ctx->wave.removed.begin() + ctx->wave.roff[s + 1]);
-    std::vector<uint32_t> off(1, 0u), pods;
-    {
-        std::vector<uint32_t> cnt(N1, 0u), at(N1, 0u);
-        for (uint32_t k = ctx->wave.voff[s]; k < ctx->wave.voff[s + 1]; k++) cnt[ctx->wave.place[ctx->wave.vanished[k]]]++;
-        for (uint32_t g : nodes) { at[g] = off.back(); off.push_back(off.back() + cnt[g]); }
-        pods.resize(off.back());
-        for (uint32_t k = ctx->wave.voff[s]; k < ctx->wave.voff[s + 1]; k++) {
-            const uint32_t q = ctx->wave.vanished[k];
-            pods[at[ctx->wave.place[q]]++] = q;
-        }
-    }
-    // ---- on the device, timed: the slot's state into the base, the scatter, the return ----
-    CU(ctx->wave.d_nodes.upload(nodes.data(), nodes.size(), st));
-    CU(ctx->wave.d_off.upload(off.data(), off.size(), st));
-    CU(ctx->wave.d_pods.upload(pods.data(), pods.size(), st));
-    CU(cudaEventRecord(ctx->ev0, st));
-    CU(S.state.each(B.state, true, [&](auto &d, auto &c, uint64_t k) {
-        return cudaMemcpyAsync(d.p, c.p + (size_t)s * k, k * sizeof(*d.p), cudaMemcpyDeviceToDevice, st);
-    }));
-    if (ne) {
-        const uint32_t grid = std::min<uint32_t>((ne + 255) / 256, (uint32_t)ctx->sms * 4);
-        simon_wave_scatter<<<grid, 256, 0, st>>>(ctx->drain.d_pods.p + b, ctx->drain.d_node.p + b, ctx->drain.d_gpu.p + b, ne, S.out_node.p,
-                                                 S.out_gpu.p);
-        CU(cudaGetLastError());
-        ctx->launches++;
-    }
-    if (!nodes.empty()) {
-        SkParams Ps;
-        fill_params(ctx, S, Ps);
-        simon_wave_return<<<((uint32_t)nodes.size() + 127) / 128, 128, 0, st>>>(Ps, ctx->wave.d_nodes.p, ctx->wave.d_off.p, ctx->wave.d_pods.p,
-                                                                                 (uint32_t)nodes.size());
-        CU(cudaGetLastError());
-        ctx->launches++;
-    }
-    CU(cudaEventRecord(ctx->ev1, st));
-    // the mirror's slot words: the evicted pods' and the returned DaemonSet pods' changed
-    if (ctx->pods.n_pods) CU(cudaMemcpyAsync(ctx->wave.slots.data(), S.out_gpu.p, 4ull * ctx->pods.n_pods, cudaMemcpyDeviceToHost, st));
-    const cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
-    CU(cudaEventElapsedTime(&ctx->wave.commit_ms, ctx->ev0, ctx->ev1));
-    ctx->last_ms = ctx->wave.commit_ms;
-    for (uint32_t i = 0; i < ne; i++) ctx->wave.place[ctx->drain.pods[b + i]] = node[i];
-    // the batch's slots describe the old base: no other scenario of it may be committed
-    ctx->valid.drop(WAVE_BATCH);
-    return SIMON_OK;
-}
-
-extern "C" int simon_wave_commit_retire(simon_ctx *ctx, uint32_t scenario) {
-    if (!ctx) return SIMON_ERR_INVALID;
-    if (!ctx->valid.has(WAVE_BASE)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_commit_retire without a wave base (simon_wave_begin)");
-    if (!ctx->valid.has(WAVE_BATCH)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_commit_retire: no wave batch since the base changed");
-    if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u of a batch of %u", scenario, ctx->drain.n);
-    const uint32_t s = scenario;
+// simon_wave_commit (retire false: the scenario's removed nodes return with their DaemonSet pods) and simon_wave_commit_retire (retire:
+// its joined nodes become present, and the present nodes it removed retire; their DaemonSet pods, placed or pending, stop existing)
+static int wave_commit(simon_ctx *ctx, uint32_t s, bool retire) {
+    const char *what = retire ? "simon_wave_commit_retire" : "simon_wave_commit";
+    if (!ctx->valid.has(WAVE_BASE)) return fail(ctx, SIMON_ERR_STATE, "%s without a wave base (simon_wave_begin)", what);
+    if (!ctx->valid.has(WAVE_BATCH))
+        return fail(ctx, SIMON_ERR_STATE, "%s: no %s batch since the base changed", what, retire ? "wave" : "simon_wave_run");
+    if (s >= ctx->bout.n) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u of a batch of %u", s, ctx->bout.n);
+    if (!retire && ctx->wave.joined) return fail(ctx, SIMON_ERR_INVALID, "simon_wave_commit: the last wave batch joined nodes (simon_wave_commit_retire)");
     if (ctx->drain.nfail[s]) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u leaves %u evicted pods unscheduled", s, ctx->drain.nfail[s]);
     if (ctx->wave.jfail[s]) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u leaves %u join pods unscheduled", s, ctx->wave.jfail[s]);
     if (ctx->drain.boff[s + 1] > ctx->drain.boff[s])
@@ -2046,91 +2039,102 @@ extern "C" int simon_wave_commit_retire(simon_ctx *ctx, uint32_t scenario) {
     CU(cudaSetDevice(ctx->device));
     ScenPool &S = ctx->single, &B = ctx->batch;
     cudaStream_t st = ctx->stream;
-    // ---- on the host: the scenario's device list (join pods, then evicted pods) and their nodes; the retired nodes (the present nodes
-    // it removed) and their DaemonSet pods (its vanished pods), which stop existing ----
+    const uint32_t N1 = std::max(1u, ctx->snap.N);
+    // ---- on the host: the scenario's device list (join pods, then evicted pods) and their nodes; the nodes reset to empty (those it
+    // removed; retiring, the present ones) and its vanished pods, which return to them grouped by node, pod order kept, or, retiring,
+    // stop existing with the retired nodes' pending DaemonSet pods ----
     const uint32_t b = ctx->wave.dstart[s], nl = ctx->wave.dstart[s + 1] - b;
-    std::vector<uint32_t> list(nl);
+    std::vector<uint32_t> list(ctx->wave.jpods.begin() + ctx->wave.joff[s], ctx->wave.jpods.begin() + ctx->wave.joff[s + 1]);
+    list.insert(list.end(), ctx->drain.pods.begin() + ctx->drain.off[s], ctx->drain.pods.begin() + ctx->drain.off[s + 1]);
     std::vector<int32_t> node(nl);
-    if (nl) {
-        CU(cudaMemcpy(list.data(), ctx->drain.d_pods.p + b, 4ull * nl, cudaMemcpyDeviceToHost));
-        CU(cudaMemcpy(node.data(), ctx->drain.d_node.p + b, 4ull * nl, cudaMemcpyDeviceToHost));
-    }
-    std::vector<uint32_t> gone;
+    if (nl) CU(cudaMemcpy(node.data(), ctx->bout.d_node.p + b, 4ull * nl, cudaMemcpyDeviceToHost));
+    std::vector<uint32_t> nodes;
     for (uint32_t k = ctx->wave.roff[s]; k < ctx->wave.roff[s + 1]; k++)
-        if (ctx->wave.present[ctx->wave.removed[k]] == 1) gone.push_back(ctx->wave.removed[k]);
-    std::vector<uint32_t> van(ctx->wave.vanished.begin() + ctx->wave.voff[s], ctx->wave.vanished.begin() + ctx->wave.voff[s + 1]);
-    {
-        // the retired nodes' DaemonSet pods that were pending in the base stop existing too
-        std::vector<uint8_t> retiring(std::max(1u, ctx->snap.N), 0u);
-        for (uint32_t g : gone) retiring[g] = 1;
+        if (!retire || ctx->wave.present[ctx->wave.removed[k]] == 1) nodes.push_back(ctx->wave.removed[k]);
+    std::vector<uint32_t> pods(ctx->wave.vanished.begin() + ctx->wave.voff[s], ctx->wave.vanished.begin() + ctx->wave.voff[s + 1]);
+    std::vector<uint32_t> off(nodes.size() + 1, 0u);
+    if (retire) {
+        std::vector<uint8_t> retiring(N1, 0u);
+        for (uint32_t g : nodes) retiring[g] = 1;
         for (uint32_t q = 0; q < ctx->pods.n_pods; q++)
-            if (ctx->pods.h_guard[q] >= 0 && retiring[ctx->pods.h_guard[q]] && ctx->wave.place[q] == -1) van.push_back(q);
+            if (ctx->pods.h_guard[q] >= 0 && retiring[ctx->pods.h_guard[q]] && ctx->wave.place[q] == -1) pods.push_back(q);
+    } else {
+        std::vector<uint32_t> cnt(N1, 0u), at(N1, 0u), back(pods.size());
+        for (uint32_t q : pods) cnt[ctx->wave.place[q]]++;
+        for (size_t k = 0; k < nodes.size(); k++) { at[nodes[k]] = off[k]; off[k + 1] = off[k] + cnt[nodes[k]]; }
+        for (uint32_t q : pods) back[at[ctx->wave.place[q]]++] = q;
+        pods.swap(back);
     }
-    std::vector<int32_t> van_node(van.size(), -3);
-    std::vector<uint32_t> van_gpu(van.size(), 0u), off(gone.size() + 1, 0u);
-    // ---- on the device, timed: the slot's state into the base, the scatter of the placed pods and of the pods that stop existing, the
-    // retired nodes reset to empty.  The reset reuses simon_wave_return with no pods to add back: its first part is exactly the reset,
-    // and nothing returns ----
-    CU(ctx->wave.d_nodes.upload(gone.data(), gone.size(), st));
+    // ---- on the device, timed: the slot's state into the base, the scatter of the device list and of the pods that stop existing (to
+    // -3, without GPU slots), the reset nodes emptied and given back their returning pods ----
+    const size_t n_gone = retire ? pods.size() : 0;
+    const std::vector<int32_t> gone_node(n_gone, -3);
+    const std::vector<uint32_t> gone_gpu(n_gone, 0u);
+    CU(ctx->wave.d_nodes.upload(nodes.data(), nodes.size(), st));
     CU(ctx->wave.d_off.upload(off.data(), off.size(), st));
-    CU(ctx->wave.d_pods.upload(van.data(), van.size(), st));
-    CU(ctx->wave.d_vnode.upload(van_node.data(), van_node.size(), st));
-    CU(ctx->wave.d_vgpu.upload(van_gpu.data(), van_gpu.size(), st));
+    CU(ctx->wave.d_pods.upload(pods.data(), pods.size(), st));
+    CU(ctx->wave.d_vnode.upload(gone_node.data(), n_gone, st));
+    CU(ctx->wave.d_vgpu.upload(gone_gpu.data(), n_gone, st));
     CU(cudaEventRecord(ctx->ev0, st));
     CU(S.state.each(B.state, true, [&](auto &d, auto &c, uint64_t k) {
         return cudaMemcpyAsync(d.p, c.p + (size_t)s * k, k * sizeof(*d.p), cudaMemcpyDeviceToDevice, st);
     }));
-    auto scatter = [&](const uint32_t *pods, const int32_t *nd, const uint32_t *gpu, uint32_t cnt) -> cudaError_t {
+    auto scatter = [&](const uint32_t *p, const int32_t *nd, const uint32_t *gpu, uint32_t cnt) -> cudaError_t {
         if (!cnt) return cudaSuccess;
         const uint32_t grid = std::min<uint32_t>((cnt + 255) / 256, (uint32_t)ctx->sms * 4);
-        simon_wave_scatter<<<grid, 256, 0, st>>>(pods, nd, gpu, cnt, S.out_node.p, S.out_gpu.p);
+        simon_wave_scatter<<<grid, 256, 0, st>>>(p, nd, gpu, cnt, S.out_node.p, S.out_gpu.p);
         ctx->launches++;
         return cudaGetLastError();
     };
-    CU(scatter(ctx->drain.d_pods.p + b, ctx->drain.d_node.p + b, ctx->drain.d_gpu.p + b, nl));
-    CU(scatter(ctx->wave.d_pods.p, ctx->wave.d_vnode.p, ctx->wave.d_vgpu.p, (uint32_t)van.size()));
-    if (!gone.empty()) {
+    CU(scatter(ctx->drain.d_pods.p + b, ctx->bout.d_node.p + b, ctx->bout.d_gpu.p + b, nl));
+    CU(scatter(ctx->wave.d_pods.p, ctx->wave.d_vnode.p, ctx->wave.d_vgpu.p, (uint32_t)n_gone));
+    if (!nodes.empty()) {
         SkParams Ps;
         fill_params(ctx, S, Ps);
-        simon_wave_return<<<((uint32_t)gone.size() + 127) / 128, 128, 0, st>>>(Ps, ctx->wave.d_nodes.p, ctx->wave.d_off.p, ctx->wave.d_pods.p,
-                                                                                (uint32_t)gone.size());
+        simon_wave_return<<<((uint32_t)nodes.size() + 127) / 128, 128, 0, st>>>(Ps, ctx->wave.d_nodes.p, ctx->wave.d_off.p, ctx->wave.d_pods.p,
+                                                                                 (uint32_t)nodes.size());
         CU(cudaGetLastError());
         ctx->launches++;
     }
     CU(cudaEventRecord(ctx->ev1, st));
+    // the mirror's slot words: the device list's and the returned DaemonSet pods' changed
     if (ctx->pods.n_pods) CU(cudaMemcpyAsync(ctx->wave.slots.data(), S.out_gpu.p, 4ull * ctx->pods.n_pods, cudaMemcpyDeviceToHost, st));
     const cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
     CU(cudaEventElapsedTime(&ctx->wave.commit_ms, ctx->ev0, ctx->ev1));
     ctx->last_ms = ctx->wave.commit_ms;
     for (uint32_t k = 0; k < nl; k++) ctx->wave.place[list[k]] = node[k];
-    for (uint32_t q : van) ctx->wave.place[q] = -3;
-    for (uint32_t k = ctx->wave.jnoff[s]; k < ctx->wave.jnoff[s + 1]; k++) ctx->wave.present[ctx->wave.jnodes[k]] = 1;
-    for (uint32_t g : gone) ctx->wave.present[g] = 2;
+    if (retire) {
+        for (uint32_t q : pods) ctx->wave.place[q] = -3;
+        for (uint32_t k = ctx->wave.jnoff[s]; k < ctx->wave.jnoff[s + 1]; k++) ctx->wave.present[ctx->wave.jnodes[k]] = 1;
+        for (uint32_t g : nodes) ctx->wave.present[g] = 2;
+    }
+    // the batch's slots describe the old base: no other scenario of it may be committed
     ctx->valid.drop(WAVE_BATCH);
     return SIMON_OK;
+}
+
+extern "C" int simon_wave_commit(simon_ctx *ctx, uint32_t scenario) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    return wave_commit(ctx, scenario, false);
+}
+
+extern "C" int simon_wave_commit_retire(simon_ctx *ctx, uint32_t scenario) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    return wave_commit(ctx, scenario, true);
 }
 
 extern "C" int simon_wave_join_download(simon_ctx *ctx, uint32_t scenario, uint32_t *join_pod, int32_t *node, uint32_t *gpu_slots, int64_t *score,
                                         uint32_t *fail_counts, uint32_t *fail_pod) {
     if (!ctx) return SIMON_ERR_INVALID;
     if (!ctx->valid.has(WAVE_BATCH)) return fail(ctx, SIMON_ERR_STATE, "simon_wave_join_download: no wave batch since the base changed");
-    if (scenario >= ctx->drain.n) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u of a batch of %u", scenario, ctx->drain.n);
+    if (scenario >= ctx->bout.n) return fail(ctx, SIMON_ERR_INVALID, "wave scenario %u of a batch of %u", scenario, ctx->bout.n);
     CU(cudaSetDevice(ctx->device));
-    const uint32_t h = ctx->wave.joff[scenario], nj = ctx->wave.joff[scenario + 1] - h, b = ctx->wave.dstart[scenario];
+    const uint32_t h = ctx->wave.joff[scenario], nj = ctx->wave.joff[scenario + 1] - h;
     const uint32_t nf = std::min(ctx->wave.jfail[scenario], ctx->drain.max);
     if (join_pod) std::copy(ctx->wave.jpods.begin() + h, ctx->wave.jpods.begin() + h + nj, join_pod);
-    if (node && nj) CU(cudaMemcpy(node, ctx->drain.d_node.p + b, 4ull * nj, cudaMemcpyDeviceToHost));
-    if (gpu_slots && nj) CU(cudaMemcpy(gpu_slots, ctx->drain.d_gpu.p + b, 4ull * nj, cudaMemcpyDeviceToHost));
-    if (score && nj) {
-        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(cudaMemcpy(score, ctx->drain.d_score.p + b, 8ull * nj, cudaMemcpyDeviceToHost));
-        else memset(score, 0, 8ull * nj);
-    }
-    if (fail_counts && nf)
-        CU(cudaMemcpy(fail_counts, ctx->drain.d_fail_counts.p + (size_t)scenario * ctx->drain.max * SIMON_N_FAIL_CODES,
-                      4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
-    if (fail_pod && nf) CU(cudaMemcpy(fail_pod, ctx->drain.d_fail_pod.p + (size_t)scenario * ctx->drain.max, 4ull * nf, cudaMemcpyDeviceToHost));
-    return SIMON_OK;
+    const int rc = batch_download(ctx, ctx->wave.dstart[scenario], nj, node, gpu_slots, score);
+    return rc ? rc : batch_fail_download(ctx, (size_t)scenario * ctx->drain.max, nf, fail_counts, fail_pod);
 }
 
 extern "C" int simon_wave_presence(simon_ctx *ctx, uint8_t *state) {
@@ -2179,32 +2183,16 @@ extern "C" int simon_probe_run(simon_ctx *ctx, const int32_t *placed, const simo
         any_local |= ctx->valid.has(STORAGE) && ctx->storage.h_class_local[ctx->pods.h_class[q]];
     }
     if (out_local && !ctx->valid.has(STORAGE)) return fail(ctx, SIMON_ERR_STATE, "simon_probe_run: out_local without simon_storage_upload");
-    CU(cudaSetDevice(ctx->device));
-    {
-        // the per-replica outputs (node, GPU slots, score: 16 B per replica) and one failure record per probe
-        size_t fr = 0, tot = 0;
-        CU(cudaMemGetInfo(&fr, &tot));
-        const uint64_t held = 16ull * ctx->probe.d_node.cap;
-        const uint64_t need = 16ull * total + (4ull * SIMON_N_FAIL_CODES + 16) * n;
-        if (total >= (1ull << 32) || need > (uint64_t)fr + held)
-            return fail(ctx, SIMON_ERR_LIMIT, "simon_probe_run: outputs of %llu replicas (%llu bytes) do not fit the device (%llu bytes free)",
-                        (unsigned long long)total, (unsigned long long)need, (unsigned long long)fr);
-    }
-    ctx->last_launch = simon_launch_info{};
-    // the batch pool is no longer a drain or grow batch's, nor are its Open-Local slices another storage batch's
-    ctx->valid.drop(DRAIN_BATCH | WAVE_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
-    if (n == 0) return SIMON_OK;
+    rc = batch_begin(ctx);
+    if (rc || n == 0) return rc;
     cudaStream_t st = ctx->stream;
     ScenPool &B = ctx->batch;
     const bool storage = ctx->valid.has(STORAGE);
     // ---- geometry, the batch pool and the outputs (allocations before the timed work): every probe runs on all nodes in index order,
-    // the order of the live run ----
-    uint32_t CS, TPB, NPT;
-    size_t smem;
+    // the order of the live run; its replicas' outputs max_replicas apart, one failure record each ----
+    Geometry g;
     const Family fam = any_local ? PROBE_LOCAL : PROBE;
-    rc = choose_geometry(ctx, N, CS, TPB, NPT, smem, n, fam);
-    if (rc) return rc;
-    rc = size_pool(ctx, B, n, false, false);
+    rc = batch_pool(ctx, N, n, fam, g);
     if (rc) return rc;
     std::vector<uint32_t> pods(n);
     ctx->probe.off.assign(n + 1, 0u);
@@ -2214,38 +2202,22 @@ extern "C" int simon_probe_run(simon_ctx *ctx, const int32_t *placed, const simo
     }
     CU(ctx->probe.d_pod.upload(pods.data(), n, st));
     CU(ctx->probe.d_off.upload(ctx->probe.off.data(), n + 1, st));
-    CU(ctx->probe.d_node.alloc(total)); CU(ctx->probe.d_gpu.alloc(total));
-    if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(ctx->probe.d_score.alloc(total));
-    CU(ctx->probe.d_fail_counts.alloc((size_t)n * SIMON_N_FAIL_CODES)); CU(ctx->probe.d_fail_pod.alloc(n));
     std::vector<SkScenario> h(n);
-    for (uint32_t i = 0; i < n; i++) {
-        h[i] = fill_scen(B, i, N, true);
-        h[i].out_node = ctx->probe.d_node.p; h[i].out_gpu = ctx->probe.d_gpu.p;
-        h[i].out_score = (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) ? ctx->probe.d_score.p : nullptr;
-        h[i].fail_counts = ctx->probe.d_fail_counts.p + (size_t)i * SIMON_N_FAIL_CODES;
-        h[i].fail_pod = ctx->probe.d_fail_pod.p + i;
-    }
-    CU(B.scen.upload(h.data(), n, st));
+    for (uint32_t i = 0; i < n; i++) h[i] = fill_scen(B, i, N, true);
+    char outputs[96];
+    snprintf(outputs, sizeof(outputs), "simon_probe_run: outputs of %llu replicas", (unsigned long long)total);
+    rc = batch_outputs(ctx, n, total, 0, 1, h, outputs);
+    if (rc) return rc;
     // ---- setup: the live state in every slot, with its Open-Local state when storage is uploaded (live_batch_setup) ----
     SkParams Pb;
-    rc = live_batch_setup(ctx, placed, P, n, storage, ctx->probe.d_fail_counts.p, (size_t)n * SIMON_N_FAIL_CODES, Pb);
+    rc = live_batch_setup(ctx, placed, P, n, storage, Pb);
     if (rc) return rc;
-    CU(cudaEventRecord(ctx->evm, st));
-    // ---- placement of every probe's replicas, one failure record each ----
+    // ---- placement of every probe's replicas ----
     Pb.probe_pod = ctx->probe.d_pod.p; Pb.probe_off = ctx->probe.d_off.p;
-    Pb.first = 0; Pb.count = 0; Pb.max_fail = 1; Pb.npt = NPT;
-    rc = launch(ctx, Pb, n, CS, TPB, smem, false, fam);
-    if (rc) return rc;
-    CU(cudaEventRecord(ctx->ev1, st));
     std::vector<simon_scenario_result> res;
-    rc = live_batch_reduce(ctx, n, out_local != nullptr, res, out_local);
+    rc = batch_place(ctx, Pb, n, g, fam, true, storage, res, out_local, ctx->probe.setup_ms, ctx->probe.place_ms);
     if (rc) return rc;
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
     ctx->valid.set(LIVE);
-    CU(cudaEventElapsedTime(&ctx->probe.setup_ms, ctx->ev0, ctx->evm));
-    CU(cudaEventElapsedTime(&ctx->probe.place_ms, ctx->evm, ctx->ev1));
-    CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     ctx->probe.placed.resize(n);
     for (uint32_t i = 0; i < n; i++) {
         simon_probe_result &o = out[i];
@@ -2254,34 +2226,20 @@ extern "C" int simon_probe_run(simon_ctx *ctx, const int32_t *placed, const simo
         o.req_mcpu = res[i].req_mcpu; o.alloc_mcpu = res[i].alloc_mcpu; o.req_mem = res[i].req_mem; o.alloc_mem = res[i].alloc_mem;
         ctx->probe.placed[i] = o.n_placed;
     }
-    ctx->probe.n = n;
     ctx->valid.set(PROBE_BATCH);
-    if (storage) {
-        ctx->storage_batch.n = n;           // simon_scenarios_storage_download serves this batch
-        ctx->valid.set(STORAGE_BATCH);
-    }
     return SIMON_OK;
 }
 
 extern "C" int simon_probe_download(simon_ctx *ctx, uint32_t probe, int32_t *node, uint32_t *gpu_slots, int64_t *score, uint32_t *fail_counts) {
     if (!ctx) return SIMON_ERR_INVALID;
     if (!ctx->valid.has(PROBE_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_probe_run batch since the last upload, or a drain batch after it");
-    if (probe >= ctx->probe.n) return fail(ctx, SIMON_ERR_INVALID, "probe %u of a batch of %u", probe, ctx->probe.n);
+    if (probe >= ctx->bout.n) return fail(ctx, SIMON_ERR_INVALID, "probe %u of a batch of %u", probe, ctx->bout.n);
     CU(cudaSetDevice(ctx->device));
     const uint32_t b = ctx->probe.off[probe], k = ctx->probe.placed[probe];
     const bool stopped = k < ctx->probe.off[probe + 1] - b;          // Unschedulable: its failure record was written
-    if (node && k) CU(cudaMemcpy(node, ctx->probe.d_node.p + b, 4ull * k, cudaMemcpyDeviceToHost));
-    if (gpu_slots && k) CU(cudaMemcpy(gpu_slots, ctx->probe.d_gpu.p + b, 4ull * k, cudaMemcpyDeviceToHost));
-    if (score && k) {
-        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(cudaMemcpy(score, ctx->probe.d_score.p + b, 8ull * k, cudaMemcpyDeviceToHost));
-        else memset(score, 0, 8ull * k);
-    }
-    if (fail_counts) {
-        if (stopped) CU(cudaMemcpy(fail_counts, ctx->probe.d_fail_counts.p + (size_t)probe * SIMON_N_FAIL_CODES, 4ull * SIMON_N_FAIL_CODES,
-                                   cudaMemcpyDeviceToHost));
-        else memset(fail_counts, 0, 4ull * SIMON_N_FAIL_CODES);
-    }
-    return SIMON_OK;
+    if (fail_counts && !stopped) memset(fail_counts, 0, 4ull * SIMON_N_FAIL_CODES);
+    const int rc = batch_download(ctx, b, k, node, gpu_slots, score);
+    return rc ? rc : batch_fail_download(ctx, probe, stopped ? 1u : 0u, fail_counts, nullptr);
 }
 
 extern "C" int simon_probe_times(simon_ctx *ctx, float *setup_ms, float *place_ms) {
@@ -2326,79 +2284,37 @@ extern "C" int simon_grow_run(simon_ctx *ctx, const int32_t *placed, uint32_t n_
     }
     if (out_local && !ctx->valid.has(STORAGE)) return fail(ctx, SIMON_ERR_STATE, "simon_grow_run: out_local without simon_storage_upload");
     const uint32_t T = P - n_prefix;
-    CU(cudaSetDevice(ctx->device));
-    {
-        // the per-tail-pod outputs (node, GPU slots, score: 16 B per pod and scenario) and one failure record per tail pod and scenario
-        size_t fr = 0, tot = 0;
-        CU(cudaMemGetInfo(&fr, &tot));
-        const uint64_t cells = (uint64_t)n * T + n_prefix;
-        const uint64_t held = 16ull * ctx->grow.d_node.cap + (4ull * SIMON_N_FAIL_CODES + 4) * ctx->grow.d_fail_pod.cap;
-        const uint64_t need = 16ull * cells + (4ull * SIMON_N_FAIL_CODES + 4) * n * T;
-        if (cells >= (1ull << 32) || need > (uint64_t)fr + held)
-            return fail(ctx, SIMON_ERR_LIMIT, "simon_grow_run: outputs of %u scenarios x %u tail pods (%llu bytes) do not fit the device (%llu bytes free)",
-                        n, T, (unsigned long long)need, (unsigned long long)fr);
-    }
-    ctx->last_launch = simon_launch_info{};
-    // the batch pool is no longer a drain or probe batch's, nor are its Open-Local slices another storage batch's
-    ctx->valid.drop(DRAIN_BATCH | WAVE_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
-    if (n == 0) return SIMON_OK;
-    cudaStream_t st = ctx->stream;
-    ScenPool &B = ctx->batch;
+    rc = batch_begin(ctx);
+    if (rc || n == 0) return rc;
     const bool storage = ctx->valid.has(STORAGE);
-    // ---- geometry of the batch placement variants, the batch pool and the outputs (allocations before the timed work) ----
-    uint32_t CS, TPB, NPT;
-    size_t smem;
-    rc = choose_geometry(ctx, max_active, CS, TPB, NPT, smem, n);
+    // ---- geometry of the batch placement variants, the batch pool and the outputs (allocations before the timed work): tail failure
+    // records per scenario ----
+    Geometry g;
+    rc = batch_pool(ctx, max_active, n, PLACE, g);
     if (rc) return rc;
-    rc = size_pool(ctx, B, n, false, false);
-    if (rc) return rc;
-    const size_t cells = (size_t)n * T + n_prefix, rows = std::max<size_t>(1, (size_t)n * T);
-    const bool scores = ctx->opt_flags & SIMON_OPT_RECORD_SCORES;
-    CU(ctx->grow.d_node.alloc(cells)); CU(ctx->grow.d_gpu.alloc(cells));
-    if (scores) CU(ctx->grow.d_score.alloc(cells));
-    CU(ctx->grow.d_fail_counts.alloc(rows * SIMON_N_FAIL_CODES)); CU(ctx->grow.d_fail_pod.alloc(rows));
     std::vector<SkScenario> h;
     CU(batch_scenarios(ctx, scen, n, h));
-    for (uint32_t i = 0; i < n; i++) {
-        const size_t base = (size_t)i * T;
-        h[i].out_node = ctx->grow.d_node.p + base; h[i].out_gpu = ctx->grow.d_gpu.p + base;
-        h[i].out_score = scores ? ctx->grow.d_score.p + base : nullptr;
-        h[i].fail_counts = ctx->grow.d_fail_counts.p + base * SIMON_N_FAIL_CODES;
-        h[i].fail_pod = ctx->grow.d_fail_pod.p + base;
-    }
-    CU(B.scen.upload(h.data(), n, st));
+    char outputs[96];
+    snprintf(outputs, sizeof(outputs), "simon_grow_run: outputs of %u scenarios x %u tail pods", n, T);
+    rc = batch_outputs(ctx, n, (uint64_t)n * T + n_prefix, T, T, h, outputs);
+    if (rc) return rc;
     // ---- setup: the live state of the prefix in every slot, with its Open-Local state when storage is uploaded ----
     SkParams Pb;
-    rc = live_batch_setup(ctx, placed, n_prefix, n, storage, ctx->grow.d_fail_counts.p, rows * SIMON_N_FAIL_CODES, Pb);
+    rc = live_batch_setup(ctx, placed, n_prefix, n, storage, Pb);
     if (rc) return rc;
-    CU(cudaEventRecord(ctx->evm, st));
     // ---- placement of every scenario's tail, on its active nodes ----
-    if (T) {
-        Pb.first = n_prefix; Pb.count = T; Pb.max_fail = T; Pb.npt = NPT;
-        rc = launch(ctx, Pb, n, CS, TPB, smem, false);
-        if (rc) return rc;
-    }
-    CU(cudaEventRecord(ctx->ev1, st));
+    Pb.first = n_prefix; Pb.count = T;
     std::vector<simon_scenario_result> res;
-    rc = live_batch_reduce(ctx, n, out_local != nullptr, res, out_local);
+    rc = batch_place(ctx, Pb, n, g, PLACE, T > 0, storage, res, out_local, ctx->grow.setup_ms, ctx->grow.place_ms);
     if (rc) return rc;
-    cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return fail(ctx, SIMON_ERR_CUDA, "kernel failed: %s", cudaGetErrorString(e));
     ctx->valid.set(LIVE);
-    CU(cudaEventElapsedTime(&ctx->grow.setup_ms, ctx->ev0, ctx->evm));
-    CU(cudaEventElapsedTime(&ctx->grow.place_ms, ctx->evm, ctx->ev1));
-    CU(cudaEventElapsedTime(&ctx->last_ms, ctx->ev0, ctx->ev1));
     ctx->grow.nfail.resize(n);
     for (uint32_t i = 0; i < n; i++) {
         out[i] = res[i];
         ctx->grow.nfail[i] = res[i].n_unscheduled;
     }
-    ctx->grow.n = n; ctx->grow.n_prefix = n_prefix; ctx->grow.tail = T;
+    ctx->grow.n_prefix = n_prefix; ctx->grow.tail = T;
     ctx->valid.set(GROW_BATCH);
-    if (storage) {
-        ctx->storage_batch.n = n;           // simon_scenarios_storage_download serves this batch
-        ctx->valid.set(STORAGE_BATCH);
-    }
     return SIMON_OK;
 }
 
@@ -2406,20 +2322,11 @@ extern "C" int simon_grow_download(simon_ctx *ctx, uint32_t scenario, int32_t *n
                                    uint32_t *fail_counts, uint32_t *fail_pod) {
     if (!ctx) return SIMON_ERR_INVALID;
     if (!ctx->valid.has(GROW_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_grow_run batch since the last upload, or a drain or probe batch after it");
-    if (scenario >= ctx->grow.n) return fail(ctx, SIMON_ERR_INVALID, "grow scenario %u of a batch of %u", scenario, ctx->grow.n);
+    if (scenario >= ctx->bout.n) return fail(ctx, SIMON_ERR_INVALID, "grow scenario %u of a batch of %u", scenario, ctx->bout.n);
     CU(cudaSetDevice(ctx->device));
     const uint32_t T = ctx->grow.tail, nf = std::min(ctx->grow.nfail[scenario], T);
-    const size_t at = (size_t)scenario * T + ctx->grow.n_prefix, base = (size_t)scenario * T;
-    if (node && T) CU(cudaMemcpy(node, ctx->grow.d_node.p + at, 4ull * T, cudaMemcpyDeviceToHost));
-    if (gpu_slots && T) CU(cudaMemcpy(gpu_slots, ctx->grow.d_gpu.p + at, 4ull * T, cudaMemcpyDeviceToHost));
-    if (score && T) {
-        if (ctx->opt_flags & SIMON_OPT_RECORD_SCORES) CU(cudaMemcpy(score, ctx->grow.d_score.p + at, 8ull * T, cudaMemcpyDeviceToHost));
-        else memset(score, 0, 8ull * T);
-    }
-    if (fail_counts && nf)
-        CU(cudaMemcpy(fail_counts, ctx->grow.d_fail_counts.p + base * SIMON_N_FAIL_CODES, 4ull * nf * SIMON_N_FAIL_CODES, cudaMemcpyDeviceToHost));
-    if (fail_pod && nf) CU(cudaMemcpy(fail_pod, ctx->grow.d_fail_pod.p + base, 4ull * nf, cudaMemcpyDeviceToHost));
-    return SIMON_OK;
+    const int rc = batch_download(ctx, (size_t)scenario * T + ctx->grow.n_prefix, T, node, gpu_slots, score);
+    return rc ? rc : batch_fail_download(ctx, (size_t)scenario * T, nf, fail_counts, fail_pod);
 }
 
 extern "C" int simon_grow_times(simon_ctx *ctx, float *setup_ms, float *place_ms) {

@@ -395,6 +395,34 @@ class Engine:
         self._check(lib().simon_drain_budget(self.h, C.byref(per), C.byref(free)))
         return int(per.value), int(free.value)
 
+    def _chunked(self, n: int, chunk: Optional[int], times, run, extra: int = 0):
+        """Entries [0, n) in batches of `chunk` entries, or of as many as fit: drain_budget()'s per-scenario bytes plus `extra` per
+        entry, in DRAIN_MEM_FRACTION of the free bytes.  run(b, m) runs entries [b, b + m) as one batch and returns their dicts; after
+        it, times(h, &setup_ms, &place_ms) reads the batch's device times.  -> (the dicts of every entry, dict(chunks,
+        scenario_bytes, chunk, setup_ms / place_ms summed over the batches, launches: last_launch() of each batch))."""
+        per, free = self.drain_budget()
+        per += extra
+        if chunk is None:
+            chunk = max(1, int(free * self.DRAIN_MEM_FRACTION) // max(per, 1))
+        out = []
+        info = dict(chunks=0, scenario_bytes=per, chunk=chunk, setup_ms=0.0, place_ms=0.0, launches=[])
+        for b in range(0, n, chunk):
+            out.extend(run(b, min(chunk, n - b)))
+            su, pm = C.c_float(0), C.c_float(0)
+            self._check(times(self.h, C.byref(su), C.byref(pm)))
+            info["chunks"] += 1
+            info["setup_ms"] += float(su.value)
+            info["place_ms"] += float(pm.value)
+            info["launches"].append(self.last_launch())
+        return out, info
+
+    def _download(self, fn, i: int, *specs):
+        """fn(h, i, *arrays) into zero arrays, one per spec (rows, dtype) or (rows, dtype, columns), each at least one row long: -> the
+        arrays cut to their rows."""
+        arrs = [np.zeros((max(s[0], 1),) + tuple(s[2:]), s[1]) for s in specs]
+        self._check(fn(self.h, i, *[a.ctypes.data for a in arrs]))
+        return [a[:s[0]] for a, s in zip(arrs, specs)]
+
     def drain_run(self, placed, remain_lists: List[np.ndarray], detail: bool = True, chunk: Optional[int] = None, local: bool = False):
         """Drains on the live state `placed` (out_node of a full placement of the pod list): each entry of remain_lists lists the
         nodes that remain, in their nodeTree.list() order.  The list runs in batches (chunks) sized so that one batch's pooled state
@@ -410,30 +438,17 @@ class Engine:
         scenario_storage_state(i) then describes drain i of the last chunk."""
         L = lib()
         pl = np.ascontiguousarray(placed, dtype=np.int32)
-        n = len(remain_lists)
-        per, free = self.drain_budget()
-        if chunk is None:
-            chunk = max(1, int(free * self.DRAIN_MEM_FRACTION) // max(per, 1))
-        out = []
-        info = dict(chunks=0, scenario_bytes=per, chunk=chunk, setup_ms=0.0, place_ms=0.0, launches=[])
-        for b in range(0, n, chunk):
-            part = remain_lists[b:b + chunk]
-            m = len(part)
-            arr, keep = self._scenario_array(part)
+
+        def run(b, m):
+            arr, keep = self._scenario_array(remain_lists[b:b + m])
             res = (abi.SimonDrainResult * m)()
             if local:
                 loc = (abi.SimonScenarioLocalResult * m)()
                 self._check(L.simon_drain_run_local(self.h, pl.ctypes.data, arr, m, res, loc))
             else:
                 self._check(L.simon_drain_run(self.h, pl.ctypes.data, arr, m, res))
-            su, pm = C.c_float(0), C.c_float(0)
-            self._check(L.simon_drain_times(self.h, C.byref(su), C.byref(pm)))
-            info["chunks"] += 1
-            info["setup_ms"] += float(su.value)
-            info["place_ms"] += float(pm.value)
-            info["launches"].append(self.last_launch())
-            out.extend(self._drain_results(res, loc if local else None, detail))
-        self.last_drain = info
+            return self._drain_results(res, loc if local else None, detail)
+        out, self.last_drain = self._chunked(len(remain_lists), chunk, L.simon_drain_times, run)
         return out
 
     def _drain_results(self, res, loc, detail: bool) -> List[dict]:
@@ -447,22 +462,11 @@ class Engine:
             if loc is not None:
                 d["vg_requested"], d["vg_capacity"] = int(loc[i].vg_requested), int(loc[i].vg_capacity)
             if detail:
-                ne, nb, nf = r.n_evicted, r.n_blocked, r.n_unscheduled
-                ev = np.zeros(max(ne, 1), np.uint32)
-                node = np.zeros(max(ne, 1), np.int32)
-                slots = np.zeros(max(ne, 1), np.uint32)
-                score = np.zeros(max(ne, 1), np.int64)
-                blk = np.zeros(max(nb, 1), np.uint32)
-                fc = np.zeros((max(nf, 1), abi.N_FAIL_CODES), np.uint32)
-                fp = np.zeros(max(nf, 1), np.uint32)
-                self._check(L.simon_drain_download(self.h, i, ev.ctypes.data, node.ctypes.data, slots.ctypes.data, score.ctypes.data,
-                                                   blk.ctypes.data, fc.ctypes.data, fp.ctypes.data))
-                nv = r.n_pdb_violated
-                vp = np.zeros(max(nv, 1), np.uint32)
-                vc = np.zeros(max(nv, 1), np.uint32)
-                self._check(L.simon_drain_pdb_download(self.h, i, vp.ctypes.data, vc.ctypes.data))
-                d.update(evicted=ev[:ne], node=node[:ne], gpu_slots=slots[:ne], score=score[:ne], blocked=blk[:nb],
-                         fail_counts=fc[:nf], fail_pod=fp[:nf], pdb_violated=vp[:nv], pdb_evicted=vc[:nv])
+                ne, nb, nf, nv = r.n_evicted, r.n_blocked, r.n_unscheduled, r.n_pdb_violated
+                d.update(zip(("evicted", "node", "gpu_slots", "score", "blocked", "fail_counts", "fail_pod"),
+                             self._download(L.simon_drain_download, i, (ne, np.uint32), (ne, np.int32), (ne, np.uint32), (ne, np.int64),
+                                            (nb, np.uint32), (nf, np.uint32, abi.N_FAIL_CODES), (nf, np.uint32))))
+                d.update(zip(("pdb_violated", "pdb_evicted"), self._download(L.simon_drain_pdb_download, i, (nv, np.uint32), (nv, np.uint32))))
             out.append(d)
         return out
 
@@ -488,50 +492,33 @@ class Engine:
         n_join_placed, n_join_unscheduled and, with detail, join_pods, join_node, join_gpu_slots, join_score, join_fail_counts and
         join_fail_pod."""
         L = lib()
-        n = len(remain_lists)
-        if chunk is None:
-            per, free = self.drain_budget()
-            chunk = max(1, int(free * self.DRAIN_MEM_FRACTION) // max(per, 1))
-        out = []
-        for b in range(0, n, chunk):
-            part = remain_lists[b:b + chunk]
-            arr, keep = self._scenario_array(part)
-            res = (abi.SimonDrainResult * len(part))()
+
+        def run(b, m):
+            arr, keep = self._scenario_array(remain_lists[b:b + m])
+            res = (abi.SimonDrainResult * m)()
             if joins is None:
-                self._check(L.simon_wave_run(self.h, arr, len(part), res))
+                self._check(L.simon_wave_run(self.h, arr, m, res))
             else:
-                jarr, jkeep = self._scenario_array(joins[b:b + chunk])
-                jres = (abi.SimonJoinResult * len(part))()
-                self._check(L.simon_wave_run_join(self.h, arr, jarr, len(part), res, jres))
-            self._wave = (list(remain_lists), None if joins is None else list(joins), b, len(part))
-            su, pm, cm = C.c_float(0), C.c_float(0), C.c_float(0)
-            self._check(L.simon_wave_times(self.h, C.byref(su), C.byref(pm), C.byref(cm)))
-            self.last_wave["batches"] += 1
-            self.last_wave["setup_ms"] += float(su.value)
-            self.last_wave["place_ms"] += float(pm.value)
-            self.last_wave["launches"].append(self.last_launch())
+                jarr, jkeep = self._scenario_array(joins[b:b + m])
+                jres = (abi.SimonJoinResult * m)()
+                self._check(L.simon_wave_run_join(self.h, arr, jarr, m, res, jres))
+            self._wave = (list(remain_lists), None if joins is None else list(joins), b, m)
             part_out = self._drain_results(res, None, detail)
             if joins is not None:
                 for i, (d, r) in enumerate(zip(part_out, jres)):
-                    d.update(n_join=r.n_join, n_join_placed=r.n_placed, n_join_unscheduled=r.n_unscheduled)
+                    nj, nf = r.n_join, r.n_unscheduled
+                    d.update(n_join=nj, n_join_placed=r.n_placed, n_join_unscheduled=nf)
                     if detail:
-                        d.update(self._join_detail(i, r))
-            out.extend(part_out)
+                        d.update(zip(("join_pods", "join_node", "join_gpu_slots", "join_score", "join_fail_counts", "join_fail_pod"),
+                                     self._download(L.simon_wave_join_download, i, (nj, np.uint32), (nj, np.int32), (nj, np.uint32),
+                                                    (nj, np.int64), (nf, np.uint32, abi.N_FAIL_CODES), (nf, np.uint32))))
+            return part_out
+        out, info = self._chunked(len(remain_lists), chunk, lambda h, su, pm: L.simon_wave_times(h, su, pm, None), run)
+        self.last_wave["batches"] += info["chunks"]
+        self.last_wave["setup_ms"] += info["setup_ms"]
+        self.last_wave["place_ms"] += info["place_ms"]
+        self.last_wave["launches"] += info["launches"]
         return out
-
-    def _join_detail(self, i: int, r) -> dict:
-        """simon_wave_join_download of scenario i of the last wave batch, whose join counts are r."""
-        nj, nf = r.n_join, r.n_unscheduled
-        jp = np.zeros(max(nj, 1), np.uint32)
-        node = np.zeros(max(nj, 1), np.int32)
-        slots = np.zeros(max(nj, 1), np.uint32)
-        score = np.zeros(max(nj, 1), np.int64)
-        fc = np.zeros((max(nf, 1), abi.N_FAIL_CODES), np.uint32)
-        fp = np.zeros(max(nf, 1), np.uint32)
-        self._check(lib().simon_wave_join_download(self.h, i, jp.ctypes.data, node.ctypes.data, slots.ctypes.data, score.ctypes.data,
-                                                   fc.ctypes.data, fp.ctypes.data))
-        return dict(join_pods=jp[:nj], join_node=node[:nj], join_gpu_slots=slots[:nj], join_score=score[:nj], join_fail_counts=fc[:nf],
-                    join_fail_pod=fp[:nf])
 
     def wave_commit(self, i: int, retire: bool = False):
         """simon_wave_commit of entry i of the last wave_run's remain_lists: it becomes the next base.  When entry i was not in the last
@@ -586,27 +573,14 @@ class Engine:
                 raise RuntimeError(f"probe {i}: {P} pods + {r} replicas of pod {q} exceed its class's int32 bounds "
                                    f"({limit[int(cls[q])]} pods)")
         local = getattr(self.c, "storage", None) is not None
-        n = len(probes)
-        per, free = self.drain_budget()
-        if chunk is None:
-            chunk = max(1, int(free * self.DRAIN_MEM_FRACTION) // max(per, 1))
-        out = []
-        info = dict(chunks=0, scenario_bytes=per, chunk=chunk, setup_ms=0.0, place_ms=0.0, launches=[])
-        for b in range(0, max(n, 1), chunk):
-            part = probes[b:b + chunk]
-            m = len(part)
+
+        def run(b, m):
+            part = probes[b:b + m]
             arr = (abi.SimonProbe * max(m, 1))(*[abi.SimonProbe(q, r) for q, r in part])
             res = (abi.SimonProbeResult * max(m, 1))()
             loc = (abi.SimonScenarioLocalResult * max(m, 1))() if local else None
             self._check(L.simon_probe_run(self.h, pl.ctypes.data, arr, m, res, loc))
-            if m == 0:
-                break
-            su, pm = C.c_float(0), C.c_float(0)
-            self._check(L.simon_probe_times(self.h, C.byref(su), C.byref(pm)))
-            info["chunks"] += 1
-            info["setup_ms"] += float(su.value)
-            info["place_ms"] += float(pm.value)
-            info["launches"].append(self.last_launch())
+            out = []
             for i in range(m):
                 r = res[i]
                 d = dict(n_placed=r.n_placed, stop_reason=r.stop_reason, req_mcpu=r.req_mcpu, alloc_mcpu=r.alloc_mcpu,
@@ -615,14 +589,14 @@ class Engine:
                     d["vg_requested"], d["vg_capacity"] = int(loc[i].vg_requested), int(loc[i].vg_capacity)
                 if detail:
                     k = r.n_placed
-                    node = np.zeros(max(k, 1), np.int32)
-                    slots = np.zeros(max(k, 1), np.uint32)
-                    score = np.zeros(max(k, 1), np.int64)
-                    fc = np.zeros(abi.N_FAIL_CODES, np.uint32)
-                    self._check(L.simon_probe_download(self.h, i, node.ctypes.data, slots.ctypes.data, score.ctypes.data, fc.ctypes.data))
-                    d.update(node=node[:k], gpu_slots=slots[:k], score=score[:k], fail_counts=fc)
+                    d.update(zip(("node", "gpu_slots", "score", "fail_counts"),
+                                 self._download(L.simon_probe_download, i, (k, np.int32), (k, np.uint32), (k, np.int64),
+                                                (abi.N_FAIL_CODES, np.uint32))))
                 out.append(d)
-        self.last_probe = info
+            return out
+        out, self.last_probe = self._chunked(len(probes), chunk, L.simon_probe_times, run)
+        if not probes:
+            run(0, 0)           # no batch, but simon_probe_run still checks `placed` and drops the last batch
         return out
 
     # ---- grow batches (simon_grow_run) ----
@@ -641,26 +615,13 @@ class Engine:
         P = self.c.pods_dims["n_pods"]
         T = max(P - int(n_prefix), 0)
         local = getattr(self.c, "storage", None) is not None
-        n = len(scenarios)
-        per, free = self.drain_budget()
-        per += (16 + 4 * abi.N_FAIL_CODES + 4) * T
-        if chunk is None:
-            chunk = max(1, int(free * self.DRAIN_MEM_FRACTION) // max(per, 1))
-        out = []
-        info = dict(chunks=0, scenario_bytes=per, chunk=chunk, setup_ms=0.0, place_ms=0.0, launches=[])
-        for b in range(0, n, chunk):
-            part = scenarios[b:b + chunk]
-            m = len(part)
-            arr, keep = self._scenario_array(part)
+
+        def run(b, m):
+            arr, keep = self._scenario_array(scenarios[b:b + m])
             res = (abi.SimonScenarioResult * m)()
             loc = (abi.SimonScenarioLocalResult * m)() if local else None
             self._check(L.simon_grow_run(self.h, pl.ctypes.data if n_prefix else None, int(n_prefix), arr, m, res, loc))
-            su, pm = C.c_float(0), C.c_float(0)
-            self._check(L.simon_grow_times(self.h, C.byref(su), C.byref(pm)))
-            info["chunks"] += 1
-            info["setup_ms"] += float(su.value)
-            info["place_ms"] += float(pm.value)
-            info["launches"].append(self.last_launch())
+            out = []
             for i, r in enumerate(res):
                 d = dict(n_unscheduled=r.n_unscheduled, n_scheduled=r.n_scheduled, req_mcpu=r.req_mcpu, alloc_mcpu=r.alloc_mcpu,
                          req_mem=r.req_mem, alloc_mem=r.alloc_mem)
@@ -668,14 +629,10 @@ class Engine:
                     d["vg_requested"], d["vg_capacity"] = int(loc[i].vg_requested), int(loc[i].vg_capacity)
                 if detail:
                     nf = r.n_unscheduled
-                    node = np.zeros(max(T, 1), np.int32)
-                    slots = np.zeros(max(T, 1), np.uint32)
-                    score = np.zeros(max(T, 1), np.int64)
-                    fc = np.zeros((max(nf, 1), abi.N_FAIL_CODES), np.uint32)
-                    fp = np.zeros(max(nf, 1), np.uint32)
-                    self._check(L.simon_grow_download(self.h, i, node.ctypes.data, slots.ctypes.data, score.ctypes.data, fc.ctypes.data,
-                                                      fp.ctypes.data))
-                    d.update(node=node[:T], gpu_slots=slots[:T], score=score[:T], fail_counts=fc[:nf], fail_pod=fp[:nf])
+                    d.update(zip(("node", "gpu_slots", "score", "fail_counts", "fail_pod"),
+                                 self._download(L.simon_grow_download, i, (T, np.int32), (T, np.uint32), (T, np.int64),
+                                                (nf, np.uint32, abi.N_FAIL_CODES), (nf, np.uint32))))
                 out.append(d)
-        self.last_grow = info
+            return out
+        out, self.last_grow = self._chunked(len(scenarios), chunk, L.simon_grow_times, run, extra=(16 + 4 * abi.N_FAIL_CODES + 4) * T)
         return out

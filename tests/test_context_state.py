@@ -154,6 +154,122 @@ def test_each_event_drops_exactly_its_table_row(event):
         eng.close()
 
 
+def _batch_kinds(c, out):
+    """kind -> a batch of that kind on an engine whose live placement is `out` (of _local_case()), returning its results: drains and
+    waves remove node 0; the joining wave starts from a base without the last node (no pod is bound to it) and joins it."""
+    from simon_b200 import scaledown
+    P, N = len(out), c.n_nodes
+    remain, every = [np.arange(1, N, dtype=np.uint32)], [np.arange(N, dtype=np.uint32)]
+    absent = N - 1
+    assert not (np.asarray(c.pods["pod_fixed_node"]) == absent).any()
+    local = np.asarray(c.storage.class_local)[np.asarray(c.pods["pod_class"])]
+    guard, fixed = scaledown.pod_guard(c), np.asarray(c.pods["pod_fixed_node"])
+    probe = next(q for q in range(P) if fixed[q] == -1 and guard[q] == -1 and not local[q] and out[q] >= 0)
+
+    def wave(e, joins):
+        if joins is None:
+            e.wave_begin(out)
+        else:
+            e.wave_begin(np.where(out == absent, -1, out), np.arange(N) != absent)
+        return e.wave_run(remain, joins)
+    return {
+        "drain_run": lambda e: e.drain_run(out, remain),
+        "drain_run_local": lambda e: e.drain_run(out, remain, local=True),
+        "wave_run": lambda e: wave(e, None),
+        "wave_run_join": lambda e: wave(e, [np.array([absent], np.uint32)]),
+        "probe_run": lambda e: e.probe_run(out, [(probe, 2)]),
+        "grow_run": lambda e: e.grow_run(out, P // 2, every),
+        "scenarios_run_local": lambda e: e.run_scenarios_local(every),
+    }
+
+
+# batch kind -> the downloads its batch serves, and the code each answers right after it (None: simon_wave_commit's own refusals of
+# the batch's first scenario)
+BATCH_SERVES = {
+    "drain_run": {"drain": 0, "drain_pdb": 0},
+    "drain_run_local": {"drain": 0, "drain_pdb": 0, "scenario_storage": 0},
+    "wave_run": {"drain": 0, "drain_pdb": 0, "wave_join": 0, "wave_commit": None},
+    "wave_run_join": {"drain": 0, "drain_pdb": 0, "wave_join": 0, "wave_commit": -1},       # it joined a node: commit_retire only
+    "probe_run": {"probe": 0, "scenario_storage": 0},
+    "grow_run": {"grow": 0, "scenario_storage": 0},
+    "scenarios_run_local": {"scenario_storage": 0},
+}
+# what a later batch of a kind leaves of an earlier one: a storage batch keeps the drain, probe and grow batches (not a wave batch,
+# whose slots it overwrote); every other kind replaces them all
+BATCH_KEEPS = {"scenarios_run_local": {"drain", "drain_pdb", "probe", "grow"}}
+# batch kind -> its *_times entry point
+BATCH_TIMES = {"drain_run": "drain", "drain_run_local": "drain", "wave_run": "drain", "wave_run_join": "drain", "probe_run": "probe",
+               "grow_run": "grow"}
+
+
+def _batch_answers(eng):
+    """download -> return code of every batch download of scenario 0, and simon_wave_commit last (a commit that succeeds ends the
+    wave batch)."""
+    from simon_b200.engine import lib
+    L, h = lib(), eng.h
+    return {
+        "drain": L.simon_drain_download(h, 0, *[None] * 7),
+        "drain_pdb": L.simon_drain_pdb_download(h, 0, None, None),
+        "wave_join": L.simon_wave_join_download(h, 0, *[None] * 6),
+        "probe": L.simon_probe_download(h, 0, *[None] * 4),
+        "grow": L.simon_grow_download(h, 0, *[None] * 5),
+        "scenario_storage": L.simon_scenarios_storage_download(h, 0, None, None),
+        "wave_commit": L.simon_wave_commit(h, 0),
+    }
+
+
+def _batch_times(eng):
+    from simon_b200.engine import lib
+    out = {}
+    for name in ("drain", "probe", "grow"):
+        su, pm = C.c_float(0), C.c_float(0)
+        eng._check(getattr(lib(), f"simon_{name}_times")(eng.h, C.byref(su), C.byref(pm)))
+        out[name] = (su.value, pm.value)
+    return out
+
+
+@pytest.mark.gpu
+def test_batch_downloads_and_times_after_each_pair_of_batch_kinds():
+    """For every ordered pair of batch kinds, a batch of the first then one of the second: each batch download answers as the second
+    batch leaves it (BATCH_SERVES, BATCH_KEEPS, SIMON_ERR_STATE otherwise), and the *_times entry points of the kinds the second
+    batch is not keep the values the first batch left."""
+    from simon_b200.engine import Engine
+    c = _local_case()
+    wrong = []
+    with Engine(c, device=0) as eng:
+        out = eng.schedule()[0]
+    kinds = _batch_kinds(c, out)
+
+    def served(kind, res, d):
+        code = BATCH_SERVES[kind][d]
+        if code is None:
+            r = res[0]
+            code = 0 if r["n_unscheduled"] == r["n_blocked"] == r["n_pdb_violated"] == 0 else -1
+        return code
+    for first in kinds:
+        for second in kinds:
+            with Engine(c, device=0) as eng:
+                eng.schedule()
+                res1 = kinds[first](eng)
+                t1 = _batch_times(eng)
+                res2 = kinds[second](eng)
+                t2 = _batch_times(eng)
+                got = _batch_answers(eng)
+            for d, rc in got.items():
+                if d in BATCH_SERVES[second]:
+                    want = served(second, res2, d)
+                elif d in BATCH_SERVES[first] and d in BATCH_KEEPS.get(second, ()):
+                    want = served(first, res1, d)
+                else:
+                    want = ERR_STATE
+                if rc != want:
+                    wrong.append(f"{first} then {second}: {d} answers {rc}, not {want}")
+            for name in t1:
+                if name != BATCH_TIMES.get(second) and t2[name] != t1[name]:
+                    wrong.append(f"{first} then {second}: simon_{name}_times changed from {t1[name]} to {t2[name]}")
+    assert not wrong, "\n".join(wrong)
+
+
 GPU_CASE = ("c3", dict(n_nodes=400, n_workloads=80, replicas=10, n_apps=2, seed_no=21, gpu_pct=25))
 
 
