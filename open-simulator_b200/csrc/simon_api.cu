@@ -15,6 +15,7 @@
 #include "simon_kernel.cu"   // single translation unit: kernel + host API
 #include "simon_moves.cu"    // candidate-move scoring kernels (config 5)
 #include "simon_pdb.cuh"     // PodDisruptionBudget counts and marks (drains, move runs, plans): kernels in simon_pdb.cu
+#include "simon_trace.cuh"   // trace replay: removal and sample kernels in simon_trace.cu
 
 namespace {
 
@@ -249,6 +250,7 @@ enum Data : uint32_t {
     GROW_BATCH = 1u << 15,
     WAVE_BASE = 1u << 16,       // the single-scenario pool holds a wave base (simon_wave_begin, simon_wave_commit) and wave.place / slots mirror it
     WAVE_BATCH = 1u << 17,      // the last drain batch is a wave batch from the current base (simon_wave_run)
+    TRACE_BATCH = 1u << 18,
 };
 
 struct Validity {
@@ -259,7 +261,7 @@ struct Validity {
     void drop(uint32_t d) {
         static constexpr uint32_t derived[][2] = {
             {SNAPSHOT, POD_SET},
-            {POD_SET, STORAGE | PDB_TABLE | LIVE | WAVE_BASE | PLAN | DRAIN_BATCH | PROBE_BATCH | GROW_BATCH | MOVE_LIST | SCOPE_PREP | STATIC_FILL | EXPLAIN_SET},
+            {POD_SET, STORAGE | PDB_TABLE | LIVE | WAVE_BASE | PLAN | DRAIN_BATCH | PROBE_BATCH | GROW_BATCH | TRACE_BATCH | MOVE_LIST | SCOPE_PREP | STATIC_FILL | EXPLAIN_SET},
             {STORAGE, DEVICES | STORAGE_BATCH | LIVE | WAVE_BASE | SCOPE_PREP},     // SCOPE_PREP: the move-class records exclude local classes
             {DEVICES, STORAGE_BATCH | LIVE | WAVE_BASE},
             {MOVE_LIST, MOVE_RUN},
@@ -298,6 +300,7 @@ struct simon_ctx {
         // (-4) before a storage upload takes its local classes off (d_pod_fixed holds the result)
         std::vector<int32_t> h_fixed, h_guard, h_class, fixed_dev, fixed_cur;     // fixed_cur: what d_pod_fixed holds
         std::vector<uint8_t> bypass;
+        std::vector<uint8_t> gpu_wide;      // per class: GPU-share with more than 15 slots, which a slot word cannot state per device
         DevBuf<uint32_t> d_sig_class;       // a class per static signature (dense fill of the static verdict cache)
         uint32_t max_fail = 0;
         DevBuf<unsigned long long> d_stats, d_scache;
@@ -396,6 +399,19 @@ struct simon_ctx {
         std::vector<uint32_t> nfail;
         float setup_ms = 0.f, place_ms = 0.f;
     } grow;
+    // the last trace batch (simon_trace_run): scenarios replaying events over the tail [n_prefix, n_prefix + tail), whose per-pod
+    // outputs and failure records are laid out as a grow batch's; each one's failed creates; on the device the deleted pods of every
+    // delete run (event order), the per-scenario SkTraceAcc words and the samples [n][n_samples]; the device times of the setup and
+    // of the runs, the runs and the launches of the runs and samples
+    struct {
+        uint32_t n_prefix = 0, tail = 0, n_samples = 0, runs = 0;
+        uint64_t launches = 0;
+        std::vector<uint32_t> nfail;
+        DevBuf<uint32_t> d_del;
+        DevBuf<SkTraceAcc> d_acc;
+        DevBuf<simon_trace_point> d_points;
+        float setup_ms = 0.f, run_ms = 0.f;
+    } trace;
     // the wave base (simon_wave_begin): the single-scenario pool's state and its per-pod results (out_node, out_gpu) are the base, and
     // place / slots their host mirror; of the last wave batch, each scenario's removed nodes (CSR roff / removed, index order) and
     // vanished pods (CSR voff / vanished, pod order), which return with them; on the device the returned nodes and their pods (CSR) of the last commit, and its device time.
@@ -1233,6 +1249,11 @@ int simon_pods_upload(simon_ctx *ctx, const simon_podset *p) {
     ps.h_fixed.assign(p->pod_fixed_node, p->pod_fixed_node + p->n_pods);
     ps.h_guard.assign(guard.begin(), guard.begin() + p->n_pods);
     ps.h_class.assign(p->pod_class, p->pod_class + p->n_pods);
+    ps.gpu_wide.assign(std::max(1u, p->n_classes), 0);
+    for (uint32_t c = 0; c < p->n_classes; c++) {
+        const int64_t *cw = p->class_blob + p->class_off[c];
+        ps.gpu_wide[c] = cw[SCW_GPU_MEM] > 0 && cw[SCW_GPU_COUNT] > 15;
+    }
     int rc = upload_class_marks(ctx, nullptr);
     if (rc) return rc;
     ps.max_fail = std::max(1u, p->n_pods);      // every pod of the list may fail: one histogram row each (96 B)
@@ -1577,12 +1598,12 @@ static int live_batch_setup(simon_ctx *ctx, const int32_t *placed, uint32_t n_pr
     return rc ? rc : batch_from_single(ctx, n, local, Pb);
 }
 
-// A drain, probe or grow batch's first step after its refusals: the batch pool, its Open-Local slices and the output block are no
+// A drain, probe, grow or trace batch's first step after its refusals: the batch pool, its Open-Local slices and the output block are no
 // longer the last batch's, and no placement kernel of this call has run
 static int batch_begin(simon_ctx *ctx) {
     CU(cudaSetDevice(ctx->device));
     ctx->last_launch = simon_launch_info{};
-    ctx->valid.drop(DRAIN_BATCH | WAVE_BATCH | PROBE_BATCH | GROW_BATCH | STORAGE_BATCH);
+    ctx->valid.drop(DRAIN_BATCH | WAVE_BATCH | PROBE_BATCH | GROW_BATCH | TRACE_BATCH | STORAGE_BATCH);
     return SIMON_OK;
 }
 
@@ -1624,20 +1645,20 @@ static int batch_outputs(simon_ctx *ctx, uint32_t n, uint64_t cells, uint32_t st
     return SIMON_OK;
 }
 
-// After a batch's setup (timed from ctx->ev0): when `place`, its launch of family fam on geometry g (one failure record per row of the
-// output block), timed from ctx->evm to ctx->ev1; each scenario's sums over its active nodes (simon_scen_reduce) into res and, when
-// out_local is not null, its VG sums into out_local; then the synchronisation and the device times of the setup and the placement.
-// local: the batch pool's Open-Local slices are this batch's, which simon_scenarios_storage_download serves.
-static int batch_place(simon_ctx *ctx, SkParams &Pb, uint32_t n, const Geometry &g, Family fam, bool place, bool local,
-                       std::vector<simon_scenario_result> &res, simon_scenario_local_result *out_local, float &setup_ms, float &place_ms) {
+// A batch's launch of family fam on geometry g, one failure record per row of the output block; enqueued only, on the ctx stream.
+static int batch_launch(simon_ctx *ctx, SkParams &Pb, uint32_t n, const Geometry &g, Family fam) {
+    Pb.max_fail = ctx->bout.rows; Pb.npt = g.NPT;
+    return launch(ctx, Pb, n, g.CS, g.TPB, g.smem, false, fam);
+}
+
+// After a batch's placement launches (timed from ctx->evm to ctx->ev1): each scenario's sums over its active nodes (simon_scen_reduce)
+// into res and, when out_local is not null, its VG sums into out_local; then the synchronisation and the device times of the setup
+// (ctx->ev0 to ctx->evm) and the placement.  local: the batch pool's Open-Local slices are this batch's, which
+// simon_scenarios_storage_download serves.
+static int batch_finish(simon_ctx *ctx, uint32_t n, bool local, std::vector<simon_scenario_result> &res, simon_scenario_local_result *out_local,
+                        float &setup_ms, float &place_ms) {
     ScenPool &B = ctx->batch;
     cudaStream_t st = ctx->stream;
-    CU(cudaEventRecord(ctx->evm, st));
-    if (place) {
-        Pb.max_fail = ctx->bout.rows; Pb.npt = g.NPT;
-        const int rc = launch(ctx, Pb, n, g.CS, g.TPB, g.smem, false, fam);
-        if (rc) return rc;
-    }
     CU(cudaEventRecord(ctx->ev1, st));
     simon_scen_reduce<<<n, 256, 0, st>>>(B.scen.p, ctx->snap.d_alloc_mcpu.p, ctx->snap.d_alloc_mem.p, B.results.p);
     CU(cudaGetLastError());
@@ -1659,6 +1680,17 @@ static int batch_place(simon_ctx *ctx, SkParams &Pb, uint32_t n, const Geometry 
         ctx->valid.set(STORAGE_BATCH);
     }
     return SIMON_OK;
+}
+
+// After a batch's setup (timed from ctx->ev0): when `place`, its launch (batch_launch), timed from ctx->evm; then batch_finish.
+static int batch_place(simon_ctx *ctx, SkParams &Pb, uint32_t n, const Geometry &g, Family fam, bool place, bool local,
+                       std::vector<simon_scenario_result> &res, simon_scenario_local_result *out_local, float &setup_ms, float &place_ms) {
+    CU(cudaEventRecord(ctx->evm, ctx->stream));
+    if (place) {
+        const int rc = batch_launch(ctx, Pb, n, g, fam);
+        if (rc) return rc;
+    }
+    return batch_finish(ctx, n, local, res, out_local, setup_ms, place_ms);
 }
 
 // k per-pod outputs of the last batch from position `at` into whichever of node, gpu_slots and score is not null (scores: zeros when
@@ -2333,6 +2365,201 @@ extern "C" int simon_grow_times(simon_ctx *ctx, float *setup_ms, float *place_ms
     if (!ctx) return SIMON_ERR_INVALID;
     if (setup_ms) *setup_ms = ctx->grow.setup_ms;
     if (place_ms) *place_ms = ctx->grow.place_ms;
+    return SIMON_OK;
+}
+
+// ---- trace replay -----------------------------------------------------------------------------------------------------------------
+// The setup is a grow batch's (live_batch_setup, outputs laid out as there).  Then every run is enqueued without a host synchronisation:
+// a create run is one launch of the batch placement variants over its pod range [first, first + count); a delete run is one
+// simon_trace_remove launch; a sample, one simon_trace_sample launch after the run that ends at it.  The placement kernel restarts its
+// failure count at every launch: the removal and sample launches fold each create run's counts into SkTraceAcc and move the scenario's
+// record pointers past that run's records (simon_trace.cuh), so the failure records of a scenario follow each other in event order.
+extern "C" int simon_trace_run(simon_ctx *ctx, const int32_t *placed, uint32_t n_prefix, const simon_trace_event *events, uint32_t n_events,
+                               const simon_scenario *scen, uint32_t n, const uint32_t *samples, uint32_t n_samples, simon_trace_result *out) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(POD_SET)) return fail(ctx, SIMON_ERR_STATE, "simon_trace_run before uploads");
+    const uint32_t P = ctx->pods.n_pods, N = ctx->snap.N;
+    // ---- refusals before any device work: the prefix, the node lists, the tail, the events, the samples ----
+    if (n_prefix > P) return fail(ctx, SIMON_ERR_INVALID, "simon_trace_run: n_prefix %u above the %u pods", n_prefix, P);
+    if ((n_prefix && !placed) || (n_events && !events) || (n_samples && !samples) || (n && !out))
+        return fail(ctx, SIMON_ERR_INVALID, "simon_trace_run: NULL argument");
+    int rc = check_prefix(ctx, placed, n_prefix);
+    if (rc) return rc;
+    std::vector<uint32_t> all;
+    std::vector<simon_scenario> every;
+    if (!scen) {
+        all.resize(N);
+        for (uint32_t g = 0; g < N; g++) all[g] = g;
+        every.assign(n, simon_scenario{N, 0u, all.data()});
+        scen = every.data();
+    }
+    for (uint32_t i = 0; i < n; i++)
+        if (scen[i].n_nodes == 0) return fail(ctx, SIMON_ERR_INVALID, "trace scenario %u has no node", i);
+    uint32_t max_active = 0;
+    rc = scenario_lists(ctx, scen, n, "trace scenario", max_active);
+    if (rc) return rc;
+    const uint32_t N1 = std::max(1u, N);
+    uint32_t placed_prefix = 0;
+    {
+        std::vector<uint8_t> held(N1, 0);
+        std::vector<uint32_t> nodes;
+        for (uint32_t q = 0; q < n_prefix; q++)
+            if (placed[q] >= 0) {
+                placed_prefix++;
+                if (!held[placed[q]]) { held[placed[q]] = 1; nodes.push_back((uint32_t)placed[q]); }
+            }
+        for (uint32_t i = 0; i < n; i++) {
+            const int32_t *rank = ctx->batch.h_rank.data() + (size_t)i * N1;
+            for (uint32_t g : nodes)
+                if (rank[g] < 0) return fail(ctx, SIMON_ERR_INVALID, "trace scenario %u leaves out node %u, which holds a placed prefix pod", i, g);
+        }
+    }
+    const bool storage = ctx->valid.has(STORAGE);
+    auto local_class = [&](uint32_t q) { return storage && ctx->storage.h_class_local[ctx->pods.h_class[q]]; };
+    for (uint32_t q = n_prefix; q < P; q++)
+        if (ctx->pods.h_fixed[q] >= 0) return fail(ctx, SIMON_ERR_INVALID, "simon_trace_run: tail pod %u is bound by spec.nodeName", q);
+    // runs: [event begin, event end) of one op, ended early by a sample; creates give a pod range, deletes a range of the delete list
+    struct Run { uint32_t op, b, e, first, count, del; int32_t sample; };
+    std::vector<Run> runs;
+    std::vector<uint32_t> del;
+    {
+        std::vector<uint8_t> gone(std::max(1u, P), 0);
+        uint32_t next = n_prefix, si = 0;
+        for (uint32_t k = 0; k < n_events; k++) {
+            const uint32_t op = events[k].op, q = events[k].pod;
+            if (op == SIMON_TRACE_CREATE) {
+                if (q != next) return fail(ctx, SIMON_ERR_INVALID, "trace event %u creates pod %u, not the next tail pod %u", k, q, next);
+                if (q >= P) return fail(ctx, SIMON_ERR_INVALID, "trace event %u creates pod %u past the tail", k, q);
+                if (local_class(q)) return fail(ctx, SIMON_ERR_INVALID, "trace event %u creates pod %u, which has Open-Local volumes", k, q);
+                next++;
+            } else if (op == SIMON_TRACE_DELETE) {
+                if (q >= P) return fail(ctx, SIMON_ERR_INVALID, "trace event %u deletes pod %u, out of range", k, q);
+                if (q >= n_prefix && q >= next) return fail(ctx, SIMON_ERR_INVALID, "trace event %u deletes pod %u before its create", k, q);
+                if (gone[q]) return fail(ctx, SIMON_ERR_INVALID, "trace event %u deletes pod %u again", k, q);
+                if (ctx->pods.h_guard[q] >= 0) return fail(ctx, SIMON_ERR_INVALID, "trace event %u deletes pod %u, a DaemonSet pod", k, q);
+                if (local_class(q)) return fail(ctx, SIMON_ERR_INVALID, "trace event %u deletes pod %u, which has Open-Local volumes", k, q);
+                if (ctx->pods.gpu_wide[ctx->pods.h_class[q]])
+                    return fail(ctx, SIMON_ERR_INVALID, "trace event %u deletes pod %u, whose GPU-share slots its slot word cannot state", k, q);
+                gone[q] = 1;
+                del.push_back(q);
+            } else {
+                return fail(ctx, SIMON_ERR_INVALID, "trace event %u: unknown op %u", k, op);
+            }
+            if (si < n_samples && samples[si] < k) return fail(ctx, SIMON_ERR_INVALID, "trace samples are not strictly ascending");
+            const bool sampled = si < n_samples && samples[si] == k;
+            if (runs.empty() || runs.back().op != op || runs.back().sample >= 0)
+                runs.push_back(Run{op, k, k, q, 0, (uint32_t)del.size() - (op == SIMON_TRACE_DELETE ? 1u : 0u), -1});
+            Run &r = runs.back();
+            r.e = k + 1;
+            r.count++;
+            if (sampled) r.sample = (int32_t)si++;
+        }
+        if (next != P) return fail(ctx, SIMON_ERR_INVALID, "simon_trace_run: the trace creates %u of the %u tail pods", next - n_prefix, P - n_prefix);
+        if (si < n_samples) return fail(ctx, SIMON_ERR_INVALID, "trace sample %u is not an event index in ascending order", si);
+    }
+    const uint32_t T = P - n_prefix;
+    rc = batch_begin(ctx);
+    if (rc || n == 0) return rc;
+    cudaStream_t st = ctx->stream;
+    ScenPool &S = ctx->single, &B = ctx->batch;
+    // ---- geometry of the batch placement variants, the batch pool, the outputs and the trace's own buffers (allocations before the
+    // timed work) ----
+    Geometry g;
+    rc = batch_pool(ctx, max_active, n, PLACE, g);
+    if (rc) return rc;
+    std::vector<SkScenario> h;
+    CU(batch_scenarios(ctx, scen, n, h));
+    char outputs[96];
+    snprintf(outputs, sizeof(outputs), "simon_trace_run: outputs of %u scenarios x %u tail pods", n, T);
+    rc = batch_outputs(ctx, n, (uint64_t)n * T + n_prefix, T, T, h, outputs);
+    if (rc) return rc;
+    auto &tr = ctx->trace;
+    CU(tr.d_del.upload(del.data(), del.size(), st));
+    CU(tr.d_acc.alloc(n));
+    CU(cudaMemsetAsync(tr.d_acc.p, 0, sizeof(SkTraceAcc) * (size_t)n, st));
+    {
+        // the samples, asked against the free memory only when their buffer must grow, as batch_outputs asks for the outputs
+        const uint64_t pts = (uint64_t)n * n_samples, need = pts * sizeof(simon_trace_point);
+        size_t fr = 0, tot = 0;
+        if (pts > tr.d_points.cap) CU(cudaMemGetInfo(&fr, &tot));
+        if (pts > tr.d_points.cap && need > (uint64_t)fr + sizeof(simon_trace_point) * tr.d_points.cap)
+            return fail(ctx, SIMON_ERR_LIMIT, "simon_trace_run: %u samples of %u scenarios (%llu bytes) do not fit the device (%llu bytes free)",
+                        n_samples, n, (unsigned long long)need, (unsigned long long)fr);
+        CU(tr.d_points.alloc((size_t)pts));
+    }
+    // ---- setup: the live state of the prefix in every slot, with its Open-Local state when storage is uploaded ----
+    SkParams Pb;
+    rc = live_batch_setup(ctx, placed, n_prefix, n, storage, Pb);
+    if (rc) return rc;
+    // ---- every run, then the samples that end at it, enqueued back to back ----
+    CU(cudaEventRecord(ctx->evm, st));
+    const uint64_t launches0 = ctx->launches;
+    for (const Run &r : runs) {
+        if (r.op == SIMON_TRACE_CREATE) {
+            Pb.first = r.first; Pb.count = r.count;
+            rc = batch_launch(ctx, Pb, n, g, PLACE);
+            if (rc) return rc;
+        } else {
+            CU(simon_trace_launch_remove(st, (uint32_t)ctx->sms * 4u, Pb, B.scen.p, n, tr.d_del.p + r.del, r.count, ctx->d_prefix.p, S.out_gpu.p,
+                                         n_prefix, ctx->bout.d_node.p, ctx->bout.d_gpu.p, T, tr.d_acc.p));
+            ctx->launches++;
+        }
+        if (r.sample >= 0) {
+            CU(simon_trace_launch_sample(st, Pb, B.scen.p, n, tr.d_acc.p, placed_prefix, r.e - 1, tr.d_points.p, n_samples, (uint32_t)r.sample));
+            ctx->launches++;
+        }
+    }
+    tr.launches = ctx->launches - launches0;
+    std::vector<simon_scenario_result> res;
+    rc = batch_finish(ctx, n, storage, res, nullptr, tr.setup_ms, tr.run_ms);
+    if (rc) return rc;
+    ctx->valid.set(LIVE);
+    std::vector<SkTraceAcc> acc(n);
+    CU(cudaMemcpy(acc.data(), tr.d_acc.p, sizeof(SkTraceAcc) * (size_t)n, cudaMemcpyDeviceToHost));
+    tr.nfail.resize(n);
+    for (uint32_t i = 0; i < n; i++) {
+        // the last create run's counts are folded only when a removal or a sample follows it
+        simon_trace_result &o = out[i];
+        o.n_scheduled = acc[i].sched + res[i].n_scheduled;
+        o.n_unscheduled = acc[i].fail + res[i].n_unscheduled;
+        o.n_removed = acc[i].removed;
+        o.n_running = placed_prefix + o.n_scheduled - o.n_removed;
+        o.req_mcpu = res[i].req_mcpu; o.alloc_mcpu = res[i].alloc_mcpu; o.req_mem = res[i].req_mem; o.alloc_mem = res[i].alloc_mem;
+        tr.nfail[i] = o.n_unscheduled;
+    }
+    tr.n_prefix = n_prefix; tr.tail = T; tr.n_samples = n_samples; tr.runs = (uint32_t)runs.size();
+    ctx->valid.set(TRACE_BATCH);
+    return SIMON_OK;
+}
+
+extern "C" int simon_trace_download(simon_ctx *ctx, uint32_t scenario, int32_t *node, uint32_t *gpu_slots, int64_t *score,
+                                    uint32_t *fail_counts, uint32_t *fail_pod) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(TRACE_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_trace_run batch since the last upload, or another batch after it");
+    if (scenario >= ctx->bout.n) return fail(ctx, SIMON_ERR_INVALID, "trace scenario %u of a batch of %u", scenario, ctx->bout.n);
+    CU(cudaSetDevice(ctx->device));
+    const uint32_t T = ctx->trace.tail, nf = std::min(ctx->trace.nfail[scenario], T);
+    const int rc = batch_download(ctx, (size_t)scenario * T + ctx->trace.n_prefix, T, node, gpu_slots, score);
+    return rc ? rc : batch_fail_download(ctx, (size_t)scenario * T, nf, fail_counts, fail_pod);
+}
+
+extern "C" int simon_trace_samples_download(simon_ctx *ctx, uint32_t scenario, simon_trace_point *points) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (!ctx->valid.has(TRACE_BATCH)) return fail(ctx, SIMON_ERR_STATE, "no simon_trace_run batch since the last upload, or another batch after it");
+    if (scenario >= ctx->bout.n) return fail(ctx, SIMON_ERR_INVALID, "trace scenario %u of a batch of %u", scenario, ctx->bout.n);
+    CU(cudaSetDevice(ctx->device));
+    const uint32_t ns = ctx->trace.n_samples;
+    if (points && ns)
+        CU(cudaMemcpy(points, ctx->trace.d_points.p + (size_t)scenario * ns, sizeof(simon_trace_point) * ns, cudaMemcpyDeviceToHost));
+    return SIMON_OK;
+}
+
+extern "C" int simon_trace_times(simon_ctx *ctx, float *setup_ms, float *run_ms, uint32_t *n_runs, uint64_t *n_launches) {
+    if (!ctx) return SIMON_ERR_INVALID;
+    if (setup_ms) *setup_ms = ctx->trace.setup_ms;
+    if (run_ms) *run_ms = ctx->trace.run_ms;
+    if (n_runs) *n_runs = ctx->trace.runs;
+    if (n_launches) *n_launches = ctx->trace.launches;
     return SIMON_OK;
 }
 

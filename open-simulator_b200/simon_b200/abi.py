@@ -63,6 +63,8 @@ PROBE_STOP_UNSCHEDULABLE, PROBE_STOP_MAX_REPLICAS = 1, 2
 EXPLAIN_MAX_TOP = 16
 EXPLAIN_WORDS = 10
 EXPLAIN_NOT_RUN = -4
+# simon_trace_event ops
+TRACE_CREATE, TRACE_DELETE = 1, 2
 
 
 class SimonSnapshot(C.Structure):
@@ -130,6 +132,26 @@ class SimonProbe(C.Structure):
 class SimonProbeResult(C.Structure):
     _fields_ = [("n_placed", C.c_uint32), ("stop_reason", C.c_uint32),
                 ("req_mcpu", C.c_int64), ("alloc_mcpu", C.c_int64), ("req_mem", C.c_int64), ("alloc_mem", C.c_int64)]
+
+
+class SimonTraceEvent(C.Structure):
+    _fields_ = [("op", C.c_uint32), ("pod", C.c_uint32)]
+
+
+class SimonTraceResult(C.Structure):
+    _fields_ = [("n_scheduled", C.c_uint32), ("n_unscheduled", C.c_uint32), ("n_removed", C.c_uint32), ("n_running", C.c_uint32),
+                ("req_mcpu", C.c_int64), ("alloc_mcpu", C.c_int64), ("req_mem", C.c_int64), ("alloc_mem", C.c_int64)]
+
+
+class SimonTracePoint(C.Structure):
+    _fields_ = [("event", C.c_uint32), ("n_running", C.c_uint32), ("n_failed", C.c_uint32), ("idle_devices", C.c_uint32),
+                ("partial_devices", C.c_uint32), ("reserved", C.c_uint32),
+                ("req_mcpu", C.c_int64), ("alloc_mcpu", C.c_int64), ("req_mem", C.c_int64), ("alloc_mem", C.c_int64),
+                ("gpu_used", C.c_int64), ("gpu_total", C.c_int64)]
+
+
+# simon_trace_point, as the structured array Engine.trace_run returns
+TRACE_POINT_DTYPE = np.dtype(SimonTracePoint)
 
 
 class SimonMovesResult(C.Structure):
@@ -308,6 +330,10 @@ SIGNATURES = {
     "simon_grow_run": (_I, [_P, _P, _U32, _P, _U32, _P, _P]),
     "simon_grow_download": (_I, [_P, _U32] + [_P] * 5),
     "simon_grow_times": (_I, [_P, _PF, _PF]),
+    "simon_trace_run": (_I, [_P, _P, _U32, _P, _U32, _P, _U32, _P, _U32, _P]),
+    "simon_trace_download": (_I, [_P, _U32] + [_P] * 5),
+    "simon_trace_samples_download": (_I, [_P, _U32, _P]),
+    "simon_trace_times": (_I, [_P, _PF, _PF, C.POINTER(C.c_uint32), _PU64]),
     "simon_pdbs_upload": (_I, [_P, _P]),
     "simon_pdbs_allowed": (_I, [_P, _P]),
     "simon_host_go118_sort": (_I, [_P, _U32, _P]),

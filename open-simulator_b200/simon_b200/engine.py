@@ -636,3 +636,54 @@ class Engine:
             return out
         out, self.last_grow = self._chunked(len(scenarios), chunk, L.simon_grow_times, run, extra=(16 + 4 * abi.N_FAIL_CODES + 4) * T)
         return out
+
+    # ---- trace replay (simon_trace_run) ----
+    def trace_run(self, placed, n_prefix: int, events, scenarios: Optional[List[np.ndarray]] = None, samples=None, detail: bool = True,
+                  chunk: Optional[int] = None) -> List[dict]:
+        """Replay `events` ((op, pod) pairs, op abi.TRACE_CREATE / abi.TRACE_DELETE) on the live state placed[:n_prefix] in each scenario
+        (scenarios: node lists as grow_run takes them; None: one scenario on every node in index order).  samples: ascending event
+        indices after which the state is recorded.  The scenarios run in batches sized as grow_run sizes them (chunk: an explicit batch
+        size).  Returns one dict per scenario: n_scheduled / n_unscheduled (creates placed and failed), n_removed (deletes that took a
+        pod off a node), n_running and the sums req_mcpu / alloc_mcpu / req_mem / alloc_mem after the last event, samples (a structured
+        array of abi.TRACE_POINT_DTYPE); with detail also node, gpu_slots and score per tail pod [n_pods - n_prefix], and fail_counts
+        [n_unscheduled][24] and fail_pod.  self.last_trace: chunks, scenario_bytes, setup_ms / place_ms (device time summed over the
+        batches), runs and launches of the runs and samples (summed), launches (last_launch() of each batch)."""
+        L = lib()
+        pl = np.ascontiguousarray(np.asarray(placed)[:n_prefix], dtype=np.int32)
+        P = self.c.pods_dims["n_pods"]
+        T = max(P - int(n_prefix), 0)
+        ev = np.ascontiguousarray(np.asarray(events, dtype=np.uint32).reshape(-1, 2))
+        sm = np.ascontiguousarray(np.asarray([] if samples is None else samples, dtype=np.uint32))
+        ns = len(sm)
+        single = scenarios is None
+        n_scen = 1 if single else len(scenarios)
+        info = dict(runs=0, run_launches=0)
+
+        def run(b, m):
+            arr, keep = (None, None) if single else self._scenario_array(scenarios[b:b + m])
+            res = (abi.SimonTraceResult * max(m, 1))()
+            self._check(L.simon_trace_run(self.h, pl.ctypes.data if n_prefix else None, int(n_prefix), ev.ctypes.data if len(ev) else None,
+                                          len(ev), arr, m, sm.ctypes.data if ns else None, ns, res))
+            nr, nl = C.c_uint32(0), C.c_uint64(0)
+            self._check(L.simon_trace_times(self.h, None, None, C.byref(nr), C.byref(nl)))
+            info["runs"] += nr.value
+            info["run_launches"] += nl.value
+            out = []
+            for i in range(m):
+                r = res[i]
+                d = dict(n_scheduled=r.n_scheduled, n_unscheduled=r.n_unscheduled, n_removed=r.n_removed, n_running=r.n_running,
+                         req_mcpu=r.req_mcpu, alloc_mcpu=r.alloc_mcpu, req_mem=r.req_mem, alloc_mem=r.alloc_mem)
+                pts = np.zeros(max(ns, 1), abi.TRACE_POINT_DTYPE)
+                self._check(L.simon_trace_samples_download(self.h, i, pts.ctypes.data))
+                d["samples"] = pts[:ns]
+                if detail:
+                    nf = r.n_unscheduled
+                    d.update(zip(("node", "gpu_slots", "score", "fail_counts", "fail_pod"),
+                                 self._download(L.simon_trace_download, i, (T, np.int32), (T, np.uint32), (T, np.int64),
+                                                (nf, np.uint32, abi.N_FAIL_CODES), (nf, np.uint32))))
+                out.append(d)
+            return out
+        out, self.last_trace = self._chunked(n_scen, 1 if single else chunk, lambda h, su, pm: L.simon_trace_times(h, su, pm, None, None),
+                                             run, extra=(16 + 4 * abi.N_FAIL_CODES + 4) * T + C.sizeof(abi.SimonTracePoint) * ns)
+        self.last_trace.update(info)
+        return out

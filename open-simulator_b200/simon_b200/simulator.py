@@ -726,6 +726,27 @@ class Simulator:
         self.last_grow_timing = tm
         return res
 
+    def ReplayTrace(self, events, new_node: Optional[Obj] = None, kmax: int = 0, samples: int = 100):
+        """trace.TraceResult: the trace `events` (trace.Event; trace.from_lifetimes builds them) replayed on the live session: creates
+        are placed on the state the events before them leave, deletes take pods off their nodes, and a failed create is not retried.
+        With new_node, scenario k is the session's nodes plus k copies of it, for every k in 0..kmax in one device batch; MinNodes is the
+        least k without a failed create, and AllFromMinNodes says whether every k above it has none too (with churn, feasibility is not
+        monotone in k).  Per k: creates, failures (UnscheduledPod with the FitError text and the event .Time), deletes, the first
+        failure's time and `samples` samples of the state with their times; at MinNodes (kmax when none) every created pod's node and
+        gpu-index.  The superset runs on a device context of its own; the session is not changed."""
+        from . import trace
+        from .engine import Engine
+        self._live()
+        if kmax < 0:
+            raise ValueError(f"ReplayTrace: kmax must be at least 0 (got {kmax})")
+        if new_node is not None and (not isinstance(new_node, dict) or new_node.get("kind") != "Node"):
+            raise ValueError("ReplayTrace: new_node is not a Node")
+        ts = trace.build(self, events, new_node, kmax)
+        with Engine(ts.compiled, device=self.options.device, record_scores=self.options.record_scores) as eng:
+            res = trace.replay(eng, ts, samples)
+            self.last_trace = eng.last_trace
+        return res
+
     def PlanNodeReplacement(self, nodes: List[str], new_node: Obj, count: Optional[int] = None, max_surge: int = 1,
                             max_unavailable: int = 0, order: str = "utilisation", kmax: Optional[int] = None):
         """replace.ReplacementPlan: the old nodes `nodes` replaced by copies of `new_node` in surge waves.  Each wave joins the next
