@@ -6,25 +6,10 @@ all words 0.  expected(...) runs the oracle pod by pod and calls it for every ex
 engine's records (Engine.explanations) with them."""
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 
-from checkers import build_checker
+import checkers
 from simon_b200 import abi
-
-_LIB = None
-
-
-def lib():
-    """The checker, built by the recipe of tests/checkers.py (it includes no other checker source)."""
-    global _LIB
-    if _LIB is None:
-        L = C.CDLL(build_checker("explain_oracle", []))
-        L.simon_oracle_last_reasons.restype = None
-        L.simon_oracle_last_reasons.argtypes = [C.c_void_p, C.c_void_p]
-        _LIB = L
-    return _LIB
 
 
 def record(node: int, reached: bool, reasons, detail, top_k: int, order=None) -> dict:
@@ -55,7 +40,6 @@ def expected(c, pods, top_k: int, open_local: bool = False, threads: int = 1) ->
     o = Oracle(c, threads=threads, open_local=open_local)
     o.enable_dump()
     fixed = c.pods["pod_fixed_node"]
-    reasons = np.zeros(max(c.n_nodes, 1), np.uint32)
     out, pos = [], 0
     for q in pods:
         q = int(q)
@@ -63,12 +47,11 @@ def expected(c, pods, top_k: int, open_local: bool = False, threads: int = 1) ->
             o.schedule(pos, q - pos)
         node = int(o.schedule(q, 1)[0][0])
         reached = fixed[q] == -1 and node != -3
+        reasons = detail = None
         if reached:
-            lib().simon_oracle_last_reasons(o.h, reasons.ctypes.data)
+            reasons = checkers.last_reasons(o)
             _code, detail = o.last_detail()
-        else:
-            detail = None
-        out.append(record(node, reached, reasons[:c.n_nodes], detail, top_k))
+        out.append(record(node, reached, reasons, detail, top_k))
         pos = q + 1
     o.close()
     return out

@@ -8,8 +8,7 @@ import re
 import numpy as np
 import pytest
 
-import moves_plan_oracle as MP
-import moves_plan_pdb_oracle as MPP
+import checkers
 from util import make_case
 
 NO_MOVE, MAX_MOVES = 1, 2
@@ -179,7 +178,7 @@ def test_pdb_checker_equals_stepwise_pdb_less_checker(seed):
     max_moves = 40
     o = Oracle(c)
     o.schedule()
-    ref = MPP.plan_pdb(o, mv, out, o.gpu_slot_words(), max_moves, 1, 0, t.pod_off, t.pod_pdb, allowed)
+    ref = checkers.plan_pdb(o, mv, out, o.gpu_slot_words(), max_moves, 1, 0, t.pod_off, t.pod_pdb, allowed)
     o.close()
     # the second mechanism
     o = Oracle(c)
@@ -194,7 +193,7 @@ def test_pdb_checker_equals_stepwise_pdb_less_checker(seed):
                 excluded.add(q)
         keep = np.array([int(m[0]) not in excluded for m in mv], bool)
         idx = np.nonzero(keep)[0]
-        r = MP.plan(o, mv[idx], placement, slots, 1, 1, 0)
+        r = checkers.plan(o, mv[idx], placement, slots, 1, 1, 0)
         if not len(r["steps"]):
             stop = r["stop_reason"]
             break
@@ -332,7 +331,6 @@ def test_allowed_after_schedule_resume_and_drain():
 
 @pytest.mark.gpu
 def test_drain_sweep_pdb_violations():
-    import drain_oracle as DO
     from simon_b200 import disruption, scaledown
     from simon_b200.engine import Engine
     p, c = make_case("mix", seed_no=104, n_nodes=60, n_workloads=40, max_replicas=8)
@@ -363,7 +361,7 @@ def test_drain_sweep_pdb_violations():
     np.testing.assert_array_equal(o.schedule()[0], out)
     rng = np.random.RandomState(1)
     for g in rng.choice(c.n_nodes, 8, replace=False).tolist():
-        ev = DO.drain(o, out, remain[g])["evicted"]
+        ev = checkers.drain(o, out, remain[g])["evicted"]
         want = violations_ref(pdbs, c.pod_recs, [int(q) for q in ev], allowed)
         assert dict(zip(res[g]["pdb_violated"].tolist(), res[g]["pdb_evicted"].tolist())) == want
     o.close()
@@ -425,7 +423,7 @@ def _plan_vs_checker(c, mv, t, max_moves, scope=0, rebuild=True, static_cache=Tr
     np.testing.assert_array_equal(allowed, t.allowed(out))
     o = Oracle(c)
     assert np.array_equal(o.schedule()[0], out)
-    ref = MPP.plan_pdb(o, mv, out, o.gpu_slot_words(), max_moves, 1, scope, t.pod_off, t.pod_pdb, allowed)
+    ref = checkers.plan_pdb(o, mv, out, o.gpu_slot_words(), max_moves, 1, scope, t.pod_off, t.pod_pdb, allowed)
     o.close()
     got = _steps(r)
     assert got.tolist() == ref["steps"].tolist()

@@ -1,7 +1,7 @@
 """Node drains (simon_drain_run, simon_b200.scaledown) and the scale-down planner.
 
 CPU: remaining-node orders against node_tree_list, the classification of a removed node's pods, the planner's prefix rule with a
-fake runner, the drain checker (tests/drain_oracle.c) on hand-derived answers.  GPU: every drain kernel variant against the checker,
+fake runner, the drain checker (tests/checkers.c) on hand-derived answers.  GPU: every drain kernel variant against the checker,
 drains against the recompile + simon_schedule_resume equivalence that pins the definition, the live state after a drain batch, and
 the session entry points end to end."""
 import numpy as np
@@ -44,14 +44,14 @@ def known_answer():
 
 def checker_runner(c, placed):
     """plan_scale_down's runner on the CPU: the drain checker, plus the occupancy sums of its end state."""
-    import drain_oracle
+    import checkers
     o, _ = _live(c)
     ac, am = c.snap["alloc_mcpu"], c.snap["alloc_mem"]
 
     def run(remain_lists):
         out = []
         for rl in remain_lists:
-            r = drain_oracle.drain(o, placed, rl)
+            r = checkers.drain(o, placed, rl)
             st = o.state()
             idx = np.asarray(rl, dtype=np.int64)
             r.update(req_mcpu=int(st["req_mcpu"][idx].sum()), alloc_mcpu=int(ac[idx].sum()),
@@ -154,12 +154,12 @@ def test_gpu_index_joins_one_device_per_slot_with_dashes():
 
 
 def test_checker_with_nothing_removed_reproduces_the_live_state():
-    import drain_oracle
+    import checkers
     for seed in (0, 4):
         c = _compiled(*synth.make_mix(seed_no=seed, n_nodes=30))
         o, placed = _live(c)
         st, ext, slots = o.state(), o.state_ext(), o.gpu_slot_words()
-        r = drain_oracle.drain(o, placed, np.arange(c.n_nodes))
+        r = checkers.drain(o, placed, np.arange(c.n_nodes))
         assert (r["n_evicted"], r["n_blocked"], r["n_vanished"]) == (0, 0, 0)
         for k, v in o.state().items():
             assert np.array_equal(v, st[k]), k
@@ -224,7 +224,7 @@ def _assert_drain_equal(a, b, what):
 @pytest.mark.gpu
 @pytest.mark.parametrize("kernel", sorted(DRAIN_VARIANTS))
 def test_drain_variant_matches_checker(kernel):
-    import drain_oracle
+    import checkers
     from simon_b200.engine import Engine
     cs, t, big = DRAIN_VARIANTS[kernel]
     rng = np.random.default_rng(11)
@@ -238,7 +238,7 @@ def test_drain_variant_matches_checker(kernel):
             got = eng.drain_run(placed, remain)
             assert eng.last_launch()["kernel"] == kernel
         for d, rl, g in zip(drains, remain, got):
-            want = drain_oracle.drain(o, placed, rl)
+            want = checkers.drain(o, placed, rl)
             _assert_drain_equal(g, want, f"{kernel} seed {seed} drain {d}")
             pos = g["node"] >= 0
             assert np.array_equal(g["score"][pos], want["score"][pos]), d

@@ -3,7 +3,7 @@ tables that tests/test_zz_explain_probe_edges_gpu.py runs, checked on the CPU.
 
 The GPU file runs the explain kernels (simon_explain_kernel_*) and the probe kernels (simon_probe_kernel_*) on every builder of
 test_engine_limits.py and every case of test_score_ranges.py, at the geometries of GEOMS, and compares them exactly with
-explain_oracle.expected and probe_oracle.probe.  Two cases are new here:
+explain_oracle.expected and checkers.probe.  Two cases are new here:
   * wrap_case: zone_case(65537, 20, 3) of test_zz_large_cluster_gpu, whose explained records have known answers (rejected counts and
     feasible counts past 16 bits);
   * bound_case: a Deployment with a preferred podAffinity term to its own label on the zone key, of weight BOUND_W, so that its
@@ -160,13 +160,13 @@ def test_bound_case_reaches_the_affinity_guard():
 def test_bound_case_probe_on_the_checker():
     """On the CPU checker: the probe of lim - n_pods replicas places them all, every pod in z0, and the last replica sees a raw
     InterPodAffinity score within 2 w of 2^31 - 1."""
-    import probe_oracle
+    import checkers
     from oracle.binding import Oracle
     p, c = bound_case()
     o = Oracle(c)
     placed = o.schedule()[0]
     R = bound_limit(c) - c.pods_dims["n_pods"]
-    want = probe_oracle.probe(o, placed, 0, R)
+    want = checkers.probe(o, placed, 0, R)
     o.close()
     assert want["n_placed"] == R and want["stop_reason"] == abi.PROBE_STOP_MAX_REPLICAS
     zones = np.array([c.node_names[g].startswith("n") for g in np.concatenate([placed, want["node"]])])

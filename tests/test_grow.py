@@ -2,7 +2,7 @@
 
 The superset a session grows into: its pod list first and unchanged, then the pool DaemonSet pods guarded by their copies, then the
 apps' pods; the placements remapped by node name; scenario k = 0 in the session's node order.  The search (grow.plan) runs here on the
-grow checker (tests/grow_oracle.c) on hand-derived cases; the shared k search gives apply.auto_add_nodes what its own loop gave; and
+grow checker (tests/checkers.c) on hand-derived cases; the shared k search gives apply.auto_add_nodes what its own loop gave; and
 the host refusals."""
 import copy
 
@@ -70,10 +70,10 @@ class CheckerEngine:
         self.batches = []
 
     def grow_run(self, placed, n_prefix, scenarios, detail=True, chunk=None):
-        import grow_oracle
+        import checkers
         out = []
         for nodes in scenarios:
-            r = grow_oracle.grow(self.o, placed, n_prefix, nodes)
+            r = checkers.grow(self.o, placed, n_prefix, nodes)
             st = self.o.state()
             act = np.asarray(nodes, np.int64)
             r.update(req_mcpu=int(st["req_mcpu"][act].sum()), alloc_mcpu=int(self.c.snap["alloc_mcpu"][act].sum()),

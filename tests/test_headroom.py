@@ -1,6 +1,6 @@
 """Scheduling headroom probes (simon_probe_run, Engine.probe_run, simon_b200.headroom, Simulator.Headroom).
 
-CPU: the probe checker (tests/probe_oracle.c) on hand-derived answers with their exact FitError texts, the host's refusals through a
+CPU: the probe checker (tests/checkers.c) on hand-derived answers with their exact FitError texts, the host's refusals through a
 fake runner, the compiler's per-class pod limit against its own guards, and the variant tables.  GPU: every probe kernel variant against
 the checker, probes against the recompile + simon_schedule_resume equivalence that pins the definition, the context state a probe batch
 leaves, chunking, the C-entry refusals and the session end to end."""
@@ -79,11 +79,11 @@ class CheckerEngine:
         self.calls = []
 
     def probe_run(self, placed, probes, detail=True):
-        import probe_oracle
+        import checkers
         self.calls.append(list(probes))
         out = []
         for q, r in probes:
-            d = probe_oracle.probe(self.o, placed, q, r)
+            d = checkers.probe(self.o, placed, q, r)
             st = self.o.state()
             d.update(req_mcpu=int(st["req_mcpu"].sum()), alloc_mcpu=int(self.c.snap["alloc_mcpu"].sum()),
                      req_mem=int(st["req_mem"].sum()), alloc_mem=int(self.c.snap["alloc_mem"].sum()))

@@ -1,5 +1,5 @@
 """Migration plans (simon_moves_plan, rebalance.py): a sequence of applied moves, each chosen on the state the earlier ones leave.
-CPU: the plan checker (tests/moves_plan_oracle.c) against a plan made by rebuilding the oracle from scratch before every step, and
+CPU: the plan checker (tests/checkers.c) against a plan made by rebuilding the oracle from scratch before every step, and
 the host-side helpers (candidate lists, MigrationPlan formatting).  GPU: the engine's plans against the checker, step by step and in
 their end state, plus the live state left untouched, an independent rebuild of the end state, refusals and the session entry point."""
 import copy
@@ -7,8 +7,7 @@ import copy
 import numpy as np
 import pytest
 
-import moves_plan_oracle as MP
-import moves_scope_oracle as MS
+import checkers
 from util import make_case
 
 GPU, HARD = 1, 2
@@ -29,7 +28,7 @@ def _sampled(out, c, n, seed=11):
 
 def _checker(c, mv, max_moves, min_gain=1, scope=0, class_local=None):
     o, out = _oracle_state(c)
-    res = MP.plan(o, mv, out, o.gpu_slot_words(), max_moves, min_gain, scope, class_local=class_local)
+    res = checkers.plan(o, mv, out, o.gpu_slot_words(), max_moves, min_gain, scope, class_local=class_local)
     o.close()
     res["live"] = out
     return res
@@ -60,7 +59,7 @@ def _rebuild_plan(p, c, out, mv, max_moves, min_gain, scope):
         pos[keep] = np.arange(len(keep))
         sel = np.nonzero(pos[mv[:, 0]] >= 0)[0]
         mv2 = np.stack([pos[mv[sel, 0]], mv[sel, 1]], 1).astype(np.uint32)
-        gain, code, _ = MS.moves_score(o2, mv2, out2, scope)
+        gain, code, _ = checkers.moves_score(o2, mv2, out2, scope)
         o2.close()
         ok = (code == 0) & np.array([int(mv[m, 0]) not in moved for m in sel], bool)
         if not ok.any():
@@ -197,7 +196,7 @@ def _engine_vs_checker(c, mv, max_moves, min_gain=1, scope=0, class_local=None, 
         from oracle.binding import Oracle
         o = Oracle(cf)
         o.schedule()
-        ref = MP.plan(o, mv, live, np.zeros(len(live), np.uint32), max_moves, min_gain, scope, class_local=class_local)
+        ref = checkers.plan(o, mv, live, np.zeros(len(live), np.uint32), max_moves, min_gain, scope, class_local=class_local)
         o.close()
         ref["live"] = live
     with Engine(c, device=0, static_cache=static_cache) as eng:

@@ -1,10 +1,10 @@
 """Move scope (simon_moves_set_scope): candidate moves of GPU-share classes and of classes with DoNotSchedule spread constraints.
-CPU: the scoped checker (tests/moves_scope_oracle.c, the oracle's own cycle stages) against the unscoped oracle, hand-derived known
+CPU: the scoped checker (tests/checkers.c, the oracle's own cycle stages) against the unscoped oracle, hand-derived known
 answers, and an object-level replay of sampled moves.  GPU: the engine's scoped runs against the checker."""
 import numpy as np
 import pytest
 
-import moves_scope_oracle as MS
+import checkers
 from simon_b200.abi import SFC_GPU, SFC_PTS_MISSING, SFC_PTS_SKEW, SFC_STATIC
 from util import make_case
 
@@ -58,7 +58,7 @@ def test_scope0_checker_equals_moves_score(kind, kw, n):
     p, c, o, out = _state(kind, **kw)
     mv = _moves(out, c, n)
     g0, c0 = o.moves_score(mv, out)
-    g1, c1, sl = MS.moves_score(o, mv, out, 0)
+    g1, c1, sl = checkers.moves_score(o, mv, out, 0)
     np.testing.assert_array_equal(c1, c0)
     np.testing.assert_array_equal(g1, g0)
     assert sl is None
@@ -73,7 +73,7 @@ def test_scope_bits_change_only_admitted_not_movable_codes(kind, kw, n):
     need = _needs(c)
     cls = c.pods["pod_class"][np.minimum(mv[:, 0], len(out) - 1)]
     for scope in (GPU, HARD, GPU | HARD):
-        g, code, sl = MS.moves_score(o, mv, out, scope)
+        g, code, sl = checkers.moves_score(o, mv, out, scope)
         admitted = (c0 == abi.MOVE_NOT_MOVABLE) & (need[cls] > 0) & ((need[cls] & ~scope) == 0)
         np.testing.assert_array_equal(code[~admitted], c0[~admitted])
         np.testing.assert_array_equal(g[~admitted], g0[~admitted])
@@ -100,14 +100,14 @@ def test_open_local_and_pinned_classes_stay_not_movable():
     cls = c.pods["pod_class"][np.minimum(mv[:, 0], len(out) - 1)]
     placed = (out[np.minimum(mv[:, 0], len(out) - 1)] >= 0) & (mv[:, 0] < len(out))
     for scope in (0, GPU | HARD):
-        g, code, _ = MS.moves_score(o, mv, out, scope, class_local=loc)
+        g, code, _ = checkers.moves_score(o, mv, out, scope, class_local=loc)
         sel = placed & (loc[cls] == 1) & (out[np.minimum(mv[:, 0], len(out) - 1)] != mv[:, 1])
         assert sel.sum() > 0 and (code[sel] == abi.MOVE_NOT_MOVABLE).all()
     # pinned (DaemonSet) classes of a mix cluster
     p, c2, o2, out2 = _state("mix", seed_no=103, n_nodes=95, n_workloads=40, max_replicas=7)
     mv2 = _moves(out2, c2, 20000)
     pinned = _needs(c2)[c2.pods["pod_class"][np.minimum(mv2[:, 0], len(out2) - 1)]] == -1
-    g, code, _ = MS.moves_score(o2, mv2, out2, GPU | HARD)
+    g, code, _ = checkers.moves_score(o2, mv2, out2, GPU | HARD)
     g0, c0 = o2.moves_score(mv2, out2)
     assert pinned.sum() > 0
     np.testing.assert_array_equal(code[pinned], c0[pinned])
@@ -174,14 +174,14 @@ def test_gpu_share_known_answers():
     at = dict(zip(names, out.tolist()))
     assert at["g12"] == B and at["big"] == T
     assert all(at[m] == S for m in ("m4", "m5", "d8", "d10"))
-    used = MS.gpu_used(o)
+    used = checkers.gpu_used(o)
     assert used[0, B] == 12 * GI and used[1, B] == 0
     pod = {nm: i for i, nm in enumerate(names)}
     mv = np.array([[pod[m], B] for m in ("m4", "m5", "d8", "d10", "big")] + [[pod["m4"], NO]], np.uint32)
     g0, c0 = o.moves_score(mv, out)
     assert (c0 == abi.MOVE_NOT_MOVABLE).all()                 # without the scope, GPU-share pods are not candidates
-    g, code, slots = MS.moves_score(o, mv, out, GPU)
-    assert MS.moves_score(o, mv, out, HARD)[1].tolist() == c0.tolist()
+    g, code, slots = checkers.moves_score(o, mv, out, GPU)
+    assert checkers.moves_score(o, mv, out, HARD)[1].tolist() == c0.tolist()
     want = [
         (0, 1),             # m4, 4 GiB: fits both devices (4, 16 free); the tightest is device 0, exactly full
         (0, 1 << 4),        # m5, 5 GiB: only device 1 holds it
@@ -247,8 +247,8 @@ def test_hard_spread_known_answers():
     assert out[p] == A1
     mv = np.array([[p, B1], [p, A2], [p, N0], [p, C1], [p, X1]], np.uint32)
     assert (o.moves_score(mv, out)[1] == abi.MOVE_NOT_MOVABLE).all()
-    g, code, _ = MS.moves_score(o, mv, out, HARD)
-    assert MS.moves_score(o, mv, out, GPU)[1].tolist() == [abi.MOVE_NOT_MOVABLE] * 5
+    g, code, _ = checkers.moves_score(o, mv, out, HARD)
+    assert checkers.moves_score(o, mv, out, GPU)[1].tolist() == [abi.MOVE_NOT_MOVABLE] * 5
     assert code.tolist() == [
         1 << SFC_PTS_SKEW,      # b1: p leaves A, so A = 0 and the minimum drops to 0: 1 + 1 - 0 > 1 (without the removal: 1 + 1 - 1 = 1)
         0,                          # a2: A's count without p is 0: 0 + 1 - 0 = 1
@@ -272,7 +272,7 @@ def test_scoped_moves_replay_on_objects(kind, kw, seed):
     p, c, o, out = _state(kind, **kw)
     need = _needs(c)
     mv = _moves(out, c, 20000, seed=seed)
-    g, code, _ = MS.moves_score(o, mv, out, HARD)
+    g, code, _ = checkers.moves_score(o, mv, out, HARD)
     cls = c.pods["pod_class"][np.minimum(mv[:, 0], len(out) - 1)]
     pre = np.array([bool(r.node_name) for r in p.pods])
     cand = np.nonzero((need[cls] == HARD) & (code < (1 << 24)) & ~pre[np.minimum(mv[:, 0], len(out) - 1)])[0]
@@ -313,7 +313,7 @@ def _stage_of(code):
 def _engine_vs_checker(c, o, out, mv, scope, class_local=None, static_cache=True):
     from simon_b200 import moves as M
     from simon_b200.engine import Engine
-    gain, code, slots = MS.moves_score(o, mv, out, scope, class_local=class_local)
+    gain, code, slots = checkers.moves_score(o, mv, out, scope, class_local=class_local)
     with Engine(c, device=0, static_cache=static_cache) as eng:
         np.testing.assert_array_equal(eng.schedule()[0], out)
         eng.moves_set_scope(scope)

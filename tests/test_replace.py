@@ -1,10 +1,10 @@
 """Node-pool replacement (simon_b200.replace, Simulator.PlanNodeReplacement, simon_wave_run_join / simon_wave_commit_retire) on the
-CPU: the planner on the replacement checker (tests/replace_oracle.c) against hand-derived answers, and the host refusals."""
+CPU: the planner on the wave checker (tests/checkers.c) against hand-derived answers, and the host refusals."""
 import numpy as np
 import pytest
 
-import grow_oracle
-from replace_oracle import OracleRunner
+import checkers
+from checkers import OracleRunner
 from simon_b200 import grow, objects as O, replace, simulator
 from test_grow import _dep, _ds, _node, session
 
@@ -29,7 +29,7 @@ def plan_cpu(sim, nodes, spec, kmax=None, caps=(100, 100), **kw):
     c, placed, present, pool, copies, pdbs = replace.superset(sim, nodes, spec, kmax)
     o = Oracle(c)
     n_prefix = len(sim.placements)
-    grow_oracle.grow(o, placed, n_prefix, np.nonzero(present)[0].astype(np.uint32))
+    checkers.grow(o, placed, n_prefix, np.nonzero(present)[0].astype(np.uint32))
     runner = OracleRunner(o, pdbs)
     plan = replace.plan_replacement(c, placed, runner, present, pool, copies, caps=caps, pdbs=pdbs, **kw)
     o.close()

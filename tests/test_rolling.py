@@ -1,4 +1,4 @@
-"""Rolling node maintenance (simon_b200.rolling, simon_wave_*) on the CPU: the planner on the wave checker (tests/rolling_oracle.c)
+"""Rolling node maintenance (simon_b200.rolling, simon_wave_*) on the CPU: the planner on the wave checker (tests/checkers.c)
 against hand-derived answers, the planner's rules and refusals on fake runners, the ABI and the session's refusals without a
 device."""
 import numpy as np
@@ -44,13 +44,13 @@ def four_nodes(replicas=8, pods=()):
 
 
 def _checker_plan(c, pdb_objs=None, **kw):
-    import rolling_oracle
+    import checkers
     from oracle.binding import Oracle
     from simon_b200.disruption import compile_pdbs
     o = Oracle(c)
     placed = o.schedule()[0]
     pdbs = compile_pdbs(pdb_objs, c) if pdb_objs else None
-    runner = rolling_oracle.OracleRunner(o, pdbs)
+    runner = checkers.OracleRunner(o, pdbs)
     kw.setdefault("caps", (100, 100))
     return rolling.plan_rolling(c, placed, runner, pdbs=pdbs, **kw), placed, runner
 
@@ -151,14 +151,14 @@ def test_given_order_against_utilisation():
 def test_checker_waves_keep_the_state_consistent_on_mixed_clusters(seed):
     """On a mixed cluster each committed base equals the state its placement leaves when every pod sits where the base says, up to
     GPU devices: node sums and pod counts match a drain checker run with nothing removed from that placement."""
-    import drain_oracle
+    import checkers
     from oracle.binding import Oracle
     c = _compiled(*synth.make_mix(seed_no=seed, n_nodes=30))
     plan, _placed, runner = _checker_plan(c, max_unavailable=3)
     assert plan.TotalWaves + len(plan.Skipped) <= c.n_nodes and plan.TotalWaves > 0
     final, _slots = runner.placement()
     o2 = Oracle(c)
-    drain_oracle.drain(o2, final, np.arange(c.n_nodes, dtype=np.uint32))
+    checkers.drain(o2, final, np.arange(c.n_nodes, dtype=np.uint32))
     want, got = o2.state(), runner.o.state()
     for k in ("req_mcpu", "req_mem", "req_eph", "nz_mcpu", "nz_mem", "num_pods"):
         assert np.array_equal(got[k], want[k]), k

@@ -1,6 +1,6 @@
 """Trace replay (simon_trace_run, Engine.trace_run, simon_b200.trace, Simulator.ReplayTrace) on the CPU.
 
-The replay (trace.build + trace.replay) runs here on the trace checker (tests/trace_oracle.c), which applies one event at a time with the
+The replay (trace.build + trace.replay) runs here on the trace checker (tests/checkers.c), which applies one event at a time with the
 oracle's own primitives, on hand-derived cases: a delete that frees room for a later create, required anti-affinity unblocked by
 deleting the peer, spread skew falling after deletes, a GPU-share device freed and reused, a host port freed, extended resources, a
 deleted pre-bound pod; the host refusals; and the ordering rule of trace.from_lifetimes."""
@@ -49,10 +49,10 @@ class CheckerEngine:
         self.o = Oracle(c)
 
     def trace_run(self, placed, n_prefix, events, scenarios=None, samples=None, detail=True, chunk=None):
-        import trace_oracle
+        import checkers
         out = []
         for nodes in scenarios:
-            r = trace_oracle.trace(self.o, placed, n_prefix, nodes, events)
+            r = checkers.trace(self.o, placed, n_prefix, nodes, events)
             idx = np.asarray([] if samples is None else samples, np.int64)
             pts = np.zeros(len(idx), abi.TRACE_POINT_DTYPE)
             pts["event"] = idx

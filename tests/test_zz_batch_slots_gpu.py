@@ -5,7 +5,7 @@ their node-slot loops with run-time slot counts.  Their variant tests use 40- an
 node, but production batches on 10,000 nodes run at 2 to 4 slots per thread.  Here each of them, the
 large-cluster ones included, runs at two forced geometries of 2 or more slots on the 1,200-node dense mix
 (test_zz_kernel_variants_gpu._dense) or on a 1,000-node Open-Local mixed cluster with devices (test_open_local_oracle.make_mixed_local),
-and every drain and probe is compared with tests/drain_oracle.c and tests/probe_oracle.c.  The 256-thread and large-cluster kernels
+and every drain and probe is compared with the drain and probe checkers (tests/checkers.c).  The 256-thread and large-cluster kernels
 also run at 16 or more slots on one CTA.  The 320-thread kernels run at 4 slots on one CTA, and the 384-thread ones at 3 on one CTA
 (Open-Local) or 2 on two (dense: one CTA's shared memory does not hold 1,200 nodes at 352 threads).  8 slots at 257 or more threads
 would need more than 2,000 node slots in one CTA.  The checkers' answers do not depend on the geometry, so each family's are computed once.
@@ -160,9 +160,9 @@ def _vg_sums(c, vg, rl):
 
 
 def checker_drains(c, placed, drains):
-    """tests/drain_oracle.c on a fresh oracle: per drain the checker's result, its occupancy sums and, with Open-Local, the VG sums
+    """The drain checker on a fresh oracle: per drain the checker's result, its occupancy sums and, with Open-Local, the VG sums
     and the VG and device state; -> (remaining-node lists, answers, the live VG and device state)."""
-    import drain_oracle
+    import checkers
     local = getattr(c, "storage", None) is not None
     order = scaledown.NodeOrder(c)
     remain = [order.remaining(d) for d in drains]
@@ -172,7 +172,7 @@ def checker_drains(c, placed, drains):
         live = o.storage_state() if local else None
         wants = []
         for rl in remain:
-            w = drain_oracle.drain(o, placed, rl)
+            w = checkers.drain(o, placed, rl)
             w.update(_occupancy(c, o.state(), rl))
             if local:
                 vg, dev = o.storage_state()
@@ -185,16 +185,16 @@ def checker_drains(c, placed, drains):
 
 
 def checker_probes(c, placed, probes):
-    """tests/probe_oracle.c on a fresh oracle: per probe the checker's result, the request sums over every node and, with Open-Local,
+    """The probe checker on a fresh oracle: per probe the checker's result, the request sums over every node and, with Open-Local,
     the VG sum and the VG and device state."""
-    import probe_oracle
+    import checkers
     local = getattr(c, "storage", None) is not None
     o = _oracle(c)
     try:
         np.testing.assert_array_equal(o.schedule()[0], placed)
         wants = []
         for q, r in probes:
-            w = probe_oracle.probe(o, placed, q, r)
+            w = checkers.probe(o, placed, q, r)
             st = o.state()
             w.update(req_mcpu=int(st["req_mcpu"].sum()), req_mem=int(st["req_mem"].sum()))
             if local:
@@ -348,8 +348,7 @@ def test_production_batches_10000_nodes_in_the_engines_geometry():
     probes of up to 64 replicas, each batch in one launch of the geometry the engine picks for it.  That geometry holds each
     scenario in 2 or more node slots per thread, and the batch has more CTAs than the device has SMs (one CTA per SM at this shared
     memory), so its scenarios run in several waves.  12 drains and 8 probes are compared with the checkers."""
-    import drain_oracle
-    import probe_oracle
+    import checkers
     import torch
     from test_drain import _assert_drain_equal
     from test_zz_headroom_gpu import _assert_probe_equal, _probe_pods
@@ -381,7 +380,7 @@ def test_production_batches_10000_nodes_in_the_engines_geometry():
     t0 = time.perf_counter()
     try:
         for j in sample:
-            w = drain_oracle.drain(o, placed, remain[j])
+            w = checkers.drain(o, placed, remain[j])
             _assert_drain_equal(got[j], w, f"drain {j}")
             np.testing.assert_array_equal(got[j]["score"], w["score"], err_msg=f"drain {j}: scores")
             occ = _occupancy(c, o.state(), remain[j])
@@ -394,7 +393,7 @@ def test_production_batches_10000_nodes_in_the_engines_geometry():
     try:
         for j in range(0, 32, 4):
             q, r = probes[j]
-            _assert_probe_equal(gotp[j], probe_oracle.probe(o, placed, q, r), f"probe {q} x {r}")
+            _assert_probe_equal(gotp[j], checkers.probe(o, placed, q, r), f"probe {q} x {r}")
     finally:
         o.close()
     t_probes = time.perf_counter() - t0

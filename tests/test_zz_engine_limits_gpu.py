@@ -115,7 +115,7 @@ def test_resume_from_half_rebuilds_the_state(name):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", sorted(BUILDERS))
 def test_drains_match_checker(name):
-    import drain_oracle
+    import checkers
     from oracle.binding import Oracle
     from simon_b200 import scaledown
     from test_drain import _assert_drain_equal
@@ -130,7 +130,7 @@ def test_drains_match_checker(name):
     with _engine(c, record_scores=True) as eng:
         got = eng.drain_run(placed, remain)
     for d, rl, g in zip(drains, remain, got):
-        want = drain_oracle.drain(o, placed, rl)
+        want = checkers.drain(o, placed, rl)
         _assert_drain_equal(g, want, f"{name} drain {d}")
         pos = g["node"] >= 0
         assert np.array_equal(g["score"][pos], want["score"][pos]), d

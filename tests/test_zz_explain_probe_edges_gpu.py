@@ -1,5 +1,5 @@
 """Explained decisions (simon_explain_kernel_*) and headroom probes (simon_probe_kernel_*) at the engine limits, the score-range edges
-and past 65,536 nodes, against the CPU checkers (explain_oracle.expected, probe_oracle.probe), exactly.
+and past 65,536 nodes, against the CPU checkers (explain_oracle.expected, checkers.probe), exactly.
 
 A. Every builder of test_engine_limits.py, every pod explained at top_k 16 (15 extra max-reductions per decision) on the geometries
    of test_explain_probe_edges.limit_geoms, and without the static-verdict cache on three of them; one run at top_k 1.
@@ -250,12 +250,12 @@ def test_simulator_explain_open_local_session():
 
 def _want_probes(c, placed, probes, open_local=False):
     """The checker's probes, with the occupancy sums the engine reports."""
-    import probe_oracle
+    import checkers
     from oracle.binding import Oracle
     o = Oracle(c, threads=THREADS, open_local=open_local)
     out = []
     for q, r in probes:
-        w = probe_oracle.probe(o, placed, q, r)
+        w = checkers.probe(o, placed, q, r)
         st = o.state()
         w["sums"] = (int(st["req_mcpu"].sum()), int(c.snap["alloc_mcpu"].sum()), int(st["req_mem"].sum()), int(c.snap["alloc_mem"].sum()))
         out.append(w)

@@ -1,7 +1,7 @@
 """Grow batches on the device (simon_grow_run, Engine.grow_run, Simulator.PlanAddNodes).
 
 Every batch placement variant a grow batch launches - with and without the static-verdict cache, the large-cluster variant and forced
-geometries with several node slots per thread - against the grow checker (tests/grow_oracle.c) on plain, GPU-share and Open-Local
+geometries with several node slots per thread - against the grow checker (tests/checkers.c) on plain, GPU-share and Open-Local
 clusters; the recompile-and-resume equivalence that pins the definition; chunking; the batch pool shared with drains and probes; the
 C-entry refusals; and PlanAddNodes end to end on the reference example."""
 import copy
@@ -74,14 +74,14 @@ def _case(kind, n_nodes=200):
 def _check(eng, gs, raw, sids):
     """Every scenario of `raw` (Engine.grow_run with detail) against the grow checker, the Open-Local state too."""
     from oracle.binding import Oracle
-    import grow_oracle
+    import checkers
     c = gs.compiled
     local = c.storage is not None
     o = Oracle(c, open_local=local)
     try:
         for i, (sid, r) in enumerate(zip(sids, raw)):
             sc = gs.scenarios[sid]
-            w = grow_oracle.grow(o, gs.placed, gs.n_prefix, sc.nodes)
+            w = checkers.grow(o, gs.placed, gs.n_prefix, sc.nodes)
             for key in ("node", "score", "gpu_slots", "fail_counts", "fail_pod"):
                 assert np.array_equal(r[key], w[key]), (sid, key)
             assert (r["n_scheduled"], r["n_unscheduled"]) == (w["n_scheduled"], w["n_unscheduled"]), sid

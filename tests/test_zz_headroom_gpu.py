@@ -1,4 +1,4 @@
-"""Headroom probes on the device (simon_probe_run): every probe kernel variant against the CPU checker (tests/probe_oracle.c), with and
+"""Headroom probes on the device (simon_probe_run): every probe kernel variant against the CPU checker (tests/checkers.c), with and
 without the static-verdict cache, the recompile + simon_schedule_resume equivalence that pins the definition on the workload and the
 template path, the context state a probe batch leaves, chunking, the C-entry refusals and the session end to end."""
 import copy
@@ -44,7 +44,7 @@ def _assert_probe_equal(g, want, what):
 
 @pytest.mark.parametrize("kernel", sorted(PROBE_VARIANTS))
 def test_probe_variant_matches_checker(kernel):
-    import probe_oracle
+    import checkers
     from oracle.binding import Oracle
     cs, t, big = PROBE_VARIANTS[kernel]
     rng = np.random.default_rng(23)
@@ -62,7 +62,7 @@ def test_probe_variant_matches_checker(kernel):
                 li = eng.last_launch()
                 assert li["kernel"] == kernel and li["n_scenarios"] == len(probes) and li["large"] == big, li
             for (q, r), g in zip(probes, got):
-                want = probe_oracle.probe(o, placed, q, r)
+                want = checkers.probe(o, placed, q, r)
                 _assert_probe_equal(g, want, f"{kernel} seed {seed} pod {q} static_cache {static_cache}")
                 st = o.state()
                 assert (g["req_mcpu"], g["req_mem"]) == (int(st["req_mcpu"].sum()), int(st["req_mem"].sum()))
@@ -74,7 +74,7 @@ def test_probe_variant_matches_checker(kernel):
 @pytest.mark.parametrize("kernel", sorted(PROBE_LOCAL_VARIANTS))
 def test_probe_local_variant_matches_storage_checker(kernel):
     """The Open-Local family against the checker on the oracle with Open-Local: replicas, VG sums and each probe's VG and device state."""
-    import probe_oracle
+    import checkers
     from oracle.binding import Oracle
     cs, t, big = PROBE_LOCAL_VARIANTS[kernel]
     seed = 61 + sorted(PROBE_LOCAL_VARIANTS).index(kernel)
@@ -95,7 +95,7 @@ def test_probe_local_variant_matches_storage_checker(kernel):
             assert li["kernel"] == kernel and li["local"] and li["large"] == big, li
             states = [eng.scenario_storage_state(i) for i in range(len(probes))]
         for (q, r), g, (bvg, bdev) in zip(probes, got, states):
-            want = probe_oracle.probe(o, placed, q, r)
+            want = checkers.probe(o, placed, q, r)
             _assert_probe_equal(g, want, f"{kernel} pod {q}")
             vg, dev = o.storage_state()
             np.testing.assert_array_equal(bvg, vg, err_msg=f"pod {q}: VG state")

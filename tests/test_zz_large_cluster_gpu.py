@@ -131,12 +131,12 @@ def test_single_flip_fast_path_fires_on_the_large_variant():
 def test_zone_flip_probe_stops_when_nothing_is_feasible(n_a):
     """A headroom probe of the Deployment's pod on the empty cluster places replica 1 on zone a, replica 2 on zone b after the
     wrap-sized flip (score 0) and stops at replica 3, where no node is feasible (the probe's stop reads the feasible count)."""
-    import probe_oracle
+    import checkers
     from oracle.binding import Oracle
     c = zone_case(n_a, 1, 3)
     placed = np.full(c.pods_dims["n_pods"], -1, np.int32)
     o = Oracle(c, threads=THREADS)
-    want = probe_oracle.probe(o, placed, 0, 5)
+    want = checkers.probe(o, placed, 0, 5)
     o.close()
     assert want["n_placed"] == 2 and want["stop_reason"] == abi.PROBE_STOP_UNSCHEDULABLE and want["score"][1] == 0
     with _engine(c) as eng:
@@ -307,7 +307,7 @@ def _live(size):
 
 @pytest.mark.parametrize("size", sorted(SIZES))
 def test_drains(size):
-    import drain_oracle
+    import checkers
     from simon_b200 import scaledown
     from test_drain import _assert_drain_equal
     c, o, placed = _live(size)
@@ -321,7 +321,7 @@ def test_drains(size):
         for li in eng.last_drain["launches"]:
             _assert_large(li, c.n_nodes, li["n_scenarios"])
     for d, rl, g in zip(drains, remain, got):
-        want = drain_oracle.drain(o, placed, rl)
+        want = checkers.drain(o, placed, rl)
         _assert_drain_equal(g, want, f"drain of {len(d)} nodes")
         pos = g["node"] >= 0
         np.testing.assert_array_equal(g["score"][pos], want["score"][pos])
@@ -331,7 +331,7 @@ def test_drains(size):
 
 @pytest.mark.parametrize("size", sorted(SIZES))
 def test_probes(size):
-    import probe_oracle
+    import checkers
     from test_zz_headroom_gpu import _probe_pods
     c, o, placed = _live(size)      # an oracle of its own: see test_open_local_place_drain_probe_70k
     probes = list(zip(_probe_pods(c, np.random.default_rng(11), 4), (1, 7, 40, 200)))
@@ -340,7 +340,7 @@ def test_probes(size):
         for li in eng.last_probe["launches"]:
             _assert_large(li, c.n_nodes, li["n_scenarios"])
     for (q, r), g in zip(probes, got):
-        want = probe_oracle.probe(o, placed, q, r)
+        want = checkers.probe(o, placed, q, r)
         assert (g["n_placed"], g["stop_reason"]) == (want["n_placed"], want["stop_reason"]), (q, r)
         for k in ("node", "score", "gpu_slots", "fail_counts"):
             np.testing.assert_array_equal(g[k], want[k], err_msg=f"probe {q} of {r}: {k}")
@@ -384,8 +384,7 @@ def local_oracle_full():
 
 
 def test_open_local_place_drain_probe_70k():
-    import drain_oracle
-    import probe_oracle
+    import checkers
     from oracle.binding import Oracle
     from simon_b200 import scaledown
     from test_zz_headroom_gpu import _probe_pods
@@ -417,7 +416,7 @@ def test_open_local_place_drain_probe_70k():
                 _assert_large(li, c.n_nodes, li["n_scenarios"])
             states = [eng.scenario_storage_state(i) for i in range(len(drains))] if eng.last_drain["chunks"] == 1 else None
         for j, (d, rl, g) in enumerate(zip(drains, remain, got)):
-            want = drain_oracle.drain(o, placed, rl)
+            want = checkers.drain(o, placed, rl)
             for k in ("n_evicted", "n_placed", "n_unscheduled", "n_blocked", "n_vanished"):
                 assert g[k] == want[k], (d, k)
             for k in ("evicted", "node", "score", "gpu_slots", "blocked", "fail_pod", "fail_counts"):
@@ -446,7 +445,7 @@ def test_open_local_place_drain_probe_70k():
                 _assert_large(li, c.n_nodes, li["n_scenarios"])
             pstates = [eng.scenario_storage_state(i) for i in range(len(probes))] if eng.last_probe["chunks"] == 1 else None
         for j, ((q, r), g) in enumerate(zip(probes, gotp)):
-            want = probe_oracle.probe(o, placed, q, r)
+            want = checkers.probe(o, placed, q, r)
             assert (g["n_placed"], g["stop_reason"]) == (want["n_placed"], want["stop_reason"]), (q, r)
             for k in ("node", "score", "gpu_slots", "fail_counts"):
                 np.testing.assert_array_equal(g[k], want[k], err_msg=f"probe {q} of {r}: {k}")

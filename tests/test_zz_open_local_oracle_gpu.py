@@ -1,7 +1,7 @@
 """Every Open-Local kernel path against the CPU oracle with Open-Local (Oracle(c, open_local=True)) on clusters that mix it with
 every other plugin (test_open_local_oracle.make_mixed_local): placement with each simon_local_kernel_* variant, the per-node totals
 and verdicts of sampled pods, scenario batches (simon_scenarios_run_local), resumed runs (simon_schedule_resume) and drains with
-each simon_drain_local_kernel_* variant (simon_drain_run_local, against tests/drain_oracle.c on the storage oracle)."""
+each simon_drain_local_kernel_* variant (simon_drain_run_local, against the drain checker on the storage oracle)."""
 import functools
 import os
 
@@ -185,10 +185,10 @@ def test_resume_from_the_oracle_prefix(n_nodes, seed):
 @pytest.mark.parametrize("kernel", sorted(DRAIN_LOCAL_VARIANTS))
 def test_drain_local_kernel_matches_storage_oracle(kernel):
     """simon_drain_run_local with each drain-local kernel, from the oracle's full placement (the engine's own), against
-    tests/drain_oracle.c on the oracle with Open-Local (local volumes move, so class_local is not passed): the evicted pods, their
+    The drain checker on the oracle with Open-Local (local volumes move, so class_local is not passed): the evicted pods, their
     nodes, scores, GPU slots and failures, the VG sums over the remaining annotated nodes, and each drain's VG and device state
     (remaining nodes: the drain oracle's; removed nodes: the live state)."""
-    import drain_oracle
+    import checkers
     cs, t, big = DRAIN_LOCAL_VARIANTS[kernel]
     n_nodes, seed = 120, 41 + sorted(DRAIN_LOCAL_VARIANTS).index(kernel)
     c = cluster(n_nodes, seed)
@@ -211,7 +211,7 @@ def test_drain_local_kernel_matches_storage_oracle(kernel):
     moved = 0
     try:
         for j, (d, rl, g) in enumerate(zip(drains, remain, got)):
-            r = drain_oracle.drain(o, placed, rl)
+            r = checkers.drain(o, placed, rl)
             for k in ("n_evicted", "n_placed", "n_unscheduled", "n_blocked", "n_vanished"):
                 assert g[k] == r[k], (d, k)
             for k in ("evicted", "node", "score", "gpu_slots", "blocked", "fail_pod", "fail_counts"):

@@ -1,5 +1,5 @@
 """Node-pool replacement on the device (simon_wave_begin_pool / simon_wave_run_join / simon_wave_commit_retire, Engine.wave_*,
-Simulator.PlanNodeReplacement) against the replacement checker (tests/replace_oracle.c): whole plans run in lockstep on both, every
+Simulator.PlanNodeReplacement) against the wave checker (tests/checkers.c): whole plans run in lockstep on both, every
 batch and every committed base compared, at the four drain geometries, without the static-verdict cache and with PDBs; every wave
 batch against the compile-and-resume definition on clusters without GPU share; a GPU-share case where a rebuild would give a moved pod
 another device; the C-entry refusals; session safety."""
@@ -9,7 +9,7 @@ import re
 import numpy as np
 import pytest
 
-import grow_oracle
+import checkers
 from simon_b200 import objects as O, replace, rolling, synth
 from simon_b200.quantity import Quantity
 from test_grow import session
@@ -26,8 +26,7 @@ class LockstepRunner(rolling.WaveRunner):
     base's placement, slot words, node states, node aggregates, scalars and GPU memory."""
 
     def __init__(self, eng, o, pdbs=None, kernel=None):
-        import replace_oracle
-        self.eng, self.chk, self.kernel = eng, replace_oracle.OracleRunner(o, pdbs), kernel
+        self.eng, self.chk, self.kernel = eng, checkers.OracleRunner(o, pdbs), kernel
         self.dev = rolling.EngineRunner(eng)
         self.batches = self.commits = 0
 
@@ -92,7 +91,7 @@ def _lockstep(sim, nodes, spec, eng_kw=None, pdb_objs=None, kernel=None, **kw):
     if pdb_objs:
         pdbs = compile_pdbs(pdb_objs, c)
     o = Oracle(c, threads=8)
-    grow_oracle.grow(o, placed, len(sim.placements), np.nonzero(present)[0].astype(np.uint32))
+    checkers.grow(o, placed, len(sim.placements), np.nonzero(present)[0].astype(np.uint32))
     with Engine(c, record_scores=True, **(eng_kw or {})) as eng:
         if pdbs is not None:
             eng.pdbs_upload(pdbs)

@@ -1,5 +1,5 @@
 """Rolling node maintenance on the device (simon_wave_*, Engine.wave_*, Simulator.PlanRollingMaintenance) against the wave checker
-(tests/rolling_oracle.c): full plans run in lockstep on both, every batch and every committed base compared; wave batches against
+(tests/checkers.c): full plans run in lockstep on both, every batch and every committed base compared; wave batches against
 simon_drain_run from the same placement; a GPU-share case where a rebuild would give a moved pod other devices; session safety."""
 import numpy as np
 import pytest
@@ -26,8 +26,8 @@ class LockstepRunner(rolling.WaveRunner):
     the same batch (clusters without GPU share)."""
 
     def __init__(self, eng, o, pdbs=None, drain_eng=None, kernel=None):
-        import rolling_oracle
-        self.eng, self.chk, self.drain_eng, self.kernel = eng, rolling_oracle.OracleRunner(o, pdbs), drain_eng, kernel
+        import checkers
+        self.eng, self.chk, self.drain_eng, self.kernel = eng, checkers.OracleRunner(o, pdbs), drain_eng, kernel
         self.dev = rolling.EngineRunner(eng)
         self.batches = 0
 

@@ -143,7 +143,7 @@ def test_scenario_batch_matches_oracle_same_key():
 def test_drain_batch_matches_checker_same_key(kernel):
     """Drains take each evicted pod's counter increments out of the live state (as many as its class's multiplicity) before
     placing it again: against the drain checker, which rebuilds every drain's state from empty."""
-    import drain_oracle
+    import checkers
     from simon_b200 import scaledown
     cs, t, big = TD.DRAIN_VARIANTS[kernel]
     rng = np.random.default_rng(5)
@@ -158,7 +158,7 @@ def test_drain_batch_matches_checker_same_key(kernel):
             assert eng.last_launch()["kernel"] == kernel
         n_evicted = 0
         for d, rl, g in zip(drains, remain, got):
-            want = drain_oracle.drain(o, placed, rl)
+            want = checkers.drain(o, placed, rl)
             TD._assert_drain_equal(g, want, f"{kernel} seed {seed} drain {d}")
             n_evicted += g["n_evicted"]
         assert n_evicted > 0

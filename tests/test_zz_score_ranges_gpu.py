@@ -90,7 +90,7 @@ def test_scenario_batch_matches_oracle(name):
 
 @pytest.mark.parametrize("name", NA_CASES + PTS_CASES)
 def test_drains_match_checker(name):
-    import drain_oracle
+    import checkers
     from oracle.binding import Oracle
     from simon_b200 import scaledown
     from simon_b200.engine import Engine
@@ -105,7 +105,7 @@ def test_drains_match_checker(name):
     with Engine(c, device=0, record_scores=True) as eng:
         got = eng.drain_run(placed, remain)
     for d, rl, g in zip(drains, remain, got):
-        want = drain_oracle.drain(o, placed, rl)
+        want = checkers.drain(o, placed, rl)
         _assert_drain_equal(g, want, f"{name} drain {d}")
         pos = g["node"] >= 0
         assert pos.any() and np.array_equal(g["score"][pos], want["score"][pos]), d

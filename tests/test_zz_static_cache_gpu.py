@@ -132,7 +132,7 @@ def test_scenario_batch_matches_oracle_uncached(kernel, cs, t, big):
 
 @pytest.mark.parametrize("kernel", sorted(TD.DRAIN_VARIANTS))
 def test_drain_variant_matches_checker_uncached(kernel):
-    import drain_oracle
+    import checkers
     from simon_b200 import scaledown, synth
     cs, t, big = TD.DRAIN_VARIANTS[kernel]
     rng = np.random.default_rng(11)
@@ -146,7 +146,7 @@ def test_drain_variant_matches_checker_uncached(kernel):
             got = eng.drain_run(placed, remain)
             assert eng.last_launch()["kernel"] == kernel
         for d, rl, g in zip(drains, remain, got):
-            want = drain_oracle.drain(o, placed, rl)
+            want = checkers.drain(o, placed, rl)
             TD._assert_drain_equal(g, want, f"{kernel} seed {seed} drain {d} uncached")
             pos = g["node"] >= 0
             assert np.array_equal(g["score"][pos], want["score"][pos]), d

@@ -1,7 +1,7 @@
 """Trace replay on the device (simon_trace_run, Engine.trace_run, Simulator.ReplayTrace).
 
 Every run of a trace - creates placed by the batch placement variants, deletes by simon_trace_remove, samples by simon_trace_sample -
-against the trace checker (tests/trace_oracle.c), which applies one event at a time: nodes, GPU slot words, scores, failure histograms
+against the trace checker (tests/checkers.c), which applies one event at a time: nodes, GPU slot words, scores, failure histograms
 and the samples after every event.  The own-score cache and feasible-set summary hazards a removal creates are built on purpose; random
 mixes run under forced geometries, with the static-verdict cache off and on the large-cluster variant; a trace without deletes equals a
 grow batch; each scenario of a batch equals the same trace alone; the C-entry refusals; ReplayTrace end to end with a sweep over k."""
@@ -63,7 +63,7 @@ def _random_trace(gs, rng, p_delete=0.4, max_run=4):
 
 
 def _check(eng, gs, events, scenarios, what=""):
-    import trace_oracle
+    import checkers
     from oracle.binding import Oracle
     E = len(events)
     # every 7th event and the last: most runs hold several events, as without samples
@@ -71,7 +71,7 @@ def _check(eng, gs, events, scenarios, what=""):
     got = eng.trace_run(gs.placed, gs.n_prefix, events, scenarios, samples=at, detail=True)
     o = Oracle(gs.compiled)
     for i, nodes in enumerate(scenarios):
-        want = trace_oracle.trace(o, gs.placed, gs.n_prefix, nodes, events)
+        want = checkers.trace(o, gs.placed, gs.n_prefix, nodes, events)
         g = got[i]
         w = f"{what} scenario {i}"
         np.testing.assert_array_equal(g["node"], want["node"], err_msg=w)

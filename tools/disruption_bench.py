@@ -64,11 +64,11 @@ with Engine(live, device=0) as eng:
                                blocked=r["pdb_blocked"],
                                exhausted=len(disruption.exhausted(t, allowed, r["steps"]["pod"])) if t is not None else 0))
             if k != "none" and a.check and _ == 0:
-                import moves_plan_pdb_oracle as MPP
+                import checkers
                 from oracle.binding import Oracle
                 o = Oracle(live)
                 o.schedule()
-                ref = MPP.plan_pdb(o, mv, out, o.gpu_slot_words(), a.check, 1, 0, t.pod_off, t.pod_pdb, allowed)
+                ref = checkers.plan_pdb(o, mv, out, o.gpu_slot_words(), a.check, 1, 0, t.pod_off, t.pod_pdb, allowed)
                 o.close()
                 s = r["steps"][:a.check]
                 got = np.stack([s["move"], s["pod"], s["from"], s["to"], s["gain"], s["gpu_slots"]], 1).astype(np.int64)

@@ -55,12 +55,12 @@ with Engine(live, device=0) as eng:
           f"{pass_ms * 1e3:.1f} us -> apply + loop {(r['kernel_ms'] / max(n, 1) - pass_ms) * 1e3:.1f} us per step; "
           f"gains {int(r['steps']['gain'][0]) if n else None} .. {int(r['steps']['gain'][-1]) if n else None}", flush=True)
     if a.check:
-        import moves_plan_oracle as MP
+        import checkers
         from oracle.binding import Oracle
         o = Oracle(live)
         o.schedule()
         t2 = time.perf_counter()
-        ref = MP.plan(o, mv, out, o.gpu_slot_words(), a.check)
+        ref = checkers.plan(o, mv, out, o.gpu_slot_words(), a.check)
         cpu = time.perf_counter() - t2
         same = np.array_equal(ref["steps"], steps_of(r)[:a.check])
         print(f"C5 checker: first {a.check} steps identical: {same}; CPU checker {cpu / a.check * 1e3:.0f} ms per step", flush=True)

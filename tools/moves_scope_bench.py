@@ -1,6 +1,6 @@
 """Move scope timing: 1M candidate moves on a 10k-node cluster whose GPU-share pods were placed by the engine (so they hold device
 memory), scored unscoped and with GPU share + hard spread in scope, alternating, on the same list; then 20,000 moves against the
-scoped checker (tests/moves_scope_oracle.c on the CPU oracle)."""
+scoped checker (tests/checkers.c on the CPU oracle)."""
 import argparse
 import os
 import sys
@@ -70,13 +70,13 @@ nm0, nm1 = int((runs[0]["code"] == abi.MOVE_NOT_MOVABLE).sum()), int((code == ab
 print(f"NOT_MOVABLE: {nm0} unscoped -> {nm1} scoped ({nm0 - nm1} moves left it); feasible {runs[0]['n_feasible']} -> {runs[SCOPE]['n_feasible']}; "
       f"feasible GPU-share moves with device slots: {int((runs[SCOPE]['gpu_slots'] != 0).sum())}")
 if a.check:
-    import moves_scope_oracle as MS
+    import checkers
     from oracle.binding import Oracle
     t1 = time.time()
     o = Oracle(c, threads=min(32, os.cpu_count() or 1))
     ref = o.schedule()[0]
     same = bool(np.array_equal(ref, out))
-    g, cd, sl = MS.moves_score(o, mv[:a.check], out, SCOPE)
+    g, cd, sl = checkers.moves_score(o, mv[:a.check], out, SCOPE)
     ok = same and np.array_equal(g, runs[SCOPE]["gain"][:a.check]) and np.array_equal(cd, code[:a.check]) and \
         np.array_equal(sl, runs[SCOPE]["gpu_slots"][:a.check])
     print(f"checker on {a.check} moves: {'PASS' if ok else 'FAIL'} (placements equal: {same}; {time.time() - t1:.0f} s)")

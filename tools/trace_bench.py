@@ -4,7 +4,7 @@ The session is synth.make_c3 (GPU share on about --gpu-pct % of the nodes) after
 session's own pod shapes (bare copies of its non-DaemonSet pods' templates), arriving as a Poisson process with exponential lifetimes,
 and also deletes --session-deletes of the session's placed pods at uniform times.  Prints one JSON line: the card and its power limit,
 compile time, and per batch the runs, launches, device time (setup, runs), wall clock, decisions/s and device time per run; the first
---check events are checked against the CPU trace checker (tests/trace_oracle.c).
+--check events are checked against the CPU trace checker (tests/checkers.c).
 
   python tools/trace_bench.py [--nodes 10000] [--creates 50000] [--kmax 8]"""
 from __future__ import annotations
@@ -108,11 +108,11 @@ def main():
             if name == "replay":
                 first = raw[0]
     if a.check:
-        import trace_oracle
+        import checkers
         from oracle.binding import Oracle
         ev = ts.events[:a.check]
         o = Oracle(ts.compiled)
-        w = trace_oracle.trace(o, ts.placed, ts.n_prefix, ts.scenarios[0].nodes, ev)
+        w = checkers.trace(o, ts.placed, ts.n_prefix, ts.scenarios[0].nodes, ev)
         created = ev[ev[:, 0] == 1][:, 1].astype(np.int64) - ts.n_prefix
         bad = int((first["node"][created] != w["node"][created]).sum() + (first["gpu_slots"][created] != w["gpu_slots"][created]).sum())
         out["check"] = dict(events=int(len(ev)), creates=int(len(created)), mismatches=bad)
